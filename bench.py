@@ -14,6 +14,7 @@ generation:
 
     python bench.py [--gpus N] [--steps K] [--warmup W]              our CUDA path (one JSON line on rank 0)
     python bench.py --impl reference ...                            the CPU reference arm (oracle port, all host threads)
+    python bench.py ... --dump-outputs DIR                          also write what the timed steps computed as DIR/*.npy
 
 value    = whole-job codec tokens/s, device-timed (CUDA events on the launching stream, max over ranks), inputs resident
            in HBM.  tts: K timed steps form a window CENTRED on the mean context of the 16 s generation (ctx 231 -> 881,
@@ -41,7 +42,9 @@ import torch  # noqa: E402
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=600)
+    ap.add_argument("--steps", type=int, default=None,
+                    help="tts: timed decode steps (default 600); reference arm: decode steps of the CPU sample (1..64, "
+                         "default 64); edit: not accepted (the whole session is timed)")
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="tts", choices=["tts", "edit"])
@@ -55,6 +58,8 @@ def parse():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--e2e-repeats", type=int, default=3)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the token rows they produced (rank 0) as DIR/<name>.npy (float64)")
     a = ap.parse_args()
     if a.batch is None:
         a.batch = 32 if a.workload == "tts" else 16
@@ -62,6 +67,17 @@ def parse():
         a.text_len = 80 if a.workload == "tts" else 160
     if a.prompt is None:
         a.prompt = 150 if a.workload == "tts" else 800
+    if a.steps is not None and a.steps < 1:
+        ap.error("--steps must be >= 1")
+    if a.workload == "edit" and a.impl == "ours" and a.steps is not None:
+        ap.error("--steps: the edit workload times its whole session (prefill + every decode step)")
+    if a.impl == "reference":
+        if a.steps is None:
+            a.steps = 64
+        elif a.steps > 64:
+            ap.error("--steps: the CPU reference arm times at most 64 decode steps")
+    elif a.steps is None:
+        a.steps = 600
     return a
 
 
@@ -70,7 +86,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth, not measured)"
 
 
 def make_model(args):
@@ -101,7 +117,7 @@ def make_model_inputs(args, device=None):          # kept for scripts/
 
 class ClockSampler:
     """SM clock and throttle reasons sampled in-process through NVML every few ms DURING the timed region
-    (B200_PROFILING.md: a run that saw hw_slowdown / thermal slowdown, or clocks stuck low for no reason, is rejected)."""
+    (a run that saw hw_slowdown / thermal slowdown, or clocks stuck low for no reason, is not a valid measurement)."""
 
     def __init__(self, index, period=0.003):
         self.index, self.period, self.rows, self.stop_flag, self.th, self.err = index, period, [], False, None, None
@@ -207,12 +223,12 @@ def workload_config(args, cfg, world=1):
                             f"reference's length cap",
                 "batch_total": args.batch, "n_codebooks": cfg.n_codebooks, "kv_cache": args.kv,
                 "sampling": "top_k=40, top_p=1.0, temperature=1.0, one Philox stream per utterance (seed 1 + id)",
-                "l2": "per-step working set (1.65 GB weights + KV) >> 126 MB L2: no flush needed"}
+                "l2": "per-step working set (1.65 GB weights + KV) >> 50 MB L2: no flush needed"}
     return {"workload": f"giga{args.model} TTS decode, B={args.batch}/GPU independent utterances (different on every rank), "
                         f"K={cfg.n_codebooks}, text {args.text_len}, prompt {args.prompt} frames, 16 s ctx "
                         f"({args.text_len + args.prompt + 1} -> {args.text_len + args.text_len * 10 + 1})",
             "batch_per_gpu": args.batch, "n_codebooks": cfg.n_codebooks, "kv_cache": args.kv,
-            "l2": "per-step working set (1.65 GB weights + >=0.9 GB KV) >> 126 MB L2: no flush needed",
+            "l2": "per-step working set (1.65 GB weights + >=0.9 GB KV) >> 50 MB L2: no flush needed",
             "sampling": "top_k=40, top_p=1.0, temperature=1.0, one Philox stream per utterance (seed 1 + global id), generated "
                         "inside the sampler kernel"}
 
@@ -223,7 +239,7 @@ def run_reference(args):
         return
     cfg, sd = make_model(args)
     utts = make_utterances(args, cfg, range(1))
-    steps = max(1, min(args.steps, 64))
+    steps = args.steps
     warm = max(0, min(args.warmup, 2))
     cb, ms = cpu_baseline(args, cfg, sd, utts, steps + warm)
     line = {"impl": "reference", "metric": "codec tokens/s (830M TTS decode)", "value": cb["value"], "unit": "codec tokens/s",
@@ -232,22 +248,6 @@ def run_reference(args):
             "config": workload_config(args, cfg, args.gpus), "cpu_baseline": cb,
             "e2e": {"value": cb["value"], "unit": "codec tokens/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     print(json.dumps(line))
-
-
-def traffic_record(kernel_name):
-    """DRAM bytes per launch of the dominant kernel from the committed ncu capture of THIS build (profiles/r02_ncu_traffic.json,
-    written by scripts/ncu_traffic.py from `ncu --set full`); None when no capture of this kernel is committed."""
-    p = os.path.join(ROOT, "profiles", "r02_ncu_traffic.json")
-    if not os.path.exists(p):
-        return None
-    try:
-        rec = json.load(open(p))
-    except Exception:
-        return None
-    for k, v in rec.items():
-        if k.split("(")[0].strip() and k.split("(")[0].strip() in kernel_name:
-            return v
-    return None
 
 
 class Dist:
@@ -301,9 +301,32 @@ def profile_pass(lib, eng, sess, nprof):
     return list(msb), list(cnt)
 
 
-KERNEL_NAMES = ["gemm_w_xT_cluster(tcgen05, cluster split-K)", "attn_rows_kernel(paged KV, TMA bulk, split ctx)",
+KERNEL_NAMES = ["gemm_w_xT_cluster(wgmma, cluster split-K)", "attn_rows_kernel(paged KV, TMA bulk, split ctx)",
                 "ln_rows_kernel", "(unused)", "sampler_kernel", "step_prep_kernel",
-                "mega_step_kernel(persistent decode step: TMA weight/KV ring, tcgen05, stream-K)"]
+                "mega_step_kernel(persistent decode step: TMA weight/KV ring, wgmma, stream-K)"]
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """write {name: array} as out_dir/<name>.npy in float64 (token ids are exact in it), at most 64 MB in all: larger
+    outputs are replaced by a fixed, seeded sample of their flattened elements (<name>.npy) and its indices
+    (<name>_index.npy)"""
+    import numpy as np
+    arrays = {k: np.ascontiguousarray(np.asarray(v, dtype=np.float64)) for k, v in arrays.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        keep = (DUMP_LIMIT_BYTES // 2) / total            # sample + index of the same length
+        rng = np.random.default_rng(0)
+        sampled = {}
+        for k, a in arrays.items():
+            idx = np.sort(rng.choice(a.size, size=max(1, int(a.size * keep)), replace=False))
+            sampled[k], sampled[k + "_index"] = a.reshape(-1)[idx], idx.astype(np.float64)
+        arrays = sampled
+    os.makedirs(out_dir, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a)
 
 
 def run_tts(args, D):
@@ -321,7 +344,10 @@ def run_tts(args, D):
     cap = args.text_len * (cfg.encodec_sr // 5)
     S_total = cap - (args.prompt + 1) - 2                  # decode steps until the length cap fires
     W = max(3, args.warmup)
-    Ksteps = max(1, min(args.steps, S_total - W - 10))
+    max_steps = S_total - W - 10                           # the window must end before the length cap
+    if not 1 <= args.steps <= max_steps:
+        raise SystemExit(f"--steps {args.steps}: this workload allows 1 .. {max_steps} timed steps with --warmup {args.warmup}")
+    Ksteps = args.steps
     start = max(W, (S_total - Ksteps) // 2)                # window centred on the mean context of the generation
     model.configure_engine(max_slots=B, max_seq_len=(args.text_len + cap + 64 + 255) // 256 * 256, kv_dtype=args.kv,
                            max_new_tokens=cap + 64)
@@ -355,6 +381,12 @@ def run_tts(args, D):
     assert not any(s.done for s in st)
     tok_s = world * B * K * Ksteps / (ms * 1e-3)
     ctx1 = ctx0 + Ksteps
+    if args.dump_outputs and rank == 0:
+        # what a caller of the session receives: every utterance's delayed token rows so far [B, steps, K], and the
+        # rows the last timed step produced [B, K]
+        import numpy as np
+        rows = np.stack([sess.raw_tokens(i) for i in range(B)], 0)
+        dump_outputs(args.dump_outputs, {"tts_token_rows": rows, "tts_last_step_tokens": rows[:, -1, :]})
 
     # ------------------------------------------------------------------ roofline: profiled pass (same engine state)
     roof = step_roof = None
@@ -387,11 +419,8 @@ def run_tts(args, D):
         # which serialises launches, so only the share is used) x the timed step / launches per step
         dur = (msb[dom] / total) * (ms / Ksteps * 1e-3) / (cnt[dom] / nprof)
         ach = bytes_per_launch / dur / 1e9
-        tr = traffic_record(KERNEL_NAMES[dom])
         roof = {"bound": "hbm", "kernel": KERNEL_NAMES[dom], "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                "traffic": tr["dram_bytes_per_launch"] if tr else None,
-                "traffic_source": (tr.get("source") if tr else "no ncu --set full capture of this kernel committed under profiles/"),
-                "traffic_capture": tr,
+                "traffic": None, "traffic_source": "not measured (no profiler capture of this build)", "traffic_capture": None,
                 "algorithmic_bytes_per_launch": bytes_per_launch, "avg_launch_us": dur * 1e6,
                 "isolated_launch_us": msb[dom] / cnt[dom] * 1e3, "peak_source": peak_src, "ctx": ctx_used, "by_kernel": shares,
                 "note": "avg_launch_us = share of the step (event-per-launch pass at ctx %.0f) x timed step / launches per step; "
@@ -482,6 +511,9 @@ def run_edit(args, D):
     clk = clocks.stop()
     launches = lib.vcb_counter(model._eng, b"launches") - l0
     ms = D.max(ev0.elapsed_time(ev1))
+    if args.dump_outputs and rank == 0:
+        # the edited token matrices [K, T'] of this rank's utterances, as inference_many returns them
+        dump_outputs(args.dump_outputs, {f"edit_tokens_{i:02d}": r[0].cpu().numpy() for i, r in zip(mine, res)})
     # generated frames replace the 100-frame span: T' = T - 100 + generated
     gen_frames_total = D.sum(sum(int(r.shape[-1]) - (args.prompt - 100) for r in res))
     tok_s = gen_frames_total * K / (ms * 1e-3)

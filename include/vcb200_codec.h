@@ -1,7 +1,7 @@
 /* vcb200_codec.h -- C ABI of the EnCodec decoder (token -> waveform) and encoder (waveform -> token) in libvcb200.so.
  *
  * Replaces AudioTokenizer.decode (reference data/tokenizer.py:131-133), i.e. audiocraft's
- * EncodecModel.decode = ResidualVectorQuantizer.decode + SEANetDecoder, with hand-written sm_100a kernels
+ * EncodecModel.decode = ResidualVectorQuantizer.decode + SEANetDecoder, with hand-written sm_90a kernels
  * (RVQ gather-sum, implicit-GEMM Conv1d / ConvTranspose1d with fused ELU / bias / residual, LSTM).
  * Same conventions as vcb200.h: plain pointers, 0 on success, vcb_last_error() for the message.
  */

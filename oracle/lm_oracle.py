@@ -18,7 +18,7 @@ reference itself, imported and run by tests/golden/make_golden.py (same weights,
 identical token ids and logits); fixtures are committed under tests/golden/.
 
 Numerics policy knob: ``kv_round_bf16`` rounds projected K/V to bf16 before use/caching (what the
-B200 path's bf16 paged KV cache does).  With it off, and noise drawn from the global CPU generator,
+H100 path's bf16 paged KV cache does).  With it off, and noise drawn from the global CPU generator,
 this module is operation-for-operation the reference's fp32 path.
 
 torch.multinomial(p, 1) is restated as argmax(p / q), q ~ Exp(1) drawn with

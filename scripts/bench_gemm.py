@@ -1,4 +1,4 @@
-"""Micro-benchmark of the tcgen05 GEMM kernel over the 830M decode shapes (run on the GPU box)."""
+"""Micro-benchmark of the wgmma GEMM kernel over the 830M decode shapes (run on the GPU box)."""
 import ctypes as C
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -156,6 +156,9 @@ def part_b(out, t0):
         out[f"logits_{pol}"] = np.stack([traces[i] for i in TRACE_UTTS]).astype(np.float32)   # [utt, step, K, V]
         del oracle
     lm_oracle.sample_rows = orig
+    # three files of < 1 MB each (tests/golden_util.headline_fixture merges them)
+    for pol in ("fp32", "bf16"):
+        np.savez_compressed(os.path.join(HERE, f"lm_830m_b32_logits_{pol}.npz"), **{f"logits_{pol}": out.pop(f"logits_{pol}")})
     np.savez_compressed(os.path.join(HERE, "lm_830m_b32.npz"), **out)
     meta = dict(n_steps=N_STEPS, prompts=PROMPTS, text_len=TEXT_LEN, kw=KW, trace_utts=TRACE_UTTS, trace_steps=TRACE_STEPS,
                 pinned=pinned, pinned_ckpt_seed=3, ckpt_seed=0, noise_seed="1 + i", data_seed="100 + i")

@@ -51,7 +51,11 @@ def cpu_noise_fn(seed):
 def headline_fixture():
     with open(os.path.join(GOLDEN, "lm_830m_b32.json")) as f:
         meta = json.load(f)
-    return meta, np.load(os.path.join(GOLDEN, "lm_830m_b32.npz"))
+    # stored as three files of < 1 MB each: token rows / sensitivities / pinned utterances, and the traced logits per KV policy
+    g = dict(np.load(os.path.join(GOLDEN, "lm_830m_b32.npz")))
+    for kv in ("fp32", "bf16"):
+        g.update(np.load(os.path.join(GOLDEN, f"lm_830m_b32_logits_{kv}.npz")))
+    return meta, g
 
 
 def suppress_end_tokens(cfg, sd):

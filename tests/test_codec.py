@@ -145,7 +145,7 @@ def _counter(tok, name):
 
 @pytest.mark.gpu
 def test_tensor_core_decoder_runs_the_default_codec():
-    """The default 16 kHz codec must decode on the tcgen05 path (csrc/codec_tc.cu), not fall back to the CUDA-core kernels.
+    """The default 16 kHz codec must decode on the tensor-core path (csrc/codec_tc.cu), not fall back to the CUDA-core kernels.
     Tolerance (stated for the 3-pass bf16 hi/lo product, fp32 accumulation): waveform SNR >= 80 dB against the fp32 oracle
     and max |err| <= 2e-4 of the peak."""
     cfg = eo.default_config()

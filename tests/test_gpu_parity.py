@@ -1,6 +1,6 @@
 """-m gpu: the CUDA path (through the C ABI) against the golden fixtures of the real reference and the CPU oracle.
 
-Numerics policy under test (DESIGN.md): GEMM weights bf16 (the synthetic checkpoints are bf16-representable, so
+Numerics policy under test: GEMM weights bf16 (the synthetic checkpoints are bf16-representable, so
 the fp32 reference saw the same weights), activations split hi+lo bf16 (>= 16 mantissa bits), fp32 accumulation
 and fp32 everywhere else.  With kv_dtype=fp32 the engine follows the unmodified reference; with the default
 bf16 KV cache it follows the oracle's kv_round_bf16 policy.  Token ids must be IDENTICAL; raw logits agree to
@@ -35,7 +35,7 @@ def _model(cfg, sd, kv="fp32"):
 @pytest.mark.parametrize("simt", [1, 0])
 @pytest.mark.parametrize("shape", [(256, 256, 4), (768, 256, 32), (2052, 1024, 32), (1024, 4096, 128), (6144, 2048, 7)])
 def test_gemm_tcgen05_vs_fp32(shape, simt):
-    """Bring-up check of the tcgen05/TMA GEMM (and its CUDA-core cross-check twin) against torch fp32."""
+    """Bring-up check of the wgmma/TMA GEMM (and its CUDA-core cross-check twin) against torch fp32."""
     from voicecraft_b200 import _lib
     lib = _lib.load()
     N, K, B = shape
@@ -289,7 +289,7 @@ def test_full_size_830M_first_steps_match_oracle(wide, monkeypatch):
 
 @pytest.mark.parametrize("shape", [(256, 256, 40), (768, 256, 300), (1024, 4096, 1000), (6144, 2048, 513), (384, 512, 129)])
 def test_gemm_rows_vs_fp32(shape):
-    """Rows-as-M tcgen05 GEMM of the wide prefill path (csrc/gemm_rows.cu) against torch fp64: 256-wide tiles (even number
+    """Rows-as-M wgmma GEMM of the wide prefill path (csrc/gemm_rows.cu) against torch fp64: 256-wide tiles (even number
     of 128-feature blocks), 128-wide tiles (odd: 384), ragged last row tile."""
     from voicecraft_b200 import _lib
     lib = _lib.load()
@@ -401,8 +401,8 @@ def test_headline_830M_b32_matches_oracle(kv):
     assert worst <= LOGIT_TOL, f"max |logit - oracle| = {worst}"
     for i, (s, k, mg) in first_div.items():
         assert mg < SENS_TOL[kv], f"utterance {i} differs at step {s} codebook {k} where the oracle's decision is robust to {mg:.3g}"
-    # 109 of the 8192 bf16-policy samples sit within SENS_TOL of a flip; with ~1e-3 of logit noise a handful of them go
-    # the other way (5 on the first B200 run).  More than 8 divergent utterances would mean noise well above that.
+    # 109 of the 8192 bf16-policy samples sit within SENS_TOL of a flip; with ~1e-3 of logit noise a handful of them may go
+    # the other way.  More than 8 divergent utterances would mean noise well above that.
     assert identical >= (32 if kv == "fp32" else 24), f"{identical}/32 utterances token-identical ({first_div})"
 
 

@@ -72,7 +72,7 @@ def test_topk1_is_argmax():
 
 
 def test_kv_bf16_policy_is_close():
-    """Rounding cached K/V to bf16 (the B200 default) moves logits by ~1e-3 at most on the tiny model."""
+    """Rounding cached K/V to bf16 (the H100 default) moves logits by ~1e-3 at most on the tiny model."""
     name = "tts_topk40"
     res, trace, g = _run_oracle(name, CASES[name], kv_round_bf16=True)
     ref0 = g["trace_logits"][0]

@@ -1,7 +1,7 @@
 """ctypes binding of libvcb200.so (C ABI declared in include/vcb200.h).
 
 The shared library is built in-tree by ``__graft_entry__.build()`` / ``make -C voicecraft_b200/csrc``.
-There is deliberately no fallback: if the library is missing or no sm_100 GPU is present, loading or
+There is deliberately no fallback: if the library is missing or no sm_90 GPU is present, loading or
 ``vcb_create`` fails loudly (the product path never routes through a CPU implementation).
 """
 import ctypes as C

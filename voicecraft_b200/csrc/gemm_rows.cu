@@ -2,7 +2,7 @@
 //
 //   out[r][n] = epilogue( sum_k (Xhi[r,k] + Xlo[r,k]) * W[n,k] + bias[n] )        r = token row, n = output feature
 //
-// gemm_tcgen05.cu keeps the WEIGHTS as the 128-lane operand and at most 128 token rows as the UMMA N dimension: right
+// gemm_tcgen05.cu keeps the WEIGHTS as the 128-row operand and at most 128 token rows as the MMA N dimension: right
 // for decode (every weight byte is used once per step), wrong for a prompt of thousands of rows, where it streams the
 // whole matrix once per 128 rows and spends most of each launch in the per-row epilogue.  Here a CTA owns a
 // [128 rows] x [BN features] output tile:
@@ -11,11 +11,12 @@
 //               (D += Ahi.B^T ; D += Alo.B^T), so the second pass costs no extra weight traffic.
 //   B operand = the pre-tiled weights of gemm_tcgen05.cu, unchanged: BN/128 consecutive 16 KB blocks of one k-block,
 //               stacked in shared memory, are exactly a K-major SWIZZLE_128B operand of BN rows.
-//   D         = fp32 in TMEM, lane = token row, column = feature (BN <= 256 columns).
+//   D         = fp32 in registers (wgmma): each of two warpgroups multiplies 64 token rows x BN features, then stages
+//               its accumulators in the (by then idle) pipeline shared memory, row = token, column = feature.
 // No split-K, no cluster: with >= 512 rows there are enough tiles (e.g. QKV at d = 2048: 24 x rows/128 CTAs), and the
 // weights (<= 34 MB per matrix) stay L2-resident across the row tiles.
-// Warp roles as in gemm_tcgen05.cu: w0 TMA producer, w1 TMEM alloc + MMA issuer, w2..w9 epilogue (two sets of four,
-// each set covers the 128 TMEM lanes and takes half of the columns).
+// Warp roles as in gemm_tcgen05.cu: w0 TMA producer, w1..w3 idle, w4..w11 MMA + epilogue (two warpgroups; in the
+// epilogue each covers all 128 rows and takes half of the columns).
 // Epilogues: EPI_QKV (q -> fp32 rows, k/v -> paged KV cache), EPI_RESID (x += y + b), EPI_ACT (ReLU/GELU -> hi/lo
 // planes), EPI_LOGITS (plain fp32 rows; bring-up tests).  A thread owns one token row and 32 consecutive features
 // per step, so every access is a run of 16-byte vectors.
@@ -26,10 +27,10 @@
 
 namespace vcb {
 
-static constexpr int RG_BM = 128;     // token rows per CTA (UMMA M)
+static constexpr int RG_BM = 128;     // token rows per CTA (2 x wgmma M)
 static constexpr int RG_BK = 64;      // K elements per stage (one 128-byte swizzle row of bf16)
 static constexpr int RG_EPI_WARPS = 8;
-static constexpr int RG_THREADS = 64 + 32 * RG_EPI_WARPS;
+static constexpr int RG_THREADS = 128 + 32 * RG_EPI_WARPS;
 
 template <int BN, int STAGES>
 struct RowsSmem {
@@ -37,7 +38,9 @@ struct RowsSmem {
     static constexpr int B_BYTES = BN * RG_BK * 2;
     static constexpr int STAGE_BYTES = 2 * A_BYTES + B_BYTES;
     static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
-    static constexpr int TOTAL = BAR_OFFSET + (2 * STAGES + 1) * 8 + 16;
+    static constexpr int TOTAL = BAR_OFFSET + 2 * STAGES * 8;
+    static constexpr int ACC_LD = BN + 4;                           // staged accumulators [128][ACC_LD] fp32, conflict-free rows
+    static_assert(RG_BM * ACC_LD * 4 <= BAR_OFFSET, "staged accumulators alias the pipeline stages");
 };
 
 __device__ __forceinline__ float act_fn(float v, int kind) {
@@ -132,8 +135,6 @@ gemm_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     extern __shared__ __align__(1024) uint8_t smem[];       // SWIZZLE_128B tiles need 1024-byte alignment
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tmem_full = empty_bar + STAGES;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -148,9 +149,8 @@ gemm_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         tma_prefetch_desc(&tmW);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], RG_EPI_WARPS);        // one arrival per MMA warp
         }
-        mbar_init(tmem_full, 1);
         mbar_fence_init();
         // weights never depend on the previous kernel: the first stages' weight tiles go in flight before the wait
         for (int i = 0; i < pre; ++i) {
@@ -161,14 +161,7 @@ gemm_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                 tma_load_2d(b + j * (128 * RG_BK * 2), &tmW, &full_bar[i], 0, ((mt0 + j) * total_kb + i) * 128);
         }
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, BN);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp == 0) {
         // ===== TMA producer ==========================================================================
@@ -193,50 +186,57 @@ gemm_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer ============================================================================
-        constexpr uint32_t idesc = umma_idesc_bf16_f32(RG_BM, BN);
-        int stage = 0, phase = 0;
+    } else if (warp >= 4) {
+        // ===== MMA: warpgroup `half` multiplies token rows [64 half, 64 half + 64) x all BN features =====================
+        const int q = warp & 3;
+        const int half = (warp - 4) >> 2;
+        float acc[BN / 2];
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+        int stage = 0, phase = 0, prev = -1;
         for (int i = 0; i < total_kb; ++i) {
             mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t a_addr = smem_u32(smem + stage * L::STAGE_BYTES);
-                const uint64_t hi_desc = umma_desc_kmajor_sw128(a_addr);
-                const uint64_t lo_desc = umma_desc_kmajor_sw128(a_addr + L::A_BYTES);
-                const uint64_t b_desc = umma_desc_kmajor_sw128(a_addr + 2 * L::A_BYTES);
-#pragma unroll
-                for (int k = 0; k < RG_BK / 16; ++k) {      // +32 B per 16 K-elements inside the swizzle row
-                    umma_bf16(tmem_base, hi_desc + 2 * k, b_desc + 2 * k, idesc, (i | k) != 0);
-                    umma_bf16(tmem_base, lo_desc + 2 * k, b_desc + 2 * k, idesc, 1u);
-                }
-                umma_commit(&empty_bar[stage]);             // frees the smem slot when the MMAs retire
-                if (i == total_kb - 1) umma_commit(tmem_full);
-            }
+            const uint32_t a_addr = smem_u32(smem + stage * L::STAGE_BYTES) + half * 64 * 128;
+            const uint32_t b_addr = smem_u32(smem + stage * L::STAGE_BYTES + 2 * L::A_BYTES);
+            wg_fence();
+            wg_mma_kblock<BN>(acc, a_addr, b_addr);
+            wg_mma_kblock<BN>(acc, a_addr + L::A_BYTES, b_addr);
+            wg_commit();
+            wg_wait1();                                     // k-block i-1's MMAs are complete, i's may still run
             __syncwarp();
+            if (lane == 0 && prev >= 0) mbar_arrive(&empty_bar[prev]);   // this warp's MMAs have read that slot
+            prev = stage;
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-    } else {
-        // ===== epilogue: TMEM -> registers -> fused epilogue, one token row per thread ================
-        const int q = warp & 3;                             // TMEM lane quarter this warp may read
-        const int half = (warp - 2) >> 2;                   // which half of the columns
+        wg_wait0();
+        wg_acc_fence(acc);
+        // stage the accumulators in shared memory once BOTH warpgroups are done reading the pipeline slots
+        float* sacc = reinterpret_cast<float*>(smem);
+        asm volatile("bar.sync 1, %0;" ::"n"(32 * RG_EPI_WARPS) : "memory");
+        {
+            const int r = half * 64 + q * 16 + (lane >> 2);
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const int c = 8 * j + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(sacc + r * L::ACC_LD + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+                *reinterpret_cast<float2*>(sacc + (r + 8) * L::ACC_LD + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+            }
+        }
+        asm volatile("bar.sync 1, %0;" ::"n"(32 * RG_EPI_WARPS) : "memory");
+        // ===== epilogue: one token row per thread, 32 consecutive features per step =====================================
         const int row = r0 + q * 32 + lane;
-        mbar_wait(tmem_full, 0);
-        tc_fence_after();
         pdl_wait();                                         // residual rows / KV positions come from earlier kernels
-        const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
+        const float* arow = sacc + (q * 32 + lane) * L::ACC_LD;
 #pragma unroll 1
         for (int c = half * (BN / 2); c < (half + 1) * (BN / 2); c += 32) {
             float v[32];
-            tmem_ld_32x32(lane_addr + c, v);                // warp-collective: outside the row / feature guards
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) {
+                const float4 t = *reinterpret_cast<const float4*>(arow + c + j);
+                v[j] = t.x; v[j + 1] = t.y; v[j + 2] = t.z; v[j + 3] = t.w;
+            }
             if (row < rows && n0 + c < Nout) rows_epilogue32(ep, row, n0 + c, v);
         }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, BN);
     }
 }
 

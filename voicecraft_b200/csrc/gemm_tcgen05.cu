@@ -5,11 +5,12 @@
 //   A operand = weight matrix W [Nout, Kdim] bf16, PRE-TILED in HBM: tile (mt, kb) = W[mt*128.., kb*64..] is one
 //               contiguous 16 KB block [128 rows][64 cols] at block index mt*KB + kb (pack_weight_tiles), so every
 //               TMA box is a single sequential DRAM burst (a row-major matrix would scatter a box over 128 DRAM
-//               pages -- measured 18% DRAM utilisation in ncu).  TMA SWIZZLE_128B into smem.
+//               pages).  TMA SWIZZLE_128B into smem.
 //   B operand = activations  X [2*Bpad, Kdim] bf16: rows [0,Bpad) = hi parts, rows [Bpad,2*Bpad) = lo parts
-//               (x ~= hi + lo, see split_bf16): one UMMA of N = 2*Bpad columns covers both; the tensor pipe is
-//               >80% idle in this HBM-bound regime, so the second half is free and buys ~16 mantissa bits.
-//   D         = fp32 accumulator in TMEM, 128 lanes (= output features) x 2*Bpad columns
+//               (x ~= hi + lo, see split_bf16): one MMA of N = 2*Bpad columns covers both; this regime is HBM-bound,
+//               so the tensor cores have the room, and the second half buys ~16 mantissa bits.
+//   D         = fp32 accumulators in registers (wgmma): 128 output features x 2*Bpad columns per CTA, 64 features per
+//               warpgroup issue (one warpgroup covers both 64-feature halves when Bpad <= 32)
 //
 // Split-K without a workspace: the S CTAs of a thread-block cluster each stream one K slice of the same 128-feature
 // weight tile (so >=128 CTAs pull HBM even for a 2048 x 2048 matrix), then reduce-scatter their accumulators
@@ -21,8 +22,8 @@
 //     EPI_RESID  x += y + bias                                            (transformer.py:321-329)
 //     EPI_ACT    ReLU / exact GELU -> bf16 hi/lo rows of the next GEMM      (transformer.py:387, voicecraft.py:183)
 //     EPI_LOGITS fp32 logits                                              (voicecraft.py:1085)
-// Warp roles: w0 TMA producer, w1 TMEM alloc + MMA issuer (one elected thread issues tcgen05.mma), w2..w5 epilogue
-// (plus w6..w9 for tiles with >= 64 token rows).  Prompt batches use the rows-as-M kernel in gemm_rows.cu instead.
+// Warp roles: w0 TMA producer, w1..w3 idle (the MMA warpgroups must start on a warpgroup boundary), w4..w7 MMA +
+// epilogue (plus w8..w11 for tiles with >= 64 token rows).  Prompt batches use the rows-as-M kernel in gemm_rows.cu instead.
 #include "vcb_internal.h"
 
 #include <algorithm>
@@ -31,12 +32,13 @@
 
 namespace vcb {
 
-static constexpr int GEMM_BM = 128;   // output features per CTA (UMMA M)
+static constexpr int GEMM_BM = 128;   // output features per CTA (2 x wgmma M)
 static constexpr int GEMM_BK = 64;    // K elements per pipeline stage (= 128 B of bf16 = one swizzle row)
-// threads per CTA: w0 TMA, w1 MMA, then 4 epilogue warps (one per TMEM lane quarter); tiles with >= 64 token rows get a
-// second set of 4 that takes the other half of the rows (the epilogue, not the weight stream, dominates those launches)
+// threads per CTA: warpgroup 0 (w0 TMA), then one MMA + epilogue warpgroup; tiles with >= 64 token rows get a second one:
+// each then multiplies 64 of the 128 features (accumulators: Bpad registers per thread) and takes half of the rows in
+// the epilogue (the epilogue, not the weight stream, dominates those launches)
 constexpr int gemm_epi_warps(int bn) { return bn >= 128 ? 8 : 4; }
-constexpr int gemm_threads(int bn) { return 64 + 32 * gemm_epi_warps(bn); }
+constexpr int gemm_threads(int bn) { return 128 + 32 * gemm_epi_warps(bn); }
 
 template <int BN, int STAGES>
 struct GemmSmem {
@@ -46,7 +48,7 @@ struct GemmSmem {
     static constexpr int RED_OFFSET = STAGES * STAGE_BYTES;
     static constexpr int RED_BYTES = (BN / 2) * GEMM_BM * 4;          // [S][R][128] fp32 with S*R = Bpad
     static constexpr int BAR_OFFSET = RED_OFFSET + RED_BYTES;
-    static constexpr int TOTAL = BAR_OFFSET + (2 * STAGES + 2) * 8 + 8;       // full[S] empty[S] tmem_full red_full + tmem slot
+    static constexpr int TOTAL = BAR_OFFSET + (2 * STAGES + 1) * 8;           // full[S] empty[S] red_full
 };
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
@@ -70,15 +72,9 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t local_smem_addr, uint32_t 
 // Asynchronous store into a peer CTA's shared memory that counts its bytes on the peer's mbarrier: the owner of the
 // rows learns that every partial has landed from its own barrier -- no cluster-wide barrier (and no GPU-scope
 // membar, which is what barrier.cluster.arrive.release costs) between the accumulators and the epilogue.
-__device__ __forceinline__ void st_async_f32(uint32_t remote_addr, uint32_t remote_bar, float v) {
-    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.f32 [%0], %1, [%2];" ::"r"(remote_addr), "f"(v),
-                 "r"(remote_bar)
-                 : "memory");
-}
-__device__ __forceinline__ void st_async_f32x4(uint32_t remote_addr, uint32_t remote_bar, float a, float b, float c, float d) {
-    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v4.f32 [%0], {%1, %2, %3, %4}, [%5];" ::"r"(
-                     remote_addr),
-                 "f"(a), "f"(b), "f"(c), "f"(d), "r"(remote_bar)
+__device__ __forceinline__ void st_async_f32x2(uint32_t remote_addr, uint32_t remote_bar, float a, float b) {
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];" ::"r"(remote_addr),
+                 "f"(a), "f"(b), "r"(remote_bar)
                  : "memory");
 }
 // bounded wait: a byte-count mismatch would otherwise hang the GPU; ~1 s of polling, then trap (surfaces as a CUDA error)
@@ -164,15 +160,14 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                   const void* pf_ptr, unsigned long long pf_bytes, const GemmGroup grp) {
     using L = GemmSmem<BN, STAGES>;
     constexpr int BPAD = BN / 2;
-    constexpr int HALVES = gemm_epi_warps(BN) / 4;          // epilogue warp sets, each covering all 128 TMEM lanes
+    constexpr int HALVES = gemm_epi_warps(BN) / 4;          // MMA + epilogue warpgroups
+    constexpr int MH = 2 / HALVES;                          // 64-feature halves multiplied by each warpgroup
     constexpr int EPI_THREADS = 32 * gemm_epi_warps(BN);
     extern __shared__ __align__(1024) uint8_t smem[];       // SWIZZLE_128B tiles need 1024-byte alignment
     float* red = reinterpret_cast<float*>(smem + L::RED_OFFSET);
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
     uint64_t* empty_bar = full_bar + STAGES;
-    uint64_t* tmem_full = empty_bar + STAGES;
-    uint64_t* red_full = tmem_full + 1;                     // all S partials of my R rows have landed in `red`
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(red_full + 1);
+    uint64_t* red_full = empty_bar + STAGES;                // all S partials of my R rows have landed in `red`
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -196,9 +191,8 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         tma_prefetch_desc(&tmB);
         for (int s = 0; s < STAGES; ++s) {
             mbar_init(&full_bar[s], 1);
-            mbar_init(&empty_bar[s], 1);
+            mbar_init(&empty_bar[s], gemm_epi_warps(BN));  // one arrival per MMA warp
         }
-        mbar_init(tmem_full, 1);
         mbar_init(red_full, 1);
         mbar_fence_init();
         // every CTA of the cluster sends all of my R rows x 128 features (fp32), armed before anyone can send
@@ -214,21 +208,14 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         // (bit 63 of pf_bytes: issue it after this CTA's last weight load instead -- HBM idles during the epilogue)
         if (!(pf_bytes >> 63)) prefetch_l2_slice(pf_ptr, pf_bytes, blockIdx.x, gridDim.x);
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, BN < 32 ? 32 : BN);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     cluster_sync_all();             // CTA-wide sync + "every CTA of the cluster has started and armed its barrier"
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     // per-feature epilogue constants (bias / LN-fold vector / next gamma) are model weights, never written by a kernel:
     // the epilogue warps fetch them while the mainloop runs, off the critical tail
     float w_bias = 0.f, w_cv = 0.f, w_gnext = 0.f;
     float e_mean = 0.f, e_rstd = 0.f;                       // LayerNorm statistics of row z*R + lane (BPAD <= 32, see below)
     float e_x[4] = {0.f, 0.f, 0.f, 0.f};                    // residual rows fetched early (R == 4)
     bool e_x_valid = false;
-    if (warp >= 2) {
+    if (warp >= 4) {
         const int m = m0 + (warp & 3) * 32 + lane;
         if (m < Nout) {
             const float* bias_ptr = grp.bias ? grp.bias[grp_i] : ep.bias;
@@ -259,31 +246,11 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             }
             if (pf_bytes >> 63) prefetch_l2_slice(pf_ptr, pf_bytes & ~(1ull << 63), blockIdx.x, gridDim.x);
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer ============================================================================
-        constexpr uint32_t idesc = umma_idesc_bf16_f32(GEMM_BM, BN);
-        int stage = 0, phase = 0;
-        for (int i = 0; i < nkb; ++i) {
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            if (lane == 0) {
-                const uint32_t a_addr = smem_u32(smem + stage * L::STAGE_BYTES);
-                const uint64_t a_desc = umma_desc_kmajor_sw128(a_addr);
-                const uint64_t b_desc = umma_desc_kmajor_sw128(a_addr + L::A_BYTES);
-#pragma unroll
-                for (int k = 0; k < GEMM_BK / 16; ++k)     // +32 B per 16 K-elements inside the swizzle row
-                    umma_bf16(tmem_base, a_desc + 2 * k, b_desc + 2 * k, idesc, (i | k) != 0);
-                umma_commit(&empty_bar[stage]);             // frees the smem slot when the MMAs retire
-                if (i == nkb - 1) umma_commit(tmem_full);   // accumulator complete
-            }
-            __syncwarp();
-            if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-    } else {
-        // ===== epilogue part 1: TMEM -> registers -> reduce-scatter over the cluster (DSMEM) =========
-        const int q = warp & 3;                             // TMEM lane quarter owned by this warp
-        const int half = (warp - 2) >> 2;                   // which set of 4 epilogue warps (0 unless HALVES == 2)
-        const int ml = q * 32 + lane;                       // feature inside the tile
+    } else if (warp >= 4) {
+        // ===== MMA mainloop, then reduce-scatter of the accumulators over the cluster (DSMEM) ==========
+        const int q = warp & 3;                             // warp inside its warpgroup
+        const int half = (warp - 4) >> 2;                   // which warpgroup (0 unless HALVES == 2)
+        const int ml = q * 32 + lane;                       // feature inside the tile (epilogue part 2 layout)
         const int R = BPAD / S;                             // token rows owned by each CTA (power of two)
         const int shR = 31 - __clz(R);
         // While the mainloop runs: everything the epilogue needs from EARLIER kernels.  With a folded LayerNorm that is the
@@ -323,73 +290,79 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 e_x_valid = true;
             }
         }
-        if (nkb > 0) {
-            mbar_wait(tmem_full, 0);
-            tc_fence_after();
+        // mainloop: this warpgroup's MH x 64 features x BN columns, every k-block of my K slice
+        float acc[MH][BN / 2];
+#pragma unroll
+        for (int h = 0; h < MH; ++h)
+#pragma unroll
+            for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
+        {
+            int stage = 0, phase = 0, prev = -1;
+            for (int i = 0; i < nkb; ++i) {
+                mbar_wait(&full_bar[stage], phase);
+                const uint32_t a_addr = smem_u32(smem + stage * L::STAGE_BYTES);
+                wg_fence();
+#pragma unroll
+                for (int h = 0; h < MH; ++h)
+                    wg_mma_kblock<BN>(acc[h], a_addr + (half * MH + h) * 64 * 128, a_addr + L::A_BYTES);
+                wg_commit();
+                wg_wait1();                                 // k-block i-1's MMAs are complete, i's may still run
+                __syncwarp();
+                if (lane == 0 && prev >= 0) mbar_arrive(&empty_bar[prev]);   // this warp's MMAs have read that slot
+                prev = stage;
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+            wg_wait0();
+            __syncwarp();
+            if (lane == 0 && prev >= 0) mbar_arrive(&empty_bar[prev]);
         }
-        if (threadIdx.x == 64) tl_mark(0x120 + ep.mode);
-        const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
+#pragma unroll
+        for (int h = 0; h < MH; ++h) wg_acc_fence(acc[h]);
+        if (threadIdx.x == 128) tl_mark(0x120 + ep.mode);
         const uint32_t red_addr = smem_u32(red);
         const uint32_t bar_addr = smem_u32(red_full);
-        constexpr int CH = BPAD < 32 ? 16 : 32;
-        // red layout in the owner: [writer z][feature ml][R rows] -- a thread's R partials for one owner are contiguous
-        // (16-byte vector stores when R >= 4).  All Bpad rows are sent, valid or not: the byte count is a constant.
-#pragma unroll 1
-        for (int c = half * (BPAD / HALVES); c < (half + 1) * (BPAD / HALVES); c += CH) {
-            float hi[CH], lo[CH];
-            if (nkb > 0) {
-                if constexpr (CH == 32) {
-                    tmem_ld_32x32(lane_addr + c, hi);
-                    tmem_ld_32x32(lane_addr + BPAD + c, lo);
-                } else {
-                    tmem_ld_32x16(lane_addr + c, hi);
-                    tmem_ld_32x16(lane_addr + BPAD + c, lo);
-                }
-            } else {
+        // red layout in the owner: [writer z][feature][R rows].  A thread holds two features (f, f + 8) x pairs of adjacent
+        // token rows (8-byte stores; R >= 2 keeps a pair inside one owner).  All Bpad rows are sent, valid or not: the byte
+        // count is a constant.
 #pragma unroll
-                for (int j = 0; j < CH; ++j) hi[j] = lo[j] = 0.f;
-            }
+        for (int h = 0; h < MH; ++h) {
 #pragma unroll
-            for (int j = 0; j < CH; j += 4) {
-                const int row = c + j;
-                if (S == 1) {
-                    // no split: the partials stay in this CTA -- plain shared stores, handed over by a named barrier
-                    // (a 1-CTA cluster has no peer to st.async to; compute-sanitizer rejects the remote form there)
-                    *reinterpret_cast<float4*>(red + (static_cast<size_t>(ml) << shR) + row) =
-                        make_float4(hi[j] + lo[j], hi[j + 1] + lo[j + 1], hi[j + 2] + lo[j + 2], hi[j + 3] + lo[j + 3]);
-                } else if (R >= 4) {
-                    const int owner = row >> shR, rr = row & (R - 1);
-                    const uint32_t off = static_cast<uint32_t>((((z << 7) + ml) << shR) + rr) << 2;
-                    st_async_f32x4(mapa_u32(red_addr + off, owner), mapa_u32(bar_addr, owner), hi[j] + lo[j],
-                                   hi[j + 1] + lo[j + 1], hi[j + 2] + lo[j + 2], hi[j + 3] + lo[j + 3]);
-                } else {
+            for (int jb = 0; jb < BPAD / 8; ++jb) {
+                const int row = 8 * jb + 2 * (lane & 3);
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        const int owner = (row + u) >> shR, rr = (row + u) & (R - 1);
-                        const uint32_t off = static_cast<uint32_t>((((z << 7) + ml) << shR) + rr) << 2;
-                        st_async_f32(mapa_u32(red_addr + off, owner), mapa_u32(bar_addr, owner), hi[j + u] + lo[j + u]);
+                for (int e = 0; e < 2; ++e) {
+                    const int f = (half * MH + h) * 64 + q * 16 + (lane >> 2) + 8 * e;
+                    const float s0 = acc[h][4 * jb + 2 * e] + acc[h][4 * (jb + BPAD / 8) + 2 * e];
+                    const float s1 = acc[h][4 * jb + 2 * e + 1] + acc[h][4 * (jb + BPAD / 8) + 2 * e + 1];
+                    if (S == 1) {
+                        // no split: the partials stay in this CTA -- plain shared stores, handed over by a named barrier
+                        // (a 1-CTA cluster has no peer to st.async to)
+                        *reinterpret_cast<float2*>(red + (static_cast<size_t>(f) << shR) + row) = make_float2(s0, s1);
+                    } else {
+                        const int owner = row >> shR, rr = row & (R - 1);
+                        const uint32_t off = static_cast<uint32_t>((((z << 7) + f) << shR) + rr) << 2;
+                        st_async_f32x2(mapa_u32(red_addr + off, owner), mapa_u32(bar_addr, owner), s0, s1);
                     }
                 }
             }
         }
-        tc_fence_before();
-        if (threadIdx.x == 64) tl_mark(0x140 + ep.mode);
+        if (threadIdx.x == 128) tl_mark(0x140 + ep.mode);
     }
-    if (warp >= 2) {
+    if (warp >= 4) {
         if (S == 1) asm volatile("bar.sync 4, %0;" ::"n"(EPI_THREADS) : "memory");   // every epilogue thread stored its partials
         else mbar_wait_bounded(red_full, 0);                // all S partials of my rows have landed (async stores counted)
-        if (threadIdx.x == 64) tl_mark(0x150 + ep.mode);
+        if (threadIdx.x == 128) tl_mark(0x150 + ep.mode);
         // ===== epilogue part 2: fixed-order sum of the S partials of my R rows + fused epilogue =======
-        // scratch aliases pipeline stage 0: every TMA write / MMA read of this CTA's stages has retired (tmem_full), and
-        // peers only ever write into `red`.  (Static __shared__ here would cost the second resident CTA per SM.)
+        // scratch aliases pipeline stage 0: every TMA write / MMA read of this CTA's stages has retired (both warpgroups
+        // sent their partials after their last wgmma completed), and peers only ever write into `red`.  (Static __shared__ here would cost the second resident CTA per SM.)
         float* s_mean = reinterpret_cast<float*>(smem);
         float* s_rstd = s_mean + GEMM_BM;
         float (*s_part_all)[4][4][2] = reinterpret_cast<float (*)[4][4][2]>(s_rstd + GEMM_BM);
         const int q = warp & 3;
-        const int half = (warp - 2) >> 2;
+        const int half = (warp - 4) >> 2;
         float (*s_part)[4][2] = s_part_all[half];
         const int ml = q * 32 + lane;
-        const int et = static_cast<int>(threadIdx.x) - 64;  // index among the epilogue threads
+        const int et = static_cast<int>(threadIdx.x) - 128; // index among the epilogue threads
         const int m = m0 + ml;
         const int R = BPAD / S;
         const bool valid_m = m < Nout;
@@ -485,14 +458,10 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 else asm volatile("bar.sync 3, 128;" ::: "memory");
             }
         }
-        if (threadIdx.x == 64) tl_mark(0x160 + ep.mode);
+        if (threadIdx.x == 128) tl_mark(0x160 + ep.mode);
     }
     __syncthreads();
     if (threadIdx.x == 0) { tl_mark(0x130 + ep.mode); tl_mark_all(0x130 + ep.mode); }
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, BN < 32 ? 32 : BN);
-    }
 }
 
 void gemm_timeline_set(unsigned long long* buf, unsigned int* cnt) {
@@ -502,7 +471,7 @@ void gemm_timeline_set(unsigned long long* buf, unsigned int* cnt) {
 
 // ---------------------------------------------------------------------------------------------------
 // Bring-up / cross-check kernel: same contract on CUDA cores (one warp per output feature, no split).
-// Selected with VCB_GEMM_IMPL=simt; never the default.  It exists so a tcgen05 descriptor bug can be told
+// Selected with VCB_GEMM_IMPL=simt; never the default.  It exists so a wgmma descriptor bug can be told
 // apart from a bug anywhere else in the step.
 // ---------------------------------------------------------------------------------------------------
 // element (m, k) of the pre-tiled weight layout
@@ -702,7 +671,8 @@ int gemm_launch(const GemmCall& g, cudaStream_t st) {
     }
     const int total_kb = g.Kdim / GEMM_BK;
     const int kbps = (total_kb + g.splits - 1) / g.splits;
-    if (g.splits < 1 || g.splits > 8 || (g.splits & (g.splits - 1)) || g.bpad % g.splits ||
+    // (g.bpad / g.splits >= 2: the reduce-scatter sends pairs of adjacent token rows to one owner)
+    if (g.splits < 1 || g.splits > 8 || (g.splits & (g.splits - 1)) || g.bpad % g.splits || g.bpad / g.splits < 2 ||
         (g.splits - 1) * kbps >= total_kb) {
         set_error("gemm: bad split count %d for %d k-blocks, bpad %d", g.splits, total_kb, g.bpad);
         return -1;
@@ -721,9 +691,8 @@ int gemm_launch(const GemmCall& g, cudaStream_t st) {
     }
 }
 
-// Cluster size (= K splits), a power of two <= 8.  Measured on B200 (scripts/bench_gemm.py, profiles/r01_gemm_micro.txt):
-// the kernel has a ~7 us latency floor, so the grid should reach >= ~1.3 CTAs per SM in ONE wave of co-resident CTAs
-// (2 per SM) while every split keeps >= 4 k-blocks.
+// Cluster size (= K splits), a power of two <= 8: the kernel has a latency floor of several microseconds, so the grid
+// should reach about one CTA per SM in ONE wave of co-resident CTAs (2 per SM) while every split keeps >= 4 k-blocks.
 int gemm_pick_splits(int Nout, int Kdim, int num_sms) {
     const int tiles = (Nout + GEMM_BM - 1) / GEMM_BM;
     const int total_kb = Kdim / GEMM_BK;

@@ -51,7 +51,7 @@ using namespace vcb;
 struct vcb_engine {
     vcb_config cfg;
     ModelDims m;
-    int num_sms = 148;
+    int num_sms = 132;
     int kv_fp32 = 0;
     int max_pages_per_slot = 0, n_pages = 0;
     std::vector<int> free_pages;
@@ -266,8 +266,8 @@ int run_gemm(vcb_engine* e, const Matrix& W, const CUtensorMap* tmB, const __nv_
     g.splits = gemm_pick_splits(W.rows, kdim, e->num_sms);
     for (const auto& o : e->opt_splits)          // experiment knob VCB_SPLITS="<N>x<K>:<S>,..."
         if (o[0] == W.rows && o[1] == kdim) g.splits = o[2];
-    // >= 64 rows: the per-CTA epilogue / DSMEM exchange grows with the rows, so half the cluster size wins
-    // (scripts/bench_gemm.py at B = 64 / 128: QKV 22.4 -> 17.5 us, out 16.4 -> 10.9, FFN1 23.0 -> 18.0, FFN2 25.4 -> 19.7 at B = 64)
+    // >= 64 rows: the per-CTA epilogue / DSMEM exchange grows with the rows, so a smaller cluster pays off (compare with
+    // scripts/bench_gemm.py, which times the decode GEMMs at a given split count)
     if (bpad >= 64 && g.splits > 1) g.splits /= 2;
     if (e->opt_gemm_maxctas > 0) {          // experiment knob: keep every GEMM to one CTA per SM (PDL ping-pong)
         const int tiles = (W.rows + 127) / 128;
@@ -300,8 +300,8 @@ int launch_attn_hd(vcb_engine* e, const Layer& Ly, int rows, int bpad, int max_c
     const int per_sm = std::max(1, std::min(4, (227 * 1024) / (L::TOTAL + 1024)));
     int grid = std::min(n_rh * nch, e->num_sms * per_sm);
     if (e->opt_att_balance) {
-        // equal item counts per CTA: 512 items on 296 CTAs would leave 80 CTAs idle for the whole second pass and the
-        // kernel finishing at the pace of the 2-item CTAs; 256 CTAs x 2 items keep every stream alive until the end
+        // equal item counts per CTA: with a few more items than CTAs, most CTAs would idle through the second pass while
+        // the kernel finishes at the pace of the 2-item CTAs; fewer CTAs with the same item count each stay busy to the end
         const int items = n_rh * nch, passes = (items + grid - 1) / grid;
         grid = (items + passes - 1) / passes;
     }
@@ -875,8 +875,8 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
     VCB_CUDA_OK(cudaSetDevice(cfg->device));
     cudaDeviceProp prop;
     VCB_CUDA_OK(cudaGetDeviceProperties(&prop, cfg->device));
-    if (prop.major != 10) {
-        set_error("libvcb200 is built for sm_100a only; device %d is sm_%d%d", cfg->device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        set_error("libvcb200 is built for sm_90a only; device %d is sm_%d%d", cfg->device, prop.major, prop.minor);
         return -2;
     }
     vcb_engine* e = new vcb_engine();
@@ -1471,7 +1471,7 @@ int vcb_debug_gemm(const float* W_dev, const float* X_dev, float* out_dev, int32
     }
     __nv_bfloat16 *w = nullptr, *x = nullptr;
     float* zb = nullptr;
-    int num_sms = 148;
+    int num_sms = 132;
     cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, 0);
     if (splits <= 0) splits = gemm_pick_splits(N, Kd, num_sms);
     while (splits > 1 && bpad % splits) splits /= 2;
@@ -1531,7 +1531,7 @@ int vcb_bench_gemm(int32_t N, int32_t Kd, int32_t B, int32_t splits, int32_t sta
     const int bpad = bpad_for(B);
     __nv_bfloat16 *w = nullptr, *x = nullptr;
     float *zb = nullptr, *out = nullptr;
-    int num_sms = 148;
+    int num_sms = 132;
     cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, 0);
     if (splits <= 0) splits = gemm_pick_splits(N, Kd, num_sms);
     while (splits > 1 && bpad % splits) splits /= 2;

@@ -1,4 +1,4 @@
-// Device kernels of the codec-LM decode path (everything except the tcgen05 GEMM).
+// Device kernels of the codec-LM decode path (everything except the tensor-core GEMMs).
 // All of them are HBM/L2-bound integer or fp32 work: coalesced 16-byte accesses, warp-level reductions,
 // TMA bulk copies for the paged KV cache.  Included only by lm_engine.cu.
 #pragma once
@@ -201,7 +201,7 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
 
 // Persistent, warp-specialised version: grid = a few CTAs per SM; each CTA walks a static list of work items
 // (row*head, context chunk).  Warp 4 is the TMA producer: it runs ahead ACROSS items, so the HBM stream never drains
-// at an item boundary (short CTAs with a cold start were the measured loss: 45% DRAM utilisation in ncu).
+// at an item boundary (short CTAs with a cold start leave HBM idle).
 // Warps 0..ATT_CWARPS-1 consume pages: scores -> online softmax -> PV, release the stage through an mbarrier.
 template <typename KVT, int HD>
 __global__ void __launch_bounds__(ATT_THREADS + 32)
@@ -452,7 +452,7 @@ step_prep_kernel(const int* __restrict__ slots, int n, SlotState* __restrict__ s
             split_bf16(gamma0[c] * v, hi, lo);
             act[static_cast<size_t>(r) * d + c] = hi;
             act[static_cast<size_t>(r + bpad) * d + c] = lo;
-            if (act_tiled) {       // persistent step kernel: the same operand as the pre-swizzled image of its UMMA tiles (mega_step.cu)
+            if (act_tiled) {       // persistent step kernel: the same operand as the pre-swizzled image of its MMA tiles (mega_step.cu)
                 const int kk = c & 63, rows2 = 2 * bpad;
                 const size_t t0 = static_cast<size_t>(c >> 6) * rows2;
                 act_tiled[(t0 + r) * 64 + ((((kk >> 3) ^ (r & 7)) << 3) | (kk & 7))] = hi;

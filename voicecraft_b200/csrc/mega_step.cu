@@ -2,9 +2,8 @@
 // x L, then the logit heads) in ONE launch on a grid of one CTA per SM.  (transformer.py:321-329, 473-488; activation.py:536-638;
 // voicecraft.py:181-185, 1085-1087.)
 //
-// Why (profiles/r01_timeline_all_v4.txt, VERDICT r01 item 3): as 84 separate kernels the step is latency-chain bound -- every
-// GEMM stops the HBM stream for a launch boundary, a pipeline ramp and an epilogue tail; 66 GEMM launches ran at 0.33 of the
-// HBM roofline.  Neither the weights nor the cached K/V pages depend on the activations of the step, so here ONE producer
+// Why: as 84 separate kernels the step is a latency chain -- every GEMM stops the HBM stream for a launch boundary, a
+// pipeline ramp and an epilogue tail.  Neither the weights nor the cached K/V pages depend on the activations of the step, so here ONE producer
 // thread per SM streams them, in schedule order, through a single ring of 16 KB shared-memory slots and never waits for
 // anything but a free slot: while a phase's dependency chain (flag -> activation tiles -> MMA -> split-K reduce -> epilogue
 // -> flag) resolves, the ring already fills with the next phases' weight blocks / KV slabs.
@@ -12,9 +11,9 @@
 //   * work split ("stream-K"): a GEMM phase is the list of its 16 KB weight blocks (tile-major, k-minor); an attention
 //     phase is the list of (row, head, page) units.  CTA c takes the contiguous range [c*T/G, (c+1)*T/G) of either list:
 //     every SM streams the same number of bytes (+-1 block) per phase, whatever the matrix shape or the context lengths.
-//   * roles: warp 0 ring producer (weights + K/V, TMA), warp 1 MMA issuer (tcgen05, fp32 accumulators in TMEM, 4 stages),
-//     warp 2 activation (B operand) producer -- the only one that waits for the previous phase --, warps 4..11 workers
-//     (GEMM epilogues / attention math).
+//   * roles: warp 0 ring producer (weights + K/V, TMA), warp 2 activation (B operand) producer -- the only one that waits
+//     for the previous phase --, warp 3 L2 prefetcher, warps 4..11 workers: two warpgroups that multiply a GEMM tile
+//     (wgmma, 64 features each, fp32 accumulators in registers) and run its epilogue, or do the attention math.
 //   * split-K without clusters: a CTA's partial of a tile goes to an L2-resident workspace; the last CTA to arrive
 //     (atomic counter) sums all partials in contributor order (deterministic) and runs the fused epilogue of
 //     gemm_tcgen05.cu (QKV append, residual + next LayerNorm operand and statistics, ReLU/GELU, logits).
@@ -32,13 +31,11 @@
 namespace vcb {
 
 static constexpr int MG_THREADS = 384;
-static constexpr int MG_WORKERS = 256;
 static constexpr int MG_SLOT = 16384;          // ring slot = one 128 x 64 bf16 weight block = one bf16 K (or V) slab
 static constexpr int MG_NS_MAX = 13;           // ring slots (MegaArgs::ns of them are used)
 static constexpr int MG_NB_MAX = 8;            // activation (B operand) ring slots (MegaArgs::nb)
 static constexpr int MG_POOL = 14 * 16384;     // bytes shared by the two rings: ns * 16 KB + nb * 8 KB <= MG_POOL
 static constexpr int MG_BSLOT = 8192;          // 64 rows (32 hi + 32 lo) x 64 k, bf16
-static constexpr int MG_NACC = 4;              // TMEM accumulator stages
 static constexpr int MG_HD = 128;
 static constexpr int MG_PAGE = 64;
 static constexpr int MG_CHUNK = 4;             // attention: pages per work item (a chunk of one (row, head))
@@ -48,8 +45,8 @@ static constexpr int MG_PSTR = 132;            // floats per page partial: acc[1
 struct MegaSmem {
     static constexpr int RING = 0;                                  // ns slots, then the B ring (attention scratch aliases it)
     static constexpr int BAR = MG_POOL;
-    static constexpr int NBAR = 2 * MG_NS_MAX + 2 * MG_NB_MAX + 2 * MG_NACC;
-    static constexpr int MISC = BAR + NBAR * 8;                    // tmem slot, flags, producer progress, page-count table
+    static constexpr int NBAR = 2 * MG_NS_MAX + 2 * MG_NB_MAX;
+    static constexpr int MISC = BAR + NBAR * 8;                    // flags, producer progress, page-count table
     static constexpr int TOTAL = MISC + 32 + 34 * 4 + 64;
     // attention scratch, aliased onto the B ring (idle during an attention phase)
     static constexpr int A_STATE = 0;                               // per-warp chunk states [8][MG_PSTR] floats
@@ -98,7 +95,7 @@ __device__ __forceinline__ void mg_wait(uint64_t* bar, uint32_t parity, unsigned
 }
 // Bounded wait for a phase completion counter.  The spin uses relaxed (L1-bypassing) loads and ONE acquire fence at the
 // end: an ld.acquire.gpu in the loop invalidates the SM's L1 on every iteration (CCTL.IVALL), which turned every
-// descriptor / bias read of the epilogue warps on the same SM into an L2 round trip (measured: ~18 us per phase).
+// descriptor / bias read of the epilogue warps on the same SM into an L2 round trip.
 __device__ __forceinline__ void mg_wait_flag(const unsigned int* flag, unsigned int target, unsigned int* dbg, unsigned int role,
                                              unsigned int phase) {
     unsigned long long t0 = 0;
@@ -186,8 +183,8 @@ __device__ __forceinline__ size_t mg_act_off(int k, int row, int rows2) {
 // ------------------------------------------------------------------------------------------------------------------------
 // Split-K hand-over of one output tile, reduce-scatter through L2: every CTA that contributed a partial of the tile
 // ("contributor" s = 0 .. S-1 in CTA order = ascending k) takes the token rows [s*BPAD/S, (s+1)*BPAD/S), sums the S partials
-// of those rows in contributor order (deterministic) and runs the fused epilogue on them.  (A single "last arriver"
-// reading all S x 16 KB through one SM's L2 port was measured at 3.5 us for S = 10.)
+// of those rows in contributor order (deterministic) and runs the fused epilogue on them.  (A single "last arriver" would
+// read all S x 16 KB partials through one SM's L2 port.)
 // Thread mapping: lane -> features 4*lane .. 4*lane+3 of the tile; warp wq -> rows row_begin + wq + 8j.
 // mg_epi_prefetch loads everything that does not depend on the other contributors (issued BEFORE waiting for them).
 // ------------------------------------------------------------------------------------------------------------------------
@@ -408,8 +405,7 @@ __device__ __forceinline__ void mg_load_kv(const KVT* p, float (&out)[N]) {
 
 template <int BPAD, typename KVT>
 __global__ void __launch_bounds__(MG_THREADS, 1) mega_step_kernel(const __grid_constant__ MegaArgs A) {
-    constexpr int BN = 2 * BPAD;                          // UMMA N: hi rows + lo rows
-    constexpr int HB = BPAD / 2;                          // rows per worker group in the TMEM read-out
+    constexpr int BN = 2 * BPAD;                          // MMA N: hi rows + lo rows
     constexpr int B_BYTES = BN * 64 * 2;
     constexpr int TPS = MG_SLOT / (MG_HD * static_cast<int>(sizeof(KVT)));   // tokens per ring slot: 64 (bf16) / 32 (fp32)
     constexpr int NSL = MG_PAGE / TPS;                    // ring slots per K (or V) slab
@@ -422,9 +418,6 @@ __global__ void __launch_bounds__(MG_THREADS, 1) mega_step_kernel(const __grid_c
     uint64_t* empty = full + MG_NS_MAX;
     uint64_t* bfull = empty + MG_NS_MAX;
     uint64_t* bempty = bfull + MG_NB_MAX;
-    uint64_t* accfull = bempty + MG_NB_MAX;
-    uint64_t* accempty = accfull + MG_NACC;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + L::MISC);
     int* s_flag = reinterpret_cast<int*>(smem + L::MISC + 8);
     volatile uint32_t* s_prod = reinterpret_cast<volatile uint32_t*>(smem + L::MISC + 16);   // ring items issued so far
     int* s_cum = reinterpret_cast<int*>(smem + L::MISC + 32);           // [33] prefix sum of pages per row
@@ -436,15 +429,11 @@ __global__ void __launch_bounds__(MG_THREADS, 1) mega_step_kernel(const __grid_c
     if (threadIdx.x == 0) {
         for (uint32_t i = 0; i < MG_NS; ++i) {
             mbar_init(&full[i], 1);
-            mbar_init(&empty[i], 8);          // weights: 7 lanes of the MMA warp + its commit; K/V slabs: the 8 worker warps
+            mbar_init(&empty[i], 8);          // the 8 worker warps (weights: after their MMAs; K/V slabs: after the math)
         }
         for (uint32_t i = 0; i < MG_NB; ++i) {
             mbar_init(&bfull[i], 1);
-            mbar_init(&bempty[i], 1);
-        }
-        for (int i = 0; i < MG_NACC; ++i) {
-            mbar_init(&accfull[i], 1);
-            mbar_init(&accempty[i], 8);
+            mbar_init(&bempty[i], 8);
         }
         mbar_fence_init();
         *s_prod = 0u;
@@ -456,21 +445,13 @@ __global__ void __launch_bounds__(MG_THREADS, 1) mega_step_kernel(const __grid_c
         }
         s_cum[32] = c;
     }
-    if (warp == 1) {
-        tmem_alloc(tmem_slot, 512);
-        tmem_relinquish();
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const long long U = static_cast<long long>(A.H) * s_cum[32];     // attention units of this step
     int u0, u1;
     const int Ue = mg_eff(U, G);
     mg_range(U, cta, Ue, u0, u1);
     u0 = mg_chunk_align(s_cum, A.H, u0, U);            // a CTA owns the chunks that START in its share of the units
     u1 = mg_chunk_align(s_cum, A.H, u1, U);
-    const int att_items = (u1 - u0) * 2 * NSL;                        // ring items of one attention phase (this CTA)
 
     if (warp == 0) {
         // ===== ring producer: weight blocks and K/V slabs of every phase, in schedule order ==============================
@@ -483,9 +464,8 @@ __global__ void __launch_bounds__(MG_THREADS, 1) mega_step_kernel(const __grid_c
                 if (it >= MG_NS) mg_wait(&empty[s], ((it / MG_NS) - 1) & 1, A.dbg, 0, p);
                 // Bound the loads IN FLIGHT (issued, not landed), not just the ring's capacity: this SM's memory pipe serves
                 // requests roughly in order, so the activation tiles / partials a phase hand-over is waiting for queue behind
-                // whatever the ring still has outstanding (11 x 16 KB at this SM's ~44 GB/s HBM share = 4 us of backlog;
-                // measured as ~0.6 us per activation tile).  `flight` x 16 KB keeps HBM saturated (Little: ~45 KB per SM)
-                // while landed slots still pile up to the ring's depth during a dependency chain.
+                // whatever the ring still has outstanding.  `flight` x 16 KB in flight keeps HBM busy while landed slots
+                // still pile up to the ring's depth during a dependency chain.
                 while (it - landed >= flight) {
                     mg_wait(&full[landed % MG_NS], (landed / MG_NS) & 1, A.dbg, 9, p);
                     ++landed;
@@ -543,50 +523,6 @@ __global__ void __launch_bounds__(MG_THREADS, 1) mega_step_kernel(const __grid_c
                     }
                 }
                 mg_tl(A, p, 7);
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer ========================================================================================================
-        constexpr uint32_t idesc = umma_idesc_bf16_f32(128, BN);
-        uint32_t it = 0, bit = 0, seg = 0;
-        for (int p = 0; p < A.nph; ++p) {
-            const MegaPhase& P = ph[p];
-            if (P.type != MEGA_GEMM) {
-                it += att_items;
-                continue;
-            }
-            const long long T = static_cast<long long>(P.groups) * P.tiles_per_group * P.kb;
-            int b0, b1;
-            const int Ge = mg_eff(T, G);
-                    mg_range(T, cta, Ge, b0, b1);
-            int blk = b0;
-            while (blk < b1) {
-                const int tile = blk / P.kb;
-                const int seg_end = min(b1, (tile + 1) * P.kb);
-                const int stage = seg % MG_NACC;
-                if (seg >= MG_NACC) mg_wait(&accempty[stage], ((seg / MG_NACC) - 1) & 1, A.dbg, 1, p);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + stage * BN;
-                for (bool first = true; blk < seg_end; ++blk, ++it, ++bit, first = false) {
-                    const int s = it % MG_NS, bs = bit % MG_NB;
-                    mg_wait(&full[s], (it / MG_NS) & 1, A.dbg, 1, p);
-                    mg_wait(&bfull[bs], (bit / MG_NB) & 1, A.dbg, 2, p);
-                    tc_fence_after();
-                    if (lane >= 1 && lane < 8) mbar_arrive(&empty[s]);      // 7 of the slot's 8 release arrivals
-                    if (lane == 0) {
-                        if (first && blk == b0) mg_tl(A, p, 5);
-                        const uint64_t a_desc = umma_desc_kmajor_sw128(smem_u32(ring + s * MG_SLOT));
-                        const uint64_t b_desc = umma_desc_kmajor_sw128(smem_u32(bring + bs * MG_BSLOT));
-#pragma unroll
-                        for (int k = 0; k < 4; ++k) umma_bf16(d_tmem, a_desc + 2 * k, b_desc + 2 * k, idesc, (first && k == 0) ? 0u : 1u);
-                        umma_commit(&empty[s]);                             // the 8th: when these MMAs have read the slot
-                        umma_commit(&bempty[bs]);
-                        if (blk == seg_end - 1) umma_commit(&accfull[stage]);
-                        if (blk == b1 - 1) mg_tl(A, p, 6);
-                    }
-                    __syncwarp();
-                }
-                ++seg;
             }
         }
     } else if (warp == 2) {
@@ -685,9 +621,9 @@ __global__ void __launch_bounds__(MG_THREADS, 1) mega_step_kernel(const __grid_c
         // ===== workers: GEMM epilogues / attention ========================================================================
         const int wtid = threadIdx.x - 128;             // 0..255
         const int wq = wtid >> 5;                        // worker warp 0..7
-        const int q = warp & 3;                          // TMEM lane quarter this warp may read
-        const int grp = wq >> 2;                         // which half of the rows in the TMEM read-out
-        uint32_t it = 0, seg = 0;
+        const int q = warp & 3;                          // warp inside its warpgroup
+        const int grp = wq >> 2;                         // worker warpgroup: features [64 grp, 64 grp + 64) of a tile
+        uint32_t it = 0, bit = 0;
         for (int p = 0; p < A.nph; ++p) {
             const MegaPhase& P = ph[p];
             if (P.type == MEGA_GEMM) {
@@ -700,43 +636,41 @@ __global__ void __launch_bounds__(MG_THREADS, 1) mega_step_kernel(const __grid_c
                 while (blk < b1) {
                     const int tile = blk / P.kb;
                     const int seg_end = min(b1, (tile + 1) * P.kb);
-                    it += seg_end - blk;
-                    blk = seg_end;
-                    const int stage = seg % MG_NACC;
-                    mg_wait(&accfull[stage], (seg / MG_NACC) & 1, A.dbg, 4, p);
-                    tc_fence_after();
-                    ++seg;
-                    if (wtid == 0) mg_tl(A, p, 1);
-                    // ---- TMEM -> registers: feature = TMEM lane, my group's half of the rows (hi + lo columns) ----------
-                    const uint32_t taddr = tmem_base + stage * BN + (static_cast<uint32_t>(q * 32) << 16);
-                    float v[HB];
-                    {
-                        float hi[16], lo[16];
-                        if constexpr (HB == 16) {
-                            tmem_ld_32x16(taddr + grp * HB, hi);
-                            tmem_ld_32x16(taddr + BPAD + grp * HB, lo);
+                    float acc[BN / 2];
 #pragma unroll
-                            for (int j = 0; j < 16; ++j) v[j] = hi[j] + lo[j];
-                        } else {
-                            // BPAD = 16: one 16-column load covers both groups' rows; each group keeps its 8
-                            tmem_ld_32x16(taddr, hi);
-                            tmem_ld_32x16(taddr + BPAD, lo);
-#pragma unroll
-                            for (int j = 0; j < HB; ++j) v[j] = grp ? hi[HB + j] + lo[HB + j] : hi[j] + lo[j];
+                    for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+                    for (; blk < seg_end; ++blk, ++it, ++bit) {
+                        const int s = it % MG_NS, bs = bit % MG_NB;
+                        mg_wait(&full[s], (it / MG_NS) & 1, A.dbg, 1, p);
+                        mg_wait(&bfull[bs], (bit / MG_NB) & 1, A.dbg, 2, p);
+                        wg_fence();
+                        wg_mma_kblock<BN>(acc, smem_u32(ring + s * MG_SLOT) + grp * 64 * 128, smem_u32(bring + bs * MG_BSLOT));
+                        wg_commit();
+                        wg_wait0();
+                        __syncwarp();
+                        if (lane == 0) {                             // this warp's MMAs have read both slots
+                            mbar_arrive(&empty[s]);
+                            mbar_arrive(&bempty[bs]);
                         }
                     }
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&accempty[stage]);
-                    // ---- my partial of this tile -> workspace [row][feature] ---------------------------------------------------
-                    const int ml = q * 32 + lane;
-                    float* pdst = A.part + (static_cast<size_t>(cta) * MEGA_MAXSEG + (tile - first_tile)) * BPAD * 128 + ml;
+                    wg_acc_fence(acc);
+                    if (wtid == 0) mg_tl(A, p, 1);
+                    // ---- my partial of this tile (hi + lo columns) -> workspace [row][feature] ---------------------------------
+                    float* pdst = A.part + (static_cast<size_t>(cta) * MEGA_MAXSEG + (tile - first_tile)) * BPAD * 128;
 #pragma unroll
-                    for (int j = 0; j < HB; ++j) __stcg(pdst + (grp * HB + j) * 128, v[j]);
+                    for (int jb = 0; jb < BPAD / 8; ++jb) {
+                        const int row = 8 * jb + 2 * (lane & 3);
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int f = grp * 64 + q * 16 + (lane >> 2) + 8 * e;
+                            __stcg(pdst + row * 128 + f, acc[4 * jb + 2 * e] + acc[4 * (jb + BPAD / 8) + 2 * e]);
+                            __stcg(pdst + (row + 1) * 128 + f, acc[4 * jb + 2 * e + 1] + acc[4 * (jb + BPAD / 8) + 2 * e + 1]);
+                        }
+                    }
                     // publish my partial: the block barrier orders every worker's stores before thread 0's GPU-scope fence
                     // (fences are cumulative), then count in.  ALL my partials of the phase go out before I wait for anybody:
                     // waiting per tile would chain the tiles (tile t+1's partial stuck behind the wait for tile t's last
-                    // contributor -- measured as a 48-tile domino, 60 us per phase).
+                    // contributor, a domino across the phase's tiles).
                     mg_bar_workers();
                     if (wtid == 0) {
                         __threadfence();
@@ -781,8 +715,7 @@ __global__ void __launch_bounds__(MG_THREADS, 1) mega_step_kernel(const __grid_c
                 // into V -- no block barrier per page.  Per chunk the 8 warp states fold in warp order, chunks fold in chunk
                 // order: every result is a fixed-order fold that depends only on the row's own context (a row's tokens do
                 // not depend on what else is in the batch).
-                // The page loop is ISSUE-bound on CUDA cores (measured: ~650 SASS instructions per page and warp took 1.5 us
-                // per page, twice the HBM time of the page), so it is written for instruction count:
+                // The page loop is issue-bound on CUDA cores rather than HBM-bound, so it is written for instruction count:
                 //   * 4 lanes per key (32 dims each): one pass of 4 x LDS.128 + 32 FMA covers the warp's 8 keys, 2 shuffles
                 //   * scores in the log2 domain: q is staged once per chunk as q * (scale * log2 e), probabilities are exp2
                 //   * the current position's key / value (from this step's QKV epilogue, not from the page) is ONE extra key
@@ -1045,12 +978,6 @@ __global__ void __launch_bounds__(MG_THREADS, 1) mega_step_kernel(const __grid_c
                 }
             }
         }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
     }
 }
 

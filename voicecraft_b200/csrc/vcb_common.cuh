@@ -1,5 +1,5 @@
-// Common device helpers for the sm_100a kernels: mbarrier / TMA / tcgen05 PTX wrappers, small math utils.
-// Everything here is hand-written PTX for Blackwell (no CUTLASS dependency).
+// Common device helpers for the sm_90a kernels: mbarrier / TMA / wgmma PTX wrappers, small math utils.
+// Everything here is hand-written PTX for Hopper (no CUTLASS dependency).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -103,7 +103,7 @@ __device__ __forceinline__ void tma_bulk_g2s(void* smem_dst, const void* gsrc, u
 }
 
 // L2 cache policies / prefetch.  Streams that are touched once per step (KV pages, weight tiles) are loaded with
-// evict_first so they do not push the *prefetched* next-kernel weights out of the 126 MB L2.
+// evict_first so they do not push the *prefetched* next-kernel weights out of the 50 MB L2.
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {
     uint64_t p;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
@@ -147,8 +147,8 @@ static __constant__ unsigned long long* g_tl_buf = nullptr;   // constant bank: 
 static __constant__ unsigned int* g_tl_cnt = nullptr;
 __device__ __forceinline__ void tl_mark(unsigned int tag) {
 #ifndef VCB_TIMELINE
-    (void)tag;                                   // compiled out by default: even the disabled check costs 2.7 % of a decode step
-    return;                                      // (profiles/r02_exp_timeline_marks.json); `make TIMELINE=1` builds it in
+    (void)tag;                                   // compiled out by default: even the disabled check is a load per mark on the
+    return;                                      // latency-bound decode chain; `make TIMELINE=1` builds it in
 #endif
     if (g_tl_buf != nullptr && blockIdx.x == 0 && blockIdx.y == 0) {
         unsigned long long t;
@@ -183,89 +183,75 @@ __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;"
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, TMEM load
+// wgmma (sm_90a): one warpgroup (4 aligned warps) computes D[64 x N] += A[64 x 16] * B[N x 16]^T, both operands K-major
+// in shared memory, fp32 accumulators in registers.  Accumulator fragment of thread t of the warpgroup (warp w = t / 32,
+// lane l): for every 8-column block j, d[4j + 0..1] = row 16w + l/4, columns 8j + 2(l%4) + 0..1, and d[4j + 2..3] = the
+// same columns of row 16w + l/4 + 8.
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc];  bf16 inputs, fp32 accumulate, single-CTA
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// all but the most recent group complete: the MMAs of k-block i run while k-block i+1 is issued
+__device__ __forceinline__ void wg_wait1() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
+// orders every later use of the accumulators after wg_wait0() (the asm outputs of wgmma are only valid once it returns)
+template <int N>
+__device__ __forceinline__ void wg_acc_fence(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// 32 lanes x 32 columns of fp32: thread t of the warp receives lane (base_lane + t), columns [col, col+32)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, float (&v)[32]) {
-    uint32_t r[32];
+__device__ __forceinline__ void wgmma_m64n16(float* d, uint64_t a_desc, uint64_t b_desc) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a_desc), "l"(b_desc));
 }
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, float (&v)[16]) {
-    uint32_t r[16];
+__device__ __forceinline__ void wgmma_m64n32(float* d, uint64_t a_desc, uint64_t b_desc) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a_desc), "l"(b_desc));
+}
+__device__ __forceinline__ void wgmma_m64n64(float* d, uint64_t a_desc, uint64_t b_desc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc));
 }
 
 // K-major operand tile in shared memory, rows of 128 bytes (64 bf16), 128B swizzle (what TMA SWIZZLE_128B writes):
-// 8-row x 128B swizzle atoms, atoms stacked every 1024 B.  Descriptor layout = cute::UMMA::SmemDescriptor (sm100):
-//   [0,14) start>>4 | [16,30) LBO>>4 (unused for swizzled K-major) | [32,46) SBO>>4 | [46,48) version=1 |
-//   [61,64) layout (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw128(uint32_t smem_addr) {
+// 8-row x 128B swizzle atoms, atoms stacked every 1024 B.  sm_90 matrix descriptor:
+//   [0,14) start>>4 | [16,30) LBO>>4 (unused for swizzled K-major) | [32,46) SBO>>4 | [62,64) layout (1 = SWIZZLE_128B)
+// Advancing 16 K-elements inside the swizzle row is +32 B = +2 on the start field; 64 rows further is +8192 B.
+__device__ __forceinline__ uint64_t gmma_desc_kmajor_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
     d |= static_cast<uint64_t>(1) << 16;                       // LBO (ignored), canonical value 1
     d |= static_cast<uint64_t>(1024 >> 4) << 32;               // SBO: 8 rows * 128 B
-    d |= static_cast<uint64_t>(1) << 46;                       // descriptor version (Blackwell)
-    d |= static_cast<uint64_t>(2) << 61;                       // SWIZZLE_128B
+    d |= static_cast<uint64_t>(1) << 62;                       // SWIZZLE_128B
     return d;
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor) for kind::f16: bf16 x bf16 -> fp32, both K-major.
-__host__ __device__ constexpr uint32_t umma_idesc_bf16_f32(int M, int N) {
-    return (1u << 4)                                  // c_format = F32
-           | (1u << 7)                                // a_format = BF16
-           | (1u << 10)                               // b_format = BF16
-           | (static_cast<uint32_t>(N >> 3) << 17)    // n_dim
-           | (static_cast<uint32_t>(M >> 4) << 24);   // m_dim
+
+// D[64 x N] += A[64 rows at a_addr] * B[N rows at b_addr]^T over one 64-wide k-block (4 x k16), N issued in pieces of at
+// most 64 columns.  Called by all 128 threads of a warpgroup between wg_fence() and wg_commit().
+template <int N>
+__device__ __forceinline__ void wg_mma_kblock(float (&d)[N / 2], uint32_t a_addr, uint32_t b_addr) {
+    static_assert(N % 16 == 0 && (N <= 64 || N % 64 == 0), "N: 16, 32, 64 or a multiple of 64");
+    constexpr int NC = N < 64 ? N : 64;
+    const uint64_t a = gmma_desc_kmajor_sw128(a_addr), b = gmma_desc_kmajor_sw128(b_addr);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+#pragma unroll
+        for (int n0 = 0; n0 < N; n0 += NC) {
+            const uint64_t bk = b + static_cast<uint64_t>(n0 * 8) + 2 * k;     // n0 rows * 128 B, >> 4
+            if constexpr (NC == 64) wgmma_m64n64(d + n0 / 2, a + 2 * k, bk);
+            else if constexpr (NC == 32) wgmma_m64n32(d + n0 / 2, a + 2 * k, bk);
+            else wgmma_m64n16(d + n0 / 2, a + 2 * k, bk);
+        }
+    }
 }
 
 }  // namespace vcb

@@ -32,7 +32,7 @@ struct GemmEpilogue {
     float* out = nullptr;
     int ld_out = 0, col_off = 0, act_kind = 0, bpad_out = 0;
     // LayerNorm folded into this GEMM (the B operand is gamma*x, not LN(x)):
-    //   y = rstd[row] * (acc - mean[row] * cvec[m]) + bias[m]   with bias := b + W.beta, cvec := W.gamma   (DESIGN.md section 4)
+    //   y = rstd[row] * (acc - mean[row] * cvec[m]) + bias[m]   with bias := b + W.beta, cvec := W.gamma   (DESIGN.md section 4.1)
     int ln_fold = 0, stats_tiles = 0;
     const float* cvec = nullptr;
     const float* stats = nullptr;         // [tile][STATS_ROWS][2] partial (sum x, sum x^2) written by the producer
@@ -71,7 +71,7 @@ struct MegaPhase {
     int done_target = 0;                      // completions that finish this phase (tiles, or CTAs for ATTN)
 };
 struct MegaArgs {
-    // Activation (B) operands: 0 act_d, 1 act_d2, 2 act_f, 3 act_h, each stored as the shared-memory IMAGE of its UMMA tiles:
+    // Activation (B) operands: 0 act_d, 1 act_d2, 2 act_f, 3 act_h, each stored as the shared-memory IMAGE of its MMA tiles:
     // [K/64 k-blocks][2*bpad rows (hi rows, then lo rows)][64] bf16 with the 128-byte swizzle already applied (16-byte chunk c
     // of row r sits at chunk c ^ (r & 7)), so a tile is one contiguous 2*bpad*128-byte bulk copy -- no tensor map, no 64
     // scattered 128-byte rows per tile (see mg_act_off in mega_step.cu).

@@ -50,7 +50,7 @@ def is_gemm_weight(key):
 
 def make_state_dict(cfg, seed=0, bf16_exact=True, logit_scale=2.0, dtype=torch.float32):
     """Random checkpoint with the reference's keys.  ``bf16_exact`` rounds the GEMM matrices to
-    bf16-representable fp32 values, so an fp32 reference run and the bf16-weight B200 path see
+    bf16-representable fp32 values, so an fp32 reference run and the bf16-weight H100 path see
     identical weights."""
     g = torch.Generator(device="cpu").manual_seed(seed)
     K, D, H, L = cfg.n_codebooks, cfg.d_model, cfg.nhead, cfg.num_decoder_layers

@@ -4,7 +4,7 @@
 reference's ``[(codes[1,K,T], None)]`` and returns the waveform ``[1, channels, T*hop]``; ``encode(wav[1,C,N])`` returns the
 reference's ``[(codes[1,K,T], None)]`` (:127-129).  Instead of audiocraft's ``CompressionSolver.model_from_checkpoint`` +
 ``EncodecModel.decode / encode`` (:109-110, :128, :133) the weights are handed to libvcb200.so, which runs RVQ and the
-SEANet decoder / encoder as sm_100a kernels.  No PyTorch / CPU fallback.  The text tokenizer (espeak) is out of scope.
+SEANet decoder / encoder as sm_90a kernels.  No PyTorch / CPU fallback.  The text tokenizer (espeak) is out of scope.
 """
 import ctypes as C
 from types import SimpleNamespace
@@ -127,7 +127,7 @@ class AudioTokenizer:
         if self._eng is not None:
             return self._eng
         if self._device.type != "cuda":
-            raise _lib.VcbError("AudioTokenizer (B200) has no CPU path: construct it with a CUDA device")
+            raise _lib.VcbError("AudioTokenizer (H100) has no CPU path: construct it with a CUDA device")
         lib = _lib.load()
         c = self.config
         cfg = _codec_lib.enc_config(n_q=c.n_q, bins=c.bins, dimension=c.dimension, n_filters=c.n_filters,

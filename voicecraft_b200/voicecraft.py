@@ -1,11 +1,11 @@
-"""B200-native drop-in for the inference surface of the reference's ``models/voicecraft.py``.
+"""H100-native drop-in for the inference surface of the reference's ``models/voicecraft.py``.
 
 Same constructor (``VoiceCraft(args)`` / ``VoiceCraft(config=dict)``), same ``state_dict`` keys, same
 ``inference_tts`` / ``inference_tts_batch`` / ``inference`` signatures and return shapes
 (reference models/voicecraft.py:97-121, 561-573, 908-920, 1156-1169).  The module only *holds* the
-parameters; every inference call goes through libvcb200.so (hand-written sm_100a kernels: paged-KV
-attention, tcgen05 GEMMs, fused sampler).  There is no PyTorch / CPU fallback: without the extension or
-without a Blackwell GPU the calls raise.
+parameters; every inference call goes through libvcb200.so (hand-written sm_90a kernels: paged-KV
+attention, wgmma GEMMs, fused sampler).  There is no PyTorch / CPU fallback: without the extension or
+without an H100 (sm_90) GPU the calls raise.
 
 Random numbers: the reference samples with ``torch.multinomial(softmax(l), 1)``, which ATen evaluates as
 ``argmax(softmax(l) / q)`` with ``q = empty_like(p).exponential_(1)`` from the device's global generator.
@@ -163,7 +163,7 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     # training surface: out of scope for this build (SURVEY.md section 8f)
     # ------------------------------------------------------------------------------------------------
     def forward(self, batch):
-        raise NotImplementedError("training forward is out of scope of the B200 decode engine "
+        raise NotImplementedError("training forward is out of scope of the H100 decode engine "
                                   "(reference models/voicecraft.py:472-559)")
 
     def prepare_mask_intervals(self, y_lens):
@@ -224,7 +224,7 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     def _engine(self, need_slots=1, need_seq=0):
         dev = self.mask_embedding.device
         if dev.type != "cuda":
-            raise _lib.VcbError("VoiceCraft (B200) has no CPU path: move the model to a CUDA device (`.to('cuda')`)")
+            raise _lib.VcbError("VoiceCraft (H100) has no CPU path: move the model to a CUDA device (`.to('cuda')`)")
         o = self._eng_opts
         held = sum(len(s.slots) for s in self._sessions if s._open)
         need_slots += held
