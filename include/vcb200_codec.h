@@ -44,7 +44,32 @@ int enc_decode(enc_engine* e, const int64_t* codes_dev, float* wav_dev, int32_t 
  * ResidualVectorQuantizer.encode).  Needs the "enc.*" weights: "enc.conv_in.weight", "enc.down{i}.res{j}.conv1.weight",
  * "enc.down{i}.conv.weight" (strided), "enc.lstm.*", "enc.conv_out.weight". */
 int enc_encode(enc_engine* e, const float* wav_dev, int64_t* codes_dev, int32_t B, int32_t N, void* stream);
-int64_t enc_counter(enc_engine* e, const char* name); /* "launches", "hop", "flops_per_frame", "tc_enabled", "tc_decodes" */
+/* "launches", "hop", "flops_per_frame", "tc_enabled", "tc_decodes", "stream_decodes", "stream_min_frames" (frames a fresh
+ * stream's first enc_stream_decode needs; -1 without the tensor-core decoder), "stream_state_bytes" (carried state per stream) */
+int64_t enc_counter(enc_engine* e, const char* name);
+
+/* Streaming decode: waveform chunk by chunk while the tokens are still being generated.  The decoder is causal, so a chunk
+ * only needs the left context the previous chunk ended with: for every layer that reads earlier rows, the last rows of its
+ * input (kept as the decoder keeps its activations), and the LSTM's (h, c).  With that state carried, the concatenated
+ * chunks are bit-identical to one enc_decode of the whole sequence.
+ *
+ * Synchronisation: enc_stream_decode checks the codes on the device and waits for that check, and copies a small per-call
+ * table to the device; the decode itself is asynchronous on `stream`.  One enc_stream is used from one CUDA stream, and the
+ * calls of one enc_engine (enc_decode, enc_stream_decode) must not overlap: they share its workspace. */
+typedef struct enc_stream enc_stream;
+/* state for up to max_streams concurrent utterances; fails where the tensor-core decoder does not cover the codec
+ * (non-causal codec, VCB_CODEC_TC=0, ...) */
+int enc_stream_create(enc_engine* e, int32_t max_streams, enc_stream** out);
+int enc_stream_destroy(enc_stream* s);
+/* the listed streams start over at frame 0 on their next decode */
+int enc_stream_reset(enc_stream* s, const int32_t* ids_host, int32_t n);
+/* codes [B][n_q][T] int64 (device) -> wav [B][channels][T*hop] fp32 (device).  Row b continues stream ids_host[b]:
+ * samples [0, lens_host[b]*hop) are the waveform of that stream's next lens_host[b] frames, bit-identical to the same
+ * samples of enc_decode over the stream's whole code sequence; later samples are unspecified.
+ * Rejected before any stream changes: an id outside [0, max_streams) or twice in the call, lens outside [1, T], a fresh
+ * stream's first call with fewer than "stream_min_frames" frames, any code (padding included) outside [0, bins). */
+int enc_stream_decode(enc_engine* e, enc_stream* s, const int32_t* ids_host, const int32_t* lens_host, int32_t B,
+                      const int64_t* codes_dev, int32_t T, float* wav_dev, void* stream);
 /* Debug / tests: an intermediate tensor of the last enc_decode on the tensor-core path ("z", "x0", "u0", "x1.raw", "x1.elu",
  * "h1.0", "o1.0", ...), reassembled from its bf16 (hi, lo) planes as fp32 [B][C][halo + T] on the host.  dims = {B, C, halo + T,
  * halo}; host_out == NULL only queries dims.  The up-sampling stages share two workspace arenas, so after a full decode only

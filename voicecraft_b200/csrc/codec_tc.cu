@@ -69,6 +69,7 @@ struct TcCall {
     __nv_bfloat16* hseq;               // planes [T+1][Bcap][H]; slot t+1 = h_t
     long long h_plane;
     int t_step, Bcap, H;
+    const int* stab;                   // stream decode: per utterance {id, valid frames, continuing, 0}; c frozen past its frames
     TcTap taps[TC_MAX_KB];
 };
 
@@ -190,8 +191,10 @@ __device__ __forceinline__ void tc_epilogue_lstm(const TcCall& c, int b, int n0,
         cs[u] = fg * cs[u] + ig * gg;
         h[u] = og * tanhf(cs[u]);
     }
+    if (c.stab == nullptr || c.t_step < c.stab[4 * b + 1]) {    // a stream's c stays at its last valid step
 #pragma unroll
-    for (int u = 0; u < U; u += 4) *reinterpret_cast<float4*>(cp + u) = make_float4(cs[u], cs[u + 1], cs[u + 2], cs[u + 3]);
+        for (int u = 0; u < U; u += 4) *reinterpret_cast<float4*>(cp + u) = make_float4(cs[u], cs[u + 1], cs[u + 2], cs[u + 3]);
+    }
     __nv_bfloat16* hp = c.hseq + (tb + c.Bcap) * c.H + j0;          // slot t+1
     const float* sk = c.elu != nullptr ? c.skip + tb * c.H + j0 : nullptr;
     __nv_bfloat16* op = c.elu != nullptr ? c.elu + (b * c.o_sb + c.t_step * c.o_st + c.o_off) * c.o_ld + j0 : nullptr;
@@ -413,6 +416,51 @@ tc_diag_sum_kernel(const float* __restrict__ P, int k, float bias, float* __rest
     out[static_cast<size_t>(b) * T + t] = acc;
 }
 
+// Stream decode: carry the left context of one plane across calls.  Block b = utterance b of the call, which continues
+// stream table[4b] with table[4b+1] valid frames (table[4b+2] = 1: the stream has decoded frames before).  Launched after the
+// plane's producer and before its consumer:
+//   restore  a continuing stream's halo rows t = -halo..-1 <- its saved tail (they replace the reflect / zero padding);
+//   save     the stream's saved tail <- rows [len*up - halo, len*up), which reach back into the restored halo when len*up < halo.
+// The saved tail is stored exactly as the plane stores it (bf16 hi and lo planes, or fp32), [plane][halo rows][row_bytes].
+// One block owns one stream (the ids of a call are distinct), and the block barrier orders reading the old tail before
+// writing the new one.
+struct CarryArgs {
+    uint8_t* base;                     // plane storage; the second plane (lo) at + plane_bytes (0: a single plane)
+    long long plane_bytes;
+    long long sb, st, off;             // row(b, t) = b*sb + t*st + off
+    int row_bytes;                     // multiple of 16
+    int halo, up;                      // rows carried; plane rows per frame
+    int restore, save;
+    const int* table;
+    uint8_t* state;
+    long long state_stride, state_off; // stream id's tail at state + id*state_stride + state_off
+};
+
+__global__ void __launch_bounds__(256) tc_carry_kernel(const __grid_constant__ CarryArgs a) {
+    pdl_launch_dependents();
+    pdl_wait();                                                     // the producer has written the plane
+    const int b = blockIdx.x;
+    const int id = a.table[4 * b], len = a.table[4 * b + 1], cont = a.table[4 * b + 2];
+    const int per_row = a.row_bytes / 16, per_plane = a.halo * per_row;
+    const int n = (a.plane_bytes ? 2 : 1) * per_plane;
+    uint4* s = reinterpret_cast<uint4*>(a.state + id * a.state_stride + a.state_off);
+    auto at = [&](int i, int t) {
+        const int p = i / per_plane, r = i - p * per_plane, col = r % per_row;
+        return reinterpret_cast<uint4*>(a.base + p * a.plane_bytes + (b * a.sb + t * a.st + a.off) * a.row_bytes) + col;
+    };
+    if (a.restore && cont)
+        for (int i = threadIdx.x; i < n; i += blockDim.x) *at(i, (i % per_plane) / per_row - a.halo) = s[i];
+    __syncthreads();
+    if (a.save)
+        for (int i = threadIdx.x; i < n; i += blockDim.x) s[i] = *at(i, len * a.up - a.halo + (i % per_plane) / per_row);
+}
+
+// codes outside [0, bins) -> *bad = 1
+__global__ void tc_codes_check_kernel(const long long* __restrict__ codes, long long n, int bins, int* bad) {
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x)
+        if (codes[i] < 0 || codes[i] >= bins) *bad = 1;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------------
@@ -472,6 +520,7 @@ struct TcCodec {
     size_t ws_bytes = 0;
     size_t ws_limit = 0;
     int min_T = 8;
+    size_t stream_bytes = 0;           // carried state of one stream (stream decode)
     bool profile = false;
     std::vector<std::pair<std::string, float>> prof;
     struct Dbg { Plane p; const __nv_bfloat16* ptr; int B; };
@@ -756,9 +805,10 @@ struct Prof {
     }
 };
 
-// One chunk of B utterances.  dry = only measure the workspace (returns bytes through *need).
+// One chunk of B utterances.  dry = only measure the workspace (returns bytes through *need).  sc = stream decode: every
+// plane a layer reads as left context, and the LSTM state, continue the utterance's stream (tc_carry_kernel).
 int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T, cudaStream_t st, int64_t* launches, bool dry,
-                    size_t* need) {
+                    size_t* need, const TcStreamCtx* sc) {
     const enc_config& cf = tc->cfg;
     const int Bcap = (B + 127) / 128 * 128;
     const int H = tc->ch0;
@@ -817,6 +867,45 @@ int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
         if (raw) p.raw = static_cast<__nv_bfloat16*>(b.take(plane_bytes(p, 1)));
         if (elu) p.elu = static_cast<__nv_bfloat16*>(b.take(plane_bytes(p, 1)));
     };
+    // stream decode: the state of a stream is laid out in the order the carries run (tc_stream_state_bytes is the total)
+    size_t soff = 0;
+    auto take_state = [&](size_t bytes) {
+        const size_t o = soff;
+        soff += bytes;
+        return o;
+    };
+    auto carry = [&](void* base, long long plane_bytes, long long sb, long long stt, long long off, int row_bytes, int halo, int up,
+                     int restore, int save, size_t state_off) -> int {
+        CarryArgs a;
+        a.base = static_cast<uint8_t*>(base);
+        a.plane_bytes = plane_bytes;
+        a.sb = sb; a.st = stt; a.off = off;
+        a.row_bytes = row_bytes;
+        a.halo = halo; a.up = up;
+        a.restore = restore; a.save = save;
+        a.table = sc->table;
+        a.state = sc->state;
+        a.state_stride = static_cast<long long>(tc->stream_bytes);
+        a.state_off = static_cast<long long>(state_off);
+        cudaLaunchConfig_t lc = {};
+        lc.gridDim = dim3(B);
+        lc.blockDim = dim3(256);
+        lc.stream = st;
+        cudaLaunchAttribute at[1];
+        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        at[0].val.programmaticStreamSerializationAllowed = 1;
+        lc.attrs = at;
+        lc.numAttrs = 1;
+        VCB_CUDA_OK(cudaLaunchKernelEx(&lc, tc_carry_kernel, a));
+        ++*launches;
+        return 0;
+    };
+    // a plane's halo: restore a continuing stream's tail over the padding the producer wrote, save the new tail
+    auto carry_plane = [&](const Plane& p, __nv_bfloat16* base, int up) -> int {
+        if (sc == nullptr || p.halo == 0) return 0;
+        const size_t o = take_state(static_cast<size_t>(p.halo) * p.C * 4);
+        return carry(base, p.plane() * 2, p.sb, p.st, p.off, p.C * 2, p.halo, up, 1, 1, o);
+    };
 
     Prof pf{tc, st};
     CUtensorMap mA, mB;
@@ -845,6 +934,7 @@ int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
                                                                  Z.plane(), cf.n_q, tc->D, Z.C, T, Z.Tp, Z.halo, Z.halo_zero);
     VCB_CUDA_OK(cudaGetLastError());
     ++*launches;
+    if (carry_plane(Z, Z.raw, 1)) return -1;
     pf.end();
     // ---- conv_in
     pf.begin("conv_in");
@@ -863,6 +953,7 @@ int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
         if (plane_map(&mA, Z.raw, Z)) return -1;
         if (tc_launch(tc, mA, mA, tc->conv_in, c, (Z.rcap + TC_BM - 1) / TC_BM, st)) return -1;
         ++*launches;
+        if (nl == 0 && carry_plane(U0, U0.elu, 1)) return -1;
     }
     pf.end();
     // ---- LSTM stack with skip
@@ -905,6 +996,18 @@ int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
                 c.skip = x0f;
                 set_out(c, U0, false, true);
             }
+            // stream decode: h_{-1} (slot 0) and c continue the stream; after the layer, h of the last valid step (slot
+            // frames) and the frozen c are saved.  As a time-major plane with one halo row, row(b, t) = (t + 1) * Bcap + b.
+            float* cl = c.cst;
+            size_t oh = 0, oc = 0;
+            if (sc != nullptr) {
+                c.stab = sc->table;
+                oh = take_state(static_cast<size_t>(H) * 4);
+                oc = take_state(static_cast<size_t>(H) * 4);
+                if (carry(hs.raw, hs.plane() * 2, hs.sb, hs.st, hs.off, H * 2, 1, 1, 1, 0, oh) ||
+                    carry(cl, 0, 1, 0, 0, H * 4, 1, 1, 1, 0, oc))
+                    return -1;
+            }
             if (plane_map(&mA, hs.raw, hs)) return -1;
             const int mt = (B + TC_BM - 1) / TC_BM;
             // 128-column tiles would move fewer bytes through L2 per step (VCB_CODEC_LSTM_WIDE=1); 64-column tiles keep
@@ -917,9 +1020,13 @@ int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
                 if (tc_launch(tc, mA, mA, sg, c, mt, st)) return -1;
             }
             *launches += T;
+            if (sc != nullptr && (carry(hs.raw, hs.plane() * 2, hs.sb, hs.st, hs.off, H * 2, 1, 1, 0, 1, oh) ||
+                                  carry(cl, 0, 1, 0, 0, H * 4, 1, 1, 0, 1, oc)))
+                return -1;
         }
         pf.end();
     }
+    if (nl > 0 && carry_plane(U0, U0.elu, 1)) return -1;
     // ---- up-sampling stages
     Plane cur = U0;                                                // ELU'd input of the next ConvTranspose
     int ch = H, t_cur = T, side = 0;
@@ -944,9 +1051,10 @@ int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
             if (tc_launch(tc, mA, mA, tc->up[i], c, (cur.rcap + TC_BM - 1) / TC_BM, st)) return -1;
             ++*launches;
         }
-        pf.end();
         ch = cout;
         t_cur *= r;
+        if (carry_plane(X, X.elu, t_cur / T)) return -1;
+        pf.end();
         int dil = 1;
         for (int j = 0; j < cf.n_residual_layers; ++j, dil *= cf.dilation_base) {
             const bool last_res = j == cf.n_residual_layers - 1;
@@ -989,6 +1097,7 @@ int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
                 if (tc_launch(tc, mA, mB, tc->res2[i][j], c, (X.rcap + TC_BM - 1) / TC_BM, st)) return -1;
                 ++*launches;
             }
+            if (carry_plane(O, O.elu, t_cur / T)) return -1;
             pf.end();
             X = O;
             side ^= 1;
@@ -1033,7 +1142,32 @@ int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
     }
     pf.end();
     pf.finish();
+    if (sc != nullptr && soff != tc->stream_bytes) {
+        set_error("codec_tc: stream state layout mismatch (%zu carried, %zu per stream)", soff, tc->stream_bytes);
+        return -1;
+    }
     return 0;
+}
+
+// bytes of carried state per stream, in the carry order of decode_chunk_tc: the latent Z, the LSTM (h, c) per layer, U0, then
+// per stage the ConvTranspose output and every residual-block output; a plane carries its halo rows as bf16 hi + lo
+size_t stream_state_bytes(const TcCodec* tc) {
+    const enc_config& cf = tc->cfg;
+    const int H = tc->ch0, kres = cf.residual_kernel_size, kout = cf.last_kernel_size;
+    size_t rows_x_c = static_cast<size_t>(cf.kernel_size - 1) * tc->Dp + static_cast<size_t>(cpad(H));
+    size_t bytes = static_cast<size_t>(cf.lstm) * H * 8;
+    int ch = H;
+    for (int i = 0; i < cf.n_ratios; ++i) {
+        const int cout = ch / 2;
+        const bool last_stage = i == cf.n_ratios - 1;
+        rows_x_c += static_cast<size_t>(cf.n_residual_layers > 0 ? kres - 1 : (last_stage ? kout - 1 : 1)) * cpad(cout);
+        for (int j = 0, d = 1; j < cf.n_residual_layers; ++j, d *= cf.dilation_base) {
+            const bool last_res = j == cf.n_residual_layers - 1;
+            rows_x_c += static_cast<size_t>(!last_res ? (kres - 1) * d * cf.dilation_base : (last_stage ? kout - 1 : 1)) * cpad(cout);
+        }
+        ch = cout;
+    }
+    return bytes + rows_x_c * 4;
 }
 
 }  // namespace
@@ -1146,6 +1280,7 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w
         }
     }
     tc->min_T = std::max(tc->min_T, std::max(cfg.kernel_size, cfg.last_kernel_size) + 1);
+    tc->stream_bytes = stream_state_bytes(tc);
     if (rc) {
         tc_codec_destroy(tc);
         return -1;
@@ -1156,14 +1291,15 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w
 
 bool tc_codec_accepts(const TcCodec* c, int B, int T) { return c != nullptr && B >= 1 && T >= c->min_T; }
 
-int tc_codec_decode(TcCodec* tc, const int64_t* codes, float* wav, int B, int T, cudaStream_t st, int64_t* launches) {
+int tc_codec_decode(TcCodec* tc, const int64_t* codes, float* wav, int B, int T, cudaStream_t st, int64_t* launches,
+                    const TcStreamCtx* sc) {
     tc->prof.clear();
     // chunk the batch so the workspace stays under the limit -- and halve the chunk again if the device cannot give that much
     int chunk = B;
     size_t need = 0;
     for (;;) {
         int64_t dummy = 0;
-        if (decode_chunk_tc(tc, nullptr, nullptr, chunk, T, st, &dummy, true, &need)) return -1;
+        if (decode_chunk_tc(tc, nullptr, nullptr, chunk, T, st, &dummy, true, &need, nullptr)) return -1;
         if (need > tc->ws_limit && chunk > 1) {
             chunk = (chunk + 1) / 2;
             continue;
@@ -1191,10 +1327,27 @@ int tc_codec_decode(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
     }
     for (int b0 = 0; b0 < B; b0 += chunk) {
         const int nb = std::min(chunk, B - b0);
+        TcStreamCtx part;
+        if (sc != nullptr) part = TcStreamCtx{sc->table + 4 * b0, sc->state};
         if (decode_chunk_tc(tc, codes + static_cast<size_t>(b0) * tc->cfg.n_q * T, wav + static_cast<size_t>(b0) * T * tc->hop, nb, T, st,
-                            launches, false, nullptr))
+                            launches, false, nullptr, sc != nullptr ? &part : nullptr))
             return -1;
     }
+    return 0;
+}
+
+size_t tc_stream_state_bytes(const TcCodec* c) { return c->stream_bytes; }
+
+int tc_stream_min_frames(const TcCodec* c) { return c->min_T; }
+
+int tc_codes_check(const int64_t* codes, long long n, int bins, int* bad_dev, int* bad_host, cudaStream_t st) {
+    VCB_CUDA_OK(cudaMemsetAsync(bad_dev, 0, sizeof(int), st));
+    const long long blocks = std::min<long long>((n + 255) / 256, 1024);
+    tc_codes_check_kernel<<<static_cast<unsigned>(std::max<long long>(blocks, 1)), 256, 0, st>>>(reinterpret_cast<const long long*>(codes),
+                                                                                              n, bins, bad_dev);
+    VCB_CUDA_OK(cudaGetLastError());
+    VCB_CUDA_OK(cudaMemcpyAsync(bad_host, bad_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
+    VCB_CUDA_OK(cudaStreamSynchronize(st));
     return 0;
 }
 

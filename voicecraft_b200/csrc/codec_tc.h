@@ -16,9 +16,23 @@ struct TcCodec;
 // 0: built; 1: this configuration is outside what the tensor-core path covers (why -> *reason, static string); -1: error.
 int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w_dev,
                    const std::map<std::string, std::vector<int64_t>>& shapes, TcCodec** out, const char** reason);
+// Stream decode (enc_stream_decode): utterance b of the call continues stream table[4b] with table[4b+1] valid frames;
+// table[4b+2] = 1 if that stream has decoded frames before (its left context and LSTM state come from `state`), 0 if fresh.
+struct TcStreamCtx {
+    const int* table;                  // device [B][4]: id, valid frames, continuing, unused
+    uint8_t* state;                    // device [max_streams][tc_stream_state_bytes]
+};
+
 // whether (B, T) can run here (T long enough for every reflect padding)
 bool tc_codec_accepts(const TcCodec* c, int B, int T);
-int tc_codec_decode(TcCodec* c, const int64_t* codes_dev, float* wav_dev, int B, int T, cudaStream_t st, int64_t* launches);
+// sc == nullptr: a whole-utterance decode; otherwise every row b < lens continues its stream (rows past it are unspecified)
+int tc_codec_decode(TcCodec* c, const int64_t* codes_dev, float* wav_dev, int B, int T, cudaStream_t st, int64_t* launches,
+                    const TcStreamCtx* sc = nullptr);
+size_t tc_stream_state_bytes(const TcCodec* c);
+// frames a fresh stream's first decode needs (every reflect padding mirrors valid rows)
+int tc_stream_min_frames(const TcCodec* c);
+// *bad_host = whether any of the n codes lies outside [0, bins); waits for the stream
+int tc_codes_check(const int64_t* codes_dev, long long n, int bins, int* bad_dev, int* bad_host, cudaStream_t st);
 void tc_codec_destroy(TcCodec* c);
 // per-layer device times of the last decode when VCB_CODEC_PROFILE=1 (name, ms), in launch order
 const std::vector<std::pair<std::string, float>>& tc_codec_profile(const TcCodec* c);

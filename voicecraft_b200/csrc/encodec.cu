@@ -282,6 +282,16 @@ struct enc_engine {
     TcCodec* tc = nullptr;              // tensor-core decoder (codec_tc.cu); null = configuration not covered
     const char* tc_reason = "";
     int64_t tc_decodes = 0;
+    int64_t stream_decodes = 0;
+};
+
+struct enc_stream {
+    enc_engine* e = nullptr;
+    int max_streams = 0;
+    uint8_t* state = nullptr;           // [max_streams][tc_stream_state_bytes]
+    int* table = nullptr;               // [max_streams][4] per-call table (TcStreamCtx)
+    int* bad = nullptr;                 // codes check flag
+    std::vector<int64_t> frames;        // frames decoded so far, per stream (0 = fresh)
 };
 
 namespace {
@@ -735,7 +745,121 @@ int64_t enc_counter(enc_engine* e, const char* name) {
     if (!strcmp(name, "flops_per_frame")) return static_cast<int64_t>(e->flops_per_frame);
     if (!strcmp(name, "tc_enabled")) return e->tc != nullptr;
     if (!strcmp(name, "tc_decodes")) return e->tc_decodes;
+    if (!strcmp(name, "stream_decodes")) return e->stream_decodes;
+    if (!strcmp(name, "stream_min_frames")) return e->tc ? tc_stream_min_frames(e->tc) : -1;
+    if (!strcmp(name, "stream_state_bytes")) return e->tc ? static_cast<int64_t>(tc_stream_state_bytes(e->tc)) : -1;
     return -1;
+}
+
+int enc_stream_create(enc_engine* e, int32_t max_streams, enc_stream** out) {
+    if (!e || !out || !e->finalized) {
+        set_error("codec stream: engine not finalized");
+        return -1;
+    }
+    *out = nullptr;
+    if (!e->tc) {
+        set_error("codec stream: streaming runs only on the tensor-core decoder, which does not cover this codec (%s)", e->tc_reason);
+        return -1;
+    }
+    if (max_streams < 1) {
+        set_error("codec stream: max_streams = %d", max_streams);
+        return -1;
+    }
+    VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
+    enc_stream* s = new enc_stream();
+    s->e = e;
+    s->max_streams = max_streams;
+    s->frames.assign(max_streams, 0);
+    const size_t bytes = static_cast<size_t>(max_streams) * tc_stream_state_bytes(e->tc);
+    if (cudaMalloc(reinterpret_cast<void**>(&s->state), bytes) != cudaSuccess ||
+        cudaMalloc(reinterpret_cast<void**>(&s->table), static_cast<size_t>(max_streams) * 4 * sizeof(int)) != cudaSuccess ||
+        cudaMalloc(reinterpret_cast<void**>(&s->bad), sizeof(int)) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("codec stream: cannot allocate the state of %d streams (%zu bytes)", max_streams, bytes);
+        enc_stream_destroy(s);
+        return -1;
+    }
+    *out = s;
+    return 0;
+}
+
+int enc_stream_destroy(enc_stream* s) {
+    if (!s) return 0;
+    cudaSetDevice(s->e->cfg.device);
+    cudaDeviceSynchronize();
+    cudaFree(s->state);
+    cudaFree(s->table);
+    cudaFree(s->bad);
+    delete s;
+    return 0;
+}
+
+int enc_stream_reset(enc_stream* s, const int32_t* ids_host, int32_t n) {
+    if (!s || (n > 0 && !ids_host)) {
+        set_error("codec stream: null argument");
+        return -1;
+    }
+    for (int i = 0; i < n; ++i)
+        if (ids_host[i] < 0 || ids_host[i] >= s->max_streams) {
+            set_error("codec stream: id %d outside [0, %d)", ids_host[i], s->max_streams);
+            return -1;
+        }
+    for (int i = 0; i < n; ++i) s->frames[ids_host[i]] = 0;
+    return 0;
+}
+
+int enc_stream_decode(enc_engine* e, enc_stream* s, const int32_t* ids_host, const int32_t* lens_host, int32_t B,
+                      const int64_t* codes_dev, int32_t T, float* wav_dev, void* stream) {
+    if (!e || !s || s->e != e || !ids_host || !lens_host || !codes_dev || !wav_dev) {
+        set_error("codec stream: null argument or a stream of another engine");
+        return -1;
+    }
+    if (B < 1 || B > s->max_streams || T < 1) {
+        set_error("codec stream: B = %d (max_streams %d), T = %d", B, s->max_streams, T);
+        return -1;
+    }
+    // everything is validated before any stream changes
+    const int min_frames = tc_stream_min_frames(e->tc);
+    std::vector<char> seen(s->max_streams, 0);
+    std::vector<int> table(static_cast<size_t>(B) * 4);
+    for (int b = 0; b < B; ++b) {
+        const int id = ids_host[b], len = lens_host[b];
+        if (id < 0 || id >= s->max_streams) {
+            set_error("codec stream: row %d: id %d outside [0, %d)", b, id, s->max_streams);
+            return -1;
+        }
+        if (seen[id]) {
+            set_error("codec stream: id %d appears twice in one call", id);
+            return -1;
+        }
+        seen[id] = 1;
+        if (len < 1 || len > T) {
+            set_error("codec stream: row %d: %d frames outside [1, T = %d]", b, len, T);
+            return -1;
+        }
+        if (s->frames[id] == 0 && len < min_frames) {
+            set_error("codec stream: stream %d starts with %d frames; a fresh stream needs at least %d", id, len, min_frames);
+            return -1;
+        }
+        table[4 * b] = id;
+        table[4 * b + 1] = len;
+        table[4 * b + 2] = s->frames[id] > 0;
+        table[4 * b + 3] = 0;
+    }
+    VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int bad = 0;
+    if (tc_codes_check(codes_dev, static_cast<long long>(B) * e->cfg.n_q * T, e->cfg.bins, s->bad, &bad, st)) return -1;
+    if (bad) {
+        set_error("codec stream: a code lies outside [0, %d)", e->cfg.bins);
+        return -1;
+    }
+    VCB_CUDA_OK(cudaMemcpyAsync(s->table, table.data(), table.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+    const TcStreamCtx ctx{s->table, s->state};
+    if (tc_codec_decode(e->tc, codes_dev, wav_dev, B, T, st, &e->launches, &ctx)) return -1;
+    for (int b = 0; b < B; ++b) s->frames[ids_host[b]] += lens_host[b];
+    e->stream_decodes++;
+    return 0;
 }
 
 }  // extern "C"

@@ -199,6 +199,70 @@ class AudioTokenizer:
         """Reference signature: frames = [(codes[1,K,T], None)] (data/tokenizer.py:131-133)."""
         return self.decode_codes(frames[0][0])
 
+    def open_stream(self, max_streams: int = 1) -> "CodecStream":
+        """Incremental decode of up to `max_streams` utterances (enc_stream_decode): see CodecStream."""
+        return CodecStream(self, max_streams)
+
+
+class CodecStream:
+    """Waveform of a growing code sequence, chunk by chunk.  Stream i's chunks, concatenated, are bit-identical to
+    ``decode_codes`` of its whole sequence: the causal decoder carries every layer's left context and the LSTM state from
+    one chunk to the next.  A stream's first chunk needs at least ``min_frames`` frames.  Runs only on the tensor-core
+    decoder; opening one on a codec it does not cover raises VcbError.  Use it from one CUDA stream at a time."""
+
+    def __init__(self, tokenizer: AudioTokenizer, max_streams: int = 1):
+        self._tok = tokenizer
+        self._lib = _lib.load()
+        eng = tokenizer._engine()
+        h = C.c_void_p()
+        with torch.cuda.device(tokenizer.device):
+            _lib.check(self._lib.enc_stream_create(eng, int(max_streams), C.byref(h)))
+        self._h = h
+        self.max_streams = int(max_streams)
+        self.min_frames = int(self._lib.enc_counter(eng, b"stream_min_frames"))
+
+    @torch.no_grad()
+    def decode(self, codes: torch.Tensor, ids=None, lens=None) -> torch.Tensor:
+        """codes [B,K,T] -> wav [B,channels,T*hop].  Row b continues stream ids[b] (default b) by its next lens[b] frames
+        (default T); samples [0, lens[b]*hop) of row b are that audio, later samples are unspecified.  Every code, padding
+        included, must lie in [0, bins).  Runs on the current CUDA stream."""
+        if self._h is None:
+            raise _lib.VcbError("CodecStream is closed")
+        assert codes.ndim == 3 and codes.shape[1] == self._tok.config.n_q, codes.shape
+        B, _, T = codes.shape
+        ids = list(range(B)) if ids is None else [int(i) for i in ids]
+        lens = [T] * B if lens is None else [int(n) for n in lens]
+        if len(ids) != B or len(lens) != B:
+            raise ValueError(f"CodecStream.decode: {B} rows, {len(ids)} ids, {len(lens)} lens")
+        codes = codes.to(self._tok.device).long().contiguous()
+        wav = torch.empty(B, self._tok.channels, T * self._tok.hop, device=self._tok.device, dtype=torch.float32)
+        with torch.cuda.device(self._tok.device):
+            _lib.check(self._lib.enc_stream_decode(self._tok._engine(), self._h, (C.c_int32 * B)(*ids), (C.c_int32 * B)(*lens), B,
+                                                   codes.data_ptr(), T, wav.data_ptr(), torch.cuda.current_stream().cuda_stream))
+        return wav
+
+    def reset(self, ids):
+        """The listed streams start over at frame 0."""
+        ids = [int(i) for i in ids]
+        _lib.check(self._lib.enc_stream_reset(self._h, (C.c_int32 * max(len(ids), 1))(*ids), len(ids)))
+
+    def close(self):
+        if self._h is not None:
+            self._lib.enc_stream_destroy(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
 
 def save_wav(path, wav: torch.Tensor, sample_rate: int):
     """Write a decoded waveform ([1, C, N] / [C, N] / [N] float in [-1, 1]) as 16-bit PCM -- the serialisation step of the

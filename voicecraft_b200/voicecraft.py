@@ -23,6 +23,7 @@ import ctypes as C
 import logging
 import os
 from argparse import Namespace
+from types import SimpleNamespace
 from typing import Dict, List, Optional
 
 import numpy as np
@@ -370,7 +371,8 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
 
     @staticmethod
     def _undelay(rows: np.ndarray, K: int) -> np.ndarray:
-        """rows [n,K] (delayed, as sampled) -> [K, n-K]   (reference voicecraft.py:1126-1137)."""
+        """rows [n,K] (delayed, as sampled) -> [K, n-K]   (reference voicecraft.py:1126-1137).  For a finished
+        generation n-K == final_frames(rows, K, end): the frames before the end token."""
         n = rows.shape[0]
         return np.stack([rows[k: n - (K - k), k] for k in range(K)], axis=0)
 
@@ -614,6 +616,224 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         finally:
             sess.close()
 
+    # ------------------------------------------------------------------------------------------------
+    # streaming: audio while the tokens are generated (TtsStream)
+    # ------------------------------------------------------------------------------------------------
+    def inference_tts_many_stream(self, xs, ys, tokenizer, chunk_frames: int = 25, poll_every: int = 8, seeds=None, **kw):
+        """inference_tts_many with the audio handed out while it is generated: iterates (i, wav [1, channels, n*hop]),
+        utterance i's chunks in order; concatenated they equal ``tokenizer.decode_codes(gen_i)``.  Afterwards
+        ``.results`` equals what inference_tts_many returns.  `seeds` as in open_tts_session."""
+        sess = self.open_tts_session(xs, ys, seeds=seeds, **kw)
+        return TtsStream(sess, tokenizer, chunk_frames, poll_every)
+
+    def inference_tts_stream(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, tokenizer, chunk_frames: int = 25,
+                             poll_every: int = 8, top_k: int = -100, top_p: float = 1.0, temperature: float = 1.0,
+                             stop_repetition: int = 3, silence_tokens: List[int] = [1388, 1898, 131]):
+        """inference_tts with the audio handed out while it is generated: iterates wav chunks [1, channels, n*hop] whose
+        concatenation equals ``tokenizer.decode([(gen, None)])``.  Afterwards ``.result`` is (res, gen), what inference_tts
+        returns: the utterance samples from the device generator's stream at its current offset and leaves it advanced by
+        the steps it ran, as inference_tts does."""
+        assert x.ndim == 2 and x.shape[0] == 1 and x_lens.ndim == 1 and y.ndim == 3 and y.shape[0] == 1, (x.shape, y.shape)
+        dev = self.mask_embedding.device
+        gen_state = None if self.noise_fn is not None else torch.cuda.default_generators[dev.index or 0]
+
+        def finish(st):
+            st.result = st.results[0]
+            if gen_state is not None:
+                gen_state.set_offset(int(st.sess.status[0].rng_offset))
+        # one utterance: the session's default stream is the device generator's (seed, offset), like _device_rng
+        sess = self.open_tts_session([x], [y], top_k=top_k, top_p=top_p, temperature=temperature,
+                                     stop_repetition=stop_repetition, silence_tokens=silence_tokens)
+        ts = _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every, on_finish=finish)
+        return ts
+
+
+def _end_token(a) -> int:
+    """the token that ends a TTS generation in codebook 0 (reference voicecraft.py:1034-1045)"""
+    return a.eos if a.eos > 0 else a.eog
+
+
+def final_frames(rows: np.ndarray, K: int, end: int) -> int:
+    """How many leading frames of the delayed token rows [n,K] are final: frame t is final once rows up to t+K-1 exist
+    (its last codebook has been sampled) and rows[t, 0] is not the end token.  Frames are final in order, so the answer
+    only grows as rows are added; for a finished generation it is n-K (what _undelay returns)."""
+    m = max(0, rows.shape[0] - K + 1)
+    hit = np.flatnonzero(rows[:m, 0] == end)
+    return int(hit[0]) if hit.size else m
+
+
+def frame_codes(rows: np.ndarray, K: int, t0: int, t1: int) -> np.ndarray:
+    """frames [t0, t1) of the delayed rows, un-delayed: [K, t1-t0] with [k, t] = rows[t + k, k]"""
+    return np.stack([rows[t0 + k: t1 + k, k] for k in range(K)], axis=0)
+
+
+class TtsStream:
+    """Audio of a DecodeSession while it generates (VoiceCraft.inference_tts_stream / inference_tts_many_stream).
+
+    Iterating runs the session: every `poll_every` steps it polls, reads the token rows and sends each utterance's newly
+    final frames to the codec (a CodecStream on a second CUDA stream) -- all utterances with enough new frames in one call.
+    The next decode steps are enqueued before the chunk's waveform is waited for.  A chunk is the waveform of those frames,
+    bit-identical to the same samples of ``decode_codes`` of the utterance's whole generation.  An utterance's first
+    chunk waits for max(chunk_frames, min_frames) frames; one that ends with fewer than min_frames frames is decoded in one
+    ``decode_codes`` call.  Yields (i, wav [1, channels, n*hop]).  After the iteration, ``results`` holds what
+    ``DecodeSession.results()`` returns.  Closing it early (break, close(), garbage collection) releases the session's
+    engine slots and the codec streams."""
+
+    def __init__(self, sess: "DecodeSession", tokenizer, chunk_frames: int = 25, poll_every: int = 8, on_finish=None):
+        if chunk_frames < 1 or poll_every < 1:
+            raise ValueError("chunk_frames and poll_every must be >= 1")
+        # the generator holds this state, not the TtsStream: dropping the TtsStream closes it at once (no reference cycle)
+        st = self._st = SimpleNamespace(sess=sess, tok=tokenizer, chunk_frames=int(chunk_frames), poll_every=int(poll_every),
+                                        results=None, result=None, first_audio_steps=None, on_finish=on_finish, codec=None)
+        self._it = None
+        try:
+            st.codec = tokenizer.open_stream(max_streams=sess.B)
+            st.cstream = torch.cuda.Stream(device=sess.dev)
+        except Exception:
+            self.close()
+            raise
+        self._it = self._run(st)
+
+    @property
+    def results(self):
+        return self._st.results
+
+    @property
+    def result(self):
+        return self._st.result
+
+    @property
+    def first_audio_steps(self):
+        """session steps taken when the first chunk was handed out"""
+        return self._st.first_audio_steps
+
+    @property
+    def sess(self):
+        return self._st.sess
+
+    def __iter__(self):
+        return self
+
+    def __next__(self):
+        return next(self._it)
+
+    def close(self):
+        st = getattr(self, "_st", None)
+        if st is None:
+            return
+        if self._it is not None:
+            self._it.close()
+        if st.codec is not None:
+            st.codec.close()
+            st.codec = None
+        st.sess.close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @staticmethod
+    def _codes(st, i, rows, t0, t1):
+        """frames [t0, t1) of utterance i as codec codes [K, n]; a non-audio token never reaches the codec"""
+        a = st.sess.model.args
+        c = frame_codes(rows, st.sess.K, t0, t1) - (int(a.n_special) if a.special_first else 0)
+        bad = np.argwhere((c < 0) | (c >= st.tok.config.bins))
+        if bad.size:
+            k, t = int(bad[0][0]), int(bad[0][1])
+            raise _lib.VcbError(f"utterance {i}: frame {t0 + t} holds the non-audio token {int(rows[t0 + t + k, k])} in "
+                                f"codebook {k}; it has no waveform")
+        return c
+
+    @staticmethod
+    @torch.no_grad()
+    def _run(st):
+        sess, K, dev = st.sess, st.sess.K, st.sess.dev
+        end = _end_token(sess.model.args)
+        B, hop = sess.B, st.tok.hop
+        pushed = [0] * B                     # frames sent to the codec
+        closed = [False] * B                 # all of the utterance's audio has been handed out
+        first = max(st.chunk_frames, st.codec.min_frames)
+        try:
+            with torch.cuda.device(dev):
+                sess.sample()
+                while sess.steps % st.poll_every:
+                    sess.step()
+                while True:
+                    done = sess.all_done()
+                    ids, lens, chunks, whole = [], [], [], []
+                    for i in range(B):
+                        if closed[i]:
+                            continue
+                        fin = bool(sess.status[i].done)
+                        rows = sess.model._read_rows(sess.eng, sess.slots[i], sess.status[i].n_steps, sess.stream)
+                        f = final_frames(rows, K, end)
+                        new = f - pushed[i]
+                        if pushed[i] == 0 and fin and f < st.codec.min_frames:
+                            closed[i] = True
+                            if f > 0:
+                                whole.append((i, TtsStream._codes(st, i, rows, 0, f)))
+                            continue
+                        if new > 0 and (fin or new >= (first if pushed[i] == 0 else st.chunk_frames)):
+                            ids.append(i)
+                            lens.append(new)
+                            chunks.append(TtsStream._codes(st, i, rows, pushed[i], f))
+                            pushed[i] = f
+                        closed[i] = fin and pushed[i] == f
+                    wav = None
+                    if ids or whole:                 # the codec works on its own CUDA stream ...
+                        with torch.cuda.stream(st.cstream):
+                            if ids:
+                                T = max(lens)
+                                codes = np.zeros((len(ids), K, T), dtype=np.int64)
+                                for j, c in enumerate(chunks):
+                                    codes[j, :, :lens[j]] = c
+                                wav = st.codec.decode(torch.from_numpy(codes).to(dev), ids=ids, lens=lens)
+                            whole = [(i, st.tok.decode_codes(torch.from_numpy(c).unsqueeze(0).to(dev))) for i, c in whole]
+                        ev = torch.cuda.Event()
+                        ev.record(st.cstream)
+                    if not done:                     # ... while the next steps are already queued on the LM's
+                        for _ in range(st.poll_every):
+                            sess.step()
+                    if ids or whole:
+                        ev.synchronize()
+                        cur = torch.cuda.current_stream(dev)
+                        out = []
+                        if wav is not None:
+                            wav.record_stream(cur)
+                            out += [(i, wav[j:j + 1, :, :lens[j] * hop]) for j, i in enumerate(ids)]
+                        for i, w in whole:
+                            w.record_stream(cur)
+                            out.append((i, w))
+                        for i, w in sorted(out, key=lambda p: p[0]):
+                            if st.first_audio_steps is None:
+                                st.first_audio_steps = sess.steps
+                            yield i, w
+                    if done and all(closed):
+                        break
+                st.results = sess.results()
+                if st.on_finish is not None:
+                    st.on_finish(st)
+        finally:
+            if st.codec is not None:
+                st.codec.close()
+                st.codec = None
+            sess.close()
+
+
+class _SingleTtsStream(TtsStream):
+    """TtsStream of one utterance (inference_tts_stream): yields the wav chunks alone; ``result`` = (res, gen)"""
+
+    def __next__(self):
+        return next(self._it)[1]
+
 
 class DecodeSession:
     """A batch of independent utterances resident in the engine, one slot and one random stream each."""
@@ -759,10 +979,8 @@ class DecodeSession:
                 continue
             if st[i].done:
                 gen = torch.from_numpy(VoiceCraft._undelay(rows, self.K)).to(self.dev)
-            else:       # truncated session: drop the still-delayed tail
-                n = rows.shape[0]
-                gen = torch.from_numpy(np.stack([rows[k: n - (self.K - 1) + k, k] for k in range(self.K)], 0)).to(self.dev) \
-                    if n >= self.K else torch.zeros(self.K, 0, dtype=torch.long, device=self.dev)
+            else:       # truncated session: the final frames only (the still-delayed tail is dropped)
+                gen = torch.from_numpy(frame_codes(rows, self.K, 0, final_frames(rows, self.K, _end_token(a)))).to(self.dev)
             res = torch.cat([self.y0[i], gen], dim=1).unsqueeze(0)
             if a.special_first:
                 res, gen = res - int(a.n_special), gen - int(a.n_special)
