@@ -10,6 +10,12 @@ Every non-audio token except the length cap's end token is suppressed, so every 
 
     python scripts/bench_stream.py [--batch 32] [--chunk-frames 25] [--poll-every 8] [--repeats 2]   -> one JSON line
 
+--queue N instead serves N utterances with B slots, their text lengths spread by a fixed seed over
+[--text-len-min, --text-len] (with equal lengths every utterance ends at the same step and continuous batching has nothing
+to gain), two arms alternating in one call:
+  batcher  all N submitted to ContinuousBatcher(max_concurrency=B).stream();
+  static   ceil(N/B) consecutive inference_tts_many_stream calls of B utterances.
+
 value = codec tokens/s of the streaming arm, tokens to waveform end to end; first_audio_ms (median / max over the
 utterances) and seconds_to_all_audio for both arms, wall clock from the call's start; card name, power limit and SM clock
 read in the same call.
@@ -40,6 +46,8 @@ def parse():
     ap.add_argument("--chunk-frames", type=int, default=25)
     ap.add_argument("--poll-every", type=int, default=8)
     ap.add_argument("--repeats", type=int, default=2, help="timed calls per arm after one untimed warm-up of each")
+    ap.add_argument("--queue", type=int, default=0, help="serve this many utterances: batcher stream vs static batches")
+    ap.add_argument("--text-len-min", type=int, default=40, help="--queue: shortest text (the longest is --text-len)")
     a = ap.parse_args()
     a.workload = "tts"
     return a
@@ -73,8 +81,13 @@ def main():
         for t in (cfg.empty_token, cfg.audio_pad_token):
             sd[f"predict_layer.{k}.2.bias"][t] = -1e4
     K, B = cfg.n_codebooks, args.batch
-    utts = bench.make_utterances(args, cfg, range(B))
-    seeds = [1 + i for i in range(B)]
+    if args.queue:
+        from voicecraft_b200 import synthetic
+        lens = torch.randint(args.text_len_min, args.text_len + 1, (args.queue,), generator=torch.Generator().manual_seed(0))
+        utts = [synthetic.synthetic_utterance(cfg, 100 + i, int(n), args.prompt) for i, n in enumerate(lens)]
+    else:
+        utts = bench.make_utterances(args, cfg, range(B))
+    seeds = [1 + i for i in range(len(utts))]
     model = VoiceCraft(cfg)
     model.load_state_dict(sd)
     model = model.to(dev).eval()
@@ -86,6 +99,8 @@ def main():
     xs = [u[0].to(dev) for u in utts]
     ys = [u[2].to(dev) for u in utts]
     kw = dict(top_k=40, top_p=1.0, temperature=1.0, stop_repetition=3)
+    if args.queue:
+        return queue(args, cfg, model, tok, xs, ys, seeds, kw)
 
     def streaming():
         first = {}
@@ -134,6 +149,64 @@ def main():
         "streaming": s, "batch": arms["batch"], "gpu": gpu_identity(0), "clocks": clk,
         "note": "wall clock from the call's start, median of %d alternating calls per arm after one untimed warm-up of each; "
                 "batch arm: first audio = all audio" % max(1, args.repeats)}))
+
+
+def queue(args, cfg, model, tok, xs, ys, seeds, kw):
+    from voicecraft_b200.voicecraft import ContinuousBatcher
+    K, B, N = cfg.n_codebooks, args.batch, len(xs)
+
+    def batcher():
+        first = {}
+        t0 = time.perf_counter()
+        cb = ContinuousBatcher(model, max_concurrency=B, poll_every=args.poll_every, **kw)
+        for x, y, s in zip(xs, ys, seeds):
+            cb.submit(x, y, seed=s)
+        it = cb.stream(tok, chunk_frames=args.chunk_frames)
+        for t, _, _ in it:
+            first.setdefault(t, time.perf_counter() - t0)
+        torch.cuda.synchronize()
+        return [first[t] for t in range(N)], time.perf_counter() - t0, sum(int(r[1].shape[-1]) for r in cb.results), \
+            it.push_host_seconds
+
+    def static():
+        first, frames, push_s = {}, 0, 0.0
+        t0 = time.perf_counter()
+        for b in range(0, N, B):
+            ts = model.inference_tts_many_stream(xs[b:b + B], ys[b:b + B], tok, chunk_frames=args.chunk_frames,
+                                                 poll_every=args.poll_every, seeds=seeds[b:b + B], **kw)
+            for i, _ in ts:
+                first.setdefault(b + i, time.perf_counter() - t0)
+            frames += sum(int(r[1].shape[-1]) for r in ts.results)
+            push_s += ts.push_host_seconds
+        torch.cuda.synchronize()
+        return [first[t] for t in range(N)], time.perf_counter() - t0, frames, push_s
+
+    batcher(), static()                          # untimed warm-up
+    clocks = bench.ClockSampler(0)
+    clocks.start()
+    runs = {"batcher": [], "static": []}
+    for _ in range(max(1, args.repeats)):
+        runs["batcher"].append(batcher())
+        runs["static"].append(static())
+    clk = clocks.stop()
+    arms = {}
+    for name, rs in runs.items():
+        r = sorted(rs, key=lambda v: v[1])[len(rs) // 2]          # the median call by total time
+        fa = sorted(r[0])
+        arms[name] = {"first_audio_ms": {"median": statistics.median(fa) * 1e3, "p90": fa[int(0.9 * (len(fa) - 1))] * 1e3,
+                                         "max": fa[-1] * 1e3},
+                      "seconds_to_all_audio": r[1], "generated_frames": r[2],
+                      "codec_tokens_per_s": r[2] * K / r[1], "push_host_ms": r[3] * 1e3, "seconds_all": [v[1] for v in rs]}
+    print(json.dumps({
+        "metric": f"seconds to all audio (giga{args.model} streaming TTS, {N} queued utterances, {B} slots)",
+        "value": arms["batcher"]["seconds_to_all_audio"], "unit": "s", "n_gpus": 1, "higher_is_better": False,
+        "dtype": "bf16", "data": "synthetic",
+        "config": dict(bench.workload_config(args, cfg, 1), queue=N, text_len_min=args.text_len_min,
+                       codec="16 kHz EnCodec decoder (4 x 2048, n_filters 64, LSTM 2), seeded random weights",
+                       chunk_frames=args.chunk_frames, poll_every=args.poll_every),
+        "batcher": arms["batcher"], "static": arms["static"], "gpu": gpu_identity(0), "clocks": clk,
+        "note": "wall clock from the call's start, median of %d alternating calls per arm after one untimed warm-up of each; "
+                "push_host_ms: host time in the push step outside the device waits" % max(1, args.repeats)}))
 
 
 if __name__ == "__main__":

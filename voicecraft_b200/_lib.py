@@ -53,6 +53,9 @@ PROTOTYPES = {
     "vcb_sample": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.POINTER(vcb_sampling), C.c_void_p]),
     "vcb_decode_step": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.POINTER(vcb_sampling), C.c_void_p]),
     "vcb_poll": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.POINTER(vcb_status), C.c_void_p]),
+    "vcb_poll_frames": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_int64,
+                                  C.c_int64, C.c_void_p, C.POINTER(vcb_status), C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                  C.c_void_p]),
     "vcb_read_tokens": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_void_p]),
     "vcb_release": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "vcb_debug_logits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),

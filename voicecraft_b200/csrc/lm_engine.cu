@@ -91,6 +91,11 @@ struct vcb_engine {
     const int *cur_pages = nullptr;   // = row_pages during decode steps, null during prefill
     const int *cur_forced = nullptr;  // = row_forced during decode steps, null for vcb_sample
     std::vector<char> slot_rng;       // host mirror: the slot's group generates its own sampling noise
+    std::vector<char> slot_edit;      // host mirror: the slot decodes an edit prompt
+    std::vector<int> slot_copies;     // host mirror: n_copies of the slot's prompt (best-of-N group size)
+    std::vector<int> slot_final;      // final frames vcb_poll_frames last reported for the slot (they only grow)
+    PollFramesRec *pf_rec = nullptr, *h_pf_rec = nullptr;   // vcb_poll_frames results: device, pinned host [max_slots]
+    int64_t n_poll_frames = 0;
     int *all_rows = nullptr;          // prefill row tables: 5 arrays of all_rows_cap ints (seq, pos, slot, last, page)
     size_t all_rows_cap = 0;
     const int *cur_slot = nullptr, *cur_pos = nullptr, *cur_last = nullptr, *cur_page = nullptr;   // tables used by forward_rows
@@ -912,6 +917,9 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
     e->slot_pages.resize(cfg->max_slots);
     e->slot_group.assign(cfg->max_slots, -1);
     e->slot_rng.assign(cfg->max_slots, 0);
+    e->slot_edit.assign(cfg->max_slots, 0);
+    e->slot_copies.assign(cfg->max_slots, 0);
+    e->slot_final.assign(cfg->max_slots, 0);
     for (int g = cfg->max_slots - 1; g >= 0; --g) e->free_groups.push_back(g);
     e->layers.resize(m.L);
     e->h2.resize(m.K);
@@ -952,13 +960,14 @@ int vcb_destroy(vcb_engine* e) {
     for (auto& M : e->h2) cudaFree(M.w);
     void* ptrs[] = {e->b_h1, e->d_h2_maps, e->d_bias2, e->d_E_audio, e->pe, e->x_rows, e->qbuf, e->logits, e->att_ws, e->att_cnt, e->ln_stats, e->x_slot, e->h_slot,
                     e->act_d, e->act_d2, e->act_f, e->act_h, e->row_slot, e->row_pos, e->row_last, e->row_page, e->row_forced, e->row_pages, e->all_rows, e->page_table, e->wx, e->wq, e->w_att_ws, e->w_att_cnt, e->wact_d, e->wact_f,
-                    e->d_slots, e->tok_log, e->dbg_logits, e->st, e->gr, e->d_seqs};
+                    e->d_slots, e->tok_log, e->dbg_logits, e->st, e->gr, e->d_seqs, e->pf_rec};
     for (void* p : ptrs) cudaFree(p);
     void* mptrs[] = {e->d_mega_ph[0], e->d_mega_ph[1], e->d_wmaps, e->d_wptrs, e->mega_flags, e->mega_tile_cnt, e->mega_part, e->knew, e->vnew,
                      e->mega_att_ws, e->mega_att_cnt, e->mega_tl, e->mact_d, e->mact_d2, e->mact_f, e->mact_h};
     for (void* p : mptrs) cudaFree(p);
     if (e->mega_dbg_h) cudaFreeHost(e->mega_dbg_h);
     if (e->h_stage) cudaFreeHost(e->h_stage);
+    if (e->h_pf_rec) cudaFreeHost(e->h_pf_rec);
     if (e->stage_ev) cudaEventDestroy(e->stage_ev);
     delete e;
     return 0;
@@ -1114,8 +1123,9 @@ int vcb_finalize_weights(vcb_engine* e) {
             dalloc(&e->d_slots, R) || dalloc(&e->page_table, static_cast<size_t>(S) * e->max_pages_per_slot) ||
             dalloc(&e->tok_log, static_cast<size_t>(S) * e->cfg.max_new_tokens * m.K) ||
             dalloc(&e->dbg_logits, static_cast<size_t>(R) * m.K * m.V) || dalloc(&e->st, S) || dalloc(&e->gr, S) ||
-            dalloc(&e->d_seqs, S))
+            dalloc(&e->d_seqs, S) || dalloc(&e->pf_rec, S))
             return -1;
+        VCB_CUDA_OK(cudaMallocHost(reinterpret_cast<void**>(&e->h_pf_rec), static_cast<size_t>(S) * sizeof(PollFramesRec)));
         e->all_rows_cap = static_cast<size_t>(S) * e->cfg.max_seq_len;
         if (dalloc(&e->all_rows, 5 * e->all_rows_cap)) return -1;
         e->h_stage_ints = 4096;
@@ -1223,6 +1233,9 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
             const int slot = P.slot + c;
             e->slot_group[slot] = gid;
             e->slot_rng[slot] = P.rng_threads != 0;
+            e->slot_edit[slot] = P.mode == VCB_MODE_EDIT;
+            e->slot_copies[slot] = P.n_copies;
+            e->slot_final[slot] = 0;
             auto& pg = e->slot_pages[slot];
             pg.clear();
             for (int p = 0; p < e->max_pages_per_slot; ++p) {
@@ -1423,6 +1436,81 @@ int vcb_poll(vcb_engine* e, const int32_t* slots, int32_t n, vcb_status* out, vo
         out[i].n_spans_done = G.n_spans_done;
         for (int j = 0; j < 8; ++j) out[i].span_ends[j] = G.span_ends[j];
         out[i].rng_offset = (static_cast<uint64_t>(G.off_hi) << 32) | G.off_lo;
+    }
+    return 0;
+}
+
+// Streaming: vcb_poll plus each listed slot's newly final frames as codec codes (poll_frames_kernel), behind one wait.
+// Everything is validated on the host first: `from` may not exceed the final frames this call last reported for the
+// slot, which never exceeds the slot's final frames now (frames only become final).
+int vcb_poll_frames(vcb_engine* e, const int32_t* slots, int32_t n, const int32_t* from_host, int32_t max_frames,
+                    int64_t code_offset, int64_t bins, int64_t* codes_dev, vcb_status* status_host, int32_t* final_host,
+                    int32_t* bad_host, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!e || !e->finalized || !slots || !from_host || !codes_dev || !status_host || !final_host || !bad_host || n < 1 ||
+        n > e->cfg.max_slots || max_frames < 1 || bins < 1) {
+        set_error("vcb_poll_frames: bad argument (n=%d, max_frames=%d, bins=%lld)", n, max_frames, static_cast<long long>(bins));
+        return -1;
+    }
+    for (int i = 0; i < n; ++i) {
+        const int slot = slots[i];
+        if (slot < 0 || slot >= e->cfg.max_slots || e->slot_group[slot] < 0) {
+            set_error("slot %d is not open", slot);
+            return -1;
+        }
+        if (e->slot_edit[slot] || e->slot_copies[slot] != 1) {
+            set_error("vcb_poll_frames: slot %d decodes %s: only single TTS utterances stream", slot,
+                      e->slot_edit[slot] ? "an edit prompt" : "a best-of-N group");
+            return -1;
+        }
+        if (from_host[i] < 0 || from_host[i] > e->slot_final[slot]) {
+            set_error("vcb_poll_frames: slot %d: from %d outside [0, %d], the final frames reported so far", slot, from_host[i],
+                      e->slot_final[slot]);
+            return -1;
+        }
+    }
+    VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
+    const ModelDims& m = e->m;
+    PollFramesArgs a;
+    a.st = e->st;
+    a.gr = e->gr;
+    a.tok_log = e->tok_log;
+    a.code_offset = code_offset;
+    a.bins = bins;
+    a.max_steps = e->cfg.max_new_tokens;
+    a.K = m.K;
+    a.end = m.eos > 0 ? m.eos : m.eog;          // the token that ends a TTS generation in codebook 0
+    a.max_frames = max_frames;
+    for (int b = 0; b < n; b += PF_MAX_SLOTS) {
+        const int nb = std::min(n - b, PF_MAX_SLOTS);
+        for (int i = 0; i < nb; ++i) {
+            a.slots[i] = slots[b + i];
+            a.from[i] = from_host[b + i];
+        }
+        a.codes = reinterpret_cast<long long*>(codes_dev) + static_cast<size_t>(b) * m.K * max_frames;
+        a.rec = e->pf_rec + b;
+        poll_frames_kernel<<<nb, 256, 0, st>>>(a);
+        VCB_CUDA_OK(cudaGetLastError());
+        LAUNCH_COUNT(e);
+    }
+    VCB_CUDA_OK(cudaMemcpyAsync(e->h_pf_rec, e->pf_rec, static_cast<size_t>(n) * sizeof(PollFramesRec), cudaMemcpyDeviceToHost, st));
+    if (sync_or_report(e, cudaStreamSynchronize(st), "vcb_poll_frames")) return -1;
+    e->n_poll_frames += 1;
+    for (int i = 0; i < n; ++i) {
+        const PollFramesRec& r = e->h_pf_rec[i];
+        vcb_status& o = status_host[i];
+        o.done = r.done;
+        o.forced = r.forced;
+        o.n_steps = r.n_steps;
+        o.keep = r.keep;
+        o.n_spans_done = r.n_spans_done;
+        for (int j = 0; j < 8; ++j) o.span_ends[j] = r.span_ends[j];
+        o.rng_offset = (static_cast<uint64_t>(r.off_hi) << 32) | r.off_lo;
+        final_host[i] = r.final_frames;
+        bad_host[3 * i] = r.bad_frame;
+        bad_host[3 * i + 1] = r.bad_k;
+        bad_host[3 * i + 2] = r.bad_tok;
+        e->slot_final[slots[i]] = std::max(e->slot_final[slots[i]], r.final_frames);
     }
     return 0;
 }
@@ -1639,6 +1727,7 @@ int64_t vcb_counter(vcb_engine* e, const char* name) {
     if (!strcmp(name, "launches")) return e->n_launches;
     if (!strcmp(name, "num_sms")) return e->num_sms;
     if (!strcmp(name, "mega_grid")) return e->mega_grid;
+    if (!strcmp(name, "poll_frames")) return e->n_poll_frames;
     if (!strcmp(name, "kv_bytes_per_token")) return static_cast<int64_t>(e->m.L) * 2 * e->m.d * (e->kv_fp32 ? 4 : 2);
     return -1;
 }

@@ -990,4 +990,84 @@ __global__ void delay_pattern_kernel(const long long* __restrict__ z, long long*
     }
 }
 
+// ---------------------------------------------------------------------------------------------------
+// Streaming gather (vcb_poll_frames): one block per listed slot.  Frame t is final once the token log holds rows up to
+// t+K-1 and rows[t][0] is not the end token.  Only rows [from, n_steps-K+1) are scanned: the caller's `from` frames are
+// final already.  The new frames are written un-delayed as codec codes [K][max_frames] with zero padding, the first code
+// outside [0, bins) (lowest frame, then codebook) is recorded, and the slot's status is copied next to the result.
+// ---------------------------------------------------------------------------------------------------
+constexpr int PF_MAX_SLOTS = 128;          // listed slots per launch (the lists travel as kernel parameters)
+constexpr int PF_NO_BAD = 0x7fffffff;
+
+struct PollFramesRec {         // one listed slot: its vcb_status fields + the gather's result (copied to the host in one piece)
+    int done, forced, n_steps, keep, n_spans_done;
+    int span_ends[8];
+    unsigned int off_lo, off_hi;
+    int final_frames, bad_frame, bad_k, bad_tok;
+};
+
+struct PollFramesArgs {
+    int slots[PF_MAX_SLOTS], from[PF_MAX_SLOTS];
+    const SlotState* st;
+    const GroupState* gr;
+    const int* tok_log;        // [max_slots][max_steps][K]
+    long long* codes;          // [n][K][max_frames], from this launch's first listed slot on
+    PollFramesRec* rec;        // [n], same offset
+    long long code_offset, bins;
+    int max_steps, K, end, max_frames;
+};
+
+__global__ void __launch_bounds__(256) poll_frames_kernel(const __grid_constant__ PollFramesArgs a) {
+    __shared__ int s_end, s_bad;
+    const int i = blockIdx.x, slot = a.slots[i], from = a.from[i], K = a.K, tid = threadIdx.x;
+    const SlotState& S = a.st[slot];
+    const int n_steps = S.n_steps;
+    const int* log = a.tok_log + static_cast<size_t>(slot) * a.max_steps * K;
+    const int m = max(0, n_steps - K + 1);             // frames whose last codebook has been sampled
+    if (tid == 0) {
+        s_end = m;
+        s_bad = PF_NO_BAD;
+    }
+    __syncthreads();
+    for (int t = from + tid; t < m; t += blockDim.x)   // a thread's first hit is its lowest: the block minimum is the end
+        if (log[static_cast<size_t>(t) * K] == a.end) {
+            atomicMin(&s_end, t);
+            break;
+        }
+    __syncthreads();
+    const int fin = max(s_end, from);
+    const int n_new = min(fin - from, a.max_frames);
+    long long* out = a.codes + static_cast<size_t>(i) * K * a.max_frames;
+    for (int j = tid; j < K * a.max_frames; j += blockDim.x) {
+        const int k = j / a.max_frames, t = j - k * a.max_frames;
+        long long c = 0;                               // padding: the codec rejects any code outside [0, bins)
+        if (t < n_new) {
+            c = log[static_cast<size_t>(from + t + k) * K + k] - a.code_offset;
+            if (c < 0 || c >= a.bins) atomicMin(&s_bad, t * K + k);
+        }
+        out[j] = c;
+    }
+    __syncthreads();
+    if (tid != 0) return;
+    const GroupState& G = a.gr[S.group];
+    PollFramesRec r;
+    r.done = G.done;
+    r.forced = S.forced;
+    r.n_steps = n_steps;
+    r.keep = G.keep;
+    r.n_spans_done = G.n_spans_done;
+    for (int j = 0; j < 8; ++j) r.span_ends[j] = G.span_ends[j];
+    r.off_lo = G.off_lo;
+    r.off_hi = G.off_hi;
+    r.final_frames = fin;
+    r.bad_frame = r.bad_k = r.bad_tok = -1;
+    if (s_bad != PF_NO_BAD) {
+        const int t = s_bad / K, k = s_bad - t * K;
+        r.bad_frame = from + t;
+        r.bad_k = k;
+        r.bad_tok = log[static_cast<size_t>(from + t + k) * K + k];
+    }
+    a.rec[i] = r;
+}
+
 }  // namespace vcb

@@ -22,6 +22,7 @@ import copy
 import ctypes as C
 import logging
 import os
+import time
 from argparse import Namespace
 from types import SimpleNamespace
 from typing import Dict, List, Optional
@@ -684,7 +685,8 @@ class TtsStream:
             raise ValueError("chunk_frames and poll_every must be >= 1")
         # the generator holds this state, not the TtsStream: dropping the TtsStream closes it at once (no reference cycle)
         st = self._st = SimpleNamespace(sess=sess, tok=tokenizer, chunk_frames=int(chunk_frames), poll_every=int(poll_every),
-                                        results=None, result=None, first_audio_steps=None, on_finish=on_finish, codec=None)
+                                        results=None, result=None, first_audio_steps=None, on_finish=on_finish, codec=None,
+                                        push=None)
         self._it = None
         try:
             st.codec = tokenizer.open_stream(max_streams=sess.B)
@@ -706,6 +708,11 @@ class TtsStream:
     def first_audio_steps(self):
         """session steps taken when the first chunk was handed out"""
         return self._st.first_audio_steps
+
+    @property
+    def push_host_seconds(self):
+        """host time spent in the push steps so far, outside the device waits"""
+        return self._st.push.host_s if self._st.push is not None else 0.0
 
     @property
     def sess(self):
@@ -741,82 +748,32 @@ class TtsStream:
             pass
 
     @staticmethod
-    def _codes(st, i, rows, t0, t1):
-        """frames [t0, t1) of utterance i as codec codes [K, n]; a non-audio token never reaches the codec"""
-        a = st.sess.model.args
-        c = frame_codes(rows, st.sess.K, t0, t1) - (int(a.n_special) if a.special_first else 0)
-        bad = np.argwhere((c < 0) | (c >= st.tok.config.bins))
-        if bad.size:
-            k, t = int(bad[0][0]), int(bad[0][1])
-            raise _lib.VcbError(f"utterance {i}: frame {t0 + t} holds the non-audio token {int(rows[t0 + t + k, k])} in "
-                                f"codebook {k}; it has no waveform")
-        return c
-
-    @staticmethod
     @torch.no_grad()
     def _run(st):
-        sess, K, dev = st.sess, st.sess.K, st.sess.dev
-        end = _end_token(sess.model.args)
-        B, hop = sess.B, st.tok.hop
-        pushed = [0] * B                     # frames sent to the codec
-        closed = [False] * B                 # all of the utterance's audio has been handed out
-        first = max(st.chunk_frames, st.codec.min_frames)
+        sess = st.sess
         try:
-            with torch.cuda.device(dev):
+            with torch.cuda.device(sess.dev):
+                push = _PushStep(sess.model, sess.eng, sess.stream, st.tok, st.codec, st.cstream, st.chunk_frames,
+                                 st.poll_every, strict=True)
+                st.push = push
+                live = [_Utterance(s, i, f"utterance {i}") for i, s in enumerate(sess.slots)]
                 sess.sample()
                 while sess.steps % st.poll_every:
                     sess.step()
                 while True:
-                    done = sess.all_done()
-                    ids, lens, chunks, whole = [], [], [], []
-                    for i in range(B):
-                        if closed[i]:
+                    def advance(status):             # the next steps are queued while the codec works
+                        if not all(s.done for s in status):
+                            for _ in range(st.poll_every):
+                                sess.step()
+                    status, out, _ = push([r for r in live if not r.closed], advance)
+                    done = all(s.done for s in status)
+                    for r, w in out:
+                        if w is None:
                             continue
-                        fin = bool(sess.status[i].done)
-                        rows = sess.model._read_rows(sess.eng, sess.slots[i], sess.status[i].n_steps, sess.stream)
-                        f = final_frames(rows, K, end)
-                        new = f - pushed[i]
-                        if pushed[i] == 0 and fin and f < st.codec.min_frames:
-                            closed[i] = True
-                            if f > 0:
-                                whole.append((i, TtsStream._codes(st, i, rows, 0, f)))
-                            continue
-                        if new > 0 and (fin or new >= (first if pushed[i] == 0 else st.chunk_frames)):
-                            ids.append(i)
-                            lens.append(new)
-                            chunks.append(TtsStream._codes(st, i, rows, pushed[i], f))
-                            pushed[i] = f
-                        closed[i] = fin and pushed[i] == f
-                    wav = None
-                    if ids or whole:                 # the codec works on its own CUDA stream ...
-                        with torch.cuda.stream(st.cstream):
-                            if ids:
-                                T = max(lens)
-                                codes = np.zeros((len(ids), K, T), dtype=np.int64)
-                                for j, c in enumerate(chunks):
-                                    codes[j, :, :lens[j]] = c
-                                wav = st.codec.decode(torch.from_numpy(codes).to(dev), ids=ids, lens=lens)
-                            whole = [(i, st.tok.decode_codes(torch.from_numpy(c).unsqueeze(0).to(dev))) for i, c in whole]
-                        ev = torch.cuda.Event()
-                        ev.record(st.cstream)
-                    if not done:                     # ... while the next steps are already queued on the LM's
-                        for _ in range(st.poll_every):
-                            sess.step()
-                    if ids or whole:
-                        ev.synchronize()
-                        cur = torch.cuda.current_stream(dev)
-                        out = []
-                        if wav is not None:
-                            wav.record_stream(cur)
-                            out += [(i, wav[j:j + 1, :, :lens[j] * hop]) for j, i in enumerate(ids)]
-                        for i, w in whole:
-                            w.record_stream(cur)
-                            out.append((i, w))
-                        for i, w in sorted(out, key=lambda p: p[0]):
-                            if st.first_audio_steps is None:
-                                st.first_audio_steps = sess.steps
-                            yield i, w
-                    if done and all(closed):
+                        if st.first_audio_steps is None:
+                            st.first_audio_steps = sess.steps
+                        yield r.cid, w
+                    if done and all(r.closed for r in live):
                         break
                 st.results = sess.results()
                 if st.on_finish is not None:
@@ -826,6 +783,111 @@ class TtsStream:
                 st.codec.close()
                 st.codec = None
             sess.close()
+
+
+class _Utterance:
+    """An utterance of a streaming loop: engine slot, codec stream id, frames sent to the codec (pushed), all of its audio
+    handed out (closed)."""
+    __slots__ = ("slot", "cid", "label", "ticket", "pushed", "closed", "n_steps")
+
+    def __init__(self, slot, cid, label, ticket=None):
+        self.slot, self.cid, self.label, self.ticket = slot, cid, label, ticket
+        self.pushed, self.closed, self.n_steps = 0, False, 0
+
+
+class _PushStep:
+    """One poll of a streaming loop (TtsStream, ContinuousBatcher.stream).  vcb_poll_frames gathers the live utterances'
+    newly final frames on the device behind one wait; those with enough new frames go to the codec in one ragged call on
+    a second CUDA stream; the caller's next decode steps are enqueued; then the waveform is waited for.
+
+    An utterance (_Utterance) has its first chunk waits for max(chunk_frames, min_frames) frames, later ones for chunk_frames,
+    the last one takes what is left; one that ends with fewer than min_frames frames is decoded whole (decode_codes).
+    A chunk holding a non-audio code fails its utterance before any of its codes reach the codec: `strict` raises
+    VcbError before the codec is called at all."""
+
+    def __init__(self, model, eng, stream, tokenizer, codec, cstream, chunk_frames, poll_every, strict):
+        a = model.args
+        self.lib, self.eng, self.stream, self.tok, self.codec, self.cstream = _lib.load(), eng, stream, tokenizer, codec, cstream
+        self.dev, self.K, self.strict = model.mask_embedding.device, a.n_codebooks, strict
+        self.chunk_frames, self.first = chunk_frames, max(chunk_frames, codec.min_frames)
+        # new frames at one poll: fewer than a chunk's threshold were left over, plus at most one per row sampled since the
+        # last poll (a newly admitted utterance: its first sample and poll_every steps)
+        self.max_frames = self.first + poll_every + 1
+        self.offset = int(a.n_special) if a.special_first else 0
+        self.host_s = 0.0                    # host time in the step, outside the three device waits
+
+    def __call__(self, live, advance):
+        """live: utterances that are not closed.  advance(status) enqueues the next decode steps.  Returns (status, out,
+        failed): out lists (utterance, wav [1, channels, n*hop], or None when it closes with no new frames) in `live`
+        order; failed maps a failed utterance to its message.  Raises VcbError when a slot ran out of engine capacity."""
+        t_in = time.perf_counter()
+        n, mf, lib = len(live), self.max_frames, self.lib
+        codes = torch.empty((n, self.K, mf), dtype=torch.int64, device=self.dev)     # fresh: the codec stream reads it
+        status, final, bad = (_lib.vcb_status * n)(), (C.c_int32 * n)(), (C.c_int32 * (3 * n))()
+        t0 = time.perf_counter()
+        _lib.check(lib.vcb_poll_frames(self.eng, (C.c_int32 * n)(*[r.slot for r in live]), n,
+                                       (C.c_int32 * n)(*[r.pushed for r in live]), mf, self.offset,
+                                       int(self.tok.config.bins), codes.data_ptr(), status, final, bad, self.stream))
+        waited = time.perf_counter() - t0
+        if any(s.done == 2 for s in status):
+            raise _lib.VcbError("decode stopped: engine capacity (max_new_tokens / max_seq_len) exhausted; "
+                                "raise it with configure_engine()")
+        push, whole, failed = {}, {}, {}
+        for j, r in enumerate(live):
+            fin, f = bool(status[j].done), int(final[j])
+            new = f - r.pushed
+            if r.pushed == 0 and fin and f < self.codec.min_frames:
+                whole[j] = f
+            elif new > 0 and (fin or new >= (self.first if r.pushed == 0 else self.chunk_frames)):
+                push[j] = min(new, mf)
+            else:
+                r.closed = fin and r.pushed == f
+                continue
+            if bad[3 * j] >= 0:
+                failed[r] = (f"{r.label}: frame {bad[3 * j]} holds the non-audio token {bad[3 * j + 2]} in codebook "
+                             f"{bad[3 * j + 1]}; it has no waveform")
+                push.pop(j, None)
+                whole.pop(j, None)
+                r.closed = True
+                continue
+            r.pushed += push[j] if j in push else f
+            r.closed = fin and r.pushed == f
+        if failed and self.strict:
+            raise _lib.VcbError(next(iter(failed.values())))
+        wav, wavs = None, {}
+        if push or any(whole.values()):      # the codec works on its own CUDA stream ...
+            with torch.cuda.stream(self.cstream):
+                codes.record_stream(self.cstream)
+                if push:
+                    rows = list(push)
+                    wav = self.codec.decode(codes[rows, :, :max(push.values())], ids=[live[j].cid for j in rows],
+                                            lens=list(push.values()))
+                for j, f in whole.items():
+                    if f > 0:
+                        wavs[j] = self.tok.decode_codes(codes[j:j + 1, :, :f])
+            ev = torch.cuda.Event()
+            ev.record(self.cstream)
+        t1 = time.perf_counter()
+        advance(status)                      # ... while the next steps are already queued on the LM's
+        t2 = time.perf_counter()
+        out = []
+        if wav is not None or wavs:
+            ev.synchronize()
+            cur = torch.cuda.current_stream(self.dev)
+            if wav is not None:
+                wav.record_stream(cur)
+                for b, (j, nw) in enumerate(push.items()):
+                    wavs[j] = wav[b:b + 1, :, :nw * self.tok.hop]
+            for w in wavs.values():
+                w.record_stream(cur)
+        t3 = time.perf_counter()
+        for j, r in enumerate(live):
+            if j in wavs:
+                out.append((r, wavs[j]))
+            elif r.closed and r not in failed:
+                out.append((r, None))
+        self.host_s += (time.perf_counter() - t_in) - waited - (t2 - t1) - (t3 - t2)
+        return status, out, failed
 
 
 class _SingleTtsStream(TtsStream):
@@ -1003,6 +1065,8 @@ class ContinuousBatcher:
     are read, its slot and KV pages are released and the next queued utterance is prefilled into the free slot while the
     others keep decoding.  Every utterance owns its random stream (`seed`), so its result is exactly what
     ``torch.manual_seed(seed); model.inference_tts(x, x_lens, y, ...)`` returns, whatever it was batched with.
+    run() returns the token lists once the queue has drained; stream() hands out every utterance's audio while it is
+    generated and takes submit() / cancel() during the iteration.
     """
 
     def __init__(self, model: "VoiceCraft", max_concurrency=32, poll_every=8, top_k=-100, top_p=1.0, temperature=1.0,
@@ -1011,68 +1075,111 @@ class ContinuousBatcher:
         self.sp = model._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens)
         self.queue, self.slots, self._open = [], [], False
         self.stats = dict(steps=0, prefills=0, max_active=0)
+        self.results, self.errors = [], {}
+        self._live = None                  # the running stream()'s state
 
     def submit(self, x, y, seed=None):
-        """x [1,L] int64, y [1,T,K] int64 (host or device).  Returns the ticket (index into run()'s result list)."""
+        """x [1,L] int64, y [1,T,K] int64 (host or device).  Returns the ticket (index into run()'s result list / results).
+        While a stream() runs, the utterance is admitted at one of its next polls; one that does not fit the engine it
+        sized raises VcbError and is not queued."""
+        st = self._live
+        if st is not None:
+            job = self._job(x, y, seed)
+            if job["need_seq"] > st.max_seq:
+                raise _lib.VcbError(f"utterance needs {job['need_seq']} positions, the streaming engine holds {st.max_seq}: "
+                                    "configure_engine(max_seq_len=...) before stream()")
+            st.jobs.append(job)
+            self.results.append(None)
         self.queue.append((x, y, seed))
         return len(self.queue) - 1
 
+    def cancel(self, ticket) -> bool:
+        """stream(): a queued ticket is never admitted, an active one's slot is released at the next poll and nothing
+        more is yielded for it; results[ticket] stays None.  False if the ticket already handed out its last chunk."""
+        st = self._live
+        if st is None or not 0 <= ticket < len(st.jobs):
+            raise _lib.VcbError(f"no ticket {ticket} in a running stream()")
+        if ticket in st.ended:
+            return False
+        st.cancelled.add(ticket)
+        return True
+
+    def _job(self, x, y, seed):
+        m, a = self.model, self.model.args
+        K, dev = a.n_codebooks, m.mask_embedding.device
+        x = x.to(dev, non_blocking=True)
+        y = y.to(dev, non_blocking=True)
+        if a.special_first:
+            y = y + int(a.n_special)
+        yk = y.transpose(2, 1)[0].long().contiguous()
+        shifted, _ = m.shift([[yk]])
+        prompt = shifted[0][0][:, : -(K - 1)] if K > 1 else shifted[0][0]
+        y_tok = prompt.transpose(1, 0).contiguous()
+        x_ids = x[0].long().contiguous()
+        m._check_ids(x_ids, y_tok)
+        cap = int(x.shape[1]) * (int(a.encodec_sr) // 5)
+        need_seq = int(x.shape[1]) + max(int(y_tok.shape[0]), cap + 1) + K + 8
+        return dict(x_ids=x_ids, y_tok=y_tok, yk=yk, seed=seed, need_seq=need_seq)
+
+    def _admit(self, eng, new, jobs, stream):
+        """one packed prefill + the first sampling step of the newcomers [(slot, ticket)]"""
+        m, lib = self.model, _lib.load()
+        dev = m.mask_embedding.device
+        gen0 = torch.cuda.default_generators[dev.index or 0]
+        seed0, threads = int(gen0.initial_seed()), m._rng_threads(dev, m.args.n_codebooks * m.n_audio_tokens[0])
+        P = (_lib.vcb_prompt * len(new))()
+        for j, (slot, ji) in enumerate(new):
+            J = jobs[ji]
+            P[j] = _lib.vcb_prompt(slot=slot, n_copies=1, mode=0, x_len=int(J["x_ids"].shape[0]),
+                                   text_ids_dev=J["x_ids"].data_ptr(), y_len=int(J["y_tok"].shape[0]),
+                                   y_tokens_dev=J["y_tok"].data_ptr(), mask_rows_dev=None, n_more_spans=0)
+            P[j].rng_seed = (int(J["seed"]) if J["seed"] is not None else seed0 + ji) & 0xFFFFFFFFFFFFFFFF
+            P[j].rng_offset = 0
+            P[j].rng_threads = threads
+        _lib.check(lib.vcb_prefill(eng, P, len(new), stream))
+        c_new = (C.c_int32 * len(new))(*[s for s, _ in new])
+        _lib.check(lib.vcb_sample(eng, c_new, len(new), None, C.byref(self.sp), stream))
+        self.stats["prefills"] += 1
+
+    def _result(self, eng, slot, n_steps, job, stream):
+        """(res, gen) of a finished slot, as inference_tts returns them"""
+        m, a = self.model, self.model.args
+        rows = m._read_rows(eng, slot, n_steps, stream)
+        gen = torch.from_numpy(VoiceCraft._undelay(rows, a.n_codebooks)).to(m.mask_embedding.device)
+        res = torch.cat([job["yk"], gen], dim=1).unsqueeze(0)
+        if a.special_first:
+            res, gen = res - int(a.n_special), gen - int(a.n_special)
+        return res, gen.unsqueeze(0)
+
     @torch.no_grad()
     def run(self):
-        m, a = self.model, self.model.args
+        m = self.model
         if m.noise_fn is not None:
             raise _lib.VcbError("ContinuousBatcher uses the per-utterance device generators (model.noise_fn must be None)")
-        K, dev, lib = a.n_codebooks, m.mask_embedding.device, _lib.load()
-        V = m.n_audio_tokens[0]
-        jobs, need_seq = [], 0
-        for x, y, seed in self.queue:
-            x = x.to(dev, non_blocking=True)
-            y = y.to(dev, non_blocking=True)
-            if a.special_first:
-                y = y + int(a.n_special)
-            yk = y.transpose(2, 1)[0].long().contiguous()
-            shifted, _ = m.shift([[yk]])
-            prompt = shifted[0][0][:, : -(K - 1)] if K > 1 else shifted[0][0]
-            y_tok = prompt.transpose(1, 0).contiguous()
-            x_ids = x[0].long().contiguous()
-            m._check_ids(x_ids, y_tok)
-            cap = int(x.shape[1]) * (int(a.encodec_sr) // 5)
-            need_seq = max(need_seq, int(x.shape[1]) + max(int(y_tok.shape[0]), cap + 1) + K + 8)
-            jobs.append(dict(x_ids=x_ids, y_tok=y_tok, yk=yk, seed=seed))
+        if self._live is not None:
+            raise _lib.VcbError("a stream() of this ContinuousBatcher is running")
+        dev, lib = m.mask_embedding.device, _lib.load()
+        jobs = [self._job(x, y, seed) for x, y, seed in self.queue]
         n_slots = min(self.B, max(1, len(jobs)))
-        eng = m._engine(need_slots=n_slots, need_seq=need_seq)
+        eng = m._engine(need_slots=n_slots, need_seq=max([J["need_seq"] for J in jobs], default=0))
         base = m._free_slots(n_slots, m._eng_opts["max_slots"])
         self.slots, self._open = [base + i for i in range(n_slots)], True
         m._sessions.add(self)
-        gen0 = torch.cuda.default_generators[dev.index or 0]
-        seed0, threads = int(gen0.initial_seed()), m._rng_threads(dev, K * V)
         free, active, results, nxt = list(self.slots), {}, [None] * len(jobs), 0
         try:
             with torch.cuda.device(dev):
                 stream = torch.cuda.current_stream().cuda_stream
                 steps = 0
                 while nxt < len(jobs) or active:
-                    # ---- refill free slots from the queue: one packed prefill + the first sampling step of the newcomers
+                    # ---- refill free slots from the queue
                     new = []
                     while free and nxt < len(jobs):
                         new.append((free.pop(0), nxt))
                         nxt += 1
                     if new:
-                        P = (_lib.vcb_prompt * len(new))()
-                        for j, (slot, ji) in enumerate(new):
-                            J = jobs[ji]
-                            P[j] = _lib.vcb_prompt(slot=slot, n_copies=1, mode=0, x_len=int(J["x_ids"].shape[0]),
-                                                   text_ids_dev=J["x_ids"].data_ptr(), y_len=int(J["y_tok"].shape[0]),
-                                                   y_tokens_dev=J["y_tok"].data_ptr(), mask_rows_dev=None, n_more_spans=0)
-                            P[j].rng_seed = (int(J["seed"]) if J["seed"] is not None else seed0 + ji) & 0xFFFFFFFFFFFFFFFF
-                            P[j].rng_offset = 0
-                            P[j].rng_threads = threads
-                        _lib.check(lib.vcb_prefill(eng, P, len(new), stream))
+                        self._admit(eng, new, jobs, stream)
                         for slot, ji in new:
                             active[slot] = ji
-                        c_new = (C.c_int32 * len(new))(*[s for s, _ in new])
-                        _lib.check(lib.vcb_sample(eng, c_new, len(new), None, C.byref(self.sp), stream))
-                        self.stats["prefills"] += 1
                     order = sorted(active)
                     c_slots = (C.c_int32 * len(order))(*order)
                     self.stats["max_active"] = max(self.stats["max_active"], len(order))
@@ -1088,12 +1195,7 @@ class ContinuousBatcher:
                                                 "raise it with configure_engine()")
                         if st.done:
                             ji = active.pop(slot)
-                            rows = m._read_rows(eng, slot, st.n_steps, stream)
-                            gen = torch.from_numpy(VoiceCraft._undelay(rows, K)).to(dev)
-                            res = torch.cat([jobs[ji]["yk"], gen], dim=1).unsqueeze(0)
-                            if a.special_first:
-                                res, gen = res - int(a.n_special), gen - int(a.n_special)
-                            results[ji] = (res, gen.unsqueeze(0))
+                            results[ji] = self._result(eng, slot, st.n_steps, jobs[ji], stream)
                             lib.vcb_release(eng, slot, 1)
                             free.append(slot)
                 self.stats["steps"] = steps
@@ -1104,3 +1206,151 @@ class ContinuousBatcher:
             m._sessions.discard(self)
             self.queue = []
         return results
+
+    def stream(self, tokenizer, chunk_frames: int = 25) -> "BatcherStream":
+        """run() with every utterance's audio handed out while it is generated: iterates (ticket, wav [1, channels, n*hop],
+        last).  A ticket's chunks, concatenated, equal ``tokenizer.decode_codes(gen)``; its last chunk has last=True
+        (an utterance that generated no frame yields one empty wav).  submit() and cancel() may be called from the loop
+        body.  Afterwards ``results[ticket]`` is (res, gen) as run() returns it, None for a cancelled or failed ticket;
+        ``errors[ticket]`` says why a ticket failed (a final frame holding a non-audio token: it yields (ticket, None,
+        True) and the others go on).  The engine gets `max_concurrency` slots, each with its own codec stream id."""
+        return BatcherStream(self, tokenizer, chunk_frames)
+
+
+class BatcherStream:
+    """Iterator of ContinuousBatcher.stream().  Closing it early (break, close(), garbage collection) releases the
+    batcher's engine slots and the codec streams."""
+
+    def __init__(self, cb: ContinuousBatcher, tokenizer, chunk_frames: int = 25):
+        m = cb.model
+        if m.noise_fn is not None:
+            raise _lib.VcbError("ContinuousBatcher uses the per-utterance device generators (model.noise_fn must be None)")
+        if cb._live is not None:
+            raise _lib.VcbError("a stream() of this ContinuousBatcher is already running")
+        if chunk_frames < 1:
+            raise ValueError("chunk_frames must be >= 1")
+        self._it = None
+        jobs = [cb._job(x, y, seed) for x, y, seed in cb.queue]
+        eng = m._engine(need_slots=cb.B, need_seq=max([J["need_seq"] for J in jobs], default=0))
+        base = m._free_slots(cb.B, m._eng_opts["max_slots"])
+        # the generator holds this state, not the BatcherStream: dropping the BatcherStream closes it at once
+        st = self._st = SimpleNamespace(cb=cb, eng=eng, base=base, max_seq=m._eng_opts["max_seq_len"], jobs=jobs,
+                                        cancelled=set(), ended=set(), tok=tokenizer, chunk_frames=int(chunk_frames),
+                                        dev=m.mask_embedding.device, codec=None, push=None)
+        cb.slots, cb._open = [base + i for i in range(cb.B)], True
+        m._sessions.add(cb)
+        cb.results, cb.errors, cb._live = [None] * len(jobs), {}, st
+        try:
+            st.codec = tokenizer.open_stream(max_streams=cb.B)
+            st.cstream = torch.cuda.Stream(device=st.dev)
+        except Exception:
+            self.close()
+            raise
+        self._it = self._run(st)
+
+    @property
+    def push_host_seconds(self):
+        """host time spent in the push steps so far, outside the device waits"""
+        return self._st.push.host_s if self._st.push is not None else 0.0
+
+    def __iter__(self):
+        return self
+
+    def __next__(self):
+        return next(self._it)
+
+    def close(self):
+        st = getattr(self, "_st", None)
+        if st is None:
+            return
+        if self._it is not None:
+            self._it.close()
+        BatcherStream._finish(st)
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @staticmethod
+    def _finish(st):
+        cb = st.cb
+        if cb._live is not st:
+            return
+        lib = _lib.load()
+        for slot in cb.slots:                # releasing a slot that is not open does nothing
+            lib.vcb_release(st.eng, slot, 1)
+        if st.codec is not None:
+            st.codec.close()
+            st.codec = None
+        cb._open, cb._live, cb.queue = False, None, []
+        cb.model._sessions.discard(cb)
+
+    @staticmethod
+    @torch.no_grad()
+    def _run(st):
+        cb, m, lib = st.cb, st.cb.model, _lib.load()
+        free, active, nxt = list(cb.slots), {}, 0        # active: slot -> _Utterance
+        try:
+            with torch.cuda.device(st.dev):
+                stream = torch.cuda.current_stream().cuda_stream
+                push = st.push = _PushStep(m, st.eng, stream, st.tok, st.codec, st.cstream, st.chunk_frames, cb.poll_every,
+                                           strict=False)
+                empty = torch.zeros(1, st.tok.channels, 0, device=st.dev)
+                while True:
+                    # ---- finished, failed and cancelled utterances leave
+                    for slot, r in list(active.items()):
+                        if r.closed or r.ticket in st.cancelled:
+                            if r.closed and r.ticket not in cb.errors:
+                                cb.results[r.ticket] = cb._result(st.eng, slot, r.n_steps, st.jobs[r.ticket], stream)
+                            lib.vcb_release(st.eng, slot, 1)
+                            del active[slot]
+                            free.append(slot)
+                    # ---- free slots take the next queued tickets; each slot owns codec stream id slot - base
+                    new = []
+                    while free and nxt < len(st.jobs):
+                        if nxt not in st.cancelled:
+                            new.append((free.pop(0), nxt))
+                        nxt += 1
+                    if new:
+                        cb._admit(st.eng, new, st.jobs, stream)
+                        st.codec.reset([slot - st.base for slot, _ in new])
+                        for slot, t in new:
+                            active[slot] = _Utterance(slot, slot - st.base, f"ticket {t}", ticket=t)
+                    if not active:
+                        break
+                    live = [active[s] for s in sorted(active)]
+                    cb.stats["max_active"] = max(cb.stats["max_active"], len(live))
+
+                    def advance(status):
+                        go = [r.slot for r, s in zip(live, status) if not s.done and not r.closed]
+                        if go:
+                            c_go = (C.c_int32 * len(go))(*go)
+                            for _ in range(cb.poll_every):
+                                _lib.check(lib.vcb_decode_step(st.eng, c_go, len(go), None, C.byref(cb.sp), stream))
+                            cb.stats["steps"] += cb.poll_every
+                    status, out, failed = push(live, advance)
+                    wavs = dict(out)
+                    for r, s in zip(live, status):
+                        r.n_steps = s.n_steps
+                        if r in failed:
+                            cb.errors[r.ticket] = failed[r]
+                        if r.closed:
+                            st.ended.add(r.ticket)
+                    for r in live:
+                        if r.ticket in st.cancelled and not r.closed:
+                            continue
+                        if r in failed:
+                            yield r.ticket, None, True
+                        elif r in wavs:
+                            w = wavs[r]
+                            yield r.ticket, (empty if w is None else w), r.closed
+        finally:
+            BatcherStream._finish(st)
