@@ -157,7 +157,8 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         self._eng_opts = dict(max_slots=8, max_seq_len=2048, max_new_tokens=4096, kv_dtype="bf16")
         self.noise_fn = None          # optional: callable(shape, device) -> fp32 Exp(1) tensor on `device`
         self.poll_every = 4           # inference_tts*: poll the done flag every N steps (device generator only)
-        self._sessions = set()        # open DecodeSessions (they hold engine slots; the engine is not rebuilt under them)
+        self._sessions = {}           # first slot -> slot list of every group held by a call, session or batcher (the engine
+                                      # is not rebuilt under them); read and written by _free_slots / _take_slots / _release_slots
         self.last_stats = {}
         self.trace_logits = None      # set to a list to collect the raw logits [n*K, V] of every sampling step
 
@@ -184,29 +185,54 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
 
     def _drop_engine(self):
         if getattr(self, "_eng", None) is not None:
-            live = [s for s in getattr(self, "_sessions", ()) if s._open]
-            if live:
-                raise _lib.VcbError(f"{len(live)} DecodeSession(s) still hold slots of this engine: close them before "
+            held = getattr(self, "_sessions", {})
+            if held:
+                raise _lib.VcbError(f"{len(held)} DecodeSession(s) still hold slots of this engine: close them before "
                                     "reconfiguring / moving / reloading the model")
             _lib.load().vcb_destroy(self._eng)
         self._eng = None
         self._eng_key = None
 
     def _free_slots(self, n, eng_slots):
-        """first of n consecutive engine slots not held by an open session (single calls and sessions share one engine)"""
-        used = set()
-        for s in self._sessions:
-            if s._open:
-                used.update(s.slots)
+        """first of n consecutive engine slots that no group holds"""
+        used = {s for slots in self._sessions.values() for s in slots}
         for base in range(0, eng_slots - n + 1):
             if not any((base + i) in used for i in range(n)):
                 return base
         raise _lib.VcbError("no free engine slots")
 
+    def _take_slots(self, n, need_seq=0):
+        """Hold n consecutive free engine slots: (engine, slot list).  Single calls, sessions and batchers share one engine;
+        it grows first when it is too small for the slots already held plus n, or for `need_seq` positions, but not while
+        anything is held.  Give the slots back with _release_slots."""
+        o = self._eng_opts
+        held = sum(len(s) for s in self._sessions.values())
+        if held + n > o["max_slots"] or need_seq > o["max_seq_len"]:
+            if held:
+                raise _lib.VcbError(f"engine too small (max_slots={o['max_slots']}, max_seq_len={o['max_seq_len']}) and "
+                                    f"{held} slot(s) are held by open DecodeSessions: close them or configure_engine() first")
+            o["max_slots"] = max(o["max_slots"], n)
+            o["max_seq_len"] = max(o["max_seq_len"], (need_seq + 255) // 256 * 256)
+            self._drop_engine()
+        eng = self._engine()
+        base = self._free_slots(n, o["max_slots"])
+        slots = self._sessions[base] = list(range(base, base + n))
+        return eng, slots
+
+    def _release_slots(self, held, starts=None, n_copies=1, keep_held=False):
+        """vcb_release the groups of n_copies slots that begin at `starts` (default: all of `held`, a list _take_slots
+        returned; releasing a slot that is not open does nothing), then give `held` back unless keep_held.  Does nothing
+        once `held` was given back."""
+        if self._sessions.get(held[0]) is not held:
+            return
+        for s in held[::n_copies] if starts is None else starts:
+            _lib.load().vcb_release(self._eng, s, n_copies)
+        if not keep_held:
+            del self._sessions[held[0]]
+
     def __del__(self):
         try:
-            for sess in list(getattr(self, "_sessions", ())):
-                sess.close()
+            self._sessions.clear()
             self._drop_engine()
         except Exception:
             pass
@@ -223,20 +249,11 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
             self._drop_engine()
         return out
 
-    def _engine(self, need_slots=1, need_seq=0):
+    def _engine(self):
         dev = self.mask_embedding.device
         if dev.type != "cuda":
             raise _lib.VcbError("VoiceCraft (H100) has no CPU path: move the model to a CUDA device (`.to('cuda')`)")
         o = self._eng_opts
-        held = sum(len(s.slots) for s in self._sessions if s._open)
-        need_slots += held
-        if need_slots > o["max_slots"] or need_seq > o["max_seq_len"]:
-            if held:
-                raise _lib.VcbError(f"engine too small (max_slots={o['max_slots']}, max_seq_len={o['max_seq_len']}) and "
-                                    f"{held} slot(s) are held by open DecodeSessions: close them or configure_engine() first")
-            o["max_slots"] = max(o["max_slots"], need_slots)
-            o["max_seq_len"] = max(o["max_seq_len"], (need_seq + 255) // 256 * 256)
-            self._drop_engine()
         key = (dev.index or 0, tuple(sorted(o.items())))
         if self._eng is not None and self._eng_key == key:
             return self._eng
@@ -310,60 +327,6 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
             patterns.append(pats)
         return shifted_y, patterns
 
-    def _run(self, eng, slots, n_rows, sp, stream, max_steps=None, speculative=False):
-        """prefill is done; run sample / decode_step until every listed slot's group is done.
-
-        Device generator (noise_fn is None): the sampler draws from the group's own Philox stream; a finished group
-        ignores further steps and consumes nothing, so the done flag is polled only every `poll_every` steps
-        (speculative, TTS) and the generator still ends exactly where the reference's would."""
-        lib = _lib.load()
-        a = self.args
-        dev = self.mask_embedding.device
-        K, V = a.n_codebooks, self.n_audio_tokens[0]
-        n = len(slots)
-        c_slots = (C.c_int32 * n)(*slots)
-        host_noise = self.noise_fn is not None
-        buf = torch.empty((n_rows * K, V), device=dev, dtype=torch.float32) if host_noise else None
-        status = (_lib.vcb_status * n)()
-        def trace():
-            if self.trace_logits is not None:
-                t = torch.empty(n_rows * K, V, device=dev, dtype=torch.float32)
-                _lib.check(lib.vcb_debug_logits(eng, t.data_ptr(), n_rows * K))
-                self.trace_logits.append(t)
-        every = max(1, int(self.poll_every)) if (speculative and not host_noise and self.trace_logits is None) else 1
-        noise = self._draw_noise(buf).data_ptr() if host_noise else None
-        _lib.check(lib.vcb_sample(eng, c_slots, n, noise, C.byref(sp), stream))
-        trace()
-        steps = 1
-        while True:
-            if steps % every == 0 or every == 1:
-                _lib.check(lib.vcb_poll(eng, c_slots, n, status, stream))
-                if any(s.done == 2 for s in status):
-                    raise _lib.VcbError("decode stopped: engine capacity (max_new_tokens / max_seq_len) exhausted; "
-                                        "raise it with configure_engine()")
-                if all(s.done for s in status):
-                    break
-            if max_steps is not None and steps >= max_steps:
-                break
-            forced = every == 1 and any(s.forced for s in status)
-            if host_noise and not forced:                # forced hand-over steps consume no random numbers
-                noise = self._draw_noise(buf).data_ptr()
-            _lib.check(lib.vcb_decode_step(eng, c_slots, n, noise, C.byref(sp), stream))
-            if not forced:
-                trace()
-            steps += 1
-        return status
-
-    def _device_rng(self, P, dev, n_rows):
-        """hand the model device's default generator stream to the prompt (no-op with a caller noise_fn)"""
-        if self.noise_fn is not None:
-            return None
-        gen = torch.cuda.default_generators[dev.index or 0]
-        P.rng_seed = int(gen.initial_seed()) & 0xFFFFFFFFFFFFFFFF
-        P.rng_offset = int(gen.get_offset())
-        P.rng_threads = self._rng_threads(dev, n_rows * self.args.n_codebooks * self.n_audio_tokens[0])
-        return gen
-
     def _read_rows(self, eng, slot, n_steps, stream):
         K = self.args.n_codebooks
         buf = (C.c_int32 * (n_steps * K))()
@@ -395,56 +358,21 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         return self._tts_impl(x, x_lens, y, top_k, top_p, temperature, stop_repetition, silence_tokens, batch_size)
 
     def _tts_impl(self, x, x_lens, y, top_k, top_p, temperature, stop_repetition, silence_tokens, n_copies):
-        a = self.args
-        K = a.n_codebooks
         assert x.ndim == 2, x.shape
         assert x_lens.ndim == 1, x_lens.shape
         assert y.ndim == 3, y.shape
-        dev = self.mask_embedding.device
-        x = x.to(dev)
-        y = y.to(dev)
-        if a.special_first:
-            y = y + int(a.n_special)
-        y = y.transpose(2, 1)                                     # [1,T,K] -> [1,K,T]
-        assert y.shape[0] == 1 and y.shape[1] == K, y.shape
+        assert y.shape[0] == 1 and y.shape[2] == self.args.n_codebooks, y.transpose(2, 1).shape
         logging.info(f"silence tokens: {silence_tokens}, note that if you are not using the pretrained encodec "
                      f"6f79c6a8, make sure you specified it yourself, rather than using the default")
-        shifted, _ = self.shift([[y[0].long()]])
-        prompt = shifted[0][0][:, : -(K - 1)] if K > 1 else shifted[0][0]     # voicecraft.py:967
-        y_tok = prompt.transpose(1, 0).contiguous()                           # [T+1, K]
-        x_len, y_len = int(x.shape[1]), int(y_tok.shape[0])
-        cap = x_len * (int(a.encodec_sr) // 5)
-        need_seq = x_len + max(y_len, cap + 1) + K + 8
-        eng = self._engine(need_slots=n_copies, need_seq=need_seq)
-        lib = _lib.load()
-        x_ids = x[0].long().contiguous()
-        self._check_ids(x_ids, y_tok)
-        sp = self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens)
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream().cuda_stream
-            base = self._free_slots(n_copies, self._eng_opts["max_slots"])
-            P = _lib.vcb_prompt(slot=base, n_copies=n_copies, mode=0, x_len=x_len, text_ids_dev=x_ids.data_ptr(),
-                                y_len=y_len, y_tokens_dev=y_tok.data_ptr(), mask_rows_dev=None, n_more_spans=0)
-            gen_state = self._device_rng(P, dev, n_copies)
-            _lib.check(lib.vcb_prefill(eng, C.byref(P), 1, stream))      # a failed prefill holds nothing
-            try:
-                slots = [base + i for i in range(n_copies)]
-                status = self._run(eng, slots, n_copies, sp, stream, speculative=True)
-                keep = status[0].keep if n_copies > 1 else 0
-                rows = self._read_rows(eng, base + keep, status[keep].n_steps, stream)
-                if gen_state is not None:
-                    gen_state.set_offset(int(status[0].rng_offset))
-            finally:
-                lib.vcb_release(eng, base, n_copies)
-        gen = torch.from_numpy(self._undelay(rows, K)).to(dev)
-        res = torch.cat([y[0].long(), gen], dim=1).unsqueeze(0)
-        expected = y.shape[2] + rows.shape[0] - K
-        assert res.shape == torch.Size((1, K, expected)), f"res.shape: {res.shape}, expected_y_len: {expected}"
-        if a.special_first:
-            res = res - int(a.n_special)
-            gen = gen - int(a.n_special)
-        self.last_stats = dict(steps=int(rows.shape[0]), keep=int(keep))
-        return res, gen.unsqueeze(0)
+        sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
+                             n_copies=n_copies)
+        try:
+            (res, gen), = sess._run_single()
+        finally:
+            sess.close()
+        keep = sess._kept(0, sess.status)
+        self.last_stats = dict(steps=int(sess.status[keep].n_steps), keep=int(keep))
+        return res, gen
 
     # ------------------------------------------------------------------------------------------------
     # speech editing  (reference voicecraft.py:561-906)
@@ -506,63 +434,20 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     def inference(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, mask_interval: torch.Tensor,
                   top_k: int = -100, top_p: float = 1.0, temperature: float = 1.0, stop_repetition: int = -1,
                   kvcache: int = 1, silence_tokens: List[int] = [1388, 1898, 131]) -> torch.Tensor:
-        a = self.args
-        K = a.n_codebooks
         assert x.ndim == 2, x.shape
         assert x_lens.ndim == 1, x_lens.shape
         assert y.ndim == 3, y.shape
-        dev = self.mask_embedding.device
-        x = x.to(dev)
-        y = y.to(dev)
-        if a.special_first:
-            y = y + int(a.n_special)
-        y = y.transpose(2, 1)
-        assert y.shape[0] == 1 and y.shape[1] == K, y.shape
+        assert y.shape[0] == 1 and y.shape[2] == self.args.n_codebooks, y.transpose(2, 1).shape
         assert mask_interval.shape == torch.Size((1, mask_interval.shape[1], 2)), mask_interval
-        spans = [(int(s), int(e)) for s, e in mask_interval[0].tolist()]
-        if len(spans) > min(8, int(a.max_n_spans)):
-            raise ValueError(f"{len(spans)} masked spans: at most min(8, max_n_spans={a.max_n_spans}) per utterance")
         logging.info(f"silence tokens: {silence_tokens}, note that if you are not using the pretrained encodec "
                      f"6f79c6a8, make sure you specified it yourself, rather than using the default")
-        y0 = y[0].long().contiguous()
-        y_tok, mask_rows, more_vals, non_mask = self._edit_prompt(y0, spans)
-        x_len, y_len = int(x.shape[1]), int(y_tok.shape[0])
-        cap = x_len * 10
-        need_seq = x_len + max(y_len, cap + 1) + (K + 3) * (len(spans) + 1) + 8
-        eng = self._engine(need_slots=1, need_seq=need_seq)
-        lib = _lib.load()
-        x_ids = x[0].long().contiguous()
-        self._check_ids(x_ids, y_tok)
-        sp = self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens)
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream().cuda_stream
-            base = self._free_slots(1, self._eng_opts["max_slots"])
-            P = _lib.vcb_prompt(slot=base, n_copies=1, mode=1, x_len=x_len, text_ids_dev=x_ids.data_ptr(), y_len=y_len,
-                                y_tokens_dev=y_tok.data_ptr(), mask_rows_dev=mask_rows.data_ptr(),
-                                n_more_spans=len(more_vals))
-            for i, v in enumerate(more_vals):
-                P.more_mask_rows[i] = int(v)
-            gen_state = self._device_rng(P, dev, 1)
-            _lib.check(lib.vcb_prefill(eng, C.byref(P), 1, stream))      # a failed prefill holds nothing
-            try:
-                status = self._run(eng, [base], 1, sp, stream)
-                rows = self._read_rows(eng, base, status[0].n_steps, stream)
-                ends = [status[0].span_ends[i] for i in range(status[0].n_spans_done)]
-                if gen_state is not None:
-                    gen_state.set_offset(int(status[0].rng_offset))
-            finally:
-                lib.vcb_release(eng, base, 1)
-        assert len(ends) == len(spans), f"len(generated): {len(ends)}, num_mask: {len(spans)}"
-        pieces, lo = [], 0
-        for (s0, s1), hi in zip(non_mask, ends):
-            pieces.append(y0[:, s0:s1])
-            pieces.append(torch.from_numpy(self._undelay(rows[lo:hi], K)).to(dev))
-            lo = hi
-        pieces.append(y0[:, non_mask[-1][0]: non_mask[-1][1]])
-        res = torch.cat(pieces, dim=1).unsqueeze(0)
-        if a.special_first:
-            res = res - int(a.n_special)
-        self.last_stats = dict(steps=int(rows.shape[0]))
+        sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
+                             mask_intervals=[mask_interval], n_copies=1)
+        try:
+            (res, _), = sess._run_single()
+        finally:
+            sess.close()
+        self.last_stats = dict(steps=int(sess.status[0].n_steps))
         return res
 
     # ------------------------------------------------------------------------------------------------
@@ -580,16 +465,7 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     @torch.no_grad()
     def inference_many(self, xs, ys, mask_intervals, poll_every: int = 4, **kw):
         """Batched counterpart of `inference` (speech editing) for independent utterances."""
-        sess = self.open_edit_session(xs, ys, mask_intervals, **kw)
-        try:
-            sess.sample()
-            while True:
-                if sess.steps % poll_every == 0 and sess.all_done():
-                    break
-                sess.step()
-            return [r[0] for r in sess.results()]
-        finally:
-            sess.close()
+        return [r[0] for r in self.open_edit_session(xs, ys, mask_intervals, **kw)._run_many(poll_every)]
 
     def open_tts_session(self, xs, ys, top_k=-100, top_p=1.0, temperature=1.0, stop_repetition=3,
                          silence_tokens=(1388, 1898, 131), seeds=None, noise_fns=None):
@@ -606,16 +482,7 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     @torch.no_grad()
     def inference_tts_many(self, xs, ys, poll_every: int = 8, **kw):
         """Returns a list of (res [1,K,T+G], gen [1,K,G]) like inference_tts, one per utterance."""
-        sess = self.open_tts_session(xs, ys, **kw)
-        try:
-            sess.sample()
-            while True:
-                if sess.steps % poll_every == 0 and sess.all_done():
-                    break
-                sess.step()
-            return sess.results()
-        finally:
-            sess.close()
+        return self.open_tts_session(xs, ys, **kw)._run_many(poll_every)
 
     # ------------------------------------------------------------------------------------------------
     # streaming: audio while the tokens are generated (TtsStream)
@@ -635,18 +502,9 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         returns: the utterance samples from the device generator's stream at its current offset and leaves it advanced by
         the steps it ran, as inference_tts does."""
         assert x.ndim == 2 and x.shape[0] == 1 and x_lens.ndim == 1 and y.ndim == 3 and y.shape[0] == 1, (x.shape, y.shape)
-        dev = self.mask_embedding.device
-        gen_state = None if self.noise_fn is not None else torch.cuda.default_generators[dev.index or 0]
-
-        def finish(st):
-            st.result = st.results[0]
-            if gen_state is not None:
-                gen_state.set_offset(int(st.sess.status[0].rng_offset))
-        # one utterance: the session's default stream is the device generator's (seed, offset), like _device_rng
-        sess = self.open_tts_session([x], [y], top_k=top_k, top_p=top_p, temperature=temperature,
-                                     stop_repetition=stop_repetition, silence_tokens=silence_tokens)
-        ts = _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every, on_finish=finish)
-        return ts
+        sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
+                             n_copies=1)
+        return _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every)
 
 
 def _end_token(a) -> int:
@@ -668,55 +526,126 @@ def frame_codes(rows: np.ndarray, K: int, t0: int, t1: int) -> np.ndarray:
     return np.stack([rows[t0 + k: t1 + k, k] for k in range(K)], axis=0)
 
 
-class TtsStream:
-    """Audio of a DecodeSession while it generates (VoiceCraft.inference_tts_stream / inference_tts_many_stream).
+def _check_capacity(status):
+    """a slot that ran out of max_new_tokens / max_seq_len stops with done == 2"""
+    if any(s.done == 2 for s in status):
+        raise _lib.VcbError("decode stopped: engine capacity (max_new_tokens / max_seq_len) exhausted; "
+                            "raise it with configure_engine()")
 
-    Iterating runs the session: every `poll_every` steps it polls, reads the token rows and sends each utterance's newly
-    final frames to the codec (a CodecStream on a second CUDA stream) -- all utterances with enough new frames in one call.
-    The next decode steps are enqueued before the chunk's waveform is waited for.  A chunk is the waveform of those frames,
-    bit-identical to the same samples of ``decode_codes`` of the utterance's whole generation.  An utterance's first
-    chunk waits for max(chunk_frames, min_frames) frames; one that ends with fewer than min_frames frames is decoded in one
-    ``decode_codes`` call.  Yields (i, wav [1, channels, n*hop]).  After the iteration, ``results`` holds what
-    ``DecodeSession.results()`` returns.  Closing it early (break, close(), garbage collection) releases the session's
-    engine slots and the codec streams."""
 
-    def __init__(self, sess: "DecodeSession", tokenizer, chunk_frames: int = 25, poll_every: int = 8, on_finish=None):
-        if chunk_frames < 1 or poll_every < 1:
-            raise ValueError("chunk_frames and poll_every must be >= 1")
-        # the generator holds this state, not the TtsStream: dropping the TtsStream closes it at once (no reference cycle)
-        st = self._st = SimpleNamespace(sess=sess, tok=tokenizer, chunk_frames=int(chunk_frames), poll_every=int(poll_every),
-                                        results=None, result=None, first_audio_steps=None, on_finish=on_finish, codec=None,
-                                        push=None)
-        self._it = None
+class _Prompt:
+    """One utterance's prompt, held on the model's device: the TTS layout (the prompt delayed by the codebook pattern,
+    reference voicecraft.py:961-967) or, given `spans`, the speech-editing layout (VoiceCraft._edit_prompt).  `need_seq`
+    bounds the engine positions its generation can reach.  Raises ValueError on more than 8 spans; the caller checks the
+    id ranges (VoiceCraft._check_ids) before it takes a slot."""
+
+    def __init__(self, model, x, y, spans=None):
+        a = model.args
+        K, dev = a.n_codebooks, model.mask_embedding.device
+        self.model, self.spans = model, spans
+        x = x.to(dev, non_blocking=True)
+        y = y.to(dev, non_blocking=True)
+        if a.special_first:
+            y = y + int(a.n_special)
+        self.y0 = y.transpose(2, 1)[0].long().contiguous()                       # [1,T,K] -> [K,T]
+        self.x_ids = x[0].long().contiguous()
+        x_len = int(self.x_ids.shape[0])
+        if spans is None:
+            shifted, _ = model.shift([[self.y0]])
+            prompt = shifted[0][0][:, : -(K - 1)] if K > 1 else shifted[0][0]     # voicecraft.py:967
+            self.y_tok = prompt.transpose(1, 0).contiguous()                      # [T+1, K]
+            self.mask_rows, self.more_vals = None, []
+            cap, extra = x_len * (int(a.encodec_sr) // 5), K
+        else:
+            if len(spans) > min(8, int(a.max_n_spans)):
+                raise ValueError(f"{len(spans)} masked spans: at most min(8, max_n_spans={a.max_n_spans}) per utterance")
+            self.y_tok, self.mask_rows, self.more_vals, self.non_mask = model._edit_prompt(self.y0, spans)
+            cap, extra = x_len * 10, (K + 3) * (len(spans) + 1)
+        self.need_seq = x_len + max(int(self.y_tok.shape[0]), cap + 1) + extra + 8
+
+    def fill(self, slot, n_copies, seed=None, offset=0):
+        """its vcb_prompt in slots slot .. slot+n_copies-1, sampling from the Philox stream of a torch CUDA generator at
+        (seed, offset); seed None: host noise"""
+        P = _lib.vcb_prompt(slot=slot, n_copies=n_copies, mode=0 if self.spans is None else 1,
+                            x_len=int(self.x_ids.shape[0]), text_ids_dev=self.x_ids.data_ptr(),
+                            y_len=int(self.y_tok.shape[0]), y_tokens_dev=self.y_tok.data_ptr(),
+                            mask_rows_dev=None if self.mask_rows is None else self.mask_rows.data_ptr(),
+                            n_more_spans=len(self.more_vals))
+        for i, v in enumerate(self.more_vals):
+            P.more_mask_rows[i] = int(v)
+        if seed is not None:
+            m = self.model
+            P.rng_seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+            P.rng_offset = int(offset)
+            # the group's draw per sampling step is [n_copies*K, V], as the reference's multinomial
+            P.rng_threads = m._rng_threads(self.y0.device, n_copies * m.args.n_codebooks * m.n_audio_tokens[0])
+        return P
+
+    def result(self, rows, st):
+        """(res [1,K,T+G], gen [1,K,G]) as inference_tts returns them, or (res, None) with res as inference returns it,
+        from the utterance's delayed token rows [n,K] and its vcb_status.  A TTS utterance that is not done (a truncated
+        session) keeps its final frames only: the still-delayed tail is dropped."""
+        a = self.model.args
+        K, dev = a.n_codebooks, self.y0.device
+        gen = None
+        if self.spans is None:
+            n = rows.shape[0] - K if st.done else final_frames(rows, K, _end_token(a))
+            gen = torch.from_numpy(frame_codes(rows, K, 0, n)).to(dev)
+            res = torch.cat([self.y0, gen], dim=1).unsqueeze(0)
+            expected = self.y0.shape[1] + n
+            assert res.shape == torch.Size((1, K, expected)), f"res.shape: {res.shape}, expected_y_len: {expected}"
+        else:
+            assert st.done, "edit session results() needs finished utterances"
+            ends = [st.span_ends[j] for j in range(st.n_spans_done)]
+            assert len(ends) == len(self.spans), f"len(generated): {len(ends)}, num_mask: {len(self.spans)}"
+            pieces, lo = [], 0
+            for (s0, s1), hi in zip(self.non_mask, ends):
+                pieces.append(self.y0[:, s0:s1])
+                pieces.append(torch.from_numpy(VoiceCraft._undelay(rows[lo:hi], K)).to(dev))
+                lo = hi
+            pieces.append(self.y0[:, self.non_mask[-1][0]: self.non_mask[-1][1]])
+            res = torch.cat(pieces, dim=1).unsqueeze(0)
+        if a.special_first:
+            res = res - int(a.n_special)
+            gen = None if gen is None else gen - int(a.n_special)
+        return res, None if gen is None else gen.unsqueeze(0)
+
+
+def _prefill(eng, prompts, stream):
+    """one packed prefill of [(_Prompt, slot, n_copies, seed, offset)] (see _Prompt.fill); a failed prefill holds nothing"""
+    P = (_lib.vcb_prompt * len(prompts))()
+    for j, (p, *where) in enumerate(prompts):
+        P[j] = p.fill(*where)
+    _lib.check(_lib.load().vcb_prefill(eng, P, len(prompts), stream))
+
+
+class _AudioStream:
+    """The iterator of a streaming loop (TtsStream, BatcherStream).  Its state `st` is held by the loop's generator
+    `_run(st)`, not by the iterator, so dropping the iterator closes it at once (no reference cycle).  Closing it early
+    (break, close(), garbage collection) runs `_finish(st)`, which releases the engine slots and the codec streams."""
+
+    def _start(self, st, n_streams):
+        """open n_streams codec streams and the codec's CUDA stream on st.dev, then the loop"""
+        self._st, self._it = st, None
+        st.codec = st.push = None
         try:
-            st.codec = tokenizer.open_stream(max_streams=sess.B)
-            st.cstream = torch.cuda.Stream(device=sess.dev)
+            st.codec = st.tok.open_stream(max_streams=n_streams)
+            st.cstream = torch.cuda.Stream(device=st.dev)
         except Exception:
             self.close()
             raise
         self._it = self._run(st)
 
-    @property
-    def results(self):
-        return self._st.results
-
-    @property
-    def result(self):
-        return self._st.result
-
-    @property
-    def first_audio_steps(self):
-        """session steps taken when the first chunk was handed out"""
-        return self._st.first_audio_steps
+    @staticmethod
+    def _close_codec(st):
+        if st.codec is not None:
+            st.codec.close()
+            st.codec = None
 
     @property
     def push_host_seconds(self):
         """host time spent in the push steps so far, outside the device waits"""
         return self._st.push.host_s if self._st.push is not None else 0.0
-
-    @property
-    def sess(self):
-        return self._st.sess
 
     def __iter__(self):
         return self
@@ -730,10 +659,7 @@ class TtsStream:
             return
         if self._it is not None:
             self._it.close()
-        if st.codec is not None:
-            st.codec.close()
-            st.codec = None
-        st.sess.close()
+        self._finish(st)
 
     def __enter__(self):
         return self
@@ -746,6 +672,43 @@ class TtsStream:
             self.close()
         except Exception:
             pass
+
+
+class TtsStream(_AudioStream):
+    """Audio of a DecodeSession while it generates (VoiceCraft.inference_tts_stream / inference_tts_many_stream).
+
+    Iterating runs the session: every `poll_every` steps it polls, reads the token rows and sends each utterance's newly
+    final frames to the codec (a CodecStream on a second CUDA stream) -- all utterances with enough new frames in one call.
+    The next decode steps are enqueued before the chunk's waveform is waited for.  A chunk is the waveform of those frames,
+    bit-identical to the same samples of ``decode_codes`` of the utterance's whole generation.  An utterance's first
+    chunk waits for max(chunk_frames, min_frames) frames; one that ends with fewer than min_frames frames is decoded in one
+    ``decode_codes`` call.  Yields (i, wav [1, channels, n*hop]).  After the iteration, ``results`` holds what
+    ``DecodeSession.results()`` returns.  Closing it early (break, close(), garbage collection) releases the session's
+    engine slots and the codec streams."""
+
+    def __init__(self, sess: "DecodeSession", tokenizer, chunk_frames: int = 25, poll_every: int = 8):
+        if chunk_frames < 1 or poll_every < 1:
+            raise ValueError("chunk_frames and poll_every must be >= 1")
+        self._start(SimpleNamespace(sess=sess, dev=sess.dev, tok=tokenizer, chunk_frames=int(chunk_frames),
+                                    poll_every=int(poll_every), results=None, first_audio_steps=None), sess.B)
+
+    @property
+    def results(self):
+        return self._st.results
+
+    @property
+    def first_audio_steps(self):
+        """session steps taken when the first chunk was handed out"""
+        return self._st.first_audio_steps
+
+    @property
+    def sess(self):
+        return self._st.sess
+
+    @staticmethod
+    def _finish(st):
+        _AudioStream._close_codec(st)
+        st.sess.close()
 
     @staticmethod
     @torch.no_grad()
@@ -776,23 +739,18 @@ class TtsStream:
                     if done and all(r.closed for r in live):
                         break
                 st.results = sess.results()
-                if st.on_finish is not None:
-                    st.on_finish(st)
         finally:
-            if st.codec is not None:
-                st.codec.close()
-                st.codec = None
-            sess.close()
+            TtsStream._finish(st)
 
 
 class _Utterance:
     """An utterance of a streaming loop: engine slot, codec stream id, frames sent to the codec (pushed), all of its audio
-    handed out (closed)."""
-    __slots__ = ("slot", "cid", "label", "ticket", "pushed", "closed", "n_steps")
+    handed out (closed), its vcb_status at the last poll."""
+    __slots__ = ("slot", "cid", "label", "ticket", "pushed", "closed", "status")
 
     def __init__(self, slot, cid, label, ticket=None):
         self.slot, self.cid, self.label, self.ticket = slot, cid, label, ticket
-        self.pushed, self.closed, self.n_steps = 0, False, 0
+        self.pushed, self.closed, self.status = 0, False, None
 
 
 class _PushStep:
@@ -829,9 +787,7 @@ class _PushStep:
                                        (C.c_int32 * n)(*[r.pushed for r in live]), mf, self.offset,
                                        int(self.tok.config.bins), codes.data_ptr(), status, final, bad, self.stream))
         waited = time.perf_counter() - t0
-        if any(s.done == 2 for s in status):
-            raise _lib.VcbError("decode stopped: engine capacity (max_new_tokens / max_seq_len) exhausted; "
-                                "raise it with configure_engine()")
+        _check_capacity(status)
         push, whole, failed = {}, {}, {}
         for j, r in enumerate(live):
             fin, f = bool(status[j].done), int(final[j])
@@ -896,123 +852,132 @@ class _SingleTtsStream(TtsStream):
     def __next__(self):
         return next(self._it)[1]
 
+    @property
+    def result(self):
+        return None if self.results is None else self.results[0]
+
 
 class DecodeSession:
     """A batch of independent utterances resident in the engine, one slot and one random stream each."""
 
-    def __init__(self, model: "VoiceCraft", xs, ys, sp, mask_intervals=None, seeds=None, noise_fns=None):
-        a = model.args
-        self.edit = mask_intervals is not None
-        self.non_mask = []
-        K = a.n_codebooks
+    def __init__(self, model: "VoiceCraft", xs, ys, sp, mask_intervals=None, seeds=None, noise_fns=None, *, n_copies=None):
+        """n_copies (the single calls inference_tts, inference_tts_batch, inference and inference_tts_stream): the one
+        utterance is sampled in n_copies slots (best-of-N) from the device generator's stream at its current offset, and
+        results() leaves the generator advanced as the single call does."""
+        K = model.args.n_codebooks
         dev = model.mask_embedding.device
         self.model, self.sp, self.dev, self.K = model, sp, dev, K
-        self.B = len(xs)
+        self.B, self.V, self.n_copies = len(xs), model.n_audio_tokens[0], n_copies or 1
         self.lib = _lib.load()
-        self._open = False
-        self.slots = []
-        prompts, keep_alive, need_seq = [], [], 0
-        self.y0 = []
+        self.edit = mask_intervals is not None
         if seeds is not None and len(seeds) != self.B:
             raise ValueError("seeds: one per utterance")
         if noise_fns is not None and len(noise_fns) != self.B:
             raise ValueError("noise_fns: one per utterance")
-        for x, y in zip(xs, ys):
+        self.prompts = []
+        for i, (x, y) in enumerate(zip(xs, ys)):
             assert x.ndim == 2 and y.ndim == 3 and y.shape[2] == K
-            x = x.to(dev, non_blocking=True)
-            y = y.to(dev, non_blocking=True)
-            if a.special_first:
-                y = y + int(a.n_special)
-            yk = y.transpose(2, 1)[0].long().contiguous()
-            idx = len(prompts)
-            if self.edit:
-                spans = [(int(s), int(e)) for s, e in mask_intervals[idx][0].tolist()]
-                if len(spans) > min(8, int(a.max_n_spans)):
-                    raise ValueError(f"{len(spans)} masked spans: at most min(8, max_n_spans={a.max_n_spans}) per utterance")
-                y_tok, mask_rows, more_vals, non_mask = model._edit_prompt(yk, spans)
-                self.non_mask.append(non_mask)
-                cap = int(x.shape[1]) * 10
-                extra = (K + 3) * (len(spans) + 1)
-            else:
-                shifted, _ = model.shift([[yk]])
-                prompt = shifted[0][0][:, : -(K - 1)] if K > 1 else shifted[0][0]
-                y_tok = prompt.transpose(1, 0).contiguous()
-                mask_rows, more_vals = None, []
-                cap = int(x.shape[1]) * (int(a.encodec_sr) // 5)
-                extra = K
-            x_ids = x[0].long().contiguous()
-            keep_alive += [y_tok, x_ids, mask_rows]
-            self.y0.append(yk)
-            need_seq = max(need_seq, int(x.shape[1]) + max(int(y_tok.shape[0]), cap + 1) + extra + 8)
-            prompts.append((int(x.shape[1]), x_ids, int(y_tok.shape[0]), y_tok, mask_rows, more_vals))
+            spans = [(int(s), int(e)) for s, e in mask_intervals[i][0].tolist()] if self.edit else None
+            self.prompts.append(_Prompt(model, x, y, spans))
         # one range check for the whole batch (the reference's embedding lookups raise on a bad id)
-        model._check_ids(torch.cat([p[1] for p in prompts]), torch.cat([p[3].reshape(-1) for p in prompts]))
-        self.eng = model._engine(need_slots=self.B, need_seq=need_seq)
-        self.V = model.n_audio_tokens[0]
-        base = model._free_slots(self.B, model._eng_opts["max_slots"])
-        slots = [base + i for i in range(self.B)]
-        # random streams: caller noise (model.noise_fn: one [B*K,V] draw per step; noise_fns: one [K,V] draw per utterance
-        # and step) or, by default, one Philox stream per utterance generated inside the sampler kernel
-        self._noise_fns = noise_fns
-        self._host_noise = noise_fns is not None or model.noise_fn is not None
-        self._buf = torch.empty((self.B * K, self.V), device=dev, dtype=torch.float32) if self._host_noise else None
-        gen = torch.cuda.default_generators[dev.index or 0]
-        seed0, off0 = int(gen.initial_seed()), int(gen.get_offset())
-        threads = model._rng_threads(dev, K * self.V)
-        P = (_lib.vcb_prompt * self.B)()
-        for i, (xl, x_ids, yl, y_tok, mask_rows, more_vals) in enumerate(prompts):
-            P[i] = _lib.vcb_prompt(slot=slots[i], n_copies=1, mode=1 if self.edit else 0, x_len=xl, text_ids_dev=x_ids.data_ptr(),
-                                   y_len=yl, y_tokens_dev=y_tok.data_ptr(),
-                                   mask_rows_dev=mask_rows.data_ptr() if mask_rows is not None else None,
-                                   n_more_spans=len(more_vals))
-            for j, v in enumerate(more_vals):
-                P[i].more_mask_rows[j] = int(v)
-            if not self._host_noise:
-                P[i].rng_seed = (int(seeds[i]) if seeds is not None else seed0 + i) & 0xFFFFFFFFFFFFFFFF
-                P[i].rng_offset = 0 if seeds is not None else off0
-                P[i].rng_threads = threads
-        self.c_slots = (C.c_int32 * self.B)(*slots)
-        self.status = (_lib.vcb_status * self.B)()
-        self.steps = 0
-        with torch.cuda.device(dev):
-            self.stream = torch.cuda.current_stream().cuda_stream
-            _lib.check(self.lib.vcb_prefill(self.eng, P, self.B, self.stream))     # a failed prefill holds nothing
-        self.slots = slots
-        self._open = True
-        model._sessions.add(self)
-        self._keep_alive = keep_alive
+        model._check_ids(torch.cat([p.x_ids for p in self.prompts]), torch.cat([p.y_tok.reshape(-1) for p in self.prompts]))
+        self.eng, self.slots = model._take_slots(self.B * self.n_copies, max(p.need_seq for p in self.prompts))
+        try:
+            n = len(self.slots)
+            # random streams: caller noise (model.noise_fn: one [B*K,V] draw per step; noise_fns: one [K,V] draw per
+            # utterance and step) or, by default, one Philox stream per utterance generated inside the sampler kernel
+            self._noise_fns = noise_fns
+            self._host_noise = noise_fns is not None or model.noise_fn is not None
+            self._buf = torch.empty((n * K, self.V), device=dev, dtype=torch.float32) if self._host_noise else None
+            gen = torch.cuda.default_generators[dev.index or 0]
+            seed0, off0 = int(gen.initial_seed()), int(gen.get_offset())
+            self._gen = gen if n_copies is not None and not self._host_noise else None
+            # (seed, offset) per utterance; a single call's (seed0, off0) is the device generator's own stream
+            streams = [(None, 0) if self._host_noise else (seeds[i], 0) if seeds is not None else (seed0 + i, off0)
+                       for i in range(self.B)]
+            self.c_slots = (C.c_int32 * n)(*self.slots)
+            self.status = (_lib.vcb_status * n)()
+            self.steps = 0
+            with torch.cuda.device(dev):
+                self.stream = torch.cuda.current_stream().cuda_stream
+                _prefill(self.eng, [(p, self.slots[i * self.n_copies], self.n_copies, *streams[i])
+                                    for i, p in enumerate(self.prompts)], self.stream)
+        except BaseException:
+            self.close()                     # a failed prefill holds nothing: give the slots back
+            raise
 
-    def _noise(self):
+    def _noise(self, draw=True):
+        """the host noise buffer (None: the device streams), refilled unless draw is False"""
         if not self._host_noise:
             return None
-        if self._noise_fns is not None:
+        if draw and self._noise_fns is not None:
             K = self.K
             for i, fn in enumerate(self._noise_fns):
                 self._buf[i * K:(i + 1) * K].copy_(fn((K, self.V), self.dev).to(device=self.dev, dtype=torch.float32))
-        else:
+        elif draw:
             self.model._draw_noise(self._buf)
         return self._buf.data_ptr()
 
+    def _launch(self, fn, noise):
+        _lib.check(fn(self.eng, self.c_slots, len(self.slots), noise, C.byref(self.sp), self.stream))
+        self.steps += 1
+
     def sample(self):
         """first sampling step (on the prefill's last hidden states)"""
-        _lib.check(self.lib.vcb_sample(self.eng, self.c_slots, self.B, self._noise(), C.byref(self.sp), self.stream))
-        self.steps += 1
+        self._launch(self.lib.vcb_sample, self._noise())
 
     def step(self):
         # edit sessions: forced hand-over steps of individual utterances ignore their noise rows / consume no draw
-        _lib.check(self.lib.vcb_decode_step(self.eng, self.c_slots, self.B, self._noise(), C.byref(self.sp), self.stream))
-        self.steps += 1
+        self._launch(self.lib.vcb_decode_step, self._noise())
 
     def poll(self):
-        _lib.check(self.lib.vcb_poll(self.eng, self.c_slots, self.B, self.status, self.stream))
+        _lib.check(self.lib.vcb_poll(self.eng, self.c_slots, len(self.slots), self.status, self.stream))
         return self.status
 
     def all_done(self):
         st = self.poll()
-        if any(s.done == 2 for s in st):
-            raise _lib.VcbError("decode stopped: engine capacity (max_new_tokens / max_seq_len) exhausted; "
-                                "raise it with configure_engine()")
+        _check_capacity(st)
         return all(s.done for s in st)
+
+    def _run_many(self, poll_every):
+        """inference_many / inference_tts_many: sample and step until every utterance is done, polling every
+        `poll_every` steps; returns results() and closes the session"""
+        try:
+            self.sample()
+            while True:
+                if self.steps % poll_every == 0 and self.all_done():
+                    break
+                self.step()
+            return self.results()
+        finally:
+            self.close()
+
+    def _run_single(self):
+        """The loop of a single call; returns results().  The done flag is polled every model.poll_every steps: a finished
+        group ignores further steps and consumes nothing, so the device generator still ends exactly where the reference's
+        would.  Edits, host noise and trace_logits poll every step; a forced hand-over step then draws no host noise and
+        appends no trace."""
+        m = self.model
+        every = 1 if (self.edit or self._host_noise or m.trace_logits is not None) else max(1, int(m.poll_every))
+        with torch.cuda.device(self.dev):
+            self.sample()
+            self._trace()
+            while True:
+                if self.steps % every == 0 and self.all_done():
+                    break
+                forced = every == 1 and any(s.forced for s in self.status)
+                self._launch(self.lib.vcb_decode_step, self._noise(draw=not forced))
+                if not forced:
+                    self._trace()
+            return self._results(self.status)
+
+    def _trace(self):
+        """append the raw logits [n*K, V] of the last sampling step to model.trace_logits (when it is a list)"""
+        if self.model.trace_logits is not None:
+            rows = len(self.slots) * self.K
+            t = torch.empty(rows, self.V, device=self.dev, dtype=torch.float32)
+            _lib.check(self.lib.vcb_debug_logits(self.eng, t.data_ptr(), rows))
+            self.model.trace_logits.append(t)
 
     def raw_tokens(self, i):
         """delayed token rows [n_steps, K] of utterance i (host numpy)"""
@@ -1020,41 +985,24 @@ class DecodeSession:
         return self.model._read_rows(self.eng, self.slots[i], st[i].n_steps, self.stream)
 
     def results(self):
+        return self._results(self.poll())
+
+    def _kept(self, i, st):
+        """index in `st` of utterance i's result: the copy of its best-of-N group that ended first, or its slot"""
+        j = i * self.n_copies
+        return j + (st[j].keep if self.n_copies > 1 else 0)
+
+    def _results(self, st):
         out = []
-        a = self.model.args
-        st = self.poll()
-        for i in range(self.B):
-            rows = self.model._read_rows(self.eng, self.slots[i], st[i].n_steps, self.stream)
-            if self.edit:
-                assert st[i].done, "edit session results() needs finished utterances"
-                ends = [st[i].span_ends[j] for j in range(st[i].n_spans_done)]
-                pieces, lo = [], 0
-                for (s0, s1), hi in zip(self.non_mask[i], ends):
-                    pieces.append(self.y0[i][:, s0:s1])
-                    pieces.append(torch.from_numpy(VoiceCraft._undelay(rows[lo:hi], self.K)).to(self.dev))
-                    lo = hi
-                pieces.append(self.y0[i][:, self.non_mask[i][-1][0]: self.non_mask[i][-1][1]])
-                res = torch.cat(pieces, dim=1).unsqueeze(0)
-                if a.special_first:
-                    res = res - int(a.n_special)
-                out.append((res, None))
-                continue
-            if st[i].done:
-                gen = torch.from_numpy(VoiceCraft._undelay(rows, self.K)).to(self.dev)
-            else:       # truncated session: the final frames only (the still-delayed tail is dropped)
-                gen = torch.from_numpy(frame_codes(rows, self.K, 0, final_frames(rows, self.K, _end_token(a)))).to(self.dev)
-            res = torch.cat([self.y0[i], gen], dim=1).unsqueeze(0)
-            if a.special_first:
-                res, gen = res - int(a.n_special), gen - int(a.n_special)
-            out.append((res, gen.unsqueeze(0)))
+        for i, p in enumerate(self.prompts):
+            j = self._kept(i, st)
+            out.append(p.result(self.model._read_rows(self.eng, self.slots[j], st[j].n_steps, self.stream), st[j]))
+        if self._gen is not None:
+            self._gen.set_offset(int(st[0].rng_offset))
         return out
 
     def close(self):
-        if self._open:
-            for s in self.slots:
-                self.lib.vcb_release(self.eng, s, 1)
-            self._open = False
-        self.model._sessions.discard(self)
+        self.model._release_slots(self.slots, n_copies=self.n_copies)
 
 
 class ContinuousBatcher:
@@ -1073,7 +1021,7 @@ class ContinuousBatcher:
                  stop_repetition=3, silence_tokens=(1388, 1898, 131)):
         self.model, self.B, self.poll_every = model, int(max_concurrency), max(1, int(poll_every))
         self.sp = model._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens)
-        self.queue, self.slots, self._open = [], [], False
+        self.queue = []
         self.stats = dict(steps=0, prefills=0, max_active=0)
         self.results, self.errors = [], {}
         self._live = None                  # the running stream()'s state
@@ -1085,8 +1033,8 @@ class ContinuousBatcher:
         st = self._live
         if st is not None:
             job = self._job(x, y, seed)
-            if job["need_seq"] > st.max_seq:
-                raise _lib.VcbError(f"utterance needs {job['need_seq']} positions, the streaming engine holds {st.max_seq}: "
+            if job[0].need_seq > st.max_seq:
+                raise _lib.VcbError(f"utterance needs {job[0].need_seq} positions, the streaming engine holds {st.max_seq}: "
                                     "configure_engine(max_seq_len=...) before stream()")
             st.jobs.append(job)
             self.results.append(None)
@@ -1105,51 +1053,24 @@ class ContinuousBatcher:
         return True
 
     def _job(self, x, y, seed):
-        m, a = self.model, self.model.args
-        K, dev = a.n_codebooks, m.mask_embedding.device
-        x = x.to(dev, non_blocking=True)
-        y = y.to(dev, non_blocking=True)
-        if a.special_first:
-            y = y + int(a.n_special)
-        yk = y.transpose(2, 1)[0].long().contiguous()
-        shifted, _ = m.shift([[yk]])
-        prompt = shifted[0][0][:, : -(K - 1)] if K > 1 else shifted[0][0]
-        y_tok = prompt.transpose(1, 0).contiguous()
-        x_ids = x[0].long().contiguous()
-        m._check_ids(x_ids, y_tok)
-        cap = int(x.shape[1]) * (int(a.encodec_sr) // 5)
-        need_seq = int(x.shape[1]) + max(int(y_tok.shape[0]), cap + 1) + K + 8
-        return dict(x_ids=x_ids, y_tok=y_tok, yk=yk, seed=seed, need_seq=need_seq)
+        """(prompt, seed) of a ticket; raises IndexError on an out-of-range id"""
+        p = _Prompt(self.model, x, y)
+        self.model._check_ids(p.x_ids, p.y_tok)
+        return p, seed
 
     def _admit(self, eng, new, jobs, stream):
         """one packed prefill + the first sampling step of the newcomers [(slot, ticket)]"""
         m, lib = self.model, _lib.load()
-        dev = m.mask_embedding.device
-        gen0 = torch.cuda.default_generators[dev.index or 0]
-        seed0, threads = int(gen0.initial_seed()), m._rng_threads(dev, m.args.n_codebooks * m.n_audio_tokens[0])
-        P = (_lib.vcb_prompt * len(new))()
-        for j, (slot, ji) in enumerate(new):
-            J = jobs[ji]
-            P[j] = _lib.vcb_prompt(slot=slot, n_copies=1, mode=0, x_len=int(J["x_ids"].shape[0]),
-                                   text_ids_dev=J["x_ids"].data_ptr(), y_len=int(J["y_tok"].shape[0]),
-                                   y_tokens_dev=J["y_tok"].data_ptr(), mask_rows_dev=None, n_more_spans=0)
-            P[j].rng_seed = (int(J["seed"]) if J["seed"] is not None else seed0 + ji) & 0xFFFFFFFFFFFFFFFF
-            P[j].rng_offset = 0
-            P[j].rng_threads = threads
-        _lib.check(lib.vcb_prefill(eng, P, len(new), stream))
+        seed0 = int(torch.cuda.default_generators[m.mask_embedding.device.index or 0].initial_seed())
+        _prefill(eng, [(jobs[t][0], slot, 1, seed0 + t if jobs[t][1] is None else jobs[t][1], 0) for slot, t in new],
+                 stream)
         c_new = (C.c_int32 * len(new))(*[s for s, _ in new])
         _lib.check(lib.vcb_sample(eng, c_new, len(new), None, C.byref(self.sp), stream))
         self.stats["prefills"] += 1
 
-    def _result(self, eng, slot, n_steps, job, stream):
+    def _result(self, eng, slot, st, job, stream):
         """(res, gen) of a finished slot, as inference_tts returns them"""
-        m, a = self.model, self.model.args
-        rows = m._read_rows(eng, slot, n_steps, stream)
-        gen = torch.from_numpy(VoiceCraft._undelay(rows, a.n_codebooks)).to(m.mask_embedding.device)
-        res = torch.cat([job["yk"], gen], dim=1).unsqueeze(0)
-        if a.special_first:
-            res, gen = res - int(a.n_special), gen - int(a.n_special)
-        return res, gen.unsqueeze(0)
+        return job[0].result(self.model._read_rows(eng, slot, st.n_steps, stream), st)
 
     @torch.no_grad()
     def run(self):
@@ -1161,11 +1082,8 @@ class ContinuousBatcher:
         dev, lib = m.mask_embedding.device, _lib.load()
         jobs = [self._job(x, y, seed) for x, y, seed in self.queue]
         n_slots = min(self.B, max(1, len(jobs)))
-        eng = m._engine(need_slots=n_slots, need_seq=max([J["need_seq"] for J in jobs], default=0))
-        base = m._free_slots(n_slots, m._eng_opts["max_slots"])
-        self.slots, self._open = [base + i for i in range(n_slots)], True
-        m._sessions.add(self)
-        free, active, results, nxt = list(self.slots), {}, [None] * len(jobs), 0
+        eng, slots = m._take_slots(n_slots, max([p.need_seq for p, _ in jobs], default=0))
+        free, active, results, nxt = list(slots), {}, [None] * len(jobs), 0
         try:
             with torch.cuda.device(dev):
                 stream = torch.cuda.current_stream().cuda_stream
@@ -1189,21 +1107,16 @@ class ContinuousBatcher:
                         steps += 1
                     status = (_lib.vcb_status * len(order))()
                     _lib.check(lib.vcb_poll(eng, c_slots, len(order), status, stream))
+                    _check_capacity(status)
                     for slot, st in zip(order, status):
-                        if st.done == 2:
-                            raise _lib.VcbError("decode stopped: engine capacity (max_new_tokens / max_seq_len) exhausted; "
-                                                "raise it with configure_engine()")
                         if st.done:
                             ji = active.pop(slot)
-                            results[ji] = self._result(eng, slot, st.n_steps, jobs[ji], stream)
-                            lib.vcb_release(eng, slot, 1)
+                            results[ji] = self._result(eng, slot, st, jobs[ji], stream)
+                            m._release_slots(slots, [slot], keep_held=True)
                             free.append(slot)
                 self.stats["steps"] = steps
         finally:
-            for slot in list(active):
-                lib.vcb_release(eng, slot, 1)
-            self._open = False
-            m._sessions.discard(self)
+            m._release_slots(slots, list(active))
             self.queue = []
         return results
 
@@ -1217,7 +1130,7 @@ class ContinuousBatcher:
         return BatcherStream(self, tokenizer, chunk_frames)
 
 
-class BatcherStream:
+class BatcherStream(_AudioStream):
     """Iterator of ContinuousBatcher.stream().  Closing it early (break, close(), garbage collection) releases the
     batcher's engine slots and the codec streams."""
 
@@ -1229,75 +1142,29 @@ class BatcherStream:
             raise _lib.VcbError("a stream() of this ContinuousBatcher is already running")
         if chunk_frames < 1:
             raise ValueError("chunk_frames must be >= 1")
-        self._it = None
         jobs = [cb._job(x, y, seed) for x, y, seed in cb.queue]
-        eng = m._engine(need_slots=cb.B, need_seq=max([J["need_seq"] for J in jobs], default=0))
-        base = m._free_slots(cb.B, m._eng_opts["max_slots"])
-        # the generator holds this state, not the BatcherStream: dropping the BatcherStream closes it at once
-        st = self._st = SimpleNamespace(cb=cb, eng=eng, base=base, max_seq=m._eng_opts["max_seq_len"], jobs=jobs,
-                                        cancelled=set(), ended=set(), tok=tokenizer, chunk_frames=int(chunk_frames),
-                                        dev=m.mask_embedding.device, codec=None, push=None)
-        cb.slots, cb._open = [base + i for i in range(cb.B)], True
-        m._sessions.add(cb)
+        eng, slots = m._take_slots(cb.B, max([p.need_seq for p, _ in jobs], default=0))
+        st = SimpleNamespace(cb=cb, eng=eng, slots=slots, max_seq=m._eng_opts["max_seq_len"], jobs=jobs,
+                             cancelled=set(), ended=set(), tok=tokenizer, chunk_frames=int(chunk_frames),
+                             dev=m.mask_embedding.device)
         cb.results, cb.errors, cb._live = [None] * len(jobs), {}, st
-        try:
-            st.codec = tokenizer.open_stream(max_streams=cb.B)
-            st.cstream = torch.cuda.Stream(device=st.dev)
-        except Exception:
-            self.close()
-            raise
-        self._it = self._run(st)
-
-    @property
-    def push_host_seconds(self):
-        """host time spent in the push steps so far, outside the device waits"""
-        return self._st.push.host_s if self._st.push is not None else 0.0
-
-    def __iter__(self):
-        return self
-
-    def __next__(self):
-        return next(self._it)
-
-    def close(self):
-        st = getattr(self, "_st", None)
-        if st is None:
-            return
-        if self._it is not None:
-            self._it.close()
-        BatcherStream._finish(st)
-
-    def __enter__(self):
-        return self
-
-    def __exit__(self, *exc):
-        self.close()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._start(st, cb.B)
 
     @staticmethod
     def _finish(st):
         cb = st.cb
         if cb._live is not st:
             return
-        lib = _lib.load()
-        for slot in cb.slots:                # releasing a slot that is not open does nothing
-            lib.vcb_release(st.eng, slot, 1)
-        if st.codec is not None:
-            st.codec.close()
-            st.codec = None
-        cb._open, cb._live, cb.queue = False, None, []
-        cb.model._sessions.discard(cb)
+        cb.model._release_slots(st.slots)    # every slot: releasing one that is not open does nothing
+        _AudioStream._close_codec(st)
+        cb._live, cb.queue = None, []
 
     @staticmethod
     @torch.no_grad()
     def _run(st):
         cb, m, lib = st.cb, st.cb.model, _lib.load()
-        free, active, nxt = list(cb.slots), {}, 0        # active: slot -> _Utterance
+        base = st.slots[0]
+        free, active, nxt = list(st.slots), {}, 0        # active: slot -> _Utterance
         try:
             with torch.cuda.device(st.dev):
                 stream = torch.cuda.current_stream().cuda_stream
@@ -1309,8 +1176,8 @@ class BatcherStream:
                     for slot, r in list(active.items()):
                         if r.closed or r.ticket in st.cancelled:
                             if r.closed and r.ticket not in cb.errors:
-                                cb.results[r.ticket] = cb._result(st.eng, slot, r.n_steps, st.jobs[r.ticket], stream)
-                            lib.vcb_release(st.eng, slot, 1)
+                                cb.results[r.ticket] = cb._result(st.eng, slot, r.status, st.jobs[r.ticket], stream)
+                            m._release_slots(st.slots, [slot], keep_held=True)
                             del active[slot]
                             free.append(slot)
                     # ---- free slots take the next queued tickets; each slot owns codec stream id slot - base
@@ -1321,9 +1188,9 @@ class BatcherStream:
                         nxt += 1
                     if new:
                         cb._admit(st.eng, new, st.jobs, stream)
-                        st.codec.reset([slot - st.base for slot, _ in new])
+                        st.codec.reset([slot - base for slot, _ in new])
                         for slot, t in new:
-                            active[slot] = _Utterance(slot, slot - st.base, f"ticket {t}", ticket=t)
+                            active[slot] = _Utterance(slot, slot - base, f"ticket {t}", ticket=t)
                     if not active:
                         break
                     live = [active[s] for s in sorted(active)]
@@ -1339,7 +1206,7 @@ class BatcherStream:
                     status, out, failed = push(live, advance)
                     wavs = dict(out)
                     for r, s in zip(live, status):
-                        r.n_steps = s.n_steps
+                        r.status = s
                         if r in failed:
                             cb.errors[r.ticket] = failed[r]
                         if r.closed:
