@@ -35,19 +35,24 @@ def _model(cfg, sd, kv="fp32"):
 @pytest.mark.parametrize("simt", [1, 0])
 @pytest.mark.parametrize("shape", [(256, 256, 4), (768, 256, 32), (2052, 1024, 32), (1024, 4096, 128), (6144, 2048, 7)])
 def test_gemm_tcgen05_vs_fp32(shape, simt):
-    """Bring-up check of the wgmma/TMA GEMM (and its CUDA-core cross-check twin) against torch fp32."""
+    """Bring-up check of the wgmma/TMA GEMM (and its CUDA-core cross-check twin) against torch fp32: the engine's split
+    count (0) and every split count the kernel accepts for the shape."""
     from voicecraft_b200 import _lib
     lib = _lib.load()
     N, K, B = shape
     g = torch.Generator(device="cpu").manual_seed(N + K + B)
     W = torch.randn(N, K, generator=g).to(torch.bfloat16).float().cuda()
     X = torch.randn(B, K, generator=g).cuda()
-    out = torch.zeros(B, N, device="cuda")
-    _lib.check(lib.vcb_debug_gemm(W.data_ptr(), X.data_ptr(), out.data_ptr(), N, K, B, 0, simt))
     ref = (X.double() @ W.double().t()).float()
-    err = (out - ref).abs().max().item()
     scale = ref.abs().max().item()
-    assert err <= 2e-4 * max(scale, 1.0), f"shape={shape} simt={simt} err={err} scale={scale}"
+    bpad = 16 if B <= 16 else 32 if B <= 32 else 64 if B <= 64 else 128
+    kb = K // 64
+    legal = [s for s in (1, 2, 4, 8) if bpad % s == 0 and bpad // s >= 2 and (s - 1) * ((kb + s - 1) // s) < kb]
+    for splits in [0] + ([] if simt else legal):
+        out = torch.zeros(B, N, device="cuda")
+        _lib.check(lib.vcb_debug_gemm(W.data_ptr(), X.data_ptr(), out.data_ptr(), N, K, B, splits, simt))
+        err = (out - ref).abs().max().item()
+        assert err <= 2e-4 * max(scale, 1.0), f"shape={shape} simt={simt} splits={splits} err={err} scale={scale}"
 
 
 def _run_case(name, case, kv):

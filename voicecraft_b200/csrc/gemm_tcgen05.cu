@@ -261,24 +261,7 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             pdl_wait();
             if (ep.ln_fold && lane < R) {
                 const int row = z * R + lane;
-                if (row < nvalid) {
-                    float s1 = 0.f, s2 = 0.f;
-                    for (int t0 = 0; t0 < ep.stats_tiles; t0 += 16) {
-                        float2 v[16];
-#pragma unroll
-                        for (int i = 0; i < 16; ++i)
-                            v[i] = (t0 + i < ep.stats_tiles)
-                                       ? *reinterpret_cast<const float2*>(ep.stats + (static_cast<size_t>(t0 + i) * STATS_ROWS + row) * 2)
-                                       : make_float2(0.f, 0.f);
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) {
-                            s1 += v[i].x;
-                            s2 += v[i].y;
-                        }
-                    }
-                    e_mean = s1 * ep.inv_d;
-                    e_rstd = 1.0f / sqrtf(fmaxf(s2 * ep.inv_d - e_mean * e_mean, 0.f) + ep.ln_eps);
-                }
+                if (row < nvalid) ln_row_stats(ep.stats, ep.stats_tiles, ep.ln_d, row, ep.inv_d, ep.ln_eps, e_mean, e_rstd);
             }
             // ... and, when this CTA owns a single group of 4 rows (the out-projection and FFN2 at B = 32: R = 4), the
             // residual rows it is going to update
@@ -374,22 +357,7 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 float mean = 0.f, rstd = 0.f;
                 if (row < nvalid) {
                     // 16 tiles = one batch of independent 8-byte loads (a single L2 round trip), summed in tile order
-                    float s1 = 0.f, s2 = 0.f;
-                    for (int t0 = 0; t0 < ep.stats_tiles; t0 += 16) {
-                        float2 v[16];
-#pragma unroll
-                        for (int i = 0; i < 16; ++i)
-                            v[i] = (t0 + i < ep.stats_tiles)
-                                       ? *reinterpret_cast<const float2*>(ep.stats + (static_cast<size_t>(t0 + i) * STATS_ROWS + row) * 2)
-                                       : make_float2(0.f, 0.f);
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) {
-                            s1 += v[i].x;
-                            s2 += v[i].y;
-                        }
-                    }
-                    mean = s1 * ep.inv_d;
-                    rstd = 1.0f / sqrtf(fmaxf(s2 * ep.inv_d - mean * mean, 0.f) + ep.ln_eps);
+                    ln_row_stats(ep.stats, ep.stats_tiles, ep.ln_d, row, ep.inv_d, ep.ln_eps, mean, rstd);
                 }
                 s_mean[rr] = mean;
                 s_rstd[rr] = rstd;
@@ -425,7 +393,10 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             }
             if (valid_m) apply_epilogue4(ep, row0, nrows, m, sum, bias, xnew, colx, e_x_valid ? e_x : nullptr);
             if (ep.emit) {
-                // next GEMM's operand gamma_next * x_new (hi/lo) and this tile's (sum x, sum x^2) per row
+                // next GEMM's operand gamma_next * x_new (hi/lo) and this tile's (sum x, M2 about the tile mean) per row:
+                // each warp sums its 32 features, and their powers shifted by one of them (lane 0's, within the row's
+                // spread of the others), which gives the warp's M2 without cancellation; the 4 warps combine below
+                const int nw = min(32, max(0, Nout - (m0 + q * 32)));      // valid features of this warp
                 float p1[4], p2[4];
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
@@ -436,8 +407,10 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         ep.next_act[static_cast<size_t>(row0 + u) * ep.next_ld + m] = hi;
                         ep.next_act[static_cast<size_t>(row0 + u + ep.next_bpad) * ep.next_ld + m] = lo;
                     }
+                    const float dv = ok ? xnew[u] - __shfl_sync(0xffffffffu, xnew[u], 0) : 0.f;
                     p1[u] = warp_sum(ok ? xnew[u] : 0.f);
-                    p2[u] = warp_sum(ok ? xnew[u] * xnew[u] : 0.f);
+                    const float q1 = warp_sum(dv), q2 = warp_sum(dv * dv);
+                    p2[u] = nw > 0 ? fmaxf(q2 - q1 * q1 / static_cast<float>(nw), 0.f) : 0.f;
                 }
                 if (lane == 0) {
 #pragma unroll
@@ -448,11 +421,18 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 }
                 if (half == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
                 else asm volatile("bar.sync 3, 128;" ::: "memory");
-                if (ml < 8) {
-                    const int u = ml >> 1, w = ml & 1;
-                    if (u < nrows)
-                        ep.stats_out[(static_cast<size_t>(mt) * STATS_ROWS + row0 + u) * 2 + w] =
-                            s_part[0][u][w] + s_part[1][u][w] + s_part[2][u][w] + s_part[3][u][w];
+                if (ml < 4 && ml < nrows) {
+                    const int u = ml;
+                    const float sum = s_part[0][u][0] + s_part[1][u][0] + s_part[2][u][0] + s_part[3][u][0];
+                    const float tmean = sum / static_cast<float>(min(GEMM_BM, Nout - m0));
+                    float m2 = 0.f;
+#pragma unroll
+                    for (int w = 0; w < 4; ++w) {
+                        const int nw = min(32, Nout - (m0 + w * 32));
+                        if (nw > 0) m2 += ln_tile_m2(static_cast<float>(nw), s_part[w][u][0], s_part[w][u][1], tmean);
+                    }
+                    *reinterpret_cast<float2*>(ep.stats_out + (static_cast<size_t>(mt) * STATS_ROWS + row0 + u) * 2) =
+                        make_float2(sum, m2);
                 }
                 if (half == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
                 else asm volatile("bar.sync 3, 128;" ::: "memory");
@@ -497,29 +477,41 @@ __global__ void gemm_w_xT_simt(const __nv_bfloat16* __restrict__ W, const __nv_b
         acc = warp_sum(acc);
         if (lane == 0) {
             if (ep.ln_fold) {
-                float s1 = 0.f, s2 = 0.f;
-                for (int t = 0; t < ep.stats_tiles; ++t) {
-                    s1 += ep.stats[(static_cast<size_t>(t) * STATS_ROWS + j) * 2];
-                    s2 += ep.stats[(static_cast<size_t>(t) * STATS_ROWS + j) * 2 + 1];
-                }
-                const float mean = s1 * ep.inv_d;
-                const float rstd = 1.0f / sqrtf(fmaxf(s2 * ep.inv_d - mean * mean, 0.f) + ep.ln_eps);
+                float mean, rstd;
+                ln_row_stats(ep.stats, ep.stats_tiles, ep.ln_d, j, ep.inv_d, ep.ln_eps, mean, rstd);
                 acc = rstd * (acc - mean * ep.cvec[warp]);
             }
             const float sum[4] = {acc, 0.f, 0.f, 0.f};
             float xnew[4];
             apply_epilogue4(ep, j, 1, warp, sum, ep.bias[warp], xnew);
-            if (ep.emit) {
+            if (ep.emit) {       // the row statistics of x_new follow in tile_stats_kernel, once every feature is written
                 __nv_bfloat16 hi, lo;
                 split_bf16(ep.next_gamma[warp] * xnew[0], hi, lo);
                 ep.next_act[static_cast<size_t>(j) * ep.next_ld + warp] = hi;
                 ep.next_act[static_cast<size_t>(j + ep.next_bpad) * ep.next_ld + warp] = lo;
-                // one "tile" per feature group of 128, accumulated with atomics (cross-check path only)
-                atomicAdd(&ep.stats_out[(static_cast<size_t>(warp / GEMM_BM) * STATS_ROWS + j) * 2], xnew[0]);
-                atomicAdd(&ep.stats_out[(static_cast<size_t>(warp / GEMM_BM) * STATS_ROWS + j) * 2 + 1], xnew[0] * xnew[0]);
             }
         }
     }
+}
+
+// Row statistics of the cross-check path's x_new (EPI_RESID + emit): per 128-feature tile and row, (sum x, M2 about the
+// tile mean) -- what the tensor-core epilogue leaves.  One 128-thread CTA per (tile, row).
+__global__ void __launch_bounds__(128) tile_stats_kernel(const float* __restrict__ x, int ld, int Nout, float* __restrict__ stats) {
+    __shared__ float red[4];
+    const int t = blockIdx.x, r = blockIdx.y, m = t * GEMM_BM + threadIdx.x;
+    const int n = min(GEMM_BM, Nout - t * GEMM_BM);
+    const float v = m < Nout ? x[static_cast<size_t>(r) * ld + m] : 0.f;
+    auto block_sum = [&](float s) {
+        s = warp_sum(s);
+        __syncthreads();
+        if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+        __syncthreads();
+        return red[0] + red[1] + red[2] + red[3];
+    };
+    const float s1 = block_sum(v);
+    const float dv = m < Nout ? v - s1 / static_cast<float>(n) : 0.f;
+    const float m2 = block_sum(dv * dv);
+    if (threadIdx.x == 0) *reinterpret_cast<float2*>(stats + (static_cast<size_t>(t) * STATS_ROWS + r) * 2) = make_float2(s1, m2);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -667,6 +659,11 @@ int gemm_launch(const GemmCall& g, cudaStream_t st) {
         dim3 grid((g.Nout * 32 + 255) / 256, 1, 1);
         gemm_w_xT_simt<<<grid, 256, 0, st>>>(g.W, g.X, g.ep, g.Nout, g.Kdim, g.ldx, g.bpad, g.b_col_off, g.nvalid);
         VCB_CUDA_OK(cudaGetLastError());
+        if (g.ep.emit && g.nvalid > 0) {
+            tile_stats_kernel<<<dim3((g.Nout + GEMM_BM - 1) / GEMM_BM, g.nvalid), GEMM_BM, 0, st>>>(g.ep.x, g.ep.ld_out, g.Nout,
+                                                                                                  g.ep.stats_out);
+            VCB_CUDA_OK(cudaGetLastError());
+        }
         return 0;
     }
     const int total_kb = g.Kdim / GEMM_BK;

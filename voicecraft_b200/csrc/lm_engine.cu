@@ -12,6 +12,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <utility>
 
 namespace vcb {
 
@@ -79,7 +80,7 @@ struct vcb_engine {
     int opt_fold = 1;
     float *att_ws = nullptr;          // split-context attention partials [rows*H][att_maxch][hd+2]
     int *att_cnt = nullptr;           // per (row, head) arrival counters
-    int att_maxch = 1, att_chunk_pages = 16;
+    int att_maxch = 1, att_chunk_pages = ATT_CHUNK_PAGES;
     std::vector<float*> h_bias2;      // host copy of the K second-stage bias pointers
     std::vector<int> h_seq_len;       // host mirror of SlotState::seq_len (upper bound for the attention grid)
     __nv_bfloat16 *act_d = nullptr, *act_d2 = nullptr, *act_f = nullptr, *act_h = nullptr;
@@ -236,8 +237,8 @@ int upload_ints(vcb_engine* e, const int* src, size_t n, int* dst, cudaStream_t 
 // Launch with the programmatic-dependent-launch attribute (when enabled): the kernel may be scheduled while its
 // predecessor is still running; every such kernel orders its data accesses with griddepcontrol.wait (pdl_wait()).
 template <typename... KArgs, typename... Args>
-cudaError_t launch_k(vcb_engine* e, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
-                     Args&&... args) {
+cudaError_t launch_k_pdl(int pdl, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                         Args&&... args) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = grid;
     cfg.blockDim = block;
@@ -247,8 +248,27 @@ cudaError_t launch_k(vcb_engine* e, void (*kern)(KArgs...), dim3 grid, dim3 bloc
     at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     at[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = at;
-    cfg.numAttrs = e->opt_pdl ? 1 : 0;
+    cfg.numAttrs = pdl ? 1 : 0;
     return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+}
+
+template <typename... KArgs, typename... Args>
+cudaError_t launch_k(vcb_engine* e, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                     Args&&... args) {
+    return launch_k_pdl(e->opt_pdl, kern, grid, block, smem, st, std::forward<Args>(args)...);
+}
+
+// Split count of a decode GEMM from the tile / k-block rule's choice `s`: >= 64 rows take half of it (the per-CTA epilogue /
+// DSMEM exchange grows with the rows, so a smaller cluster pays off -- compare with scripts/bench_gemm.py, which times the
+// decode GEMMs at a given split count), `maxctas` > 0 caps tiles * splits, and the split count divides bpad.
+int decode_splits(int s, int Nout, int bpad, int maxctas) {
+    if (bpad >= 64 && s > 1) s /= 2;
+    if (maxctas > 0) {          // experiment knob: keep every GEMM to one CTA per SM (PDL ping-pong)
+        const int tiles = (Nout + 127) / 128;
+        while (s > 1 && tiles * s > maxctas) s /= 2;
+    }
+    while (s > 1 && bpad % s) s /= 2;
+    return s;
 }
 
 int run_gemm(vcb_engine* e, const Matrix& W, const CUtensorMap* tmB, const __nv_bfloat16* X, int ldx, int bpad,
@@ -268,17 +288,10 @@ int run_gemm(vcb_engine* e, const Matrix& W, const CUtensorMap* tmB, const __nv_
     g.Kdim = kdim;
     g.ldx = ldx;
     g.bpad = bpad;
-    g.splits = gemm_pick_splits(W.rows, kdim, e->num_sms);
+    int splits = gemm_pick_splits(W.rows, kdim, e->num_sms);
     for (const auto& o : e->opt_splits)          // experiment knob VCB_SPLITS="<N>x<K>:<S>,..."
-        if (o[0] == W.rows && o[1] == kdim) g.splits = o[2];
-    // >= 64 rows: the per-CTA epilogue / DSMEM exchange grows with the rows, so a smaller cluster pays off (compare with
-    // scripts/bench_gemm.py, which times the decode GEMMs at a given split count)
-    if (bpad >= 64 && g.splits > 1) g.splits /= 2;
-    if (e->opt_gemm_maxctas > 0) {          // experiment knob: keep every GEMM to one CTA per SM (PDL ping-pong)
-        const int tiles = (W.rows + 127) / 128;
-        while (g.splits > 1 && tiles * g.splits > e->opt_gemm_maxctas) g.splits /= 2;
-    }
-    while (g.splits > 1 && bpad % g.splits) g.splits /= 2;
+        if (o[0] == W.rows && o[1] == kdim) splits = o[2];
+    g.splits = decode_splits(splits, W.rows, bpad, e->opt_gemm_maxctas);
     g.stages = e->opt_gemm_stages;
     g.b_col_off = b_col_off;
     g.nvalid = nvalid;
@@ -289,44 +302,88 @@ int run_gemm(vcb_engine* e, const Matrix& W, const CUtensorMap* tmB, const __nv_
     return gemm_launch(g, st);
 }
 
+// One launch of attn_rows_kernel over `rows` rows of H heads whose contexts are at most max_ctx tokens.  The engine and
+// vcb_debug_attention both go through here, so the chunk count, grid and balance decisions under test are the engine's.
+struct AttnLaunch {
+    const float* q = nullptr;             // [rows][H][hd]
+    const void *kpool = nullptr, *vpool = nullptr;
+    const int *page_table = nullptr, *row_slot = nullptr, *row_pos = nullptr;
+    const int* row_pages = nullptr;       // [rows][max_pages] or null: pages through page_table + row_slot
+    int max_pages = 0, rows = 0, H = 0, hd = 0, kv_fp32 = 0, max_ctx = 0;
+    __nv_bfloat16* act = nullptr;         // hi rows [rows][ld_act], lo rows bpad rows further
+    int ld_act = 0, bpad = 0;
+    float* ws = nullptr;                  // [rows * H][maxch][hd + 2]
+    int* cnt = nullptr;                   // [rows * H], zero between launches (the merging CTA resets its counter)
+    int maxch = 1, chunk_pages = 16, num_sms = 132, balance = 1, pdl = 0;
+};
+
 template <typename KVT, int HD>
-int launch_attn_hd(vcb_engine* e, const Layer& Ly, int rows, int bpad, int max_ctx, cudaStream_t st) {
-    const ModelDims& m = e->m;
-    const float scale = 1.0f / sqrtf(static_cast<float>(m.hd));
+int launch_attn_hd(const AttnLaunch& a, cudaStream_t st) {
+    const float scale = 1.0f / sqrtf(static_cast<float>(HD));
     using L = AttSmem<KVT, HD>;
     static bool set = false;
     if (!set) {
         VCB_CUDA_OK(cudaFuncSetAttribute(attn_rows_kernel<KVT, HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
         set = true;
     }
-    const int npages = (max_ctx + KV_PAGE - 1) / KV_PAGE;
-    const int nch = std::min(e->att_maxch, std::max(1, (npages + e->att_chunk_pages - 1) / e->att_chunk_pages));
-    const int n_rh = rows * m.H;
+    const int npages = (a.max_ctx + KV_PAGE - 1) / KV_PAGE;
+    const int nch = std::min(a.maxch, std::max(1, (npages + a.chunk_pages - 1) / a.chunk_pages));
+    const int n_rh = a.rows * a.H;
     const int per_sm = std::max(1, std::min(4, (227 * 1024) / (L::TOTAL + 1024)));
-    int grid = std::min(n_rh * nch, e->num_sms * per_sm);
-    if (e->opt_att_balance) {
+    int grid = std::min(n_rh * nch, a.num_sms * per_sm);
+    if (a.balance) {
         // equal item counts per CTA: with a few more items than CTAs, most CTAs would idle through the second pass while
         // the kernel finishes at the pace of the 2-item CTAs; fewer CTAs with the same item count each stay busy to the end
         const int items = n_rh * nch, passes = (items + grid - 1) / grid;
         grid = (items + passes - 1) / passes;
     }
-    ProfScope ps(e, PC_ATTN, st);
-    VCB_CUDA_OK(launch_k(e, attn_rows_kernel<KVT, HD>, dim3(grid), dim3(ATT_THREADS + 32), L::TOTAL, st,
-                         static_cast<const float*>(e->cur_q ? e->cur_q : e->qbuf),
-                         static_cast<const KVT*>(Ly.kpool), static_cast<const KVT*>(Ly.vpool), e->page_table,
-                         e->max_pages_per_slot, e->cur_slot, e->cur_pos, m.H, e->cur_act_d ? e->cur_act_d : e->act_d, m.d, bpad,
-                         scale, e->cur_att_ws ? e->cur_att_ws : e->att_ws, e->cur_att_cnt ? e->cur_att_cnt : e->att_cnt,
-                         e->att_maxch, e->att_chunk_pages, n_rh, nch, e->cur_pages));
-    LAUNCH_COUNT(e);
+    VCB_CUDA_OK(launch_k_pdl(a.pdl, attn_rows_kernel<KVT, HD>, dim3(grid), dim3(ATT_THREADS + 32), L::TOTAL, st, a.q,
+                             static_cast<const KVT*>(a.kpool), static_cast<const KVT*>(a.vpool), a.page_table, a.max_pages,
+                             a.row_slot, a.row_pos, a.H, a.act, a.ld_act, a.bpad, scale, a.ws, a.cnt, a.maxch, a.chunk_pages,
+                             n_rh, nch, a.row_pages));
     return 0;
 }
 
+int launch_attn_rows(const AttnLaunch& a, cudaStream_t st) {
+    if (a.hd != 64 && a.hd != 128) {
+        set_error("attention: head dim %d (64 or 128 supported)", a.hd);
+        return -1;
+    }
+    if (a.kv_fp32)
+        return a.hd == 128 ? launch_attn_hd<float, 128>(a, st) : launch_attn_hd<float, 64>(a, st);
+    return a.hd == 128 ? launch_attn_hd<__nv_bfloat16, 128>(a, st) : launch_attn_hd<__nv_bfloat16, 64>(a, st);
+}
+
 int launch_attn(vcb_engine* e, const Layer& Ly, int rows, int bpad, int max_ctx, cudaStream_t st) {
-    if (e->kv_fp32)
-        return e->m.hd == 128 ? launch_attn_hd<float, 128>(e, Ly, rows, bpad, max_ctx, st)
-                              : launch_attn_hd<float, 64>(e, Ly, rows, bpad, max_ctx, st);
-    return e->m.hd == 128 ? launch_attn_hd<__nv_bfloat16, 128>(e, Ly, rows, bpad, max_ctx, st)
-                          : launch_attn_hd<__nv_bfloat16, 64>(e, Ly, rows, bpad, max_ctx, st);
+    const ModelDims& m = e->m;
+    AttnLaunch a;
+    a.q = e->cur_q ? e->cur_q : e->qbuf;
+    a.kpool = Ly.kpool;
+    a.vpool = Ly.vpool;
+    a.page_table = e->page_table;
+    a.row_slot = e->cur_slot;
+    a.row_pos = e->cur_pos;
+    a.row_pages = e->cur_pages;
+    a.max_pages = e->max_pages_per_slot;
+    a.rows = rows;
+    a.H = m.H;
+    a.hd = m.hd;
+    a.kv_fp32 = e->kv_fp32;
+    a.max_ctx = max_ctx;
+    a.act = e->cur_act_d ? e->cur_act_d : e->act_d;
+    a.ld_act = m.d;
+    a.bpad = bpad;
+    a.ws = e->cur_att_ws ? e->cur_att_ws : e->att_ws;
+    a.cnt = e->cur_att_cnt ? e->cur_att_cnt : e->att_cnt;
+    a.maxch = e->att_maxch;
+    a.chunk_pages = e->att_chunk_pages;
+    a.num_sms = e->num_sms;
+    a.balance = e->opt_att_balance;
+    a.pdl = e->opt_pdl;
+    ProfScope ps(e, PC_ATTN, st);
+    if (launch_attn_rows(a, st)) return -1;
+    LAUNCH_COUNT(e);
+    return 0;
 }
 
 int launch_ln(vcb_engine* e, const float* x_in, const int* src_index, int bpad, const float* g, const float* b, int rows,
@@ -360,6 +417,7 @@ int forward_rows(vcb_engine* e, int rows, int max_ctx, bool fold, cudaStream_t s
         ep.stats = e->ln_stats;
         ep.stats_tiles = tiles;
         ep.inv_d = 1.0f / static_cast<float>(m.d);
+        ep.ln_d = m.d;
         ep.ln_eps = 1e-5f;
     };
     auto set_emit = [&](GemmEpilogue& ep, const float* gamma_next, __nv_bfloat16* dst) {
@@ -534,7 +592,7 @@ int mega_build(vcb_engine* e, int bpad) {
     std::vector<MegaPhase> ph;
     auto fold = [&](GemmEpilogue& ep, const float* cvec, const float* bprime, int tiles) {
         ep.ln_fold = 1; ep.cvec = cvec; ep.bias = bprime; ep.stats = e->ln_stats; ep.stats_tiles = tiles;
-        ep.inv_d = 1.0f / static_cast<float>(m.d); ep.ln_eps = 1e-5f;
+        ep.inv_d = 1.0f / static_cast<float>(m.d); ep.ln_d = m.d; ep.ln_eps = 1e-5f;
     };
     auto emit = [&](GemmEpilogue& ep, const float* gamma_next, __nv_bfloat16* dst) {
         ep.emit = 1; ep.next_gamma = gamma_next; ep.next_act = dst; ep.next_ld = m.d; ep.next_bpad = bpad; ep.stats_out = e->ln_stats;
@@ -767,6 +825,7 @@ int sample_rows(vcb_engine* e, int n, const float* h_src, const int* h_index, co
         ea.stats = e->ln_stats;
         ea.stats_tiles = (m.d + 127) / 128;
         ea.inv_d = 1.0f / static_cast<float>(m.d);
+        ea.ln_d = m.d;
     }
     ea.act = e->act_h;
     ea.ld_out = KH;
@@ -1549,25 +1608,63 @@ int vcb_debug_logits(vcb_engine* e, float* out_dev, int32_t n_rows) {
     return 0;
 }
 
+}  // extern "C"
+
+namespace {
+
+// device allocations of a debug hook: zero-filled, freed on every return path
+struct HookBufs {
+    std::vector<void*> p;
+    template <typename T>
+    int alloc(T** out, size_t n) {
+        *out = nullptr;
+        VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(out), std::max<size_t>(n, 1) * sizeof(T)));
+        p.push_back(*out);
+        VCB_CUDA_OK(cudaMemset(*out, 0, std::max<size_t>(n, 1) * sizeof(T)));
+        return 0;
+    }
+    ~HookBufs() {
+        cudaDeviceSynchronize();            // nothing enqueued by the hook may still use the buffers
+        for (void* q : p) cudaFree(q);
+    }
+};
+
+int hook_num_sms() {
+    int n = 132;
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, 0);
+    return n;
+}
+
+// hi + lo activation rows -> fp32 rows [rows][cols] (debug hooks).  With `pos`, a row whose pos < 0 keeps its `out` values
+// unless the kernel under test wrote its act row: the hook fills act with 0xffff, a bf16 NaN that split_bf16 never produces.
+__global__ void join_hilo_kernel(const __nv_bfloat16* __restrict__ act, int ld, int bpad, int cols, const int* __restrict__ pos,
+                                 float* __restrict__ out) {
+    const int r = blockIdx.y;
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= cols) return;
+    const __nv_bfloat16 hi = act[static_cast<size_t>(r) * ld + c], lo = act[static_cast<size_t>(r + bpad) * ld + c];
+    if (pos && pos[r] < 0 && __bfloat16_as_ushort(hi) == 0xffff && __bfloat16_as_ushort(lo) == 0xffff) return;
+    out[static_cast<size_t>(r) * cols + c] = __bfloat162float(hi) + __bfloat162float(lo);
+}
+
+}  // namespace
+
+extern "C" {
+
 // Bring-up hook: out[b][n] = sum_k W[n][k] * X[b][k] through the production GEMM (bf16 weights, hi/lo activations).
 int vcb_debug_gemm(const float* W_dev, const float* X_dev, float* out_dev, int32_t N, int32_t Kd, int32_t B,
                    int32_t splits, int32_t simt) {
     const int bpad = bpad_for(B);
-    if (B > 128 || Kd % 64) {
-        set_error("vcb_debug_gemm: B <= 128 and K %% 64 == 0 required");
+    if (B < 1 || B > 128 || Kd % 64) {
+        set_error("vcb_debug_gemm: 1 <= B <= 128 and K %% 64 == 0 required");
         return -1;
     }
+    HookBufs hb;
     __nv_bfloat16 *w = nullptr, *x = nullptr;
     float* zb = nullptr;
-    int num_sms = 132;
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, 0);
-    if (splits <= 0) splits = gemm_pick_splits(N, Kd, num_sms);
-    while (splits > 1 && bpad % splits) splits /= 2;
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&w), packed_weight_elems(N, Kd) * 2));
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&x), static_cast<size_t>(2 * bpad) * Kd * 2));
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&zb), static_cast<size_t>(N) * 4));
-    VCB_CUDA_OK(cudaMemset(x, 0, static_cast<size_t>(2 * bpad) * Kd * 2));
-    VCB_CUDA_OK(cudaMemset(zb, 0, static_cast<size_t>(N) * 4));
+    if (splits <= 0) splits = decode_splits(gemm_pick_splits(N, Kd, hook_num_sms()), N, bpad, 0);
+    if (hb.alloc(&w, packed_weight_elems(N, Kd)) || hb.alloc(&x, static_cast<size_t>(2 * bpad) * Kd) || hb.alloc(&zb, N))
+        return -1;
     CUtensorMap tmA, tmB;
     if (pack_weight(W_dev, w, N, Kd, &tmA)) return -1;
     split_rows_kernel<<<dim3((Kd + 255) / 256, B), 256>>>(X_dev, Kd, x, Kd, bpad);
@@ -1579,7 +1676,122 @@ int vcb_debug_gemm(const float* W_dev, const float* X_dev, float* out_dev, int32
     g.Nout = N; g.Kdim = Kd; g.ldx = Kd; g.bpad = bpad; g.splits = splits; g.nvalid = B; g.simt = simt;
     if (gemm_launch(g, 0)) return -1;
     VCB_CUDA_OK(cudaDeviceSynchronize());
-    cudaFree(w); cudaFree(x); cudaFree(zb);
+    return 0;
+}
+
+// Parity hook of the paged attention (attn_rows_kernel) with the engine's launch decisions; see include/vcb200.h.
+int vcb_debug_attention(const float* q_dev, const void* kpool_dev, const void* vpool_dev, int32_t kv_fp32,
+                        const int32_t* row_pages_dev, const int32_t* page_table_dev, const int32_t* row_slot_dev,
+                        const int32_t* pos_dev, int32_t rows, int32_t H, int32_t hd, int32_t max_pages, int32_t chunk_pages,
+                        int32_t balance, int32_t repeats, float* out_dev) {
+    if (rows < 1 || H < 1 || (hd != 64 && hd != 128) || max_pages < 1 || repeats < 1 || !q_dev || !kpool_dev || !vpool_dev ||
+        !pos_dev || !out_dev || (!row_pages_dev && (!page_table_dev || !row_slot_dev))) {
+        set_error("vcb_debug_attention: bad argument");
+        return -1;
+    }
+    std::vector<int> pos(rows);
+    VCB_CUDA_OK(cudaMemcpy(pos.data(), pos_dev, rows * sizeof(int), cudaMemcpyDeviceToHost));
+    int max_ctx = 1;
+    for (int p : pos) {
+        if (p >= max_pages * KV_PAGE) {
+            set_error("vcb_debug_attention: position %d beyond %d pages", p, max_pages);
+            return -1;
+        }
+        max_ctx = std::max(max_ctx, p + 1);
+    }
+    AttnLaunch a;
+    a.q = q_dev;
+    a.kpool = kpool_dev;
+    a.vpool = vpool_dev;
+    a.page_table = page_table_dev;
+    a.row_slot = row_slot_dev;
+    a.row_pos = pos_dev;
+    a.row_pages = row_pages_dev;
+    a.max_pages = max_pages;
+    a.rows = rows;
+    a.H = H;
+    a.hd = hd;
+    a.kv_fp32 = kv_fp32;
+    a.max_ctx = max_ctx;
+    a.ld_act = H * hd;
+    a.bpad = rows;
+    a.chunk_pages = chunk_pages > 0 ? chunk_pages : ATT_CHUNK_PAGES;
+    a.maxch = std::max(1, (max_pages + a.chunk_pages - 1) / a.chunk_pages);      // as the engine sizes it from max_seq_len
+    a.num_sms = hook_num_sms();
+    a.balance = balance;
+    HookBufs hb;
+    if (hb.alloc(&a.act, static_cast<size_t>(2 * rows) * a.ld_act) ||
+        hb.alloc(&a.ws, static_cast<size_t>(rows) * H * a.maxch * (hd + 2)) || hb.alloc(&a.cnt, static_cast<size_t>(rows) * H))
+        return -1;
+    VCB_CUDA_OK(cudaMemset(a.act, 0xff, static_cast<size_t>(2 * rows) * a.ld_act * sizeof(__nv_bfloat16)));
+    for (int i = 0; i < repeats; ++i)
+        if (launch_attn_rows(a, 0)) return -1;
+    join_hilo_kernel<<<dim3((a.ld_act + 255) / 256, rows), 256>>>(a.act, a.ld_act, rows, a.ld_act, pos_dev, out_dev);
+    VCB_CUDA_OK(cudaGetLastError());
+    VCB_CUDA_OK(cudaDeviceSynchronize());
+    return 0;
+}
+
+// Parity hook of the decode pair "out-projection -> LN2 -> FFN1" on the per-kernel GEMM path; see include/vcb200.h.
+int vcb_debug_fold_chain(const float* x_dev, const float* a_dev, const float* W1_dev, const float* b1_dev,
+                         const float* gamma_dev, const float* beta_dev, const float* W2_dev, const float* b2_dev, int32_t B,
+                         int32_t d, int32_t N2, int32_t relu, int32_t fold, int32_t splits1, int32_t splits2, float* xnew_dev,
+                         float* y_dev) {
+    if (B < 1 || B > 128 || d < 128 || d > 4096 || d % 128 || N2 < 1) {
+        set_error("vcb_debug_fold_chain: 1 <= B <= 128, d %% 128 == 0, 128 <= d <= 4096, N2 >= 1 required");
+        return -1;
+    }
+    const int bpad = bpad_for(B), dtiles = d / 128, num_sms = hook_num_sms();
+    HookBufs hb;
+    __nv_bfloat16 *w1 = nullptr, *w2 = nullptr, *act_a = nullptr, *act_2 = nullptr, *act_f = nullptr;
+    float *stats = nullptr, *cvec = nullptr, *bprime = nullptr;
+    if (hb.alloc(&w1, packed_weight_elems(d, d)) || hb.alloc(&w2, packed_weight_elems(N2, d)) ||
+        hb.alloc(&act_a, static_cast<size_t>(2 * bpad) * d) || hb.alloc(&act_2, static_cast<size_t>(2 * bpad) * d) ||
+        hb.alloc(&act_f, static_cast<size_t>(2 * bpad) * N2) || hb.alloc(&stats, static_cast<size_t>(dtiles) * STATS_ROWS * 2) ||
+        hb.alloc(&cvec, N2) || hb.alloc(&bprime, N2))
+        return -1;
+    CUtensorMap tm1, tm2, tmA, tm2B;
+    if (pack_weight(W1_dev, w1, d, d, &tm1) || pack_weight(W2_dev, w2, N2, d, &tm2)) return -1;
+    split_rows_kernel<<<dim3((d + 255) / 256, B), 256>>>(a_dev, d, act_a, d, bpad);
+    VCB_CUDA_OK(cudaGetLastError());
+    VCB_CUDA_OK(cudaMemcpy(xnew_dev, x_dev, static_cast<size_t>(B) * d * sizeof(float), cudaMemcpyDeviceToDevice));
+    if (make_tmap_bf16_2d(&tmA, act_a, 2 * bpad, d, d, 2 * bpad) || make_tmap_bf16_2d(&tm2B, act_2, 2 * bpad, d, d, 2 * bpad))
+        return -1;
+    auto pick = [&](int s, int Nout) { return s > 0 ? s : decode_splits(gemm_pick_splits(Nout, d, num_sms), Nout, bpad, 0); };
+    // out-projection + residual: x_new = x + a W1^T + b1 (fold: also gamma * x_new as hi/lo rows + per-tile row statistics)
+    GemmCall g1;
+    g1.tmA = &tm1; g1.tmB = &tmA; g1.W = w1; g1.X = act_a;
+    g1.ep.mode = EPI_RESID; g1.ep.bias = b1_dev; g1.ep.x = xnew_dev; g1.ep.ld_out = d;
+    if (fold) {
+        g1.ep.emit = 1; g1.ep.next_gamma = gamma_dev; g1.ep.next_act = act_2; g1.ep.next_ld = d; g1.ep.next_bpad = bpad;
+        g1.ep.stats_out = stats;
+    }
+    g1.Nout = d; g1.Kdim = d; g1.ldx = d; g1.bpad = bpad; g1.splits = pick(splits1, d); g1.nvalid = B;
+    if (gemm_launch(g1, 0)) return -1;
+    GemmCall g2;
+    g2.tmA = &tm2; g2.tmB = &tm2B; g2.W = w2; g2.X = act_2;
+    if (fold) {
+        if (ln_fold_vectors(w2, gamma_dev, beta_dev, b2_dev, cvec, bprime, N2, d)) return -1;
+        g2.ep.ln_fold = 1; g2.ep.cvec = cvec; g2.ep.bias = bprime; g2.ep.stats = stats; g2.ep.stats_tiles = dtiles;
+        g2.ep.inv_d = 1.0f / static_cast<float>(d); g2.ep.ln_d = d; g2.ep.ln_eps = 1e-5f;
+    } else {                                  // prefill arithmetic: two-pass LayerNorm rows, then a plain GEMM
+        if (d <= 2048) ln_rows_kernel<8><<<B, 256>>>(xnew_dev, nullptr, gamma_dev, beta_dev, act_2, d, bpad, d, 1e-5f);
+        else ln_rows_kernel<16><<<B, 256>>>(xnew_dev, nullptr, gamma_dev, beta_dev, act_2, d, bpad, d, 1e-5f);
+        VCB_CUDA_OK(cudaGetLastError());
+        g2.ep.bias = b2_dev;
+    }
+    if (relu) {
+        g2.ep.mode = EPI_ACT; g2.ep.act = act_f; g2.ep.ld_out = N2; g2.ep.act_kind = 1; g2.ep.bpad_out = bpad;
+    } else {
+        g2.ep.mode = EPI_LOGITS; g2.ep.out = y_dev; g2.ep.ld_out = N2; g2.ep.col_off = 0;
+    }
+    g2.Nout = N2; g2.Kdim = d; g2.ldx = d; g2.bpad = bpad; g2.splits = pick(splits2, N2); g2.nvalid = B;
+    if (gemm_launch(g2, 0)) return -1;
+    if (relu) {
+        join_hilo_kernel<<<dim3((N2 + 255) / 256, B), 256>>>(act_f, N2, bpad, N2, nullptr, y_dev);
+        VCB_CUDA_OK(cudaGetLastError());
+    }
+    VCB_CUDA_OK(cudaDeviceSynchronize());
     return 0;
 }
 

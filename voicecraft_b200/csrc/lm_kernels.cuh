@@ -10,6 +10,7 @@ static constexpr int KV_PAGE = 64;          // tokens per KV page
 static constexpr int ATT_CWARPS = 8;            // consumer warps per CTA
 static constexpr int ATT_THREADS = ATT_CWARPS * 32;
 static constexpr int ATT_STAGES = 3;
+static constexpr int ATT_CHUNK_PAGES = 16;      // default pages per attention work item (VCB_ATT_CHUNK_PAGES overrides)
 
 __device__ __forceinline__ float block_sum_256(float v, float* red /*[8]*/) {
     v = warp_sum(v);
@@ -459,11 +460,16 @@ step_prep_kernel(const int* __restrict__ slots, int n, SlotState* __restrict__ s
                 act_tiled[(t0 + r + bpad) * 64 + ((((kk >> 3) ^ ((r + bpad) & 7)) << 3) | (kk & 7))] = lo;
             }
             s1 += v;
-            s2 += v * v;
         }
     }
     if (gamma0) {
+        // one statistics tile of all d features: (sum x, M2 about the row mean), see ln_tile_m2
         s1 = block_sum_256(s1, red);
+        const float mean = s1 / static_cast<float>(d);
+        for (int c = threadIdx.x; c < d; c += blockDim.x) {
+            const float dv = x_slot[static_cast<size_t>(slot) * d + c] - mean;
+            s2 = fmaf(dv, dv, s2);
+        }
         s2 = block_sum_256(s2, red);
         if (threadIdx.x == 0) {
             stats[static_cast<size_t>(r) * 2] = s1;

@@ -39,7 +39,7 @@ static constexpr int MG_BSLOT = 8192;          // 64 rows (32 hi + 32 lo) x 64 k
 static constexpr int MG_HD = 128;
 static constexpr int MG_PAGE = 64;
 static constexpr int MG_CHUNK = 4;             // attention: pages per work item (a chunk of one (row, head))
-static constexpr int MG_MAXCH = 16;            // chunks per item the in-CTA fold can hold (contexts up to 4096 tokens)
+static constexpr int MG_MAXCH = 16;            // chunks per item the in-CTA fold can hold (4096 tokens; longer: workspace fold)
 static constexpr int MG_PSTR = 132;            // floats per page partial: acc[128], m, l, pad
 
 struct MegaSmem {
@@ -222,16 +222,24 @@ __device__ __forceinline__ void mg_epi_prefetch(const MegaArgs& A, const MegaPha
         R.rpos[j] = (live && ep.mode == EPI_QKV) ? ep.row_pos[row] : -1;
         R.rpage[j] = (live && ep.mode == EPI_QKV) ? ep.row_page[row] : 0;
         if (ep.ln_fold && live) {
-            float s1 = 0.f, s2 = 0.f;
-            for (int t = lane; t < ep.stats_tiles; t += 32) {
-                const float2 v = __ldcg(reinterpret_cast<const float2*>(ep.stats + (static_cast<size_t>(t) * STATS_ROWS + row) * 2));
-                s1 += v.x;
-                s2 += v.y;
+            // lane t holds tile t (of each group of 32): the row sum, then the tiles' M2 about the row mean (see ln_tile_m2)
+            float2 v[4];
+            float s1 = 0.f, m2 = 0.f;
+#pragma unroll
+            for (int b = 0; b < 4; ++b) {
+                const int t = 32 * b + lane;
+                v[b] = t < ep.stats_tiles ? __ldcg(reinterpret_cast<const float2*>(ep.stats + (static_cast<size_t>(t) * STATS_ROWS + row) * 2))
+                                          : make_float2(0.f, 0.f);
+                s1 += v[b].x;
             }
-            s1 = warp_sum(s1);
-            s2 = warp_sum(s2);
-            R.mean[j] = s1 * ep.inv_d;
-            R.rstd[j] = 1.0f / sqrtf(fmaxf(s2 * ep.inv_d - R.mean[j] * R.mean[j], 0.f) + ep.ln_eps);
+            const float mean = warp_sum(s1) * ep.inv_d;
+#pragma unroll
+            for (int b = 0; b < 4; ++b) {
+                const int t = 32 * b + lane;
+                if (t < ep.stats_tiles) m2 += ln_tile_m2(ln_tile_n(t, ep.stats_tiles, ep.ln_d), v[b].x, v[b].y, mean);
+            }
+            R.mean[j] = mean;
+            R.rstd[j] = 1.0f / sqrtf(warp_sum(m2) * ep.inv_d + ep.ln_eps);
         }
         if (ep.mode == EPI_RESID && live && m0 < Nout)
             R.xold[j] = __ldcg(reinterpret_cast<const float4*>(ep.x + static_cast<size_t>(row) * ep.ld_out + m0));
@@ -347,10 +355,11 @@ __device__ __forceinline__ void mg_epi_finish(const MegaArgs& A, const MegaPhase
             }
         }
         if (ep.emit) {
-            // next GEMM's operand gamma_next * x_new (hi/lo) and this tile's (sum x, sum x^2) of the row: a warp holds
-            // exactly the 128 features of the tile for this row
+            // next GEMM's operand gamma_next * x_new (hi/lo) and this tile's (sum x, M2 about the tile mean) of the row: a
+            // warp holds exactly the 128 features of the tile for this row
+            const bool mine = row_ok && m0 < Nout;
             float p1 = 0.f, p2 = 0.f;
-            if (row_ok && m0 < Nout) {
+            if (mine) {
                 float hi[4], lo[4];
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
@@ -358,13 +367,17 @@ __device__ __forceinline__ void mg_epi_finish(const MegaArgs& A, const MegaPhase
                     hi[i] = mg_bf16_round(v);
                     lo[i] = v - hi[i];
                     p1 += xn[i];
-                    p2 += xn[i] * xn[i];
                 }
                 __stcg(reinterpret_cast<uint2*>(ep.next_act + mg_act_off(m0, row, 2 * ep.next_bpad)), mg_pack_bf16x4(hi[0], hi[1], hi[2], hi[3]));
                 __stcg(reinterpret_cast<uint2*>(ep.next_act + mg_act_off(m0, row + ep.next_bpad, 2 * ep.next_bpad)),
                        mg_pack_bf16x4(lo[0], lo[1], lo[2], lo[3]));
             }
             p1 = warp_sum(p1);
+            const float tmean = p1 / static_cast<float>(max(1, min(128, Nout - tl * 128)));
+            if (mine) {
+#pragma unroll
+                for (int i = 0; i < 4; ++i) p2 = fmaf(xn[i] - tmean, xn[i] - tmean, p2);
+            }
             p2 = warp_sum(p2);
             if (lane == 0 && row_ok)
                 __stcg(reinterpret_cast<float2*>(ep.stats_out + (static_cast<size_t>(tl) * STATS_ROWS + row) * 2), make_float2(p1, p2));
@@ -878,7 +891,9 @@ __global__ void __launch_bounds__(MG_THREADS, 1) mega_step_kernel(const __grid_c
                     const int n_chunks = (npg + MG_CHUNK - 1) / MG_CHUNK, cidx = pg / MG_CHUNK;
                     const size_t ocol = static_cast<size_t>(h) * MG_HD;
                     const long long ui0 = static_cast<long long>(A.H) * s_cum[r] + static_cast<long long>(h) * npg;   // item's first unit
-                    const bool spans = ui0 < u0 || ui0 + static_cast<long long>(n_chunks - 1) * MG_CHUNK >= u1;        // chunks owned by other CTAs too
+                    // chunks owned by other CTAs too, or more chunks than cs_sm holds (contexts over MG_MAXCH * MG_CHUNK pages):
+                    // the chunk states go through the workspace, which has room for max_pages of them per (row, head)
+                    const bool spans = n_chunks > MG_MAXCH || ui0 < u0 || ui0 + static_cast<long long>(n_chunks - 1) * MG_CHUNK >= u1;
                     const bool item_ends_here = pe == npg || u + (pe - pg) >= u1;   // my last chunk of this item
                     float* wsi = A.att_ws + static_cast<size_t>(rh) * A.max_pages * MG_PSTR;
                     if (wtid < MG_HD) {

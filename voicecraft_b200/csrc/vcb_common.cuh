@@ -24,6 +24,22 @@ void set_error(const char* fmt, ...);
 const char* get_error();
 
 // ------------------------------------------------------------------------------------------------
+// LayerNorm row statistics of the folded LayerNorm: per tile of features the producer leaves (sum x, M2 = sum (x - tile
+// mean)^2); consumers combine the tiles in tile order as mean = sum / d, M2 = sum_t (M2_t + n_t (mean_t - mean)^2).
+// Centred partials keep the variance exact to fp32 rounding of the spread, where E[x^2] - mean^2 loses (mean/std)^2 of it;
+// the terms are independent (no dependent division chain ahead of a GEMM mainloop).
+// ------------------------------------------------------------------------------------------------
+// features in tile t of `tiles` tiles over d features (a single tile holds the whole row, else 128 per tile)
+__device__ __forceinline__ float ln_tile_n(int t, int tiles, int d) {
+    return tiles == 1 ? static_cast<float>(d) : static_cast<float>(min(128, d - 128 * t));
+}
+// one tile's contribution to the row's M2 given the row mean
+__device__ __forceinline__ float ln_tile_m2(float n, float sum, float m2, float mean) {
+    const float dm = (n == 128.f ? sum * 0.0078125f : sum / n) - mean;
+    return fmaf(n * dm, dm, m2);
+}
+
+// ------------------------------------------------------------------------------------------------
 // bf16 split:  x ~= hi + lo with hi = bf16(x), lo = bf16(x - hi).  Residual error <= 2^-17 |x|.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16& hi, __nv_bfloat16& lo) {

@@ -33,9 +33,9 @@ struct GemmEpilogue {
     int ld_out = 0, col_off = 0, act_kind = 0, bpad_out = 0;
     // LayerNorm folded into this GEMM (the B operand is gamma*x, not LN(x)):
     //   y = rstd[row] * (acc - mean[row] * cvec[m]) + bias[m]   with bias := b + W.beta, cvec := W.gamma   (DESIGN.md section 4.1)
-    int ln_fold = 0, stats_tiles = 0;
+    int ln_fold = 0, stats_tiles = 0, ln_d = 0;   // ln_d: features of a row (1 tile: all of them, else 128 per tile)
     const float* cvec = nullptr;
-    const float* stats = nullptr;         // [tile][STATS_ROWS][2] partial (sum x, sum x^2) written by the producer
+    const float* stats = nullptr;         // [tile][STATS_ROWS][2] (sum x, sum (x - tile mean)^2) written by the producer
     float inv_d = 0.f, ln_eps = 1e-5f;
     // EPI_RESID producer side: also emit gamma_next * x_new as hi/lo rows + this tile's row statistics
     int emit = 0, next_ld = 0, next_bpad = 0;
@@ -48,6 +48,36 @@ struct GemmEpilogue {
     float* vnew = nullptr;
 };
 static constexpr int STATS_ROWS = 128;
+
+// mean and rstd of `row` from the per-tile (sum, M2) partials a producer left (tile order, see ln_tile_m2); up to 16 tiles
+// (d <= 2048) are one batch of independent loads, read once
+__device__ __forceinline__ void ln_row_stats(const float* stats, int tiles, int d, int row, float inv_d, float eps, float& mean,
+                                             float& rstd) {
+    auto load = [&](int t) {
+        return t < tiles ? *reinterpret_cast<const float2*>(stats + (static_cast<size_t>(t) * STATS_ROWS + row) * 2)
+                         : make_float2(0.f, 0.f);
+    };
+    float2 v[16];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) v[i] = load(i);
+    float s1 = 0.f, m2 = 0.f;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) s1 += v[i].x;
+    for (int t0 = 16; t0 < tiles; t0 += 16)
+#pragma unroll
+        for (int i = 0; i < 16; ++i) s1 += load(t0 + i).x;
+    mean = s1 * inv_d;
+#pragma unroll
+    for (int i = 0; i < 16; ++i)
+        if (i < tiles) m2 += ln_tile_m2(ln_tile_n(i, tiles, d), v[i].x, v[i].y, mean);
+    for (int t0 = 16; t0 < tiles; t0 += 16)
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+            const float2 w = load(t0 + i);
+            if (t0 + i < tiles) m2 += ln_tile_m2(ln_tile_n(t0 + i, tiles, d), w.x, w.y, mean);
+        }
+    rstd = 1.0f / sqrtf(m2 * inv_d + eps);
+}
 
 // ---------------------------------------------------------------------------------------------------
 // Persistent decode-step kernel (mega_step.cu): one launch runs every layer of a decode step.
