@@ -34,7 +34,7 @@ def _model(cfg, sd, kv="fp32"):
 
 @pytest.mark.parametrize("simt", [1, 0])
 @pytest.mark.parametrize("shape", [(256, 256, 4), (768, 256, 32), (2052, 1024, 32), (1024, 4096, 128), (6144, 2048, 7)])
-def test_gemm_tcgen05_vs_fp32(shape, simt):
+def test_gemm_wgmma_vs_fp32(shape, simt):
     """Bring-up check of the wgmma/TMA GEMM (and its CUDA-core cross-check twin) against torch fp32: the engine's split
     count (0) and every split count the kernel accepts for the shape."""
     from voicecraft_b200 import _lib

@@ -2,20 +2,20 @@
 //
 //   out[r][n] = epilogue( sum_k (Xhi[r,k] + Xlo[r,k]) * W[n,k] + bias[n] )        r = token row, n = output feature
 //
-// gemm_tcgen05.cu keeps the WEIGHTS as the 128-row operand and at most 128 token rows as the MMA N dimension: right
+// gemm_wgmma.cu keeps the WEIGHTS as the 128-row operand and at most 128 token rows as the MMA N dimension: right
 // for decode (every weight byte is used once per step), wrong for a prompt of thousands of rows, where it streams the
 // whole matrix once per 128 rows and spends most of each launch in the per-row epilogue.  Here a CTA owns a
 // [128 rows] x [BN features] output tile:
 //   A operand = activations, bf16 [2][rcap][K]: plane 0 = hi parts, plane 1 = lo parts (x ~= hi + lo, split_bf16);
 //               both 128 x 64 tiles of a k-block are multiplied with the SAME weight tile into the SAME accumulator
 //               (D += Ahi.B^T ; D += Alo.B^T), so the second pass costs no extra weight traffic.
-//   B operand = the pre-tiled weights of gemm_tcgen05.cu, unchanged: BN/128 consecutive 16 KB blocks of one k-block,
+//   B operand = the pre-tiled weights of gemm_wgmma.cu, unchanged: BN/128 consecutive 16 KB blocks of one k-block,
 //               stacked in shared memory, are exactly a K-major SWIZZLE_128B operand of BN rows.
 //   D         = fp32 in registers (wgmma): each of two warpgroups multiplies 64 token rows x BN features, then stages
 //               its accumulators in the (by then idle) pipeline shared memory, row = token, column = feature.
 // No split-K, no cluster: with >= 512 rows there are enough tiles (e.g. QKV at d = 2048: 24 x rows/128 CTAs), and the
 // weights (<= 34 MB per matrix) stay L2-resident across the row tiles.
-// Warp roles as in gemm_tcgen05.cu: w0 TMA producer, w1..w3 idle, w4..w11 MMA + epilogue (two warpgroups; in the
+// Warp roles as in gemm_wgmma.cu: w0 TMA producer, w1..w3 idle, w4..w11 MMA + epilogue (two warpgroups; in the
 // epilogue each covers all 128 rows and takes half of the columns).
 // Epilogues: EPI_QKV (q -> fp32 rows, k/v -> paged KV cache), EPI_RESID (x += y + b), EPI_ACT (ReLU/GELU -> hi/lo
 // planes), EPI_LOGITS (plain fp32 rows; bring-up tests).  A thread owns one token row and 32 consecutive features

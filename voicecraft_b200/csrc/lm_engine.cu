@@ -89,8 +89,6 @@ struct vcb_engine {
     int *row_page = nullptr;          // KV page of every row's position (step_prep / prefill fill it)
     int *row_forced = nullptr;        // decode steps: SlotState::forced per row as of step_prep (sampler snapshot)
     int *row_pages = nullptr;         // decode steps: per-row copy of the slot's page list [rows][max_pages_per_slot]
-    const int *cur_pages = nullptr;   // = row_pages during decode steps, null during prefill
-    const int *cur_forced = nullptr;  // = row_forced during decode steps, null for vcb_sample
     std::vector<char> slot_rng;       // host mirror: the slot's group generates its own sampling noise
     std::vector<char> slot_edit;      // host mirror: the slot decodes an edit prompt
     std::vector<int> slot_copies;     // host mirror: n_copies of the slot's prompt (best-of-N group size)
@@ -99,7 +97,6 @@ struct vcb_engine {
     int64_t n_poll_frames = 0;
     int *all_rows = nullptr;          // prefill row tables: 5 arrays of all_rows_cap ints (seq, pos, slot, last, page)
     size_t all_rows_cap = 0;
-    const int *cur_slot = nullptr, *cur_pos = nullptr, *cur_last = nullptr, *cur_page = nullptr;   // tables used by forward_rows
     int *d_slots = nullptr;
     std::vector<int> last_slots;      // host mirror of d_slots (skip re-upload when unchanged)
     int *tok_log = nullptr;
@@ -122,10 +119,6 @@ struct vcb_engine {
     int* w_att_cnt = nullptr;
     __nv_bfloat16 *wact_d = nullptr, *wact_f = nullptr;
     CUtensorMap tm_wact_d, tm_wact_f;
-    // buffers the attention / LayerNorm launchers work on (narrow decode buffers unless a wide prefill pass is running)
-    float *cur_q = nullptr, *cur_att_ws = nullptr;
-    int* cur_att_cnt = nullptr;
-    __nv_bfloat16* cur_act_d = nullptr;
     // persistent decode-step kernel (mega_step.cu): phase tables per bpad (16 / 32), flags, split-K workspace
     int opt_mega = 0, mega_grid = 0, mega_nph = 0, mega_cnt_stride = 0;      // VCB_MEGA=1: decode steps through the persistent kernel
     MegaPhase* d_mega_ph[2] = {nullptr, nullptr};
@@ -354,27 +347,205 @@ int launch_attn_rows(const AttnLaunch& a, cudaStream_t st) {
     return a.hd == 128 ? launch_attn_hd<__nv_bfloat16, 128>(a, st) : launch_attn_hd<__nv_bfloat16, 64>(a, st);
 }
 
-int launch_attn(vcb_engine* e, const Layer& Ly, int rows, int bpad, int max_ctx, cudaStream_t st) {
+// A GEMM's B operand: hi rows, then lo rows `bpad` rows further, and the tensor map the GEMM loads them through
+struct Plane {
+    __nv_bfloat16* act = nullptr;
+    const CUtensorMap* tm = nullptr;
+};
+
+// One pass of `rows` rows through the layers or the logit heads: the rows' tables and the buffers the pass works on.
+// The launchers below read a pass's rows and buffers from here only.
+struct Pass {
+    int rows = 0;
+    int bpad = 0;                             // rows from a plane's hi rows to its lo rows (wide prefill: wide_rows)
+    int max_ctx = 1;                          // longest context of a row (attention grid)
+    bool fold = false;                        // LayerNorm folded into the GEMM epilogues
+    bool wide = false;                        // GEMMs through the rows-as-M kernel (gemm_rows.cu), else the cluster decode GEMM
+    const int *slot = nullptr, *pos = nullptr, *last = nullptr, *page = nullptr;
+    const int* pages = nullptr;               // [rows][max_pages_per_slot] page lists, or null: pages through page_table + slot
+    const int* forced = nullptr;              // decode steps: SlotState::forced per row as of step_prep (sampler snapshot)
+    float* x = nullptr;                       // residual rows
+    const int* x_index = nullptr;             // heads of vcb_sample: row r's hidden state is x[x_index[r]] (null: x[r])
+    float* q = nullptr;
+    Plane act_d, act_d2, act_f, act_h;        // LayerNorm / attention output, folded FFN1 input, FFN1 output, heads hidden
+    float* att_ws = nullptr;
+    int* att_cnt = nullptr;
+};
+
+// a pass over at most MAX_ROWS rows on the decode buffers (row tables left to the caller)
+Pass narrow_pass(vcb_engine* e, int rows, bool fold) {
+    Pass p;
+    p.rows = rows;
+    p.bpad = bpad_for(rows);
+    const int bi = bpad_idx(p.bpad);
+    p.fold = fold;
+    p.x = e->x_rows;
+    p.q = e->qbuf;
+    p.act_d = {e->act_d, &e->tm_act_d[bi]};
+    p.act_d2 = {e->act_d2, &e->tm_act_d2[bi]};
+    p.act_f = {e->act_f, &e->tm_act_f[bi]};
+    p.act_h = {e->act_h, &e->tm_act_h[bi]};
+    p.att_ws = e->att_ws;
+    p.att_cnt = e->att_cnt;
+    return p;
+}
+
+// a decode step of n rows: the row tables step_prep_kernel fills
+Pass step_pass(vcb_engine* e, int n, bool fold) {
+    Pass p = narrow_pass(e, n, fold);
+    p.slot = e->row_slot;
+    p.pos = e->row_pos;
+    p.last = e->row_last;
+    p.page = e->row_page;
+    p.pages = e->row_pages;
+    p.forced = e->row_forced;
+    return p;
+}
+
+// a wide prefill chunk of at most wide_rows rows on the wide planes (row tables left to the caller)
+Pass wide_pass(vcb_engine* e, int rows) {
+    Pass p;
+    p.rows = rows;
+    p.bpad = e->wide_rows;
+    p.wide = true;
+    p.x = e->wx;
+    p.q = e->wq;
+    p.act_d = {e->wact_d, &e->tm_wact_d};
+    p.act_f = {e->wact_f, &e->tm_wact_f};
+    p.att_ws = e->w_att_ws;
+    p.att_cnt = e->w_att_cnt;
+    return p;
+}
+
+// Consumer side of a folded LayerNorm: the B operand is gamma * x (hi/lo) and the producer left the row statistics of
+// `tiles` tiles in `stats`; bias := b + W.beta (`bprime`), cvec := W.gamma (DESIGN.md section 4.1)
+void fold_epilogue(GemmEpilogue& ep, const float* cvec, const float* bprime, const float* stats, int tiles, int d) {
+    ep.ln_fold = 1;
+    ep.cvec = cvec;
+    ep.bias = bprime;
+    ep.stats = stats;
+    ep.stats_tiles = tiles;
+    ep.inv_d = 1.0f / static_cast<float>(d);
+    ep.ln_d = d;
+    ep.ln_eps = 1e-5f;
+}
+
+// Producer side: a residual epilogue also emits gamma_next * x_new as hi/lo rows of `dst` (never the buffer the GEMM is
+// still reading as its B operand) and the row statistics of its tile to `stats`
+void emit_epilogue(GemmEpilogue& ep, const float* gamma_next, __nv_bfloat16* dst, int d, int bpad, float* stats) {
+    ep.emit = 1;
+    ep.next_gamma = gamma_next;
+    ep.next_act = dst;
+    ep.next_ld = d;
+    ep.next_bpad = bpad;
+    ep.stats_out = stats;
+}
+
+// The GEMM epilogues of layer l in pass p: QKV (+KV append), out-projection (+residual), FFN1 (+ReLU), FFN2 (+residual).
+// With p.fold the consumers fold LN1 / LN2 and the residual GEMMs emit the next LayerNorm's operand; layer 0 reads the
+// one statistics tile of step_prep_kernel.
+struct LayerEpilogues {
+    GemmEpilogue qkv, out, ff1, ff2;
+};
+
+LayerEpilogues layer_epilogues(const vcb_engine* e, int l, const Pass& p) {
+    const ModelDims& m = e->m;
+    const Layer& Ly = e->layers[l];
+    const int dtiles = (m.d + 127) / 128;
+    LayerEpilogues r;
+    GemmEpilogue& q = r.qkv;
+    q.mode = EPI_QKV;
+    q.bias = Ly.b_qkv;
+    q.qbuf = p.q;
+    q.kpool = Ly.kpool;
+    q.vpool = Ly.vpool;
+    q.page_table = e->page_table;
+    q.row_slot = p.slot;
+    q.row_pos = p.pos;
+    q.row_page = p.page;
+    q.kv_fp32 = e->kv_fp32;
+    q.max_pages = e->max_pages_per_slot;
+    q.page_size = KV_PAGE;
+    q.d = m.d;
+    q.H = m.H;
+    q.hd = m.hd;
+    r.out.mode = EPI_RESID;
+    r.out.bias = Ly.b_out;
+    r.out.x = p.x;
+    r.out.ld_out = m.d;
+    r.ff1.mode = EPI_ACT;
+    r.ff1.bias = Ly.b_ff1;
+    r.ff1.act = p.act_f.act;
+    r.ff1.ld_out = m.F;
+    r.ff1.act_kind = 1;
+    r.ff1.bpad_out = p.bpad;
+    r.ff2.mode = EPI_RESID;
+    r.ff2.bias = Ly.b_ff2;
+    r.ff2.x = p.x;
+    r.ff2.ld_out = m.d;
+    if (p.fold) {
+        fold_epilogue(r.qkv, Ly.c_qkv, Ly.bp_qkv, e->ln_stats, l == 0 ? 1 : dtiles, m.d);
+        emit_epilogue(r.out, Ly.ln2_g, p.act_d2.act, m.d, p.bpad, e->ln_stats);
+        fold_epilogue(r.ff1, Ly.c_ff1, Ly.bp_ff1, e->ln_stats, dtiles, m.d);
+        emit_epilogue(r.ff2, l + 1 < m.L ? e->layers[l + 1].ln1_g : e->lnf_g, p.act_d.act, m.d, p.bpad, e->ln_stats);
+    }
+    return r;
+}
+
+// first stage of the logit heads (stacked predict_layer.{k}.0, GELU); with p.fold the final LayerNorm is folded in
+GemmEpilogue heads_epilogue(const vcb_engine* e, const Pass& p) {
+    const ModelDims& m = e->m;
+    GemmEpilogue ep;
+    ep.mode = EPI_ACT;
+    ep.bias = e->b_h1;
+    ep.act = p.act_h.act;
+    ep.ld_out = m.K * m.Hh;
+    ep.act_kind = 2;
+    ep.bpad_out = p.bpad;
+    if (p.fold) fold_epilogue(ep, e->c_h1, e->bp_h1, e->ln_stats, (m.d + 127) / 128, m.d);
+    return ep;
+}
+
+// W times the plane `in` for the pass's rows.  `next`: the weights the following GEMM streams, prefetched into L2 by the
+// decode GEMM (VCB_PREFETCH)
+int pass_gemm(vcb_engine* e, const Pass& p, const Matrix& W, const Plane& in, const GemmEpilogue& ep, cudaStream_t st,
+              const Matrix* next) {
+    if (!p.wide) return run_gemm(e, W, in.tm, in.act, W.cols, p.bpad, p.rows, 0, W.cols, ep, st, next);
+    RowsGemmCall g;
+    g.tmX = in.tm;
+    g.tmW = &W.tm;
+    g.ep = ep;
+    g.rows = p.rows;
+    g.rcap = p.bpad;
+    g.Nout = W.rows;
+    g.Kdim = W.cols;
+    g.pdl = e->opt_pdl;
+    LAUNCH_COUNT(e);
+    ProfScope ps(e, PC_GEMM, st);
+    return gemm_rows_launch(g, st);
+}
+
+int launch_attn(vcb_engine* e, const Pass& p, const Layer& Ly, cudaStream_t st) {
     const ModelDims& m = e->m;
     AttnLaunch a;
-    a.q = e->cur_q ? e->cur_q : e->qbuf;
+    a.q = p.q;
     a.kpool = Ly.kpool;
     a.vpool = Ly.vpool;
     a.page_table = e->page_table;
-    a.row_slot = e->cur_slot;
-    a.row_pos = e->cur_pos;
-    a.row_pages = e->cur_pages;
+    a.row_slot = p.slot;
+    a.row_pos = p.pos;
+    a.row_pages = p.pages;
     a.max_pages = e->max_pages_per_slot;
-    a.rows = rows;
+    a.rows = p.rows;
     a.H = m.H;
     a.hd = m.hd;
     a.kv_fp32 = e->kv_fp32;
-    a.max_ctx = max_ctx;
-    a.act = e->cur_act_d ? e->cur_act_d : e->act_d;
+    a.max_ctx = p.max_ctx;
+    a.act = p.act_d.act;
     a.ld_act = m.d;
-    a.bpad = bpad;
-    a.ws = e->cur_att_ws ? e->cur_att_ws : e->att_ws;
-    a.cnt = e->cur_att_cnt ? e->cur_att_cnt : e->att_cnt;
+    a.bpad = p.bpad;
+    a.ws = p.att_ws;
+    a.cnt = p.att_cnt;
     a.maxch = e->att_maxch;
     a.chunk_pages = e->att_chunk_pages;
     a.num_sms = e->num_sms;
@@ -386,105 +557,41 @@ int launch_attn(vcb_engine* e, const Layer& Ly, int rows, int bpad, int max_ctx,
     return 0;
 }
 
-int launch_ln(vcb_engine* e, const float* x_in, const int* src_index, int bpad, const float* g, const float* b, int rows,
-              cudaStream_t st) {
+// LayerNorm of the pass's residual rows (p.x, through p.x_index) into the hi/lo rows of p.act_d
+int launch_ln(vcb_engine* e, const Pass& p, const float* g, const float* b, cudaStream_t st) {
     const int d = e->m.d;
     ProfScope ps(e, PC_LN, st);
-    __nv_bfloat16* dst = e->cur_act_d ? e->cur_act_d : e->act_d;
-    if (d <= 2048)
-        VCB_CUDA_OK(launch_k(e, ln_rows_kernel<8>, dim3(rows), dim3(256), 0, st, x_in, src_index, g, b, dst, d, bpad, d, 1e-5f));
-    else
-        VCB_CUDA_OK(launch_k(e, ln_rows_kernel<16>, dim3(rows), dim3(256), 0, st, x_in, src_index, g, b, dst, d, bpad, d, 1e-5f));
+    auto* kern = d <= 2048 ? ln_rows_kernel<8> : ln_rows_kernel<16>;
+    VCB_CUDA_OK(launch_k(e, kern, dim3(p.rows), dim3(256), 0, st, p.x, p.x_index, g, b, p.act_d.act, d, p.bpad, d, 1e-5f));
     LAUNCH_COUNT(e);
     return 0;
 }
 
-// All transformer layers over `rows` rows whose embeddings are in x_rows and (slot,pos) in cur_slot/cur_pos.
-// (transformer.py:321-329, 473-488)
-//   fold = false (prefill): 7 launches per layer: LN1, QKV GEMM (+KV append), attention, out GEMM (+residual), LN2,
-//                           FFN1 GEMM (+ReLU), FFN2 GEMM (+residual)
-//   fold = true  (decode):  5 launches per layer: LayerNorm is folded into the consuming GEMM's epilogue; the producing
-//                           GEMM (or step_prep for layer 0) emits gamma*x as hi/lo rows plus per-tile row statistics.
-int forward_rows(vcb_engine* e, int rows, int max_ctx, bool fold, cudaStream_t st) {
+// All transformer layers over the pass's rows, whose embeddings are in p.x.  (transformer.py:321-329, 473-488)
+//   fold = false (prefill, VCB_FOLD=0, VCB_GEMM_IMPL=simt): 7 launches per layer: LN1, QKV GEMM (+KV append), attention,
+//                out GEMM (+residual), LN2, FFN1 GEMM (+ReLU), FFN2 GEMM (+residual)
+//   fold = true  (decode): 5 launches per layer: LayerNorm is folded into the consuming GEMM's epilogue; the producing
+//                GEMM (or step_prep for layer 0) emits gamma*x as hi/lo rows plus per-tile row statistics.
+int forward_layers(vcb_engine* e, const Pass& p, cudaStream_t st) {
     const ModelDims& m = e->m;
-    const int bpad = bpad_for(rows);
-    const int bi = bpad_idx(bpad);
-    const int dtiles = (m.d + 127) / 128;
-    auto set_fold = [&](GemmEpilogue& ep, const float* cvec, const float* bprime, int tiles) {
-        ep.ln_fold = 1;
-        ep.cvec = cvec;
-        ep.bias = bprime;
-        ep.stats = e->ln_stats;
-        ep.stats_tiles = tiles;
-        ep.inv_d = 1.0f / static_cast<float>(m.d);
-        ep.ln_d = m.d;
-        ep.ln_eps = 1e-5f;
-    };
-    auto set_emit = [&](GemmEpilogue& ep, const float* gamma_next, __nv_bfloat16* dst) {
-        ep.emit = 1;
-        ep.next_gamma = gamma_next;
-        ep.next_act = dst;               // never the buffer this GEMM is still reading as its B operand
-        ep.next_ld = m.d;
-        ep.next_bpad = bpad;
-        ep.stats_out = e->ln_stats;
-    };
     for (int l = 0; l < m.L; ++l) {
         const Layer& Ly = e->layers[l];
-        if (!fold && launch_ln(e, e->x_rows, nullptr, bpad, Ly.ln1_g, Ly.ln1_b, rows, st)) return -1;
-        GemmEpilogue ep;
-        ep.mode = EPI_QKV;
-        ep.bias = Ly.b_qkv;
-        ep.qbuf = e->qbuf;
-        ep.kpool = Ly.kpool;
-        ep.vpool = Ly.vpool;
-        ep.page_table = e->page_table;
-        ep.row_slot = e->cur_slot;
-        ep.row_pos = e->cur_pos;
-        ep.row_page = e->cur_page;
-        ep.kv_fp32 = e->kv_fp32;
-        ep.max_pages = e->max_pages_per_slot;
-        ep.page_size = KV_PAGE;
-        ep.d = m.d;
-        ep.H = m.H;
-        ep.hd = m.hd;
-        if (fold) set_fold(ep, Ly.c_qkv, Ly.bp_qkv, l == 0 ? 1 : dtiles);
-        if (run_gemm(e, Ly.qkv, &e->tm_act_d[bi], e->act_d, m.d, bpad, rows, 0, m.d, ep, st, &Ly.out)) return -1;
-        if (launch_attn(e, Ly, rows, bpad, max_ctx, st)) return -1;
-        GemmEpilogue er;
-        er.mode = EPI_RESID;
-        er.bias = Ly.b_out;
-        er.x = e->x_rows;
-        er.ld_out = m.d;
-        if (fold) set_emit(er, Ly.ln2_g, e->act_d2);
-        if (run_gemm(e, Ly.out, &e->tm_act_d[bi], e->act_d, m.d, bpad, rows, 0, m.d, er, st, &Ly.ff1)) return -1;
-        if (!fold && launch_ln(e, e->x_rows, nullptr, bpad, Ly.ln2_g, Ly.ln2_b, rows, st)) return -1;
-        GemmEpilogue ea;
-        ea.mode = EPI_ACT;
-        ea.bias = Ly.b_ff1;
-        ea.act = e->act_f;
-        ea.ld_out = m.F;
-        ea.act_kind = 1;
-        ea.bpad_out = bpad;
-        if (fold) set_fold(ea, Ly.c_ff1, Ly.bp_ff1, dtiles);
-        if (run_gemm(e, Ly.ff1, fold ? &e->tm_act_d2[bi] : &e->tm_act_d[bi], fold ? e->act_d2 : e->act_d, m.d, bpad, rows, 0,
-                     m.d, ea, st, &Ly.ff2))
+        const LayerEpilogues ep = layer_epilogues(e, l, p);
+        if (!p.fold && launch_ln(e, p, Ly.ln1_g, Ly.ln1_b, st)) return -1;
+        if (pass_gemm(e, p, Ly.qkv, p.act_d, ep.qkv, st, &Ly.out) || launch_attn(e, p, Ly, st) ||
+            pass_gemm(e, p, Ly.out, p.act_d, ep.out, st, &Ly.ff1))
             return -1;
-        GemmEpilogue e2;
-        e2.mode = EPI_RESID;
-        e2.bias = Ly.b_ff2;
-        e2.x = e->x_rows;
-        e2.ld_out = m.d;
-        if (fold) set_emit(e2, l + 1 < m.L ? e->layers[l + 1].ln1_g : e->lnf_g, e->act_d);
-        if (run_gemm(e, Ly.ff2, &e->tm_act_f[bi], e->act_f, m.F, bpad, rows, 0, m.F, e2, st,
-                     l + 1 < m.L ? &e->layers[l + 1].qkv : &e->h1))
+        if (!p.fold && launch_ln(e, p, Ly.ln2_g, Ly.ln2_b, st)) return -1;
+        if (pass_gemm(e, p, Ly.ff1, p.fold ? p.act_d2 : p.act_d, ep.ff1, st, &Ly.ff2) ||
+            pass_gemm(e, p, Ly.ff2, p.act_f, ep.ff2, st, l + 1 < m.L ? &e->layers[l + 1].qkv : &e->h1))
             return -1;
     }
     return 0;
 }
 
-// Prefill over many rows at once (gemm_rows.cu): same layer sequence as forward_rows(fold = false), but every GEMM sees
-// all `rows` (<= wide_rows) rows as its M dimension; activations live in the wide planes [2][wide_rows][.] (the lo
-// plane starts wide_rows rows after the hi plane, which is what the LN / attention kernels take as their `bpad`).
+// Prefill over many rows at once (gemm_rows.cu): a wide pass through forward_layers (fold = false) whose GEMMs see all
+// its rows (<= wide_rows) as their M dimension; activations live in the wide planes [2][wide_rows][.] (the lo plane
+// starts wide_rows rows after the hi plane, which is what the LN / attention kernels take as their `bpad`).
 bool wide_usable(const vcb_engine* e) {
     const ModelDims& m = e->m;
     return e->opt_prefill_wide && !e->opt_simt && m.hd % 32 == 0 && gemm_rows_supported(3 * m.d, m.d, m.hd) &&
@@ -517,86 +624,21 @@ int wide_alloc(vcb_engine* e) {
     return 0;
 }
 
-int forward_rows_wide(vcb_engine* e, int rows, int max_ctx, cudaStream_t st) {
-    const ModelDims& m = e->m;
-    const int W = e->wide_rows;
-    auto gemm = [&](const Matrix& Wt, const CUtensorMap* tmX, int kdim, const GemmEpilogue& ep) {
-        RowsGemmCall g;
-        g.tmX = tmX;
-        g.tmW = &Wt.tm;
-        g.ep = ep;
-        g.rows = rows;
-        g.rcap = W;
-        g.Nout = Wt.rows;
-        g.Kdim = kdim;
-        g.pdl = e->opt_pdl;
-        LAUNCH_COUNT(e);
-        ProfScope ps(e, PC_GEMM, st);
-        return gemm_rows_launch(g, st);
-    };
-    for (int l = 0; l < m.L; ++l) {
-        const Layer& Ly = e->layers[l];
-        if (launch_ln(e, e->wx, nullptr, W, Ly.ln1_g, Ly.ln1_b, rows, st)) return -1;
-        GemmEpilogue ep;
-        ep.mode = EPI_QKV;
-        ep.bias = Ly.b_qkv;
-        ep.qbuf = e->wq;
-        ep.kpool = Ly.kpool;
-        ep.vpool = Ly.vpool;
-        ep.page_table = e->page_table;
-        ep.row_slot = e->cur_slot;
-        ep.row_pos = e->cur_pos;
-        ep.row_page = e->cur_page;
-        ep.kv_fp32 = e->kv_fp32;
-        ep.max_pages = e->max_pages_per_slot;
-        ep.page_size = KV_PAGE;
-        ep.d = m.d;
-        ep.H = m.H;
-        ep.hd = m.hd;
-        if (gemm(Ly.qkv, &e->tm_wact_d, m.d, ep)) return -1;
-        if (launch_attn(e, Ly, rows, W, max_ctx, st)) return -1;
-        GemmEpilogue er;
-        er.mode = EPI_RESID;
-        er.bias = Ly.b_out;
-        er.x = e->wx;
-        er.ld_out = m.d;
-        if (gemm(Ly.out, &e->tm_wact_d, m.d, er)) return -1;
-        if (launch_ln(e, e->wx, nullptr, W, Ly.ln2_g, Ly.ln2_b, rows, st)) return -1;
-        GemmEpilogue ea;
-        ea.mode = EPI_ACT;
-        ea.bias = Ly.b_ff1;
-        ea.act = e->wact_f;
-        ea.ld_out = m.F;
-        ea.act_kind = 1;
-        ea.bpad_out = W;
-        if (gemm(Ly.ff1, &e->tm_wact_d, m.d, ea)) return -1;
-        GemmEpilogue e2;
-        e2.mode = EPI_RESID;
-        e2.bias = Ly.b_ff2;
-        e2.x = e->wx;
-        e2.ld_out = m.d;
-        if (gemm(Ly.ff2, &e->tm_wact_f, m.F, e2)) return -1;
-    }
-    return 0;
-}
-
-int launch_sampler(vcb_engine* e, int n, const float* noise, const vcb_sampling* sp, cudaStream_t st);
+int launch_sampler(vcb_engine* e, const Pass& p, const float* noise, const vcb_sampling* sp, cudaStream_t st);
 
 // ---- decode step through the persistent kernel (mega_step.cu) ---------------------------------------------------------------
 // Phase table of one decode step for a given bpad: L x (QKV, attention, out-proj, FFN1, FFN2), heads stage 1, heads stage 2
-// (one grouped phase over the K codebooks).  Epilogues are exactly forward_rows(fold = true) / sample_rows(fold = true).
+// (one grouped phase over the K codebooks).  The epilogues are those of a folded decode step of bpad rows
+// (layer_epilogues, heads_epilogue), writing the kernel's activation images instead of the planes.
 int mega_build(vcb_engine* e, int bpad) {
     const ModelDims& m = e->m;
     const int which = bpad == 32;
-    const int dtiles = m.d / 128;
+    Pass p = step_pass(e, bpad, true);
+    p.act_d = {e->mact_d, nullptr};
+    p.act_d2 = {e->mact_d2, nullptr};
+    p.act_f = {e->mact_f, nullptr};
+    p.act_h = {e->mact_h, nullptr};
     std::vector<MegaPhase> ph;
-    auto fold = [&](GemmEpilogue& ep, const float* cvec, const float* bprime, int tiles) {
-        ep.ln_fold = 1; ep.cvec = cvec; ep.bias = bprime; ep.stats = e->ln_stats; ep.stats_tiles = tiles;
-        ep.inv_d = 1.0f / static_cast<float>(m.d); ep.ln_d = m.d; ep.ln_eps = 1e-5f;
-    };
-    auto emit = [&](GemmEpilogue& ep, const float* gamma_next, __nv_bfloat16* dst) {
-        ep.emit = 1; ep.next_gamma = gamma_next; ep.next_act = dst; ep.next_ld = m.d; ep.next_bpad = bpad; ep.stats_out = e->ln_stats;
-    };
     auto gemm = [&](const CUtensorMap* tm, const void* const* wp, int Nout, int Kdim, int b_map) {
         MegaPhase P;
         P.type = MEGA_GEMM;
@@ -613,12 +655,11 @@ int mega_build(vcb_engine* e, int bpad) {
         const Layer& Ly = e->layers[l];
         const CUtensorMap* tm = e->d_wmaps + 4 * l;
         const void* const* wp = e->d_wptrs + 4 * l;
+        const LayerEpilogues ep = layer_epilogues(e, l, p);
         MegaPhase q = gemm(tm + 0, wp + 0, 3 * m.d, m.d, 0);
-        q.ep.mode = EPI_QKV; q.ep.qbuf = e->qbuf; q.ep.kpool = Ly.kpool; q.ep.vpool = Ly.vpool; q.ep.page_table = e->page_table;
-        q.ep.row_slot = e->row_slot; q.ep.row_pos = e->row_pos; q.ep.row_page = e->row_page; q.ep.kv_fp32 = e->kv_fp32;
-        q.ep.max_pages = e->max_pages_per_slot; q.ep.page_size = KV_PAGE; q.ep.d = m.d; q.ep.H = m.H; q.ep.hd = m.hd;
-        q.ep.knew = e->knew; q.ep.vnew = e->vnew;
-        fold(q.ep, Ly.c_qkv, Ly.bp_qkv, l == 0 ? 1 : dtiles);
+        q.ep = ep.qkv;
+        q.ep.knew = e->knew;
+        q.ep.vnew = e->vnew;
         ph.push_back(q);
         MegaPhase a;
         a.type = MEGA_ATTN;
@@ -627,22 +668,17 @@ int mega_build(vcb_engine* e, int bpad) {
         a.done_target = e->mega_grid;
         ph.push_back(a);
         MegaPhase o = gemm(tm + 1, wp + 1, m.d, m.d, 0);
-        o.ep.mode = EPI_RESID; o.ep.bias = Ly.b_out; o.ep.x = e->x_rows; o.ep.ld_out = m.d;
-        emit(o.ep, Ly.ln2_g, e->mact_d2);
+        o.ep = ep.out;
         ph.push_back(o);
         MegaPhase f1 = gemm(tm + 2, wp + 2, m.F, m.d, 1);
-        f1.ep.mode = EPI_ACT; f1.ep.act = e->mact_f; f1.ep.ld_out = m.F; f1.ep.act_kind = 1; f1.ep.bpad_out = bpad;
-        fold(f1.ep, Ly.c_ff1, Ly.bp_ff1, dtiles);
+        f1.ep = ep.ff1;
         ph.push_back(f1);
         MegaPhase f2 = gemm(tm + 3, wp + 3, m.d, m.F, 2);
-        f2.ep.mode = EPI_RESID; f2.ep.bias = Ly.b_ff2; f2.ep.x = e->x_rows; f2.ep.ld_out = m.d;
-        emit(f2.ep, l + 1 < m.L ? e->layers[l + 1].ln1_g : e->lnf_g, e->mact_d);
+        f2.ep = ep.ff2;
         ph.push_back(f2);
     }
-    const int KH = m.K * m.Hh;
-    MegaPhase h1 = gemm(e->d_wmaps + 4 * m.L, e->d_wptrs + 4 * m.L, KH, m.d, 0);
-    h1.ep.mode = EPI_ACT; h1.ep.act = e->mact_h; h1.ep.ld_out = KH; h1.ep.act_kind = 2; h1.ep.bpad_out = bpad;
-    fold(h1.ep, e->c_h1, e->bp_h1, dtiles);
+    MegaPhase h1 = gemm(e->d_wmaps + 4 * m.L, e->d_wptrs + 4 * m.L, m.K * m.Hh, m.d, 0);
+    h1.ep = heads_epilogue(e, p);
     ph.push_back(h1);
     MegaPhase h2 = gemm(e->d_h2_maps, e->d_wptrs + 4 * m.L + 1, m.V, m.Hh, 3);
     h2.groups = m.K;
@@ -741,13 +777,12 @@ int mega_setup(vcb_engine* e) {
 
 int mega_step(vcb_engine* e, int n, cudaStream_t st) {
     const ModelDims& m = e->m;
-    const int bpad = bpad_for(n), bi = bpad_idx(bpad);
+    const int bpad = bpad_for(n);
     MegaArgs a;
     a.bbase[0] = e->mact_d;
     a.bbase[1] = e->mact_d2;
     a.bbase[2] = e->mact_f;
     a.bbase[3] = e->mact_h;
-    (void)bi;
     a.ph = e->d_mega_ph[bpad == 32];
     a.nph = e->mega_nph;
     a.nvalid = n;
@@ -806,38 +841,21 @@ int noise_required(vcb_engine* e, const int32_t* slots, int n, const float* nois
     return 0;
 }
 
-// final LayerNorm + logit heads + fused sampler for the n listed slots (d_slots already uploaded).
-// h_src/h_index: hidden states [.., d] and optional row indirection (prefill: h_slot[slot]; decode: x_rows[row]).
-int sample_rows(vcb_engine* e, int n, const float* h_src, const int* h_index, const float* noise, const vcb_sampling* sp,
-                bool fold, cudaStream_t st) {
+// final LayerNorm + logit heads + fused sampler for the pass's rows, those of the slots in d_slots (already uploaded).
+// Their hidden states are p.x, through p.x_index (vcb_sample: h_slot[slot]; decode: x_rows[row]).
+int sample_rows(vcb_engine* e, const Pass& p, const float* noise, const vcb_sampling* sp, cudaStream_t st) {
     const ModelDims& m = e->m;
-    const int bpad = bpad_for(n), bi = bpad_idx(bpad);
+    const int n = p.rows, bpad = p.bpad;
     // fold: the last FFN2 epilogue already left lnf_gamma * x (hi/lo) and the row statistics for the heads GEMM
-    if (!fold && launch_ln(e, h_src, h_index, bpad, e->lnf_g, e->lnf_b, n, st)) return -1;
+    if (!p.fold && launch_ln(e, p, e->lnf_g, e->lnf_b, st)) return -1;
     const int KH = m.K * m.Hh;
-    GemmEpilogue ea;
-    ea.mode = EPI_ACT;
-    ea.bias = e->b_h1;
-    if (fold) {
-        ea.ln_fold = 1;
-        ea.cvec = e->c_h1;
-        ea.bias = e->bp_h1;
-        ea.stats = e->ln_stats;
-        ea.stats_tiles = (m.d + 127) / 128;
-        ea.inv_d = 1.0f / static_cast<float>(m.d);
-        ea.ln_d = m.d;
-    }
-    ea.act = e->act_h;
-    ea.ld_out = KH;
-    ea.act_kind = 2;
-    ea.bpad_out = bpad;
-    if (run_gemm(e, e->h1, &e->tm_act_d[bi], e->act_d, m.d, bpad, n, 0, m.d, ea, st, &e->h2[0])) return -1;
+    if (pass_gemm(e, p, e->h1, p.act_d, heads_epilogue(e, p), st, &e->h2[0])) return -1;
     const int ldl = m.K * m.Vpad;
     if (!e->opt_simt) {
         // the K second-stage heads as ONE grouped launch (blockIdx.y = codebook)
         GemmCall g;
         g.tmA = &e->h2[0].tm;
-        g.tmB = &e->tm_act_h[bi];
+        g.tmB = p.act_h.tm;
         g.ep.mode = EPI_LOGITS;
         g.ep.bias = e->h_bias2[0];
         g.ep.out = e->logits;
@@ -866,20 +884,22 @@ int sample_rows(vcb_engine* e, int n, const float* h_src, const int* h_index, co
             el.out = e->logits;
             el.ld_out = ldl;
             el.col_off = k * m.Vpad;
-            if (run_gemm(e, e->h2[k], &e->tm_act_h[bi], e->act_h, KH, bpad, n, k * m.Hh, m.Hh, el, st,
+            if (run_gemm(e, e->h2[k], p.act_h.tm, p.act_h.act, KH, bpad, n, k * m.Hh, m.Hh, el, st,
                          k + 1 < m.K ? &e->h2[k + 1] : &e->layers[0].qkv))
                 return -1;
         }
     }
-    return launch_sampler(e, n, noise, sp, st);
+    return launch_sampler(e, p, noise, sp, st);
 }
 
-int launch_sampler(vcb_engine* e, int n, const float* noise, const vcb_sampling* sp, cudaStream_t st) {
+// fused sampler over the pass's rows, one CTA per (row, codebook)
+int launch_sampler(vcb_engine* e, const Pass& p, const float* noise, const vcb_sampling* sp, cudaStream_t st) {
     const ModelDims& m = e->m;
+    const int n = p.rows;
     const int ldl = m.K * m.Vpad;
     SamplerArgs a;
     a.slots = e->d_slots;
-    a.row_forced = e->cur_forced;
+    a.row_forced = p.forced;
     a.n = n;
     a.st = e->st;
     a.gr = e->gr;
@@ -1345,60 +1365,29 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
     VCB_CUDA_OK(cudaMemcpy(t_slot, r_slot.data(), total_rows * sizeof(int), cudaMemcpyHostToDevice));
     VCB_CUDA_OK(cudaMemcpy(t_last, r_last.data(), total_rows * sizeof(int), cudaMemcpyHostToDevice));
     VCB_CUDA_OK(cudaMemcpy(t_page, r_page.data(), total_rows * sizeof(int), cudaMemcpyHostToDevice));
-    // ---- wide prefill: thousands of rows per pass through the rows-as-M GEMM ------------------------------
-    if (wide_usable(e) && total_rows >= static_cast<size_t>(e->opt_prefill_wide)) {
+    // ---- wide prefill: thousands of rows per pass through the rows-as-M GEMM; else <= 128 rows per pass --------
+    const bool wide = wide_usable(e) && total_rows >= static_cast<size_t>(e->opt_prefill_wide);
+    if (wide) {
         if (!e->wide_rows) e->wide_rows = static_cast<int>(std::min<size_t>(4096, (e->all_rows_cap + 127) / 128 * 128));
         if (wide_alloc(e)) return -1;
-        const size_t W = static_cast<size_t>(e->wide_rows);
-        e->cur_q = e->wq;
-        e->cur_act_d = e->wact_d;
-        e->cur_att_ws = e->w_att_ws;
-        e->cur_att_cnt = e->w_att_cnt;
-        int rc = 0;
-        for (size_t off = 0; off < total_rows && !rc; off += W) {
-            const int rows = static_cast<int>(std::min<size_t>(W, total_rows - off));
-            e->cur_slot = t_slot + off;
-            e->cur_pos = t_pos + off;
-            e->cur_last = t_last + off;
-            e->cur_page = t_page + off;
-            e->cur_pages = nullptr;
-            embed_rows_kernel<<<rows, 256, 0, st>>>(e->d_seqs, t_seq + off, t_pos + off, e->wx, m.d, m.K, e->E_text,
-                                                    e->d_E_audio, e->mask_emb, e->pe, e->alpha_t, e->alpha_a);
-            LAUNCH_COUNT(e);
-            int max_ctx = 1;
-            for (int r = 0; r < rows; ++r) max_ctx = std::max(max_ctx, r_pos[off + r] + 1);
-            rc = forward_rows_wide(e, rows, max_ctx, st);
-            if (!rc) {
-                ProfScope ps(e, PC_LN, st);
-                gather_rows_kernel<<<rows, 256, 0, st>>>(e->wx, e->h_slot, e->cur_last, m.d);
-                LAUNCH_COUNT(e);
-            }
-        }
-        e->cur_q = nullptr;
-        e->cur_act_d = nullptr;
-        e->cur_att_ws = nullptr;
-        e->cur_att_cnt = nullptr;
-        if (rc) return -1;
-        VCB_CUDA_OK(cudaGetLastError());
-        return 0;
     }
-    for (size_t off = 0; off < total_rows; off += vcb_engine::MAX_ROWS) {
-        const int rows = static_cast<int>(std::min<size_t>(vcb_engine::MAX_ROWS, total_rows - off));
-        e->cur_slot = t_slot + off;
-        e->cur_pos = t_pos + off;
-        e->cur_last = t_last + off;
-        e->cur_page = t_page + off;
-        e->cur_pages = nullptr;
-        embed_rows_kernel<<<rows, 256, 0, st>>>(e->d_seqs, t_seq + off, t_pos + off, e->x_rows, m.d, m.K, e->E_text,
+    const size_t chunk = wide ? static_cast<size_t>(e->wide_rows) : static_cast<size_t>(vcb_engine::MAX_ROWS);
+    for (size_t off = 0; off < total_rows; off += chunk) {
+        const int rows = static_cast<int>(std::min(chunk, total_rows - off));
+        Pass p = wide ? wide_pass(e, rows) : narrow_pass(e, rows, false);
+        p.slot = t_slot + off;
+        p.pos = t_pos + off;
+        p.last = t_last + off;
+        p.page = t_page + off;
+        embed_rows_kernel<<<rows, 256, 0, st>>>(e->d_seqs, t_seq + off, t_pos + off, p.x, m.d, m.K, e->E_text,
                                                 e->d_E_audio, e->mask_emb, e->pe, e->alpha_t, e->alpha_a);
         VCB_CUDA_OK(cudaGetLastError());
         LAUNCH_COUNT(e);
-        int max_ctx = 1;
-        for (int r = 0; r < rows; ++r) max_ctx = std::max(max_ctx, r_pos[off + r] + 1);
-        if (forward_rows(e, rows, max_ctx, false, st)) return -1;
+        for (int r = 0; r < rows; ++r) p.max_ctx = std::max(p.max_ctx, r_pos[off + r] + 1);
+        if (forward_layers(e, p, st)) return -1;
         {
             ProfScope ps(e, PC_LN, st);
-            gather_rows_kernel<<<rows, 256, 0, st>>>(e->x_rows, e->h_slot, e->cur_last, m.d);
+            gather_rows_kernel<<<rows, 256, 0, st>>>(p.x, e->h_slot, p.last, m.d);
         }
         VCB_CUDA_OK(cudaGetLastError());
         LAUNCH_COUNT(e);
@@ -1416,8 +1405,10 @@ int vcb_sample(vcb_engine* e, const int32_t* slots, int32_t n, const float* exp_
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
     if (upload_slots(e, slots, n, st)) return -1;
     if (noise_required(e, slots, n, exp_noise_dev)) return -1;
-    e->cur_forced = nullptr;
-    return sample_rows(e, n, e->h_slot, e->d_slots, exp_noise_dev, sp, false, st);
+    Pass p = narrow_pass(e, n, false);
+    p.x = e->h_slot;
+    p.x_index = e->d_slots;
+    return sample_rows(e, p, exp_noise_dev, sp, st);
 }
 
 int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float* exp_noise_dev, const vcb_sampling* sp,
@@ -1430,32 +1421,26 @@ int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float*
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
     if (upload_slots(e, slots, n, st)) return -1;
     if (noise_required(e, slots, n, exp_noise_dev)) return -1;
-    e->cur_forced = e->row_forced;
     const bool fold = e->opt_fold && !e->opt_simt;
+    Pass p = step_pass(e, n, fold);
     {
         ProfScope ps(e, PC_MISC, st);
         VCB_CUDA_OK(launch_k(e, step_prep_kernel, dim3(n), dim3(256), 0, st, e->d_slots, n, e->st, e->gr, e->row_slot,
                              e->row_pos, e->row_last, e->x_slot, e->x_rows, e->m.d,
-                             fold ? e->layers[0].ln1_g : static_cast<const float*>(nullptr), e->act_d, bpad_for(n),
+                             fold ? e->layers[0].ln1_g : static_cast<const float*>(nullptr), e->act_d, p.bpad,
                              e->ln_stats, e->page_table, e->max_pages_per_slot, e->row_page, e->row_pages, e->row_forced,
                              e->mega_flags, e->mega_flags ? e->mega_nph : 0, reinterpret_cast<unsigned int*>(e->mega_tile_cnt),
                              e->mega_flags ? e->mega_nph * e->mega_cnt_stride : 0,
                              (fold && e->mega_grid > 0 && n <= 32) ? e->mact_d : static_cast<__nv_bfloat16*>(nullptr)));
     }
     LAUNCH_COUNT(e);
-    e->cur_slot = e->row_slot;
-    e->cur_pos = e->row_pos;
-    e->cur_last = e->row_last;
-    e->cur_page = e->row_page;
-    e->cur_pages = e->row_pages;
-    int max_ctx = 1;
-    for (int i = 0; i < n; ++i) max_ctx = std::max(max_ctx, ++e->h_seq_len[slots[i]]);
+    for (int i = 0; i < n; ++i) p.max_ctx = std::max(p.max_ctx, ++e->h_seq_len[slots[i]]);
     if (fold && e->mega_grid > 0 && n <= 32) {
         if (mega_step(e, n, st)) return -1;
-        return launch_sampler(e, n, exp_noise_dev, sp, st);
+        return launch_sampler(e, p, exp_noise_dev, sp, st);
     }
-    if (forward_rows(e, n, max_ctx, fold, st)) return -1;
-    return sample_rows(e, n, e->x_rows, nullptr, exp_noise_dev, sp, fold, st);
+    if (forward_layers(e, p, st)) return -1;
+    return sample_rows(e, p, exp_noise_dev, sp, st);
 }
 
 // a failed synchronisation: if the persistent kernel's watchdog fired, say where (the record is in mapped host memory)
@@ -1612,9 +1597,10 @@ int vcb_debug_logits(vcb_engine* e, float* out_dev, int32_t n_rows) {
 
 namespace {
 
-// device allocations of a debug hook: zero-filled, freed on every return path
+// device allocations and events of a debug hook: buffers zero-filled, both freed on every return path
 struct HookBufs {
     std::vector<void*> p;
+    std::vector<cudaEvent_t> ev;
     template <typename T>
     int alloc(T** out, size_t n) {
         *out = nullptr;
@@ -1623,9 +1609,15 @@ struct HookBufs {
         VCB_CUDA_OK(cudaMemset(*out, 0, std::max<size_t>(n, 1) * sizeof(T)));
         return 0;
     }
+    int event(cudaEvent_t* out) {
+        VCB_CUDA_OK(cudaEventCreate(out));
+        ev.push_back(*out);
+        return 0;
+    }
     ~HookBufs() {
         cudaDeviceSynchronize();            // nothing enqueued by the hook may still use the buffers
         for (void* q : p) cudaFree(q);
+        for (cudaEvent_t q : ev) cudaEventDestroy(q);
     }
 };
 
@@ -1762,18 +1754,14 @@ int vcb_debug_fold_chain(const float* x_dev, const float* a_dev, const float* W1
     GemmCall g1;
     g1.tmA = &tm1; g1.tmB = &tmA; g1.W = w1; g1.X = act_a;
     g1.ep.mode = EPI_RESID; g1.ep.bias = b1_dev; g1.ep.x = xnew_dev; g1.ep.ld_out = d;
-    if (fold) {
-        g1.ep.emit = 1; g1.ep.next_gamma = gamma_dev; g1.ep.next_act = act_2; g1.ep.next_ld = d; g1.ep.next_bpad = bpad;
-        g1.ep.stats_out = stats;
-    }
+    if (fold) emit_epilogue(g1.ep, gamma_dev, act_2, d, bpad, stats);
     g1.Nout = d; g1.Kdim = d; g1.ldx = d; g1.bpad = bpad; g1.splits = pick(splits1, d); g1.nvalid = B;
     if (gemm_launch(g1, 0)) return -1;
     GemmCall g2;
     g2.tmA = &tm2; g2.tmB = &tm2B; g2.W = w2; g2.X = act_2;
     if (fold) {
         if (ln_fold_vectors(w2, gamma_dev, beta_dev, b2_dev, cvec, bprime, N2, d)) return -1;
-        g2.ep.ln_fold = 1; g2.ep.cvec = cvec; g2.ep.bias = bprime; g2.ep.stats = stats; g2.ep.stats_tiles = dtiles;
-        g2.ep.inv_d = 1.0f / static_cast<float>(d); g2.ep.ln_d = d; g2.ep.ln_eps = 1e-5f;
+        fold_epilogue(g2.ep, cvec, bprime, stats, dtiles, d);
     } else {                                  // prefill arithmetic: two-pass LayerNorm rows, then a plain GEMM
         if (d <= 2048) ln_rows_kernel<8><<<B, 256>>>(xnew_dev, nullptr, gamma_dev, beta_dev, act_2, d, bpad, d, 1e-5f);
         else ln_rows_kernel<16><<<B, 256>>>(xnew_dev, nullptr, gamma_dev, beta_dev, act_2, d, bpad, d, 1e-5f);
@@ -1802,13 +1790,11 @@ int vcb_debug_gemm_rows(const float* W_dev, const float* X_dev, float* out_dev, 
         return -1;
     }
     const int rcap = (rows + 127) / 128 * 128;
+    HookBufs hb;
     __nv_bfloat16 *w = nullptr, *x = nullptr;
     float* zb = nullptr;
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&w), packed_weight_elems(N, Kd) * 2));
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&x), static_cast<size_t>(2 * rcap) * Kd * 2));
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&zb), static_cast<size_t>(N) * 4));
-    VCB_CUDA_OK(cudaMemset(x, 0, static_cast<size_t>(2 * rcap) * Kd * 2));
-    VCB_CUDA_OK(cudaMemset(zb, 0, static_cast<size_t>(N) * 4));
+    if (hb.alloc(&w, packed_weight_elems(N, Kd)) || hb.alloc(&x, static_cast<size_t>(2 * rcap) * Kd) || hb.alloc(&zb, N))
+        return -1;
     CUtensorMap tmW, tmX;
     if (pack_weight(W_dev, w, N, Kd, &tmW)) return -1;
     split_rows_kernel<<<dim3((Kd + 255) / 256, rows), 256>>>(X_dev, Kd, x, Kd, rcap);
@@ -1820,7 +1806,6 @@ int vcb_debug_gemm_rows(const float* W_dev, const float* X_dev, float* out_dev, 
     g.rows = rows; g.rcap = rcap; g.Nout = N; g.Kdim = Kd;
     if (gemm_rows_launch(g, 0)) return -1;
     VCB_CUDA_OK(cudaDeviceSynchronize());
-    cudaFree(w); cudaFree(x); cudaFree(zb);
     return 0;
 }
 
@@ -1829,20 +1814,18 @@ int vcb_debug_gemm_rows(const float* W_dev, const float* X_dev, float* out_dev, 
 int vcb_bench_gemm(int32_t N, int32_t Kd, int32_t B, int32_t splits, int32_t stages, int32_t pdl, int32_t iters,
                    int32_t ncopies, float* us_out) {
     const int bpad = bpad_for(B);
+    HookBufs hb;
     __nv_bfloat16 *w = nullptr, *x = nullptr;
     float *zb = nullptr, *out = nullptr;
-    int num_sms = 132;
-    cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, 0);
-    if (splits <= 0) splits = gemm_pick_splits(N, Kd, num_sms);
+    cudaEvent_t a, b;
+    if (splits <= 0) splits = gemm_pick_splits(N, Kd, hook_num_sms());
     while (splits > 1 && bpad % splits) splits /= 2;
     const size_t wn = packed_weight_elems(N, Kd);
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&w), wn * 2 * ncopies));
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&x), static_cast<size_t>(2 * bpad) * Kd * 2));
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&zb), static_cast<size_t>(N) * 4));
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&out), static_cast<size_t>(bpad) * N * 4));
+    if (hb.alloc(&w, wn * ncopies) || hb.alloc(&x, static_cast<size_t>(2 * bpad) * Kd) || hb.alloc(&zb, N) ||
+        hb.alloc(&out, static_cast<size_t>(bpad) * N) || hb.event(&a) || hb.event(&b))
+        return -1;
     VCB_CUDA_OK(cudaMemset(w, 0x11, wn * 2 * ncopies));
     VCB_CUDA_OK(cudaMemset(x, 0x11, static_cast<size_t>(2 * bpad) * Kd * 2));
-    VCB_CUDA_OK(cudaMemset(zb, 0, static_cast<size_t>(N) * 4));
     std::vector<CUtensorMap> tmA(ncopies);
     CUtensorMap tmB;
     for (int c = 0; c < ncopies; ++c)
@@ -1852,9 +1835,6 @@ int vcb_bench_gemm(int32_t N, int32_t Kd, int32_t B, int32_t splits, int32_t sta
     g.tmB = &tmB; g.X = x;
     g.ep.mode = EPI_LOGITS; g.ep.bias = zb; g.ep.out = out; g.ep.ld_out = N; g.ep.col_off = 0;
     g.Nout = N; g.Kdim = Kd; g.ldx = Kd; g.bpad = bpad; g.splits = splits; g.nvalid = B; g.stages = stages; g.pdl = pdl;
-    cudaEvent_t a, b;
-    cudaEventCreate(&a);
-    cudaEventCreate(&b);
     for (int it = -3; it < iters; ++it) {
         if (it == 0) cudaEventRecord(a, 0);
         g.tmA = &tmA[(it + 3) % ncopies];
@@ -1866,8 +1846,6 @@ int vcb_bench_gemm(int32_t N, int32_t Kd, int32_t B, int32_t splits, int32_t sta
     float ms = 0.f;
     cudaEventElapsedTime(&ms, a, b);
     *us_out = ms * 1e3f / iters;
-    cudaEventDestroy(a); cudaEventDestroy(b);
-    cudaFree(w); cudaFree(x); cudaFree(zb); cudaFree(out);
     return 0;
 }
 

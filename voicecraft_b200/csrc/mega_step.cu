@@ -16,7 +16,7 @@
 //     (wgmma, 64 features each, fp32 accumulators in registers) and run its epilogue, or do the attention math.
 //   * split-K without clusters: a CTA's partial of a tile goes to an L2-resident workspace; the last CTA to arrive
 //     (atomic counter) sums all partials in contributor order (deterministic) and runs the fused epilogue of
-//     gemm_tcgen05.cu (QKV append, residual + next LayerNorm operand and statistics, ReLU/GELU, logits).
+//     gemm_wgmma.cu (QKV append, residual + next LayerNorm operand and statistics, ReLU/GELU, logits).
 //   * phase hand-over: one completion counter per phase (tiles done / CTAs done), release/acquire at GPU scope; data that
 //     crossed CTAs is read with ld.global.cg (L1 is not coherent inside one kernel) or by TMA after fence.proxy.async.
 //   * attention: same math as attn_rows_kernel (lm_kernels.cuh), but the current token's k/v come from the QKV epilogue's

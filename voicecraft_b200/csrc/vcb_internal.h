@@ -9,7 +9,7 @@
 namespace vcb {
 
 // ---------------------------------------------------------------------------------------------------
-// GEMM (gemm_tcgen05.cu)
+// GEMM (gemm_wgmma.cu)
 // ---------------------------------------------------------------------------------------------------
 enum { EPI_QKV = 0, EPI_RESID = 1, EPI_ACT = 2, EPI_LOGITS = 3 };
 
