@@ -188,10 +188,13 @@ def test_codec_stream_bit_identical_real_shape():
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", ["small_constpad", "two_res_no_lstm", "ws_chunked"])
+@pytest.mark.parametrize("name", ["small_constpad", "two_res_no_lstm", "ws_chunked", "convout_tc", "lstm_wide"])
 def test_codec_stream_bit_identical_variants(name, monkeypatch):
-    if name == "ws_chunked":                                   # a 20 MB workspace: the batch is decoded one utterance at a time
-        monkeypatch.setenv("VCB_CODEC_WS_GB", "0.02")
+    knobs = {"ws_chunked": ("VCB_CODEC_WS_GB", "0.02"),        # a 20 MB workspace: the batch is decoded one utterance at a time
+             "convout_tc": ("VCB_CODEC_CONVOUT_TC", "1"),      # the final conv as one 7-tap GEMM
+             "lstm_wide": ("VCB_CODEC_LSTM_WIDE", "1")}        # 128-column LSTM step tiles
+    if name in knobs:
+        monkeypatch.setenv(*knobs[name])
         cfg, seed = eo.default_config(), 6
     else:
         over, seed = SMALL[name]

@@ -502,6 +502,52 @@ struct Plane {                         // an activation tensor in the workspace
     long long plane() const { return static_cast<long long>(rcap) * C; }
 };
 
+// ---- the decoder plan: the layer sequence over a table of tensors, independent of (B, T).  The launches, the workspace,
+// the stream-state layout and min_T are all derived from it.
+enum { FORM_RAW = 1, FORM_ELU = 2 };
+// HALO_UNWRITTEN: the rows exist (the tensor shares its block input's row geometry) but nothing stores or reads them
+enum { HALO_REFLECT, HALO_ZERO, HALO_UNWRITTEN };
+enum { HOME_ARENA0, HOME_ARENA1, HOME_HIDDEN, HOME_FIXED };   // ping-pong arenas of the stages, hidden arena, fixed region
+
+struct PlanTensor {
+    int C = 0, halo = 0, halo_kind = HALO_ZERO;
+    int up = 1;                        // rows per frame: the product of the ratios so far
+    bool tm = false;                   // time-major, row = (t + halo) * Bcap + b (LSTM planes); else utterance-major
+    int forms = 0;                     // FORM_RAW | FORM_ELU stored
+    int home = HOME_FIXED;
+    bool carried = false;              // stream decode carries its halo rows (of the ELU'd form if stored, else raw) ...
+    size_t state_off = 0;              // ... at this offset of a stream's state
+    std::string dbg_raw, dbg_elu;      // enc_debug_tensor names of the two forms ("": not exposed)
+};
+
+enum { L_RVQ, L_CONV, L_LSTM_IH, L_LSTM_STEPS, L_CONV_OUT_SPLIT, L_CONV_OUT };
+enum { F32_NONE, F32_X0, F32_PRE, F32_COPART, F32_WAV };      // fp32 destination of a GEMM
+
+struct PlanLayer {
+    int kind = L_CONV;
+    const char* label = "";            // VCB_CODEC_PROFILE
+    const TcGemm* g = nullptr;
+    int in = -1, in_form = FORM_RAW;   // A source 0
+    int in2 = -1;                      // A source 1, raw form: the block input of a residual tail (shortcut)
+    int out = -1, out_forms = 0;
+    int f32 = F32_NONE;
+    int nstore = 0;                    // GEMM columns stored
+    int lstm = -1;                     // LSTM layer
+    size_t h_off = 0, c_off = 0;       // LSTM steps: the layer's carried h and c in a stream's state
+};
+
+struct PlanStage { int up, C, Ch; };   // rows per frame, padded channels of the block tensors and of the hidden tensor
+
+struct TcPlan {
+    std::vector<PlanTensor> tensors;
+    std::vector<PlanLayer> layers;
+    std::vector<PlanStage> stages;
+    int u0 = -1;                       // input of the first ConvTranspose (its zero halo is cleared before every chunk)
+    int arena_halo = 1;                // halo rows every arena is sized for
+    int min_T = 8;
+    size_t stream_bytes = 0;           // carried state of one stream
+};
+
 }  // namespace
 
 struct TcCodec {
@@ -511,16 +557,14 @@ struct TcCodec {
     TcGemm conv_in, conv_out;
     TcGemm conv_out_p;                 // final conv as per-tap partial products (N = k), summed by tc_diag_sum_kernel
     bool co_split = false;
-    int lstm_wide = -1;                // VCB_CODEC_LSTM_WIDE: force 64- (0) or 128-column (1) step tiles
     float co_bias = 0.f;
-    std::vector<TcGemm> pre, step, step_wide, up;   // step: 64-column tiles (<= 128 utterances), step_wide: 128-column tiles
+    std::vector<TcGemm> pre, step, up; // step: 64-column tiles, or 128 with VCB_CODEC_LSTM_WIDE=1
     std::vector<std::vector<TcGemm>> res1, res2;
+    TcPlan plan;
     std::vector<void*> owned;
     uint8_t* ws = nullptr;
     size_t ws_bytes = 0;
     size_t ws_limit = 0;
-    int min_T = 8;
-    size_t stream_bytes = 0;           // carried state of one stream (stream decode)
     bool profile = false;
     std::vector<std::pair<std::string, float>> prof;
     struct Dbg { Plane p; const __nv_bfloat16* ptr; int B; };
@@ -675,32 +719,12 @@ int tc_launch_t(const CUtensorMap& a0, const CUtensorMap& a1, const TcGemm& g, c
         attr_set = true;
     }
     const long long tiles = static_cast<long long>(c.mtiles) * c.ntiles;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(static_cast<unsigned>(std::min<long long>(tiles, num_sms)), 1, 1);
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.dynamicSmemBytes = L::TOTAL;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    VCB_CUDA_OK(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, STAGES, CW>, a0, a1, g.tmW, c));
+    VCB_CUDA_OK(launch_k_pdl(1, conv_tc_kernel<BN, STAGES, CW>, dim3(static_cast<unsigned>(std::min<long long>(tiles, num_sms))),
+                             dim3(TC_THREADS), L::TOTAL, st, a0, a1, g.tmW, c));
     return 0;
 }
 
-int tc_launch(TcCodec* tc, const CUtensorMap& a0, const CUtensorMap& a1, const TcGemm& g, TcCall& c, int mtiles, cudaStream_t st) {
-    c.total_kb = g.total_kb;
-    c.ntiles = g.ntiles;
-    c.mtiles = mtiles;
-    c.bias = g.bias;
-    c.up = g.up;
-    c.Cout = g.Cout;
-    for (int i = 0; i < g.total_kb; ++i) c.taps[i] = g.taps[i];
-    if (static_cast<long long>(mtiles) * g.ntiles > 0x7fffffffll) {
-        set_error("codec_tc: too many tiles");
-        return -1;
-    }
+int tc_launch(TcCodec* tc, const CUtensorMap& a0, const CUtensorMap& a1, const TcGemm& g, const TcCall& c, cudaStream_t st) {
     const int sms = tc_num_sms(tc);
     if (g.BN == 128) return tc_launch_t<128, 2, 32>(a0, a1, g, c, sms, st);
     if (g.BN == 64) return tc_launch_t<64, 4, 16>(a0, a1, g, c, sms, st);
@@ -712,69 +736,33 @@ int plane_map(CUtensorMap* tm, const __nv_bfloat16* base, const Plane& p) {
     return make_tmap_bf16_2d(tm, base, 2ull * p.rcap, p.C, p.C, TC_BM);
 }
 
-void set_in(TcCall& c, const Plane& p, int B) {
-    c.rows_total = p.rcap;
-    c.rcap[0] = p.rcap;
-    c.in_tm = p.tm;
-    c.in_div = p.tm ? static_cast<int>(p.st) : p.Tp;
-    c.in_halo = p.halo;
-    c.T_in = p.T;
-    c.B = B;
-}
+inline int bcap(int B) { return (B + 127) / 128 * 128; }
 
-void set_out(TcCall& c, const Plane& p, bool raw, bool elu) {
-    c.raw = raw ? p.raw : nullptr;
-    c.elu = elu ? p.elu : nullptr;
-    c.o_plane = p.plane();
-    c.o_ld = p.C;
-    c.o_sb = p.sb;
-    c.o_st = p.st;
-    c.o_off = p.off;
-    c.o_halo = p.halo;
-    c.o_halo_zero = p.halo_zero;
-}
-
-struct Bump {
-    uint8_t* base;
-    size_t off = 0;
-    void* take(size_t bytes) {
-        void* p = base ? base + off : nullptr;
-        off += align_up(bytes, 1024);
-        return p;
+// a plan tensor's rows for a chunk of B utterances of T frames: utterance-major, every utterance = halo rows + its rows; or
+// time-major, row = (t + halo) * Bcap + b
+Plane geometry(const PlanTensor& t, int B, int T) {
+    Plane p;
+    p.C = t.C;
+    p.T = T * t.up;
+    p.Tp = p.T + t.halo;
+    p.halo = t.halo;
+    p.halo_zero = t.halo_kind == HALO_ZERO;
+    p.tm = t.tm;
+    if (t.tm) {
+        const int Bc = bcap(B);
+        p.rcap = p.Tp * Bc;
+        p.sb = 1;
+        p.st = Bc;
+        p.off = static_cast<long long>(t.halo) * Bc;
+    } else {
+        p.rcap = std::max(B * p.Tp, TC_BM);               // (a TMA box never taller than its tensor)
+        p.sb = p.Tp;
+        p.st = 1;
+        p.off = t.halo;
     }
-};
-
-// utterance-major tensor: every utterance = halo rows + T rows
-Plane make_um(int C, int B, int T, int halo, int halo_zero) {
-    Plane p;
-    p.C = C;
-    p.T = T;
-    p.Tp = T + halo;
-    p.halo = halo;
-    p.halo_zero = halo_zero;
-    p.rcap = std::max(B * p.Tp, TC_BM);               // (a TMA box never taller than its tensor)
-    p.sb = p.Tp;
-    p.st = 1;
-    p.off = halo;
-    p.tm = 0;
     return p;
 }
-// time-major tensor: row = (t + halo) * Bcap + b
-Plane make_tm(int C, int Bcap, int T, int halo) {
-    Plane p;
-    p.C = C;
-    p.T = T;
-    p.Tp = T + halo;
-    p.halo = halo;
-    p.halo_zero = 1;
-    p.rcap = (T + halo) * Bcap;
-    p.sb = 1;
-    p.st = Bcap;
-    p.off = static_cast<long long>(halo) * Bcap;
-    p.tm = 1;
-    return p;
-}
-size_t plane_bytes(const Plane& p, int forms) { return static_cast<size_t>(p.rcap) * p.C * 2 * 2 * forms; }
+size_t form_bytes(const Plane& p) { return static_cast<size_t>(p.rcap) * p.C * 2 * 2; }   // hi + lo planes of one form
 
 struct Prof {
     TcCodec* tc;
@@ -805,369 +793,345 @@ struct Prof {
     }
 };
 
-// One chunk of B utterances.  dry = only measure the workspace (returns bytes through *need).  sc = stream decode: every
-// plane a layer reads as left context, and the LSTM state, continue the utterance's stream (tc_carry_kernel).
-int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T, cudaStream_t st, int64_t* launches, bool dry,
-                    size_t* need, const TcStreamCtx* sc) {
+// The decoder's layers in launch order.  Every halo rule is here: a causal convolution reads (k-1)*dilation rows above its
+// output row, so its input keeps that many halo rows, padded like the reference (reflect or zeros); a ConvTranspose reads
+// x[t-1], so its input keeps one zero row.  A stream's state holds the carried tensors and the LSTM (h, c) per layer, in
+// the order the carries run.
+void build_plan(TcCodec* tc) {
     const enc_config& cf = tc->cfg;
-    const int Bcap = (B + 127) / 128 * 128;
-    const int H = tc->ch0;
-    const int nl = cf.lstm;
-    const int kin = cf.kernel_size, kres = cf.residual_kernel_size, kout = cf.last_kernel_size;
-    const int hz = cf.pad_reflect ? 0 : 1;
-    Bump ws{dry ? nullptr : tc->ws};
-    auto take_planes = [&](Plane& p, bool raw, bool elu) {
-        if (raw) p.raw = static_cast<__nv_bfloat16*>(ws.take(plane_bytes(p, 1)));
-        if (elu) p.elu = static_cast<__nv_bfloat16*>(ws.take(plane_bytes(p, 1)));
+    TcPlan& pl = tc->plan;
+    const int H = tc->ch0, nl = cf.lstm, nres = cf.n_residual_layers;
+    const int kres = cf.residual_kernel_size, kout = cf.last_kernel_size;
+    const int pad = cf.pad_reflect ? HALO_REFLECT : HALO_ZERO;
+    auto tensor = [&](int C, int halo, int kind, int up, bool tm, int forms, int home, bool carried, std::string dbg_raw,
+                      std::string dbg_elu) {
+        PlanTensor t;
+        t.C = C; t.halo = halo; t.halo_kind = kind; t.up = up; t.tm = tm;
+        t.forms = forms; t.home = home; t.carried = carried;
+        t.dbg_raw = std::move(dbg_raw);
+        t.dbg_elu = std::move(dbg_elu);
+        pl.tensors.push_back(t);
+        return static_cast<int>(pl.tensors.size()) - 1;
     };
-    // ---- fixed tensors
-    Plane Z = make_um(tc->Dp, B, T, kin - 1, hz);
-    take_planes(Z, true, false);
-    Plane U0 = make_um(cpad(H), B, T, 1, 1);                       // input of the first ConvTranspose: ELU'd, zero halo
-    take_planes(U0, false, true);
-    Plane X0 = make_tm(H, Bcap, T, 0);                             // conv_in output (LSTM input), time-major
-    Plane HS[2] = {make_tm(H, Bcap, T, 1), make_tm(H, Bcap, T, 1)};
-    float *x0f = nullptr, *pre = nullptr, *cst = nullptr;
-    if (nl > 0) {
-        take_planes(X0, true, false);
-        take_planes(HS[0], true, false);
-        if (nl > 1) take_planes(HS[1], true, false);
-        x0f = static_cast<float*>(ws.take(static_cast<size_t>(T) * Bcap * H * 4));
-        pre = static_cast<float*>(ws.take(static_cast<size_t>(T) * Bcap * 4 * H * 4));
-        cst = static_cast<float*>(ws.take(static_cast<size_t>(nl) * Bcap * H * 4));
-    }
-    // ---- arenas of the up-sampling stages: block input X (raw + ELU), hidden, block output
-    size_t arenaX = 0, arenaH = 0;
-    {
-        int ch = H, t = T;
-        for (int i = 0; i < cf.n_ratios; ++i) {
-            t *= cf.ratios[i];
-            ch /= 2;
-            int maxhalo = std::max(kout - 1, 1);
-            for (int j = 0, d = 1; j < cf.n_residual_layers; ++j, d *= cf.dilation_base) maxhalo = std::max(maxhalo, (kres - 1) * d);
-            const size_t rows = static_cast<size_t>(B) * (t + maxhalo);
-            arenaX = std::max(arenaX, align_up(rows * cpad(ch) * 4, 1024) * 2);
-            arenaH = std::max(arenaH, align_up(rows * cpad(ch / cf.compress) * 4, 1024));
+    auto layer = [](int kind, const char* label, const TcGemm* g, int nstore, int in, int in_form, int out, int out_forms, int f32) {
+        PlanLayer L;
+        L.kind = kind; L.label = label; L.g = g; L.nstore = nstore;
+        L.in = in; L.in_form = in_form; L.out = out; L.out_forms = out_forms; L.f32 = f32;
+        return L;
+    };
+    auto add = [&](PlanLayer L) {
+        if (L.kind == L_LSTM_STEPS) {
+            L.h_off = pl.stream_bytes;
+            L.c_off = pl.stream_bytes + static_cast<size_t>(H) * 4;
+            pl.stream_bytes += static_cast<size_t>(H) * 8;
         }
-    }
-    uint8_t* ar[2];
-    ar[0] = static_cast<uint8_t*>(ws.take(arenaX));
-    ar[1] = static_cast<uint8_t*>(ws.take(arenaX));
-    uint8_t* arh = static_cast<uint8_t*>(ws.take(arenaH));
-    float* copart = nullptr;                                       // per-tap partial products of the final conv
-    if (tc->co_split) {
-        int t = T;
-        for (int i = 0; i < cf.n_ratios; ++i) t *= cf.ratios[i];
-        copart = static_cast<float*>(ws.take((static_cast<size_t>(B) * (t + std::max(kout - 1, 1)) + TC_BM) * DS_LD * 4));
-    }
-    if (need) *need = ws.off;
-    if (dry) return 0;
-    auto place = [&](Plane& p, uint8_t* base, bool raw, bool elu) {
-        Bump b{base};
-        if (raw) p.raw = static_cast<__nv_bfloat16*>(b.take(plane_bytes(p, 1)));
-        if (elu) p.elu = static_cast<__nv_bfloat16*>(b.take(plane_bytes(p, 1)));
+        if (L.out >= 0) {
+            PlanTensor& t = pl.tensors[L.out];
+            if (t.carried && t.halo > 0) {
+                t.state_off = pl.stream_bytes;
+                pl.stream_bytes += static_cast<size_t>(t.halo) * t.C * 4;
+            }
+        }
+        pl.layers.push_back(L);
     };
-    // stream decode: the state of a stream is laid out in the order the carries run (tc_stream_state_bytes is the total)
-    size_t soff = 0;
-    auto take_state = [&](size_t bytes) {
-        const size_t o = soff;
-        soff += bytes;
+    // the input of a ConvTranspose, or of the final conv after the last stage
+    auto feed = [&](bool last_stage, int& halo, int& kind) {
+        halo = last_stage ? kout - 1 : 1;
+        kind = last_stage ? pad : HALO_ZERO;
+    };
+
+    const int z = tensor(tc->Dp, cf.kernel_size - 1, pad, 1, false, FORM_RAW, HOME_FIXED, true, "z", "");
+    pl.u0 = tensor(cpad(H), 1, HALO_ZERO, 1, false, FORM_ELU, HOME_FIXED, true, "", "u0");
+    int x0 = -1, hs[2] = {-1, -1};
+    if (nl > 0) {
+        x0 = tensor(H, 0, HALO_ZERO, 1, true, FORM_RAW, HOME_FIXED, false, "x0", "");
+        for (int l = 0; l < std::min(nl, 2); ++l)                 // h planes: slot t+1 = h_t, layers alternate
+            hs[l] = tensor(H, 1, HALO_ZERO, 1, true, FORM_RAW, HOME_FIXED, false, "hs" + std::to_string(l), "");
+    }
+    add(layer(L_RVQ, "rvq", nullptr, 0, -1, 0, z, FORM_RAW, F32_NONE));
+    if (nl > 0) add(layer(L_CONV, "conv_in", &tc->conv_in, cpad(H), z, FORM_RAW, x0, FORM_RAW, F32_X0));
+    else add(layer(L_CONV, "conv_in", &tc->conv_in, cpad(H), z, FORM_RAW, pl.u0, FORM_ELU, F32_NONE));
+    for (int l = 0; l < nl; ++l) {
+        PlanLayer ih = layer(L_LSTM_IH, "lstm_ih", &tc->pre[l], 4 * H, l == 0 ? x0 : hs[(l - 1) & 1], FORM_RAW, -1, 0, F32_PRE);
+        ih.lstm = l;
+        add(ih);
+        // the last layer's epilogue writes ELU(h + skip) straight into the first ConvTranspose's input
+        const bool last = l == nl - 1;
+        PlanLayer steps = layer(L_LSTM_STEPS, "lstm_steps", &tc->step[l], 4 * H, hs[l & 1], FORM_RAW, last ? pl.u0 : -1,
+                                last ? FORM_ELU : 0, F32_NONE);
+        steps.lstm = l;
+        add(steps);
+    }
+    // up-sampling stages: ConvTranspose -> X; per residual block conv1 (on ELU(X)) -> hidden, then conv2 (on the hidden) +
+    // shortcut (on raw X) -> O, the next block's X.  X and O alternate between the two arenas.
+    int cur = pl.u0, ch = H, up = 1, side = HOME_ARENA0;
+    for (int i = 0; i < cf.n_ratios; ++i) {
+        const int r = cf.ratios[i], cout = ch / 2, hidden = cout / cf.compress;
+        const bool last_stage = i == cf.n_ratios - 1;
+        const std::string s = std::to_string(i + 1);
+        ch = cout;
+        up *= r;
+        pl.stages.push_back(PlanStage{up, cpad(cout), cpad(hidden)});
+        int halo = kres - 1, kind = pad;
+        if (nres == 0) feed(last_stage, halo, kind);
+        int x = tensor(cpad(cout), halo, kind, up, false, (nres > 0 ? FORM_RAW : 0) | FORM_ELU, side, true,
+                       nres > 0 ? "x" + s + ".raw" : "", "x" + s + ".elu");
+        add(layer(L_CONV, "convtr", &tc->up[i], r * cpad(cout), cur, FORM_ELU, x, pl.tensors[x].forms, F32_NONE));
+        for (int j = 0, dil = 1; j < nres; ++j, dil *= cf.dilation_base) {
+            const std::string sj = s + "." + std::to_string(j);
+            const int hd = tensor(cpad(hidden), pl.tensors[x].halo, HALO_UNWRITTEN, up, false, FORM_ELU, HOME_HIDDEN, false, "",
+                                  "h" + sj);
+            add(layer(L_CONV, "res_conv1", &tc->res1[i][j], cpad(hidden), x, FORM_ELU, hd, FORM_ELU, F32_NONE));
+            // the next block's conv1 reads (kres-1) * its dilation rows back.  min_T takes this term for the last block too.
+            const int next = (kres - 1) * dil * cf.dilation_base;
+            pl.min_T = std::max(pl.min_T, next + 2);
+            halo = next;
+            kind = pad;
+            if (j == nres - 1) feed(last_stage, halo, kind);
+            const int o = tensor(cpad(cout), halo, kind, up, false, (j < nres - 1 ? FORM_RAW : 0) | FORM_ELU, side ^ 1, true, "",
+                                 "o" + sj);
+            PlanLayer tail = layer(L_CONV, "res_conv2", &tc->res2[i][j], cpad(cout), hd, FORM_ELU, o, pl.tensors[o].forms, F32_NONE);
+            tail.in2 = x;
+            add(tail);
+            x = o;
+            side ^= 1;
+        }
+        cur = x;
+        side ^= 1;                                                 // the next ConvTranspose must not write over `cur`
+    }
+    // final conv: k <= DS_LD partial products (the first 16-column chunk), or one output column (f_valid = 1)
+    if (tc->co_split) add(layer(L_CONV_OUT_SPLIT, "conv_out", &tc->conv_out_p, 16, cur, FORM_ELU, -1, 0, F32_COPART));
+    else add(layer(L_CONV_OUT, "conv_out", &tc->conv_out, 32, cur, FORM_ELU, -1, 0, F32_WAV));
+    pl.min_T = std::max(pl.min_T, std::max(cf.kernel_size, kout) + 1);
+    for (const PlanTensor& t : pl.tensors)
+        if (t.home != HOME_FIXED) pl.arena_halo = std::max(pl.arena_halo, t.halo);
+}
+
+// The workspace of a chunk: the fixed tensors, the fp32 buffers, the two stage arenas, the hidden arena, the final conv's
+// partial products.  tensor[i] = offset of plan tensor i's first stored form (an ELU'd form follows a raw one).
+struct WsLayout {
+    std::vector<size_t> tensor;
+    size_t x0f = 0, pre = 0, cst = 0, copart = 0, bytes = 0;
+};
+
+WsLayout ws_layout(const TcCodec* tc, int B, int T) {
+    const TcPlan& pl = tc->plan;
+    const int Bcap = bcap(B), H = tc->ch0, nl = tc->cfg.lstm;
+    WsLayout w;
+    w.tensor.resize(pl.tensors.size());
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        const size_t o = off;
+        off += align_up(bytes, 1024);
         return o;
     };
+    for (size_t i = 0; i < pl.tensors.size(); ++i) {
+        const PlanTensor& t = pl.tensors[i];
+        if (t.home != HOME_FIXED) continue;
+        w.tensor[i] = off;
+        for (int f : {FORM_RAW, FORM_ELU})
+            if (t.forms & f) take(form_bytes(geometry(t, B, T)));
+    }
+    if (nl > 0) {
+        w.x0f = take(static_cast<size_t>(T) * Bcap * H * 4);
+        w.pre = take(static_cast<size_t>(T) * Bcap * 4 * H * 4);
+        w.cst = take(static_cast<size_t>(nl) * Bcap * H * 4);
+    }
+    size_t ax = 0, ah = 0;
+    for (const PlanStage& s : pl.stages) {
+        const size_t rows = static_cast<size_t>(B) * (T * s.up + pl.arena_halo);
+        ax = std::max(ax, align_up(rows * s.C * 4, 1024) * 2);
+        ah = std::max(ah, align_up(rows * s.Ch * 4, 1024));
+    }
+    const size_t region[3] = {take(ax), take(ax), take(ah)};
+    for (size_t i = 0; i < pl.tensors.size(); ++i)
+        if (pl.tensors[i].home != HOME_FIXED) w.tensor[i] = region[pl.tensors[i].home];
+    if (tc->co_split) {
+        const PlanTensor& in = pl.tensors[pl.layers.back().in];
+        w.copart = take((static_cast<size_t>(B) * (T * in.up + std::max(in.halo, 1)) + TC_BM) * DS_LD * 4);
+    }
+    w.bytes = off;
+    return w;
+}
+
+// One chunk of B utterances.  sc = stream decode: every plane a layer reads as left context, and the LSTM state, continue
+// the utterance's stream (tc_carry_kernel).
+int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T, cudaStream_t st, int64_t* launches,
+                    const TcStreamCtx* sc) {
+    const TcPlan& pl = tc->plan;
+    const enc_config& cf = tc->cfg;
+    const int Bcap = bcap(B), H = tc->ch0, nl = cf.lstm;
+    const WsLayout w = ws_layout(tc, B, T);
+    std::vector<Plane> P(pl.tensors.size());
+    tc->dbg.clear();
+    for (size_t i = 0; i < P.size(); ++i) {
+        const PlanTensor& t = pl.tensors[i];
+        Plane& p = P[i];
+        p = geometry(t, B, T);
+        uint8_t* base = tc->ws + w.tensor[i];
+        if (t.forms & FORM_RAW) {
+            p.raw = reinterpret_cast<__nv_bfloat16*>(base);
+            base += align_up(form_bytes(p), 1024);
+        }
+        if (t.forms & FORM_ELU) p.elu = reinterpret_cast<__nv_bfloat16*>(base);
+        if (!t.dbg_raw.empty()) tc->dbg[t.dbg_raw] = TcCodec::Dbg{p, p.raw, B};
+        if (!t.dbg_elu.empty()) tc->dbg[t.dbg_elu] = TcCodec::Dbg{p, p.elu, B};
+    }
+    float* x0f = reinterpret_cast<float*>(tc->ws + w.x0f);
+    float* pre = reinterpret_cast<float*>(tc->ws + w.pre);
+    float* cst = reinterpret_cast<float*>(tc->ws + w.cst);
+    float* copart = reinterpret_cast<float*>(tc->ws + w.copart);
+
+    // state that the kernels only ever read: U0's zero halo (the LSTM epilogue writes none), c_0 and h_{-1}
+    const Plane& u0 = P[pl.u0];
+    VCB_CUDA_OK(cudaMemset2DAsync(u0.elu, static_cast<size_t>(u0.Tp) * u0.C * 2, 0, static_cast<size_t>(u0.C) * 2, B, st));
+    VCB_CUDA_OK(cudaMemset2DAsync(u0.elu + u0.plane(), static_cast<size_t>(u0.Tp) * u0.C * 2, 0, static_cast<size_t>(u0.C) * 2, B, st));
+    auto clear_h0 = [&](const Plane& hs) -> int {
+        VCB_CUDA_OK(cudaMemsetAsync(hs.raw, 0, static_cast<size_t>(Bcap) * H * 2, st));
+        VCB_CUDA_OK(cudaMemsetAsync(hs.raw + hs.plane(), 0, static_cast<size_t>(Bcap) * H * 2, st));
+        return 0;
+    };
+    if (nl > 0) {
+        VCB_CUDA_OK(cudaMemsetAsync(cst, 0, static_cast<size_t>(nl) * Bcap * H * 4, st));
+        for (const PlanLayer& L : pl.layers)
+            if (L.kind == L_LSTM_STEPS && L.lstm < 2 && clear_h0(P[L.in])) return -1;
+    }
+
     auto carry = [&](void* base, long long plane_bytes, long long sb, long long stt, long long off, int row_bytes, int halo, int up,
                      int restore, int save, size_t state_off) -> int {
-        CarryArgs a;
-        a.base = static_cast<uint8_t*>(base);
-        a.plane_bytes = plane_bytes;
-        a.sb = sb; a.st = stt; a.off = off;
-        a.row_bytes = row_bytes;
-        a.halo = halo; a.up = up;
-        a.restore = restore; a.save = save;
-        a.table = sc->table;
-        a.state = sc->state;
-        a.state_stride = static_cast<long long>(tc->stream_bytes);
-        a.state_off = static_cast<long long>(state_off);
-        cudaLaunchConfig_t lc = {};
-        lc.gridDim = dim3(B);
-        lc.blockDim = dim3(256);
-        lc.stream = st;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = 1;
-        lc.attrs = at;
-        lc.numAttrs = 1;
-        VCB_CUDA_OK(cudaLaunchKernelEx(&lc, tc_carry_kernel, a));
+        const CarryArgs a{static_cast<uint8_t*>(base), plane_bytes, sb, stt, off, row_bytes, halo, up, restore, save, sc->table,
+                          sc->state, static_cast<long long>(pl.stream_bytes), static_cast<long long>(state_off)};
+        VCB_CUDA_OK(launch_k_pdl(1, tc_carry_kernel, dim3(B), dim3(256), 0, st, a));
         ++*launches;
         return 0;
     };
     // a plane's halo: restore a continuing stream's tail over the padding the producer wrote, save the new tail
-    auto carry_plane = [&](const Plane& p, __nv_bfloat16* base, int up) -> int {
-        if (sc == nullptr || p.halo == 0) return 0;
-        const size_t o = take_state(static_cast<size_t>(p.halo) * p.C * 4);
-        return carry(base, p.plane() * 2, p.sb, p.st, p.off, p.C * 2, p.halo, up, 1, 1, o);
+    auto carry_plane = [&](int i) -> int {
+        const PlanTensor& t = pl.tensors[i];
+        const Plane& p = P[i];
+        if (sc == nullptr || !t.carried || p.halo == 0) return 0;
+        return carry(p.elu ? p.elu : p.raw, p.plane() * 2, p.sb, p.st, p.off, p.C * 2, p.halo, t.up, 1, 1, t.state_off);
+    };
+    // stream decode: h_{-1} (slot 0) and c continue the stream; after the layer, h of the last valid step (slot frames) and
+    // the frozen c are saved.  As a time-major plane with one halo row, row(b, t) = (t + 1) * Bcap + b.
+    auto carry_lstm = [&](const PlanLayer& L, const Plane& hs, float* cl, int restore, int save) -> int {
+        if (sc == nullptr) return 0;
+        return carry(hs.raw, hs.plane() * 2, hs.sb, hs.st, hs.off, H * 2, 1, 1, restore, save, L.h_off) ||
+               carry(cl, 0, 1, 0, 0, H * 4, 1, 1, restore, save, L.c_off);
+    };
+    // the call of a plan GEMM: its weights, its A rows, its epilogue (the LSTM steps then only move t_step and row_base)
+    auto gemm_call = [&](const PlanLayer& L, TcCall& c) -> int {
+        const TcGemm& g = *L.g;
+        const Plane& in = P[L.in];
+        c = TcCall{};
+        c.mtiles = ((L.kind == L_LSTM_STEPS ? B : in.rcap) + TC_BM - 1) / TC_BM;
+        if (static_cast<long long>(c.mtiles) * g.ntiles > 0x7fffffffll) {
+            set_error("codec_tc: too many tiles");
+            return -1;
+        }
+        c.total_kb = g.total_kb;
+        c.ntiles = g.ntiles;
+        c.bias = g.bias;
+        c.up = g.up;
+        c.Cout = g.Cout;
+        std::copy(g.taps.begin(), g.taps.end(), c.taps);
+        c.Nstore = L.nstore;
+        c.rows_total = in.rcap;
+        c.rcap[0] = in.rcap;
+        c.B = B;
+        if (L.kind != L_LSTM_STEPS) {
+            c.in_tm = in.tm;
+            c.in_div = in.tm ? static_cast<int>(in.st) : in.Tp;
+            c.in_halo = in.halo;
+            c.T_in = in.T;
+        }
+        if (L.in2 >= 0) c.rcap[1] = P[L.in2].rcap;
+        if (L.out >= 0) {
+            const Plane& o = P[L.out];
+            c.raw = L.out_forms & FORM_RAW ? o.raw : nullptr;
+            c.elu = L.out_forms & FORM_ELU ? o.elu : nullptr;
+            c.o_plane = o.plane();
+            c.o_ld = o.C;
+            c.o_sb = o.sb;
+            c.o_st = o.st;
+            c.o_off = o.off;
+            c.o_halo = pl.tensors[L.out].halo_kind == HALO_UNWRITTEN ? 0 : o.halo;
+            c.o_halo_zero = o.halo_zero;
+        }
+        auto rows = [&](float* f, int ld, long long sb, long long stt, long long off) {
+            c.f32 = f;
+            c.f_ld = ld;
+            c.f_valid = ld;
+            c.f_sb = sb;
+            c.f_st = stt;
+            c.f_off = off;
+        };
+        if (L.f32 == F32_X0) rows(x0f, H, 1, Bcap, 0);                // time-major [T][Bcap][H]
+        if (L.f32 == F32_PRE) rows(pre, 4 * H, 1, Bcap, 0);           // time-major [T][Bcap][4H]
+        if (L.f32 == F32_COPART) {                                    // the input's rows, halo included
+            rows(copart, DS_LD, in.sb, 1, in.off);
+            c.in_store_halo = 1;
+        }
+        if (L.f32 == F32_WAV) {                                       // [B][T * hop]
+            rows(wav, 1, in.T, 1, 0);
+            c.f_scalar = 1;
+        }
+        if (L.kind == L_LSTM_STEPS) {
+            c.mode = TC_MODE_LSTM;
+            c.pre = pre;
+            c.cst = cst + static_cast<size_t>(L.lstm) * Bcap * H;
+            c.hseq = in.raw;
+            c.h_plane = in.plane();
+            c.Bcap = Bcap;
+            c.H = H;
+            if (L.out >= 0) c.skip = x0f;
+            if (sc != nullptr) c.stab = sc->table;
+        }
+        return 0;
     };
 
     Prof pf{tc, st};
     CUtensorMap mA, mB;
-    tc->dbg.clear();
-    auto note = [&](const std::string& name, const Plane& p, const __nv_bfloat16* ptr) { tc->dbg[name] = TcCodec::Dbg{p, ptr, B}; };
-    note("z", Z, Z.raw);
-    note("u0", U0, U0.elu);
-    if (nl > 0) {
-        note("x0", X0, X0.raw);
-        note("hs0", HS[0], HS[0].raw);
-        if (nl > 1) note("hs1", HS[1], HS[1].raw);
-    }
-    // state that the kernels only ever read: zero halos / initial LSTM state
-    VCB_CUDA_OK(cudaMemset2DAsync(U0.elu, static_cast<size_t>(U0.Tp) * U0.C * 2, 0, static_cast<size_t>(U0.C) * 2, B, st));
-    VCB_CUDA_OK(cudaMemset2DAsync(U0.elu + U0.plane(), static_cast<size_t>(U0.Tp) * U0.C * 2, 0, static_cast<size_t>(U0.C) * 2, B, st));
-    if (nl > 0) {
-        VCB_CUDA_OK(cudaMemsetAsync(cst, 0, static_cast<size_t>(nl) * Bcap * H * 4, st));
-        for (int l = 0; l < std::min(nl, 2); ++l) {
-            VCB_CUDA_OK(cudaMemsetAsync(HS[l].raw, 0, static_cast<size_t>(Bcap) * H * 2, st));
-            VCB_CUDA_OK(cudaMemsetAsync(HS[l].raw + HS[l].plane(), 0, static_cast<size_t>(Bcap) * H * 2, st));
-        }
-    }
-    // ---- RVQ decode -> latent planes
-    pf.begin("rvq");
-    tc_rvq_planes_kernel<<<dim3((T + 15) / 16, B), 128, 0, st>>>(reinterpret_cast<const long long*>(codes), tc->d_embed, Z.raw,
-                                                                 Z.plane(), cf.n_q, tc->D, Z.C, T, Z.Tp, Z.halo, Z.halo_zero);
-    VCB_CUDA_OK(cudaGetLastError());
-    ++*launches;
-    if (carry_plane(Z, Z.raw, 1)) return -1;
-    pf.end();
-    // ---- conv_in
-    pf.begin("conv_in");
-    {
-        TcCall c;
-        memset(&c, 0, sizeof(c));
-        set_in(c, Z, B);
-        c.Nstore = cpad(H);
-        if (nl > 0) {
-            set_out(c, X0, true, false);
-            c.f32 = x0f;
-            c.f_ld = H; c.f_valid = H; c.f_sb = 1; c.f_st = Bcap; c.f_off = 0;
+    TcCall c;
+    for (const PlanLayer& L : pl.layers) {
+        pf.begin(L.label);
+        if (L.kind == L_RVQ) {
+            const Plane& z = P[L.out];
+            tc_rvq_planes_kernel<<<dim3((T + 15) / 16, B), 128, 0, st>>>(reinterpret_cast<const long long*>(codes), tc->d_embed, z.raw,
+                                                                         z.plane(), cf.n_q, tc->D, z.C, T, z.Tp, z.halo, z.halo_zero);
+            VCB_CUDA_OK(cudaGetLastError());
+            ++*launches;
         } else {
-            set_out(c, U0, false, true);
-        }
-        if (plane_map(&mA, Z.raw, Z)) return -1;
-        if (tc_launch(tc, mA, mA, tc->conv_in, c, (Z.rcap + TC_BM - 1) / TC_BM, st)) return -1;
-        ++*launches;
-        if (nl == 0 && carry_plane(U0, U0.elu, 1)) return -1;
-    }
-    pf.end();
-    // ---- LSTM stack with skip
-    for (int l = 0; l < nl; ++l) {
-        const Plane& in = l == 0 ? X0 : HS[(l - 1) & 1];
-        Plane& hs = HS[l & 1];
-        if (l >= 2) {
-            VCB_CUDA_OK(cudaMemsetAsync(hs.raw, 0, static_cast<size_t>(Bcap) * H * 2, st));
-            VCB_CUDA_OK(cudaMemsetAsync(hs.raw + hs.plane(), 0, static_cast<size_t>(Bcap) * H * 2, st));
-        }
-        pf.begin("lstm_ih");
-        {
-            TcCall c;
-            memset(&c, 0, sizeof(c));
-            set_in(c, in, B);
-            c.Nstore = 4 * H;
-            c.f32 = pre;
-            c.f_ld = 4 * H; c.f_valid = 4 * H; c.f_sb = 1; c.f_st = Bcap; c.f_off = 0;
-            if (plane_map(&mA, in.raw, in)) return -1;
-            if (tc_launch(tc, mA, mA, tc->pre[l], c, (in.rcap + TC_BM - 1) / TC_BM, st)) return -1;
-            ++*launches;
-        }
-        pf.end();
-        pf.begin("lstm_steps");
-        {
-            TcCall c;
-            memset(&c, 0, sizeof(c));
-            c.mode = TC_MODE_LSTM;
-            c.rcap[0] = hs.rcap;
-            c.rows_total = hs.rcap;
-            c.B = B;
-            c.Nstore = 4 * H;
-            c.pre = pre;
-            c.cst = cst + static_cast<size_t>(l) * Bcap * H;
-            c.hseq = hs.raw;
-            c.h_plane = hs.plane();
-            c.Bcap = Bcap;
-            c.H = H;
-            if (l == nl - 1) {
-                c.skip = x0f;
-                set_out(c, U0, false, true);
-            }
-            // stream decode: h_{-1} (slot 0) and c continue the stream; after the layer, h of the last valid step (slot
-            // frames) and the frozen c are saved.  As a time-major plane with one halo row, row(b, t) = (t + 1) * Bcap + b.
-            float* cl = c.cst;
-            size_t oh = 0, oc = 0;
-            if (sc != nullptr) {
-                c.stab = sc->table;
-                oh = take_state(static_cast<size_t>(H) * 4);
-                oc = take_state(static_cast<size_t>(H) * 4);
-                if (carry(hs.raw, hs.plane() * 2, hs.sb, hs.st, hs.off, H * 2, 1, 1, 1, 0, oh) ||
-                    carry(cl, 0, 1, 0, 0, H * 4, 1, 1, 1, 0, oc))
-                    return -1;
-            }
-            if (plane_map(&mA, hs.raw, hs)) return -1;
-            const int mt = (B + TC_BM - 1) / TC_BM;
-            // 128-column tiles would move fewer bytes through L2 per step (VCB_CODEC_LSTM_WIDE=1); 64-column tiles keep
-            // more CTAs on the 16-k-block pipeline of each step
-            const bool wide = tc->lstm_wide > 0;
-            const TcGemm& sg = wide ? tc->step_wide[l] : tc->step[l];
-            for (int t = 0; t < T; ++t) {
-                c.t_step = t;
-                c.row_base = t * Bcap;
-                if (tc_launch(tc, mA, mA, sg, c, mt, st)) return -1;
-            }
-            *launches += T;
-            if (sc != nullptr && (carry(hs.raw, hs.plane() * 2, hs.sb, hs.st, hs.off, H * 2, 1, 1, 0, 1, oh) ||
-                                  carry(cl, 0, 1, 0, 0, H * 4, 1, 1, 0, 1, oc)))
+            const Plane& in = P[L.in];
+            if (gemm_call(L, c) || plane_map(&mA, L.in_form == FORM_ELU ? in.elu : in.raw, in) ||
+                (L.in2 >= 0 && plane_map(&mB, P[L.in2].raw, P[L.in2])))
                 return -1;
-        }
-        pf.end();
-    }
-    if (nl > 0 && carry_plane(U0, U0.elu, 1)) return -1;
-    // ---- up-sampling stages
-    Plane cur = U0;                                                // ELU'd input of the next ConvTranspose
-    int ch = H, t_cur = T, side = 0;
-    for (int i = 0; i < cf.n_ratios; ++i) {
-        const int r = cf.ratios[i];
-        const int cout = ch / 2, hidden = cout / cf.compress;
-        const bool last_stage = i == cf.n_ratios - 1;
-        // ConvTranspose -> X (raw + ELU, halo for the first residual conv)
-        Plane X = make_um(cpad(cout), B, t_cur * r, cf.n_residual_layers > 0 ? (kres - 1) : (last_stage ? kout - 1 : 1),
-                          cf.n_residual_layers > 0 ? hz : (last_stage ? hz : 1));
-        place(X, ar[side], cf.n_residual_layers > 0, true);
-        note("x" + std::to_string(i + 1) + ".elu", X, X.elu);
-        if (X.raw) note("x" + std::to_string(i + 1) + ".raw", X, X.raw);
-        pf.begin("convtr");
-        {
-            TcCall c;
-            memset(&c, 0, sizeof(c));
-            set_in(c, cur, B);
-            c.Nstore = r * cpad(cout);
-            set_out(c, X, cf.n_residual_layers > 0, true);
-            if (plane_map(&mA, cur.elu, cur)) return -1;
-            if (tc_launch(tc, mA, mA, tc->up[i], c, (cur.rcap + TC_BM - 1) / TC_BM, st)) return -1;
-            ++*launches;
-        }
-        ch = cout;
-        t_cur *= r;
-        if (carry_plane(X, X.elu, t_cur / T)) return -1;
-        pf.end();
-        int dil = 1;
-        for (int j = 0; j < cf.n_residual_layers; ++j, dil *= cf.dilation_base) {
-            const bool last_res = j == cf.n_residual_layers - 1;
-            // conv1 (k3, dilated) on ELU(X) -> hidden, stored ELU'd, in X's row geometry (it is an A source next to X)
-            Plane Hd = X;
-            Hd.C = cpad(hidden);
-            Hd.raw = nullptr;
-            Hd.halo_zero = 0;
-            place(Hd, arh, false, true);
-            note("h" + std::to_string(i + 1) + "." + std::to_string(j), Hd, Hd.elu);
-            pf.begin("res_conv1");
-            {
-                TcCall c;
-                memset(&c, 0, sizeof(c));
-                set_in(c, X, B);
-                c.Nstore = cpad(hidden);
-                set_out(c, Hd, false, true);
-                c.o_halo = 0;
-                if (plane_map(&mA, X.elu, X)) return -1;
-                if (tc_launch(tc, mA, mA, tc->res1[i][j], c, (X.rcap + TC_BM - 1) / TC_BM, st)) return -1;
+            const CUtensorMap& a1 = L.in2 >= 0 ? mB : mA;
+            if (L.kind == L_LSTM_STEPS) {
+                if (L.lstm >= 2 && clear_h0(in)) return -1;
+                if (carry_lstm(L, in, c.cst, 1, 0)) return -1;
+                for (int t = 0; t < T; ++t) {
+                    c.t_step = t;
+                    c.row_base = t * Bcap;
+                    if (tc_launch(tc, mA, a1, *L.g, c, st)) return -1;
+                }
+                *launches += T;
+                if (carry_lstm(L, in, c.cst, 0, 1)) return -1;
+            } else {
+                if (tc_launch(tc, mA, a1, *L.g, c, st)) return -1;
                 ++*launches;
             }
-            pf.end();
-            // conv2 (k1 on ELU(hidden)) + shortcut (k1 on raw X) -> next tensor
-            Plane O;
-            if (!last_res) O = make_um(cpad(ch), B, t_cur, (kres - 1) * dil * cf.dilation_base, hz);
-            else if (last_stage) O = make_um(cpad(ch), B, t_cur, kout - 1, hz);
-            else O = make_um(cpad(ch), B, t_cur, 1, 1);
-            place(O, ar[side ^ 1], !last_res, true);
-            note("o" + std::to_string(i + 1) + "." + std::to_string(j), O, O.elu);
-            pf.begin("res_conv2");
-            {
-                TcCall c;
-                memset(&c, 0, sizeof(c));
-                set_in(c, Hd, B);
-                c.rcap[1] = X.rcap;
-                c.Nstore = cpad(ch);
-                set_out(c, O, !last_res, true);
-                if (plane_map(&mA, Hd.elu, Hd) || plane_map(&mB, X.raw, X)) return -1;
-                if (tc_launch(tc, mA, mB, tc->res2[i][j], c, (X.rcap + TC_BM - 1) / TC_BM, st)) return -1;
+            if (L.kind == L_CONV_OUT_SPLIT) {
+                VCB_CUDA_OK(launch_k_pdl(1, tc_diag_sum_kernel, dim3((in.rcap + DS_ROWS - 1) / DS_ROWS), dim3(DS_ROWS), 0, st,
+                                         copart, cf.last_kernel_size, tc->co_bias, wav, in.rcap, in.Tp, in.halo, in.T, B));
                 ++*launches;
             }
-            if (carry_plane(O, O.elu, t_cur / T)) return -1;
-            pf.end();
-            X = O;
-            side ^= 1;
         }
-        cur = X;
-        side ^= 1;                                                 // the next ConvTranspose must not write over `cur`
+        if (L.out >= 0 && carry_plane(L.out)) return -1;
+        pf.end();
     }
-    // ---- conv_out -> waveform
-    pf.begin("conv_out");
-    if (tc->co_split) {
-        TcCall c;
-        memset(&c, 0, sizeof(c));
-        set_in(c, cur, B);
-        c.in_store_halo = 1;
-        c.Nstore = 16;
-        c.f32 = copart;
-        c.f_ld = DS_LD; c.f_valid = DS_LD; c.f_sb = cur.sb; c.f_st = 1; c.f_off = cur.off;
-        if (plane_map(&mA, cur.elu, cur)) return -1;
-        if (tc_launch(tc, mA, mA, tc->conv_out_p, c, (cur.rcap + TC_BM - 1) / TC_BM, st)) return -1;
-        cudaLaunchConfig_t lc = {};
-        lc.gridDim = dim3((cur.rcap + DS_ROWS - 1) / DS_ROWS);
-        lc.blockDim = dim3(DS_ROWS);
-        lc.stream = st;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = 1;
-        lc.attrs = at;
-        lc.numAttrs = 1;
-        VCB_CUDA_OK(cudaLaunchKernelEx(&lc, tc_diag_sum_kernel, static_cast<const float*>(copart), kout, tc->co_bias, wav, cur.rcap,
-                                       cur.Tp, cur.halo, t_cur, B));
-        *launches += 2;
-    } else {
-        TcCall c;
-        memset(&c, 0, sizeof(c));
-        set_in(c, cur, B);
-        c.Nstore = 32;
-        c.f32 = wav;
-        c.f_ld = 1; c.f_valid = 1; c.f_scalar = 1; c.f_sb = t_cur; c.f_st = 1; c.f_off = 0;
-        if (plane_map(&mA, cur.elu, cur)) return -1;
-        if (tc_launch(tc, mA, mA, tc->conv_out, c, (cur.rcap + TC_BM - 1) / TC_BM, st)) return -1;
-        ++*launches;
-    }
-    pf.end();
     pf.finish();
-    if (sc != nullptr && soff != tc->stream_bytes) {
-        set_error("codec_tc: stream state layout mismatch (%zu carried, %zu per stream)", soff, tc->stream_bytes);
-        return -1;
-    }
     return 0;
-}
-
-// bytes of carried state per stream, in the carry order of decode_chunk_tc: the latent Z, the LSTM (h, c) per layer, U0, then
-// per stage the ConvTranspose output and every residual-block output; a plane carries its halo rows as bf16 hi + lo
-size_t stream_state_bytes(const TcCodec* tc) {
-    const enc_config& cf = tc->cfg;
-    const int H = tc->ch0, kres = cf.residual_kernel_size, kout = cf.last_kernel_size;
-    size_t rows_x_c = static_cast<size_t>(cf.kernel_size - 1) * tc->Dp + static_cast<size_t>(cpad(H));
-    size_t bytes = static_cast<size_t>(cf.lstm) * H * 8;
-    int ch = H;
-    for (int i = 0; i < cf.n_ratios; ++i) {
-        const int cout = ch / 2;
-        const bool last_stage = i == cf.n_ratios - 1;
-        rows_x_c += static_cast<size_t>(cf.n_residual_layers > 0 ? kres - 1 : (last_stage ? kout - 1 : 1)) * cpad(cout);
-        for (int j = 0, d = 1; j < cf.n_residual_layers; ++j, d *= cf.dilation_base) {
-            const bool last_res = j == cf.n_residual_layers - 1;
-            rows_x_c += static_cast<size_t>(!last_res ? (kres - 1) * d * cf.dilation_base : (last_stage ? kout - 1 : 1)) * cpad(cout);
-        }
-        ch = cout;
-    }
-    return bytes + rows_x_c * 4;
 }
 
 }  // namespace
@@ -1203,7 +1167,9 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w
         if (getenv("VCB_CODEC_GRID")) tc->num_sms = std::max(1, atoi(getenv("VCB_CODEC_GRID")));
     }
     tc->profile = getenv("VCB_CODEC_PROFILE") && atoi(getenv("VCB_CODEC_PROFILE")) != 0;
-    if (getenv("VCB_CODEC_LSTM_WIDE")) tc->lstm_wide = atoi(getenv("VCB_CODEC_LSTM_WIDE"));
+    // LSTM step tiles: 128 columns move fewer bytes through L2 per step (VCB_CODEC_LSTM_WIDE=1); 64 keep more CTAs on the
+    // 16-k-block pipeline of each step
+    const int step_bn = getenv("VCB_CODEC_LSTM_WIDE") && atoi(getenv("VCB_CODEC_LSTM_WIDE")) > 0 ? 128 : 64;
     const char* lim = getenv("VCB_CODEC_WS_GB");
     tc->ws_limit = static_cast<size_t>((lim ? atof(lim) : 100.0) * (1ull << 30));
     HostW hw{w_dev, shapes};
@@ -1231,7 +1197,6 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w
     if (!rc) rc = build_conv(tc, tc->conv_in, hw, "dec.conv_in", cfg.dimension, ch0, cfg.kernel_size, 1);
     tc->pre.resize(cfg.lstm);
     tc->step.resize(cfg.lstm);
-    tc->step_wide.resize(cfg.lstm);
     for (int l = 0; l < cfg.lstm && !rc; ++l) {
         char a[96], b[96], c2[96];
         snprintf(a, sizeof(a), "dec.lstm.weight_ih_l%d", l);
@@ -1239,8 +1204,7 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w
         snprintf(c2, sizeof(c2), "dec.lstm.bias_hh_l%d", l);
         rc = build_lstm(tc, tc->pre[l], hw, a, b, c2, ch0, 0);
         snprintf(a, sizeof(a), "dec.lstm.weight_hh_l%d", l);
-        if (!rc) rc = build_lstm(tc, tc->step[l], hw, a, "", "", ch0, 64);
-        if (!rc) rc = build_lstm(tc, tc->step_wide[l], hw, a, "", "", ch0, 128);
+        if (!rc) rc = build_lstm(tc, tc->step[l], hw, a, "", "", ch0, step_bn);
     }
     tc->up.resize(cfg.n_ratios);
     tc->res1.resize(cfg.n_ratios);
@@ -1252,13 +1216,11 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w
         ch /= 2;
         tc->res1[i].resize(cfg.n_residual_layers);
         tc->res2[i].resize(cfg.n_residual_layers);
-        int dil = 1;
-        for (int j = 0; j < cfg.n_residual_layers && !rc; ++j, dil *= cfg.dilation_base) {
+        for (int j = 0, dil = 1; j < cfg.n_residual_layers && !rc; ++j, dil *= cfg.dilation_base) {
             snprintf(nm, sizeof(nm), "dec.up%d.res%d.conv1", i, j);
             rc = build_conv(tc, tc->res1[i][j], hw, nm, ch, ch / cfg.compress, cfg.residual_kernel_size, dil);
             snprintf(nm, sizeof(nm), "dec.up%d.res%d", i, j);
             if (!rc) rc = build_res_tail(tc, tc->res2[i][j], hw, nm, ch, ch / cfg.compress);
-            tc->min_T = std::max(tc->min_T, (cfg.residual_kernel_size - 1) * dil * cfg.dilation_base + 2);
         }
     }
     if (!rc) rc = build_conv(tc, tc->conv_out, hw, "dec.conv_out", ch, 1, cfg.last_kernel_size, 1, 32);
@@ -1279,27 +1241,24 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w
             tc->co_split = rc == 0;
         }
     }
-    tc->min_T = std::max(tc->min_T, std::max(cfg.kernel_size, cfg.last_kernel_size) + 1);
-    tc->stream_bytes = stream_state_bytes(tc);
     if (rc) {
         tc_codec_destroy(tc);
         return -1;
     }
+    build_plan(tc);
     *out = tc;
     return 0;
 }
 
-bool tc_codec_accepts(const TcCodec* c, int B, int T) { return c != nullptr && B >= 1 && T >= c->min_T; }
+bool tc_codec_accepts(const TcCodec* c, int B, int T) { return c != nullptr && B >= 1 && T >= c->plan.min_T; }
 
 int tc_codec_decode(TcCodec* tc, const int64_t* codes, float* wav, int B, int T, cudaStream_t st, int64_t* launches,
                     const TcStreamCtx* sc) {
     tc->prof.clear();
     // chunk the batch so the workspace stays under the limit -- and halve the chunk again if the device cannot give that much
     int chunk = B;
-    size_t need = 0;
     for (;;) {
-        int64_t dummy = 0;
-        if (decode_chunk_tc(tc, nullptr, nullptr, chunk, T, st, &dummy, true, &need, nullptr)) return -1;
+        const size_t need = ws_layout(tc, chunk, T).bytes;
         if (need > tc->ws_limit && chunk > 1) {
             chunk = (chunk + 1) / 2;
             continue;
@@ -1330,15 +1289,15 @@ int tc_codec_decode(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
         TcStreamCtx part;
         if (sc != nullptr) part = TcStreamCtx{sc->table + 4 * b0, sc->state};
         if (decode_chunk_tc(tc, codes + static_cast<size_t>(b0) * tc->cfg.n_q * T, wav + static_cast<size_t>(b0) * T * tc->hop, nb, T, st,
-                            launches, false, nullptr, sc != nullptr ? &part : nullptr))
+                            launches, sc != nullptr ? &part : nullptr))
             return -1;
     }
     return 0;
 }
 
-size_t tc_stream_state_bytes(const TcCodec* c) { return c->stream_bytes; }
+size_t tc_stream_state_bytes(const TcCodec* c) { return c->plan.stream_bytes; }
 
-int tc_stream_min_frames(const TcCodec* c) { return c->min_T; }
+int tc_stream_min_frames(const TcCodec* c) { return c->plan.min_T; }
 
 int tc_codes_check(const int64_t* codes, long long n, int bins, int* bad_dev, int* bad_host, cudaStream_t st) {
     VCB_CUDA_OK(cudaMemsetAsync(bad_dev, 0, sizeof(int), st));

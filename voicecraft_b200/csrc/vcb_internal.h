@@ -8,6 +8,24 @@
 
 namespace vcb {
 
+// Launch with the programmatic-dependent-launch attribute (when enabled): the kernel may be scheduled while its
+// predecessor is still running; every such kernel orders its data accesses with griddepcontrol.wait (pdl_wait()).
+template <typename... KArgs, typename... Args>
+cudaError_t launch_k_pdl(int pdl, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                         Args&&... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = pdl ? 1 : 0;
+    return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+}
+
 // ---------------------------------------------------------------------------------------------------
 // GEMM (gemm_wgmma.cu)
 // ---------------------------------------------------------------------------------------------------
