@@ -45,7 +45,8 @@ int enc_decode(enc_engine* e, const int64_t* codes_dev, float* wav_dev, int32_t 
  * "enc.down{i}.conv.weight" (strided), "enc.lstm.*", "enc.conv_out.weight". */
 int enc_encode(enc_engine* e, const float* wav_dev, int64_t* codes_dev, int32_t B, int32_t N, void* stream);
 /* "launches", "hop", "flops_per_frame", "tc_enabled", "tc_decodes", "stream_decodes", "stream_min_frames" (frames a fresh
- * stream's first enc_stream_decode needs; -1 without the tensor-core decoder), "stream_state_bytes" (carried state per stream) */
+ * stream's first enc_stream_decode needs; -1 without the tensor-core decoder), "stream_state_bytes" (carried state per stream);
+ * "live_bytes" / "live_handles" as vcb_counter (process-wide, valid with a NULL engine) */
 int64_t enc_counter(enc_engine* e, const char* name);
 
 /* Streaming decode: waveform chunk by chunk while the tokens are still being generated.  The decoder is causal, so a chunk

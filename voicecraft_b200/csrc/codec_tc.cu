@@ -484,8 +484,8 @@ inline float bf2f(uint16_t h) {
 }
 
 struct TcGemm {
-    __nv_bfloat16* tiles = nullptr;
-    float* bias = nullptr;
+    DevBuf<__nv_bfloat16> tiles;
+    DevBuf<float> bias;
     int N = 0, BN = 0, ntiles = 0, total_kb = 0;
     int Cout = 0, up = 1;              // column n -> (n / Cout, n % Cout)
     CUtensorMap tmW;
@@ -553,7 +553,7 @@ struct TcPlan {
 struct TcCodec {
     enc_config cfg;
     int hop = 1, D = 0, Dp = 0, ch0 = 0, num_sms = 132;
-    const float** d_embed = nullptr;
+    DevBuf<const float*> d_embed;
     TcGemm conv_in, conv_out;
     TcGemm conv_out_p;                 // final conv as per-tap partial products (N = k), summed by tc_diag_sum_kernel
     bool co_split = false;
@@ -561,9 +561,7 @@ struct TcCodec {
     std::vector<TcGemm> pre, step, up; // step: 64-column tiles, or 128 with VCB_CODEC_LSTM_WIDE=1
     std::vector<std::vector<TcGemm>> res1, res2;
     TcPlan plan;
-    std::vector<void*> owned;
-    uint8_t* ws = nullptr;
-    size_t ws_bytes = 0;
+    DevBuf<uint8_t> ws;
     size_t ws_limit = 0;
     bool profile = false;
     std::vector<std::pair<std::string, float>> prof;
@@ -575,7 +573,7 @@ namespace {
 
 inline int tc_num_sms(const TcCodec* tc) { return tc->num_sms; }
 
-int upload_gemm(TcCodec* tc, TcGemm& g, const std::vector<float>& W, const std::vector<float>& bias, int N, int Ktot, int bn_hint) {
+int upload_gemm(TcGemm& g, const std::vector<float>& W, const std::vector<float>& bias, int N, int Ktot, int bn_hint) {
     if (Ktot % TC_BK || Ktot / TC_BK > TC_MAX_KB) {
         set_error("codec_tc: K = %d outside the kernel's range", Ktot);
         return -1;
@@ -598,19 +596,17 @@ int upload_gemm(TcCodec* tc, TcGemm& g, const std::vector<float>& W, const std::
                         t[o++] = part == 0 ? hi : f2bf(w - bf2f(hi));
                     }
                 }
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&g.tiles), t.size() * 2));
-    tc->owned.push_back(g.tiles);
+    if (g.tiles.alloc(t.size())) return -1;
     VCB_CUDA_OK(cudaMemcpy(g.tiles, t.data(), t.size() * 2, cudaMemcpyHostToDevice));
     std::vector<float> bp(Npad, 0.f);
     for (int n = 0; n < N && n < static_cast<int>(bias.size()); ++n) bp[n] = bias[n];
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&g.bias), bp.size() * 4));
-    tc->owned.push_back(g.bias);
+    if (g.bias.alloc(bp.size())) return -1;
     VCB_CUDA_OK(cudaMemcpy(g.bias, bp.data(), bp.size() * 4, cudaMemcpyHostToDevice));
     return make_tmap_bf16_2d(&g.tmW, g.tiles, static_cast<uint64_t>(g.ntiles) * g.total_kb * 2 * g.BN, TC_BK, TC_BK, 2 * g.BN);
 }
 
 struct HostW {
-    const std::map<std::string, float*>& dev;
+    const std::map<std::string, DevBuf<float>>& dev;
     const std::map<std::string, std::vector<int64_t>>& shapes;
     int get(const std::string& name, std::vector<float>& out, std::vector<int64_t>* shape = nullptr) const {
         auto it = dev.find(name);
@@ -629,7 +625,7 @@ struct HostW {
 };
 
 // Conv1d weight w[Cout][Cin][k] (stride 1, dilation dil, causal) -> GEMM [Cout_pad][k * Cin_pad], tap j reads row t - (k-1-j)*dil
-int build_conv(TcCodec* tc, TcGemm& g, const HostW& hw, const std::string& name, int Cin, int Cout, int k, int dil, int bn_hint = 0) {
+int build_conv(TcGemm& g, const HostW& hw, const std::string& name, int Cin, int Cout, int k, int dil, int bn_hint = 0) {
     std::vector<float> w, b;
     if (hw.get(name + ".weight", w) || hw.get(name + ".bias", b)) return -1;
     const int Cip = cpad(Cin), Cop = Cout == 1 ? 1 : cpad(Cout);
@@ -642,11 +638,11 @@ int build_conv(TcCodec* tc, TcGemm& g, const HostW& hw, const std::string& name,
         for (int cb = 0; cb < Cip / TC_BK; ++cb) g.taps.push_back(TcTap{0, static_cast<short>((k - 1 - j) * dil), cb * TC_BK});
     g.Cout = Cop == 1 ? 32 : Cop;
     g.up = 1;
-    return upload_gemm(tc, g, W, b, Cop, Ktot, bn_hint);
+    return upload_gemm(g, W, b, Cop, Ktot, bn_hint);
 }
 
 // ConvTranspose1d weight w[Cin][Cout][2r], stride r, causal trim of the last r samples -> GEMM [r * Cout_pad][2 * Cin_pad]
-int build_convtr(TcCodec* tc, TcGemm& g, const HostW& hw, const std::string& name, int Cin, int Cout, int r) {
+int build_convtr(TcGemm& g, const HostW& hw, const std::string& name, int Cin, int Cout, int r) {
     std::vector<float> w, b;
     if (hw.get(name + ".weight", w) || hw.get(name + ".bias", b)) return -1;
     const int Cip = cpad(Cin), Cop = cpad(Cout), Ktot = 2 * Cip, N = r * Cop;
@@ -665,11 +661,11 @@ int build_convtr(TcCodec* tc, TcGemm& g, const HostW& hw, const std::string& nam
         for (int cb = 0; cb < Cip / TC_BK; ++cb) g.taps.push_back(TcTap{0, static_cast<short>(tap), cb * TC_BK});
     g.Cout = Cop;
     g.up = r;
-    return upload_gemm(tc, g, W, bias, N, Ktot, 0);
+    return upload_gemm(g, W, bias, N, Ktot, 0);
 }
 
 // residual block tail: conv2 (k = 1, on ELU(hidden)) + shortcut (k = 1, on the raw block input) as one GEMM
-int build_res_tail(TcCodec* tc, TcGemm& g, const HostW& hw, const std::string& prefix, int C, int hidden) {
+int build_res_tail(TcGemm& g, const HostW& hw, const std::string& prefix, int C, int hidden) {
     std::vector<float> w2, b2, ws, bs;
     if (hw.get(prefix + ".conv2.weight", w2) || hw.get(prefix + ".conv2.bias", b2) || hw.get(prefix + ".shortcut.weight", ws) ||
         hw.get(prefix + ".shortcut.bias", bs))
@@ -685,11 +681,11 @@ int build_res_tail(TcCodec* tc, TcGemm& g, const HostW& hw, const std::string& p
     for (int cb = 0; cb < Cp / TC_BK; ++cb) g.taps.push_back(TcTap{1, 0, cb * TC_BK});
     g.Cout = Cp;
     g.up = 1;
-    return upload_gemm(tc, g, W, bias, Cp, Ktot, 0);
+    return upload_gemm(g, W, bias, Cp, Ktot, 0);
 }
 
 // LSTM matrix [4H][H] (gate-major rows i, f, g, o) -> gate-interleaved rows n = 4*unit + gate
-int build_lstm(TcCodec* tc, TcGemm& g, const HostW& hw, const std::string& wname, const std::string& b1, const std::string& b2,
+int build_lstm(TcGemm& g, const HostW& hw, const std::string& wname, const std::string& b1, const std::string& b2,
                int H, int bn_hint) {
     std::vector<float> w, bi, bh;
     if (hw.get(wname, w)) return -1;
@@ -707,7 +703,7 @@ int build_lstm(TcCodec* tc, TcGemm& g, const HostW& hw, const std::string& wname
     for (int cb = 0; cb < H / TC_BK; ++cb) g.taps.push_back(TcTap{0, 0, cb * TC_BK});
     g.Cout = 4 * H;
     g.up = 1;
-    return upload_gemm(tc, g, W, bias, 4 * H, H, bn_hint);
+    return upload_gemm(g, W, bias, 4 * H, H, bn_hint);
 }
 
 template <int BN, int STAGES, int CW>
@@ -767,28 +763,26 @@ size_t form_bytes(const Plane& p) { return static_cast<size_t>(p.rcap) * p.C * 2
 struct Prof {
     TcCodec* tc;
     cudaStream_t st;
-    std::vector<std::pair<std::string, std::pair<cudaEvent_t, cudaEvent_t>>> ev;
+    struct Rec { std::string name; Event a, b; };
+    std::vector<Rec> ev;
     void begin(const char* name) {
         if (!tc->profile) return;
-        cudaEvent_t a, b;
-        cudaEventCreate(&a);
-        cudaEventCreate(&b);
-        cudaEventRecord(a, st);
-        ev.push_back({name, {a, b}});
+        ev.push_back({name, Event(), Event()});
+        ev.back().a.create();
+        ev.back().b.create();
+        cudaEventRecord(ev.back().a, st);
     }
     void end() {
         if (!tc->profile) return;
-        cudaEventRecord(ev.back().second.second, st);
+        cudaEventRecord(ev.back().b, st);
     }
     void finish() {
         if (!tc->profile) return;
         cudaStreamSynchronize(st);
         for (auto& e : ev) {
             float ms = 0.f;
-            cudaEventElapsedTime(&ms, e.second.first, e.second.second);
-            tc->prof.push_back({e.first, ms});
-            cudaEventDestroy(e.second.first);
-            cudaEventDestroy(e.second.second);
+            cudaEventElapsedTime(&ms, e.a, e.b);
+            tc->prof.push_back({e.name, ms});
         }
     }
 };
@@ -1136,9 +1130,9 @@ int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
 
 }  // namespace
 
-int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w_dev,
-                   const std::map<std::string, std::vector<int64_t>>& shapes, TcCodec** out, const char** reason) {
-    *out = nullptr;
+int tc_codec_build(const enc_config& cfg, const std::map<std::string, DevBuf<float>>& w_dev,
+                   const std::map<std::string, std::vector<int64_t>>& shapes, TcCodecPtr* out, const char** reason) {
+    out->reset();
     const int ch0 = cfg.n_filters << cfg.n_ratios;
     auto no = [&](const char* why) {
         *reason = why;
@@ -1154,7 +1148,7 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w
         cfg.residual_kernel_size * cpad(ch0 / 2) / TC_BK > TC_MAX_KB || cfg.last_kernel_size * cpad(cfg.n_filters) / TC_BK > TC_MAX_KB)
         return no("reduction deeper than 64 k-blocks");
     if (getenv("VCB_CODEC_TC") && atoi(getenv("VCB_CODEC_TC")) == 0) return no("disabled by VCB_CODEC_TC=0");
-    TcCodec* tc = new TcCodec();
+    TcCodecPtr tc(new TcCodec());
     tc->cfg = cfg;
     tc->D = cfg.dimension;
     tc->Dp = cpad(cfg.dimension);
@@ -1187,14 +1181,13 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w
                 emb[q] = it->second;
             }
         }
-        if (!rc && (cudaMalloc(reinterpret_cast<void**>(&tc->d_embed), cfg.n_q * sizeof(float*)) != cudaSuccess ||
+        if (!rc && (tc->d_embed.alloc(cfg.n_q) ||
                     cudaMemcpy(tc->d_embed, emb.data(), cfg.n_q * sizeof(float*), cudaMemcpyHostToDevice) != cudaSuccess)) {
             set_error("codec_tc: codebook pointer table");
             rc = -1;
         }
-        if (!rc) tc->owned.push_back(tc->d_embed);
     }
-    if (!rc) rc = build_conv(tc, tc->conv_in, hw, "dec.conv_in", cfg.dimension, ch0, cfg.kernel_size, 1);
+    if (!rc) rc = build_conv(tc->conv_in, hw, "dec.conv_in", cfg.dimension, ch0, cfg.kernel_size, 1);
     tc->pre.resize(cfg.lstm);
     tc->step.resize(cfg.lstm);
     for (int l = 0; l < cfg.lstm && !rc; ++l) {
@@ -1202,9 +1195,9 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w
         snprintf(a, sizeof(a), "dec.lstm.weight_ih_l%d", l);
         snprintf(b, sizeof(b), "dec.lstm.bias_ih_l%d", l);
         snprintf(c2, sizeof(c2), "dec.lstm.bias_hh_l%d", l);
-        rc = build_lstm(tc, tc->pre[l], hw, a, b, c2, ch0, 0);
+        rc = build_lstm(tc->pre[l], hw, a, b, c2, ch0, 0);
         snprintf(a, sizeof(a), "dec.lstm.weight_hh_l%d", l);
-        if (!rc) rc = build_lstm(tc, tc->step[l], hw, a, "", "", ch0, step_bn);
+        if (!rc) rc = build_lstm(tc->step[l], hw, a, "", "", ch0, step_bn);
     }
     tc->up.resize(cfg.n_ratios);
     tc->res1.resize(cfg.n_ratios);
@@ -1212,18 +1205,18 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w
     int ch = ch0;
     for (int i = 0; i < cfg.n_ratios && !rc; ++i) {
         snprintf(nm, sizeof(nm), "dec.up%d.convtr", i);
-        rc = build_convtr(tc, tc->up[i], hw, nm, ch, ch / 2, cfg.ratios[i]);
+        rc = build_convtr(tc->up[i], hw, nm, ch, ch / 2, cfg.ratios[i]);
         ch /= 2;
         tc->res1[i].resize(cfg.n_residual_layers);
         tc->res2[i].resize(cfg.n_residual_layers);
         for (int j = 0, dil = 1; j < cfg.n_residual_layers && !rc; ++j, dil *= cfg.dilation_base) {
             snprintf(nm, sizeof(nm), "dec.up%d.res%d.conv1", i, j);
-            rc = build_conv(tc, tc->res1[i][j], hw, nm, ch, ch / cfg.compress, cfg.residual_kernel_size, dil);
+            rc = build_conv(tc->res1[i][j], hw, nm, ch, ch / cfg.compress, cfg.residual_kernel_size, dil);
             snprintf(nm, sizeof(nm), "dec.up%d.res%d", i, j);
-            if (!rc) rc = build_res_tail(tc, tc->res2[i][j], hw, nm, ch, ch / cfg.compress);
+            if (!rc) rc = build_res_tail(tc->res2[i][j], hw, nm, ch, ch / cfg.compress);
         }
     }
-    if (!rc) rc = build_conv(tc, tc->conv_out, hw, "dec.conv_out", ch, 1, cfg.last_kernel_size, 1, 32);
+    if (!rc) rc = build_conv(tc->conv_out, hw, "dec.conv_out", ch, 1, cfg.last_kernel_size, 1, 32);
     if (!rc && cfg.last_kernel_size <= DS_LD && !(getenv("VCB_CODEC_CONVOUT_TC") && atoi(getenv("VCB_CODEC_CONVOUT_TC")))) {
         std::vector<float> w, b;
         rc = hw.get("dec.conv_out.weight", w) || hw.get("dec.conv_out.bias", b) ? -1 : 0;
@@ -1236,17 +1229,14 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w
             for (int cb = 0; cb < Cp / TC_BK; ++cb) g.taps.push_back(TcTap{0, 0, cb * TC_BK});
             g.Cout = 32;
             g.up = 1;
-            rc = upload_gemm(tc, g, W, std::vector<float>(), k, Cp, 32);
+            rc = upload_gemm(g, W, std::vector<float>(), k, Cp, 32);
             tc->co_bias = b[0];
             tc->co_split = rc == 0;
         }
     }
-    if (rc) {
-        tc_codec_destroy(tc);
-        return -1;
-    }
-    build_plan(tc);
-    *out = tc;
+    if (rc) return -1;
+    build_plan(tc.get());
+    *out = std::move(tc);
     return 0;
 }
 
@@ -1263,23 +1253,13 @@ int tc_codec_decode(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
             chunk = (chunk + 1) / 2;
             continue;
         }
-        if (need <= tc->ws_bytes) break;
-        if (tc->ws) {
-            VCB_CUDA_OK(cudaStreamSynchronize(st));
-            cudaFree(tc->ws);
-            tc->ws = nullptr;
-            tc->ws_bytes = 0;
-        }
-        const cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&tc->ws), need);
-        if (e == cudaSuccess) {
-            tc->ws_bytes = need;
-            break;
-        }
-        cudaGetLastError();                                // clear the sticky allocation error
-        tc->ws = nullptr;
+        if (need <= tc->ws.size()) break;
+        if (tc->ws) VCB_CUDA_OK(cudaStreamSynchronize(st));   // alloc releases the previous workspace first
+        if (tc->ws.alloc(need) == 0) break;
         if (chunk == 1) {
+            const std::string why = get_error();
             set_error("codec_tc: cannot allocate a %.2f GB workspace for one utterance of %d frames (%s)", need / 1073741824.0, T,
-                      cudaGetErrorString(e));
+                      why.c_str());
             return -1;
         }
         chunk = (chunk + 1) / 2;
@@ -1310,12 +1290,7 @@ int tc_codes_check(const int64_t* codes, long long n, int bins, int* bad_dev, in
     return 0;
 }
 
-void tc_codec_destroy(TcCodec* tc) {
-    if (!tc) return;
-    for (auto p : tc->owned) cudaFree(p);
-    cudaFree(tc->ws);
-    delete tc;
-}
+void TcCodecDelete::operator()(TcCodec* tc) const { delete tc; }
 
 const std::vector<std::pair<std::string, float>>& tc_codec_profile(const TcCodec* c) { return c->prof; }
 

@@ -4,18 +4,24 @@
 #include <stdint.h>
 
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
 #include "../../include/vcb200_codec.h"
+#include "vcb_internal.h"
 
 namespace vcb {
 
 struct TcCodec;
+struct TcCodecDelete {                 // the owner synchronises first: nothing queued may still use the decoder's buffers
+    void operator()(TcCodec* c) const;
+};
+using TcCodecPtr = std::unique_ptr<TcCodec, TcCodecDelete>;
 
 // 0: built; 1: this configuration is outside what the tensor-core path covers (why -> *reason, static string); -1: error.
-int tc_codec_build(const enc_config& cfg, const std::map<std::string, float*>& w_dev,
-                   const std::map<std::string, std::vector<int64_t>>& shapes, TcCodec** out, const char** reason);
+int tc_codec_build(const enc_config& cfg, const std::map<std::string, DevBuf<float>>& w_dev,
+                   const std::map<std::string, std::vector<int64_t>>& shapes, TcCodecPtr* out, const char** reason);
 // Stream decode (enc_stream_decode): utterance b of the call continues stream table[4b] with table[4b+1] valid frames;
 // table[4b+2] = 1 if that stream has decoded frames before (its left context and LSTM state come from `state`), 0 if fresh.
 struct TcStreamCtx {
@@ -33,7 +39,6 @@ size_t tc_stream_state_bytes(const TcCodec* c);
 int tc_stream_min_frames(const TcCodec* c);
 // *bad_host = whether any of the n codes lies outside [0, bins); waits for the stream
 int tc_codes_check(const int64_t* codes_dev, long long n, int bins, int* bad_dev, int* bad_host, cudaStream_t st);
-void tc_codec_destroy(TcCodec* c);
 // per-layer device times of the last decode when VCB_CODEC_PROFILE=1 (name, ms), in launch order
 const std::vector<std::pair<std::string, float>>& tc_codec_profile(const TcCodec* c);
 

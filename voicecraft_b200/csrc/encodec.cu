@@ -16,6 +16,7 @@
 #include <cmath>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -266,20 +267,19 @@ using namespace vcb;
 
 struct enc_engine {
     enc_config cfg;
-    std::map<std::string, float*> w;
+    std::map<std::string, DevBuf<float>> w;       // loaded weights and the ones enc_finalize derives (names with "__")
     std::map<std::string, std::vector<int64_t>> shapes;
-    std::vector<float*> owned;
-    float** d_embed = nullptr;
+    DevBuf<float*> d_embed;
     int hop = 1;
     bool finalized = false, has_encoder = false;
     // activation buffers for a batch chunk
-    float* buf[4] = {nullptr, nullptr, nullptr, nullptr};
+    DevBuf<float> buf[4];
     size_t buf_floats = 0;
-    float *h0 = nullptr, *h1 = nullptr, *cst = nullptr;
+    DevBuf<float> h0, h1, cst;
     int cap_B = 0, cap_T = 0;
     int64_t launches = 0;
     double flops_per_frame = 0;
-    TcCodec* tc = nullptr;              // tensor-core decoder (codec_tc.cu); null = configuration not covered
+    TcCodecPtr tc;                      // tensor-core decoder (codec_tc.cu); null = configuration not covered
     const char* tc_reason = "";
     int64_t tc_decodes = 0;
     int64_t stream_decodes = 0;
@@ -288,9 +288,9 @@ struct enc_engine {
 struct enc_stream {
     enc_engine* e = nullptr;
     int max_streams = 0;
-    uint8_t* state = nullptr;           // [max_streams][tc_stream_state_bytes]
-    int* table = nullptr;               // [max_streams][4] per-call table (TcStreamCtx)
-    int* bad = nullptr;                 // codes check flag
+    DevBuf<uint8_t> state;              // [max_streams][tc_stream_state_bytes]
+    DevBuf<int> table;                  // [max_streams][4] per-call table (TcStreamCtx)
+    DevBuf<int> bad;                    // codes check flag
     std::vector<int64_t> frames;        // frames decoded so far, per stream (0 = fresh)
 };
 
@@ -354,8 +354,10 @@ ConvArgs conv_args_strided(const enc_engine* e, const float* A, const float* bia
 
 int ensure_buffers(enc_engine* e, int B, int T) {
     if (B <= e->cap_B && T <= e->cap_T) return 0;
-    for (auto& p : e->buf) { cudaFree(p); p = nullptr; }
-    cudaFree(e->h0); cudaFree(e->h1); cudaFree(e->cst);
+    for (auto& p : e->buf) p.reset();   // all released before the larger ones are allocated
+    e->h0.reset();
+    e->h1.reset();
+    e->cst.reset();
     const enc_config& c = e->cfg;
     // widest activation: channels * time over the stack, plus the 4H x T LSTM pre-activations
     int ch = c.n_filters << c.n_ratios;
@@ -367,11 +369,10 @@ int ensure_buffers(enc_engine* e, int B, int T) {
         widest = std::max(widest, static_cast<size_t>(ch) * t);
     }
     e->buf_floats = widest * B;
-    for (auto& p : e->buf) VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&p), e->buf_floats * sizeof(float)));
+    for (auto& p : e->buf)
+        if (p.alloc(e->buf_floats)) return -1;
     const size_t hs = static_cast<size_t>(B) * (c.n_filters << c.n_ratios);
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&e->h0), hs * 4));
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&e->h1), hs * 4));
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&e->cst), hs * 4));
+    if (e->h0.alloc(hs) || e->h1.alloc(hs) || e->cst.alloc(hs)) return -1;
     e->cap_B = B;
     e->cap_T = T;
     return 0;
@@ -570,11 +571,8 @@ int enc_create(const enc_config* cfg, enc_engine** out) {
 
 int enc_destroy(enc_engine* e) {
     if (!e) return 0;
+    cudaSetDevice(e->cfg.device);
     cudaDeviceSynchronize();
-    for (auto p : e->owned) cudaFree(p);
-    for (auto p : e->buf) cudaFree(p);
-    cudaFree(e->h0); cudaFree(e->h1); cudaFree(e->cst); cudaFree(e->d_embed);
-    tc_codec_destroy(e->tc);
     delete e;
     return 0;
 }
@@ -585,11 +583,10 @@ int enc_load_weight(enc_engine* e, const char* name, const float* data, const in
     size_t n = 1;
     std::vector<int64_t> sh(shape, shape + ndim);
     for (auto s : sh) n *= static_cast<size_t>(s);
-    float* d = nullptr;
-    VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&d), n * sizeof(float)));
+    DevBuf<float> d;
+    if (d.alloc(n)) return -1;
     VCB_CUDA_OK(cudaMemcpy(d, data, n * sizeof(float), is_device_ptr ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
-    e->owned.push_back(d);
-    e->w[name] = d;
+    e->w[name] = std::move(d);         // a reloaded name releases its previous buffer
     e->shapes[name] = sh;
     e->finalized = false;
     return 0;
@@ -597,6 +594,7 @@ int enc_load_weight(enc_engine* e, const char* name, const float* data, const in
 
 int enc_finalize(enc_engine* e) {
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
+    e->finalized = false;              // the derived buffers below are replaced: unusable until this call succeeds
     const enc_config& c = e->cfg;
     char nm[128];
     std::vector<float*> emb(c.n_q);
@@ -604,35 +602,32 @@ int enc_finalize(enc_engine* e) {
         snprintf(nm, sizeof(nm), "vq.%d.embed", q);
         if (enc_need(e, nm, &emb[q])) return -1;
     }
-    if (!e->d_embed) VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&e->d_embed), c.n_q * sizeof(float*)));
+    if (e->d_embed.ensure(c.n_q)) return -1;
     VCB_CUDA_OK(cudaMemcpy(e->d_embed, emb.data(), c.n_q * sizeof(float*), cudaMemcpyHostToDevice));
     int ch = c.n_filters << c.n_ratios;
     double flops = 2.0 * c.dimension * ch * c.kernel_size;                     // per frame
     for (int l = 0; l < c.lstm; ++l) {
-        float *bi, *bh, *sum;
+        float *bi, *bh;
         snprintf(nm, sizeof(nm), "dec.lstm.bias_ih_l%d", l);
         if (enc_need(e, nm, &bi)) return -1;
         snprintf(nm, sizeof(nm), "dec.lstm.bias_hh_l%d", l);
         if (enc_need(e, nm, &bh)) return -1;
-        VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&sum), 4 * ch * sizeof(float)));
-        add_vec_kernel<<<(4 * ch + 255) / 256, 256>>>(bi, bh, sum, 4 * ch);
-        e->owned.push_back(sum);
         snprintf(nm, sizeof(nm), "dec.lstm.__bias_sum_l%d", l);
-        e->w[nm] = sum;
+        DevBuf<float>& sum = e->w[nm];
+        if (sum.alloc(4 * ch)) return -1;
+        add_vec_kernel<<<(4 * ch + 255) / 256, 256>>>(bi, bh, sum, 4 * ch);
         flops += 2.0 * 2 * 4 * ch * ch;
     }
     double t_mult = 1;
     for (int i = 0; i < c.n_ratios; ++i) {
         const int r = c.ratios[i];
-        float *wsrc, *packed;
+        float* wsrc;
         snprintf(nm, sizeof(nm), "dec.up%d.convtr.weight", i);
         if (enc_need(e, nm, &wsrc)) return -1;
-        const size_t n = static_cast<size_t>(r) * (ch / 2) * 2 * ch;
-        VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&packed), n * sizeof(float)));
-        pack_convtr_kernel<<<512, 256>>>(wsrc, packed, ch, ch / 2, r);
-        e->owned.push_back(packed);
         snprintf(nm, sizeof(nm), "dec.up%d.convtr.__packed", i);
-        e->w[nm] = packed;
+        DevBuf<float>& packed = e->w[nm];
+        if (packed.alloc(static_cast<size_t>(r) * (ch / 2) * 2 * ch)) return -1;
+        pack_convtr_kernel<<<512, 256>>>(wsrc, packed, ch, ch / 2, r);
         t_mult *= r;
         flops += t_mult * 2.0 * (2 * ch) * (ch / 2);
         ch /= 2;
@@ -646,29 +641,25 @@ int enc_finalize(enc_engine* e) {
     if (e->has_encoder) {
         const int che = c.n_filters << c.n_ratios;
         for (int l = 0; l < c.lstm; ++l) {
-            float *bi, *bh, *sum;
+            float *bi, *bh;
             snprintf(nm, sizeof(nm), "enc.lstm.bias_ih_l%d", l);
             if (enc_need(e, nm, &bi)) return -1;
             snprintf(nm, sizeof(nm), "enc.lstm.bias_hh_l%d", l);
             if (enc_need(e, nm, &bh)) return -1;
-            VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&sum), 4 * che * sizeof(float)));
-            add_vec_kernel<<<(4 * che + 255) / 256, 256>>>(bi, bh, sum, 4 * che);
-            e->owned.push_back(sum);
             snprintf(nm, sizeof(nm), "enc.lstm.__bias_sum_l%d", l);
-            e->w[nm] = sum;
+            DevBuf<float>& sum = e->w[nm];
+            if (sum.alloc(4 * che)) return -1;
+            add_vec_kernel<<<(4 * che + 255) / 256, 256>>>(bi, bh, sum, 4 * che);
         }
         for (int q = 0; q < c.n_q; ++q) {
-            float* hsn;
-            VCB_CUDA_OK(cudaMalloc(reinterpret_cast<void**>(&hsn), c.bins * sizeof(float)));
-            half_sqnorm_neg_kernel<<<(c.bins + 255) / 256, 256>>>(emb[q], hsn, c.bins, c.dimension);
-            e->owned.push_back(hsn);
             snprintf(nm, sizeof(nm), "vq.%d.__neg_half_sqnorm", q);
-            e->w[nm] = hsn;
+            DevBuf<float>& hsn = e->w[nm];
+            if (hsn.alloc(c.bins)) return -1;
+            half_sqnorm_neg_kernel<<<(c.bins + 255) / 256, 256>>>(emb[q], hsn, c.bins, c.dimension);
         }
     }
     VCB_CUDA_OK(cudaDeviceSynchronize());
-    tc_codec_destroy(e->tc);
-    e->tc = nullptr;
+    e->tc.reset();
     if (tc_codec_build(e->cfg, e->w, e->shapes, &e->tc, &e->tc_reason) < 0) return -1;
     e->finalized = true;
     return 0;
@@ -685,11 +676,11 @@ int enc_decode(enc_engine* e, const int64_t* codes_dev, float* wav_dev, int32_t 
     }
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (tc_codec_accepts(e->tc, B, T)) {
-        if (tc_codec_decode(e->tc, codes_dev, wav_dev, B, T, st, &e->launches)) return -1;
+    if (tc_codec_accepts(e->tc.get(), B, T)) {
+        if (tc_codec_decode(e->tc.get(), codes_dev, wav_dev, B, T, st, &e->launches)) return -1;
         e->tc_decodes++;
         if (getenv("VCB_CODEC_PROFILE"))
-            for (auto& pr : tc_codec_profile(e->tc)) fprintf(stderr, "[codec_tc] %-12s %9.3f ms\n", pr.first.c_str(), pr.second);
+            for (auto& pr : tc_codec_profile(e->tc.get())) fprintf(stderr, "[codec_tc] %-12s %9.3f ms\n", pr.first.c_str(), pr.second);
         return 0;
     }
     const int chunk = std::min(B, 16);
@@ -736,18 +727,20 @@ int enc_debug_tensor(enc_engine* e, const char* name, float* host_out, int64_t c
         set_error("codec: the tensor-core decoder is not active (%s)", e ? e->tc_reason : "null engine");
         return -1;
     }
-    return tc_codec_debug_tensor(e->tc, name, host_out, cap, dims);
+    return tc_codec_debug_tensor(e->tc.get(), name, host_out, cap, dims);
 }
 
 int64_t enc_counter(enc_engine* e, const char* name) {
+    if (!strcmp(name, "live_bytes")) return LiveCount::bytes;          // process-wide, valid with a null engine
+    if (!strcmp(name, "live_handles")) return LiveCount::handles;
     if (!strcmp(name, "launches")) return e->launches;
     if (!strcmp(name, "hop")) return e->hop;
     if (!strcmp(name, "flops_per_frame")) return static_cast<int64_t>(e->flops_per_frame);
     if (!strcmp(name, "tc_enabled")) return e->tc != nullptr;
     if (!strcmp(name, "tc_decodes")) return e->tc_decodes;
     if (!strcmp(name, "stream_decodes")) return e->stream_decodes;
-    if (!strcmp(name, "stream_min_frames")) return e->tc ? tc_stream_min_frames(e->tc) : -1;
-    if (!strcmp(name, "stream_state_bytes")) return e->tc ? static_cast<int64_t>(tc_stream_state_bytes(e->tc)) : -1;
+    if (!strcmp(name, "stream_min_frames")) return e->tc ? tc_stream_min_frames(e->tc.get()) : -1;
+    if (!strcmp(name, "stream_state_bytes")) return e->tc ? static_cast<int64_t>(tc_stream_state_bytes(e->tc.get())) : -1;
     return -1;
 }
 
@@ -766,20 +759,16 @@ int enc_stream_create(enc_engine* e, int32_t max_streams, enc_stream** out) {
         return -1;
     }
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
-    enc_stream* s = new enc_stream();
+    std::unique_ptr<enc_stream> s(new enc_stream());
     s->e = e;
     s->max_streams = max_streams;
     s->frames.assign(max_streams, 0);
-    const size_t bytes = static_cast<size_t>(max_streams) * tc_stream_state_bytes(e->tc);
-    if (cudaMalloc(reinterpret_cast<void**>(&s->state), bytes) != cudaSuccess ||
-        cudaMalloc(reinterpret_cast<void**>(&s->table), static_cast<size_t>(max_streams) * 4 * sizeof(int)) != cudaSuccess ||
-        cudaMalloc(reinterpret_cast<void**>(&s->bad), sizeof(int)) != cudaSuccess) {
-        cudaGetLastError();
+    const size_t bytes = static_cast<size_t>(max_streams) * tc_stream_state_bytes(e->tc.get());
+    if (s->state.alloc(bytes) || s->table.alloc(static_cast<size_t>(max_streams) * 4) || s->bad.alloc(1)) {
         set_error("codec stream: cannot allocate the state of %d streams (%zu bytes)", max_streams, bytes);
-        enc_stream_destroy(s);
         return -1;
     }
-    *out = s;
+    *out = s.release();
     return 0;
 }
 
@@ -787,9 +776,6 @@ int enc_stream_destroy(enc_stream* s) {
     if (!s) return 0;
     cudaSetDevice(s->e->cfg.device);
     cudaDeviceSynchronize();
-    cudaFree(s->state);
-    cudaFree(s->table);
-    cudaFree(s->bad);
     delete s;
     return 0;
 }
@@ -819,7 +805,7 @@ int enc_stream_decode(enc_engine* e, enc_stream* s, const int32_t* ids_host, con
         return -1;
     }
     // everything is validated before any stream changes
-    const int min_frames = tc_stream_min_frames(e->tc);
+    const int min_frames = tc_stream_min_frames(e->tc.get());
     std::vector<char> seen(s->max_streams, 0);
     std::vector<int> table(static_cast<size_t>(B) * 4);
     for (int b = 0; b < B; ++b) {
@@ -856,7 +842,7 @@ int enc_stream_decode(enc_engine* e, enc_stream* s, const int32_t* ids_host, con
     }
     VCB_CUDA_OK(cudaMemcpyAsync(s->table, table.data(), table.size() * sizeof(int), cudaMemcpyHostToDevice, st));
     const TcStreamCtx ctx{s->table, s->state};
-    if (tc_codec_decode(e->tc, codes_dev, wav_dev, B, T, st, &e->launches, &ctx)) return -1;
+    if (tc_codec_decode(e->tc.get(), codes_dev, wav_dev, B, T, st, &e->launches, &ctx)) return -1;
     for (int b = 0; b < B; ++b) s->frames[ids_host[b]] += lens_host[b];
     e->stream_decodes++;
     return 0;

@@ -2,11 +2,120 @@
 #pragma once
 #include "vcb_common.cuh"
 
+#include <algorithm>
+#include <atomic>
+#include <cstring>
 #include <string>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 namespace vcb {
+
+// ---------------------------------------------------------------------------------------------------
+// Owners of device memory, pinned host memory and events.  Every allocation and event of the library (except the
+// process-lifetime timeline buffers of vcb_timeline) lives in one of these, so whoever holds it releases it.  None of
+// them synchronises: an owner whose work may still be in flight synchronises once before releasing them.
+// ---------------------------------------------------------------------------------------------------
+struct LiveCount {                     // process-wide: what is allocated now (vcb_counter / enc_counter "live_*")
+    static inline std::atomic<long long> bytes{0}, handles{0};
+    static void add(long long b, long long h) { bytes += b; handles += h; }
+};
+
+// Owner of one allocation of n elements of T: device memory (DevBuf), or pinned host memory (PinnedBuf) -- with `mapped`,
+// host memory the device reaches through dev().  alloc(n, zero) releases the current allocation, then allocates at least
+// one element (an allocated buffer is never null), zero-filled on request; ensure() allocates only when empty.  Both
+// return 0, or -1 with the error set and the buffer empty.
+template <typename T, bool Pinned>
+class Buffer {
+public:
+    Buffer() = default;
+    Buffer(Buffer&& o) noexcept { *this = std::move(o); }
+    Buffer& operator=(Buffer&& o) noexcept {
+        if (this != &o) {
+            reset();
+            p_ = std::exchange(o.p_, nullptr);
+            d_ = std::exchange(o.d_, nullptr);
+            n_ = std::exchange(o.n_, 0);
+        }
+        return *this;
+    }
+    ~Buffer() { reset(); }
+
+    int alloc(size_t n, bool zero = false, bool mapped = false) {
+        reset();
+        const size_t bytes = std::max<size_t>(n, 1) * sizeof(T);
+        void* p = nullptr;
+        cudaError_t e = !Pinned ? cudaMalloc(&p, bytes) : mapped ? cudaHostAlloc(&p, bytes, cudaHostAllocMapped) : cudaMallocHost(&p, bytes);
+        if (e == cudaSuccess) {
+            LiveCount::add(static_cast<long long>(bytes), 1);
+            p_ = d_ = static_cast<T*>(p);
+            n_ = n;
+            if (zero && Pinned) memset(p, 0, bytes);
+            if (zero && !Pinned) e = cudaMemset(p, 0, bytes);
+            if (e == cudaSuccess && mapped) e = cudaHostGetDevicePointer(reinterpret_cast<void**>(&d_), p, 0);
+        }
+        if (e == cudaSuccess) return 0;
+        cudaGetLastError();                 // a failed allocation leaves its error for the next cudaGetLastError()
+        set_error("%s allocation of %zu bytes: %s", Pinned ? "pinned host" : "device", bytes, cudaGetErrorString(e));
+        reset();
+        return -1;
+    }
+    int ensure(size_t n, bool zero = false, bool mapped = false) { return p_ ? 0 : alloc(n, zero, mapped); }
+    void reset() {
+        if (!p_) return;
+        Pinned ? cudaFreeHost(p_) : cudaFree(p_);
+        LiveCount::add(-static_cast<long long>(std::max<size_t>(n_, 1) * sizeof(T)), -1);
+        p_ = d_ = nullptr;
+        n_ = 0;
+    }
+    T* get() const { return p_; }
+    T* dev() const { return d_; }
+    size_t size() const { return n_; }
+    operator T*() const { return p_; }
+
+private:
+    T *p_ = nullptr, *d_ = nullptr;
+    size_t n_ = 0;
+};
+template <typename T> using DevBuf = Buffer<T, false>;
+template <typename T> using PinnedBuf = Buffer<T, true>;
+
+class Event {
+public:
+    Event() = default;
+    Event(Event&& o) noexcept : ev_(std::exchange(o.ev_, nullptr)) {}
+    Event& operator=(Event&& o) noexcept {
+        if (this != &o) {
+            reset();
+            ev_ = std::exchange(o.ev_, nullptr);
+        }
+        return *this;
+    }
+    ~Event() { reset(); }
+
+    int create(unsigned flags = cudaEventDefault) {
+        reset();
+        const cudaError_t e = cudaEventCreateWithFlags(&ev_, flags);
+        if (e == cudaSuccess) {
+            LiveCount::add(0, 1);
+            return 0;
+        }
+        ev_ = nullptr;
+        set_error("event creation: %s", cudaGetErrorString(e));
+        return -1;
+    }
+    void reset() {
+        if (!ev_) return;
+        cudaEventDestroy(ev_);
+        LiveCount::add(0, -1);
+        ev_ = nullptr;
+    }
+    operator cudaEvent_t() const { return ev_; }
+
+private:
+    cudaEvent_t ev_ = nullptr;
+};
 
 // Launch with the programmatic-dependent-launch attribute (when enabled): the kernel may be scheduled while its
 // predecessor is still running; every such kernel orders its data accesses with griddepcontrol.wait (pdl_wait()).
