@@ -56,6 +56,7 @@ struct vcb_engine {
     int kv_fp32 = 0;
     int max_pages_per_slot = 0, n_pages = 0;
     std::vector<int> free_pages;
+    std::vector<int> page_refs;       // slots whose page list holds the page (a best-of-N group shares its full prompt pages)
     std::vector<std::vector<int>> slot_pages;
     std::vector<int> slot_group;      // host mirror: group id per slot (-1 closed)
     std::vector<int> free_groups;
@@ -99,8 +100,15 @@ struct vcb_engine {
     int64_t n_poll_frames = 0;
     DevBuf<int> all_rows;             // prefill row tables: 5 arrays of all_rows_cap ints (seq, pos, slot, last, page)
     size_t all_rows_cap = 0;
+    int64_t n_prefill_rows = 0;       // rows through the prefill since create
+    DevBuf<uint8_t*> d_pools;         // every layer's K pool, then every layer's V pool (fork_group_kernel)
+    DevBuf<ForkPair> d_fork;          // prefill: (leader -> member) copies of the best-of-N groups [max_slots]
     DevBuf<int> d_slots;
     std::vector<int> last_slots;      // host mirror of d_slots (skip re-upload when unchanged)
+    // decode rows in groups of one best-of-N group's consecutive slots (attn_rows_kernel<.., ATT_GMAX>): d_slots holds the
+    // n slots, then grp_first [n_row_groups + 1], then grp_shared [n_row_groups]; n_row_groups = 0: no shared group listed
+    int n_row_groups = 0;
+    std::vector<int> slot_shared;     // host mirror: full prompt pages the slot shares with its group (0: none)
     DevBuf<int> tok_log;
     DevBuf<float> dbg_logits;
     DevBuf<SlotState> st;
@@ -292,20 +300,24 @@ struct AttnLaunch {
     float* ws = nullptr;                  // [rows * H][maxch][hd + 2]
     int* cnt = nullptr;                   // [rows * H], zero between launches (the merging CTA resets its counter)
     int maxch = 1, chunk_pages = 16, num_sms = 132, balance = 1, pdl = 0;
+    // row groups (attn_rows_kernel<.., ATT_GMAX>): group g = rows grp_first[g] .. grp_first[g+1]-1 (<= ATT_GMAX), whose first
+    // grp_shared[g] pages are the same; n_groups = 0: every row on its own (GMAX = 1)
+    const int *grp_first = nullptr, *grp_shared = nullptr;
+    int n_groups = 0;
 };
 
-template <typename KVT, int HD>
+template <typename KVT, int HD, int GMAX>
 int launch_attn_hd(const AttnLaunch& a, cudaStream_t st) {
     const float scale = 1.0f / sqrtf(static_cast<float>(HD));
     using L = AttSmem<KVT, HD>;
     static bool set = false;
     if (!set) {
-        VCB_CUDA_OK(cudaFuncSetAttribute(attn_rows_kernel<KVT, HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
+        VCB_CUDA_OK(cudaFuncSetAttribute(attn_rows_kernel<KVT, HD, GMAX>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
         set = true;
     }
     const int npages = (a.max_ctx + KV_PAGE - 1) / KV_PAGE;
     const int nch = std::min(a.maxch, std::max(1, (npages + a.chunk_pages - 1) / a.chunk_pages));
-    const int n_rh = a.rows * a.H;
+    const int n_rh = (GMAX == 1 ? a.rows : a.n_groups) * a.H;      // work items per chunk: (row or row group, head)
     const int per_sm = std::max(1, std::min(4, (227 * 1024) / (L::TOTAL + 1024)));
     int grid = std::min(n_rh * nch, a.num_sms * per_sm);
     if (a.balance) {
@@ -314,11 +326,16 @@ int launch_attn_hd(const AttnLaunch& a, cudaStream_t st) {
         const int items = n_rh * nch, passes = (items + grid - 1) / grid;
         grid = (items + passes - 1) / passes;
     }
-    VCB_CUDA_OK(launch_k_pdl(a.pdl, attn_rows_kernel<KVT, HD>, dim3(grid), dim3(ATT_THREADS + 32), L::TOTAL, st, a.q,
+    VCB_CUDA_OK(launch_k_pdl(a.pdl, attn_rows_kernel<KVT, HD, GMAX>, dim3(grid), dim3(ATT_THREADS + 32), L::TOTAL, st, a.q,
                              static_cast<const KVT*>(a.kpool), static_cast<const KVT*>(a.vpool), a.page_table, a.max_pages,
                              a.row_slot, a.row_pos, a.H, a.act, a.ld_act, a.bpad, scale, a.ws, a.cnt, a.maxch, a.chunk_pages,
-                             n_rh, nch, a.row_pages));
+                             n_rh, nch, a.row_pages, a.grp_first, a.grp_shared));
     return 0;
+}
+
+template <typename KVT, int HD>
+int launch_attn_kv(const AttnLaunch& a, cudaStream_t st) {
+    return a.n_groups > 0 ? launch_attn_hd<KVT, HD, ATT_GMAX>(a, st) : launch_attn_hd<KVT, HD, 1>(a, st);
 }
 
 int launch_attn_rows(const AttnLaunch& a, cudaStream_t st) {
@@ -327,8 +344,8 @@ int launch_attn_rows(const AttnLaunch& a, cudaStream_t st) {
         return -1;
     }
     if (a.kv_fp32)
-        return a.hd == 128 ? launch_attn_hd<float, 128>(a, st) : launch_attn_hd<float, 64>(a, st);
-    return a.hd == 128 ? launch_attn_hd<__nv_bfloat16, 128>(a, st) : launch_attn_hd<__nv_bfloat16, 64>(a, st);
+        return a.hd == 128 ? launch_attn_kv<float, 128>(a, st) : launch_attn_kv<float, 64>(a, st);
+    return a.hd == 128 ? launch_attn_kv<__nv_bfloat16, 128>(a, st) : launch_attn_kv<__nv_bfloat16, 64>(a, st);
 }
 
 // A GEMM's B operand: hi rows, then lo rows `bpad` rows further, and the tensor map the GEMM loads them through
@@ -348,6 +365,8 @@ struct Pass {
     const int *slot = nullptr, *pos = nullptr, *last = nullptr, *page = nullptr;
     const int* pages = nullptr;               // [rows][max_pages_per_slot] page lists, or null: pages through page_table + slot
     const int* forced = nullptr;              // decode steps: SlotState::forced per row as of step_prep (sampler snapshot)
+    const int *grp_first = nullptr, *grp_shared = nullptr;   // decode steps: row groups (AttnLaunch), n_groups of them
+    int n_groups = 0;
     float* x = nullptr;                       // residual rows
     const int* x_index = nullptr;             // heads of vcb_sample: row r's hidden state is x[x_index[r]] (null: x[r])
     float* q = nullptr;
@@ -383,6 +402,9 @@ Pass step_pass(vcb_engine* e, int n, bool fold) {
     p.page = e->row_page;
     p.pages = e->row_pages;
     p.forced = e->row_forced;
+    p.n_groups = e->n_row_groups;
+    p.grp_first = e->d_slots + n;
+    p.grp_shared = p.grp_first + p.n_groups + 1;
     return p;
 }
 
@@ -535,6 +557,9 @@ int launch_attn(vcb_engine* e, const Pass& p, const Layer& Ly, cudaStream_t st) 
     a.num_sms = e->num_sms;
     a.balance = e->opt_att_balance;
     a.pdl = e->opt_pdl;
+    a.grp_first = p.grp_first;
+    a.grp_shared = p.grp_shared;
+    a.n_groups = p.n_groups;
     ProfScope ps(e, PC_ATTN, st);
     if (launch_attn_rows(a, st)) return -1;
     LAUNCH_COUNT(e);
@@ -797,7 +822,27 @@ int upload_slots(vcb_engine* e, const int32_t* slots, int n, cudaStream_t st) {
         }
     if (static_cast<int>(e->last_slots.size()) == n && std::equal(slots, slots + n, e->last_slots.begin())) return 0;
     e->last_slots.assign(slots, slots + n);
-    return upload_ints(e, slots, n, e->d_slots, st);
+    // row groups: runs of consecutive rows on consecutive slots of one best-of-N group with shared pages, at most
+    // ATT_GMAX rows each; every other row is a group of one
+    std::vector<int> tab(slots, slots + n), first{0}, shared;
+    bool grouped = false;
+    for (int i = 0; i < n;) {
+        const int S = e->slot_shared[slots[i]];
+        int j = i + 1;
+        while (S > 0 && j < n && j - i < ATT_GMAX && slots[j] == slots[j - 1] + 1 &&
+               e->slot_group[slots[j]] == e->slot_group[slots[i]])
+            ++j;
+        grouped |= j - i > 1;
+        first.push_back(j);
+        shared.push_back(j - i > 1 ? S : 0);
+        i = j;
+    }
+    e->n_row_groups = grouped ? static_cast<int>(shared.size()) : 0;
+    if (grouped) {
+        tab.insert(tab.end(), first.begin(), first.end());
+        tab.insert(tab.end(), shared.begin(), shared.end());
+    }
+    return upload_ints(e, tab.data(), tab.size(), e->d_slots, st);
 }
 
 // exp_noise_dev may be null only if every listed slot's group carries its own Philox stream (vcb_prompt::rng_threads)
@@ -963,11 +1008,13 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
     e->max_pages_per_slot = (cfg->max_seq_len + KV_PAGE - 1) / KV_PAGE;
     e->n_pages = e->max_pages_per_slot * cfg->max_slots;
     for (int p = e->n_pages - 1; p >= 0; --p) e->free_pages.push_back(p);
+    e->page_refs.assign(e->n_pages, 0);
     e->slot_pages.resize(cfg->max_slots);
     e->slot_group.assign(cfg->max_slots, -1);
     e->slot_rng.assign(cfg->max_slots, 0);
     e->slot_edit.assign(cfg->max_slots, 0);
     e->slot_copies.assign(cfg->max_slots, 0);
+    e->slot_shared.assign(cfg->max_slots, 0);
     e->slot_final.assign(cfg->max_slots, 0);
     e->h_seq_len.assign(cfg->max_slots, 0);
     for (int g = cfg->max_slots - 1; g >= 0; --g) e->free_groups.push_back(g);
@@ -1127,12 +1174,21 @@ int vcb_finalize_weights(vcb_engine* e) {
         e->att_ws.ensure(R * m.H * e->att_maxch * (m.hd + 2), true) || e->att_cnt.ensure(R * m.H, true) ||
         e->ln_stats.ensure(static_cast<size_t>(128) * STATS_ROWS * 2, true) || e->row_slot.ensure(R, true) ||
         e->row_pos.ensure(R, true) || e->row_last.ensure(R, true) || e->row_page.ensure(R, true) ||
-        e->row_forced.ensure(R, true) || e->row_pages.ensure(R * e->max_pages_per_slot, true) || e->d_slots.ensure(R, true) ||
+        e->row_forced.ensure(R, true) || e->row_pages.ensure(R * e->max_pages_per_slot, true) || e->d_slots.ensure(3 * R + 1, true) ||
         e->page_table.ensure(S * e->max_pages_per_slot, true) || e->tok_log.ensure(S * e->cfg.max_new_tokens * m.K, true) ||
         e->dbg_logits.ensure(R * m.K * m.V, true) || e->st.ensure(S, true) || e->gr.ensure(S, true) ||
         e->d_seqs.ensure(S, true) || e->pf_rec.ensure(S, true) || e->h_pf_rec.ensure(S) ||
-        e->all_rows.ensure(5 * e->all_rows_cap, true) || e->h_stage.ensure(e->h_stage_ints))
+        e->all_rows.ensure(5 * e->all_rows_cap, true) || e->h_stage.ensure(e->h_stage_ints) || e->d_fork.ensure(S, true) ||
+        e->d_pools.ensure(2 * m.L, true))
         return -1;
+    {
+        std::vector<uint8_t*> pools(2 * m.L);
+        for (int l = 0; l < m.L; ++l) {
+            pools[l] = e->layers[l].kpool;
+            pools[m.L + l] = e->layers[l].vpool;
+        }
+        VCB_CUDA_OK(cudaMemcpy(e->d_pools, pools.data(), pools.size() * sizeof(uint8_t*), cudaMemcpyHostToDevice));
+    }
     if (!e->stage_ev && e->stage_ev.create(cudaEventDisableTiming)) return -1;
     const int bp[4] = {16, 32, 64, 128};
     for (int i = 0; i < 4; ++i) {
@@ -1163,6 +1219,7 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
     std::vector<int> sst_slot;
     std::vector<GroupState> gst;
     std::vector<int> gst_id;
+    std::vector<ForkPair> fork;
     // ---- validate everything before touching host or device state (a failed call must leave no slot, group or page held)
     {
         size_t rows_needed = 0, pages_needed = 0;
@@ -1183,8 +1240,10 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
                 }
                 claimed[P.slot + c] = 1;
             }
-            rows_needed += static_cast<size_t>(total) * P.n_copies;
-            pages_needed += static_cast<size_t>(e->max_pages_per_slot) * P.n_copies;
+            // one prefill per group; the members share the leader's full prompt pages
+            const int shared = static_cast<int>(total / KV_PAGE);
+            rows_needed += static_cast<size_t>(total);
+            pages_needed += e->max_pages_per_slot + static_cast<size_t>(P.n_copies - 1) * (e->max_pages_per_slot - shared);
         }
         if (static_cast<size_t>(n) > e->free_groups.size()) {
             set_error("no free group");
@@ -1231,18 +1290,29 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
         es.y_len = P.y_len;
         const int seq_idx = static_cast<int>(seqs.size());
         seqs.push_back(es);
+        const int shared = total / KV_PAGE;           // full prompt pages: written by the prefill only, never by a step
         for (int c = 0; c < P.n_copies; ++c) {
             const int slot = P.slot + c;
             e->slot_group[slot] = gid;
             e->slot_rng[slot] = P.rng_threads != 0;
             e->slot_edit[slot] = P.mode == VCB_MODE_EDIT;
             e->slot_copies[slot] = P.n_copies;
+            e->slot_shared[slot] = P.n_copies > 1 ? shared : 0;
             e->slot_final[slot] = 0;
             auto& pg = e->slot_pages[slot];
             pg.clear();
             for (int p = 0; p < e->max_pages_per_slot; ++p) {
-                pg.push_back(e->free_pages.back());
-                e->free_pages.pop_back();
+                if (c > 0 && p < shared) {
+                    pg.push_back(e->slot_pages[P.slot][p]);
+                } else {
+                    pg.push_back(e->free_pages.back());
+                    e->free_pages.pop_back();
+                }
+                ++e->page_refs[pg.back()];
+            }
+            if (c > 0) {
+                const bool tail = total % KV_PAGE != 0;
+                fork.push_back({P.slot, slot, tail ? e->slot_pages[P.slot][shared] : -1, tail ? pg[shared] : -1});
             }
             SlotState S;
             memset(&S, 0, sizeof(S));
@@ -1256,7 +1326,7 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
             e->h_seq_len[slot] = total;
             sst.push_back(S);
             sst_slot.push_back(slot);
-            for (int t = 0; t < total; ++t) {
+            for (int t = 0; c == 0 && t < total; ++t) {
                 r_seq.push_back(seq_idx);
                 r_pos.push_back(t);
                 r_slot.push_back(slot);
@@ -1265,6 +1335,7 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
             }
         }
     }
+    e->last_slots.clear();                   // the row groups of the next step's slot list may have changed
     // state + page tables (synchronous copies: prefill is a once-per-utterance call)
     VCB_CUDA_OK(cudaStreamSynchronize(st));
     for (size_t i = 0; i < sst.size(); ++i) {
@@ -1276,6 +1347,8 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
     for (size_t i = 0; i < gst.size(); ++i)
         VCB_CUDA_OK(cudaMemcpy(e->gr + gst_id[i], &gst[i], sizeof(GroupState), cudaMemcpyHostToDevice));
     VCB_CUDA_OK(cudaMemcpy(e->d_seqs, seqs.data(), seqs.size() * sizeof(EmbedSeq), cudaMemcpyHostToDevice));
+    if (!fork.empty())
+        VCB_CUDA_OK(cudaMemcpy(e->d_fork, fork.data(), fork.size() * sizeof(ForkPair), cudaMemcpyHostToDevice));
     // ---- chunked prefill: <= 128 rows per pass through the same kernels as a decode step ----------------
     const size_t total_rows = r_seq.size();
     int* t_seq = e->all_rows;
@@ -1312,6 +1385,17 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
             ProfScope ps(e, PC_LN, st);
             gather_rows_kernel<<<rows, 256, 0, st>>>(p.x, e->h_slot, p.last, m.d);
         }
+        VCB_CUDA_OK(cudaGetLastError());
+        LAUNCH_COUNT(e);
+    }
+    e->n_prefill_rows += static_cast<int64_t>(total_rows);
+    if (!fork.empty()) {
+        const int page_words = static_cast<int>(static_cast<size_t>(m.H) * KV_PAGE * m.hd * (e->kv_fp32 ? 4 : 2) / 16);
+        const long long words = static_cast<long long>(fork.size()) * (2LL * m.L * page_words + m.d / 4);
+        const int grid = static_cast<int>(std::min<long long>((words + 255) / 256, 4LL * e->num_sms));
+        ProfScope ps(e, PC_MISC, st);
+        fork_group_kernel<<<grid, 256, 0, st>>>(e->d_pools, 2 * m.L, page_words, e->d_fork, static_cast<int>(fork.size()),
+                                                e->h_slot, m.d);
         VCB_CUDA_OK(cudaGetLastError());
         LAUNCH_COUNT(e);
     }
@@ -1502,11 +1586,14 @@ int vcb_release(vcb_engine* e, int32_t slot, int32_t n_copies) {
         if (s < 0 || s >= e->cfg.max_slots || e->slot_group[s] < 0) continue;
         gid = e->slot_group[s];
         e->slot_group[s] = -1;
-        for (int p : e->slot_pages[s]) e->free_pages.push_back(p);
+        for (int p : e->slot_pages[s])
+            if (--e->page_refs[p] == 0) e->free_pages.push_back(p);
         e->slot_pages[s].clear();
         VCB_CUDA_OK(cudaMemset(e->st + s, 0, sizeof(SlotState)));
     }
-    if (gid >= 0) e->free_groups.push_back(gid);
+    // the group id goes back with the last of its slots, whichever call releases it
+    if (gid >= 0 && std::find(e->slot_group.begin(), e->slot_group.end(), gid) == e->slot_group.end())
+        e->free_groups.push_back(gid);
     return 0;
 }
 
@@ -1577,11 +1664,14 @@ int vcb_debug_gemm(const float* W_dev, const float* X_dev, float* out_dev, int32
     return 0;
 }
 
-// Parity hook of the paged attention (attn_rows_kernel) with the engine's launch decisions; see include/vcb200.h.
-int vcb_debug_attention(const float* q_dev, const void* kpool_dev, const void* vpool_dev, int32_t kv_fp32,
-                        const int32_t* row_pages_dev, const int32_t* page_table_dev, const int32_t* row_slot_dev,
-                        const int32_t* pos_dev, int32_t rows, int32_t H, int32_t hd, int32_t max_pages, int32_t chunk_pages,
-                        int32_t balance, int32_t repeats, float* out_dev) {
+// Parity hooks of the paged attention (attn_rows_kernel) with the engine's launch decisions; see include/vcb200.h.
+// group_first null: every row on its own (GMAX = 1); else the row groups, checked here and split into launch groups of
+// at most ATT_GMAX rows
+static int debug_attention(const float* q_dev, const void* kpool_dev, const void* vpool_dev, int32_t kv_fp32,
+                           const int32_t* row_pages_dev, const int32_t* page_table_dev, const int32_t* row_slot_dev,
+                           const int32_t* pos_dev, int32_t rows, int32_t H, int32_t hd, int32_t max_pages, int32_t chunk_pages,
+                           int32_t balance, int32_t repeats, float* out_dev, const int32_t* group_first,
+                           const int32_t* group_shared, int32_t n_groups) {
     if (rows < 1 || H < 1 || (hd != 64 && hd != 128) || max_pages < 1 || repeats < 1 || !q_dev || !kpool_dev || !vpool_dev ||
         !pos_dev || !out_dev || (!row_pages_dev && (!page_table_dev || !row_slot_dev))) {
         set_error("vcb_debug_attention: bad argument");
@@ -1596,6 +1686,44 @@ int vcb_debug_attention(const float* q_dev, const void* kpool_dev, const void* v
             return -1;
         }
         max_ctx = std::max(max_ctx, p + 1);
+    }
+    std::vector<int> launch_groups;               // first [n + 1], then shared [n]
+    if (group_first) {
+        if (n_groups < 1 || !group_shared || !row_pages_dev || group_first[0] != 0 || group_first[n_groups] != rows) {
+            set_error("vcb_debug_attention_groups: the groups must tile rows 0 .. %d (row-pages form)", rows);
+            return -1;
+        }
+        std::vector<int> pages(static_cast<size_t>(rows) * max_pages);
+        VCB_CUDA_OK(cudaMemcpy(pages.data(), row_pages_dev, pages.size() * sizeof(int), cudaMemcpyDeviceToHost));
+        std::vector<int> first{0}, shared;
+        for (int g = 0; g < n_groups; ++g) {
+            const int r0 = group_first[g], r1 = group_first[g + 1], S = group_shared[g];
+            if (r1 <= r0 || S < 0 || S > max_pages) {
+                set_error("vcb_debug_attention_groups: group %d: rows %d .. %d, %d shared pages", g, r0, r1 - 1, S);
+                return -1;
+            }
+            int gpos = -1;
+            for (int r = r0; r < r1; ++r) {
+                if (!std::equal(pages.begin() + static_cast<size_t>(r) * max_pages,
+                                pages.begin() + static_cast<size_t>(r) * max_pages + S,
+                                pages.begin() + static_cast<size_t>(r0) * max_pages)) {
+                    set_error("vcb_debug_attention_groups: group %d: row %d's first %d pages differ from row %d's", g, r, S, r0);
+                    return -1;
+                }
+                if (pos[r] >= 0 && gpos >= 0 && pos[r] != gpos) {
+                    set_error("vcb_debug_attention_groups: group %d: positions %d and %d (members must be equal or -1)", g,
+                              gpos, pos[r]);
+                    return -1;
+                }
+                if (pos[r] >= 0) gpos = pos[r];
+            }
+            for (int r = r0; r < r1; r += ATT_GMAX) {
+                first.push_back(std::min(r1, r + ATT_GMAX));
+                shared.push_back(S);
+            }
+        }
+        launch_groups = first;
+        launch_groups.insert(launch_groups.end(), shared.begin(), shared.end());
     }
     AttnLaunch a;
     a.q = q_dev;
@@ -1619,8 +1747,15 @@ int vcb_debug_attention(const float* q_dev, const void* kpool_dev, const void* v
     a.balance = balance;
     DevBuf<__nv_bfloat16> act;
     DevBuf<float> ws;
-    DevBuf<int> cnt;
+    DevBuf<int> cnt, grp;
     const SyncOnExit sync;
+    if (!launch_groups.empty()) {
+        if (grp.alloc(launch_groups.size())) return -1;
+        VCB_CUDA_OK(cudaMemcpy(grp, launch_groups.data(), launch_groups.size() * sizeof(int), cudaMemcpyHostToDevice));
+        a.n_groups = static_cast<int>(launch_groups.size() - 1) / 2;
+        a.grp_first = grp;
+        a.grp_shared = grp + a.n_groups + 1;
+    }
     if (act.alloc(static_cast<size_t>(2 * rows) * a.ld_act, true) ||
         ws.alloc(static_cast<size_t>(rows) * H * a.maxch * (hd + 2), true) || cnt.alloc(static_cast<size_t>(rows) * H, true))
         return -1;
@@ -1634,6 +1769,26 @@ int vcb_debug_attention(const float* q_dev, const void* kpool_dev, const void* v
     VCB_CUDA_OK(cudaGetLastError());
     VCB_CUDA_OK(cudaDeviceSynchronize());
     return 0;
+}
+
+int vcb_debug_attention(const float* q_dev, const void* kpool_dev, const void* vpool_dev, int32_t kv_fp32,
+                        const int32_t* row_pages_dev, const int32_t* page_table_dev, const int32_t* row_slot_dev,
+                        const int32_t* pos_dev, int32_t rows, int32_t H, int32_t hd, int32_t max_pages, int32_t chunk_pages,
+                        int32_t balance, int32_t repeats, float* out_dev) {
+    return debug_attention(q_dev, kpool_dev, vpool_dev, kv_fp32, row_pages_dev, page_table_dev, row_slot_dev, pos_dev, rows, H,
+                           hd, max_pages, chunk_pages, balance, repeats, out_dev, nullptr, nullptr, 0);
+}
+
+int vcb_debug_attention_groups(const float* q_dev, const void* kpool_dev, const void* vpool_dev, int32_t kv_fp32,
+                               const int32_t* row_pages_dev, const int32_t* pos_dev, int32_t rows, int32_t H, int32_t hd,
+                               int32_t max_pages, int32_t chunk_pages, int32_t balance, int32_t repeats, float* out_dev,
+                               const int32_t* group_first, const int32_t* group_shared, int32_t n_groups) {
+    if (!group_first) {
+        set_error("vcb_debug_attention_groups: group_first is null");
+        return -1;
+    }
+    return debug_attention(q_dev, kpool_dev, vpool_dev, kv_fp32, row_pages_dev, nullptr, nullptr, pos_dev, rows, H, hd,
+                           max_pages, chunk_pages, balance, repeats, out_dev, group_first, group_shared, n_groups);
 }
 
 // Parity hook of the decode pair "out-projection -> LN2 -> FFN1" on the per-kernel GEMM path; see include/vcb200.h.
@@ -1832,6 +1987,8 @@ int64_t vcb_counter(vcb_engine* e, const char* name) {
     if (!strcmp(name, "num_sms")) return e->num_sms;
     if (!strcmp(name, "mega_grid")) return e->mega_grid;
     if (!strcmp(name, "poll_frames")) return e->n_poll_frames;
+    if (!strcmp(name, "kv_pages_free")) return static_cast<int64_t>(e->free_pages.size());
+    if (!strcmp(name, "prefill_rows")) return e->n_prefill_rows;
     if (!strcmp(name, "kv_bytes_per_token")) return static_cast<int64_t>(e->m.L) * 2 * e->m.d * (e->kv_fp32 ? 4 : 2);
     return -1;
 }

@@ -11,6 +11,7 @@ static constexpr int ATT_CWARPS = 8;            // consumer warps per CTA
 static constexpr int ATT_THREADS = ATT_CWARPS * 32;
 static constexpr int ATT_STAGES = 3;
 static constexpr int ATT_CHUNK_PAGES = 16;      // default pages per attention work item (VCB_ATT_CHUNK_PAGES overrides)
+static constexpr int ATT_GMAX = 8;              // rows per row group of the grouped attention (larger groups are split)
 
 __device__ __forceinline__ float block_sum_256(float v, float* red /*[8]*/) {
     v = warp_sum(v);
@@ -131,6 +132,35 @@ __global__ void gather_rows_kernel(const float* __restrict__ x_in, float* __rest
         out[static_cast<size_t>(dst) * d + c] = x_in[static_cast<size_t>(r) * d + c];
 }
 
+// Best-of-N prefill: only the group's leader runs through the layers; its members share the leader's full prompt pages
+// and get a copy of what else the prefill left for the leader: the partial tail page (every layer's K and V pool) and the
+// last hidden state the first sampling step reads.  Plain copies, so a member's bits are those its own prefill would write.
+struct ForkPair {
+    int src_slot, dst_slot;
+    int src_page, dst_page;      // partial tail page, or -1: the prompt fills its last page
+};
+
+__global__ void fork_group_kernel(uint8_t* const* __restrict__ pools /*[n_pools]*/, int n_pools, int page_words,
+                                  const ForkPair* __restrict__ pairs, int n_pairs, float* __restrict__ h_slot, int d) {
+    const long long dw = d / 4, per_pair = static_cast<long long>(n_pools) * page_words + dw;
+    const long long total = per_pair * n_pairs;
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+         i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const ForkPair f = pairs[i / per_pair];
+        const long long w = i % per_pair;
+        if (w < per_pair - dw) {
+            if (f.src_page < 0) continue;
+            const long long pool = w / page_words, o = w % page_words;
+            uint4* base = reinterpret_cast<uint4*>(pools[pool]);
+            base[static_cast<long long>(f.dst_page) * page_words + o] = base[static_cast<long long>(f.src_page) * page_words + o];
+        } else {
+            const long long c = w - (per_pair - dw);
+            float4* h = reinterpret_cast<float4*>(h_slot);
+            h[f.dst_slot * dw + c] = h[f.src_slot * dw + c];
+        }
+    }
+}
+
 // fp32 rows -> bf16 hi/lo rows (bring-up hook vcb_debug_gemm only)
 __global__ void split_rows_kernel(const float* __restrict__ x, int N, __nv_bfloat16* __restrict__ act, int ld_act,
                                   int bpad) {
@@ -200,17 +230,140 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// One page of one row's online softmax: the scores of this warp's keys (into sc, then one barrier over the consumers),
+// the running max / sum, and PV for this warp's keys.  Both instantiations of attn_rows_kernel run every row through it.
+template <typename KVT, int HD>
+__device__ __forceinline__ void att_page(const KVT* K, const KVT* V, float* sc, float* pw, const float (&q)[8], int p,
+                                         int pos, float scale, float& m_run, float& l_run, float (&acc)[HD / 32]) {
+    constexpr int LPT = HD / 8;          // lanes per key in QK
+    constexpr int TPW = 32 / LPT;        // keys per warp iteration
+    constexpr int DPT = HD / 32;         // output dims per lane in PV
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int sub = lane % LPT;
+    // ---- scores for this warp's KPW keys
+    constexpr int KPW = KV_PAGE / ATT_CWARPS;
+#pragma unroll
+    for (int itq = 0; itq < KPW / TPW; ++itq) {
+        const int t = warp * KPW + itq * TPW + lane / LPT;
+        float kv[8];
+        load_kv_vec<KVT, 8>(K + t * HD + sub * 8, kv);
+        float dsum = 0.f;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) dsum = fmaf(q[i], kv[i], dsum);
+#pragma unroll
+        for (int o = LPT / 2; o > 0; o >>= 1) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
+        if (sub == 0) sc[t] = (p * KV_PAGE + t <= pos) ? dsum * scale : -INFINITY;
+    }
+    named_bar_sync(1, ATT_THREADS);
+    // ---- online softmax bookkeeping (every warp redundantly over all 64 scores: identical m, l)
+    const float s0 = sc[lane], s1 = sc[lane + 32];
+    const float m_new = fmaxf(m_run, warp_max(fmaxf(s0, s1)));
+    const float corr = expf(m_run - m_new);
+    const float e0 = expf(s0 - m_new), e1 = expf(s1 - m_new);
+    float* mypw = pw + warp * KV_PAGE;
+    mypw[lane] = e0;
+    mypw[lane + 32] = e1;
+    l_run = l_run * corr + warp_sum(e0 + e1);
+    m_run = m_new;
+    __syncwarp();
+    // ---- PV for this warp's KPW keys
+#pragma unroll
+    for (int i = 0; i < DPT; ++i) acc[i] *= corr;
+#pragma unroll
+    for (int tt = 0; tt < KPW; ++tt) {
+        const int t = warp * KPW + tt;
+        const float pt_ = mypw[t];
+        float vv[DPT];
+        load_kv_vec<KVT, DPT>(V + t * HD + lane * DPT, vv);
+#pragma unroll
+        for (int i = 0; i < DPT; ++i) acc[i] = fmaf(pt_, vv[i], acc[i]);
+    }
+    __syncwarp();
+}
+
+// End of one (row, head, chunk): combine the consumer warps' partial outputs; a one-chunk context writes the output rows,
+// a split context publishes (o, m, l) and the last chunk to finish merges all chunks in chunk order.
+template <int HD>
+__device__ __forceinline__ void att_finish(const float (&acc)[HD / 32], float m_run, float l_run, int r, int h, int rh,
+                                           int chunk, int nch, float* red, __nv_bfloat16* __restrict__ act, int ld_act,
+                                           int bpad, float* __restrict__ ws, int* __restrict__ cnt, int maxch, int& s_last) {
+    constexpr int DPT = HD / 32;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+    for (int i = 0; i < DPT; ++i) red[warp * HD + lane * DPT + i] = acc[i];
+    named_bar_sync(1, ATT_THREADS);
+    const size_t ocol = static_cast<size_t>(h) * HD;
+    if (nch == 1) {
+        for (int dd = threadIdx.x; dd < HD; dd += ATT_THREADS) {
+            float osum = 0.f;
+#pragma unroll
+            for (int w = 0; w < ATT_CWARPS; ++w) osum += red[w * HD + dd];
+            const float o = osum / l_run;
+            __nv_bfloat16 hi, lo;
+            split_bf16(o, hi, lo);
+            act[static_cast<size_t>(r) * ld_act + ocol + dd] = hi;
+            act[static_cast<size_t>(r + bpad) * ld_act + ocol + dd] = lo;
+        }
+        named_bar_sync(1, ATT_THREADS);                   // red[] is reused by the next item
+        return;
+    }
+    float* myws = ws + (static_cast<size_t>(rh) * maxch + chunk) * (HD + 2);
+    for (int dd = threadIdx.x; dd < HD; dd += ATT_THREADS) {
+        float osum = 0.f;
+#pragma unroll
+        for (int w = 0; w < ATT_CWARPS; ++w) osum += red[w * HD + dd];
+        myws[dd] = osum;
+    }
+    if (threadIdx.x == 0) {
+        myws[HD] = m_run;
+        myws[HD + 1] = l_run;
+    }
+    __threadfence();
+    named_bar_sync(1, ATT_THREADS);
+    if (threadIdx.x == 0) s_last = (atomicAdd(&cnt[rh], 1) == nch - 1);
+    named_bar_sync(1, ATT_THREADS);
+    if (s_last) {
+        __threadfence();
+        const volatile float* base = ws + static_cast<size_t>(rh) * maxch * (HD + 2);
+        float M = -INFINITY;
+        for (int c = 0; c < nch; ++c) M = fmaxf(M, base[c * (HD + 2) + HD]);
+        for (int dd = threadIdx.x; dd < HD; dd += ATT_THREADS) {
+            float Lsum = 0.f, O = 0.f;
+            for (int c = 0; c < nch; ++c) {
+                const float w = expf(base[c * (HD + 2) + HD] - M);
+                Lsum += base[c * (HD + 2) + HD + 1] * w;
+                O += base[c * (HD + 2) + dd] * w;
+            }
+            const float o = O / Lsum;
+            __nv_bfloat16 hi, lo;
+            split_bf16(o, hi, lo);
+            act[static_cast<size_t>(r) * ld_act + ocol + dd] = hi;
+            act[static_cast<size_t>(r + bpad) * ld_act + ocol + dd] = lo;
+        }
+        if (threadIdx.x == 0) cnt[rh] = 0;
+    }
+    named_bar_sync(1, ATT_THREADS);                       // s_last / red[] reused by the next item
+}
+
 // Persistent, warp-specialised version: grid = a few CTAs per SM; each CTA walks a static list of work items
 // (row*head, context chunk).  Warp 4 is the TMA producer: it runs ahead ACROSS items, so the HBM stream never drains
 // at an item boundary (short CTAs with a cold start leave HBM idle).
 // Warps 0..ATT_CWARPS-1 consume pages: scores -> online softmax -> PV, release the stage through an mbarrier.
-template <typename KVT, int HD>
+//
+// GMAX > 1: row groups.  A work item is (row group, head, chunk); n_rh counts groups * heads.  Group g holds rows
+// grp_first[g] .. grp_first[g+1]-1 (at most GMAX), whose positions are equal or -1 (inactive: output untouched), and whose
+// first grp_shared[g] pages are the same pages (a best-of-N group's prompt).  A shared page is loaded once and the
+// consumers run every active member over it in turn, each with its own q / m / l / acc; a private page is loaded per
+// member.  Every row goes through att_page and att_finish in the same order as with GMAX = 1: its output is
+// bit-identical.
+template <typename KVT, int HD, int GMAX>
 __global__ void __launch_bounds__(ATT_THREADS + 32)
 attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, const KVT* __restrict__ vpool,
                  const int* __restrict__ page_table, int max_pages, const int* __restrict__ row_slot,
                  const int* __restrict__ row_pos, int H, __nv_bfloat16* __restrict__ act, int ld_act, int bpad,
                  float scale, float* __restrict__ ws, int* __restrict__ cnt, int maxch, int chunk_pages, int n_rh,
-                 int n_chunks, const int* __restrict__ row_pages) {
+                 int n_chunks, const int* __restrict__ row_pages, const int* __restrict__ grp_first,
+                 const int* __restrict__ grp_shared) {
     using L = AttSmem<KVT, HD>;
     constexpr int LPT = HD / 8;          // lanes per key in QK
     constexpr int TPW = 32 / LPT;        // keys per warp iteration
@@ -241,163 +394,267 @@ attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, 
     if (threadIdx.x == 0) { tl_mark(0x310); tl_mark_all(0x310); }
     const int n_items = n_rh * n_chunks;
 
-    if (warp == ATT_CWARPS) {
-        // ===== producer: one lane streams the K/V pages of every item of this CTA, in order ================
-        if (lane == 0) {
-            const uint64_t pol = l2_policy_evict_first();          // KV pages stream through L2 once per step
-            int it = 0;
-            for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-                const int chunk = item / n_rh, rh = item - chunk * n_rh;
-                const int r = rh / H, h = rh - r * H;
-                const int pos = row_pos[r];
-                if (pos < 0) continue;
-                const int npages = pos / KV_PAGE + 1;
-                const int p0 = chunk * chunk_pages;
-                if (p0 >= npages) continue;
-                const int p1 = min(npages, p0 + chunk_pages);
-                // decode steps: step_prep left a per-row copy of the slot's page list, so the first TMA issue is one
-                // L2 round trip away (row -> pages) instead of two (row -> slot -> pages)
-                const int* pt = row_pages ? row_pages + r * max_pages : page_table + row_slot[r] * max_pages;
-                for (int p = p0; p < p1; ++p, ++it) {
-                    const int s = it % ATT_STAGES;
-                    if (it >= ATT_STAGES) mbar_wait(&empty[s], ((it / ATT_STAGES) - 1) & 1);
-                    const size_t off = (static_cast<size_t>(pt[p]) * H + h) * KV_PAGE * HD;
-                    mbar_arrive_expect_tx(&full[s], 2 * L::PAGE_BYTES);
-                    tma_bulk_g2s_hint(sK + s * KV_PAGE * HD, kpool + off, L::PAGE_BYTES, &full[s], pol);
-                    tma_bulk_g2s_hint(sV + s * KV_PAGE * HD, vpool + off, L::PAGE_BYTES, &full[s], pol);
+    if constexpr (GMAX == 1) {
+        if (warp == ATT_CWARPS) {
+            // ===== producer: one lane streams the K/V pages of every item of this CTA, in order ================
+            if (lane == 0) {
+                const uint64_t pol = l2_policy_evict_first();          // KV pages stream through L2 once per step
+                int it = 0;
+                for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+                    const int chunk = item / n_rh, rh = item - chunk * n_rh;
+                    const int r = rh / H, h = rh - r * H;
+                    const int pos = row_pos[r];
+                    if (pos < 0) continue;
+                    const int npages = pos / KV_PAGE + 1;
+                    const int p0 = chunk * chunk_pages;
+                    if (p0 >= npages) continue;
+                    const int p1 = min(npages, p0 + chunk_pages);
+                    // decode steps: step_prep left a per-row copy of the slot's page list, so the first TMA issue is one
+                    // L2 round trip away (row -> pages) instead of two (row -> slot -> pages)
+                    const int* pt = row_pages ? row_pages + r * max_pages : page_table + row_slot[r] * max_pages;
+                    for (int p = p0; p < p1; ++p, ++it) {
+                        const int s = it % ATT_STAGES;
+                        if (it >= ATT_STAGES) mbar_wait(&empty[s], ((it / ATT_STAGES) - 1) & 1);
+                        const size_t off = (static_cast<size_t>(pt[p]) * H + h) * KV_PAGE * HD;
+                        mbar_arrive_expect_tx(&full[s], 2 * L::PAGE_BYTES);
+                        tma_bulk_g2s_hint(sK + s * KV_PAGE * HD, kpool + off, L::PAGE_BYTES, &full[s], pol);
+                        tma_bulk_g2s_hint(sV + s * KV_PAGE * HD, vpool + off, L::PAGE_BYTES, &full[s], pol);
+                    }
                 }
             }
+            return;
         }
-        return;
-    }
 
-    // ===== consumers ================================================================================
-    const int sub = lane % LPT;
-    int it = 0;
-    for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        const int chunk = item / n_rh, rh = item - chunk * n_rh;
-        const int r = rh / H, h = rh - r * H;
-        const int pos = row_pos[r];
-        if (pos < 0) continue;
-        const int npages = pos / KV_PAGE + 1;
-        const int p0 = chunk * chunk_pages;
-        if (p0 >= npages) continue;
-        const int p1 = min(npages, p0 + chunk_pages);
-        const int nch = (npages + chunk_pages - 1) / chunk_pages;
-        float q[8];
-        {
-            const float* qp = qbuf + (static_cast<size_t>(r) * H + h) * HD + sub * 8;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) q[i] = qp[i];
-        }
-        float m_run = -INFINITY, l_run = 0.f;
-        float acc[DPT];
-#pragma unroll
-        for (int i = 0; i < DPT; ++i) acc[i] = 0.f;
-
-        for (int p = p0; p < p1; ++p, ++it) {
-            const int s = it % ATT_STAGES;
-            mbar_wait(&full[s], (it / ATT_STAGES) & 1);
-            const KVT* K = sK + s * KV_PAGE * HD;
-            const KVT* V = sV + s * KV_PAGE * HD;
-            float* sc = sc_all + (it & 1) * KV_PAGE;
-            // ---- scores for this warp's KPW keys
-            constexpr int KPW = KV_PAGE / ATT_CWARPS;
-#pragma unroll
-            for (int itq = 0; itq < KPW / TPW; ++itq) {
-                const int t = warp * KPW + itq * TPW + lane / LPT;
-                float kv[8];
-                load_kv_vec<KVT, 8>(K + t * HD + sub * 8, kv);
-                float dsum = 0.f;
-#pragma unroll
-                for (int i = 0; i < 8; ++i) dsum = fmaf(q[i], kv[i], dsum);
-#pragma unroll
-                for (int o = LPT / 2; o > 0; o >>= 1) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
-                if (sub == 0) sc[t] = (p * KV_PAGE + t <= pos) ? dsum * scale : -INFINITY;
+        // ===== consumers ================================================================================
+        const int sub = lane % LPT;
+        int it = 0;
+        for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+            const int chunk = item / n_rh, rh = item - chunk * n_rh;
+            const int r = rh / H, h = rh - r * H;
+            const int pos = row_pos[r];
+            if (pos < 0) continue;
+            const int npages = pos / KV_PAGE + 1;
+            const int p0 = chunk * chunk_pages;
+            if (p0 >= npages) continue;
+            const int p1 = min(npages, p0 + chunk_pages);
+            const int nch = (npages + chunk_pages - 1) / chunk_pages;
+            float q[8];
+            {
+                const float* qp = qbuf + (static_cast<size_t>(r) * H + h) * HD + sub * 8;
+    #pragma unroll
+                for (int i = 0; i < 8; ++i) q[i] = qp[i];
             }
+            float m_run = -INFINITY, l_run = 0.f;
+            float acc[DPT];
+    #pragma unroll
+            for (int i = 0; i < DPT; ++i) acc[i] = 0.f;
+
+            for (int p = p0; p < p1; ++p, ++it) {
+                const int s = it % ATT_STAGES;
+                mbar_wait(&full[s], (it / ATT_STAGES) & 1);
+                const KVT* K = sK + s * KV_PAGE * HD;
+                const KVT* V = sV + s * KV_PAGE * HD;
+                float* sc = sc_all + (it & 1) * KV_PAGE;
+                // ---- scores for this warp's KPW keys
+                constexpr int KPW = KV_PAGE / ATT_CWARPS;
+    #pragma unroll
+                for (int itq = 0; itq < KPW / TPW; ++itq) {
+                    const int t = warp * KPW + itq * TPW + lane / LPT;
+                    float kv[8];
+                    load_kv_vec<KVT, 8>(K + t * HD + sub * 8, kv);
+                    float dsum = 0.f;
+    #pragma unroll
+                    for (int i = 0; i < 8; ++i) dsum = fmaf(q[i], kv[i], dsum);
+    #pragma unroll
+                    for (int o = LPT / 2; o > 0; o >>= 1) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
+                    if (sub == 0) sc[t] = (p * KV_PAGE + t <= pos) ? dsum * scale : -INFINITY;
+                }
+                named_bar_sync(1, ATT_THREADS);
+                // ---- online softmax bookkeeping (every warp redundantly over all 64 scores: identical m, l)
+                const float s0 = sc[lane], s1 = sc[lane + 32];
+                const float m_new = fmaxf(m_run, warp_max(fmaxf(s0, s1)));
+                const float corr = expf(m_run - m_new);
+                const float e0 = expf(s0 - m_new), e1 = expf(s1 - m_new);
+                float* mypw = pw + warp * KV_PAGE;
+                mypw[lane] = e0;
+                mypw[lane + 32] = e1;
+                l_run = l_run * corr + warp_sum(e0 + e1);
+                m_run = m_new;
+                __syncwarp();
+                // ---- PV for this warp's KPW keys
+    #pragma unroll
+                for (int i = 0; i < DPT; ++i) acc[i] *= corr;
+    #pragma unroll
+                for (int tt = 0; tt < KPW; ++tt) {
+                    const int t = warp * KPW + tt;
+                    const float pt_ = mypw[t];
+                    float vv[DPT];
+                    load_kv_vec<KVT, DPT>(V + t * HD + lane * DPT, vv);
+    #pragma unroll
+                    for (int i = 0; i < DPT; ++i) acc[i] = fmaf(pt_, vv[i], acc[i]);
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[s]);            // this warp is done with stage s
+            }
+            // ---- combine the 4 warps' partial outputs of this item
+    #pragma unroll
+            for (int i = 0; i < DPT; ++i) red[warp * HD + lane * DPT + i] = acc[i];
             named_bar_sync(1, ATT_THREADS);
-            // ---- online softmax bookkeeping (every warp redundantly over all 64 scores: identical m, l)
-            const float s0 = sc[lane], s1 = sc[lane + 32];
-            const float m_new = fmaxf(m_run, warp_max(fmaxf(s0, s1)));
-            const float corr = expf(m_run - m_new);
-            const float e0 = expf(s0 - m_new), e1 = expf(s1 - m_new);
-            float* mypw = pw + warp * KV_PAGE;
-            mypw[lane] = e0;
-            mypw[lane + 32] = e1;
-            l_run = l_run * corr + warp_sum(e0 + e1);
-            m_run = m_new;
-            __syncwarp();
-            // ---- PV for this warp's KPW keys
-#pragma unroll
-            for (int i = 0; i < DPT; ++i) acc[i] *= corr;
-#pragma unroll
-            for (int tt = 0; tt < KPW; ++tt) {
-                const int t = warp * KPW + tt;
-                const float pt_ = mypw[t];
-                float vv[DPT];
-                load_kv_vec<KVT, DPT>(V + t * HD + lane * DPT, vv);
-#pragma unroll
-                for (int i = 0; i < DPT; ++i) acc[i] = fmaf(pt_, vv[i], acc[i]);
+            const size_t ocol = static_cast<size_t>(h) * HD;
+            if (nch == 1) {
+                for (int dd = threadIdx.x; dd < HD; dd += ATT_THREADS) {
+                    float osum = 0.f;
+    #pragma unroll
+                    for (int w = 0; w < ATT_CWARPS; ++w) osum += red[w * HD + dd];
+                    const float o = osum / l_run;
+                    __nv_bfloat16 hi, lo;
+                    split_bf16(o, hi, lo);
+                    act[static_cast<size_t>(r) * ld_act + ocol + dd] = hi;
+                    act[static_cast<size_t>(r + bpad) * ld_act + ocol + dd] = lo;
+                }
+                named_bar_sync(1, ATT_THREADS);                   // red[] is reused by the next item
+                continue;
             }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&empty[s]);            // this warp is done with stage s
-        }
-        // ---- combine the 4 warps' partial outputs of this item
-#pragma unroll
-        for (int i = 0; i < DPT; ++i) red[warp * HD + lane * DPT + i] = acc[i];
-        named_bar_sync(1, ATT_THREADS);
-        const size_t ocol = static_cast<size_t>(h) * HD;
-        if (nch == 1) {
+            // ---- split context: publish (o, m, l); the last chunk to finish merges all chunks in chunk order
+            float* myws = ws + (static_cast<size_t>(rh) * maxch + chunk) * (HD + 2);
             for (int dd = threadIdx.x; dd < HD; dd += ATT_THREADS) {
                 float osum = 0.f;
-#pragma unroll
+    #pragma unroll
                 for (int w = 0; w < ATT_CWARPS; ++w) osum += red[w * HD + dd];
-                const float o = osum / l_run;
-                __nv_bfloat16 hi, lo;
-                split_bf16(o, hi, lo);
-                act[static_cast<size_t>(r) * ld_act + ocol + dd] = hi;
-                act[static_cast<size_t>(r + bpad) * ld_act + ocol + dd] = lo;
+                myws[dd] = osum;
             }
-            named_bar_sync(1, ATT_THREADS);                   // red[] is reused by the next item
-            continue;
-        }
-        // ---- split context: publish (o, m, l); the last chunk to finish merges all chunks in chunk order
-        float* myws = ws + (static_cast<size_t>(rh) * maxch + chunk) * (HD + 2);
-        for (int dd = threadIdx.x; dd < HD; dd += ATT_THREADS) {
-            float osum = 0.f;
-#pragma unroll
-            for (int w = 0; w < ATT_CWARPS; ++w) osum += red[w * HD + dd];
-            myws[dd] = osum;
-        }
-        if (threadIdx.x == 0) {
-            myws[HD] = m_run;
-            myws[HD + 1] = l_run;
-        }
-        __threadfence();
-        named_bar_sync(1, ATT_THREADS);
-        if (threadIdx.x == 0) s_last = (atomicAdd(&cnt[rh], 1) == nch - 1);
-        named_bar_sync(1, ATT_THREADS);
-        if (s_last) {
+            if (threadIdx.x == 0) {
+                myws[HD] = m_run;
+                myws[HD + 1] = l_run;
+            }
             __threadfence();
-            const volatile float* base = ws + static_cast<size_t>(rh) * maxch * (HD + 2);
-            float M = -INFINITY;
-            for (int c = 0; c < nch; ++c) M = fmaxf(M, base[c * (HD + 2) + HD]);
-            for (int dd = threadIdx.x; dd < HD; dd += ATT_THREADS) {
-                float Lsum = 0.f, O = 0.f;
-                for (int c = 0; c < nch; ++c) {
-                    const float w = expf(base[c * (HD + 2) + HD] - M);
-                    Lsum += base[c * (HD + 2) + HD + 1] * w;
-                    O += base[c * (HD + 2) + dd] * w;
+            named_bar_sync(1, ATT_THREADS);
+            if (threadIdx.x == 0) s_last = (atomicAdd(&cnt[rh], 1) == nch - 1);
+            named_bar_sync(1, ATT_THREADS);
+            if (s_last) {
+                __threadfence();
+                const volatile float* base = ws + static_cast<size_t>(rh) * maxch * (HD + 2);
+                float M = -INFINITY;
+                for (int c = 0; c < nch; ++c) M = fmaxf(M, base[c * (HD + 2) + HD]);
+                for (int dd = threadIdx.x; dd < HD; dd += ATT_THREADS) {
+                    float Lsum = 0.f, O = 0.f;
+                    for (int c = 0; c < nch; ++c) {
+                        const float w = expf(base[c * (HD + 2) + HD] - M);
+                        Lsum += base[c * (HD + 2) + HD + 1] * w;
+                        O += base[c * (HD + 2) + dd] * w;
+                    }
+                    const float o = O / Lsum;
+                    __nv_bfloat16 hi, lo;
+                    split_bf16(o, hi, lo);
+                    act[static_cast<size_t>(r) * ld_act + ocol + dd] = hi;
+                    act[static_cast<size_t>(r + bpad) * ld_act + ocol + dd] = lo;
                 }
-                const float o = O / Lsum;
-                __nv_bfloat16 hi, lo;
-                split_bf16(o, hi, lo);
-                act[static_cast<size_t>(r) * ld_act + ocol + dd] = hi;
-                act[static_cast<size_t>(r + bpad) * ld_act + ocol + dd] = lo;
+                if (threadIdx.x == 0) cnt[rh] = 0;
             }
-            if (threadIdx.x == 0) cnt[rh] = 0;
+            named_bar_sync(1, ATT_THREADS);                       // s_last / red[] reused by the next item
         }
-        named_bar_sync(1, ATT_THREADS);                       // s_last / red[] reused by the next item
+    } else {
+        // the row's page list, as in the GMAX = 1 producer
+        auto pages_of = [&](int r) { return row_pages ? row_pages + r * max_pages : page_table + row_slot[r] * max_pages; };
+        // the item's group: rows r0 .. r0 + size - 1, active members as a bit mask, their common position
+        auto group_of = [&](int gh, int& r0, int& size, int& h, unsigned& live, int& pos) {
+            const int g = gh / H;
+            h = gh - g * H;
+            r0 = grp_first[g];
+            size = grp_first[g + 1] - r0;
+            live = 0;
+            pos = -1;
+#pragma unroll
+            for (int j = 0; j < GMAX; ++j)
+                if (j < size && row_pos[r0 + j] >= 0) {
+                    live |= 1u << j;
+                    pos = row_pos[r0 + j];
+                }
+        };
+        if (warp == ATT_CWARPS) {
+            if (lane == 0) {
+                const uint64_t pol = l2_policy_evict_first();
+                int it = 0;
+                for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+                    const int chunk = item / n_rh, gh = item - chunk * n_rh;
+                    int r0, size, h, pos;
+                    unsigned live;
+                    group_of(gh, r0, size, h, live, pos);
+                    if (!live) continue;
+                    const int npages = pos / KV_PAGE + 1;
+                    const int p0 = chunk * chunk_pages;
+                    if (p0 >= npages) continue;
+                    const int p1 = min(npages, p0 + chunk_pages);
+                    const int S = grp_shared[gh / H];
+                    const int lead = r0 + __ffs(live) - 1;
+                    for (int p = p0; p < p1; ++p) {
+                        for (int j = 0; j < size; ++j) {
+                            if (!(live >> j & 1) || (p < S && r0 + j != lead)) continue;
+                            const int s = it % ATT_STAGES;
+                            if (it >= ATT_STAGES) mbar_wait(&empty[s], ((it / ATT_STAGES) - 1) & 1);
+                            const size_t off = (static_cast<size_t>(pages_of(r0 + j)[p]) * H + h) * KV_PAGE * HD;
+                            mbar_arrive_expect_tx(&full[s], 2 * L::PAGE_BYTES);
+                            tma_bulk_g2s_hint(sK + s * KV_PAGE * HD, kpool + off, L::PAGE_BYTES, &full[s], pol);
+                            tma_bulk_g2s_hint(sV + s * KV_PAGE * HD, vpool + off, L::PAGE_BYTES, &full[s], pol);
+                            ++it;
+                        }
+                    }
+                }
+            }
+            return;
+        }
+
+        const int sub = lane % LPT;
+        int it = 0, k = 0;          // k: score passes (one per member and page), the parity of the score buffer
+        for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+            const int chunk = item / n_rh, gh = item - chunk * n_rh;
+            int r0, size, h, pos;
+            unsigned live;
+            group_of(gh, r0, size, h, live, pos);
+            if (!live) continue;
+            const int npages = pos / KV_PAGE + 1;
+            const int p0 = chunk * chunk_pages;
+            if (p0 >= npages) continue;
+            const int p1 = min(npages, p0 + chunk_pages);
+            const int nch = (npages + chunk_pages - 1) / chunk_pages;
+            const int S = grp_shared[gh / H];
+            float q[GMAX][8], m_run[GMAX], l_run[GMAX], acc[GMAX][DPT];
+#pragma unroll
+            for (int j = 0; j < GMAX; ++j) {
+                if (live >> j & 1) {
+                    const float* qp = qbuf + (static_cast<size_t>(r0 + j) * H + h) * HD + sub * 8;
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) q[j][i] = qp[i];
+                }
+                m_run[j] = -INFINITY;
+                l_run[j] = 0.f;
+#pragma unroll
+                for (int i = 0; i < DPT; ++i) acc[j][i] = 0.f;
+            }
+            for (int p = p0; p < p1; ++p) {
+                const bool shared = p < S;
+#pragma unroll
+                for (int j = 0; j < GMAX; ++j) {
+                    if (!(live >> j & 1)) continue;
+                    const int s = it % ATT_STAGES;
+                    const bool first = !shared || (live & ((1u << j) - 1)) == 0;
+                    const bool last = !shared || (live >> (j + 1)) == 0;
+                    if (first) mbar_wait(&full[s], (it / ATT_STAGES) & 1);
+                    att_page<KVT, HD>(sK + s * KV_PAGE * HD, sV + s * KV_PAGE * HD, sc_all + (k & 1) * KV_PAGE, pw, q[j], p,
+                                      pos, scale, m_run[j], l_run[j], acc[j]);
+                    ++k;
+                    if (last) {
+                        if (lane == 0) mbar_arrive(&empty[s]);
+                        ++it;
+                    }
+                }
+            }
+#pragma unroll
+            for (int j = 0; j < GMAX; ++j)
+                if (live >> j & 1)
+                    att_finish<HD>(acc[j], m_run[j], l_run[j], r0 + j, h, (r0 + j) * H + h, chunk, nch, red, act, ld_act,
+                                   bpad, ws, cnt, maxch, s_last);
+        }
     }
     if (threadIdx.x == 0) { tl_mark(0x330); tl_mark_all(0x330); }
 }

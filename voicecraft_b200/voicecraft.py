@@ -468,20 +468,25 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         return [r[0] for r in self.open_edit_session(xs, ys, mask_intervals, **kw)._run_many(poll_every)]
 
     def open_tts_session(self, xs, ys, top_k=-100, top_p=1.0, temperature=1.0, stop_repetition=3,
-                         silence_tokens=(1388, 1898, 131), seeds=None, noise_fns=None):
+                         silence_tokens=(1388, 1898, 131), seeds=None, noise_fns=None, best_of=1):
         """xs: list of [1,L] int64, ys: list of [1,T,K] int64 (any device).  Prefills every utterance (one packed,
         chunked pass) and returns a DecodeSession whose .step() runs one decode step for all of them.
 
         seeds: one generator seed per utterance -- utterance i samples from the Philox stream of a torch CUDA generator
         seeded with seeds[i] (offset 0), i.e. its tokens equal ``torch.manual_seed(seeds[i]); inference_tts(x_i, ., y_i)``.
         Default: the device generator's current seed + i at its current offset (the global generator is left untouched).
-        noise_fns: instead, one callable(shape=[K,V], device) per utterance (tests: CPU-generator noise for the oracle)."""
+        noise_fns: instead, one callable(shape=[best_of*K,V], device) per utterance (tests: CPU-generator noise for the
+        oracle).
+        best_of: each utterance is sampled best_of times and keeps the copy that ends first, what
+        ``inference_tts_batch(x_i, ., y_i, batch_size=best_of)`` returns under the same seed.  The copies share one
+        prefill and the KV pages of the prompt's full pages."""
         return DecodeSession(self, xs, ys, self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
-                             seeds=seeds, noise_fns=noise_fns)
+                             seeds=seeds, noise_fns=noise_fns, best_of=best_of)
 
     @torch.no_grad()
     def inference_tts_many(self, xs, ys, poll_every: int = 8, **kw):
-        """Returns a list of (res [1,K,T+G], gen [1,K,G]) like inference_tts, one per utterance."""
+        """Returns a list of (res [1,K,T+G], gen [1,K,G]) like inference_tts (inference_tts_batch with best_of > 1), one
+        per utterance."""
         return self.open_tts_session(xs, ys, **kw)._run_many(poll_every)
 
     # ------------------------------------------------------------------------------------------------
@@ -491,6 +496,7 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         """inference_tts_many with the audio handed out while it is generated: iterates (i, wav [1, channels, n*hop]),
         utterance i's chunks in order; concatenated they equal ``tokenizer.decode_codes(gen_i)``.  Afterwards
         ``.results`` equals what inference_tts_many returns.  `seeds` as in open_tts_session."""
+        _no_stream_best_of(kw.get("best_of", 1))
         sess = self.open_tts_session(xs, ys, seeds=seeds, **kw)
         return TtsStream(sess, tokenizer, chunk_frames, poll_every)
 
@@ -505,6 +511,19 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
                              n_copies=1)
         return _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every)
+
+
+def _check_best_of(best_of) -> int:
+    if isinstance(best_of, bool) or int(best_of) != best_of or best_of < 1:
+        raise ValueError(f"best_of must be an integer >= 1, got {best_of!r}")
+    return int(best_of)
+
+
+def _no_stream_best_of(best_of):
+    """best-of-N keeps the copy that ends first, so which copy's audio to hand out is known only when the group ends"""
+    if _check_best_of(best_of) > 1:
+        raise ValueError(f"best_of={best_of}: streaming hands out audio while it is generated, but the kept copy of a "
+                         "best-of-N utterance is known only when its group ends; use inference_tts_many / run() instead")
 
 
 def _end_token(a) -> int:
@@ -689,6 +708,9 @@ class TtsStream(_AudioStream):
     def __init__(self, sess: "DecodeSession", tokenizer, chunk_frames: int = 25, poll_every: int = 8):
         if chunk_frames < 1 or poll_every < 1:
             raise ValueError("chunk_frames and poll_every must be >= 1")
+        if sess.n_copies > 1:
+            sess.close()
+            _no_stream_best_of(sess.n_copies)
         self._start(SimpleNamespace(sess=sess, dev=sess.dev, tok=tokenizer, chunk_frames=int(chunk_frames),
                                     poll_every=int(poll_every), results=None, first_audio_steps=None), sess.B)
 
@@ -858,16 +880,19 @@ class _SingleTtsStream(TtsStream):
 
 
 class DecodeSession:
-    """A batch of independent utterances resident in the engine, one slot and one random stream each."""
+    """A batch of independent utterances resident in the engine, one random stream each, and one slot each or, best-of-N,
+    one group of consecutive slots each."""
 
-    def __init__(self, model: "VoiceCraft", xs, ys, sp, mask_intervals=None, seeds=None, noise_fns=None, *, n_copies=None):
-        """n_copies (the single calls inference_tts, inference_tts_batch, inference and inference_tts_stream): the one
-        utterance is sampled in n_copies slots (best-of-N) from the device generator's stream at its current offset, and
-        results() leaves the generator advanced as the single call does."""
+    def __init__(self, model: "VoiceCraft", xs, ys, sp, mask_intervals=None, seeds=None, noise_fns=None, *, best_of=1,
+                 n_copies=None):
+        """best_of: each utterance is sampled in best_of slots and keeps the copy that ends first (inference_tts_batch).
+        n_copies (the single calls inference_tts, inference_tts_batch, inference and inference_tts_stream): best_of, and
+        the one utterance samples from the device generator's stream at its current offset, and results() leaves the
+        generator advanced as the single call does."""
         K = model.args.n_codebooks
         dev = model.mask_embedding.device
         self.model, self.sp, self.dev, self.K = model, sp, dev, K
-        self.B, self.V, self.n_copies = len(xs), model.n_audio_tokens[0], n_copies or 1
+        self.B, self.V, self.n_copies = len(xs), model.n_audio_tokens[0], _check_best_of(n_copies or best_of)
         self.lib = _lib.load()
         self.edit = mask_intervals is not None
         if seeds is not None and len(seeds) != self.B:
@@ -911,9 +936,9 @@ class DecodeSession:
         if not self._host_noise:
             return None
         if draw and self._noise_fns is not None:
-            K = self.K
+            R = self.n_copies * self.K             # an utterance's rows: member-major, as its group draws them
             for i, fn in enumerate(self._noise_fns):
-                self._buf[i * K:(i + 1) * K].copy_(fn((K, self.V), self.dev).to(device=self.dev, dtype=torch.float32))
+                self._buf[i * R:(i + 1) * R].copy_(fn((R, self.V), self.dev).to(device=self.dev, dtype=torch.float32))
         elif draw:
             self.model._draw_noise(self._buf)
         return self._buf.data_ptr()
@@ -980,9 +1005,13 @@ class DecodeSession:
             self.model.trace_logits.append(t)
 
     def raw_tokens(self, i):
-        """delayed token rows [n_steps, K] of utterance i (host numpy)"""
+        """delayed token rows [n_steps, K] of utterance i (host numpy); best-of-N: of its kept copy once the group has
+        decided, of its first copy before"""
         st = self.poll()
-        return self.model._read_rows(self.eng, self.slots[i], st[i].n_steps, self.stream)
+        j = i * self.n_copies
+        if self.n_copies > 1 and st[j].keep >= 0:
+            j += st[j].keep
+        return self.model._read_rows(self.eng, self.slots[j], st[j].n_steps, self.stream)
 
     def results(self):
         return self._results(self.poll())
@@ -1005,6 +1034,23 @@ class DecodeSession:
         self.model._release_slots(self.slots, n_copies=self.n_copies)
 
 
+def place_groups(free, sizes, nxt):
+    """Admission of ContinuousBatcher.run(): tickets nxt, nxt+1, ... in order, ticket t needing sizes[t] consecutive slots
+    (its best-of-N group).  Each takes the lowest run of that many consecutive slots in the set `free`; the first ticket
+    that finds none stops the admission, so a later ticket never overtakes it.  Removes the taken slots from `free` and
+    returns ([(first slot, ticket)], the next ticket to admit)."""
+    new = []
+    while nxt < len(sizes):
+        n = sizes[nxt]
+        base = next((s for s in sorted(free) if all(s + c in free for c in range(n))), None)
+        if base is None:
+            break
+        free.difference_update(range(base, base + n))
+        new.append((base, nxt))
+        nxt += 1
+    return new, nxt
+
+
 class ContinuousBatcher:
     """Continuous batching of independent TTS utterances (SURVEY.md section 8f, row f2).
 
@@ -1014,7 +1060,8 @@ class ContinuousBatcher:
     others keep decoding.  Every utterance owns its random stream (`seed`), so its result is exactly what
     ``torch.manual_seed(seed); model.inference_tts(x, x_lens, y, ...)`` returns, whatever it was batched with.
     run() returns the token lists once the queue has drained; stream() hands out every utterance's audio while it is
-    generated and takes submit() / cancel() during the iteration.
+    generated and takes submit() / cancel() during the iteration.  A best-of-N ticket (submit(..., best_of=N), run() only)
+    decodes as a group on N consecutive slots; max_concurrency counts slots.
     """
 
     def __init__(self, model: "VoiceCraft", max_concurrency=32, poll_every=8, top_k=-100, top_p=1.0, temperature=1.0,
@@ -1026,19 +1073,26 @@ class ContinuousBatcher:
         self.results, self.errors = [], {}
         self._live = None                  # the running stream()'s state
 
-    def submit(self, x, y, seed=None):
+    def submit(self, x, y, seed=None, best_of=1):
         """x [1,L] int64, y [1,T,K] int64 (host or device).  Returns the ticket (index into run()'s result list / results).
+        best_of: run() samples the utterance best_of times on consecutive slots and keeps the copy that ends first, as
+        ``torch.manual_seed(seed); inference_tts_batch(x, ., y, batch_size=best_of)`` does; the copies count against
+        max_concurrency.  stream() serves only best_of = 1.
         While a stream() runs, the utterance is admitted at one of its next polls; one that does not fit the engine it
         sized raises VcbError and is not queued."""
+        best_of = _check_best_of(best_of)
+        if best_of > self.B:
+            raise ValueError(f"best_of={best_of} copies do not fit max_concurrency={self.B} slots")
         st = self._live
         if st is not None:
+            _no_stream_best_of(best_of)
             job = self._job(x, y, seed)
             if job[0].need_seq > st.max_seq:
                 raise _lib.VcbError(f"utterance needs {job[0].need_seq} positions, the streaming engine holds {st.max_seq}: "
                                     "configure_engine(max_seq_len=...) before stream()")
             st.jobs.append(job)
             self.results.append(None)
-        self.queue.append((x, y, seed))
+        self.queue.append((x, y, seed, best_of))
         return len(self.queue) - 1
 
     def cancel(self, ticket) -> bool:
@@ -1052,20 +1106,21 @@ class ContinuousBatcher:
         st.cancelled.add(ticket)
         return True
 
-    def _job(self, x, y, seed):
-        """(prompt, seed) of a ticket; raises IndexError on an out-of-range id"""
+    def _job(self, x, y, seed, best_of=1):
+        """(prompt, seed, best_of) of a ticket; raises IndexError on an out-of-range id"""
         p = _Prompt(self.model, x, y)
         self.model._check_ids(p.x_ids, p.y_tok)
-        return p, seed
+        return p, seed, best_of
 
     def _admit(self, eng, new, jobs, stream):
-        """one packed prefill + the first sampling step of the newcomers [(slot, ticket)]"""
+        """one packed prefill + the first sampling step of the newcomers [(first slot, ticket)]"""
         m, lib = self.model, _lib.load()
         seed0 = int(torch.cuda.default_generators[m.mask_embedding.device.index or 0].initial_seed())
-        _prefill(eng, [(jobs[t][0], slot, 1, seed0 + t if jobs[t][1] is None else jobs[t][1], 0) for slot, t in new],
-                 stream)
-        c_new = (C.c_int32 * len(new))(*[s for s, _ in new])
-        _lib.check(lib.vcb_sample(eng, c_new, len(new), None, C.byref(self.sp), stream))
+        _prefill(eng, [(jobs[t][0], slot, jobs[t][2], seed0 + t if jobs[t][1] is None else jobs[t][1], 0)
+                       for slot, t in new], stream)
+        rows = [s + c for s, t in new for c in range(jobs[t][2])]
+        c_new = (C.c_int32 * len(rows))(*rows)
+        _lib.check(lib.vcb_sample(eng, c_new, len(rows), None, C.byref(self.sp), stream))
         self.stats["prefills"] += 1
 
     def _result(self, eng, slot, st, job, stream):
@@ -1080,25 +1135,23 @@ class ContinuousBatcher:
         if self._live is not None:
             raise _lib.VcbError("a stream() of this ContinuousBatcher is running")
         dev, lib = m.mask_embedding.device, _lib.load()
-        jobs = [self._job(x, y, seed) for x, y, seed in self.queue]
-        n_slots = min(self.B, max(1, len(jobs)))
-        eng, slots = m._take_slots(n_slots, max([p.need_seq for p, _ in jobs], default=0))
-        free, active, results, nxt = list(slots), {}, [None] * len(jobs), 0
+        jobs = [self._job(*q) for q in self.queue]
+        sizes = [j[2] for j in jobs]
+        n_slots = min(self.B, max(1, sum(sizes)))
+        eng, slots = m._take_slots(n_slots, max([j[0].need_seq for j in jobs], default=0))
+        free, active, results, nxt = set(slots), {}, [None] * len(jobs), 0     # active: first slot -> ticket
         try:
             with torch.cuda.device(dev):
                 stream = torch.cuda.current_stream().cuda_stream
                 steps = 0
                 while nxt < len(jobs) or active:
-                    # ---- refill free slots from the queue
-                    new = []
-                    while free and nxt < len(jobs):
-                        new.append((free.pop(0), nxt))
-                        nxt += 1
+                    # ---- refill free slot runs from the queue, strictly in ticket order
+                    new, nxt = place_groups(free, sizes, nxt)
                     if new:
                         self._admit(eng, new, jobs, stream)
                         for slot, ji in new:
                             active[slot] = ji
-                    order = sorted(active)
+                    order = sorted(s + c for s, ji in active.items() for c in range(sizes[ji]))
                     c_slots = (C.c_int32 * len(order))(*order)
                     self.stats["max_active"] = max(self.stats["max_active"], len(order))
                     # ---- decode steps for everyone until the next poll
@@ -1108,15 +1161,18 @@ class ContinuousBatcher:
                     status = (_lib.vcb_status * len(order))()
                     _lib.check(lib.vcb_poll(eng, c_slots, len(order), status, stream))
                     _check_capacity(status)
-                    for slot, st in zip(order, status):
+                    by_slot = dict(zip(order, status))
+                    for slot, ji in list(active.items()):
+                        st = by_slot[slot]
                         if st.done:
-                            ji = active.pop(slot)
-                            results[ji] = self._result(eng, slot, st, jobs[ji], stream)
-                            m._release_slots(slots, [slot], keep_held=True)
-                            free.append(slot)
+                            kept = slot + (st.keep if sizes[ji] > 1 else 0)
+                            results[ji] = self._result(eng, kept, by_slot[kept], jobs[ji], stream)
+                            m._release_slots(slots, [slot], n_copies=sizes[ji], keep_held=True)
+                            del active[slot]
+                            free.update(range(slot, slot + sizes[ji]))
                 self.stats["steps"] = steps
         finally:
-            m._release_slots(slots, list(active))
+            m._release_slots(slots, [s + c for s, ji in active.items() for c in range(sizes[ji])])
             self.queue = []
         return results
 
@@ -1142,12 +1198,15 @@ class BatcherStream(_AudioStream):
             raise _lib.VcbError("a stream() of this ContinuousBatcher is already running")
         if chunk_frames < 1:
             raise ValueError("chunk_frames must be >= 1")
-        jobs = [cb._job(x, y, seed) for x, y, seed in cb.queue]
-        eng, slots = m._take_slots(cb.B, max([p.need_seq for p, _ in jobs], default=0))
+        jobs = [cb._job(*q) for q in cb.queue]
+        eng, slots = m._take_slots(cb.B, max([j[0].need_seq for j in jobs], default=0))
+        # a queued best-of-N ticket fails (its kept copy is known only when its group ends); the others are served
+        refused = {t for t, j in enumerate(jobs) if j[2] > 1}
         st = SimpleNamespace(cb=cb, eng=eng, slots=slots, max_seq=m._eng_opts["max_seq_len"], jobs=jobs,
-                             cancelled=set(), ended=set(), tok=tokenizer, chunk_frames=int(chunk_frames),
-                             dev=m.mask_embedding.device)
-        cb.results, cb.errors, cb._live = [None] * len(jobs), {}, st
+                             cancelled=set(refused), ended=set(refused), refused=sorted(refused), tok=tokenizer,
+                             chunk_frames=int(chunk_frames), dev=m.mask_embedding.device)
+        cb.results, cb._live = [None] * len(jobs), st
+        cb.errors = {t: f"best_of={jobs[t][2]}: stream() serves only best_of=1 tickets" for t in refused}
         self._start(st, cb.B)
 
     @staticmethod
@@ -1171,6 +1230,8 @@ class BatcherStream(_AudioStream):
                 push = st.push = _PushStep(m, st.eng, stream, st.tok, st.codec, st.cstream, st.chunk_frames, cb.poll_every,
                                            strict=False)
                 empty = torch.zeros(1, st.tok.channels, 0, device=st.dev)
+                for t in st.refused:
+                    yield t, None, True
                 while True:
                     # ---- finished, failed and cancelled utterances leave
                     for slot, r in list(active.items()):
