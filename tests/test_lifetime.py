@@ -129,6 +129,15 @@ def test_debug_hooks_release_their_buffers(unchanged):
     _l.check(lib.vcb_debug_fold_chain(x.data_ptr(), a.data_ptr(), W.data_ptr(), b1.data_ptr(), gamma.data_ptr(),
                                       beta.data_ptr(), W.data_ptr(), b2.data_ptr(), B, d, d, 0, 1, 0, 0, xn.data_ptr(),
                                       y.data_ptr()))
+    # sampler: 2 rows of 3 codebooks over 2053 entries, top-k and top-p, noise drawn on the device
+    V3 = 2053
+    logits = rnd(2, 3, V3)
+    sp = _l.vcb_sampling(top_k=40, top_p=0.8, temperature=1.0, stop_repetition=3, n_silence=0)
+    state = (C.c_int32 * 14)(0, 0, 2, -1, 0, 1, 0, 1, 0, 2, -1, 0, 1, 0)
+    tok, st_out = (C.c_int32 * 6)(), (C.c_int32 * 8)()
+    _l.check(lib.vcb_debug_sampler(logits.data_ptr(), None, 5, 0, 256, C.byref(sp), 2, 3, V3, V3, V3 + 1, 0, 50, state, tok,
+                                   st_out))
+    assert all(0 <= t < V3 for t in tok)
     us = C.c_float()
     _l.check(lib.vcb_bench_gemm(N, K, B, 0, 0, 0, 3, 2, C.byref(us)))
     assert us.value > 0

@@ -60,6 +60,8 @@ PROTOTYPES = {
     "vcb_release": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "vcb_debug_logits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
     "vcb_debug_exponential": (C.c_int, [C.c_void_p, C.c_int64, C.c_uint64, C.c_uint64, C.c_int32, C.c_void_p]),
+    "vcb_debug_sampler": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int32, C.POINTER(vcb_sampling)] +
+                          [C.c_int32] * 7 + [C.POINTER(C.c_int32)] * 3),
     "vcb_debug_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "vcb_debug_gemm_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32]),
     "vcb_debug_attention": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 4 + [C.c_int32] * 7 + [C.c_void_p]),

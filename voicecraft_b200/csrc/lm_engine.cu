@@ -907,6 +907,20 @@ int sample_rows(vcb_engine* e, const Pass& p, const float* noise, const vcb_samp
     return launch_sampler(e, p, noise, sp, st);
 }
 
+SamplingParams sampling_params(const vcb_sampling* sp) {
+    SamplingParams s;
+    s.top_k = sp->top_k;
+    s.top_p = sp->top_p;
+    s.temperature = sp->temperature;
+    s.stop_repetition = sp->stop_repetition;
+    s.n_silence = std::min(sp->n_silence, 8);
+    for (int i = 0; i < 8; ++i) s.silence_tokens[i] = sp->silence_tokens[i];
+    return s;
+}
+
+// dynamic shared memory of sampler_kernel: the top-p sort buffer, then the rank of each of the V entries
+size_t sampler_smem(int V) { return SAMP_SORT_N * 8 + static_cast<size_t>(V) * 4; }
+
 // fused sampler over the pass's rows, one CTA per (row, codebook)
 int launch_sampler(vcb_engine* e, const Pass& p, const float* noise, const vcb_sampling* sp, cudaStream_t st) {
     const ModelDims& m = e->m;
@@ -938,15 +952,9 @@ int launch_sampler(vcb_engine* e, const Pass& p, const float* noise, const vcb_s
     a.eog = m.eog;
     a.eos = m.eos;
     a.encodec_sr = m.encodec_sr;
-    a.sp.top_k = sp->top_k;
-    a.sp.top_p = sp->top_p;
-    a.sp.temperature = sp->temperature;
-    a.sp.stop_repetition = sp->stop_repetition;
-    a.sp.n_silence = std::min(sp->n_silence, 8);
-    for (int i = 0; i < 8; ++i) a.sp.silence_tokens[i] = sp->silence_tokens[i];
-    const size_t dyn = SAMP_SORT_N * 8 + static_cast<size_t>(m.V) * 4;
+    a.sp = sampling_params(sp);
     ProfScope ps(e, PC_SAMPLER, st);
-    VCB_CUDA_OK(launch_k(e, sampler_kernel, dim3(n * m.K), dim3(SAMP_THREADS), dyn, st, a));
+    VCB_CUDA_OK(launch_k(e, sampler_kernel, dim3(n * m.K), dim3(SAMP_THREADS), sampler_smem(m.V), st, a));
     LAUNCH_COUNT(e);
     return 0;
 }
@@ -2003,6 +2011,132 @@ int vcb_debug_exponential(float* out_dev, int64_t numel, uint64_t seed, uint64_t
     debug_exponential_kernel<<<256, 256, 0, static_cast<cudaStream_t>(stream)>>>(out_dev, static_cast<unsigned long long>(numel), seed,
                                                                                    offset, static_cast<unsigned int>(threads));
     VCB_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+// Parity hook of the fused sampler alone: one sampling step of n one-member groups through sampler_kernel; see
+// include/vcb200.h.  Every argument is checked before anything is allocated or launched.
+int vcb_debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t seed, uint64_t offset, int32_t rng_threads,
+                      const vcb_sampling* sp, int32_t n, int32_t K, int32_t V, int32_t empty_token, int32_t eog, int32_t eos,
+                      int32_t encodec_sr, const int32_t* state_host, int32_t* tokens_host, int32_t* state_out_host) {
+    constexpr int D = 32, MAX_Y = 65536, STEPS = 4;
+    if (!logits_dev || !sp || !state_host || !tokens_host || !state_out_host || (!noise_dev && rng_threads < 1)) {
+        set_error("vcb_debug_sampler: null argument (or no noise and rng_threads < 1)");
+        return -1;
+    }
+    if (n < 1 || K < 1 || K > 8 || V < 1 || V > SAMP_MAXV * SAMP_THREADS) {
+        set_error("vcb_debug_sampler: n >= 1, 1 <= K <= 8, 1 <= V <= %d required (n=%d K=%d V=%d)",
+                  SAMP_MAXV * SAMP_THREADS, n, K, V);
+        return -1;
+    }
+    if (empty_token < 0 || empty_token >= V + 2 || eog < 0 || eog >= V + 2 || eos >= V + 2) {
+        set_error("vcb_debug_sampler: special ids must lie in [0, V+2) (eos <= 0: unused)");
+        return -1;
+    }
+    int max_y = 0;
+    for (int i = 0; i < n; ++i) {
+        const int32_t* s = state_host + 7 * i;      // mode, n_eog, cur_num_gen, prev_token, consec, x_len, y_len
+        if ((s[0] != 0 && s[0] != 1) || s[1] < 0 || s[1] >= K || s[5] < 0 || s[6] < 0 || s[6] >= MAX_Y) {
+            set_error("vcb_debug_sampler: row %d: mode in {0, 1}, 0 <= n_eog < K, x_len >= 0, 0 <= y_len < %d required", i,
+                      MAX_Y);
+            return -1;
+        }
+        max_y = std::max(max_y, s[6]);
+    }
+    const int Vpad = (V + 3) & ~3, rows = n * K;
+    DevBuf<float> logits, tables, pe, mask_emb, x_slot;
+    DevBuf<float*> E_audio;
+    DevBuf<int> slots, tok_log;
+    DevBuf<SlotState> st;
+    DevBuf<GroupState> gr;
+    const SyncOnExit sync;
+    if (logits.alloc(static_cast<size_t>(rows) * Vpad) || tables.alloc(static_cast<size_t>(K) * (V + 2) * D, true) ||
+        pe.alloc(static_cast<size_t>(max_y + 1) * D, true) || mask_emb.alloc(8 * D, true) ||
+        x_slot.alloc(static_cast<size_t>(n) * D, true) || E_audio.alloc(K) || slots.alloc(n) ||
+        tok_log.alloc(static_cast<size_t>(n) * STEPS * K, true) || st.alloc(n) || gr.alloc(n))
+        return -1;
+    // the engine's padded layout; pad columns V..Vpad-1 hold 0x70707070 = +2.98e29 (finite after any temperature >= 0.01),
+    // so a kernel that reads past V picks a pad column
+    VCB_CUDA_OK(cudaMemset(logits, 0x70, static_cast<size_t>(rows) * Vpad * sizeof(float)));
+    VCB_CUDA_OK(cudaMemcpy2D(logits, Vpad * sizeof(float), logits_dev, V * sizeof(float), V * sizeof(float), rows,
+                             cudaMemcpyDeviceToDevice));
+    std::vector<float*> ea(K);
+    for (int k = 0; k < K; ++k) ea[k] = tables + static_cast<size_t>(k) * (V + 2) * D;
+    VCB_CUDA_OK(cudaMemcpy(E_audio, ea.data(), K * sizeof(float*), cudaMemcpyHostToDevice));
+    std::vector<int> sl(n);
+    std::vector<SlotState> hs(n);
+    std::vector<GroupState> hg(n);
+    for (int i = 0; i < n; ++i) {
+        const int32_t* s = state_host + 7 * i;
+        sl[i] = i;
+        SlotState& S = hs[i];
+        S = SlotState{};
+        S.x_len = s[5];
+        S.y_len = s[6];
+        S.group = i;
+        S.prev_token = s[3];
+        S.consec = s[4];
+        S.active = 1;
+        GroupState& G = hg[i];
+        G = GroupState{};
+        G.mode = s[0];
+        G.size = 1;
+        G.n_eog = s[1];
+        G.cur_num_gen = s[2];
+        G.keep = -1;
+        G.first_slot = i;
+        if (!noise_dev) {
+            G.rng_threads = static_cast<unsigned int>(rng_threads);
+            G.seed_lo = static_cast<unsigned int>(seed);
+            G.seed_hi = static_cast<unsigned int>(seed >> 32);
+            G.off_lo = static_cast<unsigned int>(offset);
+            G.off_hi = static_cast<unsigned int>(offset >> 32);
+        }
+    }
+    VCB_CUDA_OK(cudaMemcpy(slots, sl.data(), n * sizeof(int), cudaMemcpyHostToDevice));
+    VCB_CUDA_OK(cudaMemcpy(st, hs.data(), n * sizeof(SlotState), cudaMemcpyHostToDevice));
+    VCB_CUDA_OK(cudaMemcpy(gr, hg.data(), n * sizeof(GroupState), cudaMemcpyHostToDevice));
+    SamplerArgs a;
+    a.slots = slots;
+    a.row_forced = nullptr;
+    a.n = n;
+    a.st = st;
+    a.gr = gr;
+    a.logits = logits;
+    a.ldl = K * Vpad;
+    a.noise = noise_dev;
+    a.dbg_logits = nullptr;
+    a.tok_log = tok_log;
+    a.max_steps = STEPS;
+    a.max_seq = 1 << 30;
+    a.x_slot = x_slot;
+    a.E_audio = E_audio;
+    a.mask_emb = mask_emb;
+    a.pe = pe;
+    a.alpha_a = 1.f;
+    a.d = D;
+    a.K = K;
+    a.V = V;
+    a.Vpad = Vpad;
+    a.empty_token = empty_token;
+    a.eog = eog;
+    a.eos = eos > 0 ? eos : -1;
+    a.encodec_sr = encodec_sr;
+    a.sp = sampling_params(sp);
+    sampler_kernel<<<rows, SAMP_THREADS, sampler_smem(V)>>>(a);
+    VCB_CUDA_OK(cudaGetLastError());
+    std::vector<int> toks(static_cast<size_t>(n) * STEPS * K);
+    VCB_CUDA_OK(cudaMemcpy(toks.data(), tok_log, toks.size() * sizeof(int), cudaMemcpyDeviceToHost));
+    VCB_CUDA_OK(cudaMemcpy(hs.data(), st, n * sizeof(SlotState), cudaMemcpyDeviceToHost));
+    VCB_CUDA_OK(cudaMemcpy(hg.data(), gr, n * sizeof(GroupState), cudaMemcpyDeviceToHost));
+    for (int i = 0; i < n; ++i) {
+        for (int k = 0; k < K; ++k) tokens_host[i * K + k] = toks[static_cast<size_t>(i) * STEPS * K + k];
+        int32_t* o = state_out_host + 4 * i;
+        o[0] = hs[i].prev_token;
+        o[1] = hs[i].consec;
+        o[2] = hg[i].n_eog;
+        o[3] = hg[i].done;
+    }
     return 0;
 }
 

@@ -1039,8 +1039,11 @@ __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const SamplerArgs
 #pragma unroll
         for (int j = 0; j < SAMP_MAXV; ++j) {
             const int v = tid + j * SAMP_THREADS;
-            if (v < V)   // descending by value; ties -> lower index first
-                sort_buf[v] = (static_cast<unsigned long long>(f2key(l[j])) << 32) | static_cast<uint32_t>(0xffffffffu - v);
+            // descending by value; ties -> lower index first.  -0.0 is keyed as +0.0: f2key orders it strictly below +0.0,
+            // which would rank a +0.0 at a higher index ahead of an equal -0.0
+            if (v < V)
+                sort_buf[v] = (static_cast<unsigned long long>(f2key(l[j] == 0.f ? 0.f : l[j])) << 32) |
+                              static_cast<uint32_t>(0xffffffffu - v);
         }
         __syncthreads();
         for (int size = 2; size <= SAMP_SORT_N; size <<= 1) {
