@@ -34,6 +34,7 @@ namespace vcb {
 
 static constexpr int GEMM_BM = 128;   // output features per CTA (2 x wgmma M)
 static constexpr int GEMM_BK = 64;    // K elements per pipeline stage (= 128 B of bf16 = one swizzle row)
+static constexpr int GEMM_MAX_SPLITS = 16;   // cluster size = K splits
 // threads per CTA: warpgroup 0 (w0 TMA), then one MMA + epilogue warpgroup; tiles with >= 64 token rows get a second one:
 // each then multiplies 64 of the 128 features (accumulators: Bpad registers per thread) and takes half of the rows in
 // the epilogue (the epilogue, not the weight stream, dominates those launches)
@@ -50,6 +51,18 @@ struct GemmSmem {
     static constexpr int BAR_OFFSET = RED_OFFSET + RED_BYTES;
     static constexpr int TOTAL = BAR_OFFSET + (2 * STAGES + 1) * 8;           // full[S] empty[S] red_full
 };
+
+// Pipeline stages for `bpad` token rows: 4 (64 KB of weight tiles in flight per CTA), fewer only where 4 do not fit into
+// the 227 KB of shared memory a block may opt in to on sm_90 (bpad 128: 3).  Measured on the H100 (DESIGN.md section
+// 4.1): at bpad 32 deeper pipelines (6, 8) allow one CTA per SM instead of two and gain nothing once the split count
+// follows that; at bpad 64, 4 stages beat 3 on every decode shape.
+constexpr int gemm_stages(int bpad) {
+    int s = 4;
+    while (s > 2 && s * (GEMM_BM + 2 * bpad) * GEMM_BK * 2 + bpad * GEMM_BM * 4 + (2 * s + 1) * 8 > 227 * 1024) --s;
+    return s;
+}
+static_assert(GemmSmem<64, gemm_stages(32)>::TOTAL <= 227 * 1024 && GemmSmem<256, gemm_stages(128)>::TOTAL <= 227 * 1024,
+              "gemm_stages and GemmSmem disagree on the shared memory footprint");
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
@@ -614,29 +627,70 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_
     return 0;
 }
 
+// Co-residency of one instantiation, from the occupancy API: clusters[i] = clusters of 2^i CTAs the device can hold at
+// once, 0 where it cannot place one (a cluster of 16 is non-portable: all of its CTAs must fit into one GPC at once).
+struct GemmOccupancy {
+    int clusters[5] = {};       // cluster sizes 1, 2, 4, 8, 16
+    int max_cluster = 0;        // largest size it can place; 0: the queries failed (error set)
+};
+
+// Queried once per instantiation, after opting in to its shared memory and to non-portable cluster sizes.
 template <int BN, int STAGES>
-static int launch_one(const GemmCall& g, cudaStream_t st) {
+static const GemmOccupancy& occupancy() {
+    static GemmOccupancy occ;
+    if (occ.max_cluster) return occ;
     using L = GemmSmem<BN, STAGES>;
-    static bool attr_set = false;
-    if (!attr_set) {
-        VCB_CUDA_OK(cudaFuncSetAttribute(gemm_w_xT_cluster<BN, STAGES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         L::TOTAL));
-        attr_set = true;
-        if (getenv("VCB_DEBUG_OCC")) {
-            int nb = 0;
-            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, gemm_w_xT_cluster<BN, STAGES>, gemm_threads(BN), L::TOTAL);
-            fprintf(stderr, "[vcb] gemm<%d,%d>: %d B smem, %d CTAs/SM (occupancy API)\n", BN, STAGES, L::TOTAL, nb);
-        }
+    const auto kern = gemm_w_xT_cluster<BN, STAGES>;
+    cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
+    if (err == cudaSuccess) err = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    if (err != cudaSuccess) {
+        set_error("gemm<%d,%d>: cudaFuncSetAttribute: %s", BN, STAGES, cudaGetErrorString(err));
+        return occ;
     }
+    GemmOccupancy q;
+    for (int i = 0; i < 5; ++i) {
+        cudaLaunchAttribute at;
+        at.id = cudaLaunchAttributeClusterDimension;
+        at.val.clusterDim.x = 1 << i;
+        at.val.clusterDim.y = 1;
+        at.val.clusterDim.z = 1;
+        cudaLaunchConfig_t cfg = {};
+        cfg.gridDim = dim3(1 << i);
+        cfg.blockDim = dim3(gemm_threads(BN));
+        cfg.dynamicSmemBytes = L::TOTAL;
+        cfg.attrs = &at;
+        cfg.numAttrs = 1;
+        int n = 0;
+        if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) {
+            (void)cudaGetLastError();       // a size the device rejects outright counts as "cannot be placed"
+            n = 0;
+        }
+        if (n < 1) break;
+        q.clusters[i] = n;
+        q.max_cluster = 1 << i;
+    }
+    if (!q.max_cluster) {
+        set_error("gemm<%d,%d>: the occupancy API places no CTA of %d B shared memory", BN, STAGES, L::TOTAL);
+        return occ;
+    }
+    if (getenv("VCB_DEBUG_OCC"))
+        fprintf(stderr, "[vcb] gemm<%d,%d>: %d B smem, resident clusters of 1/2/4/8/16: %d %d %d %d %d (occupancy API)\n",
+                BN, STAGES, L::TOTAL, q.clusters[0], q.clusters[1], q.clusters[2], q.clusters[3], q.clusters[4]);
+    return occ = q;
+}
+
+template <int BN, int STAGES>
+static int launch_one(const GemmCall& g, int splits, cudaStream_t st) {
+    using L = GemmSmem<BN, STAGES>;
     const int tiles = (g.Nout + GEMM_BM - 1) / GEMM_BM;
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(tiles * g.splits, g.grp.tmA ? g.groups : 1, 1);
+    cfg.gridDim = dim3(tiles * splits, g.grp.tmA ? g.groups : 1, 1);
     cfg.blockDim = dim3(gemm_threads(BN));
     cfg.dynamicSmemBytes = L::TOTAL;
     cfg.stream = st;
     cudaLaunchAttribute at[2];
     at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = g.splits;
+    at[0].val.clusterDim.x = splits;
     at[0].val.clusterDim.y = 1;
     at[0].val.clusterDim.z = 1;
     at[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -644,9 +698,61 @@ static int launch_one(const GemmCall& g, cudaStream_t st) {
     cfg.attrs = at;
     cfg.numAttrs = g.pdl ? 2 : 1;
     const int total_kb = g.Kdim / GEMM_BK;
-    const int kbps = (total_kb + g.splits - 1) / g.splits;
+    const int kbps = (total_kb + splits - 1) / splits;
     VCB_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_w_xT_cluster<BN, STAGES>, *g.tmA, *g.tmB, g.ep, g.Nout, total_kb, kbps,
                                    g.b_col_off, g.nvalid, g.pf_ptr, static_cast<unsigned long long>(g.pf_bytes), g.grp));
+    return 0;
+}
+
+struct GemmVariant {
+    const GemmOccupancy& (*occupancy)() = nullptr;
+    int (*launch)(const GemmCall&, int, cudaStream_t) = nullptr;
+};
+template <int BN, int STAGES>
+static GemmVariant variant() {
+    return {occupancy<BN, STAGES>, launch_one<BN, STAGES>};
+}
+
+// The kernel for `bpad` token rows (2 * bpad hi/lo activation rows per tile); empty for any other padding.
+static GemmVariant find_variant(int bpad) {
+    switch (bpad) {
+        case 16: return variant<32, gemm_stages(16)>();
+        case 32: return variant<64, gemm_stages(32)>();
+        case 64: return variant<128, gemm_stages(64)>();
+        case 128: return variant<256, gemm_stages(128)>();
+        default: return {};
+    }
+}
+
+// A split count the kernel can run: a power of two <= 16 that leaves each CTA of the cluster two or more token rows (the
+// reduce-scatter sends pairs of adjacent rows to one owner) and at least one k-block.
+static bool splits_legal(int s, int bpad, int total_kb) {
+    return s >= 1 && s <= GEMM_MAX_SPLITS && !(s & (s - 1)) && bpad % s == 0 && bpad / s >= 2 &&
+           (s - 1) * ((total_kb + s - 1) / s) < total_kb;
+}
+
+int gemm_launch_shape(const GemmCall& g, int cluster_cap, int& splits, int& stages) {
+    if (g.Kdim % GEMM_BK != 0 || g.Kdim <= 0) {
+        set_error("gemm: K=%d not a positive multiple of %d", g.Kdim, GEMM_BK);
+        return -1;
+    }
+    const GemmVariant v = find_variant(g.bpad);
+    if (!v.launch) {
+        set_error("gemm: unsupported bpad %d", g.bpad);
+        return -1;
+    }
+    const int total_kb = g.Kdim / GEMM_BK;
+    if (!splits_legal(g.splits, g.bpad, total_kb)) {
+        set_error("gemm: bad split count %d for %d k-blocks, bpad %d", g.splits, total_kb, g.bpad);
+        return -1;
+    }
+    int placeable = v.occupancy().max_cluster;
+    if (!placeable) return -1;
+    if (cluster_cap > 0) placeable = std::min(placeable, cluster_cap);
+    // a cluster the device cannot place falls back to the largest that it can: halving keeps the split count legal
+    splits = g.splits;
+    while (splits > placeable) splits /= 2;
+    stages = gemm_stages(g.bpad);
     return 0;
 }
 
@@ -666,36 +772,32 @@ int gemm_launch(const GemmCall& g, cudaStream_t st) {
         }
         return 0;
     }
-    const int total_kb = g.Kdim / GEMM_BK;
-    const int kbps = (total_kb + g.splits - 1) / g.splits;
-    // (g.bpad / g.splits >= 2: the reduce-scatter sends pairs of adjacent token rows to one owner)
-    if (g.splits < 1 || g.splits > 8 || (g.splits & (g.splits - 1)) || g.bpad % g.splits || g.bpad / g.splits < 2 ||
-        (g.splits - 1) * kbps >= total_kb) {
-        set_error("gemm: bad split count %d for %d k-blocks, bpad %d", g.splits, total_kb, g.bpad);
-        return -1;
-    }
-    switch (g.bpad) {
-        case 16: return launch_one<32, 4>(g, st);
-        case 32:
-            if (g.stages == 2) return launch_one<64, 2>(g, st);
-            if (g.stages == 3) return launch_one<64, 3>(g, st);
-            if (g.stages == 6) return launch_one<64, 6>(g, st);
-            if (g.stages == 8) return launch_one<64, 8>(g, st);
-            return launch_one<64, 4>(g, st);     // 4 x 24 KB + 16 KB: two CTAs per SM stay resident (PDL overlap)
-        case 64: return launch_one<128, 3>(g, st);
-        case 128: return launch_one<256, 3>(g, st);
-        default: set_error("gemm: unsupported bpad %d", g.bpad); return -1;
-    }
+    int splits = 0, stages = 0;
+    if (gemm_launch_shape(g, 0, splits, stages)) return -1;
+    return find_variant(g.bpad).launch(g, splits, st);
 }
 
-// Cluster size (= K splits), a power of two <= 8: the kernel has a latency floor of several microseconds, so the grid
-// should reach about one CTA per SM in ONE wave of co-resident CTAs (2 per SM) while every split keeps >= 4 k-blocks.
-int gemm_pick_splits(int Nout, int Kdim, int num_sms) {
-    const int tiles = (Nout + GEMM_BM - 1) / GEMM_BM;
-    const int total_kb = Kdim / GEMM_BK;
+// Cluster size (= K splits) of a launch of `groups` x ceil(Nout / 128) tiles.  `room` = CTAs of this kernel the device
+// holds at once (occupancy API).  Measured on the H100 (DESIGN.md section 4.1, scripts/bench_gemm.py), a launch is fastest
+// with about half of `room` in its grid: the weight stream then has enough CTAs pulling HBM, and the next launch in the
+// chain finds room for its CTAs, whose weight loads PDL starts under this launch's tail.  More splits than that cost more
+// in the reduce-scatter and in the successor's start than the shorter K slice gains.  So: the most splits whose grid fits
+// in room / 2; then one doubling more if that grid fills less than 3/4 of room / 2 (or the split is 1, which streams the
+// whole K per CTA), as long as the doubled grid still runs as one wave of co-resident clusters.
+int gemm_pick_splits(int Nout, int Kdim, int bpad, int groups) {
+    const GemmVariant v = find_variant(bpad);
+    if (!v.launch) return 1;                                        // (gemm_launch reports the padding)
+    const GemmOccupancy& occ = v.occupancy();
+    if (!occ.max_cluster) return 1;
+    const int clusters = (Nout + GEMM_BM - 1) / GEMM_BM * std::max(1, groups);
+    const int total_kb = Kdim / GEMM_BK, half = occ.clusters[0] / 2;
+    auto fits = [&](int s) {                // legal, placeable, and one wave
+        const int i = 31 - __builtin_clz(s);
+        return s <= occ.max_cluster && splits_legal(s, bpad, total_kb) && occ.clusters[i] >= clusters;
+    };
     int s = 1;
-    while (s < 8 && tiles * s < num_sms && total_kb / (2 * s) >= 4) s *= 2;
-    while (s > 1 && (s - 1) * ((total_kb + s - 1) / s) >= total_kb) s /= 2;
+    while (fits(2 * s) && clusters * 2 * s <= half) s *= 2;
+    if ((s == 1 || 4 * clusters * s < 3 * half) && fits(2 * s)) s *= 2;
     return s;
 }
 

@@ -120,7 +120,7 @@ struct vcb_engine {
     Event stage_ev;
 
     std::vector<std::array<int, 3>> opt_splits;
-    int opt_simt = 0, opt_pdl = 0, opt_profile = 0, opt_gemm_maxctas = 0, opt_gemm_stages = 0, opt_prefetch = 0, opt_att_balance = 1;
+    int opt_simt = 0, opt_pdl = 0, opt_profile = 0, opt_prefetch = 0, opt_att_balance = 1;
     // wide prefill (gemm_rows.cu): up to wide_rows prompt rows per pass through the layers, own activation planes;
     // opt_prefill_wide = minimum number of prompt rows that takes this path (0: never; VCB_PREFILL_WIDE)
     int opt_prefill_wide = 1, wide_rows = 0;      // 1: every prompt takes the rows-as-M path, so a row's K/V bits do not
@@ -243,19 +243,6 @@ cudaError_t launch_k(vcb_engine* e, void (*kern)(KArgs...), dim3 grid, dim3 bloc
     return launch_k_pdl(e->opt_pdl, kern, grid, block, smem, st, std::forward<Args>(args)...);
 }
 
-// Split count of a decode GEMM from the tile / k-block rule's choice `s`: >= 64 rows take half of it (the per-CTA epilogue /
-// DSMEM exchange grows with the rows, so a smaller cluster pays off -- compare with scripts/bench_gemm.py, which times the
-// decode GEMMs at a given split count), `maxctas` > 0 caps tiles * splits, and the split count divides bpad.
-int decode_splits(int s, int Nout, int bpad, int maxctas) {
-    if (bpad >= 64 && s > 1) s /= 2;
-    if (maxctas > 0) {          // experiment knob: keep every GEMM to one CTA per SM (PDL ping-pong)
-        const int tiles = (Nout + 127) / 128;
-        while (s > 1 && tiles * s > maxctas) s /= 2;
-    }
-    while (s > 1 && bpad % s) s /= 2;
-    return s;
-}
-
 int run_gemm(vcb_engine* e, const Matrix& W, const CUtensorMap* tmB, const __nv_bfloat16* X, int ldx, int bpad,
              int nvalid, int b_col_off, int kdim, const GemmEpilogue& ep, cudaStream_t st, const Matrix* next = nullptr) {
     GemmCall g;
@@ -273,11 +260,9 @@ int run_gemm(vcb_engine* e, const Matrix& W, const CUtensorMap* tmB, const __nv_
     g.Kdim = kdim;
     g.ldx = ldx;
     g.bpad = bpad;
-    int splits = gemm_pick_splits(W.rows, kdim, e->num_sms);
-    for (const auto& o : e->opt_splits)          // experiment knob VCB_SPLITS="<N>x<K>:<S>,..."
-        if (o[0] == W.rows && o[1] == kdim) splits = o[2];
-    g.splits = decode_splits(splits, W.rows, bpad, e->opt_gemm_maxctas);
-    g.stages = e->opt_gemm_stages;
+    g.splits = gemm_pick_splits(W.rows, kdim, bpad, 1);
+    for (const auto& o : e->opt_splits)          // experiment knob VCB_SPLITS="<N>x<K>:<S>,...", used as given
+        if (o[0] == W.rows && o[1] == kdim) g.splits = o[2];
     g.b_col_off = b_col_off;
     g.nvalid = nvalid;
     g.pdl = e->opt_pdl;
@@ -879,8 +864,7 @@ int sample_rows(vcb_engine* e, const Pass& p, const float* noise, const vcb_samp
         g.Kdim = m.Hh;
         g.ldx = KH;
         g.bpad = bpad;
-        g.splits = gemm_pick_splits(m.V, m.Hh, e->num_sms / std::max(1, m.K));
-        while (g.splits > 1 && bpad % g.splits) g.splits /= 2;
+        g.splits = gemm_pick_splits(m.V, m.Hh, bpad, m.K);
         g.nvalid = n;
         g.pdl = e->opt_pdl;
         g.grp.tmA = e->d_h2_maps;
@@ -1032,8 +1016,6 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
     e->opt_simt = simt && !strcmp(simt, "simt");
     const char* pdl = getenv("VCB_PDL");
     e->opt_pdl = pdl ? atoi(pdl) : 1;
-    if (getenv("VCB_GEMM_MAXCTAS")) e->opt_gemm_maxctas = atoi(getenv("VCB_GEMM_MAXCTAS"));
-    if (getenv("VCB_GEMM_STAGES")) e->opt_gemm_stages = atoi(getenv("VCB_GEMM_STAGES"));
     if (getenv("VCB_PREFETCH")) e->opt_prefetch = atoi(getenv("VCB_PREFETCH"));
     if (getenv("VCB_ATT_BALANCE")) e->opt_att_balance = atoi(getenv("VCB_ATT_BALANCE"));
     if (getenv("VCB_PREFILL_WIDE")) e->opt_prefill_wide = atoi(getenv("VCB_PREFILL_WIDE"));
@@ -1655,7 +1637,7 @@ int vcb_debug_gemm(const float* W_dev, const float* X_dev, float* out_dev, int32
     DevBuf<__nv_bfloat16> w, x;
     DevBuf<float> zb;
     const SyncOnExit sync;
-    if (splits <= 0) splits = decode_splits(gemm_pick_splits(N, Kd, hook_num_sms()), N, bpad, 0);
+    if (splits <= 0) splits = gemm_pick_splits(N, Kd, bpad, 1);
     if (w.alloc(packed_weight_elems(N, Kd), true) || x.alloc(static_cast<size_t>(2 * bpad) * Kd, true) || zb.alloc(N, true))
         return -1;
     CUtensorMap tmA, tmB;
@@ -1808,7 +1790,7 @@ int vcb_debug_fold_chain(const float* x_dev, const float* a_dev, const float* W1
         set_error("vcb_debug_fold_chain: 1 <= B <= 128, d %% 128 == 0, 128 <= d <= 4096, N2 >= 1 required");
         return -1;
     }
-    const int bpad = bpad_for(B), dtiles = d / 128, num_sms = hook_num_sms();
+    const int bpad = bpad_for(B), dtiles = d / 128;
     DevBuf<__nv_bfloat16> w1, w2, act_a, act_2, act_f;
     DevBuf<float> stats, cvec, bprime;
     const SyncOnExit sync;
@@ -1824,7 +1806,7 @@ int vcb_debug_fold_chain(const float* x_dev, const float* a_dev, const float* W1
     VCB_CUDA_OK(cudaMemcpy(xnew_dev, x_dev, static_cast<size_t>(B) * d * sizeof(float), cudaMemcpyDeviceToDevice));
     if (make_tmap_bf16_2d(&tmA, act_a, 2 * bpad, d, d, 2 * bpad) || make_tmap_bf16_2d(&tm2B, act_2, 2 * bpad, d, d, 2 * bpad))
         return -1;
-    auto pick = [&](int s, int Nout) { return s > 0 ? s : decode_splits(gemm_pick_splits(Nout, d, num_sms), Nout, bpad, 0); };
+    auto pick = [&](int s, int Nout) { return s > 0 ? s : gemm_pick_splits(Nout, d, bpad, 1); };
     // out-projection + residual: x_new = x + a W1^T + b1 (fold: also gamma * x_new as hi/lo rows + per-tile row statistics)
     GemmCall g1;
     g1.tmA = &tm1; g1.tmB = &tmA; g1.W = w1; g1.X = act_a;
@@ -1885,7 +1867,8 @@ int vcb_debug_gemm_rows(const float* W_dev, const float* X_dev, float* out_dev, 
 }
 
 // Micro-benchmark of the production GEMM alone: `iters` back-to-back launches rotating over `ncopies` weight buffers
-// (so the stream is HBM-, not L2-resident); returns the average microseconds per launch.
+// (so the stream is HBM-, not L2-resident); returns the average microseconds per launch.  `stages` > 0 must name the
+// pipeline depth the kernel for B rows is built with.
 int vcb_bench_gemm(int32_t N, int32_t Kd, int32_t B, int32_t splits, int32_t stages, int32_t pdl, int32_t iters,
                    int32_t ncopies, float* us_out) {
     const int bpad = bpad_for(B);
@@ -1893,8 +1876,9 @@ int vcb_bench_gemm(int32_t N, int32_t Kd, int32_t B, int32_t splits, int32_t sta
     DevBuf<float> zb, out;
     Event a, b;
     const SyncOnExit sync;
-    if (splits <= 0) splits = gemm_pick_splits(N, Kd, hook_num_sms());
-    while (splits > 1 && bpad % splits) splits /= 2;
+    if (splits <= 0) splits = gemm_pick_splits(N, Kd, bpad, 1);
+    int32_t shape[2];
+    if (vcb_gemm_launch_shape(N, Kd, B, splits, stages, 0, shape)) return -1;
     const size_t wn = packed_weight_elems(N, Kd);
     if (w.alloc(wn * ncopies, true) || x.alloc(static_cast<size_t>(2 * bpad) * Kd, true) || zb.alloc(N, true) ||
         out.alloc(static_cast<size_t>(bpad) * N, true) || a.create() || b.create())
@@ -1909,7 +1893,7 @@ int vcb_bench_gemm(int32_t N, int32_t Kd, int32_t B, int32_t splits, int32_t sta
     GemmCall g;
     g.tmB = &tmB; g.X = x;
     g.ep.mode = EPI_LOGITS; g.ep.bias = zb; g.ep.out = out; g.ep.ld_out = N; g.ep.col_off = 0;
-    g.Nout = N; g.Kdim = Kd; g.ldx = Kd; g.bpad = bpad; g.splits = splits; g.nvalid = B; g.stages = stages; g.pdl = pdl;
+    g.Nout = N; g.Kdim = Kd; g.ldx = Kd; g.bpad = bpad; g.splits = splits; g.nvalid = B; g.pdl = pdl;
     for (int it = -3; it < iters; ++it) {
         if (it == 0) cudaEventRecord(a, 0);
         g.tmA = &tmA[(it + 3) % ncopies];
@@ -1921,6 +1905,26 @@ int vcb_bench_gemm(int32_t N, int32_t Kd, int32_t B, int32_t splits, int32_t sta
     float ms = 0.f;
     cudaEventElapsedTime(&ms, a, b);
     *us_out = ms * 1e3f / iters;
+    return 0;
+}
+
+int vcb_gemm_launch_shape(int32_t N, int32_t Kd, int32_t B, int32_t splits, int32_t stages, int32_t cluster_cap,
+                          int32_t* out) {
+    if (B < 1 || B > 128 || N < 1 || !out) {
+        set_error("vcb_gemm_launch_shape: 1 <= B <= 128, N >= 1 and an output array required");
+        return -1;
+    }
+    GemmCall g;
+    g.Nout = N; g.Kdim = Kd; g.ldx = Kd; g.bpad = bpad_for(B); g.nvalid = B;
+    g.splits = splits > 0 ? splits : gemm_pick_splits(N, Kd, g.bpad, 1);
+    int s = 0, st = 0;
+    if (gemm_launch_shape(g, cluster_cap, s, st)) return -1;
+    if (stages > 0 && stages != st) {
+        set_error("gemm: no kernel built with %d stages for bpad %d (it has %d)", stages, g.bpad, st);
+        return -1;
+    }
+    out[0] = s;
+    out[1] = st;
     return 0;
 }
 

@@ -274,13 +274,16 @@ struct GemmCall {
     const __nv_bfloat16* X = nullptr;
     GemmEpilogue ep;
     int Nout = 0, Kdim = 0, ldx = 0, bpad = 0, splits = 1, b_col_off = 0, nvalid = 0;
-    int pdl = 0, simt = 0, stages = 0;
+    int pdl = 0, simt = 0;
     GemmGroup grp;
     int groups = 1;
     const void* pf_ptr = nullptr;       // next GEMM's weights: prefetched into L2 while this kernel runs
     size_t pf_bytes = 0;
 };
 int gemm_launch(const GemmCall& g, cudaStream_t st);
+// What gemm_launch would launch for g: the pipeline stages and the split count after the fallback to the largest cluster
+// the device can place (cluster_cap > 0: as if it could place none larger).  -1 (and the error) where gemm_launch rejects g.
+int gemm_launch_shape(const GemmCall& g, int cluster_cap, int& splits, int& stages);
 
 // Rows-as-M GEMM for prefill (gemm_rows.cu): activations [2][rcap][Kdim] (hi plane, lo plane), packed weights as above.
 struct RowsGemmCall {
@@ -291,7 +294,8 @@ struct RowsGemmCall {
 };
 bool gemm_rows_supported(int Nout, int Kdim, int hd);
 int gemm_rows_launch(const RowsGemmCall& g, cudaStream_t st);
-int gemm_pick_splits(int Nout, int Kdim, int num_sms);
+// split count (= cluster size) of a decode GEMM launch of `groups` x Nout x Kdim at bpad token rows
+int gemm_pick_splits(int Nout, int Kdim, int bpad, int groups);
 size_t packed_weight_elems(int N, int Kdim);
 int pack_weight(const float* w_f32_dev, __nv_bfloat16* out, int N, int Kdim, CUtensorMap* tm);
 int ln_fold_vectors(const __nv_bfloat16* Wp, const float* gamma, const float* beta, const float* bias, float* cvec,
