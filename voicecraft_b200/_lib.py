@@ -31,7 +31,12 @@ class vcb_prompt(C.Structure):
     _fields_ = [("slot", C.c_int32), ("n_copies", C.c_int32), ("mode", C.c_int32), ("x_len", C.c_int32),
                 ("text_ids_dev", C.c_void_p), ("y_len", C.c_int32), ("y_tokens_dev", C.c_void_p),
                 ("mask_rows_dev", C.c_void_p), ("n_more_spans", C.c_int32), ("more_mask_rows", C.c_int32 * 8),
-                ("rng_seed", C.c_uint64), ("rng_offset", C.c_uint64), ("rng_threads", C.c_int32), ("rng_reserved", C.c_int32)]
+                ("rng_seed", C.c_uint64), ("rng_offset", C.c_uint64), ("rng_threads", C.c_int32), ("rng_reserved", C.c_int32),
+                ("sampling", C.POINTER(vcb_sampling))]
+
+
+class vcb_edit_source(C.Structure):
+    _fields_ = [("orig_dev", C.c_void_p), ("T", C.c_int32), ("n_spans", C.c_int32), ("spans", (C.c_int32 * 2) * 8)]
 
 
 class vcb_status(C.Structure):
@@ -56,6 +61,9 @@ PROTOTYPES = {
     "vcb_poll_frames": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_int64,
                                   C.c_int64, C.c_void_p, C.POINTER(vcb_status), C.POINTER(C.c_int32), C.POINTER(C.c_int32),
                                   C.c_void_p]),
+    "vcb_poll_frames_ex": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.POINTER(vcb_edit_source),
+                                     C.POINTER(C.c_int32), C.c_int32, C.c_int64, C.c_int64, C.c_void_p, C.POINTER(vcb_status),
+                                     C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p]),
     "vcb_read_tokens": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_void_p]),
     "vcb_release": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "vcb_debug_logits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),

@@ -7,6 +7,7 @@
 
 #include <algorithm>
 #include <array>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -60,6 +61,7 @@ struct vcb_engine {
     std::vector<std::vector<int>> slot_pages;
     std::vector<int> slot_group;      // host mirror: group id per slot (-1 closed)
     std::vector<int> free_groups;
+    std::vector<char> group_sp;       // host mirror: the group was prefilled with its own sampling parameters (sp_tab)
 
     std::map<std::string, DevBuf<float>> f32;     // every loaded fp32 tensor (device)
     std::map<std::string, std::vector<int64_t>> shapes;
@@ -92,11 +94,13 @@ struct vcb_engine {
     DevBuf<int> row_forced;           // decode steps: SlotState::forced per row as of step_prep (sampler snapshot)
     DevBuf<int> row_pages;            // decode steps: per-row copy of the slot's page list [rows][max_pages_per_slot]
     std::vector<char> slot_rng;       // host mirror: the slot's group generates its own sampling noise
-    std::vector<char> slot_edit;      // host mirror: the slot decodes an edit prompt
+    std::vector<char> slot_edit;      // host mirror: masked spans of the slot's edit prompt (0: a TTS prompt)
     std::vector<int> slot_copies;     // host mirror: n_copies of the slot's prompt (best-of-N group size)
     std::vector<int> slot_final;      // final frames vcb_poll_frames last reported for the slot (they only grow)
     DevBuf<PollFramesRec> pf_rec;     // vcb_poll_frames results [max_slots]
     PinnedBuf<PollFramesRec> h_pf_rec;
+    DevBuf<vcb_edit_source> pf_src;   // vcb_poll_frames_ex sources [max_slots], staged through h_pf_src
+    PinnedBuf<vcb_edit_source> h_pf_src;
     int64_t n_poll_frames = 0;
     DevBuf<int> all_rows;             // prefill row tables: 5 arrays of all_rows_cap ints (seq, pos, slot, last, page)
     size_t all_rows_cap = 0;
@@ -113,6 +117,7 @@ struct vcb_engine {
     DevBuf<float> dbg_logits;
     DevBuf<SlotState> st;
     DevBuf<GroupState> gr;
+    DevBuf<SamplingParams> sp_tab;    // [max_slots] by group id: parameters of the groups prefilled with their own
     DevBuf<EmbedSeq> d_seqs;
     // pinned staging
     PinnedBuf<int> h_stage;
@@ -795,7 +800,8 @@ int mega_step(vcb_engine* e, int n, cudaStream_t st) {
     return mega_launch(a, e->mega_grid, st);
 }
 
-int upload_slots(vcb_engine* e, const int32_t* slots, int n, cudaStream_t st) {
+// the slot list of a sampling call: 1..MAX_ROWS open slots
+int check_slots(vcb_engine* e, const int32_t* slots, int n) {
     if (n < 1 || n > vcb_engine::MAX_ROWS || n > e->cfg.max_slots) {
         set_error("bad slot count %d", n);
         return -1;
@@ -805,6 +811,11 @@ int upload_slots(vcb_engine* e, const int32_t* slots, int n, cudaStream_t st) {
             set_error("slot %d is not open", slots[i]);
             return -1;
         }
+    return 0;
+}
+
+// uploads a slot list check_slots accepted
+int upload_slots(vcb_engine* e, const int32_t* slots, int n, cudaStream_t st) {
     if (static_cast<int>(e->last_slots.size()) == n && std::equal(slots, slots + n, e->last_slots.begin())) return 0;
     e->last_slots.assign(slots, slots + n);
     // row groups: runs of consecutive rows on consecutive slots of one best-of-N group with shared pages, at most
@@ -836,6 +847,18 @@ int noise_required(vcb_engine* e, const int32_t* slots, int n, const float* nois
     for (int i = 0; i < n; ++i)
         if (!e->slot_rng[slots[i]]) {
             set_error("slot %d has no device generator (vcb_prompt.rng_threads == 0): exp_noise_dev must not be null", slots[i]);
+            return -1;
+        }
+    return 0;
+}
+
+// sp may be null only if every listed slot's group was prefilled with its own parameters (vcb_prompt::sampling)
+int sampling_required(vcb_engine* e, const int32_t* slots, int n, const vcb_sampling* sp) {
+    if (sp) return 0;
+    for (int i = 0; i < n; ++i)
+        if (!e->group_sp[e->slot_group[slots[i]]]) {
+            set_error("slot %d has no sampling parameters of its own (vcb_prompt.sampling == NULL): sp must not be null",
+                      slots[i]);
             return -1;
         }
     return 0;
@@ -936,7 +959,10 @@ int launch_sampler(vcb_engine* e, const Pass& p, const float* noise, const vcb_s
     a.eog = m.eog;
     a.eos = m.eos;
     a.encodec_sr = m.encodec_sr;
-    a.sp = sampling_params(sp);
+    if (sp)
+        a.sp = sampling_params(sp);
+    else
+        a.sp_tab = e->sp_tab;
     ProfScope ps(e, PC_SAMPLER, st);
     VCB_CUDA_OK(launch_k(e, sampler_kernel, dim3(n * m.K), dim3(SAMP_THREADS), sampler_smem(m.V), st, a));
     LAUNCH_COUNT(e);
@@ -1005,6 +1031,7 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
     e->slot_group.assign(cfg->max_slots, -1);
     e->slot_rng.assign(cfg->max_slots, 0);
     e->slot_edit.assign(cfg->max_slots, 0);
+    e->group_sp.assign(cfg->max_slots, 0);
     e->slot_copies.assign(cfg->max_slots, 0);
     e->slot_shared.assign(cfg->max_slots, 0);
     e->slot_final.assign(cfg->max_slots, 0);
@@ -1167,7 +1194,8 @@ int vcb_finalize_weights(vcb_engine* e) {
         e->row_forced.ensure(R, true) || e->row_pages.ensure(R * e->max_pages_per_slot, true) || e->d_slots.ensure(3 * R + 1, true) ||
         e->page_table.ensure(S * e->max_pages_per_slot, true) || e->tok_log.ensure(S * e->cfg.max_new_tokens * m.K, true) ||
         e->dbg_logits.ensure(R * m.K * m.V, true) || e->st.ensure(S, true) || e->gr.ensure(S, true) ||
-        e->d_seqs.ensure(S, true) || e->pf_rec.ensure(S, true) || e->h_pf_rec.ensure(S) ||
+        e->d_seqs.ensure(S, true) || e->pf_rec.ensure(S, true) || e->h_pf_rec.ensure(S) || e->sp_tab.ensure(S, true) ||
+        e->pf_src.ensure(S, true) || e->h_pf_src.ensure(S) ||
         e->all_rows.ensure(5 * e->all_rows_cap, true) || e->h_stage.ensure(e->h_stage_ints) || e->d_fork.ensure(S, true) ||
         e->d_pools.ensure(2 * m.L, true))
         return -1;
@@ -1209,6 +1237,7 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
     std::vector<int> sst_slot;
     std::vector<GroupState> gst;
     std::vector<int> gst_id;
+    std::vector<std::pair<int, SamplingParams>> gsp;   // (group id, parameters) of the groups prefilled with their own
     std::vector<ForkPair> fork;
     // ---- validate everything before touching host or device state (a failed call must leave no slot, group or page held)
     {
@@ -1222,6 +1251,15 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
                 set_error("prompt %d: bad slot/length (slot=%d copies=%d x_len=%d y_len=%d max_seq_len=%d more_spans=%d; at most "
                           "8 spans per utterance)", i, P.slot, P.n_copies, P.x_len, P.y_len, e->cfg.max_seq_len, P.n_more_spans);
                 return -1;
+            }
+            if (const vcb_sampling* q = P.sampling) {
+                if (q->n_silence < 0 || q->n_silence > 8 || !std::isfinite(q->temperature) || !(q->temperature > 0.f) ||
+                    std::isnan(q->top_p)) {
+                    set_error("prompt %d: bad sampling parameters (n_silence=%d in [0, 8], temperature=%g finite and > 0, "
+                              "top_p=%g not NaN)", i, q->n_silence, static_cast<double>(q->temperature),
+                              static_cast<double>(q->top_p));
+                    return -1;
+                }
             }
             for (int c = 0; c < P.n_copies; ++c) {
                 if (e->slot_group[P.slot + c] >= 0 || claimed[P.slot + c]) {
@@ -1272,6 +1310,8 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
         G.off_hi = static_cast<unsigned int>(P.rng_offset >> 32);
         gst.push_back(G);
         gst_id.push_back(gid);
+        e->group_sp[gid] = P.sampling != nullptr;
+        if (P.sampling) gsp.emplace_back(gid, sampling_params(P.sampling));
         EmbedSeq es;
         es.text_ids = reinterpret_cast<const long long*>(P.text_ids_dev);
         es.y_tokens = reinterpret_cast<const long long*>(P.y_tokens_dev);
@@ -1285,7 +1325,7 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
             const int slot = P.slot + c;
             e->slot_group[slot] = gid;
             e->slot_rng[slot] = P.rng_threads != 0;
-            e->slot_edit[slot] = P.mode == VCB_MODE_EDIT;
+            e->slot_edit[slot] = static_cast<char>(P.mode == VCB_MODE_EDIT ? P.n_more_spans + 1 : 0);
             e->slot_copies[slot] = P.n_copies;
             e->slot_shared[slot] = P.n_copies > 1 ? shared : 0;
             e->slot_final[slot] = 0;
@@ -1336,6 +1376,8 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
     }
     for (size_t i = 0; i < gst.size(); ++i)
         VCB_CUDA_OK(cudaMemcpy(e->gr + gst_id[i], &gst[i], sizeof(GroupState), cudaMemcpyHostToDevice));
+    for (const auto& g : gsp)
+        VCB_CUDA_OK(cudaMemcpy(e->sp_tab + g.first, &g.second, sizeof(SamplingParams), cudaMemcpyHostToDevice));
     VCB_CUDA_OK(cudaMemcpy(e->d_seqs, seqs.data(), seqs.size() * sizeof(EmbedSeq), cudaMemcpyHostToDevice));
     if (!fork.empty())
         VCB_CUDA_OK(cudaMemcpy(e->d_fork, fork.data(), fork.size() * sizeof(ForkPair), cudaMemcpyHostToDevice));
@@ -1395,13 +1437,14 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
 int vcb_sample(vcb_engine* e, const int32_t* slots, int32_t n, const float* exp_noise_dev, const vcb_sampling* sp,
                void* stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (!e || !e->finalized || !slots || !sp) {
+    if (!e || !e->finalized || !slots) {
         set_error("vcb_sample: bad argument");
         return -1;
     }
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
-    if (upload_slots(e, slots, n, st)) return -1;
-    if (noise_required(e, slots, n, exp_noise_dev)) return -1;
+    if (check_slots(e, slots, n) || noise_required(e, slots, n, exp_noise_dev) || sampling_required(e, slots, n, sp) ||
+        upload_slots(e, slots, n, st))
+        return -1;
     Pass p = narrow_pass(e, n, false);
     p.x = e->h_slot;
     p.x_index = e->d_slots;
@@ -1411,13 +1454,14 @@ int vcb_sample(vcb_engine* e, const int32_t* slots, int32_t n, const float* exp_
 int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float* exp_noise_dev, const vcb_sampling* sp,
                     void* stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (!e || !e->finalized || !slots || !sp) {
+    if (!e || !e->finalized || !slots) {
         set_error("vcb_decode_step: bad argument");
         return -1;
     }
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
-    if (upload_slots(e, slots, n, st)) return -1;
-    if (noise_required(e, slots, n, exp_noise_dev)) return -1;
+    if (check_slots(e, slots, n) || noise_required(e, slots, n, exp_noise_dev) || sampling_required(e, slots, n, sp) ||
+        upload_slots(e, slots, n, st))
+        return -1;
     const bool fold = e->opt_fold && !e->opt_simt;
     Pass p = step_pass(e, n, fold);
     {
@@ -1482,16 +1526,39 @@ int vcb_poll(vcb_engine* e, const int32_t* slots, int32_t n, vcb_status* out, vo
     return 0;
 }
 
-// Streaming: vcb_poll plus each listed slot's newly final frames as codec codes (poll_frames_kernel), behind one wait.
+}  // extern "C"
+
+namespace {
+
+// an edit slot's source: its prompt's span count, spans ascending, not overlapping and inside [0, T]
+int check_edit_source(int slot, int n_spans, const vcb_edit_source& s) {
+    if (!s.orig_dev || s.n_spans < 1 || s.T < 0) {
+        set_error("vcb_poll_frames_ex: slot %d decodes an edit prompt: it needs a source (orig_dev, T, spans)", slot);
+        return -1;
+    }
+    if (s.n_spans != n_spans) {
+        set_error("vcb_poll_frames_ex: slot %d: source has %d spans, the slot's prompt %d", slot, s.n_spans, n_spans);
+        return -1;
+    }
+    for (int j = 0, lo = 0; j < n_spans; lo = s.spans[j][1], ++j)
+        if (s.spans[j][0] < lo || s.spans[j][1] < s.spans[j][0] || s.spans[j][1] > s.T) {
+            set_error("vcb_poll_frames_ex: slot %d: span %d [%d, %d) is not ascending, overlaps or leaves [0, %d]", slot, j,
+                      s.spans[j][0], s.spans[j][1], s.T);
+            return -1;
+        }
+    return 0;
+}
+
+// vcb_poll_frames (src null: edit slots are rejected) and vcb_poll_frames_ex (one source per listed slot).
 // Everything is validated on the host first: `from` may not exceed the final frames this call last reported for the
 // slot, which never exceeds the slot's final frames now (frames only become final).
-int vcb_poll_frames(vcb_engine* e, const int32_t* slots, int32_t n, const int32_t* from_host, int32_t max_frames,
-                    int64_t code_offset, int64_t bins, int64_t* codes_dev, vcb_status* status_host, int32_t* final_host,
-                    int32_t* bad_host, void* stream) {
+int poll_frames(vcb_engine* e, const int32_t* slots, int32_t n, const vcb_edit_source* src, const int32_t* from_host,
+                int32_t max_frames, int64_t code_offset, int64_t bins, int64_t* codes_dev, vcb_status* status_host,
+                int32_t* final_host, int32_t* bad_host, void* stream, const char* fn) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (!e || !e->finalized || !slots || !from_host || !codes_dev || !status_host || !final_host || !bad_host || n < 1 ||
         n > e->cfg.max_slots || max_frames < 1 || bins < 1) {
-        set_error("vcb_poll_frames: bad argument (n=%d, max_frames=%d, bins=%lld)", n, max_frames, static_cast<long long>(bins));
+        set_error("%s: bad argument (n=%d, max_frames=%d, bins=%lld)", fn, n, max_frames, static_cast<long long>(bins));
         return -1;
     }
     for (int i = 0; i < n; ++i) {
@@ -1500,18 +1567,29 @@ int vcb_poll_frames(vcb_engine* e, const int32_t* slots, int32_t n, const int32_
             set_error("slot %d is not open", slot);
             return -1;
         }
-        if (e->slot_edit[slot] || e->slot_copies[slot] != 1) {
-            set_error("vcb_poll_frames: slot %d decodes %s: only single TTS utterances stream", slot,
-                      e->slot_edit[slot] ? "an edit prompt" : "a best-of-N group");
+        if ((e->slot_edit[slot] && !src) || e->slot_copies[slot] != 1) {
+            set_error("%s: slot %d decodes %s: only single TTS utterances stream%s", fn, slot,
+                      e->slot_edit[slot] ? "an edit prompt" : "a best-of-N group",
+                      e->slot_edit[slot] ? " (edits: vcb_poll_frames_ex)" : "");
+            return -1;
+        }
+        if (src && e->slot_edit[slot] && check_edit_source(slot, e->slot_edit[slot], src[i])) return -1;
+        if (src && !e->slot_edit[slot] && (src[i].orig_dev || src[i].n_spans)) {
+            set_error("%s: slot %d decodes a TTS prompt but was given an edit source", fn, slot);
             return -1;
         }
         if (from_host[i] < 0 || from_host[i] > e->slot_final[slot]) {
-            set_error("vcb_poll_frames: slot %d: from %d outside [0, %d], the final frames reported so far", slot, from_host[i],
+            set_error("%s: slot %d: from %d outside [0, %d], the final frames reported so far", fn, slot, from_host[i],
                       e->slot_final[slot]);
             return -1;
         }
     }
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
+    if (src) {          // the previous call's copy finished before it returned: the staging buffer is free
+        memcpy(e->h_pf_src, src, static_cast<size_t>(n) * sizeof(vcb_edit_source));
+        VCB_CUDA_OK(cudaMemcpyAsync(e->pf_src, e->h_pf_src, static_cast<size_t>(n) * sizeof(vcb_edit_source),
+                                    cudaMemcpyHostToDevice, st));
+    }
     const ModelDims& m = e->m;
     PollFramesArgs a;
     a.st = e->st;
@@ -1522,6 +1600,7 @@ int vcb_poll_frames(vcb_engine* e, const int32_t* slots, int32_t n, const int32_
     a.max_steps = e->cfg.max_new_tokens;
     a.K = m.K;
     a.end = m.eos > 0 ? m.eos : m.eog;          // the token that ends a TTS generation in codebook 0
+    a.eog = m.eog;                              // ... and each span of an edit
     a.max_frames = max_frames;
     for (int b = 0; b < n; b += PF_MAX_SLOTS) {
         const int nb = std::min(n - b, PF_MAX_SLOTS);
@@ -1531,12 +1610,13 @@ int vcb_poll_frames(vcb_engine* e, const int32_t* slots, int32_t n, const int32_
         }
         a.codes = reinterpret_cast<long long*>(codes_dev) + static_cast<size_t>(b) * m.K * max_frames;
         a.rec = e->pf_rec + b;
+        a.src = src ? e->pf_src + b : nullptr;
         poll_frames_kernel<<<nb, 256, 0, st>>>(a);
         VCB_CUDA_OK(cudaGetLastError());
         LAUNCH_COUNT(e);
     }
     VCB_CUDA_OK(cudaMemcpyAsync(e->h_pf_rec, e->pf_rec, static_cast<size_t>(n) * sizeof(PollFramesRec), cudaMemcpyDeviceToHost, st));
-    if (sync_or_report(e, cudaStreamSynchronize(st), "vcb_poll_frames")) return -1;
+    if (sync_or_report(e, cudaStreamSynchronize(st), fn)) return -1;
     e->n_poll_frames += 1;
     for (int i = 0; i < n; ++i) {
         const PollFramesRec& r = e->h_pf_rec[i];
@@ -1555,6 +1635,28 @@ int vcb_poll_frames(vcb_engine* e, const int32_t* slots, int32_t n, const int32_
         e->slot_final[slots[i]] = std::max(e->slot_final[slots[i]], r.final_frames);
     }
     return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int vcb_poll_frames(vcb_engine* e, const int32_t* slots, int32_t n, const int32_t* from_host, int32_t max_frames,
+                    int64_t code_offset, int64_t bins, int64_t* codes_dev, vcb_status* status_host, int32_t* final_host,
+                    int32_t* bad_host, void* stream) {
+    return poll_frames(e, slots, n, nullptr, from_host, max_frames, code_offset, bins, codes_dev, status_host, final_host,
+                       bad_host, stream, "vcb_poll_frames");
+}
+
+int vcb_poll_frames_ex(vcb_engine* e, const int32_t* slots, int32_t n, const vcb_edit_source* src, const int32_t* from_host,
+                       int32_t max_frames, int64_t code_offset, int64_t bins, int64_t* codes_dev, vcb_status* status_host,
+                       int32_t* final_host, int32_t* bad_host, void* stream) {
+    if (!src) {
+        set_error("vcb_poll_frames_ex: src is null (one source per listed slot)");
+        return -1;
+    }
+    return poll_frames(e, slots, n, src, from_host, max_frames, code_offset, bins, codes_dev, status_host, final_host,
+                       bad_host, stream, "vcb_poll_frames_ex");
 }
 
 int vcb_read_tokens(vcb_engine* e, int32_t slot, int32_t* out_host, int32_t max_steps, void* stream) {
@@ -1582,8 +1684,10 @@ int vcb_release(vcb_engine* e, int32_t slot, int32_t n_copies) {
         VCB_CUDA_OK(cudaMemset(e->st + s, 0, sizeof(SlotState)));
     }
     // the group id goes back with the last of its slots, whichever call releases it
-    if (gid >= 0 && std::find(e->slot_group.begin(), e->slot_group.end(), gid) == e->slot_group.end())
+    if (gid >= 0 && std::find(e->slot_group.begin(), e->slot_group.end(), gid) == e->slot_group.end()) {
         e->free_groups.push_back(gid);
+        e->group_sp[gid] = 0;
+    }
     return 0;
 }
 

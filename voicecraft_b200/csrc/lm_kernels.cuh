@@ -2,6 +2,7 @@
 // All of them are HBM/L2-bound integer or fp32 work: coalesced 16-byte accesses, warp-level reductions,
 // TMA bulk copies for the paged KV cache.  Included only by lm_engine.cu.
 #pragma once
+#include "../../include/vcb200.h"
 #include "vcb_internal.h"
 
 namespace vcb {
@@ -821,15 +822,16 @@ struct SamplerArgs {
     int d, K, V, Vpad;
     int empty_token, eog, eos, encodec_sr;
     SamplingParams sp;
+    const SamplingParams* sp_tab = nullptr;   // [max_slots] by group id: each slot samples with its group's parameters; null: `sp`
 };
 
 static constexpr int SAMP_THREADS = 256;
 static constexpr int SAMP_MAXV = 12;       // V <= 3072
 static constexpr int SAMP_SORT_N = 4096;
 
-__device__ void sampler_finish_slot(const SamplerArgs& a, int slot, float* sred);
+__device__ void sampler_finish_slot(const SamplerArgs& a, const SamplingParams& sp, int slot, float* sred);
 
-__global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const SamplerArgs a) {
+__global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const __grid_constant__ SamplerArgs a) {
     __shared__ float sred[8];
     __shared__ int sidx[8];
     __shared__ int hist[256];
@@ -883,6 +885,8 @@ __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const SamplerArgs
         return;
     }
 
+    // the group's parameters or the call's; one CTA serves one (utterance, codebook), so the branches on them are uniform
+    const SamplingParams& sp = a.sp_tab ? a.sp_tab[S.group] : a.sp;
     const bool tts = G.mode == 0;
     const int E = tts ? (a.eos > 0 ? a.eos : a.eog) : a.eog;
     const int n_eog = G.n_eog, cur = G.cur_num_gen;
@@ -901,11 +905,11 @@ __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const SamplerArgs
             if (n_eog == 0) {
                 if (k >= 1 && (v == E || v == a.empty_token)) u = -10000.f;                // :1021-1023
                 if (k == 0 && tts && cur <= a.encodec_sr / 5 && v == E) u = -10000.f;     // :1024-1025
-                if (k == 0 && a.sp.stop_repetition > 0 && v == S.prev_token && S.consec > a.sp.stop_repetition) {
+                if (k == 0 && sp.stop_repetition > 0 && v == S.prev_token && S.consec > sp.stop_repetition) {
                     bool sil = false;
-                    for (int t = 0; t < a.sp.n_silence; ++t) sil |= (a.sp.silence_tokens[t] == v);
+                    for (int t = 0; t < sp.n_silence; ++t) sil |= (sp.silence_tokens[t] == v);
                     if (sil) {                                                             // :1027-1031
-                        const float f = static_cast<float>(S.consec - (a.sp.stop_repetition - 1));
+                        const float f = static_cast<float>(S.consec - (sp.stop_repetition - 1));
                         u = (u < 0.f) ? u * f : u / f;
                     }
                 }
@@ -963,15 +967,15 @@ __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const SamplerArgs
     const int argmax_raw = bi;
 
     // ---- temperature (:80-81) -----------------------------------------------------------------------
-    if (a.sp.temperature != 1.0f) {
+    if (sp.temperature != 1.0f) {
 #pragma unroll
-        for (int j = 0; j < SAMP_MAXV; ++j) l[j] = __fdiv_rn(l[j], a.sp.temperature);
-        bm = __fdiv_rn(bm, a.sp.temperature);
+        for (int j = 0; j < SAMP_MAXV; ++j) l[j] = __fdiv_rn(l[j], sp.temperature);
+        bm = __fdiv_rn(bm, sp.temperature);
     }
 
     // ---- top-k: exact k-th largest by 4-pass radix select on order-preserving keys (:38-44) ----------
-    if (a.sp.top_k > 0) {
-        const int kk = min(max(a.sp.top_k, 1), V);
+    if (sp.top_k > 0) {
+        const int kk = min(max(sp.top_k, 1), V);
         if (tid == 0) { s_prefix = 0; s_kleft = kk; }
         for (int pass = 0; pass < 4; ++pass) {
             const int shift = 24 - 8 * pass;
@@ -1033,7 +1037,7 @@ __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const SamplerArgs
     }
 
     // ---- top-p (:46-67): sort descending, softmax, cumulative sum, keep ranks < j0 ---------------------
-    if (a.sp.top_p < 1.0f) {
+    if (sp.top_p < 1.0f) {
         for (int s = tid; s < SAMP_SORT_N; s += SAMP_THREADS) sort_buf[s] = 0ull;   // pads sort last (key 0 < any real key)
         __syncthreads();
 #pragma unroll
@@ -1089,7 +1093,7 @@ __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const SamplerArgs
         for (int j = 0; j < PER; ++j) {
             run += e[j];
             const int rnk = tid * PER + j;
-            if (rnk < V && !(run / total > a.sp.top_p)) cnt++;
+            if (rnk < V && !(run / total > sp.top_p)) cnt++;
         }
         __syncthreads();
         const int j0 = static_cast<int>(block_sum_256(static_cast<float>(cnt), sred) + 0.5f) + 1;   // kept ranks: [0, j0)
@@ -1167,12 +1171,12 @@ __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const SamplerArgs
     __syncthreads();
     if (!s_flag) return;
     __threadfence();
-    sampler_finish_slot(a, slot, sred);
+    sampler_finish_slot(a, sp, slot, sred);
     if (threadIdx.x == 0) tl_mark(0x430);
 }
 
 // Last codebook row of a slot: next input embedding + silence bookkeeping; last slot of a group: group state.
-__device__ void sampler_finish_slot(const SamplerArgs& a, int slot, float* sred) {
+__device__ void sampler_finish_slot(const SamplerArgs& a, const SamplingParams& sp, int slot, float* sred) {
     SlotState& S = a.st[slot];
     GroupState& G = a.gr[S.group];
     const int tid = threadIdx.x, K = a.K;
@@ -1191,7 +1195,7 @@ __device__ void sampler_finish_slot(const SamplerArgs& a, int slot, float* sred)
     if (G.n_eog == 0) {                                                                     // :1047-1051
         const int t0 = toks[0];
         bool sil = false;
-        for (int t = 0; t < a.sp.n_silence; ++t) sil |= (a.sp.silence_tokens[t] == t0);
+        for (int t = 0; t < sp.n_silence; ++t) sil |= (sp.silence_tokens[t] == t0);
         S.consec = (sil && t0 == S.prev_token) ? S.consec + 1 : 0;
         S.prev_token = t0;
     }
@@ -1257,10 +1261,11 @@ __global__ void delay_pattern_kernel(const long long* __restrict__ z, long long*
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Streaming gather (vcb_poll_frames): one block per listed slot.  Frame t is final once the token log holds rows up to
-// t+K-1 and rows[t][0] is not the end token.  Only rows [from, n_steps-K+1) are scanned: the caller's `from` frames are
-// final already.  The new frames are written un-delayed as codec codes [K][max_frames] with zero padding, the first code
-// outside [0, bins) (lowest frame, then codebook) is recorded, and the slot's status is copied next to the result.
+// Streaming gather (vcb_poll_frames / vcb_poll_frames_ex): one block per listed slot.  TTS: frame t is final once the token
+// log holds rows up to t+K-1 and rows[t][0] is not the end token.  Only rows [from, n_steps-K+1) are scanned: the caller's
+// `from` frames are final already.  The new frames are written un-delayed as codec codes [K][max_frames] with zero padding,
+// the first code outside [0, bins) (lowest frame, then codebook) is recorded, and the slot's status is copied next to the
+// result.  An edit slot (a source with n_spans > 0) does the same over its output, see poll_frames_edit.
 // ---------------------------------------------------------------------------------------------------
 constexpr int PF_MAX_SLOTS = 128;          // listed slots per launch (the lists travel as kernel parameters)
 constexpr int PF_NO_BAD = 0x7fffffff;
@@ -1279,13 +1284,113 @@ struct PollFramesArgs {
     const int* tok_log;        // [max_slots][max_steps][K]
     long long* codes;          // [n][K][max_frames], from this launch's first listed slot on
     PollFramesRec* rec;        // [n], same offset
+    const vcb_edit_source* src;   // [n], same offset; null: every listed slot is a TTS slot
     long long code_offset, bins;
-    int max_steps, K, end, max_frames;
+    int max_steps, K, end, eog, max_frames;
 };
+
+// listed slot i's record: its status, its final frames and the first code outside [0, bins) (frame, codebook, entry)
+__device__ void pf_write_rec(const PollFramesArgs& a, int i, const SlotState& S, int fin, int bad_frame, int bad_k,
+                             int bad_tok) {
+    const GroupState& G = a.gr[S.group];
+    PollFramesRec r;
+    r.done = G.done;
+    r.forced = S.forced;
+    r.n_steps = S.n_steps;
+    r.keep = G.keep;
+    r.n_spans_done = G.n_spans_done;
+    for (int j = 0; j < 8; ++j) r.span_ends[j] = G.span_ends[j];
+    r.off_lo = G.off_lo;
+    r.off_hi = G.off_hi;
+    r.final_frames = fin;
+    r.bad_frame = bad_frame;
+    r.bad_k = bad_k;
+    r.bad_tok = bad_tok;
+    a.rec[i] = r;
+}
+
+// Edit slot i.  Its output is y0[:, 0:s1] ++ G1 ++ y0[:, e1:s2] ++ ... ++ GM ++ y0[:, eM:T] (_Prompt.result): piece p is
+// original piece p/2 for even p, generated span p/2 (un-delayed token-log rows) for odd p.  With d = n_spans_done, the final
+// pieces are those up to original piece d, then the frames of span d that the TTS rule (end token eog) makes final.
+__device__ void poll_frames_edit(const PollFramesArgs& a, int i) {
+    __shared__ int s_end, s_bad, s_np;
+    __shared__ int s_ps[2 * 8 + 2], s_src[2 * 8 + 1];   // first output frame / first y0 column or token-log row of piece p
+    const vcb_edit_source& E = a.src[i];
+    const int slot = a.slots[i], from = a.from[i], K = a.K, tid = threadIdx.x, M = E.n_spans, T = E.T;
+    const SlotState& S = a.st[slot];
+    const GroupState& G = a.gr[S.group];
+    const int n_steps = S.n_steps, d = min(G.n_spans_done, M);
+    const int lo = d > 0 ? G.span_ends[d - 1] : 0;    // first token-log row of span d
+    const int* log = a.tok_log + static_cast<size_t>(slot) * a.max_steps * K;
+    const int m = d < M ? max(0, n_steps - lo - K + 1) : 0;
+    if (tid == 0) {
+        s_end = m;
+        s_bad = PF_NO_BAD;
+    }
+    __syncthreads();
+    for (int t = tid; t < m; t += blockDim.x)
+        if (log[static_cast<size_t>(lo + t) * K] == a.eog) {
+            atomicMin(&s_end, t);
+            break;
+        }
+    __syncthreads();
+    if (tid == 0) {
+        int f = 0, p = 0;
+        for (int j = 0;; ++j) {
+            s_ps[p] = f;
+            s_src[p] = j == 0 ? 0 : E.spans[j - 1][1];
+            f += (j == M ? T : E.spans[j][0]) - s_src[p];
+            ++p;
+            if (j == M) break;
+            const int r0 = j == 0 ? 0 : G.span_ends[j - 1];
+            s_ps[p] = f;
+            s_src[p] = r0;
+            ++p;
+            if (j == d) {
+                f += s_end;
+                break;
+            }
+            f += max(0, G.span_ends[j] - r0 - K);
+        }
+        s_ps[p] = f;
+        s_np = p;
+    }
+    __syncthreads();
+    const int fin = max(s_ps[s_np], from);
+    const int n_new = min(fin - from, a.max_frames);
+    auto entry = [&](int f, int k) -> long long {      // output frame f, codebook k: the y0 or token-log entry
+        int p = 0;
+        while (p + 1 < s_np && s_ps[p + 1] <= f) ++p;
+        const int u = f - s_ps[p] + s_src[p];
+        return (p & 1) ? static_cast<long long>(log[static_cast<size_t>(u + k) * K + k]) : E.orig_dev[static_cast<size_t>(k) * T + u];
+    };
+    long long* out = a.codes + static_cast<size_t>(i) * K * a.max_frames;
+    for (int j = tid; j < K * a.max_frames; j += blockDim.x) {
+        const int k = j / a.max_frames, t = j - k * a.max_frames;
+        long long c = 0;
+        if (t < n_new) {
+            c = entry(from + t, k) - a.code_offset;
+            if (c < 0 || c >= a.bins) atomicMin(&s_bad, t * K + k);
+        }
+        out[j] = c;
+    }
+    __syncthreads();
+    if (tid != 0) return;
+    if (s_bad == PF_NO_BAD) {
+        pf_write_rec(a, i, S, fin, -1, -1, -1);
+    } else {
+        const int t = s_bad / K, k = s_bad - t * K;
+        pf_write_rec(a, i, S, fin, from + t, k, static_cast<int>(entry(from + t, k)));
+    }
+}
 
 __global__ void __launch_bounds__(256) poll_frames_kernel(const __grid_constant__ PollFramesArgs a) {
     __shared__ int s_end, s_bad;
     const int i = blockIdx.x, slot = a.slots[i], from = a.from[i], K = a.K, tid = threadIdx.x;
+    if (a.src && a.src[i].n_spans > 0) {
+        poll_frames_edit(a, i);
+        return;
+    }
     const SlotState& S = a.st[slot];
     const int n_steps = S.n_steps;
     const int* log = a.tok_log + static_cast<size_t>(slot) * a.max_steps * K;
@@ -1315,25 +1420,12 @@ __global__ void __launch_bounds__(256) poll_frames_kernel(const __grid_constant_
     }
     __syncthreads();
     if (tid != 0) return;
-    const GroupState& G = a.gr[S.group];
-    PollFramesRec r;
-    r.done = G.done;
-    r.forced = S.forced;
-    r.n_steps = n_steps;
-    r.keep = G.keep;
-    r.n_spans_done = G.n_spans_done;
-    for (int j = 0; j < 8; ++j) r.span_ends[j] = G.span_ends[j];
-    r.off_lo = G.off_lo;
-    r.off_hi = G.off_hi;
-    r.final_frames = fin;
-    r.bad_frame = r.bad_k = r.bad_tok = -1;
-    if (s_bad != PF_NO_BAD) {
+    if (s_bad == PF_NO_BAD) {
+        pf_write_rec(a, i, S, fin, -1, -1, -1);
+    } else {
         const int t = s_bad / K, k = s_bad - t * K;
-        r.bad_frame = from + t;
-        r.bad_k = k;
-        r.bad_tok = log[static_cast<size_t>(from + t + k) * K + k];
+        pf_write_rec(a, i, S, fin, from + t, k, log[static_cast<size_t>(from + t + k) * K + k]);
     }
-    a.rec[i] = r;
 }
 
 }  // namespace vcb

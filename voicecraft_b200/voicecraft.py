@@ -21,6 +21,7 @@ Out of scope (training): ``forward`` and ``prepare_mask_intervals`` raise NotImp
 import copy
 import ctypes as C
 import logging
+import math
 import os
 import time
 from argparse import Namespace
@@ -512,6 +513,29 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
                              n_copies=1)
         return _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every)
 
+    def inference_many_stream(self, xs, ys, mask_intervals, tokenizer, chunk_frames: int = 25, poll_every: int = 8,
+                              seeds=None, **kw):
+        """inference_many with the audio handed out while it is generated: iterates (i, wav [1, channels, n*hop]),
+        utterance i's chunks in order; concatenated they equal ``tokenizer.decode_codes(res_i)``, the whole edited
+        utterance.  The frames before the first masked span are final at once, so they are the first chunk.  Afterwards
+        ``.results`` equals what inference_many returns.  `seeds` as in open_tts_session; the device generators only."""
+        sess = self.open_edit_session(xs, ys, mask_intervals, seeds=seeds, **kw)
+        return TtsStream(sess, tokenizer, chunk_frames, poll_every)
+
+    def inference_stream(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, mask_interval: torch.Tensor, tokenizer,
+                         chunk_frames: int = 25, poll_every: int = 8, top_k: int = -100, top_p: float = 1.0,
+                         temperature: float = 1.0, stop_repetition: int = -1, kvcache: int = 1,
+                         silence_tokens: List[int] = [1388, 1898, 131]):
+        """inference (speech editing) with the audio handed out while it is generated: iterates wav chunks
+        [1, channels, n*hop] whose concatenation equals ``tokenizer.decode_codes(res)``, the whole edited utterance.
+        Afterwards ``.result`` is res, what inference returns, and the device generator is left where inference leaves
+        it.  The device generator only (model.noise_fn must be None)."""
+        assert x.ndim == 2 and x.shape[0] == 1 and x_lens.ndim == 1 and y.ndim == 3 and y.shape[0] == 1, (x.shape, y.shape)
+        assert mask_interval.shape == torch.Size((1, mask_interval.shape[1], 2)), mask_interval
+        sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
+                             mask_intervals=[mask_interval], n_copies=1)
+        return _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every)
+
 
 def _check_best_of(best_of) -> int:
     if isinstance(best_of, bool) or int(best_of) != best_of or best_of < 1:
@@ -543,6 +567,48 @@ def final_frames(rows: np.ndarray, K: int, end: int) -> int:
 def frame_codes(rows: np.ndarray, K: int, t0: int, t1: int) -> np.ndarray:
     """frames [t0, t1) of the delayed rows, un-delayed: [K, t1-t0] with [k, t] = rows[t + k, k]"""
     return np.stack([rows[t0 + k: t1 + k, k] for k in range(K)], axis=0)
+
+
+def _edit_pieces(rows, status, spans, T, K, eog):
+    """The final pieces of an edit's output y0[:, 0:s1] ++ G1 ++ y0[:, e1:s2] ++ ... ++ GM ++ y0[:, eM:T], in order:
+    (0, first y0 column, frames) for an original piece, (1, first token row, frames) for a generated span.  With
+    d = n_spans_done: original pieces 0..d, the spans before d, and span d's frames that final_frames makes final."""
+    M = len(spans)
+    d = min(int(status.n_spans_done), M)
+    out, r0 = [], 0
+    for j in range(M + 1):
+        c0 = 0 if j == 0 else spans[j - 1][1]
+        out.append((0, c0, (T if j == M else spans[j][0]) - c0))
+        if j == M:
+            break
+        if j == d:
+            out.append((1, r0, final_frames(rows[r0:], K, eog)))
+            break
+        end = int(status.span_ends[j])
+        out.append((1, r0, max(0, end - r0 - K)))
+        r0 = end
+    return out
+
+
+def edit_final_frames(rows: np.ndarray, status, spans, T: int, K: int, eog: int) -> int:
+    """How many leading frames of an edit's output (_Prompt.result) are final, from its delayed token rows [n,K] and its
+    vcb_status: the original pieces up to n_spans_done, the spans generated before it, and the final frames of the span
+    being generated, by final_frames' rule on the rows since it began (end token eog).  Only grows as rows are added;
+    once every span is done it is the output's length."""
+    return sum(n for _, _, n in _edit_pieces(rows, status, spans, T, K, eog))
+
+
+def edit_frame_codes(rows: np.ndarray, status, orig: np.ndarray, spans, K: int, eog: int, t0: int, t1: int) -> np.ndarray:
+    """output frames [t0, t1) of an edit (t1 <= edit_final_frames): [K, t1-t0], each from the original codes orig [K,T]
+    or un-delayed from the token rows"""
+    out, f = [np.zeros((K, 0), dtype=np.int64)], 0
+    for kind, src, n in _edit_pieces(rows, status, spans, orig.shape[1], K, eog):
+        a, b = max(t0, f), min(t1, f + n)
+        if a < b:
+            u0, u1 = src + a - f, src + b - f
+            out.append(orig[:, u0:u1] if kind == 0 else frame_codes(rows[src:], K, a - f, b - f))
+        f += n
+    return np.concatenate(out, axis=1).astype(np.int64)
 
 
 def _check_capacity(status):
@@ -582,9 +648,9 @@ class _Prompt:
             cap, extra = x_len * 10, (K + 3) * (len(spans) + 1)
         self.need_seq = x_len + max(int(self.y_tok.shape[0]), cap + 1) + extra + 8
 
-    def fill(self, slot, n_copies, seed=None, offset=0):
+    def fill(self, slot, n_copies, seed=None, offset=0, sp=None):
         """its vcb_prompt in slots slot .. slot+n_copies-1, sampling from the Philox stream of a torch CUDA generator at
-        (seed, offset); seed None: host noise"""
+        (seed, offset); seed None: host noise.  sp: the group's own vcb_sampling (vcb_decode_step with sp NULL)"""
         P = _lib.vcb_prompt(slot=slot, n_copies=n_copies, mode=0 if self.spans is None else 1,
                             x_len=int(self.x_ids.shape[0]), text_ids_dev=self.x_ids.data_ptr(),
                             y_len=int(self.y_tok.shape[0]), y_tokens_dev=self.y_tok.data_ptr(),
@@ -592,6 +658,8 @@ class _Prompt:
                             n_more_spans=len(self.more_vals))
         for i, v in enumerate(self.more_vals):
             P.more_mask_rows[i] = int(v)
+        if sp is not None:
+            P.sampling = C.pointer(sp)
         if seed is not None:
             m = self.model
             P.rng_seed = int(seed) & 0xFFFFFFFFFFFFFFFF
@@ -599,6 +667,15 @@ class _Prompt:
             # the group's draw per sampling step is [n_copies*K, V], as the reference's multinomial
             P.rng_threads = m._rng_threads(self.y0.device, n_copies * m.args.n_codebooks * m.n_audio_tokens[0])
         return P
+
+    def source(self):
+        """its vcb_edit_source for vcb_poll_frames_ex: y0 and the spans of an edit, zeros for TTS"""
+        src = _lib.vcb_edit_source()
+        if self.spans is not None:
+            src.orig_dev, src.T, src.n_spans = self.y0.data_ptr(), int(self.y0.shape[1]), len(self.spans)
+            for j, (s0, s1) in enumerate(self.spans):
+                src.spans[j][0], src.spans[j][1] = s0, s1
+        return src
 
     def result(self, rows, st):
         """(res [1,K,T+G], gen [1,K,G]) as inference_tts returns them, or (res, None) with res as inference returns it,
@@ -631,7 +708,8 @@ class _Prompt:
 
 
 def _prefill(eng, prompts, stream):
-    """one packed prefill of [(_Prompt, slot, n_copies, seed, offset)] (see _Prompt.fill); a failed prefill holds nothing"""
+    """one packed prefill of [(_Prompt, slot, n_copies, seed, offset[, sp])] (see _Prompt.fill); a failed prefill holds
+    nothing"""
     P = (_lib.vcb_prompt * len(prompts))()
     for j, (p, *where) in enumerate(prompts):
         P[j] = p.fill(*where)
@@ -711,6 +789,10 @@ class TtsStream(_AudioStream):
         if sess.n_copies > 1:
             sess.close()
             _no_stream_best_of(sess.n_copies)
+        if sess.edit and sess._host_noise:
+            sess.close()
+            raise _lib.VcbError("streaming an edit needs the device generators (model.noise_fn / noise_fns must be None): "
+                                "the polls do not follow the forced hand-over steps, so host noise would be drawn for them")
         self._start(SimpleNamespace(sess=sess, dev=sess.dev, tok=tokenizer, chunk_frames=int(chunk_frames),
                                     poll_every=int(poll_every), results=None, first_audio_steps=None), sess.B)
 
@@ -720,7 +802,7 @@ class TtsStream(_AudioStream):
 
     @property
     def first_audio_steps(self):
-        """session steps taken when the first chunk was handed out"""
+        """session steps sampled when the poll that gathered the first chunk ran"""
         return self._st.first_audio_steps
 
     @property
@@ -741,7 +823,8 @@ class TtsStream(_AudioStream):
                 push = _PushStep(sess.model, sess.eng, sess.stream, st.tok, st.codec, st.cstream, st.chunk_frames,
                                  st.poll_every, strict=True)
                 st.push = push
-                live = [_Utterance(s, i, f"utterance {i}") for i, s in enumerate(sess.slots)]
+                live = [_Utterance(s, i, f"utterance {i}", src=p.source()) for i, (s, p) in
+                        enumerate(zip(sess.slots, sess.prompts))]
                 sess.sample()
                 while sess.steps % st.poll_every:
                     sess.step()
@@ -750,34 +833,38 @@ class TtsStream(_AudioStream):
                         if not all(s.done for s in status):
                             for _ in range(st.poll_every):
                                 sess.step()
+                    polled = sess.steps
                     status, out, _ = push([r for r in live if not r.closed], advance)
                     done = all(s.done for s in status)
                     for r, w in out:
                         if w is None:
                             continue
                         if st.first_audio_steps is None:
-                            st.first_audio_steps = sess.steps
+                            st.first_audio_steps = polled
                         yield r.cid, w
                     if done and all(r.closed for r in live):
                         break
                 st.results = sess.results()
+                if sess.edit:                        # what inference_many / inference return: res alone
+                    st.results = [res for res, _ in st.results]
         finally:
             TtsStream._finish(st)
 
 
 class _Utterance:
-    """An utterance of a streaming loop: engine slot, codec stream id, frames sent to the codec (pushed), all of its audio
-    handed out (closed), its vcb_status at the last poll."""
-    __slots__ = ("slot", "cid", "label", "ticket", "pushed", "closed", "status")
+    """An utterance of a streaming loop: engine slot, codec stream id, its vcb_edit_source (_Prompt.source), frames sent
+    to the codec (pushed), all of its audio handed out (closed), its vcb_status at the last poll."""
+    __slots__ = ("slot", "cid", "label", "ticket", "src", "pushed", "closed", "status")
 
-    def __init__(self, slot, cid, label, ticket=None):
+    def __init__(self, slot, cid, label, ticket=None, src=None):
         self.slot, self.cid, self.label, self.ticket = slot, cid, label, ticket
+        self.src = _lib.vcb_edit_source() if src is None else src
         self.pushed, self.closed, self.status = 0, False, None
 
 
 class _PushStep:
-    """One poll of a streaming loop (TtsStream, ContinuousBatcher.stream).  vcb_poll_frames gathers the live utterances'
-    newly final frames on the device behind one wait; those with enough new frames go to the codec in one ragged call on
+    """One poll of a streaming loop (TtsStream, ContinuousBatcher.stream).  vcb_poll_frames_ex gathers the live
+    utterances' newly final frames (of an edit: of its whole output, original pieces included) on the device behind one wait; those with enough new frames go to the codec in one ragged call on
     a second CUDA stream; the caller's next decode steps are enqueued; then the waveform is waited for.
 
     An utterance (_Utterance) has its first chunk waits for max(chunk_frames, min_frames) frames, later ones for chunk_frames,
@@ -805,9 +892,10 @@ class _PushStep:
         codes = torch.empty((n, self.K, mf), dtype=torch.int64, device=self.dev)     # fresh: the codec stream reads it
         status, final, bad = (_lib.vcb_status * n)(), (C.c_int32 * n)(), (C.c_int32 * (3 * n))()
         t0 = time.perf_counter()
-        _lib.check(lib.vcb_poll_frames(self.eng, (C.c_int32 * n)(*[r.slot for r in live]), n,
-                                       (C.c_int32 * n)(*[r.pushed for r in live]), mf, self.offset,
-                                       int(self.tok.config.bins), codes.data_ptr(), status, final, bad, self.stream))
+        _lib.check(lib.vcb_poll_frames_ex(self.eng, (C.c_int32 * n)(*[r.slot for r in live]), n,
+                                          (_lib.vcb_edit_source * n)(*[r.src for r in live]),
+                                          (C.c_int32 * n)(*[r.pushed for r in live]), mf, self.offset,
+                                          int(self.tok.config.bins), codes.data_ptr(), status, final, bad, self.stream))
         waited = time.perf_counter() - t0
         _check_capacity(status)
         push, whole, failed = {}, {}, {}
@@ -1052,47 +1140,70 @@ def place_groups(free, sizes, nxt):
 
 
 class ContinuousBatcher:
-    """Continuous batching of independent TTS utterances (SURVEY.md section 8f, row f2).
+    """Continuous batching of independent TTS and speech-editing utterances (SURVEY.md section 8f, row f2).
 
     The reference synthesises one utterance per call in a Python loop (inference_tts_scale.py:43-105; the sentence loop of
     gradio_app.py:248-313).  Here up to `max_concurrency` utterances decode together; the moment one finishes, its tokens
     are read, its slot and KV pages are released and the next queued utterance is prefilled into the free slot while the
-    others keep decoding.  Every utterance owns its random stream (`seed`), so its result is exactly what
-    ``torch.manual_seed(seed); model.inference_tts(x, x_lens, y, ...)`` returns, whatever it was batched with.
-    run() returns the token lists once the queue has drained; stream() hands out every utterance's audio while it is
-    generated and takes submit() / cancel() during the iteration.  A best-of-N ticket (submit(..., best_of=N), run() only)
-    decodes as a group on N consecutive slots; max_concurrency counts slots.
+    others keep decoding.  Every utterance owns its random stream (`seed`) and its sampling parameters (the constructor's,
+    or those given to submit()), so its result is exactly what ``torch.manual_seed(seed); model.inference_tts(x, x_lens,
+    y, **params)`` -- or, for an edit ticket, ``model.inference(x, x_lens, y, mask_interval, **params)`` -- returns,
+    whatever it was batched with.  run() returns the token lists once the queue has drained; stream() hands out every
+    utterance's audio while it is generated and takes submit() / cancel() during the iteration.  A best-of-N ticket
+    (submit(..., best_of=N), run() only) decodes as a group on N consecutive slots; max_concurrency counts slots.
     """
 
     def __init__(self, model: "VoiceCraft", max_concurrency=32, poll_every=8, top_k=-100, top_p=1.0, temperature=1.0,
                  stop_repetition=3, silence_tokens=(1388, 1898, 131)):
         self.model, self.B, self.poll_every = model, int(max_concurrency), max(1, int(poll_every))
-        self.sp = model._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens)
+        self.defaults = dict(top_k=top_k, top_p=top_p, temperature=temperature, stop_repetition=stop_repetition,
+                             silence_tokens=silence_tokens)
         self.queue = []
         self.stats = dict(steps=0, prefills=0, max_active=0)
         self.results, self.errors = [], {}
         self._live = None                  # the running stream()'s state
 
-    def submit(self, x, y, seed=None, best_of=1):
+    def submit(self, x, y, seed=None, best_of=1, mask_interval=None, top_k=None, top_p=None, temperature=None,
+               stop_repetition=None, silence_tokens=None):
         """x [1,L] int64, y [1,T,K] int64 (host or device).  Returns the ticket (index into run()'s result list / results).
         best_of: run() samples the utterance best_of times on consecutive slots and keeps the copy that ends first, as
         ``torch.manual_seed(seed); inference_tts_batch(x, ., y, batch_size=best_of)`` does; the copies count against
         max_concurrency.  stream() serves only best_of = 1.
+        mask_interval [1,M,2]: a speech-editing ticket (best_of = 1, at most min(8, max_n_spans) spans); its result is
+        (res, None) with res what ``inference(x, ., y, mask_interval, ...)`` returns.
+        top_k, top_p, temperature, stop_repetition, silence_tokens: this ticket's sampling parameters; None takes the
+        constructor's value (not inference's or inference_tts' own defaults).
         While a stream() runs, the utterance is admitted at one of its next polls; one that does not fit the engine it
         sized raises VcbError and is not queued."""
         best_of = _check_best_of(best_of)
         if best_of > self.B:
             raise ValueError(f"best_of={best_of} copies do not fit max_concurrency={self.B} slots")
+        spans = None
+        if mask_interval is not None:
+            mi = torch.as_tensor(mask_interval)
+            if mi.ndim != 3 or mi.shape[0] != 1 or mi.shape[2] != 2:
+                raise ValueError(f"mask_interval must be [1, M, 2], got {tuple(mi.shape)}")
+            if best_of != 1:
+                raise ValueError(f"best_of={best_of}: an edit ticket takes best_of=1")
+            spans = [(int(a), int(b)) for a, b in mi[0].tolist()]
+            if len(spans) > min(8, int(self.model.args.max_n_spans)):
+                raise ValueError(f"{len(spans)} masked spans: at most min(8, max_n_spans={self.model.args.max_n_spans})")
+        given = dict(top_k=top_k, top_p=top_p, temperature=temperature, stop_repetition=stop_repetition,
+                     silence_tokens=silence_tokens)
+        params = {k: self.defaults[k] if v is None else v for k, v in given.items()}
+        if not (math.isfinite(params["temperature"]) and params["temperature"] > 0) or math.isnan(params["top_p"]):
+            raise ValueError(f"temperature must be finite and > 0 and top_p a number, got {params}")
+        sp = self.model._sampling(**params)
         st = self._live
         if st is not None:
             _no_stream_best_of(best_of)
-            job = self._job(x, y, seed)
+            job = self._job(x, y, seed, 1, spans, sp)
             if job[0].need_seq > st.max_seq:
                 raise _lib.VcbError(f"utterance needs {job[0].need_seq} positions, the streaming engine holds {st.max_seq}: "
                                     "configure_engine(max_seq_len=...) before stream()")
             st.jobs.append(job)
             self.results.append(None)
-        self.queue.append((x, y, seed, best_of))
+        self.queue.append((x, y, seed, best_of, spans, sp))
         return len(self.queue) - 1
 
     def cancel(self, ticket) -> bool:
@@ -1106,25 +1217,26 @@ class ContinuousBatcher:
         st.cancelled.add(ticket)
         return True
 
-    def _job(self, x, y, seed, best_of=1):
-        """(prompt, seed, best_of) of a ticket; raises IndexError on an out-of-range id"""
-        p = _Prompt(self.model, x, y)
+    def _job(self, x, y, seed, best_of, spans, sp):
+        """(prompt, seed, best_of, vcb_sampling) of a ticket; raises IndexError on an out-of-range id"""
+        p = _Prompt(self.model, x, y, spans)
         self.model._check_ids(p.x_ids, p.y_tok)
-        return p, seed, best_of
+        return p, seed, best_of, sp
 
     def _admit(self, eng, new, jobs, stream):
-        """one packed prefill + the first sampling step of the newcomers [(first slot, ticket)]"""
+        """one packed prefill + the first sampling step of the newcomers [(first slot, ticket)], each with its ticket's
+        sampling parameters (every sampling call of the batcher passes sp = NULL)"""
         m, lib = self.model, _lib.load()
         seed0 = int(torch.cuda.default_generators[m.mask_embedding.device.index or 0].initial_seed())
-        _prefill(eng, [(jobs[t][0], slot, jobs[t][2], seed0 + t if jobs[t][1] is None else jobs[t][1], 0)
+        _prefill(eng, [(jobs[t][0], slot, jobs[t][2], seed0 + t if jobs[t][1] is None else jobs[t][1], 0, jobs[t][3])
                        for slot, t in new], stream)
         rows = [s + c for s, t in new for c in range(jobs[t][2])]
         c_new = (C.c_int32 * len(rows))(*rows)
-        _lib.check(lib.vcb_sample(eng, c_new, len(rows), None, C.byref(self.sp), stream))
+        _lib.check(lib.vcb_sample(eng, c_new, len(rows), None, None, stream))
         self.stats["prefills"] += 1
 
     def _result(self, eng, slot, st, job, stream):
-        """(res, gen) of a finished slot, as inference_tts returns them"""
+        """(res, gen) of a finished slot, as inference_tts returns them; (res, None) of an edit, res as inference returns it"""
         return job[0].result(self.model._read_rows(eng, slot, st.n_steps, stream), st)
 
     @torch.no_grad()
@@ -1156,7 +1268,7 @@ class ContinuousBatcher:
                     self.stats["max_active"] = max(self.stats["max_active"], len(order))
                     # ---- decode steps for everyone until the next poll
                     for _ in range(self.poll_every):
-                        _lib.check(lib.vcb_decode_step(eng, c_slots, len(order), None, C.byref(self.sp), stream))
+                        _lib.check(lib.vcb_decode_step(eng, c_slots, len(order), None, None, stream))
                         steps += 1
                     status = (_lib.vcb_status * len(order))()
                     _lib.check(lib.vcb_poll(eng, c_slots, len(order), status, stream))
@@ -1178,7 +1290,9 @@ class ContinuousBatcher:
 
     def stream(self, tokenizer, chunk_frames: int = 25) -> "BatcherStream":
         """run() with every utterance's audio handed out while it is generated: iterates (ticket, wav [1, channels, n*hop],
-        last).  A ticket's chunks, concatenated, equal ``tokenizer.decode_codes(gen)``; its last chunk has last=True
+        last).  A ticket's chunks, concatenated, equal ``tokenizer.decode_codes(gen)`` (an edit ticket's:
+        ``decode_codes(res)``, the whole edited utterance, whose frames before the first masked span are its first chunk);
+        its last chunk has last=True
         (an utterance that generated no frame yields one empty wav).  submit() and cancel() may be called from the loop
         body.  Afterwards ``results[ticket]`` is (res, gen) as run() returns it, None for a cancelled or failed ticket;
         ``errors[ticket]`` says why a ticket failed (a final frame holding a non-audio token: it yields (ticket, None,
@@ -1251,7 +1365,7 @@ class BatcherStream(_AudioStream):
                         cb._admit(st.eng, new, st.jobs, stream)
                         st.codec.reset([slot - base for slot, _ in new])
                         for slot, t in new:
-                            active[slot] = _Utterance(slot, slot - base, f"ticket {t}", ticket=t)
+                            active[slot] = _Utterance(slot, slot - base, f"ticket {t}", ticket=t, src=st.jobs[t][0].source())
                     if not active:
                         break
                     live = [active[s] for s in sorted(active)]
@@ -1262,7 +1376,7 @@ class BatcherStream(_AudioStream):
                         if go:
                             c_go = (C.c_int32 * len(go))(*go)
                             for _ in range(cb.poll_every):
-                                _lib.check(lib.vcb_decode_step(st.eng, c_go, len(go), None, C.byref(cb.sp), stream))
+                                _lib.check(lib.vcb_decode_step(st.eng, c_go, len(go), None, None, stream))
                             cb.stats["steps"] += cb.poll_every
                     status, out, failed = push(live, advance)
                     wavs = dict(out)
