@@ -46,7 +46,8 @@ int enc_decode(enc_engine* e, const int64_t* codes_dev, float* wav_dev, int32_t 
 int enc_encode(enc_engine* e, const float* wav_dev, int64_t* codes_dev, int32_t B, int32_t N, void* stream);
 /* "launches", "hop", "flops_per_frame", "tc_enabled", "tc_decodes", "stream_decodes", "stream_min_frames" (frames a fresh
  * stream's first enc_stream_decode needs; -1 without the tensor-core decoder), "stream_state_bytes" (carried state per stream);
- * "live_bytes" / "live_handles" as vcb_counter (process-wide, valid with a NULL engine) */
+ * "live_bytes" / "live_handles" as vcb_counter and "resample_launches" (kernels enc_resample / enc_resampler_push enqueued) are
+ * process-wide, valid with a NULL engine */
 int64_t enc_counter(enc_engine* e, const char* name);
 
 /* Streaming decode: waveform chunk by chunk while the tokens are still being generated.  The decoder is causal, so a chunk
@@ -76,6 +77,36 @@ int enc_stream_decode(enc_engine* e, enc_stream* s, const int32_t* ids_host, con
  * halo}; host_out == NULL only queries dims.  The up-sampling stages share two workspace arenas, so after a full decode only
  * the tensors of the last stage (and "z", "x0", "u0", "hs*") still hold their values: see scripts/codec_tc_debug.py. */
 int enc_debug_tensor(enc_engine* e, const char* name, float* host_out, int64_t cap, int32_t* dims);
+
+/* Resampling: torchaudio.transforms.Resample(orig_sr, new_sr) with its defaults (sinc_interp_hann, lowpass_filter_width 6,
+ * rolloff 0.99), the conversion the reference's convert_audio applies to prompt audio (data/tokenizer.py:85-97), on the
+ * device.  With g = gcd(orig_sr, new_sr), o = orig_sr / g, n = new_sr / g and w = ceil(6 o / (0.99 min(o, n))), output
+ * sample b*n + p is sum_{i < 2w+o} table[p][i] * x[b*o + i - w] (x = 0 outside the row), summed in that order with fp32
+ * FMA; a row of L samples gives ceil(n L / o).  The resampler is independent of any enc_engine.  Its calls enqueue work
+ * on `stream` and never wait for the device; one resampler is used from one CUDA stream at a time. */
+typedef struct enc_resampler enc_resampler;
+/* table_host: fp32 [n][2w + o], the filter table torchaudio builds (voicecraft_b200.tokenizer.resample_table).  Rejected
+ * before anything is allocated: a rate <= 0, a table over 16 MB, a down-sampling ratio whose one-output input window
+ * does not fit in shared memory.  max_streams (>= 0) streams for enc_resampler_push. */
+int enc_resampler_create(int32_t orig_sr, int32_t new_sr, const float* table_host, int32_t max_streams, int32_t device,
+                         enc_resampler** out);
+int enc_resampler_destroy(enc_resampler* r);
+/* One-shot, over ragged rows: in [B][T] fp32 (device), row b's first lens_host[b] samples -> out [B][out_cap] (device),
+ * row b's first out_lens_host[b] = ceil(n lens_host[b] / o) samples. */
+int enc_resample(enc_resampler* r, const float* in_dev, const int32_t* lens_host, int32_t B, int32_t T, float* out_dev,
+                 int32_t out_cap, int32_t* out_lens_host, void* stream);
+/* Streaming: row b continues stream ids_host[b] with the first lens_host[b] (>= 0) samples of in [B][T] and emits every
+ * output whose whole input window has arrived (block b once b*o + w + o <= samples so far); with final_host[b] set (null:
+ * none) also the zero-padded tail up to ceil(n L / o), and the stream takes no more input until reset.  Row b's
+ * out_lens_host[b] outputs go to out [B][out_cap]; the counts are written before anything is enqueued.  A stream's
+ * outputs, concatenated, are bit-identical to enc_resample of its whole input.  Rejected before any stream changes: an id
+ * outside [0, max_streams) or twice in the call, a length outside [0, T], a stream past its final push, a row whose
+ * outputs exceed out_cap. */
+int enc_resampler_push(enc_resampler* r, const int32_t* ids_host, const int32_t* lens_host, const int32_t* final_host,
+                       int32_t B, const float* in_dev, int32_t T, float* out_dev, int32_t out_cap, int32_t* out_lens_host,
+                       void* stream);
+/* the listed streams start over with no input */
+int enc_resampler_reset(enc_resampler* r, const int32_t* ids_host, int32_t n);
 
 #ifdef __cplusplus
 }

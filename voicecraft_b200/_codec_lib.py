@@ -1,4 +1,4 @@
-"""ctypes prototypes of the EnCodec decode entry points (include/vcb200_codec.h)."""
+"""ctypes prototypes of the EnCodec and resampler entry points (include/vcb200_codec.h)."""
 import ctypes as C
 
 
@@ -25,6 +25,13 @@ PROTOTYPES = {
     "enc_stream_reset": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]),
     "enc_stream_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
                                     C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "enc_resampler_create": (C.c_int, [C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]),
+    "enc_resampler_destroy": (C.c_int, [C.c_void_p]),
+    "enc_resample": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_void_p, C.c_int32,
+                               C.POINTER(C.c_int32), C.c_void_p]),
+    "enc_resampler_push": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
+                                     C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_void_p]),
+    "enc_resampler_reset": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.c_int32]),
 }
 
 

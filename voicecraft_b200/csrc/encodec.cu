@@ -733,6 +733,7 @@ int enc_debug_tensor(enc_engine* e, const char* name, float* host_out, int64_t c
 int64_t enc_counter(enc_engine* e, const char* name) {
     if (!strcmp(name, "live_bytes")) return LiveCount::bytes;          // process-wide, valid with a null engine
     if (!strcmp(name, "live_handles")) return LiveCount::handles;
+    if (!strcmp(name, "resample_launches")) return resample_launches();
     if (!strcmp(name, "launches")) return e->launches;
     if (!strcmp(name, "hop")) return e->hop;
     if (!strcmp(name, "flops_per_frame")) return static_cast<int64_t>(e->flops_per_frame);

@@ -304,6 +304,9 @@ void gemm_timeline_set(unsigned long long* buf, unsigned int* cnt);
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems,
                       uint32_t box_rows);
 
+// kernels enqueued by the resampler (resample.cu), process-wide
+long long resample_launches();
+
 // ---------------------------------------------------------------------------------------------------
 // Per-utterance ("slot") and per-group device state.  A group couples the slots of one
 // inference_tts_batch call (shared codebook_eog / cur_num_gen / keep, voicecraft.py:1269-1325);

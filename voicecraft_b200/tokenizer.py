@@ -7,6 +7,10 @@ reference's ``[(codes[1,K,T], None)]`` (:127-129).  Instead of audiocraft's ``Co
 SEANet decoder / encoder as sm_90a kernels.  No PyTorch / CPU fallback.  The text tokenizer (espeak) is out of scope.
 """
 import ctypes as C
+import functools
+import math
+import struct
+from collections import namedtuple
 from types import SimpleNamespace
 from typing import Any
 
@@ -88,6 +92,118 @@ def state_dict_from_audiocraft(sd: dict, cfg) -> dict:
     return out
 
 
+RESAMPLE_TABLE_CAP = 16 << 20          # bytes of filter table a resampler may hold (44.1 kHz -> 16 kHz needs 296 KB)
+
+
+def resample_dims(orig_sr: int, new_sr: int):
+    """(o, n, w, taps) of torchaudio's Resample(orig_sr, new_sr) with its defaults: the rates over their gcd, the filter
+    half-width w = ceil(6 o / (0.99 min(o, n))) and the 2w + o taps of each of the n phases.  Raises ValueError for a
+    rate <= 0 and for a pair whose table would exceed RESAMPLE_TABLE_CAP (16000 -> 44099 Hz would need gigabytes)."""
+    if int(orig_sr) != orig_sr or int(new_sr) != new_sr or orig_sr <= 0 or new_sr <= 0:
+        raise ValueError(f"resample: sample rates must be positive integers, got {orig_sr} -> {new_sr}")
+    g = math.gcd(int(orig_sr), int(new_sr))
+    o, n = int(orig_sr) // g, int(new_sr) // g
+    w = math.ceil(6 * o / (min(o, n) * 0.99))
+    taps = 2 * w + o
+    if n * taps * 4 > RESAMPLE_TABLE_CAP:
+        raise ValueError(f"resample: {orig_sr} -> {new_sr} Hz needs a filter table of {n} phases x {taps} taps "
+                         f"({n * taps * 4} bytes), over the {RESAMPLE_TABLE_CAP}-byte cap")
+    return o, n, w, taps
+
+
+@functools.lru_cache(maxsize=None)
+def _sinc_table(o: int, n: int) -> torch.Tensor:
+    w = resample_dims(o, n)[2]
+    base = min(o, n) * 0.99
+    # tap positions in fp64; the phase offsets -p/n in fp32 (torchaudio divides an integer arange in the default dtype),
+    # promoted to fp64 by the addition.  A clean fp64 -p/n moves some taps of 44.1k <-> 16k by up to 1.3e-5.
+    pos = torch.arange(-w, w + o, dtype=torch.float64)[None, None] / o
+    t = torch.arange(0, -n, -1, dtype=torch.float32)[:, None, None] / n + pos
+    t *= base
+    t = t.clamp_(-6, 6)
+    window = torch.cos(t * math.pi / 6 / 2) ** 2          # Hann window over the 6 zero crossings
+    t *= math.pi
+    k = torch.where(t == 0, torch.tensor(1.0).to(t), t.sin() / t)
+    k *= window * (base / o)
+    return k.to(torch.float32).reshape(n, 2 * w + o).contiguous()
+
+
+def resample_table(orig_sr: int, new_sr: int) -> torch.Tensor:
+    """The filter table of torchaudio.transforms.Resample(orig_sr, new_sr) (sinc_interp_hann, lowpass_filter_width 6,
+    rolloff 0.99): fp32 [n][2w + o] on the CPU, built with the same torch ops in fp64 and rounded once, so it is
+    bit-equal to torchaudio's (functional._get_sinc_resample_kernel).  Cached per reduced (o, n)."""
+    o, n, _, _ = resample_dims(orig_sr, new_sr)
+    return _sinc_table(o, n)
+
+
+class Resampler:
+    """Owner of one enc_resampler (torchaudio's Resample(orig_sr, new_sr) on the device): one-shot over ragged rows
+    (``__call__``) and, for up to `max_streams` streams, chunk by chunk with carried state (``push``)."""
+
+    def __init__(self, orig_sr: int, new_sr: int, max_streams: int = 0, device=None):
+        self.orig_sr, self.new_sr = int(orig_sr), int(new_sr)
+        self.o, self.n, self.w, self.taps = resample_dims(orig_sr, new_sr)
+        self.device = torch.device(device if device is not None else "cuda")
+        if self.device.type != "cuda":
+            raise _lib.VcbError("the resampler runs on a CUDA device only")
+        self._lib = _lib.load()
+        self._h = None
+        table = resample_table(orig_sr, new_sr)
+        h = C.c_void_p()
+        _lib.check(self._lib.enc_resampler_create(self.orig_sr, self.new_sr, table.data_ptr(), int(max_streams),
+                                                  self.device.index or 0, C.byref(h)))
+        self._h = h
+        self.max_streams = int(max_streams)
+
+    def _out(self, rows, cap):
+        return torch.empty(max(rows, 1), max(cap, 1), device=self.device, dtype=torch.float32)
+
+    @torch.no_grad()
+    def __call__(self, x: torch.Tensor, lens=None):
+        """x [R, T] fp32 (device) -> (y [R, cap], out_lens): row r's first out_lens[r] = ceil(n lens[r] / o) samples
+        are the resampled first lens[r] (default T) samples of x[r]; cap = max(out_lens).  Current CUDA stream."""
+        x = x.to(self.device, dtype=torch.float32).contiguous()
+        R, T = x.shape
+        lens = [T] * R if lens is None else [int(v) for v in lens]
+        cap = max([-(-v * self.n // self.o) for v in lens], default=0)
+        y, out_lens = self._out(R, cap), (C.c_int32 * max(R, 1))()
+        _lib.check(self._lib.enc_resample(self._h, x.data_ptr(), (C.c_int32 * max(R, 1))(*lens), R, T, y.data_ptr(), cap,
+                                          out_lens, torch.cuda.current_stream(self.device).cuda_stream))
+        return y[:R, :cap], list(out_lens)[:R]
+
+    @torch.no_grad()
+    def push(self, x, ids, lens, final=None):
+        """Row r continues stream ids[r] with the first lens[r] samples of x [R, T] (x may be None when every length is
+        0); final[r] also emits the stream's tail.  Returns (y [R, cap], out_lens) as __call__ does."""
+        R = len(ids)
+        x = None if x is None else x.to(self.device, dtype=torch.float32).contiguous()
+        T = 0 if x is None else int(x.shape[1])
+        most = max([int(v) for v in lens], default=0)
+        cap = (self.n * (most + self.w + 2 * self.o)) // self.o + self.n + 1   # >= what any row can emit
+        y, out_lens = self._out(R, cap), (C.c_int32 * max(R, 1))()
+        fin = None if final is None else (C.c_int32 * max(R, 1))(*[int(bool(f)) for f in final])
+        _lib.check(self._lib.enc_resampler_push(self._h, (C.c_int32 * max(R, 1))(*ids), (C.c_int32 * max(R, 1))(*lens), fin, R,
+                                                0 if x is None else x.data_ptr(), T, y.data_ptr(), cap, out_lens,
+                                                torch.cuda.current_stream(self.device).cuda_stream))
+        out_lens = list(out_lens)[:R]
+        return y[:R, :max(out_lens, default=0)], out_lens
+
+    def reset(self, ids):
+        ids = [int(i) for i in ids]
+        _lib.check(self._lib.enc_resampler_reset(self._h, (C.c_int32 * max(len(ids), 1))(*ids), len(ids)))
+
+    def close(self):
+        if self._h is not None:
+            self._lib.enc_resampler_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class AudioTokenizer:
     """EnCodec audio (decode direction)."""
 
@@ -115,6 +231,7 @@ class AudioTokenizer:
         self.channels = self.config.channels
         self._sd = {k: v.detach().float() for k, v in state_dict.items()}
         self._eng = None
+        self._resamplers = {}
         self.hop = 1
         for r in self.config.ratios:
             self.hop *= int(r)
@@ -156,10 +273,35 @@ class AudioTokenizer:
 
     def __del__(self):
         try:
+            for r in self._resamplers.values():
+                r.close()
             if self._eng is not None:
                 _lib.load().enc_destroy(self._eng)
         except Exception:
             pass
+
+    @torch.no_grad()
+    def resample(self, wav: torch.Tensor, orig_sr: int, new_sr: int = None, lens=None) -> torch.Tensor:
+        """torchaudio.transforms.Resample(orig_sr, new_sr)(wav) on the device (enc_resample): wav [B, C, N] ->
+        [B, C, N'], N' = ceil(n N / o); new_sr defaults to the codec's rate.  With lens, row b holds lens[b] samples and
+        gives ceil(n lens[b] / o) samples, the rest of its row is zero.  Equal rates return wav itself."""
+        new_sr = self.sample_rate if new_sr is None else int(new_sr)
+        assert wav.ndim == 3, wav.shape
+        if int(orig_sr) == new_sr:
+            return wav
+        key = (int(orig_sr), new_sr)
+        if key not in self._resamplers:
+            self._resamplers[key] = Resampler(orig_sr, new_sr, 0, self._device)
+        rs = self._resamplers[key]
+        B, Ch, N = wav.shape
+        x = wav.to(self._device, dtype=torch.float32).contiguous().view(B * Ch, N)
+        rows = None if lens is None else [int(lens[b]) for b in range(B) for _ in range(Ch)]
+        with torch.cuda.device(self._device):
+            y, out_lens = rs(x, rows)
+        if lens is not None:
+            y.masked_fill_(torch.arange(y.shape[1], device=y.device)[None, :] >=
+                           torch.tensor(out_lens, device=y.device)[:, None], 0.0)
+        return y.reshape(B, Ch, y.shape[1])
 
     @torch.no_grad()
     def encode_codes(self, wav: torch.Tensor) -> torch.Tensor:
@@ -199,20 +341,28 @@ class AudioTokenizer:
         """Reference signature: frames = [(codes[1,K,T], None)] (data/tokenizer.py:131-133)."""
         return self.decode_codes(frames[0][0])
 
-    def open_stream(self, max_streams: int = 1) -> "CodecStream":
-        """Incremental decode of up to `max_streams` utterances (enc_stream_decode): see CodecStream."""
-        return CodecStream(self, max_streams)
+    def open_stream(self, max_streams: int = 1, sample_rate: int = None) -> "CodecStream":
+        """Incremental decode of up to `max_streams` utterances (enc_stream_decode), resampled to `sample_rate` when
+        one other than the codec's is given: see CodecStream."""
+        return CodecStream(self, max_streams, sample_rate)
 
 
 class CodecStream:
     """Waveform of a growing code sequence, chunk by chunk.  Stream i's chunks, concatenated, are bit-identical to
     ``decode_codes`` of its whole sequence: the causal decoder carries every layer's left context and the LSTM state from
     one chunk to the next.  A stream's first chunk needs at least ``min_frames`` frames.  Runs only on the tensor-core
-    decoder; opening one on a codec it does not cover raises VcbError.  Use it from one CUDA stream at a time."""
+    decoder; opening one on a codec it does not cover raises VcbError.  Use it from one CUDA stream at a time.
 
-    def __init__(self, tokenizer: AudioTokenizer, max_streams: int = 1):
+    With a `sample_rate` other than the codec's, every chunk also goes through a streaming resampler on the same CUDA
+    stream (enc_resampler_push, one resampler stream per codec stream and channel): stream i's chunks, concatenated, are
+    then bit-identical to ``tokenizer.resample(decode_codes(codes_i), codec rate, sample_rate)``, provided its last
+    chunk is marked final (``decode(..., final=)``, or ``flush`` when the utterance ends with no new frame).  A chunk
+    holds the samples whose resampling window has fully arrived, so chunk lengths vary; ``out_lens`` gives them."""
+
+    def __init__(self, tokenizer: AudioTokenizer, max_streams: int = 1, sample_rate: int = None):
         self._tok = tokenizer
         self._lib = _lib.load()
+        self._h, self._rs = None, None
         eng = tokenizer._engine()
         h = C.c_void_p()
         with torch.cuda.device(tokenizer.device):
@@ -220,33 +370,76 @@ class CodecStream:
         self._h = h
         self.max_streams = int(max_streams)
         self.min_frames = int(self._lib.enc_counter(eng, b"stream_min_frames"))
+        self.sample_rate = tokenizer.sample_rate if sample_rate is None else int(sample_rate)
+        self.out_lens = []                     # samples per row of the last decode / flush
+        if self.sample_rate != tokenizer.sample_rate:
+            try:
+                self._rs = Resampler(tokenizer.sample_rate, self.sample_rate, self.max_streams * tokenizer.channels,
+                                     tokenizer.device)
+            except Exception:
+                self.close()
+                raise
+
+    def _rows(self, ids):
+        ch = self._tok.channels
+        return [i * ch + c for i in ids for c in range(ch)]
+
+    def _resampled(self, x, ids, lens, final):
+        """push rows of x [B*channels, N] through the resampler -> wav [B, channels, n]; out_lens per utterance"""
+        ch = self._tok.channels
+        rep = (lambda v: [u for u in v for _ in range(ch)])
+        with torch.cuda.device(self._tok.device):
+            y, out_lens = self._rs.push(x, self._rows(ids), rep(lens), None if final is None else rep(final))
+        self.out_lens = out_lens[::ch]
+        return y.reshape(len(ids), ch, y.shape[1])
 
     @torch.no_grad()
-    def decode(self, codes: torch.Tensor, ids=None, lens=None) -> torch.Tensor:
-        """codes [B,K,T] -> wav [B,channels,T*hop].  Row b continues stream ids[b] (default b) by its next lens[b] frames
-        (default T); samples [0, lens[b]*hop) of row b are that audio, later samples are unspecified.  Every code, padding
-        included, must lie in [0, bins).  Runs on the current CUDA stream."""
+    def decode(self, codes: torch.Tensor, ids=None, lens=None, final=None) -> torch.Tensor:
+        """codes [B,K,T] -> wav [B,channels,N].  Row b continues stream ids[b] (default b) by its next lens[b] frames
+        (default T); samples [0, out_lens[b]) of row b are that audio, later samples are unspecified.  At the codec's
+        rate out_lens[b] = lens[b]*hop and N = T*hop; resampled, final[b] (default False) marks stream ids[b]'s last
+        chunk, which also emits the resampler's tail.  Every code, padding included, must lie in [0, bins).  Runs on the
+        current CUDA stream."""
         if self._h is None:
             raise _lib.VcbError("CodecStream is closed")
         assert codes.ndim == 3 and codes.shape[1] == self._tok.config.n_q, codes.shape
         B, _, T = codes.shape
         ids = list(range(B)) if ids is None else [int(i) for i in ids]
         lens = [T] * B if lens is None else [int(n) for n in lens]
-        if len(ids) != B or len(lens) != B:
+        if len(ids) != B or len(lens) != B or (final is not None and len(final) != B):
             raise ValueError(f"CodecStream.decode: {B} rows, {len(ids)} ids, {len(lens)} lens")
         codes = codes.to(self._tok.device).long().contiguous()
         wav = torch.empty(B, self._tok.channels, T * self._tok.hop, device=self._tok.device, dtype=torch.float32)
         with torch.cuda.device(self._tok.device):
             _lib.check(self._lib.enc_stream_decode(self._tok._engine(), self._h, (C.c_int32 * B)(*ids), (C.c_int32 * B)(*lens), B,
                                                    codes.data_ptr(), T, wav.data_ptr(), torch.cuda.current_stream().cuda_stream))
-        return wav
+        if self._rs is None:
+            self.out_lens = [n * self._tok.hop for n in lens]
+            return wav
+        hop = self._tok.hop
+        return self._resampled(wav.view(B * self._tok.channels, T * hop), ids, [n * hop for n in lens], final)
+
+    @torch.no_grad()
+    def flush(self, ids) -> torch.Tensor:
+        """Resampled streams only: end the listed streams with no new frames, emitting the resampler's tail of each ->
+        wav [len(ids), channels, n], row b's first out_lens[b] samples.  For an utterance whose last decode was not
+        marked final."""
+        if self._rs is None:
+            raise _lib.VcbError("CodecStream.flush: this stream runs at the codec's rate; there is nothing to flush")
+        ids = [int(i) for i in ids]
+        return self._resampled(None, ids, [0] * len(ids), [True] * len(ids))
 
     def reset(self, ids):
-        """The listed streams start over at frame 0."""
+        """The listed streams start over at frame 0 (and with an empty resampler)."""
         ids = [int(i) for i in ids]
         _lib.check(self._lib.enc_stream_reset(self._h, (C.c_int32 * max(len(ids), 1))(*ids), len(ids)))
+        if self._rs is not None:
+            self._rs.reset(self._rows(ids))
 
     def close(self):
+        if self._rs is not None:
+            self._rs.close()
+            self._rs = None
         if self._h is not None:
             self._lib.enc_stream_destroy(self._h)
             self._h = None
@@ -281,25 +474,98 @@ def save_wav(path, wav: torch.Tensor, sample_rate: int):
         f.writeframes(pcm.tobytes())
 
 
-def tokenize_audio(tokenizer: AudioTokenizer, audio_path: str, offset=-1, num_frames=-1):
-    """The reference's helper (data/tokenizer.py:137-149) for 16-bit PCM WAV files, without the torchaudio dependency:
-    load (optionally a window of `num_frames` samples from `offset`), mix to the codec's channel count, encode.
-    A file at another sample rate is rejected (the reference resamples with torchaudio; do that before calling)."""
-    import wave
+AudioInfo = namedtuple("AudioInfo", "sample_rate num_frames num_channels")
+
+# (format tag, bits per sample) -> (numpy dtype of a sample, divisor to [-1, 1)): torchaudio.load's scaling
+_WAV_FORMATS = {(1, 16): ("<i2", 32768.0), (1, 24): (None, 8388608.0), (1, 32): ("<i4", 2147483648.0), (3, 32): ("<f4", None)}
+
+
+def _wav_layout(f, path):
+    """RIFF/WAVE header of the open file f -> (format tag, channels, rate, bits, offset and bytes of the data chunk).
+    WAVE_FORMAT_EXTENSIBLE (0xFFFE) is reported as its sub-format's tag."""
+    head = f.read(12)
+    if len(head) < 12 or head[:4] != b"RIFF" or head[8:12] != b"WAVE":
+        raise ValueError(f"{path}: not a RIFF/WAVE file")
+    fmt = None
+    while True:
+        chunk = f.read(8)
+        if len(chunk) < 8:
+            raise ValueError(f"{path}: no data chunk")
+        cid, size = chunk[:4], struct.unpack("<I", chunk[4:])[0]
+        if cid == b"fmt ":
+            fmt = f.read(size)
+            if size & 1:
+                f.seek(1, 1)
+        elif cid == b"data":
+            if fmt is None or len(fmt) < 16:
+                raise ValueError(f"{path}: data chunk before a complete fmt chunk")
+            tag, ch, sr, _, _, bits = struct.unpack("<HHIIHH", fmt[:16])
+            if tag == 0xFFFE:
+                if len(fmt) < 26:
+                    raise ValueError(f"{path}: WAVE_FORMAT_EXTENSIBLE without a sub-format")
+                tag = struct.unpack("<H", fmt[24:26])[0]
+            start = f.tell()
+            f.seek(0, 2)
+            return tag, ch, sr, bits, start, min(size, f.tell() - start)     # a streamed file may leave size unset
+        else:
+            f.seek(size + (size & 1), 1)
+
+
+def _wav_frame_bytes(tag, ch, bits, path):
+    if (tag, bits) not in _WAV_FORMATS or ch < 1:
+        kind = {1: "PCM", 3: "IEEE float"}.get(tag, f"format tag {tag:#x}")
+        raise ValueError(f"{path}: {kind} with {bits} bits per sample and {ch} channels is not supported "
+                         "(PCM 16/24/32-bit or 32-bit float WAV)")
+    return ch * bits // 8
+
+
+def audio_info(path) -> AudioInfo:
+    """(sample_rate, num_frames, num_channels) of a WAV file: what the reference's drivers read with torchaudio.info to
+    place prompt_end_frame (tts_demo.py:177-181)."""
+    with open(path, "rb") as f:
+        tag, ch, sr, bits, _, size = _wav_layout(f, path)
+    return AudioInfo(sr, size // _wav_frame_bytes(tag, ch, bits, path), ch)
+
+
+def read_wav(path, offset: int = -1, num_frames: int = -1):
+    """WAV PCM 16/24/32-bit or IEEE float 32-bit (plain or WAVE_FORMAT_EXTENSIBLE) -> (float32 ndarray [C, N], rate),
+    scaled as torchaudio.load scales it (integers over 2^15, 2^23, 2^31).  With offset and num_frames both given, the
+    frames [offset, offset + num_frames) at the file's rate, as torchaudio.load(frame_offset=, num_frames=) reads them."""
     import numpy as np
-    with wave.open(str(audio_path), "rb") as f:
-        sr, ch, n, width = f.getframerate(), f.getnchannels(), f.getnframes(), f.getsampwidth()
-        if width != 2:
-            raise ValueError("tokenize_audio: 16-bit PCM WAV expected")
+    with open(path, "rb") as f:
+        tag, ch, sr, bits, start, size = _wav_layout(f, path)
+        fb = _wav_frame_bytes(tag, ch, bits, path)
+        n = size // fb
+        first = 0
         if offset != -1 and num_frames != -1:
-            f.setpos(min(int(offset), n))
-            n = min(int(num_frames), n - f.tell())
-        pcm = np.frombuffer(f.readframes(n), dtype="<i2").reshape(-1, ch).T.astype(np.float32) / 32768.0
-    if sr != tokenizer.sample_rate:
-        raise ValueError(f"tokenize_audio: file is {sr} Hz, the codec runs at {tokenizer.sample_rate} Hz (resample first)")
-    wav = torch.from_numpy(np.ascontiguousarray(pcm))
-    if wav.shape[0] != tokenizer.channels:                    # convert_audio (:77-99): down-mix / broadcast
+            first = min(int(offset), n)
+            n = min(int(num_frames), n - first)
+        f.seek(start + first * fb)
+        raw = f.read(n * fb)
+    dtype, scale = _WAV_FORMATS[(tag, bits)]
+    if dtype is None:                                        # 24-bit: three little-endian bytes, sign-extended
+        b = np.frombuffer(raw, dtype=np.uint8).reshape(-1, 3).astype(np.int32)
+        x = ((b[:, 0] | (b[:, 1] << 8) | (b[:, 2] << 16)) << 8) >> 8
+    else:
+        x = np.frombuffer(raw, dtype=dtype)
+    x = x.reshape(-1, ch).T
+    pcm = x.astype(np.float32) if scale is None else x.astype(np.float32) / scale
+    return np.ascontiguousarray(pcm), sr
+
+
+def tokenize_audio(tokenizer: AudioTokenizer, audio_path: str, offset=-1, num_frames=-1):
+    """The reference's helper (data/tokenizer.py:137-149) without the torchaudio dependency: load a WAV file (read_wav;
+    optionally the window of `num_frames` frames from `offset` at the file's rate), mix it to the codec's channel count
+    and resample it to the codec's rate as convert_audio does (:85-97; AudioTokenizer.resample on the device), encode."""
+    pcm, sr = read_wav(audio_path, offset, num_frames)
+    wav = torch.from_numpy(pcm)
+    if wav.shape[0] not in (1, 2):
+        raise ValueError(f"{audio_path}: audio must be mono or stereo, it has {wav.shape[0]} channels")
+    if wav.shape[0] != tokenizer.channels:                    # convert_audio (:85-95): down-mix / broadcast
         wav = wav.mean(dim=0, keepdim=True).expand(tokenizer.channels, -1) if tokenizer.channels == 1 or wav.shape[0] > 1 \
             else wav.expand(tokenizer.channels, -1)
+    wav = wav.unsqueeze(0)
     with torch.no_grad():
-        return tokenizer.encode(wav.unsqueeze(0))
+        if sr != tokenizer.sample_rate:
+            wav = tokenizer.resample(wav.to(tokenizer.device), sr)
+        return tokenizer.encode(wav)

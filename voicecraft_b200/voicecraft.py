@@ -493,17 +493,21 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     # ------------------------------------------------------------------------------------------------
     # streaming: audio while the tokens are generated (TtsStream)
     # ------------------------------------------------------------------------------------------------
-    def inference_tts_many_stream(self, xs, ys, tokenizer, chunk_frames: int = 25, poll_every: int = 8, seeds=None, **kw):
+    # Every stream takes sample_rate=: chunks at that rate instead of the codec's, resampled on the device as they are
+    # decoded (CodecStream); concatenated they equal tokenizer.resample(<the codec-rate audio>, codec rate, sample_rate).
+    def inference_tts_many_stream(self, xs, ys, tokenizer, chunk_frames: int = 25, poll_every: int = 8, seeds=None,
+                                  sample_rate: int = None, **kw):
         """inference_tts_many with the audio handed out while it is generated: iterates (i, wav [1, channels, n*hop]),
         utterance i's chunks in order; concatenated they equal ``tokenizer.decode_codes(gen_i)``.  Afterwards
         ``.results`` equals what inference_tts_many returns.  `seeds` as in open_tts_session."""
         _no_stream_best_of(kw.get("best_of", 1))
         sess = self.open_tts_session(xs, ys, seeds=seeds, **kw)
-        return TtsStream(sess, tokenizer, chunk_frames, poll_every)
+        return TtsStream(sess, tokenizer, chunk_frames, poll_every, sample_rate)
 
     def inference_tts_stream(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, tokenizer, chunk_frames: int = 25,
                              poll_every: int = 8, top_k: int = -100, top_p: float = 1.0, temperature: float = 1.0,
-                             stop_repetition: int = 3, silence_tokens: List[int] = [1388, 1898, 131]):
+                             stop_repetition: int = 3, silence_tokens: List[int] = [1388, 1898, 131],
+                             sample_rate: int = None):
         """inference_tts with the audio handed out while it is generated: iterates wav chunks [1, channels, n*hop] whose
         concatenation equals ``tokenizer.decode([(gen, None)])``.  Afterwards ``.result`` is (res, gen), what inference_tts
         returns: the utterance samples from the device generator's stream at its current offset and leaves it advanced by
@@ -511,21 +515,21 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         assert x.ndim == 2 and x.shape[0] == 1 and x_lens.ndim == 1 and y.ndim == 3 and y.shape[0] == 1, (x.shape, y.shape)
         sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
                              n_copies=1)
-        return _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every)
+        return _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every, sample_rate)
 
     def inference_many_stream(self, xs, ys, mask_intervals, tokenizer, chunk_frames: int = 25, poll_every: int = 8,
-                              seeds=None, **kw):
+                              seeds=None, sample_rate: int = None, **kw):
         """inference_many with the audio handed out while it is generated: iterates (i, wav [1, channels, n*hop]),
         utterance i's chunks in order; concatenated they equal ``tokenizer.decode_codes(res_i)``, the whole edited
         utterance.  The frames before the first masked span are final at once, so they are the first chunk.  Afterwards
         ``.results`` equals what inference_many returns.  `seeds` as in open_tts_session; the device generators only."""
         sess = self.open_edit_session(xs, ys, mask_intervals, seeds=seeds, **kw)
-        return TtsStream(sess, tokenizer, chunk_frames, poll_every)
+        return TtsStream(sess, tokenizer, chunk_frames, poll_every, sample_rate)
 
     def inference_stream(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, mask_interval: torch.Tensor, tokenizer,
                          chunk_frames: int = 25, poll_every: int = 8, top_k: int = -100, top_p: float = 1.0,
                          temperature: float = 1.0, stop_repetition: int = -1, kvcache: int = 1,
-                         silence_tokens: List[int] = [1388, 1898, 131]):
+                         silence_tokens: List[int] = [1388, 1898, 131], sample_rate: int = None):
         """inference (speech editing) with the audio handed out while it is generated: iterates wav chunks
         [1, channels, n*hop] whose concatenation equals ``tokenizer.decode_codes(res)``, the whole edited utterance.
         Afterwards ``.result`` is res, what inference returns, and the device generator is left where inference leaves
@@ -534,7 +538,7 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         assert mask_interval.shape == torch.Size((1, mask_interval.shape[1], 2)), mask_interval
         sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
                              mask_intervals=[mask_interval], n_copies=1)
-        return _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every)
+        return _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every, sample_rate)
 
 
 def _check_best_of(best_of) -> int:
@@ -726,7 +730,7 @@ class _AudioStream:
         self._st, self._it = st, None
         st.codec = st.push = None
         try:
-            st.codec = st.tok.open_stream(max_streams=n_streams)
+            st.codec = st.tok.open_stream(max_streams=n_streams, sample_rate=st.sample_rate)
             st.cstream = torch.cuda.Stream(device=st.dev)
         except Exception:
             self.close()
@@ -783,7 +787,7 @@ class TtsStream(_AudioStream):
     ``DecodeSession.results()`` returns.  Closing it early (break, close(), garbage collection) releases the session's
     engine slots and the codec streams."""
 
-    def __init__(self, sess: "DecodeSession", tokenizer, chunk_frames: int = 25, poll_every: int = 8):
+    def __init__(self, sess: "DecodeSession", tokenizer, chunk_frames: int = 25, poll_every: int = 8, sample_rate=None):
         if chunk_frames < 1 or poll_every < 1:
             raise ValueError("chunk_frames and poll_every must be >= 1")
         if sess.n_copies > 1:
@@ -794,7 +798,8 @@ class TtsStream(_AudioStream):
             raise _lib.VcbError("streaming an edit needs the device generators (model.noise_fn / noise_fns must be None): "
                                 "the polls do not follow the forced hand-over steps, so host noise would be drawn for them")
         self._start(SimpleNamespace(sess=sess, dev=sess.dev, tok=tokenizer, chunk_frames=int(chunk_frames),
-                                    poll_every=int(poll_every), results=None, first_audio_steps=None), sess.B)
+                                    poll_every=int(poll_every), results=None, first_audio_steps=None,
+                                    sample_rate=sample_rate), sess.B)
 
     @property
     def results(self):
@@ -869,6 +874,9 @@ class _PushStep:
 
     An utterance (_Utterance) has its first chunk waits for max(chunk_frames, min_frames) frames, later ones for chunk_frames,
     the last one takes what is left; one that ends with fewer than min_frames frames is decoded whole (decode_codes).
+    Resampled (a codec stream with its own sample_rate), an utterance's last push is marked final; one that ends at a
+    poll with no new frame has its resampler tail flushed, and one decoded whole is resampled in one call.  A chunk that
+    resamples to no sample is not handed out unless it closes its utterance.
     A chunk holding a non-audio code fails its utterance before any of its codes reach the codec: `strict` raises
     VcbError before the codec is called at all."""
 
@@ -877,6 +885,7 @@ class _PushStep:
         self.lib, self.eng, self.stream, self.tok, self.codec, self.cstream = _lib.load(), eng, stream, tokenizer, codec, cstream
         self.dev, self.K, self.strict = model.mask_embedding.device, a.n_codebooks, strict
         self.chunk_frames, self.first = chunk_frames, max(chunk_frames, codec.min_frames)
+        self.resampled = codec.sample_rate != tokenizer.sample_rate
         # new frames at one poll: fewer than a chunk's threshold were left over, plus at most one per row sampled since the
         # last poll (a newly admitted utterance: its first sample and poll_every steps)
         self.max_frames = self.first + poll_every + 1
@@ -898,7 +907,7 @@ class _PushStep:
                                           int(self.tok.config.bins), codes.data_ptr(), status, final, bad, self.stream))
         waited = time.perf_counter() - t0
         _check_capacity(status)
-        push, whole, failed = {}, {}, {}
+        push, whole, failed, flush = {}, {}, {}, []
         for j, r in enumerate(live):
             fin, f = bool(status[j].done), int(final[j])
             new = f - r.pushed
@@ -908,6 +917,8 @@ class _PushStep:
                 push[j] = min(new, mf)
             else:
                 r.closed = fin and r.pushed == f
+                if r.closed and r.pushed > 0 and self.resampled:     # its last push was not final: the tail is pending
+                    flush.append(j)
                 continue
             if bad[3 * j] >= 0:
                 failed[r] = (f"{r.label}: frame {bad[3 * j]} holds the non-audio token {bad[3 * j + 2]} in codebook "
@@ -920,30 +931,41 @@ class _PushStep:
             r.closed = fin and r.pushed == f
         if failed and self.strict:
             raise _lib.VcbError(next(iter(failed.values())))
-        wav, wavs = None, {}
-        if push or any(whole.values()):      # the codec works on its own CUDA stream ...
+        wav, tail, wavs = None, None, {}
+        wav_lens = tail_lens = None
+        if push or any(whole.values()) or flush:     # the codec works on its own CUDA stream ...
             with torch.cuda.stream(self.cstream):
                 codes.record_stream(self.cstream)
                 if push:
                     rows = list(push)
                     wav = self.codec.decode(codes[rows, :, :max(push.values())], ids=[live[j].cid for j in rows],
-                                            lens=list(push.values()))
+                                            lens=list(push.values()),
+                                            final=[live[j].closed for j in rows] if self.resampled else None)
+                    wav_lens = self.codec.out_lens
+                if flush:
+                    tail = self.codec.flush([live[j].cid for j in flush])
+                    tail_lens = self.codec.out_lens
                 for j, f in whole.items():
                     if f > 0:
                         wavs[j] = self.tok.decode_codes(codes[j:j + 1, :, :f])
+                        if self.resampled:
+                            wavs[j] = self.tok.resample(wavs[j], self.tok.sample_rate, self.codec.sample_rate)
             ev = torch.cuda.Event()
             ev.record(self.cstream)
         t1 = time.perf_counter()
         advance(status)                      # ... while the next steps are already queued on the LM's
         t2 = time.perf_counter()
         out = []
-        if wav is not None or wavs:
+        if wav is not None or tail is not None or wavs:
             ev.synchronize()
             cur = torch.cuda.current_stream(self.dev)
-            if wav is not None:
-                wav.record_stream(cur)
-                for b, (j, nw) in enumerate(push.items()):
-                    wavs[j] = wav[b:b + 1, :, :nw * self.tok.hop]
+            for out_wav, rows, lens in ((wav, list(push), wav_lens), (tail, flush, tail_lens)):
+                if out_wav is None:
+                    continue
+                out_wav.record_stream(cur)
+                for b, j in enumerate(rows):
+                    if lens[b] > 0:
+                        wavs[j] = out_wav[b:b + 1, :, :lens[b]]
             for w in wavs.values():
                 w.record_stream(cur)
         t3 = time.perf_counter()
@@ -1288,7 +1310,7 @@ class ContinuousBatcher:
             self.queue = []
         return results
 
-    def stream(self, tokenizer, chunk_frames: int = 25) -> "BatcherStream":
+    def stream(self, tokenizer, chunk_frames: int = 25, sample_rate: int = None) -> "BatcherStream":
         """run() with every utterance's audio handed out while it is generated: iterates (ticket, wav [1, channels, n*hop],
         last).  A ticket's chunks, concatenated, equal ``tokenizer.decode_codes(gen)`` (an edit ticket's:
         ``decode_codes(res)``, the whole edited utterance, whose frames before the first masked span are its first chunk);
@@ -1296,15 +1318,17 @@ class ContinuousBatcher:
         (an utterance that generated no frame yields one empty wav).  submit() and cancel() may be called from the loop
         body.  Afterwards ``results[ticket]`` is (res, gen) as run() returns it, None for a cancelled or failed ticket;
         ``errors[ticket]`` says why a ticket failed (a final frame holding a non-audio token: it yields (ticket, None,
-        True) and the others go on).  The engine gets `max_concurrency` slots, each with its own codec stream id."""
-        return BatcherStream(self, tokenizer, chunk_frames)
+        True) and the others go on).  The engine gets `max_concurrency` slots, each with its own codec stream id.
+        sample_rate: chunks at that rate, resampled on the device as they are decoded; concatenated they equal
+        ``tokenizer.resample(<the codec-rate audio>, codec rate, sample_rate)``."""
+        return BatcherStream(self, tokenizer, chunk_frames, sample_rate)
 
 
 class BatcherStream(_AudioStream):
     """Iterator of ContinuousBatcher.stream().  Closing it early (break, close(), garbage collection) releases the
     batcher's engine slots and the codec streams."""
 
-    def __init__(self, cb: ContinuousBatcher, tokenizer, chunk_frames: int = 25):
+    def __init__(self, cb: ContinuousBatcher, tokenizer, chunk_frames: int = 25, sample_rate=None):
         m = cb.model
         if m.noise_fn is not None:
             raise _lib.VcbError("ContinuousBatcher uses the per-utterance device generators (model.noise_fn must be None)")
@@ -1318,7 +1342,7 @@ class BatcherStream(_AudioStream):
         refused = {t for t, j in enumerate(jobs) if j[2] > 1}
         st = SimpleNamespace(cb=cb, eng=eng, slots=slots, max_seq=m._eng_opts["max_seq_len"], jobs=jobs,
                              cancelled=set(refused), ended=set(refused), refused=sorted(refused), tok=tokenizer,
-                             chunk_frames=int(chunk_frames), dev=m.mask_embedding.device)
+                             chunk_frames=int(chunk_frames), dev=m.mask_embedding.device, sample_rate=sample_rate)
         cb.results, cb._live = [None] * len(jobs), st
         cb.errors = {t: f"best_of={jobs[t][2]}: stream() serves only best_of=1 tickets" for t in refused}
         self._start(st, cb.B)
