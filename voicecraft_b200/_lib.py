@@ -75,6 +75,8 @@ PROTOTYPES = {
     "vcb_debug_attention": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 4 + [C.c_int32] * 7 + [C.c_void_p]),
     "vcb_debug_attention_groups": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 2 + [C.c_int32] * 7 +
                                    [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32]),
+    "vcb_debug_kv_quantize": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
+    "vcb_debug_kv_pages": (C.c_int, [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 2),
     "vcb_debug_fold_chain": (C.c_int, [C.c_void_p] * 8 + [C.c_int32] * 7 + [C.c_void_p] * 2),
     "vcb_timeline": (C.c_int, [C.c_int32, C.POINTER(C.c_uint64), C.c_int32, C.POINTER(C.c_int32)]),
     "vcb_bench_gemm": (C.c_int, [C.c_int32] * 8 + [C.POINTER(C.c_float)]),

@@ -49,8 +49,12 @@ __device__ __forceinline__ float act_fn(float v, int kind) {
     return v;
 }
 
-// 32 consecutive features [f0, f0+32) of token row `row`, accumulator values in v[]
-__device__ __forceinline__ void rows_epilogue32(const GemmEpilogue& ep, int row, int f0, float (&v)[32]) {
+// 32 consecutive features [f0, f0+32) of token row `row`, accumulator values in v[]; `acc` points at the staged accumulator
+// of feature f0 in the row, which holds every feature of f0's head (the fp8 KV scale is taken over the whole head).
+// kv_amax / kv_head: the fp8 amax of the head whose first feature is kv_head, kept across the calls of one row, so each
+// (row, head) amax is computed once
+__device__ __forceinline__ void rows_epilogue32(const GemmEpilogue& ep, int row, int f0, float (&v)[32], const float* acc,
+                                                float& kv_amax, int& kv_head) {
 #pragma unroll
     for (int j = 0; j < 32; ++j) v[j] += ep.bias[f0 + j];         // same address in every lane: broadcast
     switch (ep.mode) {
@@ -68,7 +72,29 @@ __device__ __forceinline__ void rows_epilogue32(const GemmEpilogue& ep, int row,
             const int h = cc / ep.hd, e0 = cc - h * ep.hd;          // hd % 32 == 0: the 32 features share a head
             const size_t off = ((static_cast<size_t>(page) * ep.H + h) * ep.page_size + pos % ep.page_size) * ep.hd + e0;
             void* pool = (part == 1) ? ep.kpool : ep.vpool;
-            if (ep.kv_fp32) {
+            if (ep.kv_fp8) {
+                // the head's values are its staged accumulators plus bias, the same fp32 sums as v[]
+                if (kv_head != f0 - e0) {
+                    kv_head = f0 - e0;
+                    kv_amax = 0.f;
+                    for (int j = 0; j < ep.hd; ++j) kv_amax = fmaxf(kv_amax, fabsf(acc[j - e0] + ep.bias[kv_head + j]));
+                }
+                float inv;
+                const float scale = kv_fp8_scale(kv_amax, inv);
+                const int t = pos % ep.page_size;
+                uint8_t* s = static_cast<uint8_t*>(pool) + (static_cast<size_t>(page) * ep.H + h) * kv_slab_bytes(KV_FP8, ep.hd);
+                uint4* dst = reinterpret_cast<uint4*>(s + t * ep.hd + e0);
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    uint32_t w[4];
+#pragma unroll
+                    for (int i = 0; i < 4; ++i)
+                        w[i] = kv_fp8_pack2(v[16 * j + 4 * i], v[16 * j + 4 * i + 1], inv) |
+                               (static_cast<uint32_t>(kv_fp8_pack2(v[16 * j + 4 * i + 2], v[16 * j + 4 * i + 3], inv)) << 16);
+                    dst[j] = make_uint4(w[0], w[1], w[2], w[3]);
+                }
+                if (e0 == 0) reinterpret_cast<float*>(s + ep.page_size * ep.hd)[t] = scale;
+            } else if (ep.kv_fp32) {
                 float4* dst = reinterpret_cast<float4*>(static_cast<float*>(pool) + off);
 #pragma unroll
                 for (int j = 0; j < 8; ++j) dst[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
@@ -227,6 +253,8 @@ gemm_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         const int row = r0 + q * 32 + lane;
         pdl_wait();                                         // residual rows / KV positions come from earlier kernels
         const float* arow = sacc + (q * 32 + lane) * L::ACC_LD;
+        float kv_amax = 0.f;
+        int kv_head = -1;
 #pragma unroll 1
         for (int c = half * (BN / 2); c < (half + 1) * (BN / 2); c += 32) {
             float v[32];
@@ -235,7 +263,7 @@ gemm_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
                 const float4 t = *reinterpret_cast<const float4*>(arow + c + j);
                 v[j] = t.x; v[j + 1] = t.y; v[j + 2] = t.z; v[j + 3] = t.w;
             }
-            if (row < rows && n0 + c < Nout) rows_epilogue32(ep, row, n0 + c, v);
+            if (row < rows && n0 + c < Nout) rows_epilogue32(ep, row, n0 + c, v, arow + c, kv_amax, kv_head);
         }
     }
 }

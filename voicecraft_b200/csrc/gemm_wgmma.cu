@@ -166,7 +166,8 @@ __device__ __forceinline__ void apply_epilogue4(const GemmEpilogue& ep, int row0
     }
 }
 
-template <int BN, int STAGES>
+// KV8: the QKV launch of an fp8-KV engine (its own instantiation, so the other epilogues keep their register budget)
+template <int BN, int STAGES, bool KV8 = false>
 __global__ void __launch_bounds__(gemm_threads(BN))
 gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const GemmEpilogue ep, int Nout, int total_kb, int kb_per_split, int b_col_off, int nvalid,
@@ -404,7 +405,49 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 }
                 sum[u] = a;
             }
-            if (valid_m) apply_epilogue4(ep, row0, nrows, m, sum, bias, xnew, colx, e_x_valid ? e_x : nullptr);
+            if (KV8 && m0 + GEMM_BM > ep.d) {
+                // fp8 K / V (a tile of K or V features, or one that straddles Q|K): each row's amax over a head is a warp
+                // max combined through shared memory behind the half's barrier, over the hd / 32 warps of the head
+                // (heads are 64-aligned, so a head never crosses a warp pair); s_part is free, QKV tiles do not emit
+                float val[4];
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    val[u] = sum[u] + bias;
+                    const float am = warp_max(u < nrows ? fabsf(val[u]) : 0.f);
+                    if (lane == 0) s_part[q][u][0] = am;
+                }
+                if (half == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
+                else asm volatile("bar.sync 3, 128;" ::: "memory");
+                const int wph = ep.hd / 32, w0 = q & ~(wph - 1);
+                float amax[4];
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    amax[u] = s_part[w0][u][0];
+                    for (int w = 1; w < wph; ++w) amax[u] = fmaxf(amax[u], s_part[w0 + w][u][0]);
+                }
+                if (half == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
+                else asm volatile("bar.sync 3, 128;" ::: "memory");
+                if (valid_m && m < ep.d) {
+                    apply_epilogue4(ep, row0, nrows, m, sum, bias, xnew);
+                } else if (valid_m) {
+                    const int part = m / ep.d, cc = m - part * ep.d, h = cc / ep.hd, e = cc - h * ep.hd;
+                    uint8_t* pool = static_cast<uint8_t*>(part == 1 ? ep.kpool : ep.vpool);
+                    const int slab = kv_slab_bytes(KV_FP8, ep.hd);
+#pragma unroll
+                    for (int u = 0; u < 4; ++u) {
+                        const int pos = u < nrows ? ep.row_pos[row0 + u] : -1;
+                        if (pos < 0) continue;
+                        const int page = ep.row_page ? ep.row_page[row0 + u]
+                                                     : ep.page_table[ep.row_slot[row0 + u] * ep.max_pages + pos / ep.page_size];
+                        const int t = pos % ep.page_size;
+                        uint8_t* s = pool + (static_cast<size_t>(page) * ep.H + h) * slab;
+                        float inv;
+                        const float scale = kv_fp8_scale(amax[u], inv);
+                        s[t * ep.hd + e] = static_cast<uint8_t>(kv_fp8_pack2(val[u], 0.f, inv) & 0xff);
+                        if (e == 0) reinterpret_cast<float*>(s + ep.page_size * ep.hd)[t] = scale;
+                    }
+                }
+            } else if (valid_m) apply_epilogue4(ep, row0, nrows, m, sum, bias, xnew, colx, e_x_valid ? e_x : nullptr);
             if (ep.emit) {
                 // next GEMM's operand gamma_next * x_new (hi/lo) and this tile's (sum x, M2 about the tile mean) per row:
                 // each warp sums its 32 features, and their powers shifted by one of them (lane 0's, within the row's
@@ -699,8 +742,19 @@ static int launch_one(const GemmCall& g, int splits, cudaStream_t st) {
     cfg.numAttrs = g.pdl ? 2 : 1;
     const int total_kb = g.Kdim / GEMM_BK;
     const int kbps = (total_kb + splits - 1) / splits;
-    VCB_CUDA_OK(cudaLaunchKernelEx(&cfg, gemm_w_xT_cluster<BN, STAGES>, *g.tmA, *g.tmB, g.ep, g.Nout, total_kb, kbps,
-                                   g.b_col_off, g.nvalid, g.pf_ptr, static_cast<unsigned long long>(g.pf_bytes), g.grp));
+    auto kern = gemm_w_xT_cluster<BN, STAGES>;
+    if (g.ep.mode == EPI_QKV && g.ep.kv_fp8) {
+        // same shared memory and cluster shapes as the plain instantiation, whose occupancy chose the split count
+        kern = gemm_w_xT_cluster<BN, STAGES, true>;
+        static bool attr_set = false;
+        if (!attr_set) {
+            VCB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
+            VCB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+            attr_set = true;
+        }
+    }
+    VCB_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, *g.tmA, *g.tmB, g.ep, g.Nout, total_kb, kbps, g.b_col_off, g.nvalid, g.pf_ptr,
+                                   static_cast<unsigned long long>(g.pf_bytes), g.grp));
     return 0;
 }
 

@@ -49,12 +49,13 @@ struct Layer {
 }  // namespace vcb
 
 using namespace vcb;
+static_assert(KV_BF16 == VCB_KV_BF16 && KV_FP32 == VCB_KV_FP32 && KV_FP8 == VCB_KV_FP8, "KV policy ids of vcb_internal.h");
 
 struct vcb_engine {
     vcb_config cfg;
     ModelDims m;
     int num_sms = 132;
-    int kv_fp32 = 0;
+    int kv_dtype = KV_BF16;           // VCB_KV_* (vcb_config.kv_dtype)
     int max_pages_per_slot = 0, n_pages = 0;
     std::vector<int> free_pages;
     std::vector<int> page_refs;       // slots whose page list holds the page (a best-of-N group shares its full prompt pages)
@@ -284,7 +285,7 @@ struct AttnLaunch {
     const void *kpool = nullptr, *vpool = nullptr;
     const int *page_table = nullptr, *row_slot = nullptr, *row_pos = nullptr;
     const int* row_pages = nullptr;       // [rows][max_pages] or null: pages through page_table + row_slot
-    int max_pages = 0, rows = 0, H = 0, hd = 0, kv_fp32 = 0, max_ctx = 0;
+    int max_pages = 0, rows = 0, H = 0, hd = 0, kv_dtype = KV_BF16, max_ctx = 0;
     __nv_bfloat16* act = nullptr;         // hi rows [rows][ld_act], lo rows bpad rows further
     int ld_act = 0, bpad = 0;
     float* ws = nullptr;                  // [rows * H][maxch][hd + 2]
@@ -333,8 +334,10 @@ int launch_attn_rows(const AttnLaunch& a, cudaStream_t st) {
         set_error("attention: head dim %d (64 or 128 supported)", a.hd);
         return -1;
     }
-    if (a.kv_fp32)
+    if (a.kv_dtype == KV_FP32)
         return a.hd == 128 ? launch_attn_kv<float, 128>(a, st) : launch_attn_kv<float, 64>(a, st);
+    if (a.kv_dtype == KV_FP8)
+        return a.hd == 128 ? launch_attn_kv<__nv_fp8_e4m3, 128>(a, st) : launch_attn_kv<__nv_fp8_e4m3, 64>(a, st);
     return a.hd == 128 ? launch_attn_kv<__nv_bfloat16, 128>(a, st) : launch_attn_kv<__nv_bfloat16, 64>(a, st);
 }
 
@@ -459,7 +462,8 @@ LayerEpilogues layer_epilogues(const vcb_engine* e, int l, const Pass& p) {
     q.row_slot = p.slot;
     q.row_pos = p.pos;
     q.row_page = p.page;
-    q.kv_fp32 = e->kv_fp32;
+    q.kv_fp32 = e->kv_dtype == KV_FP32;
+    q.kv_fp8 = e->kv_dtype == KV_FP8;
     q.max_pages = e->max_pages_per_slot;
     q.page_size = KV_PAGE;
     q.d = m.d;
@@ -535,7 +539,7 @@ int launch_attn(vcb_engine* e, const Pass& p, const Layer& Ly, cudaStream_t st) 
     a.rows = p.rows;
     a.H = m.H;
     a.hd = m.hd;
-    a.kv_fp32 = e->kv_fp32;
+    a.kv_dtype = e->kv_dtype;
     a.max_ctx = p.max_ctx;
     a.act = p.act_d.act;
     a.ld_act = m.d;
@@ -701,8 +705,9 @@ int mega_build(vcb_engine* e, int bpad) {
 int mega_setup(vcb_engine* e) {
     const ModelDims& m = e->m;
     e->mega_grid = 0;
-    if (!e->opt_mega || !e->opt_fold || e->opt_simt || m.hd != 128 || m.d % 128 || m.F % 128 || (m.K * m.Hh) % 128 || m.Hh % 64) return 0;
-    int grid = std::min(mega_max_grid(32, e->kv_fp32), mega_max_grid(16, e->kv_fp32));
+    // (the persistent kernel has no fp8 KV path: fp8 engines take the per-kernel step)
+    if (!e->opt_mega || !e->opt_fold || e->opt_simt || e->kv_dtype == KV_FP8 || m.hd != 128 || m.d % 128 || m.F % 128 || (m.K * m.Hh) % 128 || m.Hh % 64) return 0;
+    int grid = std::min(mega_max_grid(32, e->kv_dtype == KV_FP32), mega_max_grid(16, e->kv_dtype == KV_FP32));
     if (getenv("VCB_MEGA_GRID")) grid = std::min(grid, atoi(getenv("VCB_MEGA_GRID")));
     if (grid < 1) return 0;
     // a CTA's block range may touch at most MEGA_MAXSEG output tiles of a phase
@@ -772,7 +777,7 @@ int mega_step(vcb_engine* e, int n, cudaStream_t st) {
     a.nph = e->mega_nph;
     a.nvalid = n;
     a.bpad = bpad;
-    a.kv_fp32 = e->kv_fp32;
+    a.kv_fp32 = e->kv_dtype == KV_FP32;
     a.ns = e->mega_ns;
     a.nb = e->mega_nb;
     a.pf = e->mega_pf;
@@ -984,6 +989,15 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
         set_error("null argument");
         return -1;
     }
+    if (cfg->kv_dtype != VCB_KV_BF16 && cfg->kv_dtype != VCB_KV_FP32 && cfg->kv_dtype != VCB_KV_FP8) {
+        set_error("kv_dtype %d: VCB_KV_BF16 (0), VCB_KV_FP32 (1) or VCB_KV_FP8 (2)", cfg->kv_dtype);
+        return -1;
+    }
+    const char* simt = getenv("VCB_GEMM_IMPL");
+    if (simt && !strcmp(simt, "simt") && cfg->kv_dtype == VCB_KV_FP8) {
+        set_error("VCB_GEMM_IMPL=simt: the CUDA-core cross-check GEMM has no fp8 KV epilogue");
+        return -1;
+    }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         set_error("no CUDA device: libvcb200 has no CPU fallback");
@@ -1022,7 +1036,7 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
         delete e;
         return -1;
     }
-    e->kv_fp32 = cfg->kv_dtype == VCB_KV_FP32;
+    e->kv_dtype = cfg->kv_dtype;
     e->max_pages_per_slot = (cfg->max_seq_len + KV_PAGE - 1) / KV_PAGE;
     e->n_pages = e->max_pages_per_slot * cfg->max_slots;
     for (int p = e->n_pages - 1; p >= 0; --p) e->free_pages.push_back(p);
@@ -1039,7 +1053,6 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
     for (int g = cfg->max_slots - 1; g >= 0; --g) e->free_groups.push_back(g);
     e->layers.resize(m.L);
     e->h2.resize(m.K);
-    const char* simt = getenv("VCB_GEMM_IMPL");
     e->opt_simt = simt && !strcmp(simt, "simt");
     const char* pdl = getenv("VCB_PDL");
     e->opt_pdl = pdl ? atoi(pdl) : 1;
@@ -1130,8 +1143,7 @@ int vcb_finalize_weights(vcb_engine* e) {
         for (const char* w : {"self_attn.in_proj_weight", "self_attn.out_proj.weight", "linear1.weight", "linear2.weight"})
             e->f32.erase(K(w));            // bf16 copy made: drop the fp32 staging copy
         // KV pool for this layer
-        const size_t elems = static_cast<size_t>(e->n_pages) * m.H * KV_PAGE * m.hd;
-        const size_t bytes = elems * (e->kv_fp32 ? 4 : 2);
+        const size_t bytes = static_cast<size_t>(e->n_pages) * m.H * kv_slab_bytes(e->kv_dtype, m.hd);
         if (L.kpool.ensure(bytes, true) || L.vpool.ensure(bytes, true)) return -1;
     }
     if (need(e, "decoder.norm.weight", &e->lnf_g, m.d) || need(e, "decoder.norm.bias", &e->lnf_b, m.d)) return -1;
@@ -1422,7 +1434,7 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
     }
     e->n_prefill_rows += static_cast<int64_t>(total_rows);
     if (!fork.empty()) {
-        const int page_words = static_cast<int>(static_cast<size_t>(m.H) * KV_PAGE * m.hd * (e->kv_fp32 ? 4 : 2) / 16);
+        const int page_words = m.H * kv_slab_bytes(e->kv_dtype, m.hd) / 16;
         const long long words = static_cast<long long>(fork.size()) * (2LL * m.L * page_words + m.d / 4);
         const int grid = static_cast<int>(std::min<long long>((words + 255) / 256, 4LL * e->num_sms));
         ProfScope ps(e, PC_MISC, st);
@@ -1761,12 +1773,13 @@ int vcb_debug_gemm(const float* W_dev, const float* X_dev, float* out_dev, int32
 // Parity hooks of the paged attention (attn_rows_kernel) with the engine's launch decisions; see include/vcb200.h.
 // group_first null: every row on its own (GMAX = 1); else the row groups, checked here and split into launch groups of
 // at most ATT_GMAX rows
-static int debug_attention(const float* q_dev, const void* kpool_dev, const void* vpool_dev, int32_t kv_fp32,
+static int debug_attention(const float* q_dev, const void* kpool_dev, const void* vpool_dev, int32_t kv_dtype,
                            const int32_t* row_pages_dev, const int32_t* page_table_dev, const int32_t* row_slot_dev,
                            const int32_t* pos_dev, int32_t rows, int32_t H, int32_t hd, int32_t max_pages, int32_t chunk_pages,
                            int32_t balance, int32_t repeats, float* out_dev, const int32_t* group_first,
                            const int32_t* group_shared, int32_t n_groups) {
-    if (rows < 1 || H < 1 || (hd != 64 && hd != 128) || max_pages < 1 || repeats < 1 || !q_dev || !kpool_dev || !vpool_dev ||
+    if (rows < 1 || H < 1 || (hd != 64 && hd != 128) || max_pages < 1 || repeats < 1 || kv_dtype < KV_BF16 || kv_dtype > KV_FP8 ||
+        !q_dev || !kpool_dev || !vpool_dev ||
         !pos_dev || !out_dev || (!row_pages_dev && (!page_table_dev || !row_slot_dev))) {
         set_error("vcb_debug_attention: bad argument");
         return -1;
@@ -1831,7 +1844,7 @@ static int debug_attention(const float* q_dev, const void* kpool_dev, const void
     a.rows = rows;
     a.H = H;
     a.hd = hd;
-    a.kv_fp32 = kv_fp32;
+    a.kv_dtype = kv_dtype;
     a.max_ctx = max_ctx;
     a.ld_act = H * hd;
     a.bpad = rows;
@@ -1865,15 +1878,15 @@ static int debug_attention(const float* q_dev, const void* kpool_dev, const void
     return 0;
 }
 
-int vcb_debug_attention(const float* q_dev, const void* kpool_dev, const void* vpool_dev, int32_t kv_fp32,
+int vcb_debug_attention(const float* q_dev, const void* kpool_dev, const void* vpool_dev, int32_t kv_dtype,
                         const int32_t* row_pages_dev, const int32_t* page_table_dev, const int32_t* row_slot_dev,
                         const int32_t* pos_dev, int32_t rows, int32_t H, int32_t hd, int32_t max_pages, int32_t chunk_pages,
                         int32_t balance, int32_t repeats, float* out_dev) {
-    return debug_attention(q_dev, kpool_dev, vpool_dev, kv_fp32, row_pages_dev, page_table_dev, row_slot_dev, pos_dev, rows, H,
+    return debug_attention(q_dev, kpool_dev, vpool_dev, kv_dtype, row_pages_dev, page_table_dev, row_slot_dev, pos_dev, rows, H,
                            hd, max_pages, chunk_pages, balance, repeats, out_dev, nullptr, nullptr, 0);
 }
 
-int vcb_debug_attention_groups(const float* q_dev, const void* kpool_dev, const void* vpool_dev, int32_t kv_fp32,
+int vcb_debug_attention_groups(const float* q_dev, const void* kpool_dev, const void* vpool_dev, int32_t kv_dtype,
                                const int32_t* row_pages_dev, const int32_t* pos_dev, int32_t rows, int32_t H, int32_t hd,
                                int32_t max_pages, int32_t chunk_pages, int32_t balance, int32_t repeats, float* out_dev,
                                const int32_t* group_first, const int32_t* group_shared, int32_t n_groups) {
@@ -1881,8 +1894,41 @@ int vcb_debug_attention_groups(const float* q_dev, const void* kpool_dev, const 
         set_error("vcb_debug_attention_groups: group_first is null");
         return -1;
     }
-    return debug_attention(q_dev, kpool_dev, vpool_dev, kv_fp32, row_pages_dev, nullptr, nullptr, pos_dev, rows, H, hd,
+    return debug_attention(q_dev, kpool_dev, vpool_dev, kv_dtype, row_pages_dev, nullptr, nullptr, pos_dev, rows, H, hd,
                            max_pages, chunk_pages, balance, repeats, out_dev, group_first, group_shared, n_groups);
+}
+
+// Parity hooks of the fp8 KV policy: the epilogues' quantizer alone, and the raw slabs an engine wrote; see include/vcb200.h.
+int vcb_debug_kv_quantize(const float* x_dev, int32_t rows, int32_t hd, uint8_t* out_dev) {
+    if (!x_dev || !out_dev || rows < 1 || (hd != 64 && hd != 128)) {
+        set_error("vcb_debug_kv_quantize: rows >= 1, hd 64 or 128, non-null pointers required");
+        return -1;
+    }
+    kv_quantize_kernel<<<rows, hd>>>(x_dev, hd, out_dev, reinterpret_cast<float*>(out_dev + static_cast<size_t>(rows) * hd));
+    VCB_CUDA_OK(cudaGetLastError());
+    VCB_CUDA_OK(cudaDeviceSynchronize());
+    return 0;
+}
+
+int vcb_debug_kv_pages(vcb_engine* e, int32_t layer, int32_t slot, int32_t first_page, int32_t n_pages, void* k_host,
+                       void* v_host) {
+    if (!e || !k_host || !v_host || layer < 0 || layer >= e->m.L || !e->layers[layer].kpool || slot < 0 ||
+        slot >= e->cfg.max_slots || first_page < 0 || n_pages < 1 ||
+        static_cast<size_t>(first_page) + n_pages > e->slot_pages[slot].size()) {
+        set_error("vcb_debug_kv_pages: layer %d, slot %d, pages %d .. %d: not a finalized engine's layer or the slot's pages",
+                  layer, slot, first_page, first_page + n_pages - 1);
+        return -1;
+    }
+    VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
+    VCB_CUDA_OK(cudaDeviceSynchronize());
+    const size_t page_bytes = static_cast<size_t>(e->m.H) * kv_slab_bytes(e->kv_dtype, e->m.hd);
+    const Layer& Ly = e->layers[layer];
+    for (int i = 0; i < n_pages; ++i) {
+        const size_t src = static_cast<size_t>(e->slot_pages[slot][first_page + i]) * page_bytes;
+        VCB_CUDA_OK(cudaMemcpy(static_cast<uint8_t*>(k_host) + i * page_bytes, Ly.kpool + src, page_bytes, cudaMemcpyDeviceToHost));
+        VCB_CUDA_OK(cudaMemcpy(static_cast<uint8_t*>(v_host) + i * page_bytes, Ly.vpool + src, page_bytes, cudaMemcpyDeviceToHost));
+    }
+    return 0;
 }
 
 // Parity hook of the decode pair "out-projection -> LN2 -> FFN1" on the per-kernel GEMM path; see include/vcb200.h.
@@ -2086,7 +2132,13 @@ int vcb_profile_read(vcb_engine* e, double* ms_by_class, int64_t* count_by_class
 }
 
 int vcb_set_option(vcb_engine* e, const char* name, int32_t value) {
-    if (!strcmp(name, "gemm_simt")) e->opt_simt = value;
+    if (!strcmp(name, "gemm_simt")) {
+        if (value && e->kv_dtype == KV_FP8) {
+            set_error("gemm_simt: the CUDA-core cross-check GEMM has no fp8 KV epilogue");
+            return -1;
+        }
+        e->opt_simt = value;
+    }
     else if (!strcmp(name, "profile")) e->opt_profile = value;
     else if (!strcmp(name, "pdl")) e->opt_pdl = value;
     else {
@@ -2105,7 +2157,7 @@ int64_t vcb_counter(vcb_engine* e, const char* name) {
     if (!strcmp(name, "poll_frames")) return e->n_poll_frames;
     if (!strcmp(name, "kv_pages_free")) return static_cast<int64_t>(e->free_pages.size());
     if (!strcmp(name, "prefill_rows")) return e->n_prefill_rows;
-    if (!strcmp(name, "kv_bytes_per_token")) return static_cast<int64_t>(e->m.L) * 2 * e->m.d * (e->kv_fp32 ? 4 : 2);
+    if (!strcmp(name, "kv_bytes_per_token")) return static_cast<int64_t>(e->m.L) * 2 * e->m.H * kv_slab_bytes(e->kv_dtype, e->m.hd) / KV_PAGE;
     return -1;
 }
 

@@ -162,6 +162,22 @@ __global__ void fork_group_kernel(uint8_t* const* __restrict__ pools /*[n_pools]
     }
 }
 
+// The fp8 KV quantizer of the QKV epilogues alone (vcb_debug_kv_quantize): one CTA of hd threads per row
+__global__ void kv_quantize_kernel(const float* __restrict__ x, int hd, uint8_t* __restrict__ bytes, float* __restrict__ scales) {
+    __shared__ float red[4];
+    const int r = blockIdx.x, i = threadIdx.x;
+    const float v = x[static_cast<size_t>(r) * hd + i];
+    const float am = warp_max(fabsf(v));
+    if ((i & 31) == 0) red[i >> 5] = am;
+    __syncthreads();
+    float amax = red[0];
+    for (int w = 1; w < hd / 32; ++w) amax = fmaxf(amax, red[w]);
+    float inv;
+    const float scale = kv_fp8_scale(amax, inv);
+    bytes[static_cast<size_t>(r) * hd + i] = static_cast<uint8_t>(kv_fp8_pack2(v, 0.f, inv) & 0xff);
+    if (i == 0) scales[r] = scale;
+}
+
 // fp32 rows -> bf16 hi/lo rows (bring-up hook vcb_debug_gemm only)
 __global__ void split_rows_kernel(const float* __restrict__ x, int N, __nv_bfloat16* __restrict__ act, int ld_act,
                                   int bpad) {
@@ -184,9 +200,14 @@ __global__ void split_rows_kernel(const float* __restrict__ x, int N, __nv_bfloa
 //   PV : warp w owns keys [16w,16w+16) of the page, lane owns hd/32 output dims
 // Output: bf16 hi/lo rows for the out-projection GEMM.
 // ---------------------------------------------------------------------------------------------------
+// KVT: __nv_bfloat16, float, or __nv_fp8_e4m3 (fp8 slabs carry the tokens' scales after the bytes: sc = q.k * kscale * scale,
+// and PV weights e^(s - m) * vscale while l sums the unscaled e^(s - m)).
+template <typename KVT>
+constexpr int kv_dtype_of() { return sizeof(KVT) == 1 ? KV_FP8 : sizeof(KVT) == 4 ? KV_FP32 : KV_BF16; }
+
 template <typename KVT, int HD>
 struct AttSmem {
-    static constexpr int PAGE_BYTES = KV_PAGE * HD * sizeof(KVT);
+    static constexpr int PAGE_BYTES = kv_slab_bytes(kv_dtype_of<KVT>(), HD);
     static constexpr int OFF_V = ATT_STAGES * PAGE_BYTES;
     static constexpr int OFF_SC = 2 * ATT_STAGES * PAGE_BYTES;
     static constexpr int OFF_PW = OFF_SC + 2 * KV_PAGE * 4;          // scores double-buffered by page parity
@@ -197,7 +218,24 @@ struct AttSmem {
 
 template <typename KVT, int N>
 __device__ __forceinline__ void load_kv_vec(const KVT* p, float (&out)[N]) {
-    if constexpr (sizeof(KVT) == 2) {
+    if constexpr (sizeof(KVT) == 1) {
+        uint32_t w[(N + 3) / 4];
+        if constexpr (N == 8) {
+            const uint2 u = *reinterpret_cast<const uint2*>(p);
+            w[0] = u.x;
+            w[1] = u.y;
+        } else if constexpr (N == 4) {
+            w[0] = *reinterpret_cast<const uint32_t*>(p);
+        } else {
+            w[0] = *reinterpret_cast<const uint16_t*>(p);
+        }
+#pragma unroll
+        for (int i = 0; i < N / 2; ++i) {
+            const float2 f = kv_fp8_unpack2(w[i / 2] >> (16 * (i & 1)));
+            out[2 * i] = f.x;
+            out[2 * i + 1] = f.y;
+        }
+    } else if constexpr (sizeof(KVT) == 2) {
         if constexpr (N == 8) {
             const uint4 u = *reinterpret_cast<const uint4*>(p);
             const uint32_t w[4] = {u.x, u.y, u.z, u.w};
@@ -239,6 +277,9 @@ __device__ __forceinline__ void att_page(const KVT* K, const KVT* V, float* sc, 
     constexpr int LPT = HD / 8;          // lanes per key in QK
     constexpr int TPW = 32 / LPT;        // keys per warp iteration
     constexpr int DPT = HD / 32;         // output dims per lane in PV
+    constexpr bool FP8 = sizeof(KVT) == 1;
+    const float* kscale = reinterpret_cast<const float*>(K + KV_PAGE * HD);     // fp8 only: the tokens' scales
+    const float* vscale = reinterpret_cast<const float*>(V + KV_PAGE * HD);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int sub = lane % LPT;
     // ---- scores for this warp's KPW keys
@@ -253,6 +294,7 @@ __device__ __forceinline__ void att_page(const KVT* K, const KVT* V, float* sc, 
         for (int i = 0; i < 8; ++i) dsum = fmaf(q[i], kv[i], dsum);
 #pragma unroll
         for (int o = LPT / 2; o > 0; o >>= 1) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
+        if constexpr (FP8) dsum *= kscale[t];
         if (sub == 0) sc[t] = (p * KV_PAGE + t <= pos) ? dsum * scale : -INFINITY;
     }
     named_bar_sync(1, ATT_THREADS);
@@ -262,8 +304,13 @@ __device__ __forceinline__ void att_page(const KVT* K, const KVT* V, float* sc, 
     const float corr = expf(m_run - m_new);
     const float e0 = expf(s0 - m_new), e1 = expf(s1 - m_new);
     float* mypw = pw + warp * KV_PAGE;
-    mypw[lane] = e0;
-    mypw[lane + 32] = e1;
+    if constexpr (FP8) {
+        mypw[lane] = e0 * vscale[lane];
+        mypw[lane + 32] = e1 * vscale[lane + 32];
+    } else {
+        mypw[lane] = e0;
+        mypw[lane + 32] = e1;
+    }
     l_run = l_run * corr + warp_sum(e0 + e1);
     m_run = m_new;
     __syncwarp();
@@ -367,8 +414,8 @@ attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, 
                  const int* __restrict__ grp_shared) {
     using L = AttSmem<KVT, HD>;
     constexpr int LPT = HD / 8;          // lanes per key in QK
-    constexpr int TPW = 32 / LPT;        // keys per warp iteration
     constexpr int DPT = HD / 32;         // output dims per lane in PV
+    constexpr int SLAB = L::PAGE_BYTES / sizeof(KVT);        // KVT elements of one (page, head) slab: one TMA bulk copy
     extern __shared__ __align__(128) uint8_t att_smem[];
     KVT* sK = reinterpret_cast<KVT*>(att_smem);
     KVT* sV = reinterpret_cast<KVT*>(att_smem + L::OFF_V);
@@ -416,10 +463,10 @@ attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, 
                     for (int p = p0; p < p1; ++p, ++it) {
                         const int s = it % ATT_STAGES;
                         if (it >= ATT_STAGES) mbar_wait(&empty[s], ((it / ATT_STAGES) - 1) & 1);
-                        const size_t off = (static_cast<size_t>(pt[p]) * H + h) * KV_PAGE * HD;
+                        const size_t off = (static_cast<size_t>(pt[p]) * H + h) * SLAB;
                         mbar_arrive_expect_tx(&full[s], 2 * L::PAGE_BYTES);
-                        tma_bulk_g2s_hint(sK + s * KV_PAGE * HD, kpool + off, L::PAGE_BYTES, &full[s], pol);
-                        tma_bulk_g2s_hint(sV + s * KV_PAGE * HD, vpool + off, L::PAGE_BYTES, &full[s], pol);
+                        tma_bulk_g2s_hint(sK + s * SLAB, kpool + off, L::PAGE_BYTES, &full[s], pol);
+                        tma_bulk_g2s_hint(sV + s * SLAB, vpool + off, L::PAGE_BYTES, &full[s], pol);
                     }
                 }
             }
@@ -453,48 +500,7 @@ attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, 
             for (int p = p0; p < p1; ++p, ++it) {
                 const int s = it % ATT_STAGES;
                 mbar_wait(&full[s], (it / ATT_STAGES) & 1);
-                const KVT* K = sK + s * KV_PAGE * HD;
-                const KVT* V = sV + s * KV_PAGE * HD;
-                float* sc = sc_all + (it & 1) * KV_PAGE;
-                // ---- scores for this warp's KPW keys
-                constexpr int KPW = KV_PAGE / ATT_CWARPS;
-    #pragma unroll
-                for (int itq = 0; itq < KPW / TPW; ++itq) {
-                    const int t = warp * KPW + itq * TPW + lane / LPT;
-                    float kv[8];
-                    load_kv_vec<KVT, 8>(K + t * HD + sub * 8, kv);
-                    float dsum = 0.f;
-    #pragma unroll
-                    for (int i = 0; i < 8; ++i) dsum = fmaf(q[i], kv[i], dsum);
-    #pragma unroll
-                    for (int o = LPT / 2; o > 0; o >>= 1) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
-                    if (sub == 0) sc[t] = (p * KV_PAGE + t <= pos) ? dsum * scale : -INFINITY;
-                }
-                named_bar_sync(1, ATT_THREADS);
-                // ---- online softmax bookkeeping (every warp redundantly over all 64 scores: identical m, l)
-                const float s0 = sc[lane], s1 = sc[lane + 32];
-                const float m_new = fmaxf(m_run, warp_max(fmaxf(s0, s1)));
-                const float corr = expf(m_run - m_new);
-                const float e0 = expf(s0 - m_new), e1 = expf(s1 - m_new);
-                float* mypw = pw + warp * KV_PAGE;
-                mypw[lane] = e0;
-                mypw[lane + 32] = e1;
-                l_run = l_run * corr + warp_sum(e0 + e1);
-                m_run = m_new;
-                __syncwarp();
-                // ---- PV for this warp's KPW keys
-    #pragma unroll
-                for (int i = 0; i < DPT; ++i) acc[i] *= corr;
-    #pragma unroll
-                for (int tt = 0; tt < KPW; ++tt) {
-                    const int t = warp * KPW + tt;
-                    const float pt_ = mypw[t];
-                    float vv[DPT];
-                    load_kv_vec<KVT, DPT>(V + t * HD + lane * DPT, vv);
-    #pragma unroll
-                    for (int i = 0; i < DPT; ++i) acc[i] = fmaf(pt_, vv[i], acc[i]);
-                }
-                __syncwarp();
+                att_page<KVT, HD>(sK + s * SLAB, sV + s * SLAB, sc_all + (it & 1) * KV_PAGE, pw, q, p, pos, scale, m_run, l_run, acc);
                 if (lane == 0) mbar_arrive(&empty[s]);            // this warp is done with stage s
             }
             // ---- combine the 4 warps' partial outputs of this item
@@ -593,10 +599,10 @@ attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, 
                             if (!(live >> j & 1) || (p < S && r0 + j != lead)) continue;
                             const int s = it % ATT_STAGES;
                             if (it >= ATT_STAGES) mbar_wait(&empty[s], ((it / ATT_STAGES) - 1) & 1);
-                            const size_t off = (static_cast<size_t>(pages_of(r0 + j)[p]) * H + h) * KV_PAGE * HD;
+                            const size_t off = (static_cast<size_t>(pages_of(r0 + j)[p]) * H + h) * SLAB;
                             mbar_arrive_expect_tx(&full[s], 2 * L::PAGE_BYTES);
-                            tma_bulk_g2s_hint(sK + s * KV_PAGE * HD, kpool + off, L::PAGE_BYTES, &full[s], pol);
-                            tma_bulk_g2s_hint(sV + s * KV_PAGE * HD, vpool + off, L::PAGE_BYTES, &full[s], pol);
+                            tma_bulk_g2s_hint(sK + s * SLAB, kpool + off, L::PAGE_BYTES, &full[s], pol);
+                            tma_bulk_g2s_hint(sV + s * SLAB, vpool + off, L::PAGE_BYTES, &full[s], pol);
                             ++it;
                         }
                     }
@@ -641,8 +647,8 @@ attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, 
                     const bool first = !shared || (live & ((1u << j) - 1)) == 0;
                     const bool last = !shared || (live >> (j + 1)) == 0;
                     if (first) mbar_wait(&full[s], (it / ATT_STAGES) & 1);
-                    att_page<KVT, HD>(sK + s * KV_PAGE * HD, sV + s * KV_PAGE * HD, sc_all + (k & 1) * KV_PAGE, pw, q[j], p,
-                                      pos, scale, m_run[j], l_run[j], acc[j]);
+                    att_page<KVT, HD>(sK + s * SLAB, sV + s * SLAB, sc_all + (k & 1) * KV_PAGE, pw, q[j], p, pos, scale,
+                                      m_run[j], l_run[j], acc[j]);
                     ++k;
                     if (last) {
                         if (lane == 0) mbar_arrive(&empty[s]);

@@ -2,6 +2,9 @@
 #pragma once
 #include "vcb_common.cuh"
 
+#include <cuda_fp16.h>
+#include <cuda_fp8.h>
+
 #include <algorithm>
 #include <atomic>
 #include <cstring>
@@ -136,6 +139,35 @@ cudaError_t launch_k_pdl(int pdl, void (*kern)(KArgs...), dim3 grid, dim3 block,
 }
 
 // ---------------------------------------------------------------------------------------------------
+// KV cache pages (DESIGN.md section 3).  A (page, head) slab of K or V is one contiguous block: [64 tokens][hd] elements
+// (bf16 or fp32), or for the fp8 policy [64][hd] e4m3 bytes followed by the 64 tokens' fp32 scales.  Pool allocation, the
+// attention kernel, the best-of-N fork and kv_bytes_per_token all size a slab here.
+// ---------------------------------------------------------------------------------------------------
+enum { KV_BF16 = 0, KV_FP32 = 1, KV_FP8 = 2 };      // = VCB_KV_* of include/vcb200.h
+__host__ __device__ constexpr int kv_slab_bytes(int kv_dtype, int hd) {
+    return kv_dtype == KV_FP8 ? 64 * (hd + 4) : 64 * hd * (kv_dtype == KV_FP32 ? 4 : 2);
+}
+
+// FP8 policy: the hd values x of one (token, head) are stored as e4m3(x / 2^e), RNE and satfinite, with the smallest
+// e >= -126 such that max|x| <= 448 * 2^e, and 2^e as an fp32.  Scaling by a power of two is exact, so torch reproduces
+// the bytes with (x / 2^e).to(float8_e4m3fn).  kv_fp8_scale takes max|x| and returns 2^e (and 2^-e in inv).
+__device__ __forceinline__ float kv_fp8_scale(float amax, float& inv) {
+    const uint32_t b = __float_as_uint(amax) & 0x7fffffffu;
+    // amax = 1.f * 2^E <= 1.75 * 2^(8 + e)  <=>  e >= E - 8 (+1 when the mantissa exceeds 1.75); zero / subnormal: -126
+    const int e = (b >> 23) == 0 ? -126 : max(static_cast<int>(b >> 23) - 135 + ((b & 0x7fffffu) > 0x600000u), -126);
+    inv = __uint_as_float(static_cast<uint32_t>(127 - e) << 23);
+    return __uint_as_float(static_cast<uint32_t>(127 + e) << 23);
+}
+__device__ __forceinline__ uint16_t kv_fp8_pack2(float x0, float x1, float inv) {
+    return __nv_cvt_float2_to_fp8x2(make_float2(x0 * inv, x1 * inv), __NV_SATFINITE, __NV_E4M3);
+}
+// e4m3 pair (low byte first) -> fp32, exact (through f16)
+__device__ __forceinline__ float2 kv_fp8_unpack2(uint32_t v) {
+    const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(v), __NV_E4M3);
+    return __half22float2(*reinterpret_cast<const __half2*>(&h));
+}
+
+// ---------------------------------------------------------------------------------------------------
 // GEMM (gemm_wgmma.cu)
 // ---------------------------------------------------------------------------------------------------
 enum { EPI_QKV = 0, EPI_RESID = 1, EPI_ACT = 2, EPI_LOGITS = 3 };
@@ -153,6 +185,7 @@ struct GemmEpilogue {
     const int* row_pos = nullptr;
     const int* row_page = nullptr;      // optional: page index of (row_slot, row_pos), saves the dependent page-table lookup
     int kv_fp32 = 0, max_pages = 0, page_size = 64, d = 0, H = 0, hd = 0;
+    int kv_fp8 = 0;                     // e4m3 slabs (kv_slab_bytes); not taken by the persistent step kernel
     // EPI_RESID: x[row, m] += y ; EPI_ACT: act hi/lo rows ; EPI_LOGITS: out[row, col_off + m]
     float* x = nullptr;
     __nv_bfloat16* act = nullptr;

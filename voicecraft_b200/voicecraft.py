@@ -43,6 +43,9 @@ except Exception:  # pragma: no cover
     _HubBase = ()
     _HUB_KW = {}
 
+# configure_engine(kv_dtype=...) -> vcb_config.kv_dtype (VCB_KV_* of include/vcb200.h)
+KV_DTYPES = {"bf16": 0, "fp32": 1, "fp8": 2}
+
 
 def sine_pe(length: int, dim: int) -> torch.Tensor:
     """Sinusoidal table of SinePositionalEmbedding.extend_pe (embedding.py:67-92), fp32 [length, dim]."""
@@ -177,10 +180,13 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     # engine management
     # ------------------------------------------------------------------------------------------------
     def configure_engine(self, **opts):
-        """max_slots, max_seq_len, max_new_tokens, kv_dtype ('bf16' default | 'fp32').  Rebuilds lazily."""
+        """max_slots, max_seq_len, max_new_tokens, kv_dtype ('bf16' default | 'fp32' | 'fp8': e4m3 with a power-of-two
+        scale per token and head, half the cache bytes of bf16; INTEGRATION.md).  Rebuilds lazily."""
         for k in opts:
             if k not in self._eng_opts:
                 raise KeyError(k)
+        if "kv_dtype" in opts and opts["kv_dtype"] not in KV_DTYPES:
+            raise ValueError(f"kv_dtype {opts['kv_dtype']!r}: one of {sorted(KV_DTYPES)}")
         self._eng_opts.update(opts)
         self._drop_engine()
 
@@ -267,7 +273,7 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
             empty_token=a.empty_token, eog=a.eog, audio_pad_token=a.audio_pad_token, eos=a.eos if a.eos > 0 else -1,
             encodec_sr=int(a.encodec_sr), max_n_spans=a.max_n_spans, max_slots=o["max_slots"],
             max_seq_len=o["max_seq_len"], max_new_tokens=o["max_new_tokens"],
-            kv_dtype=1 if o["kv_dtype"] == "fp32" else 0, device=dev.index or 0)
+            kv_dtype=KV_DTYPES[o["kv_dtype"]], device=dev.index or 0)
         h = C.c_void_p()
         _lib.check(lib.vcb_create(C.byref(cfg), C.byref(h)))
         try:
