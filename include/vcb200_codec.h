@@ -72,10 +72,15 @@ int enc_stream_reset(enc_stream* s, const int32_t* ids_host, int32_t n);
  * stream's first call with fewer than "stream_min_frames" frames, any code (padding included) outside [0, bins). */
 int enc_stream_decode(enc_engine* e, enc_stream* s, const int32_t* ids_host, const int32_t* lens_host, int32_t B,
                       const int64_t* codes_dev, int32_t T, float* wav_dev, void* stream);
-/* Debug / tests: an intermediate tensor of the last enc_decode on the tensor-core path ("z", "x0", "u0", "x1.raw", "x1.elu",
- * "h1.0", "o1.0", ...), reassembled from its bf16 (hi, lo) planes as fp32 [B][C][halo + T] on the host.  dims = {B, C, halo + T,
- * halo}; host_out == NULL only queries dims.  The up-sampling stages share two workspace arenas, so after a full decode only
- * the tensors of the last stage (and "z", "x0", "u0", "hs*") still hold their values: see scripts/codec_tc_debug.py. */
+/* Debug / tests: an intermediate tensor of the last enc_decode on the tensor-core path ("z", "x0", "hs0", "u0", "x1.raw",
+ * "x1.elu", "h1.0", "o1.0", with several residual blocks per stage also "o1.0.raw", ...), reassembled from its bf16 (hi, lo)
+ * planes as fp32 [B][C][halo + T] on the host.  dims = {B, C, halo + T, halo}; host_out == NULL only queries dims.  "c0",
+ * "c1", ... are the LSTM layers' fp32 cell states after the last step, dims {B, C, 1, 0}.  The up-sampling stages share two
+ * workspace arenas, so after a full decode only the tensors of the last stage (and "z", "x0", "u0", "hs*", "c*") still hold
+ * their values -- unless the engine was finalized under VCB_CODEC_KEEP=1, which gives every tensor rows of its own: same
+ * kernels, launches and arithmetic, a larger workspace (tests/test_codec_numerics.py, scripts/codec_tc_debug.py).
+ * "enc.latent": under VCB_CODEC_KEEP=1, the latent the last enc_encode quantised, fp32 dims {B, dimension, T, 0}; this
+ * name does not need the tensor-core decoder.  Any other name fails where that decoder is not active. */
 int enc_debug_tensor(enc_engine* e, const char* name, float* host_out, int64_t cap, int32_t* dims);
 
 /* Resampling: torchaudio.transforms.Resample(orig_sr, new_sr) with its defaults (sinc_interp_hann, lowpass_filter_width 6,

@@ -190,73 +190,114 @@ def convtr1d(cfg, x, w, b, stride):
     return y[..., left: y.shape[-1] - right]
 
 
-def lstm(x, sd, name, layers):
-    """StreamableLSTM with skip: y = LSTM(x) + x over [T,B,C]; gate order i,f,g,o (torch.nn.LSTM)."""
+def lstm_cell(pre_t, h, c, w_hh, b):
+    """One LSTM step: pre_t = W_ih x_t [B,4C], (h, c) of the previous step -> (h, c); gate order i,f,g,o (torch.nn.LSTM)."""
+    gates = pre_t + F.linear(h, w_hh) + b
+    i, f, g_, o = gates.chunk(4, dim=-1)
+    c = torch.sigmoid(f) * c + torch.sigmoid(i) * torch.tanh(g_)
+    h = torch.sigmoid(o) * torch.tanh(c)
+    return h, c
+
+
+def lstm(x, sd, name, layers, states=None):
+    """StreamableLSTM with skip: y = LSTM(x) + x over [T,B,C], in the dtype of x.  `states` (a dict) receives every layer's
+    h and c sequences, [T,B,C], as hs{l} and c{l}."""
     T, B, C = x.shape
     inp = x
     for l in range(layers):
         w_ih, w_hh = sd[f"{name}.weight_ih_l{l}"], sd[f"{name}.weight_hh_l{l}"]
         b = sd[f"{name}.bias_ih_l{l}"] + sd[f"{name}.bias_hh_l{l}"]
-        h = torch.zeros(B, C)
-        c = torch.zeros(B, C)
-        outs = []
+        h = torch.zeros(B, C, dtype=x.dtype)
+        c = torch.zeros(B, C, dtype=x.dtype)
+        outs, cells = [], []
         pre = F.linear(inp, w_ih)                                   # [T,B,4C]
         for t in range(T):
-            gates = pre[t] + F.linear(h, w_hh) + b
-            i, f, g_, o = gates.chunk(4, dim=-1)
-            c = torch.sigmoid(f) * c + torch.sigmoid(i) * torch.tanh(g_)
-            h = torch.sigmoid(o) * torch.tanh(c)
+            h, c = lstm_cell(pre[t], h, c, w_hh, b)
             outs.append(h)
+            cells.append(c)
         inp = torch.stack(outs, dim=0)
+        if states is not None:
+            states[f"hs{l}"] = inp
+            states[f"c{l}"] = torch.stack(cells, dim=0)
     return inp + x
 
 
-@torch.no_grad()
-def decode(cfg, sd, codes):
-    """codes [B,K,T] int64 -> waveform [B,channels,T*hop] fp32."""
+def apply_layer(cfg, sd, L, inputs):
+    """One entry of layer_plan / encoder_plan.  inputs["x"] is the layer's input [B,C,T].  Where the layer applies ELU first,
+    inputs["x_elu"] replaces ELU(x) if given (then a layer that reads nothing else needs no "x"), and inputs["h_elu"] the
+    ELU'd hidden tensor of a residual block: a caller that holds these tensors as another implementation stored them checks
+    that implementation one layer at a time.  -> {"raw": output}, plus "h" (a block's ELU'd hidden tensor) or the LSTM's
+    hs{l} / c{l} sequences [B,C,T]."""
+    n, x = L["name"], inputs.get("x")
+
+    def elu(key, v):
+        return inputs[key] if key in inputs else F.elu(v)
+    if L["kind"] == "conv":
+        a = elu("x_elu", x) if L["elu_in"] else x
+        return {"raw": conv1d(cfg, a, sd[n + ".weight"], sd[n + ".bias"], L.get("dil", 1), L.get("stride", 1))}
+    if L["kind"] == "lstm":
+        states = {}
+        y = lstm(x.permute(2, 0, 1), sd, n, L["layers"], states)
+        return dict({k: v.permute(1, 2, 0) for k, v in states.items()}, raw=y.permute(1, 2, 0))
+    if L["kind"] == "convtr":
+        return {"raw": convtr1d(cfg, elu("x_elu", x), sd[n + ".weight"], sd[n + ".bias"], L["stride"])}
+    h = conv1d(cfg, elu("x_elu", x), sd[n + ".conv1.weight"], sd[n + ".conv1.bias"], L["dil"])
+    he = elu("h_elu", h)
+    h = conv1d(cfg, he, sd[n + ".conv2.weight"], sd[n + ".conv2.bias"], 1)
+    s = x if L["true_skip"] else conv1d(cfg, x, sd[n + ".shortcut.weight"], sd[n + ".shortcut.bias"], 1)
+    return {"h": he, "raw": s + h}
+
+
+def rvq_decode(sd, codes):
+    """codes [B,K,T] -> latent [B,D,T]: the sum of the codebook rows, in the codebooks' dtype."""
     B, K, T = codes.shape
-    z = torch.zeros(B, T, cfg.dimension)
-    for q in range(K):                                               # RVQ decode: sum of codebook rows
+    emb0 = sd["vq.0.embed"]
+    z = torch.zeros(B, T, emb0.shape[1], dtype=emb0.dtype)
+    for q in range(K):
         z = z + F.embedding(codes[:, q], sd[f"vq.{q}.embed"])
-    x = z.transpose(1, 2)                                            # [B,D,T]
+    return z.transpose(1, 2)
+
+
+@torch.no_grad()
+def decode(cfg, sd, codes, return_intermediates=False):
+    """codes [B,K,T] int64 -> waveform [B,channels,T*hop], in the dtype of the weights (sd.double(): a float64 run).
+    With return_intermediates also a dict of every tensor the CUDA decoder exposes, under its enc_debug_tensor name, each
+    [B,C,T_stage]: z, x0, hs{l}, c{l} (the cell state after every step), u0, x{i}.raw, x{i}.elu, h{i}.{j}, o{i}.{j}.raw,
+    o{i}.{j}, wav."""
+    x = rvq_decode(sd, codes)
+    rec = {"z": x}
     for L in layer_plan(cfg):
         n = L["name"]
-        if L["kind"] == "conv":
-            if L["elu_in"]:
-                x = F.elu(x)
-            x = conv1d(cfg, x, sd[n + ".weight"], sd[n + ".bias"], L["dil"])
+        out = apply_layer(cfg, sd, L, {"x": x})
+        x = out["raw"]
+        if n == "dec.conv_in":
+            rec["x0"] = x
+            if not cfg.lstm:
+                rec["u0"] = F.elu(x)
         elif L["kind"] == "lstm":
-            x = lstm(x.permute(2, 0, 1), sd, n, L["layers"]).permute(1, 2, 0)
+            rec.update({k: v for k, v in out.items() if k != "raw"})
+            rec["u0"] = F.elu(x)
         elif L["kind"] == "convtr":
-            x = convtr1d(cfg, F.elu(x), sd[n + ".weight"], sd[n + ".bias"], L["stride"])
-        else:
-            h = conv1d(cfg, F.elu(x), sd[n + ".conv1.weight"], sd[n + ".conv1.bias"], L["dil"])
-            h = conv1d(cfg, F.elu(h), sd[n + ".conv2.weight"], sd[n + ".conv2.bias"], 1)
-            s = x if L["true_skip"] else conv1d(cfg, x, sd[n + ".shortcut.weight"], sd[n + ".shortcut.bias"], 1)
-            x = s + h
-    return x
-
-
-def _res_block(cfg, x, sd, n, L):
-    h = conv1d(cfg, F.elu(x), sd[n + ".conv1.weight"], sd[n + ".conv1.bias"], L["dil"])
-    h = conv1d(cfg, F.elu(h), sd[n + ".conv2.weight"], sd[n + ".conv2.bias"], 1)
-    s = x if L["true_skip"] else conv1d(cfg, x, sd[n + ".shortcut.weight"], sd[n + ".shortcut.bias"], 1)
-    return s + h
+            stage = n[len("dec.up"):].split(".")[0]
+            stage = str(int(stage) + 1)
+            rec[f"x{stage}.raw"], rec[f"x{stage}.elu"] = x, F.elu(x)
+        elif L["kind"] == "res":
+            sj = stage + "." + n.rsplit("res", 1)[1]
+            rec[f"h{sj}"], rec[f"o{sj}.raw"], rec[f"o{sj}"] = out["h"], x, F.elu(x)
+    rec["wav"] = x
+    return (x, rec) if return_intermediates else x
 
 
 @torch.no_grad()
-def encode_latent(cfg, sd, wav):
-    """wav [B,channels,N] fp32 -> latent [B,dimension,T]."""
+def encode_latent(cfg, sd, wav, return_intermediates=False):
+    """wav [B,channels,N] -> latent [B,dimension,T], in the dtype of wav and the weights.  With return_intermediates also
+    {layer name: output} of every encoder_plan entry, and the latent as "enc.latent"."""
     x = wav
+    rec = {}
     for L in encoder_plan(cfg):
-        n = L["name"]
-        if L["kind"] == "conv":
-            x = conv1d(cfg, F.elu(x) if L["elu_in"] else x, sd[n + ".weight"], sd[n + ".bias"], 1, L["stride"])
-        elif L["kind"] == "lstm":
-            x = lstm(x.permute(2, 0, 1), sd, n, L["layers"]).permute(1, 2, 0)
-        else:
-            x = _res_block(cfg, x, sd, n, L)
-    return x
+        x = rec[L["name"]] = apply_layer(cfg, sd, L, {"x": x})["raw"]
+    rec["enc.latent"] = x
+    return (x, rec) if return_intermediates else x
 
 
 @torch.no_grad()

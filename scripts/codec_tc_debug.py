@@ -7,7 +7,6 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
-import torch.nn.functional as F
 
 from oracle import encodec_oracle as eo
 from voicecraft_b200 import _lib
@@ -24,44 +23,10 @@ cfg = eo.default_config(**over)
 sd = eo.make_state_dict(cfg, seed=3)
 codes = torch.randint(0, cfg.bins, (B, cfg.n_q, T), generator=torch.Generator().manual_seed(1))
 
-# ---- oracle with intermediates (same statements as eo.decode)
-ref = {}
-with torch.no_grad():
-    z = torch.zeros(B, T, cfg.dimension)
-    for q in range(cfg.n_q):
-        z = z + F.embedding(codes[:, q], sd[f"vq.{q}.embed"])
-    x = z.transpose(1, 2)
-    ref["z"] = x
-    stage = 0
-    for L in eo.layer_plan(cfg):
-        n = L["name"]
-        if L["kind"] == "conv":
-            if L["elu_in"]:
-                x = F.elu(x)
-            x = eo.conv1d(cfg, x, sd[n + ".weight"], sd[n + ".bias"], L["dil"])
-            if n == "dec.conv_in":
-                ref["x0"] = x
-                if not cfg.lstm:
-                    ref["u0"] = F.elu(x)
-        elif L["kind"] == "lstm":
-            x = eo.lstm(x.permute(2, 0, 1), sd, n, L["layers"]).permute(1, 2, 0)
-            ref["u0"] = F.elu(x)
-        elif L["kind"] == "convtr":
-            x = eo.convtr1d(cfg, F.elu(x), sd[n + ".weight"], sd[n + ".bias"], L["stride"])
-            stage += 1
-            j = 0
-            ref[f"x{stage}.raw"] = x
-            ref[f"x{stage}.elu"] = F.elu(x)
-        else:
-            h = eo.conv1d(cfg, F.elu(x), sd[n + ".conv1.weight"], sd[n + ".conv1.bias"], L["dil"])
-            ref[f"h{stage}.{j}"] = F.elu(h)
-            h = eo.conv1d(cfg, F.elu(h), sd[n + ".conv2.weight"], sd[n + ".conv2.bias"], 1)
-            s = eo.conv1d(cfg, x, sd[n + ".shortcut.weight"], sd[n + ".shortcut.bias"], 1)
-            x = s + h
-            ref[f"o{stage}.{j}"] = F.elu(x)
-            j += 1
-    wav_ref = x
+wav_ref, ref = eo.decode(cfg, sd, codes, return_intermediates=True)
+del ref["wav"]
 
+os.environ["VCB_CODEC_KEEP"] = "1"        # every stage tensor keeps rows of its own: what is printed is what the stage stored
 tok = AudioTokenizer(device="cuda:0", config=cfg, state_dict=sd)
 wav = tok.decode_codes(codes.cuda()).cpu()
 lib = _lib.load()
@@ -85,6 +50,8 @@ for name, r in ref.items():
         print(f"{name:10s} (not recorded)")
         continue
     r = r.numpy()
+    if name[0] == "c" and name[1:].isdigit():
+        r = r[:, :, -1:]                  # the decoder keeps the cell state after the last step only
     g = got[:, : r.shape[1], halo:]
     err = np.abs(g - r)
     pad = np.abs(got[:, r.shape[1]:, halo:]).max() if got.shape[1] > r.shape[1] else 0.0

@@ -564,9 +564,12 @@ struct TcCodec {
     DevBuf<uint8_t> ws;
     size_t ws_limit = 0;
     bool profile = false;
+    bool keep = false;                 // VCB_CODEC_KEEP=1: every plan tensor has its own rows, so all survive a decode
     std::vector<std::pair<std::string, float>> prof;
     struct Dbg { Plane p; const __nv_bfloat16* ptr; int B; };
     std::map<std::string, Dbg> dbg;      // tensors of the last decoded chunk (debug read-back)
+    const float* dbg_cst = nullptr;      // its final LSTM cell states [layers][dbg_Bcap][ch0] ("c0", "c1", ...)
+    int dbg_B = 0, dbg_Bcap = 0;
 };
 
 namespace {
@@ -801,7 +804,7 @@ void build_plan(TcCodec* tc) {
                       std::string dbg_elu) {
         PlanTensor t;
         t.C = C; t.halo = halo; t.halo_kind = kind; t.up = up; t.tm = tm;
-        t.forms = forms; t.home = home; t.carried = carried;
+        t.forms = forms; t.home = tc->keep ? HOME_FIXED : home; t.carried = carried;
         t.dbg_raw = std::move(dbg_raw);
         t.dbg_elu = std::move(dbg_elu);
         pl.tensors.push_back(t);
@@ -882,8 +885,8 @@ void build_plan(TcCodec* tc) {
             halo = next;
             kind = pad;
             if (j == nres - 1) feed(last_stage, halo, kind);
-            const int o = tensor(cpad(cout), halo, kind, up, false, (j < nres - 1 ? FORM_RAW : 0) | FORM_ELU, side ^ 1, true, "",
-                                 "o" + sj);
+            const int o = tensor(cpad(cout), halo, kind, up, false, (j < nres - 1 ? FORM_RAW : 0) | FORM_ELU, side ^ 1, true,
+                                 j < nres - 1 ? "o" + sj + ".raw" : "", "o" + sj);
             PlanLayer tail = layer(L_CONV, "res_conv2", &tc->res2[i][j], cpad(cout), hd, FORM_ELU, o, pl.tensors[o].forms, F32_NONE);
             tail.in2 = x;
             add(tail);
@@ -975,6 +978,9 @@ int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
     float* pre = reinterpret_cast<float*>(tc->ws + w.pre);
     float* cst = reinterpret_cast<float*>(tc->ws + w.cst);
     float* copart = reinterpret_cast<float*>(tc->ws + w.copart);
+    tc->dbg_cst = nl > 0 ? cst : nullptr;
+    tc->dbg_B = B;
+    tc->dbg_Bcap = Bcap;
 
     // state that the kernels only ever read: U0's zero halo (the LSTM epilogue writes none), c_0 and h_{-1}
     const Plane& u0 = P[pl.u0];
@@ -1161,6 +1167,7 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, DevBuf<flo
         if (getenv("VCB_CODEC_GRID")) tc->num_sms = std::max(1, atoi(getenv("VCB_CODEC_GRID")));
     }
     tc->profile = getenv("VCB_CODEC_PROFILE") && atoi(getenv("VCB_CODEC_PROFILE")) != 0;
+    tc->keep = getenv("VCB_CODEC_KEEP") && atoi(getenv("VCB_CODEC_KEEP")) != 0;
     // LSTM step tiles: 128 columns move fewer bytes through L2 per step (VCB_CODEC_LSTM_WIDE=1); 64 keep more CTAs on the
     // 16-k-block pipeline of each step
     const int step_bn = getenv("VCB_CODEC_LSTM_WIDE") && atoi(getenv("VCB_CODEC_LSTM_WIDE")) > 0 ? 128 : 64;
@@ -1295,6 +1302,19 @@ void TcCodecDelete::operator()(TcCodec* tc) const { delete tc; }
 const std::vector<std::pair<std::string, float>>& tc_codec_profile(const TcCodec* c) { return c->prof; }
 
 int tc_codec_debug_tensor(TcCodec* tc, const char* name, float* host_out, int64_t cap, int32_t* dims) {
+    if (name[0] == 'c' && name[1] >= '0' && name[1] < '0' + tc->cfg.lstm && name[2] == 0 && tc->dbg_cst != nullptr) {
+        const int B = tc->dbg_B, H = tc->ch0;                        // fp32 [B][H], the state after the last step
+        dims[0] = B; dims[1] = H; dims[2] = 1; dims[3] = 0;
+        if (host_out == nullptr) return 0;
+        if (cap < static_cast<int64_t>(B) * H) {
+            set_error("codec_tc: debug buffer too small");
+            return -1;
+        }
+        VCB_CUDA_OK(cudaDeviceSynchronize());
+        VCB_CUDA_OK(cudaMemcpy(host_out, tc->dbg_cst + static_cast<size_t>(name[1] - '0') * tc->dbg_Bcap * H,
+                               static_cast<size_t>(B) * H * 4, cudaMemcpyDeviceToHost));
+        return 0;
+    }
     auto it = tc->dbg.find(name);
     if (it == tc->dbg.end()) {
         set_error("codec_tc: no tensor '%s' in the last decode", name);

@@ -42,7 +42,8 @@ int tc_codes_check(const int64_t* codes_dev, long long n, int bins, int* bad_dev
 // per-layer device times of the last decode when VCB_CODEC_PROFILE=1 (name, ms), in launch order
 const std::vector<std::pair<std::string, float>>& tc_codec_profile(const TcCodec* c);
 
-// debug: tensor `name` of the last decoded chunk as fp32 [B][C][halo + T] (hi + lo); dims = {B, C, halo + T, halo}
+// debug: tensor `name` of the last decoded chunk as fp32 [B][C][halo + T] (hi + lo); dims = {B, C, halo + T, halo}.  With
+// VCB_CODEC_KEEP=1 at tc_codec_build no two tensors share rows, so every one of them holds what its layer stored.
 int tc_codec_debug_tensor(TcCodec* c, const char* name, float* host_out, int64_t cap, int32_t* dims);
 
 }  // namespace vcb

@@ -283,6 +283,9 @@ struct enc_engine {
     const char* tc_reason = "";
     int64_t tc_decodes = 0;
     int64_t stream_decodes = 0;
+    bool keep = false;                  // VCB_CODEC_KEEP=1: enc_encode keeps the latent it quantises ("enc.latent")
+    DevBuf<float> latent;               // [lat_B][dimension][lat_T]
+    int lat_B = 0, lat_T = 0;
 };
 
 struct enc_stream {
@@ -442,7 +445,7 @@ int res_block(enc_engine* e, const char* prefix, const float* x, float* y, float
 
 // wav [B, channels, N] -> codes [B, n_q, T]: SEANetEncoder (conv k7 -> n x [ResBlock, ELU, strided conv] -> LSTM + skip -> ELU ->
 // conv k7) and residual vector quantisation.  (reference data/tokenizer.py:127-129 -> audiocraft EncodecModel.encode)
-int encode_chunk(enc_engine* e, const float* wav, int64_t* codes, int B, int N, cudaStream_t st) {
+int encode_chunk(enc_engine* e, const float* wav, int64_t* codes, float* latent, int B, int N, cudaStream_t st) {
     const enc_config& c = e->cfg;
     char nm[128];
     float *x = e->buf[0], *y = e->buf[1], *z = e->buf[2], *pre = e->buf[3];
@@ -477,6 +480,8 @@ int encode_chunk(enc_engine* e, const float* wav, int64_t* codes, int B, int N, 
     if (conv_launch(e, conv_args(e, wt, bs, x, y, ch, c.dimension, t_cur, c.last_kernel_size, 1, 1, nullptr), B, st)) return -1;
     // ---- residual vector quantisation: y = latent [B, D, T] is consumed as the running residual
     const int T = t_cur;
+    if (latent != nullptr)
+        VCB_CUDA_OK(cudaMemcpyAsync(latent, y, static_cast<size_t>(B) * c.dimension * T * 4, cudaMemcpyDeviceToDevice, st));
     for (int q = 0; q < c.n_q; ++q) {
         float *emb, *hsn;
         snprintf(nm, sizeof(nm), "vq.%d.embed", q);
@@ -660,6 +665,7 @@ int enc_finalize(enc_engine* e) {
     }
     VCB_CUDA_OK(cudaDeviceSynchronize());
     e->tc.reset();
+    e->keep = getenv("VCB_CODEC_KEEP") && atoi(getenv("VCB_CODEC_KEEP")) != 0;
     if (tc_codec_build(e->cfg, e->w, e->shapes, &e->tc, &e->tc_reason) < 0) return -1;
     e->finalized = true;
     return 0;
@@ -713,16 +719,40 @@ int enc_encode(enc_engine* e, const float* wav_dev, int64_t* codes_dev, int32_t 
     for (int i = e->cfg.n_ratios - 1; i >= 0; --i) T = (T + e->cfg.ratios[i] - 1) / e->cfg.ratios[i];
     const int chunk = std::min(B, 16);
     if (ensure_buffers(e, chunk, (N + e->hop - 1) / e->hop + 1)) return -1;
+    const size_t lat = static_cast<size_t>(e->cfg.dimension) * T;
+    e->lat_B = 0;
+    if (e->keep) {
+        if (e->latent.size() < B * lat && e->latent.alloc(B * lat)) return -1;
+        e->lat_B = B;
+        e->lat_T = T;
+    }
     for (int b0 = 0; b0 < B; b0 += chunk) {
         const int nb = std::min(chunk, B - b0);
         if (encode_chunk(e, wav_dev + static_cast<size_t>(b0) * e->cfg.channels * N,
-                         codes_dev + static_cast<size_t>(b0) * e->cfg.n_q * T, nb, N, st))
+                         codes_dev + static_cast<size_t>(b0) * e->cfg.n_q * T, e->keep ? e->latent + b0 * lat : nullptr, nb, N, st))
             return -1;
     }
     return 0;
 }
 
 int enc_debug_tensor(enc_engine* e, const char* name, float* host_out, int64_t cap, int32_t* dims) {
+    if (e && name && !strcmp(name, "enc.latent")) {
+        if (e->lat_B == 0) {
+            set_error("codec: no enc.latent: it is kept by an enc_encode of an engine finalized under VCB_CODEC_KEEP=1");
+            return -1;
+        }
+        const int64_t n = static_cast<int64_t>(e->lat_B) * e->cfg.dimension * e->lat_T;
+        dims[0] = e->lat_B; dims[1] = e->cfg.dimension; dims[2] = e->lat_T; dims[3] = 0;
+        if (host_out == nullptr) return 0;
+        if (cap < n) {
+            set_error("codec: debug buffer too small");
+            return -1;
+        }
+        VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
+        VCB_CUDA_OK(cudaDeviceSynchronize());
+        VCB_CUDA_OK(cudaMemcpy(host_out, e->latent, n * 4, cudaMemcpyDeviceToHost));
+        return 0;
+    }
     if (!e || !e->tc) {
         set_error("codec: the tensor-core decoder is not active (%s)", e ? e->tc_reason : "null engine");
         return -1;
