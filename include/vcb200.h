@@ -35,6 +35,8 @@ typedef struct vcb_engine vcb_engine;
 enum { VCB_MODE_TTS = 0, VCB_MODE_EDIT = 1 };
 /* KV cache policy (DESIGN.md sections 2.2, 3): bf16, fp32, or e4m3 with a power-of-two fp32 scale per token and head */
 enum { VCB_KV_BF16 = 0, VCB_KV_FP32 = 1, VCB_KV_FP8 = 2 };
+/* GEMM weight policy (DESIGN.md section 2.2): bf16, or int8 with a power-of-two fp32 scale per output feature */
+enum { VCB_W_BF16 = 0, VCB_W_INT8 = 1 };
 
 /* Model hyper-parameters: the argparse Namespace the reference model is built from
  * (reference config.py:50-84, models/voicecraft.py:106-195). */
@@ -48,6 +50,8 @@ typedef struct {
     int32_t max_new_tokens; /* token-log capacity per utterance */
     int32_t kv_dtype;       /* VCB_KV_BF16 (default), VCB_KV_FP32 or VCB_KV_FP8; vcb_create rejects any other value */
     int32_t device;         /* CUDA device ordinal */
+    int32_t weight_dtype;   /* VCB_W_BF16 (default) or VCB_W_INT8 (d_model and audio_vocab_size / 2 multiples of 128);
+                             * vcb_create rejects any other value */
 } vcb_config;
 
 /* Sampling arguments of inference_tts / inference / inference_tts_batch (voicecraft.py:908-920). */
@@ -123,7 +127,7 @@ int vcb_load_weight(vcb_engine* e, const char* key, const float* data, const int
                     int32_t is_device_ptr);
 /* sinusoidal table of SinePositionalEmbedding (embedding.py:67-92), fp32 [rows][d_model] */
 int vcb_load_pe(vcb_engine* e, const float* data, int32_t rows, int32_t is_device_ptr);
-int vcb_finalize_weights(vcb_engine* e);   /* packs bf16 GEMM operands, builds TMA descriptors */
+int vcb_finalize_weights(vcb_engine* e);   /* packs the GEMM operands (bf16 or int8), builds TMA descriptors */
 
 /* ---- decode: replaces dec_forward + the sampling loop (voicecraft.py:406-470, 1018-1120) ----------- */
 /* validates every prompt first (a group needs max_pages + (n_copies-1) * (max_pages - full prompt pages) free KV pages),
@@ -188,6 +192,12 @@ int vcb_debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t 
                       int32_t encodec_sr, const int32_t* state_host, int32_t* tokens_host, int32_t* state_out_host);
 int vcb_debug_gemm(const float* W_dev /*[N][K]*/, const float* X_dev /*[B][K]*/, float* out_dev /*[B][N]*/, int32_t N,
                    int32_t K, int32_t B, int32_t splits /*<=0: auto*/, int32_t simt);
+/* the int8 weight rule of vcb_finalize_weights on fp32 W [N][K]: q_out [N][K] int8 and e_out [N] with W_deq = q * 2^e.
+ * Synchronous. */
+int vcb_debug_weight_quantize(const float* W_dev, int32_t N, int32_t K, int8_t* q_out, int32_t* e_out);
+/* vcb_debug_gemm through the int8-weight decode GEMM: W quantized by that rule (out = X W_deq^T), K % 128 == 0 */
+int vcb_debug_gemm_w8(const float* W_dev /*[N][K]*/, const float* X_dev /*[B][K]*/, float* out_dev /*[B][N]*/, int32_t N,
+                      int32_t K, int32_t B, int32_t splits /*<=0: auto*/);
 /* same check for the rows-as-M prefill GEMM (csrc/gemm_rows.cu): any number of rows, N % 128 == 0, K % 64 == 0 */
 int vcb_debug_gemm_rows(const float* W_dev /*[N][K]*/, const float* X_dev /*[rows][K]*/, float* out_dev /*[rows][N]*/,
                         int32_t N, int32_t K, int32_t rows);
@@ -249,7 +259,8 @@ int vcb_set_option(vcb_engine* e, const char* name, int32_t value);   /* "gemm_s
 /* profile mode: summed device ms and launch counts per kernel class since the last read
  * (0 gemm, 1 attention, 2 layernorm/reduce, 3 bias/act/qkv finish, 4 sampler, 5 misc) */
 int vcb_profile_read(vcb_engine* e, double* ms_by_class, int64_t* count_by_class, int32_t n_classes);
-/* "launches", "kv_bytes", "kv_pages_free", "prefill_rows" (rows through the prefill since create), ...; "live_bytes" / "live_handles" (any e, NULL included): device and pinned bytes, and allocations
+/* "launches", "kv_bytes", "kv_pages_free", "prefill_rows" (rows through the prefill since create), "weight_bytes" (device
+ * bytes of the packed GEMM operands with their int8 scales, and the int8 prefill scratch once a prefill allocated it), ...; "live_bytes" / "live_handles" (any e, NULL included): device and pinned bytes, and allocations
  * plus events, the library holds now across every engine, codec engine and stream of the process */
 int64_t vcb_counter(vcb_engine* e, const char* name);
 

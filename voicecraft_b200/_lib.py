@@ -19,7 +19,7 @@ class vcb_config(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "d_model", "nhead", "num_layers", "n_codebooks", "audio_vocab_size", "n_special", "text_vocab_rows",
         "empty_token", "eog", "audio_pad_token", "eos", "encodec_sr", "max_n_spans", "max_slots", "max_seq_len",
-        "max_new_tokens", "kv_dtype", "device")]
+        "max_new_tokens", "kv_dtype", "device", "weight_dtype")]
 
 
 class vcb_sampling(C.Structure):
@@ -71,6 +71,8 @@ PROTOTYPES = {
     "vcb_debug_sampler": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int32, C.POINTER(vcb_sampling)] +
                           [C.c_int32] * 7 + [C.POINTER(C.c_int32)] * 3),
     "vcb_debug_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "vcb_debug_weight_quantize": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "vcb_debug_gemm_w8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "vcb_debug_gemm_rows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32]),
     "vcb_debug_attention": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 4 + [C.c_int32] * 7 + [C.c_void_p]),
     "vcb_debug_attention_groups": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 2 + [C.c_int32] * 7 +

@@ -41,10 +41,11 @@ static constexpr int GEMM_MAX_SPLITS = 16;   // cluster size = K splits
 constexpr int gemm_epi_warps(int bn) { return bn >= 128 ? 8 : 4; }
 constexpr int gemm_threads(int bn) { return 128 + 32 * gemm_epi_warps(bn); }
 
-template <int BN, int STAGES>
+// W8: the stage holds one 128-k int8 weight tile (the same 16 KB) and the two 64-k activation boxes it multiplies
+template <int BN, int STAGES, bool W8 = false>
 struct GemmSmem {
     static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
-    static constexpr int B_BYTES = BN * GEMM_BK * 2;
+    static constexpr int B_BYTES = BN * GEMM_BK * 2 * (W8 ? 2 : 1);
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
     static constexpr int RED_OFFSET = STAGES * STAGE_BYTES;
     static constexpr int RED_BYTES = (BN / 2) * GEMM_BM * 4;          // [S][R][128] fp32 with S*R = Bpad
@@ -63,6 +64,59 @@ constexpr int gemm_stages(int bpad) {
 }
 static_assert(GemmSmem<64, gemm_stages(32)>::TOTAL <= 227 * 1024 && GemmSmem<256, gemm_stages(128)>::TOTAL <= 227 * 1024,
               "gemm_stages and GemmSmem disagree on the shared memory footprint");
+// Int8 weights (W8): a stage carries twice the activation bytes.  The most stages (<= 4) that still fit and keep as many
+// CTAs per SM as the bf16 kernel for `bpad`, whose occupancy chose the split count: bpad 16: 4, 32: 3, 64: 4, 128: 2.
+constexpr int gemm_smem_bytes(int bpad, int s, bool w8) {
+    return s * (GEMM_BM * GEMM_BK * 2 + (w8 ? 2 : 1) * 2 * bpad * GEMM_BK * 2) + bpad * GEMM_BM * 4 + (2 * s + 1) * 8;
+}
+constexpr int gemm_ctas_per_sm(int bytes) { return (228 * 1024) / (bytes + 1024); }
+constexpr int gemm_stages_w8(int bpad) {
+    int s = 4;
+    while (s > 2 && (gemm_smem_bytes(bpad, s, true) > 227 * 1024 ||
+                     gemm_ctas_per_sm(gemm_smem_bytes(bpad, s, true)) < gemm_ctas_per_sm(gemm_smem_bytes(bpad, gemm_stages(bpad), false))))
+        --s;
+    return s;
+}
+static_assert(GemmSmem<256, gemm_stages_w8(128), true>::TOTAL == gemm_smem_bytes(128, gemm_stages_w8(128), true) &&
+              GemmSmem<256, gemm_stages_w8(128), true>::TOTAL <= 227 * 1024,
+              "gemm_stages_w8 and GemmSmem disagree on the shared memory footprint");
+
+// Int8 weight tiles (W8).  Tile (mt, cb) = rows mt*128.., k cb*128.. is one contiguous 16 KB block [128 rows][128 bytes] at
+// block index mt*(K/128) + cb, one TMA box with SWIZZLE_128B.  Inside a row the k order is permuted so that thread t of a
+// quad finds every A fragment value it needs for the tile's eight k16 steps in the 32 bytes [32t, 32t+32): byte 32t + 4s + j
+// holds k = 16s + 2t + (j & 1) + 8 (j >> 1) -- the wgmma register fragment of A (rows g, g+8; k 2t, 2t+1, 2t+8, 2t+9) -- so
+// each row costs a thread two 16-byte shared loads per tile, and the swizzle keeps a quarter warp's loads on distinct banks.
+__host__ __device__ inline size_t w8_index(int m, int k, int Kdim) {
+    const int kc = k % 128, s = kc / 16, w = kc % 16;
+    const int pos = 32 * ((w & 7) >> 1) + 4 * s + (w & 1) + 2 * (w >> 3);
+    return ((static_cast<size_t>(m / GEMM_BM) * (Kdim / 128) + k / 128) * GEMM_BM + (m % GEMM_BM)) * 128 + pos;
+}
+
+// 4 int8 (k 2t, 2t+1, 2t+8, 2t+9) -> two bf16x2 A-fragment registers, exactly: byte u = q + 128 becomes the fp32 2^23 + u,
+// minus 2^23 + 128 gives q, whose upper 16 bits are q as a bf16 (|q| <= 128 has at most 8 significant bits)
+__device__ __forceinline__ void w8_to_bf16x2(uint32_t w, uint32_t& lo, uint32_t& hi) {
+    const uint32_t u = w ^ 0x80808080u;
+    float f[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) f[j] = __uint_as_float(__byte_perm(u, 0x4B000000u, 0x7540 + j)) - 8388736.f;
+    lo = __byte_perm(__float_as_uint(f[0]), __float_as_uint(f[1]), 0x7632);
+    hi = __byte_perm(__float_as_uint(f[2]), __float_as_uint(f[3]), 0x7632);
+}
+
+// A fragments of the eight k16 steps of one 64-row block of an int8 tile in shared memory (SWIZZLE_128B: 16-byte chunk c of
+// row r sits at chunk c ^ (r & 7)), for the thread at rows r, r + 8 and quad position t
+__device__ __forceinline__ void w8_frags(const uint8_t* tile, int r, int t, uint32_t (&f)[8][4]) {
+#pragma unroll
+    for (int p = 0; p < 2; ++p) {
+        const int row = r + 8 * p;
+        const uint8_t* base = tile + row * 128;
+        const uint4 a = *reinterpret_cast<const uint4*>(base + (((2 * t) ^ (row & 7)) << 4));
+        const uint4 b = *reinterpret_cast<const uint4*>(base + (((2 * t + 1) ^ (row & 7)) << 4));
+        const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+        for (int s = 0; s < 8; ++s) w8_to_bf16x2(w[s], f[s][p], f[s][2 + p]);
+    }
+}
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
@@ -167,12 +221,16 @@ __device__ __forceinline__ void apply_epilogue4(const GemmEpilogue& ep, int row0
 }
 
 // KV8: the QKV launch of an fp8-KV engine (its own instantiation, so the other epilogues keep their register budget)
-template <int BN, int STAGES, bool KV8 = false>
+// W8: int8 weight tiles (w8_index) with a power-of-two scale per feature (wscale, or grp.wscale per group).  The K slices are
+// the bf16 kernel's (total_kb / kb_per_split count 64-k blocks); a stage holds a 128-k tile, and a slice that begins or ends
+// halfway through one skips that half's k16 steps.  The MMA warps convert each tile to bf16 A fragments in registers and issue
+// the bf16 kernel's wgmmas in its k16 order; the fixed-order sum of the partials is multiplied by 2^e before the epilogue.
+template <int BN, int STAGES, bool KV8 = false, bool W8 = false>
 __global__ void __launch_bounds__(gemm_threads(BN))
 gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const GemmEpilogue ep, int Nout, int total_kb, int kb_per_split, int b_col_off, int nvalid,
-                  const void* pf_ptr, unsigned long long pf_bytes, const GemmGroup grp) {
-    using L = GemmSmem<BN, STAGES>;
+                  const void* pf_ptr, unsigned long long pf_bytes, const GemmGroup grp, const float* wscale) {
+    using L = GemmSmem<BN, STAGES, W8>;
     constexpr int BPAD = BN / 2;
     constexpr int HALVES = gemm_epi_warps(BN) / 4;          // MMA + epilogue warpgroups
     constexpr int MH = 2 / HALVES;                          // 64-feature halves multiplied by each warpgroup
@@ -196,7 +254,11 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const int colx = grp_i * grp.col_stride;
     const int kb0 = z * kb_per_split;
     const int nkb = max(0, min(kb_per_split, total_kb - kb0));
-    const int pre = min(nkb, STAGES);
+    // pipeline items: 64-k blocks, or (W8) the 128-k tiles t0 .. t0 + nst - 1 that hold 64-k blocks kb0 .. kb0 + nkb - 1
+    const int t0 = W8 ? kb0 / 2 : kb0;
+    const int nst = W8 ? (nkb > 0 ? (kb0 + nkb - 1) / 2 - t0 + 1 : 0) : nkb;
+    const int a_blocks = W8 ? total_kb / 2 : total_kb;      // weight tiles per 128-feature row of tiles
+    const int pre = min(nst, STAGES);
 
     pdl_launch_dependents();        // dependents may be scheduled now; their griddepcontrol.wait still orders the data
     if (threadIdx.x == 0) { tl_mark(0x100 + ep.mode); tl_mark_all(0x100 + ep.mode); }
@@ -216,7 +278,7 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const uint64_t pol = l2_policy_evict_first();      // weight tiles are read once per step
         for (int i = 0; i < pre; ++i) {
             mbar_arrive_expect_tx(&full_bar[i], L::STAGE_BYTES);
-            tma_load_2d_hint(smem + i * L::STAGE_BYTES, pA, &full_bar[i], 0, (mt * total_kb + kb0 + i) * GEMM_BM, pol);
+            tma_load_2d_hint(smem + i * L::STAGE_BYTES, pA, &full_bar[i], 0, (mt * a_blocks + t0 + i) * GEMM_BM, pol);
         }
         // keep HBM busy across the kernel boundary: pull the NEXT GEMM's weights into L2 while this one runs
         // (bit 63 of pf_bytes: issue it after this CTA's last weight load instead -- HBM idles during the epilogue)
@@ -238,6 +300,11 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             if (ep.emit) w_gnext = ep.next_gamma[m];
         }
     }
+    float w_scale = 1.f;                                    // W8: 2^e of the feature
+    if constexpr (W8) {
+        const int m = m0 + (warp & 3) * 32 + lane;
+        if (warp >= 4 && m < Nout) w_scale = (grp.wscale ? grp.wscale[grp_i] : wscale)[m];
+    }
 
     if (warp == 0) {
         // ===== TMA producer ==========================================================================
@@ -245,17 +312,30 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             pdl_wait();
             tl_mark(0x110 + ep.mode);
             tl_mark_all(0x110 + ep.mode);
-            for (int i = 0; i < pre; ++i)
-                tma_load_2d(smem + i * L::STAGE_BYTES + L::A_BYTES, &tmB, &full_bar[i],
-                            b_col_off + (kb0 + i) * GEMM_BK, 0);
+            for (int i = 0; i < pre; ++i) {
+                if constexpr (W8) {
+                    uint8_t* b = smem + i * L::STAGE_BYTES + L::A_BYTES;
+                    tma_load_2d(b, &tmB, &full_bar[i], b_col_off + (t0 + i) * 2 * GEMM_BK, 0);
+                    tma_load_2d(b + L::B_BYTES / 2, &tmB, &full_bar[i], b_col_off + ((t0 + i) * 2 + 1) * GEMM_BK, 0);
+                } else {
+                    tma_load_2d(smem + i * L::STAGE_BYTES + L::A_BYTES, &tmB, &full_bar[i],
+                                b_col_off + (kb0 + i) * GEMM_BK, 0);
+                }
+            }
             int stage = 0, phase = 0;                       // state after the first `pre` fills
             const uint64_t pol = l2_policy_evict_first();
-            for (int i = pre; i < nkb; ++i) {
+            for (int i = pre; i < nst; ++i) {
                 mbar_wait(&empty_bar[stage], phase);        // the MMA released this slot
                 mbar_arrive_expect_tx(&full_bar[stage], L::STAGE_BYTES);
                 uint8_t* a = smem + stage * L::STAGE_BYTES;
-                tma_load_2d_hint(a, pA, &full_bar[stage], 0, (mt * total_kb + kb0 + i) * GEMM_BM, pol);
-                tma_load_2d(a + L::A_BYTES, &tmB, &full_bar[stage], b_col_off + (kb0 + i) * GEMM_BK, 0);
+                tma_load_2d_hint(a, pA, &full_bar[stage], 0, (mt * a_blocks + t0 + i) * GEMM_BM, pol);
+                if constexpr (W8) {
+                    tma_load_2d(a + L::A_BYTES, &tmB, &full_bar[stage], b_col_off + (t0 + i) * 2 * GEMM_BK, 0);
+                    tma_load_2d(a + L::A_BYTES + L::B_BYTES / 2, &tmB, &full_bar[stage],
+                                b_col_off + ((t0 + i) * 2 + 1) * GEMM_BK, 0);
+                } else {
+                    tma_load_2d(a + L::A_BYTES, &tmB, &full_bar[stage], b_col_off + (kb0 + i) * GEMM_BK, 0);
+                }
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
             if (pf_bytes >> 63) prefetch_l2_slice(pf_ptr, pf_bytes & ~(1ull << 63), blockIdx.x, gridDim.x);
@@ -293,7 +373,33 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         for (int h = 0; h < MH; ++h)
 #pragma unroll
             for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
-        {
+        if constexpr (W8) {
+            // per tile: every thread converts its A fragments, the warpgroup issues the tile's k16 steps that lie in the slice,
+            // and waits for them (the fragment registers are rewritten for the next tile) before releasing the slot
+            int stage = 0, phase = 0;
+            for (int i = 0; i < nst; ++i) {
+                mbar_wait(&full_bar[stage], phase);
+                const uint8_t* tile = smem + stage * L::STAGE_BYTES;
+                const uint32_t b_addr = smem_u32(tile + L::A_BYTES);
+                const int c0 = (t0 + i) * 8;                // first k16 step of the tile
+                const int klo = max(kb0 * 4 - c0, 0), khi = min((kb0 + nkb) * 4 - c0, 8);
+                uint32_t fa[MH][8][4];
+#pragma unroll
+                for (int h = 0; h < MH; ++h) w8_frags(tile, (half * MH + h) * 64 + q * 16 + (lane >> 2), lane & 3, fa[h]);
+                wg_fence();
+#pragma unroll
+                for (int s = 0; s < 8; ++s) {
+                    if (s < klo || s >= khi) continue;      // (uniform over the warpgroup)
+#pragma unroll
+                    for (int h = 0; h < MH; ++h) wg_mma_k16_ra<BN>(acc[h], fa[h][s], b_addr + (s >> 2) * (L::B_BYTES / 2), s & 3);
+                }
+                wg_commit();
+                wg_wait0();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[stage]);
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+        } else {
             int stage = 0, phase = 0, prev = -1;
             for (int i = 0; i < nkb; ++i) {
                 mbar_wait(&full_bar[stage], phase);
@@ -392,6 +498,7 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 if (u < nrows) {
                     for (int zz = 0; zz < S; ++zz) a += red[(zz * GEMM_BM + ml) * R + rr0 + u];
                 }
+                if constexpr (W8) a *= w_scale;             // exact: a power of two
                 if (ep.ln_fold) {
                     float mean, rstd;
                     if constexpr (BPAD <= 32) {             // (uniform: every lane of the warp takes part in the shuffle)
@@ -589,16 +696,30 @@ __global__ void pack_weight_tiles_kernel(const float* __restrict__ in, __nv_bflo
     }
 }
 
-// LayerNorm folding vectors from the (bf16, pre-tiled) weight: cvec[m] = sum_k gamma[k] W[m,k],
+// element (m, k) of a packed weight as fp32: bf16 tiles, or int8 tiles times the row's 2^e (exactly W_deq)
+struct PackedBf16 {
+    const __nv_bfloat16* w;
+    __device__ float operator()(int m, int k, int Kdim) const { return __bfloat162float(w[packed_index(m, k, Kdim)]); }
+};
+struct PackedW8 {
+    const uint8_t* w;
+    const float* scale;
+    __device__ float operator()(int m, int k, int Kdim) const {
+        return static_cast<float>(static_cast<int8_t>(w[w8_index(m, k, Kdim)])) * scale[m];
+    }
+};
+
+// LayerNorm folding vectors from the pre-tiled weight: cvec[m] = sum_k gamma[k] W[m,k],
 // bprime[m] = bias[m] + sum_k beta[k] W[m,k]; one warp per output feature, fp32.
-__global__ void ln_fold_vectors_kernel(const __nv_bfloat16* __restrict__ Wp, const float* __restrict__ gamma,
+template <typename WAt>
+__global__ void ln_fold_vectors_kernel(const WAt Wp, const float* __restrict__ gamma,
                                        const float* __restrict__ beta, const float* __restrict__ bias,
                                        float* __restrict__ cvec, float* __restrict__ bprime, int N, int Kdim) {
     const int m = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (m >= N) return;
     float c = 0.f, b = 0.f;
     for (int k = lane; k < Kdim; k += 32) {
-        const float w = __bfloat162float(Wp[packed_index(m, k, Kdim)]);
+        const float w = Wp(m, k, Kdim);
         c = fmaf(gamma[k], w, c);
         b = fmaf(beta[k], w, b);
     }
@@ -612,7 +733,86 @@ __global__ void ln_fold_vectors_kernel(const __nv_bfloat16* __restrict__ Wp, con
 
 int ln_fold_vectors(const __nv_bfloat16* Wp, const float* gamma, const float* beta, const float* bias, float* cvec,
                     float* bprime, int N, int Kdim) {
-    ln_fold_vectors_kernel<<<(N * 32 + 255) / 256, 256>>>(Wp, gamma, beta, bias, cvec, bprime, N, Kdim);
+    ln_fold_vectors_kernel<<<(N * 32 + 255) / 256, 256>>>(PackedBf16{Wp}, gamma, beta, bias, cvec, bprime, N, Kdim);
+    VCB_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int ln_fold_vectors_w8(const uint8_t* W8, const float* scale, const float* gamma, const float* beta, const float* bias,
+                       float* cvec, float* bprime, int N, int Kdim) {
+    ln_fold_vectors_kernel<<<(N * 32 + 255) / 256, 256>>>(PackedW8{W8, scale}, gamma, beta, bias, cvec, bprime, N, Kdim);
+    VCB_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+// The int8 rule (DESIGN.md section 2.2), one warp per row m of fp32 W [N, K]: e = the smallest integer >= -126 with
+// max|W[m,:]| <= 127 * 2^e, q = round-half-even(W / 2^e) in [-127, 127].  With amax = f * 2^p, f in [1, 2): e = p - 6 when
+// f <= 127/64 = 1.984375 (mantissa field <= 0x7e0000), else p - 5; zero or subnormal amax: -126.  Scaling by 2^-e
+// (a normal fp32 for every such e) is exact where W / 2^e is, and rounds as the division does where it is not.
+__global__ void weight_quantize_kernel(const float* __restrict__ W, int N, int Kdim, int8_t* __restrict__ q,
+                                       int32_t* __restrict__ e_out, float* __restrict__ scale) {
+    const int m = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (m >= N) return;
+    const float* row = W + static_cast<size_t>(m) * Kdim;
+    float amax = 0.f;
+    for (int k = lane; k < Kdim; k += 32) amax = fmaxf(amax, fabsf(row[k]));
+    amax = warp_max(amax);
+    const uint32_t b = __float_as_uint(amax);
+    const int e = (b >> 23) == 0 ? -126 : max(static_cast<int>(b >> 23) - 127 - 6 + ((b & 0x7fffffu) > 0x7e0000u), -126);
+    const float inv = __uint_as_float(static_cast<uint32_t>(127 - e) << 23);
+    int8_t* qrow = q + static_cast<size_t>(m) * Kdim;
+    for (int k = lane; k < Kdim; k += 32) qrow[k] = static_cast<int8_t>(__float2int_rn(row[k] * inv));
+    if (lane == 0) {
+        if (e_out) e_out[m] = e;
+        if (scale) scale[m] = __uint_as_float(static_cast<uint32_t>(127 + e) << 23);
+    }
+}
+
+// int8 row-major [N, K] -> int8 tiles (w8_index), rows beyond N zero-filled
+__global__ void pack_w8_tiles_kernel(const int8_t* __restrict__ q, uint8_t* __restrict__ out, int N, int Kdim) {
+    const size_t total = static_cast<size_t>((N + GEMM_BM - 1) / GEMM_BM) * GEMM_BM * Kdim;
+    for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
+         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const int m = static_cast<int>(i / Kdim), k = static_cast<int>(i % Kdim);
+        out[w8_index(m, k, Kdim)] = m < N ? static_cast<uint8_t>(q[i]) : 0;
+    }
+}
+
+// int8 tiles -> the bf16 tiles of pack_weight holding W_deq = q * 2^e (exact), for the rows-as-M prefill GEMM
+__global__ void expand_w8_tiles_kernel(const uint8_t* __restrict__ in, const float* __restrict__ scale,
+                                       __nv_bfloat16* __restrict__ out, int N, int Kdim) {
+    const size_t total = static_cast<size_t>((N + GEMM_BM - 1) / GEMM_BM) * GEMM_BM * Kdim;
+    const int KB = Kdim / GEMM_BK;
+    for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < total;
+         i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+        const int c = static_cast<int>(i % GEMM_BK);
+        const int r = static_cast<int>((i / GEMM_BK) % GEMM_BM);
+        const size_t blk = i / (GEMM_BK * GEMM_BM);
+        const int m = static_cast<int>(blk / KB) * GEMM_BM + r, k = static_cast<int>(blk % KB) * GEMM_BK + c;
+        out[i] = __float2bfloat16_rn(m < N ? static_cast<float>(static_cast<int8_t>(in[w8_index(m, k, Kdim)])) * scale[m] : 0.f);
+    }
+}
+
+static int make_tmap_w8(CUtensorMap* out, const void* base, uint64_t rows);
+
+int weight_quantize(const float* W, int N, int Kdim, int8_t* q, int32_t* e, float* scale) {
+    weight_quantize_kernel<<<(N * 32 + 255) / 256, 256>>>(W, N, Kdim, q, e, scale);
+    VCB_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
+int pack_weight_w8(const int8_t* q, uint8_t* out, int N, int Kdim, CUtensorMap* tm) {
+    if (Kdim % 128) {
+        set_error("int8 weights: K=%d not a multiple of 128", Kdim);
+        return -1;
+    }
+    pack_w8_tiles_kernel<<<1024, 256>>>(q, out, N, Kdim);
+    VCB_CUDA_OK(cudaGetLastError());
+    return make_tmap_w8(tm, out, packed_weight_elems(N, Kdim) / 128);
+}
+
+int expand_weight_w8(const uint8_t* W8, const float* scale, __nv_bfloat16* out, int N, int Kdim, cudaStream_t st) {
+    expand_w8_tiles_kernel<<<1024, 256, 0, st>>>(W8, scale, out, N, Kdim);
     VCB_CUDA_OK(cudaGetLastError());
     return 0;
 }
@@ -670,6 +870,27 @@ int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_
     return 0;
 }
 
+// int8 weight tiles as `rows` rows of 128 bytes, box = one 16 KB tile, 128B swizzle
+static int make_tmap_w8(CUtensorMap* out, const void* base, uint64_t rows) {
+    PFN_encodeTiled fn = get_encode_fn();
+    if (!fn) {
+        set_error("cuTensorMapEncodeTiled entry point unavailable");
+        return -1;
+    }
+    cuuint64_t gdim[2] = {128, rows};
+    cuuint64_t gstride[1] = {128};
+    cuuint32_t box[2] = {128, GEMM_BM};
+    cuuint32_t estr[2] = {1, 1};
+    const CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), gdim, gstride, box, estr,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        set_error("cuTensorMapEncodeTiled (int8 weights) failed: %d (rows=%llu)", (int)r, (unsigned long long)rows);
+        return -1;
+    }
+    return 0;
+}
+
 // Co-residency of one instantiation, from the occupancy API: clusters[i] = clusters of 2^i CTAs the device can hold at
 // once, 0 where it cannot place one (a cluster of 16 is non-portable: all of its CTAs must fit into one GPC at once).
 struct GemmOccupancy {
@@ -678,12 +899,12 @@ struct GemmOccupancy {
 };
 
 // Queried once per instantiation, after opting in to its shared memory and to non-portable cluster sizes.
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool W8 = false>
 static const GemmOccupancy& occupancy() {
     static GemmOccupancy occ;
     if (occ.max_cluster) return occ;
-    using L = GemmSmem<BN, STAGES>;
-    const auto kern = gemm_w_xT_cluster<BN, STAGES>;
+    using L = GemmSmem<BN, STAGES, W8>;
+    const auto kern = gemm_w_xT_cluster<BN, STAGES, false, W8>;
     cudaError_t err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
     if (err == cudaSuccess) err = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
     if (err != cudaSuccess) {
@@ -722,9 +943,9 @@ static const GemmOccupancy& occupancy() {
     return occ = q;
 }
 
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool W8 = false>
 static int launch_one(const GemmCall& g, int splits, cudaStream_t st) {
-    using L = GemmSmem<BN, STAGES>;
+    using L = GemmSmem<BN, STAGES, W8>;
     const int tiles = (g.Nout + GEMM_BM - 1) / GEMM_BM;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(tiles * splits, g.grp.tmA ? g.groups : 1, 1);
@@ -742,10 +963,10 @@ static int launch_one(const GemmCall& g, int splits, cudaStream_t st) {
     cfg.numAttrs = g.pdl ? 2 : 1;
     const int total_kb = g.Kdim / GEMM_BK;
     const int kbps = (total_kb + splits - 1) / splits;
-    auto kern = gemm_w_xT_cluster<BN, STAGES>;
+    auto kern = gemm_w_xT_cluster<BN, STAGES, false, W8>;
     if (g.ep.mode == EPI_QKV && g.ep.kv_fp8) {
         // same shared memory and cluster shapes as the plain instantiation, whose occupancy chose the split count
-        kern = gemm_w_xT_cluster<BN, STAGES, true>;
+        kern = gemm_w_xT_cluster<BN, STAGES, true, W8>;
         static bool attr_set = false;
         if (!attr_set) {
             VCB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
@@ -754,7 +975,7 @@ static int launch_one(const GemmCall& g, int splits, cudaStream_t st) {
         }
     }
     VCB_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, *g.tmA, *g.tmB, g.ep, g.Nout, total_kb, kbps, g.b_col_off, g.nvalid, g.pf_ptr,
-                                   static_cast<unsigned long long>(g.pf_bytes), g.grp));
+                                   static_cast<unsigned long long>(g.pf_bytes), g.grp, g.wscale));
     return 0;
 }
 
@@ -762,9 +983,9 @@ struct GemmVariant {
     const GemmOccupancy& (*occupancy)() = nullptr;
     int (*launch)(const GemmCall&, int, cudaStream_t) = nullptr;
 };
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool W8 = false>
 static GemmVariant variant() {
-    return {occupancy<BN, STAGES>, launch_one<BN, STAGES>};
+    return {occupancy<BN, STAGES, W8>, launch_one<BN, STAGES, W8>};
 }
 
 // The kernel for `bpad` token rows (2 * bpad hi/lo activation rows per tile); empty for any other padding.
@@ -774,6 +995,16 @@ static GemmVariant find_variant(int bpad) {
         case 32: return variant<64, gemm_stages(32)>();
         case 64: return variant<128, gemm_stages(64)>();
         case 128: return variant<256, gemm_stages(128)>();
+        default: return {};
+    }
+}
+// ... and with int8 weights
+static GemmVariant find_variant_w8(int bpad) {
+    switch (bpad) {
+        case 16: return variant<32, gemm_stages_w8(16), true>();
+        case 32: return variant<64, gemm_stages_w8(32), true>();
+        case 64: return variant<128, gemm_stages_w8(64), true>();
+        case 128: return variant<256, gemm_stages_w8(128), true>();
         default: return {};
     }
 }
@@ -816,6 +1047,10 @@ int gemm_launch(const GemmCall& g, cudaStream_t st) {
         return -1;
     }
     if (g.simt) {
+        if (g.w8) {
+            set_error("gemm: the CUDA-core cross-check GEMM has no int8-weight path");
+            return -1;
+        }
         dim3 grid((g.Nout * 32 + 255) / 256, 1, 1);
         gemm_w_xT_simt<<<grid, 256, 0, st>>>(g.W, g.X, g.ep, g.Nout, g.Kdim, g.ldx, g.bpad, g.b_col_off, g.nvalid);
         VCB_CUDA_OK(cudaGetLastError());
@@ -828,7 +1063,19 @@ int gemm_launch(const GemmCall& g, cudaStream_t st) {
     }
     int splits = 0, stages = 0;
     if (gemm_launch_shape(g, 0, splits, stages)) return -1;
-    return find_variant(g.bpad).launch(g, splits, st);
+    if (!g.w8) return find_variant(g.bpad).launch(g, splits, st);
+    // int8 weights: the bf16 kernel's launch shape (split count and K slices), on 128-k tiles
+    if (g.Kdim % 128) {
+        set_error("gemm: int8 weights need K %% 128 == 0 (K=%d)", g.Kdim);
+        return -1;
+    }
+    const GemmVariant v = find_variant_w8(g.bpad);
+    const int placeable = v.occupancy().max_cluster;
+    if (placeable < splits) {
+        if (placeable) set_error("gemm: the int8-weight kernel for bpad %d places clusters of at most %d, not %d", g.bpad, placeable, splits);
+        return -1;
+    }
+    return v.launch(g, splits, st);
 }
 
 // Cluster size (= K splits) of a launch of `groups` x ceil(Nout / 128) tiles.  `room` = CTAs of this kernel the device

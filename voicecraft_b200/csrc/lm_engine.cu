@@ -1,6 +1,7 @@
 // libvcb200.so -- engine object + C ABI of the codec-LM decode path (include/vcb200.h).
 //
-// Owns: bf16 GEMM weights + their TMA descriptors, fp32 embeddings / LayerNorm / biases, the paged KV pool,
+// Owns: packed GEMM weights (bf16, or int8 with a scale per row) + their TMA descriptors, fp32 embeddings / LayerNorm /
+// biases, the paged KV pool,
 // per-slot / per-group device state, step workspaces.  The caller (Python/torch) owns inputs, outputs and the stream.
 #include "../../include/vcb200.h"
 #include "lm_kernels.cuh"
@@ -32,10 +33,16 @@ __global__ void f32_to_bf16_kernel(const float* __restrict__ in, __nv_bfloat16* 
         out[i] = __float2bfloat16_rn(in[i]);
 }
 
-struct Matrix {                 // bf16 GEMM operand + descriptor
-    DevBuf<__nv_bfloat16> w;
+struct Matrix {                 // GEMM operand + descriptor: bf16, or int8 with a power-of-two scale per row (VCB_W_INT8)
+    DevBuf<__nv_bfloat16> w;    // bf16 tiles (pack_weight)
+    DevBuf<uint8_t> w8;         // int8 tiles (pack_weight_w8)
+    DevBuf<float> scale;        // int8: 2^e per row
     int rows = 0, cols = 0;
-    CUtensorMap tm;
+    CUtensorMap tm;             // of w or w8
+    CUtensorMap tm_wide;        // int8, wide prefill: the bf16 tiles of W_deq in the engine's scratch (vcb_engine::w8_wide)
+    bool is_w8() const { return w8.get() != nullptr; }
+    const void* data() const { return is_w8() ? static_cast<const void*>(w8.get()) : static_cast<const void*>(w.get()); }
+    size_t bytes() const { return packed_weight_elems(rows, cols) * (is_w8() ? 1 : 2); }   // what the decode GEMM streams
 };
 
 struct Layer {
@@ -56,6 +63,7 @@ struct vcb_engine {
     ModelDims m;
     int num_sms = 132;
     int kv_dtype = KV_BF16;           // VCB_KV_* (vcb_config.kv_dtype)
+    int w8 = 0;                       // vcb_config.weight_dtype == VCB_W_INT8
     int max_pages_per_slot = 0, n_pages = 0;
     std::vector<int> free_pages;
     std::vector<int> page_refs;       // slots whose page list holds the page (a best-of-N group shares its full prompt pages)
@@ -72,6 +80,7 @@ struct vcb_engine {
     DevBuf<float> b_h1;                           // [K*Hh]
     DevBuf<float*> d_bias2;                       // device array of K pointers
     DevBuf<CUtensorMap> d_h2_maps;                // device array of the K second-stage weight maps (grouped launch)
+    DevBuf<float*> d_h2_scales;                   // int8: device array of their K per-row scale pointers
     DevBuf<float*> d_E_audio;                     // device array of K pointers
     DevBuf<float> pe;
     float *E_text = nullptr, *mask_emb = nullptr, *lnf_g = nullptr, *lnf_b = nullptr;   // in f32
@@ -135,6 +144,7 @@ struct vcb_engine {
     DevBuf<int> w_att_cnt;
     DevBuf<__nv_bfloat16> wact_d, wact_f;
     CUtensorMap tm_wact_d, tm_wact_f;
+    DevBuf<__nv_bfloat16> w8_wide;    // int8: W_deq of the layer matrix the next wide GEMM multiplies (largest matrix)
     // persistent decode-step kernel (mega_step.cu): phase tables per bpad (16 / 32), flags, split-K workspace
     int opt_mega = 0, mega_grid = 0, mega_nph = 0, mega_cnt_stride = 0;      // VCB_MEGA=1: decode steps through the persistent kernel
     DevBuf<MegaPhase> d_mega_ph[2];
@@ -190,15 +200,29 @@ namespace {
 int bpad_for(int rows) { return rows <= 16 ? 16 : rows <= 32 ? 32 : rows <= 64 ? 64 : 128; }
 int bpad_idx(int bpad) { return bpad == 16 ? 0 : bpad == 32 ? 1 : bpad == 64 ? 2 : 3; }
 
-// fp32 [rows, cols] on the device -> bf16, pre-tiled 128x64 blocks
-int pack_matrix(const float* src, Matrix* M, int rows, int cols) {
-    if (M->w.ensure(packed_weight_elems(rows, cols))) return -1;
+// fp32 [rows, cols] on the device -> bf16, pre-tiled 128x64 blocks; w8: int8 by the row rule, pre-tiled 128x128 blocks
+int pack_matrix(const float* src, Matrix* M, int rows, int cols, bool w8) {
     M->rows = rows;
     M->cols = cols;
-    return pack_weight(src, M->w, rows, cols, &M->tm);
+    if (!w8) {
+        if (M->w.ensure(packed_weight_elems(rows, cols))) return -1;
+        return pack_weight(src, M->w, rows, cols, &M->tm);
+    }
+    DevBuf<int8_t> q;
+    if (q.alloc(static_cast<size_t>(rows) * cols) || M->scale.alloc(rows) || M->w8.alloc(packed_weight_elems(rows, cols)))
+        return -1;
+    if (weight_quantize(src, rows, cols, q, nullptr, M->scale) || pack_weight_w8(q, M->w8, rows, cols, &M->tm)) return -1;
+    VCB_CUDA_OK(cudaDeviceSynchronize());       // q is released below
+    return 0;
 }
 
-int to_bf16_matrix(vcb_engine* e, const std::string& key, Matrix* M, int rows, int cols) {
+// LayerNorm folding vectors of a packed matrix, from the values the GEMM multiplies (W_deq for int8)
+int ln_fold(const Matrix& W, const float* gamma, const float* beta, const float* bias, float* cvec, float* bprime) {
+    return W.is_w8() ? ln_fold_vectors_w8(W.w8, W.scale, gamma, beta, bias, cvec, bprime, W.rows, W.cols)
+                     : ln_fold_vectors(W.w, gamma, beta, bias, cvec, bprime, W.rows, W.cols);
+}
+
+int to_gemm_matrix(vcb_engine* e, const std::string& key, Matrix* M, int rows, int cols) {
     auto it = e->f32.find(key);
     if (it == e->f32.end()) {
         set_error("missing weight %s", key.c_str());
@@ -209,7 +233,7 @@ int to_bf16_matrix(vcb_engine* e, const std::string& key, Matrix* M, int rows, i
         set_error("weight %s has wrong shape", key.c_str());
         return -1;
     }
-    return pack_matrix(it->second, M, rows, cols);
+    return pack_matrix(it->second, M, rows, cols, e->w8);
 }
 
 int need(vcb_engine* e, const std::string& key, float** out, size_t numel) {
@@ -253,11 +277,13 @@ int run_gemm(vcb_engine* e, const Matrix& W, const CUtensorMap* tmB, const __nv_
              int nvalid, int b_col_off, int kdim, const GemmEpilogue& ep, cudaStream_t st, const Matrix* next = nullptr) {
     GemmCall g;
     if (next && e->opt_prefetch) {
-        g.pf_ptr = next->w;
-        g.pf_bytes = packed_weight_elems(next->rows, next->cols) * 2;
+        g.pf_ptr = next->data();
+        g.pf_bytes = next->bytes();
         if (e->opt_prefetch == 2) g.pf_bytes |= (1ull << 63);        // issue at the end of the weight stream
     }
     g.tmA = &W.tm;
+    g.w8 = W.is_w8();
+    g.wscale = W.scale;
     g.tmB = tmB;
     g.W = W.w;
     g.X = X;
@@ -514,12 +540,23 @@ int pass_gemm(vcb_engine* e, const Pass& p, const Matrix& W, const Plane& in, co
     RowsGemmCall g;
     g.tmX = in.tm;
     g.tmW = &W.tm;
+    g.pdl = e->opt_pdl;
+    if (W.is_w8()) {
+        // int8: the rows-as-M GEMM multiplies W_deq in bf16, expanded into the scratch just before it (and it must not
+        // start its weight loads under the expansion: no PDL)
+        {
+            ProfScope ps(e, PC_MISC, st);
+            if (expand_weight_w8(W.w8, W.scale, e->w8_wide, W.rows, W.cols, st)) return -1;
+            LAUNCH_COUNT(e);
+        }
+        g.tmW = &W.tm_wide;
+        g.pdl = 0;
+    }
     g.ep = ep;
     g.rows = p.rows;
     g.rcap = p.bpad;
     g.Nout = W.rows;
     g.Kdim = W.cols;
-    g.pdl = e->opt_pdl;
     LAUNCH_COUNT(e);
     ProfScope ps(e, PC_GEMM, st);
     return gemm_rows_launch(g, st);
@@ -615,6 +652,14 @@ int wide_alloc(vcb_engine* e) {
     if (make_tmap_bf16_2d(&e->tm_wact_d, e->wact_d, 2 * W, m.d, m.d, 128) ||
         make_tmap_bf16_2d(&e->tm_wact_f, e->wact_f, 2 * W, m.F, m.F, 128))
         return -1;
+    if (e->w8 && !e->w8_wide) {
+        const size_t n = std::max(packed_weight_elems(3 * m.d, m.d), packed_weight_elems(m.F, m.d));
+        if (grab(e->w8_wide, n)) return -1;
+        for (Layer& L : e->layers)
+            for (Matrix* M : {&L.qkv, &L.out, &L.ff1, &L.ff2})
+                if (make_tmap_bf16_2d(&M->tm_wide, e->w8_wide, packed_weight_elems(M->rows, M->cols) / 64, 64, 64, 128))
+                    return -1;
+    }
     return 0;
 }
 
@@ -706,7 +751,7 @@ int mega_setup(vcb_engine* e) {
     const ModelDims& m = e->m;
     e->mega_grid = 0;
     // (the persistent kernel has no fp8 KV path: fp8 engines take the per-kernel step)
-    if (!e->opt_mega || !e->opt_fold || e->opt_simt || e->kv_dtype == KV_FP8 || m.hd != 128 || m.d % 128 || m.F % 128 || (m.K * m.Hh) % 128 || m.Hh % 64) return 0;
+    if (!e->opt_mega || !e->opt_fold || e->opt_simt || e->kv_dtype == KV_FP8 || e->w8 || m.hd != 128 || m.d % 128 || m.F % 128 || (m.K * m.Hh) % 128 || m.Hh % 64) return 0;
     int grid = std::min(mega_max_grid(32, e->kv_dtype == KV_FP32), mega_max_grid(16, e->kv_dtype == KV_FP32));
     if (getenv("VCB_MEGA_GRID")) grid = std::min(grid, atoi(getenv("VCB_MEGA_GRID")));
     if (grid < 1) return 0;
@@ -897,6 +942,8 @@ int sample_rows(vcb_engine* e, const Pass& p, const float* noise, const vcb_samp
         g.pdl = e->opt_pdl;
         g.grp.tmA = e->d_h2_maps;
         g.grp.bias = e->d_bias2;
+        g.w8 = e->w8;
+        g.grp.wscale = e->w8 ? static_cast<const float* const*>(e->d_h2_scales) : nullptr;
         g.grp.b_stride = m.Hh;
         g.grp.col_stride = m.Vpad;
         g.groups = m.K;
@@ -993,9 +1040,22 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
         set_error("kv_dtype %d: VCB_KV_BF16 (0), VCB_KV_FP32 (1) or VCB_KV_FP8 (2)", cfg->kv_dtype);
         return -1;
     }
+    if (cfg->weight_dtype != VCB_W_BF16 && cfg->weight_dtype != VCB_W_INT8) {
+        set_error("weight_dtype %d: VCB_W_BF16 (0) or VCB_W_INT8 (1)", cfg->weight_dtype);
+        return -1;
+    }
     const char* simt = getenv("VCB_GEMM_IMPL");
     if (simt && !strcmp(simt, "simt") && cfg->kv_dtype == VCB_KV_FP8) {
         set_error("VCB_GEMM_IMPL=simt: the CUDA-core cross-check GEMM has no fp8 KV epilogue");
+        return -1;
+    }
+    if (simt && !strcmp(simt, "simt") && cfg->weight_dtype == VCB_W_INT8) {
+        set_error("VCB_GEMM_IMPL=simt: the CUDA-core cross-check GEMM has no int8-weight path");
+        return -1;
+    }
+    if (cfg->weight_dtype == VCB_W_INT8 && (cfg->d_model % 128 || (cfg->audio_vocab_size / 2) % 128)) {
+        set_error("int8 weights: d_model and audio_vocab_size / 2 must be multiples of 128 (d=%d, vocab=%d)", cfg->d_model,
+                  cfg->audio_vocab_size);
         return -1;
     }
     int ndev = 0;
@@ -1037,6 +1097,7 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
         return -1;
     }
     e->kv_dtype = cfg->kv_dtype;
+    e->w8 = cfg->weight_dtype == VCB_W_INT8;
     e->max_pages_per_slot = (cfg->max_seq_len + KV_PAGE - 1) / KV_PAGE;
     e->n_pages = e->max_pages_per_slot * cfg->max_slots;
     for (int p = e->n_pages - 1; p >= 0; --p) e->free_pages.push_back(p);
@@ -1124,10 +1185,10 @@ int vcb_finalize_weights(vcb_engine* e) {
             snprintf(key, sizeof(key), "decoder.layers.%d.%s", l, suffix);
             return std::string(key);
         };
-        if (to_bf16_matrix(e, K("self_attn.in_proj_weight"), &L.qkv, 3 * m.d, m.d)) return -1;
-        if (to_bf16_matrix(e, K("self_attn.out_proj.weight"), &L.out, m.d, m.d)) return -1;
-        if (to_bf16_matrix(e, K("linear1.weight"), &L.ff1, m.F, m.d)) return -1;
-        if (to_bf16_matrix(e, K("linear2.weight"), &L.ff2, m.d, m.F)) return -1;
+        if (to_gemm_matrix(e, K("self_attn.in_proj_weight"), &L.qkv, 3 * m.d, m.d)) return -1;
+        if (to_gemm_matrix(e, K("self_attn.out_proj.weight"), &L.out, m.d, m.d)) return -1;
+        if (to_gemm_matrix(e, K("linear1.weight"), &L.ff1, m.F, m.d)) return -1;
+        if (to_gemm_matrix(e, K("linear2.weight"), &L.ff2, m.d, m.F)) return -1;
         if (need(e, K("self_attn.in_proj_bias"), &L.b_qkv, 3 * m.d) || need(e, K("self_attn.out_proj.bias"), &L.b_out, m.d) ||
             need(e, K("linear1.bias"), &L.b_ff1, m.F) || need(e, K("linear2.bias"), &L.b_ff2, m.d) ||
             need(e, K("norm1.weight"), &L.ln1_g, m.d) || need(e, K("norm1.bias"), &L.ln1_b, m.d) ||
@@ -1136,12 +1197,11 @@ int vcb_finalize_weights(vcb_engine* e) {
         if (L.c_qkv.ensure(3 * m.d, true) || L.bp_qkv.ensure(3 * m.d, true) || L.c_ff1.ensure(m.F, true) ||
             L.bp_ff1.ensure(m.F, true))
             return -1;
-        if (ln_fold_vectors(L.qkv.w, L.ln1_g, L.ln1_b, L.b_qkv, L.c_qkv, L.bp_qkv, 3 * m.d, m.d) ||
-            ln_fold_vectors(L.ff1.w, L.ln2_g, L.ln2_b, L.b_ff1, L.c_ff1, L.bp_ff1, m.F, m.d))
+        if (ln_fold(L.qkv, L.ln1_g, L.ln1_b, L.b_qkv, L.c_qkv, L.bp_qkv) || ln_fold(L.ff1, L.ln2_g, L.ln2_b, L.b_ff1, L.c_ff1, L.bp_ff1))
             return -1;
         VCB_CUDA_OK(cudaDeviceSynchronize());
         for (const char* w : {"self_attn.in_proj_weight", "self_attn.out_proj.weight", "linear1.weight", "linear2.weight"})
-            e->f32.erase(K(w));            // bf16 copy made: drop the fp32 staging copy
+            e->f32.erase(K(w));            // packed copy made: drop the fp32 staging copy
         // KV pool for this layer
         const size_t bytes = static_cast<size_t>(e->n_pages) * m.H * kv_slab_bytes(e->kv_dtype, m.hd);
         if (L.kpool.ensure(bytes, true) || L.vpool.ensure(bytes, true)) return -1;
@@ -1169,7 +1229,7 @@ int vcb_finalize_weights(vcb_engine* e) {
             if (need(e, key, &b0, m.Hh)) return -1;
             VCB_CUDA_OK(cudaMemcpy(e->b_h1 + static_cast<size_t>(k) * m.Hh, b0, m.Hh * 4, cudaMemcpyDeviceToDevice));
             snprintf(key, sizeof(key), "predict_layer.%d.2.weight", k);
-            if (to_bf16_matrix(e, key, &e->h2[k], m.V, m.Hh)) return -1;
+            if (to_gemm_matrix(e, key, &e->h2[k], m.V, m.Hh)) return -1;
             VCB_CUDA_OK(cudaDeviceSynchronize());
             e->f32.erase(key);
             snprintf(key, sizeof(key), "predict_layer.%d.2.bias", k);
@@ -1177,9 +1237,9 @@ int vcb_finalize_weights(vcb_engine* e) {
             snprintf(key, sizeof(key), "audio_embedding.%d.word_embeddings.weight", k);
             if (need(e, key, &ea[k], static_cast<size_t>(m.V) * m.d)) return -1;
         }
-        if (pack_matrix(stacked, &e->h1, m.K * m.Hh, m.d)) return -1;
+        if (pack_matrix(stacked, &e->h1, m.K * m.Hh, m.d, e->w8)) return -1;
         if (e->c_h1.ensure(m.K * m.Hh, true) || e->bp_h1.ensure(m.K * m.Hh, true)) return -1;
-        if (ln_fold_vectors(e->h1.w, e->lnf_g, e->lnf_b, e->b_h1, e->c_h1, e->bp_h1, m.K * m.Hh, m.d)) return -1;
+        if (ln_fold(e->h1, e->lnf_g, e->lnf_b, e->b_h1, e->c_h1, e->bp_h1)) return -1;
         VCB_CUDA_OK(cudaDeviceSynchronize());
         stacked.reset();
         if (e->d_bias2.ensure(m.K) || e->d_E_audio.ensure(m.K)) return -1;
@@ -1189,6 +1249,12 @@ int vcb_finalize_weights(vcb_engine* e) {
             for (int k = 0; k < m.K; ++k) maps[k] = e->h2[k].tm;
             if (e->d_h2_maps.ensure(m.K)) return -1;
             VCB_CUDA_OK(cudaMemcpy(e->d_h2_maps, maps.data(), m.K * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
+        }
+        if (e->w8) {
+            std::vector<float*> sc(m.K);
+            for (int k = 0; k < m.K; ++k) sc[k] = e->h2[k].scale;
+            if (e->d_h2_scales.ensure(m.K)) return -1;
+            VCB_CUDA_OK(cudaMemcpy(e->d_h2_scales, sc.data(), m.K * sizeof(float*), cudaMemcpyHostToDevice));
         }
         VCB_CUDA_OK(cudaMemcpy(e->d_bias2, b2.data(), m.K * sizeof(float*), cudaMemcpyHostToDevice));
         VCB_CUDA_OK(cudaMemcpy(e->d_E_audio, ea.data(), m.K * sizeof(float*), cudaMemcpyHostToDevice));
@@ -1770,6 +1836,47 @@ int vcb_debug_gemm(const float* W_dev, const float* X_dev, float* out_dev, int32
     return 0;
 }
 
+// The int8 weight rule of vcb_finalize_weights: q row-major [N][K], e [N].  Synchronous.
+int vcb_debug_weight_quantize(const float* W_dev, int32_t N, int32_t Kd, int8_t* q_out, int32_t* e_out) {
+    if (!W_dev || !q_out || !e_out || N < 1 || Kd < 1) {
+        set_error("vcb_debug_weight_quantize: bad argument");
+        return -1;
+    }
+    if (weight_quantize(W_dev, N, Kd, q_out, e_out, nullptr)) return -1;
+    VCB_CUDA_OK(cudaDeviceSynchronize());
+    return 0;
+}
+
+// vcb_debug_gemm's contract through the int8-weight kernel: W quantized by the engine's rule, out = X W_deq^T.
+int vcb_debug_gemm_w8(const float* W_dev, const float* X_dev, float* out_dev, int32_t N, int32_t Kd, int32_t B, int32_t splits) {
+    const int bpad = bpad_for(B);
+    if (B < 1 || B > 128 || N < 1 || Kd < 128 || Kd % 128) {
+        set_error("vcb_debug_gemm_w8: 1 <= B <= 128, N >= 1 and K %% 128 == 0 required");
+        return -1;
+    }
+    DevBuf<int8_t> q;
+    DevBuf<uint8_t> w;
+    DevBuf<float> sc, zb;
+    DevBuf<__nv_bfloat16> x;
+    const SyncOnExit sync;
+    if (splits <= 0) splits = gemm_pick_splits(N, Kd, bpad, 1);
+    if (q.alloc(static_cast<size_t>(N) * Kd) || w.alloc(packed_weight_elems(N, Kd)) || sc.alloc(N) ||
+        x.alloc(static_cast<size_t>(2 * bpad) * Kd, true) || zb.alloc(N, true))
+        return -1;
+    CUtensorMap tmA, tmB;
+    if (weight_quantize(W_dev, N, Kd, q, nullptr, sc) || pack_weight_w8(q, w, N, Kd, &tmA)) return -1;
+    split_rows_kernel<<<dim3((Kd + 255) / 256, B), 256>>>(X_dev, Kd, x, Kd, bpad);
+    VCB_CUDA_OK(cudaDeviceSynchronize());
+    if (make_tmap_bf16_2d(&tmB, x, 2 * bpad, Kd, Kd, 2 * bpad)) return -1;
+    GemmCall g;
+    g.tmA = &tmA; g.tmB = &tmB; g.X = x; g.w8 = 1; g.wscale = sc;
+    g.ep.mode = EPI_LOGITS; g.ep.bias = zb; g.ep.out = out_dev; g.ep.ld_out = N; g.ep.col_off = 0;
+    g.Nout = N; g.Kdim = Kd; g.ldx = Kd; g.bpad = bpad; g.splits = splits; g.nvalid = B;
+    if (gemm_launch(g, 0)) return -1;
+    VCB_CUDA_OK(cudaDeviceSynchronize());
+    return 0;
+}
+
 // Parity hooks of the paged attention (attn_rows_kernel) with the engine's launch decisions; see include/vcb200.h.
 // group_first null: every row on its own (GMAX = 1); else the row groups, checked here and split into launch groups of
 // at most ATT_GMAX rows
@@ -2137,6 +2244,10 @@ int vcb_set_option(vcb_engine* e, const char* name, int32_t value) {
             set_error("gemm_simt: the CUDA-core cross-check GEMM has no fp8 KV epilogue");
             return -1;
         }
+        if (value && e->w8) {
+            set_error("gemm_simt: the CUDA-core cross-check GEMM has no int8-weight path");
+            return -1;
+        }
         e->opt_simt = value;
     }
     else if (!strcmp(name, "profile")) e->opt_profile = value;
@@ -2157,6 +2268,15 @@ int64_t vcb_counter(vcb_engine* e, const char* name) {
     if (!strcmp(name, "poll_frames")) return e->n_poll_frames;
     if (!strcmp(name, "kv_pages_free")) return static_cast<int64_t>(e->free_pages.size());
     if (!strcmp(name, "prefill_rows")) return e->n_prefill_rows;
+    if (!strcmp(name, "weight_bytes")) {         // packed GEMM operands (+ int8 scales) and the int8 prefill scratch
+        int64_t b = static_cast<int64_t>(e->w8_wide.size()) * 2;
+        auto add = [&](const Matrix& M) { b += static_cast<int64_t>(M.bytes() + (M.is_w8() ? M.rows * sizeof(float) : 0)); };
+        for (const Layer& L : e->layers)
+            for (const Matrix* M : {&L.qkv, &L.out, &L.ff1, &L.ff2}) add(*M);
+        add(e->h1);
+        for (const Matrix& M : e->h2) add(M);
+        return b;
+    }
     if (!strcmp(name, "kv_bytes_per_token")) return static_cast<int64_t>(e->m.L) * 2 * e->m.H * kv_slab_bytes(e->kv_dtype, e->m.hd) / KV_PAGE;
     return -1;
 }

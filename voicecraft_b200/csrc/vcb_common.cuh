@@ -270,4 +270,41 @@ __device__ __forceinline__ void wg_mma_kblock(float (&d)[N / 2], uint32_t a_addr
     }
 }
 
+// The same k16 step with A from registers: a[4] = the thread's bf16x2 fragment (rows 16w + l/4 and + 8; k 2(l%4), +1, +8,
+// +9: a[0] row r k 2t.., a[1] row r+8, a[2] row r k 2t+8.., a[3] row r+8).  Written before the wg_fence() of the issue.
+__device__ __forceinline__ void wgmma_m64n16_ra(float* d, const uint32_t (&a)[4], uint64_t b_desc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc));
+}
+__device__ __forceinline__ void wgmma_m64n32_ra(float* d, const uint32_t (&a)[4], uint64_t b_desc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc));
+}
+__device__ __forceinline__ void wgmma_m64n64_ra(float* d, const uint32_t (&a)[4], uint64_t b_desc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc));
+}
+// wg_mma_kblock's step k (0..3) of the 64-wide k-block at b_addr, A from registers; the same N pieces in the same order
+template <int N>
+__device__ __forceinline__ void wg_mma_k16_ra(float (&d)[N / 2], const uint32_t (&a)[4], uint32_t b_addr, int k) {
+    constexpr int NC = N < 64 ? N : 64;
+    const uint64_t b = gmma_desc_kmajor_sw128(b_addr) + 2 * k;
+#pragma unroll
+    for (int n0 = 0; n0 < N; n0 += NC) {
+        const uint64_t bk = b + static_cast<uint64_t>(n0 * 8);
+        if constexpr (NC == 64) wgmma_m64n64_ra(d + n0 / 2, a, bk);
+        else if constexpr (NC == 32) wgmma_m64n32_ra(d + n0 / 2, a, bk);
+        else wgmma_m64n16_ra(d + n0 / 2, a, bk);
+    }
+}
+
 }  // namespace vcb

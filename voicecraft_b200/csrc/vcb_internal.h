@@ -298,6 +298,7 @@ struct GemmGroup {
     const CUtensorMap* tmA = nullptr;     // device array [groups]; null = plain launch
     const float* const* bias = nullptr;   // device array [groups]
     int b_stride = 0, col_stride = 0;     // added per group to the activation column offset / output column offset
+    const float* const* wscale = nullptr; // int8 weights: device array [groups] of the per-feature 2^e
 };
 
 struct GemmCall {
@@ -312,6 +313,8 @@ struct GemmCall {
     int groups = 1;
     const void* pf_ptr = nullptr;       // next GEMM's weights: prefetched into L2 while this kernel runs
     size_t pf_bytes = 0;
+    int w8 = 0;                         // tmA: int8 tiles (pack_weight_w8) with 2^e per feature in wscale (or grp.wscale)
+    const float* wscale = nullptr;
 };
 int gemm_launch(const GemmCall& g, cudaStream_t st);
 // What gemm_launch would launch for g: the pipeline stages and the split count after the fallback to the largest cluster
@@ -333,6 +336,14 @@ size_t packed_weight_elems(int N, int Kdim);
 int pack_weight(const float* w_f32_dev, __nv_bfloat16* out, int N, int Kdim, CUtensorMap* tm);
 int ln_fold_vectors(const __nv_bfloat16* Wp, const float* gamma, const float* beta, const float* bias, float* cvec,
                     float* bprime, int N, int Kdim);
+// Int8 weights (DESIGN.md section 2.2): the row rule on fp32 [N, K] (q row-major; e and / or scale = 2^e per row may be
+// null), the pre-tiled int8 layout the W8 decode GEMM streams, its bf16 expansion (W_deq in pack_weight's layout, for the
+// rows-as-M prefill GEMM) and the LayerNorm folding vectors from W_deq
+int weight_quantize(const float* W, int N, int Kdim, int8_t* q, int32_t* e, float* scale);
+int pack_weight_w8(const int8_t* q, uint8_t* out, int N, int Kdim, CUtensorMap* tm);
+int expand_weight_w8(const uint8_t* W8, const float* scale, __nv_bfloat16* out, int N, int Kdim, cudaStream_t st);
+int ln_fold_vectors_w8(const uint8_t* W8, const float* scale, const float* gamma, const float* beta, const float* bias,
+                       float* cvec, float* bprime, int N, int Kdim);
 void gemm_timeline_set(unsigned long long* buf, unsigned int* cnt);
 int make_tmap_bf16_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t ld_elems,
                       uint32_t box_rows);

@@ -45,6 +45,8 @@ except Exception:  # pragma: no cover
 
 # configure_engine(kv_dtype=...) -> vcb_config.kv_dtype (VCB_KV_* of include/vcb200.h)
 KV_DTYPES = {"bf16": 0, "fp32": 1, "fp8": 2}
+# configure_engine(weight_dtype=...) -> vcb_config.weight_dtype (VCB_W_* of include/vcb200.h)
+WEIGHT_DTYPES = {"bf16": 0, "int8": 1}
 
 
 def sine_pe(length: int, dim: int) -> torch.Tensor:
@@ -158,7 +160,7 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         # engine configuration (see configure_engine)
         self._eng = None
         self._eng_key = None
-        self._eng_opts = dict(max_slots=8, max_seq_len=2048, max_new_tokens=4096, kv_dtype="bf16")
+        self._eng_opts = dict(max_slots=8, max_seq_len=2048, max_new_tokens=4096, kv_dtype="bf16", weight_dtype="bf16")
         self.noise_fn = None          # optional: callable(shape, device) -> fp32 Exp(1) tensor on `device`
         self.poll_every = 4           # inference_tts*: poll the done flag every N steps (device generator only)
         self._sessions = {}           # first slot -> slot list of every group held by a call, session or batcher (the engine
@@ -181,12 +183,16 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     # ------------------------------------------------------------------------------------------------
     def configure_engine(self, **opts):
         """max_slots, max_seq_len, max_new_tokens, kv_dtype ('bf16' default | 'fp32' | 'fp8': e4m3 with a power-of-two
-        scale per token and head, half the cache bytes of bf16; INTEGRATION.md).  Rebuilds lazily."""
+        scale per token and head, half the cache bytes of bf16; INTEGRATION.md), weight_dtype ('bf16' default | 'int8': the
+        GEMM weights as int8 with a power-of-two scale per output feature, half the weight bytes; INTEGRATION.md).
+        Rebuilds lazily."""
         for k in opts:
             if k not in self._eng_opts:
                 raise KeyError(k)
         if "kv_dtype" in opts and opts["kv_dtype"] not in KV_DTYPES:
             raise ValueError(f"kv_dtype {opts['kv_dtype']!r}: one of {sorted(KV_DTYPES)}")
+        if "weight_dtype" in opts and opts["weight_dtype"] not in WEIGHT_DTYPES:
+            raise ValueError(f"weight_dtype {opts['weight_dtype']!r}: one of {sorted(WEIGHT_DTYPES)}")
         self._eng_opts.update(opts)
         self._drop_engine()
 
@@ -273,7 +279,7 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
             empty_token=a.empty_token, eog=a.eog, audio_pad_token=a.audio_pad_token, eos=a.eos if a.eos > 0 else -1,
             encodec_sr=int(a.encodec_sr), max_n_spans=a.max_n_spans, max_slots=o["max_slots"],
             max_seq_len=o["max_seq_len"], max_new_tokens=o["max_new_tokens"],
-            kv_dtype=KV_DTYPES[o["kv_dtype"]], device=dev.index or 0)
+            kv_dtype=KV_DTYPES[o["kv_dtype"]], device=dev.index or 0, weight_dtype=WEIGHT_DTYPES[o["weight_dtype"]])
         h = C.c_void_p()
         _lib.check(lib.vcb_create(C.byref(cfg), C.byref(h)))
         try:
