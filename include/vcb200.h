@@ -8,7 +8,8 @@
  *
  * Threading: one engine per device; calls on one engine must be serialised by the caller (the reference is
  * single-threaded Python, inference_tts_scale.py:42).  Synchronisation contract, per entry point:
- *   vcb_sample / vcb_decode_step   asynchronous on `stream` (one small pinned H2D copy when the slot list changes);
+ *   vcb_sample / vcb_decode_step   asynchronous on `stream` (one small pinned H2D copy when the slot list changes, and
+ *                                  one when a slot's KV page list grows);
  *                                  the decode loop never blocks the host
  *   vcb_prefill                    once per utterance batch: waits for `stream`, uploads the slot / page / row tables and
  *                                  the groups' sampling parameters with blocking copies, then enqueues the prefill kernels
@@ -18,8 +19,20 @@
  *                                  sources), then waits for `stream` once; the codes stay on the device, the status and
  *                                  per-slot results arrive in one small copy.  _ex reads each edit source's y0 on `stream`
  *   vcb_release                    waits for the device (the slot's KV pages go back to the free list)
+ *   vcb_swap_out                   waits for `stream`, copies the slot's state and KV pages to library-owned pinned memory
+ *                                  (one gather kernel and one D2H copy on `stream`), waits for `stream` again, then
+ *                                  releases the slot as vcb_release does
+ *   vcb_swap_in                    waits for `stream`, restores a snapshot with blocking copies and one H2D copy plus one
+ *                                  scatter kernel on `stream`, and waits for `stream` before it returns (the snapshot may
+ *                                  be freed at once)
+ *   vcb_snapshot_free              host only
  *   vcb_create / vcb_load_* / vcb_finalize_weights / vcb_destroy   blocking set-up calls
  * A call that fails leaves no slot, group or KV page held (vcb_prefill validates every prompt before it mutates state).
+ *
+ * KV pool (DESIGN.md section 3): vcb_config.kv_pool_bytes sizes the page pool; a one-copy prompt holds the pages its
+ * positions use and vcb_decode_step grows it by VCB_KV_GROW_PAGES pages at a time.  When the pool cannot cover a step,
+ * vcb_decode_step returns VCB_ERR_KV_FULL and changes nothing; the caller frees pages (vcb_release, vcb_swap_out) and
+ * calls again.
  */
 #ifndef VCB200_H_
 #define VCB200_H_
@@ -37,6 +50,13 @@ enum { VCB_MODE_TTS = 0, VCB_MODE_EDIT = 1 };
 enum { VCB_KV_BF16 = 0, VCB_KV_FP32 = 1, VCB_KV_FP8 = 2 };
 /* GEMM weight policy (DESIGN.md section 2.2): bf16, or int8 with a power-of-two fp32 scale per output feature */
 enum { VCB_W_BF16 = 0, VCB_W_INT8 = 1 };
+/* vcb_decode_step: the KV pool has too few free pages for the listed slots' next positions; nothing was enqueued or taken,
+ * and vcb_counter(e, "kv_pages_needed") is how many pages the call lacked */
+enum { VCB_ERR_KV_FULL = -3 };
+/* pages a one-copy utterance's page list grows by (64 positions each) */
+enum { VCB_KV_GROW_PAGES = 4 };
+
+typedef struct vcb_snapshot vcb_snapshot;
 
 /* Model hyper-parameters: the argparse Namespace the reference model is built from
  * (reference config.py:50-84, models/voicecraft.py:106-195). */
@@ -46,12 +66,16 @@ typedef struct {
     int32_t empty_token, eog, audio_pad_token, eos;       /* eos <= 0: unused */
     int32_t encodec_sr, max_n_spans;
     int32_t max_slots;      /* concurrently open utterances */
-    int32_t max_seq_len;    /* text + audio columns per utterance, upper bound */
+    int32_t max_seq_len;    /* text + audio columns per utterance, upper bound: sizes the page tables and the prefill row
+                             * tables; KV pages are taken as positions are written */
     int32_t max_new_tokens; /* token-log capacity per utterance */
     int32_t kv_dtype;       /* VCB_KV_BF16 (default), VCB_KV_FP32 or VCB_KV_FP8; vcb_create rejects any other value */
     int32_t device;         /* CUDA device ordinal */
     int32_t weight_dtype;   /* VCB_W_BF16 (default) or VCB_W_INT8 (d_model and audio_vocab_size / 2 multiples of 128);
                              * vcb_create rejects any other value */
+    int64_t kv_pool_bytes;  /* KV page pool: 0 = max_slots * ceil(max_seq_len / 64) pages (every slot can reach max_seq_len);
+                             * > 0: floor(kv_pool_bytes / page bytes) pages, a page being 64 positions of K and V in every
+                             * layer (vcb_counter "kv_page_bytes"); vcb_create rejects a negative value or one below a page */
 } vcb_config;
 
 /* Sampling arguments of inference_tts / inference / inference_tts_batch (voicecraft.py:908-920). */
@@ -140,7 +164,11 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
  * group was prefilled without them is rejected before anything is enqueued. */
 int vcb_sample(vcb_engine* e, const int32_t* slots, int32_t n, const float* exp_noise_dev,
                const vcb_sampling* sp, void* stream);
-/* one transformer step on the embeddings produced by the previous sample, then vcb_sample. */
+/* one transformer step on the embeddings produced by the previous sample, then vcb_sample.  Before it enqueues anything,
+ * every listed one-copy slot gets a page for the position it writes (the host bounds it by the slot's prompt length plus the
+ * steps issued since, without reading the device), VCB_KV_GROW_PAGES at a time up to ceil(max_seq_len / 64); the new page-table
+ * entries go up in one small pinned H2D copy on `stream`.  Returns VCB_ERR_KV_FULL, having done nothing, when the free list
+ * cannot cover that. */
 int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float* exp_noise_dev,
                     const vcb_sampling* sp, void* stream);
 int vcb_poll(vcb_engine* e, const int32_t* slots, int32_t n, vcb_status* out_host, void* stream);
@@ -149,6 +177,21 @@ int vcb_read_tokens(vcb_engine* e, int32_t slot, int32_t* out_host, int32_t max_
 /* closes slots slot .. slot+n_copies-1 (slots that are not open are skipped); a KV page goes back to the free list when
  * the last slot holding it is released, and a group's id with its last slot, in any release order */
 int vcb_release(vcb_engine* e, int32_t slot, int32_t n_copies);
+/* Swap a one-copy utterance out to host memory and back, byte for byte (DESIGN.md section 3).  vcb_swap_out copies what the
+ * slot's continuation depends on -- the K and V slabs of its written pages in every layer, its SlotState and GroupState
+ * (Philox offset included), its sampling parameters, token-log rows [0, n_steps), its next-input and last-hidden rows and
+ * the host-side slot flags -- into a snapshot, then releases the slot.  Rejected before anything changes: a slot that is not
+ * open or belongs to a best-of-N group.
+ * vcb_swap_in restores a snapshot of this engine into the free `slot` on newly taken pages and a free group id; rejected
+ * before anything changes: a snapshot of another engine, a slot that is open, no free group, fewer free pages than
+ * vcb_snapshot_pages.  The snapshot stays valid (and owned by the caller) either way.
+ * Snapshots hold pinned host memory (counted in "live_bytes" / "live_handles") until vcb_snapshot_free.  The engine keeps
+ * a device staging region as large as the largest utterance it swapped, at most ceil(max_seq_len / 64) pages ("swap_stage_bytes"), until
+ * vcb_destroy. */
+int vcb_swap_out(vcb_engine* e, int32_t slot, vcb_snapshot** out, void* stream);
+int vcb_swap_in(vcb_engine* e, const vcb_snapshot* snap, int32_t slot, void* stream);
+int32_t vcb_snapshot_pages(const vcb_snapshot* snap);     /* KV pages vcb_swap_in takes */
+int vcb_snapshot_free(vcb_snapshot* snap);                /* NULL: nothing */
 /* Streaming: vcb_poll, plus the newly final frames of the listed slots, un-delayed, as codec codes.
  * Waits for `stream` once.  For listed slot i: final_host[i] = frames of the slot that are final (frame t is final once the
  * token log holds rows up to t+K-1 and rows[t][0] is not the end token; for a finished generation n_steps-K).
@@ -259,7 +302,9 @@ int vcb_set_option(vcb_engine* e, const char* name, int32_t value);   /* "gemm_s
 /* profile mode: summed device ms and launch counts per kernel class since the last read
  * (0 gemm, 1 attention, 2 layernorm/reduce, 3 bias/act/qkv finish, 4 sampler, 5 misc) */
 int vcb_profile_read(vcb_engine* e, double* ms_by_class, int64_t* count_by_class, int32_t n_classes);
-/* "launches", "kv_bytes", "kv_pages_free", "prefill_rows" (rows through the prefill since create), "weight_bytes" (device
+/* "launches", "kv_bytes", "kv_pages_free", "kv_pages_total" (pool size), "kv_pages_needed" (pages the last refused
+ * vcb_decode_step lacked), "kv_page_bytes" (one page: 64 positions of K and V in every layer), "swap_stage_bytes" (device
+ * staging of the swap kernels), "prefill_rows" (rows through the prefill since create), "weight_bytes" (device
  * bytes of the packed GEMM operands with their int8 scales, and the int8 prefill scratch once a prefill allocated it), ...; "live_bytes" / "live_handles" (any e, NULL included): device and pinned bytes, and allocations
  * plus events, the library holds now across every engine, codec engine and stream of the process */
 int64_t vcb_counter(vcb_engine* e, const char* name);

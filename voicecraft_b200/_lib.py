@@ -19,7 +19,11 @@ class vcb_config(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "d_model", "nhead", "num_layers", "n_codebooks", "audio_vocab_size", "n_special", "text_vocab_rows",
         "empty_token", "eog", "audio_pad_token", "eos", "encodec_sr", "max_n_spans", "max_slots", "max_seq_len",
-        "max_new_tokens", "kv_dtype", "device", "weight_dtype")]
+        "max_new_tokens", "kv_dtype", "device", "weight_dtype")] + [("kv_pool_bytes", C.c_int64)]
+
+
+VCB_ERR_KV_FULL = -3        # vcb_decode_step: the KV pool cannot cover the listed slots' next positions; nothing was done
+KV_GROW_PAGES = 4           # pages a one-copy utterance's page list grows by (VCB_KV_GROW_PAGES)
 
 
 class vcb_sampling(C.Structure):
@@ -66,6 +70,10 @@ PROTOTYPES = {
                                      C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p]),
     "vcb_read_tokens": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_void_p]),
     "vcb_release": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
+    "vcb_swap_out": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), C.c_void_p]),
+    "vcb_swap_in": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
+    "vcb_snapshot_pages": (C.c_int32, [C.c_void_p]),
+    "vcb_snapshot_free": (C.c_int, [C.c_void_p]),
     "vcb_debug_logits": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
     "vcb_debug_exponential": (C.c_int, [C.c_void_p, C.c_int64, C.c_uint64, C.c_uint64, C.c_int32, C.c_void_p]),
     "vcb_debug_sampler": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int32, C.POINTER(vcb_sampling)] +

@@ -14,6 +14,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <utility>
 
 namespace vcb {
@@ -64,7 +65,9 @@ struct vcb_engine {
     int num_sms = 132;
     int kv_dtype = KV_BF16;           // VCB_KV_* (vcb_config.kv_dtype)
     int w8 = 0;                       // vcb_config.weight_dtype == VCB_W_INT8
+    uint64_t id = 0;                  // process-unique: a snapshot names the engine it came from
     int max_pages_per_slot = 0, n_pages = 0;
+    int64_t n_pages_needed = 0;       // pages the last refused vcb_decode_step lacked (VCB_ERR_KV_FULL)
     std::vector<int> free_pages;
     std::vector<int> page_refs;       // slots whose page list holds the page (a best-of-N group shares its full prompt pages)
     std::vector<std::vector<int>> slot_pages;
@@ -96,7 +99,8 @@ struct vcb_engine {
     DevBuf<int> att_cnt;              // per (row, head) arrival counters
     int att_maxch = 1, att_chunk_pages = ATT_CHUNK_PAGES;
     std::vector<float*> h_bias2;      // host copy of the K second-stage bias pointers
-    std::vector<int> h_seq_len;       // host mirror of SlotState::seq_len (upper bound for the attention grid)
+    std::vector<int> h_seq_len;       // host upper bound of SlotState::seq_len: the attention grid, and the position the next
+                                      // step writes (page growth)
     DevBuf<__nv_bfloat16> act_d, act_d2, act_f, act_h;
     CUtensorMap tm_act_d[4], tm_act_d2[4], tm_act_f[4], tm_act_h[4];   // bpad = 16, 32, 64, 128
     DevBuf<int> row_slot, row_pos, row_last, page_table;   // decode-step rows
@@ -133,6 +137,16 @@ struct vcb_engine {
     PinnedBuf<int> h_stage;
     static constexpr size_t h_stage_ints = 4096;
     Event stage_ev;
+    // page growth of vcb_decode_step: a ring of pinned staging entries, each reused only once the copy recorded by its
+    // event has run
+    static constexpr int GROW_RING = 16, GROW_INTS = MAX_ROWS * VCB_KV_GROW_PAGES;
+    PinnedBuf<int> grow_stage;        // [GROW_RING][GROW_INTS]
+    Event grow_ev[GROW_RING];
+    int grow_next = 0;
+    // swap: every layer's K and V slabs of one utterance's pages, contiguous (vcb_swap_out / vcb_swap_in); grown to the
+    // largest utterance swapped so far, at most max_pages_per_slot pages, kept until vcb_destroy ("swap_stage_bytes")
+    DevBuf<uint4> swap_stage;
+    DevBuf<int> swap_pages;           // [max_pages_per_slot] page list of the swap kernels
 
     std::vector<std::array<int, 3>> opt_splits;
     int opt_simt = 0, opt_pdl = 0, opt_profile = 0, opt_prefetch = 0, opt_att_balance = 1;
@@ -179,6 +193,20 @@ struct vcb_engine {
         cudaSetDevice(cfg.device);
         cudaDeviceSynchronize();
     }
+};
+
+// What vcb_swap_out copies of one utterance: everything its continuation reads (DESIGN.md section 3)
+struct vcb_snapshot {
+    uint64_t engine_id = 0;
+    int n_pages = 0;                  // written pages: ceil(seq_len / 64)
+    SlotState S;                      // group / member rewritten by vcb_swap_in
+    GroupState G;                     // Philox offset included; first_slot rewritten
+    SamplingParams sp;                // the group's own parameters (has_sp)
+    char has_sp = 0, rng = 0, edit = 0;
+    int final_frames = 0;             // slot_final
+    PinnedBuf<uint8_t> kv;            // [2L pools][n_pages][H slabs], as kv_pages_copy_kernel stages them
+    PinnedBuf<int> tok;               // token-log rows [0, n_steps) x K
+    PinnedBuf<float> rows;            // x_slot row (next input), h_slot row (last prefill hidden state)
 };
 
 enum { PC_GEMM = 0, PC_ATTN = 1, PC_LN = 2, PC_FINISH = 3, PC_SAMPLER = 4, PC_MISC = 5, PC_MEGA = 6, PC_N = 7 };
@@ -891,6 +919,82 @@ int upload_slots(vcb_engine* e, const int32_t* slots, int n, cudaStream_t st) {
     return upload_ints(e, tab.data(), tab.size(), e->d_slots, st);
 }
 
+// page-list length of a one-copy utterance that writes positions [0, pos]: whole growth chunks, at most max_pages_per_slot
+int grown_pages(const vcb_engine* e, int pos) {
+    const int want = pos / KV_PAGE + 1;
+    return std::min(e->max_pages_per_slot, (want + VCB_KV_GROW_PAGES - 1) / VCB_KV_GROW_PAGES * VCB_KV_GROW_PAGES);
+}
+
+// one KV page of every layer, K and V (the unit of kv_pool_bytes)
+size_t page_bytes_all_layers(const vcb_engine* e) {
+    return 2ull * e->m.L * e->m.H * kv_slab_bytes(e->kv_dtype, e->m.hd);
+}
+
+// a page-table row of `slot` as the device holds it: the slot's pages, then page 0 (never read: attention and the QKV
+// epilogues read positions up to the one a step writes)
+std::vector<int> page_row(const vcb_engine* e, int slot) {
+    std::vector<int> row(e->slot_pages[slot]);
+    row.resize(e->max_pages_per_slot, 0);
+    return row;
+}
+
+// Page growth of a decode step, planned on the host without touching any state: every listed one-copy slot needs a page
+// for position h_seq_len (it writes at most there).  Slots take whole chunks when the free list covers them all, else the
+// pages they need; VCB_ERR_KV_FULL (kv_pages_needed set) when it cannot cover even that.  grow: (slot, new page count).
+int plan_growth(vcb_engine* e, const int32_t* slots, int n, std::vector<std::pair<int, int>>& grow) {
+    grow.clear();
+    size_t need = 0, chunked = 0;
+    std::vector<int> want;
+    for (int i = 0; i < n; ++i) {
+        const int s = slots[i];
+        const int have = static_cast<int>(e->slot_pages[s].size());
+        const int need_s = std::min(e->max_pages_per_slot, e->h_seq_len[s] / KV_PAGE + 1);
+        if (e->slot_copies[s] != 1 || need_s <= have ||
+            std::any_of(grow.begin(), grow.end(), [s](const std::pair<int, int>& g) { return g.first == s; }))
+            continue;
+        const int chunk = grown_pages(e, e->h_seq_len[s]);
+        grow.emplace_back(s, chunk);
+        want.push_back(need_s);
+        need += need_s - have;
+        chunked += chunk - have;
+    }
+    if (need > e->free_pages.size()) {
+        e->n_pages_needed = static_cast<int64_t>(need - e->free_pages.size());
+        set_error("vcb_decode_step: KV pool full: the listed slots need %zu more pages, %zu are free", need,
+                  e->free_pages.size());
+        grow.clear();
+        return VCB_ERR_KV_FULL;
+    }
+    if (chunked > e->free_pages.size())
+        for (size_t i = 0; i < grow.size(); ++i) grow[i].second = want[i];
+    return 0;
+}
+
+// takes the planned pages and enqueues the new page-table entries on `st` (one pinned staging entry of the ring)
+int apply_growth(vcb_engine* e, const std::vector<std::pair<int, int>>& grow, cudaStream_t st) {
+    if (grow.empty()) return 0;
+    const int k = e->grow_next;
+    e->grow_next = (k + 1) % vcb_engine::GROW_RING;
+    VCB_CUDA_OK(cudaEventSynchronize(e->grow_ev[k]));
+    int* stage = e->grow_stage + static_cast<size_t>(k) * vcb_engine::GROW_INTS;
+    int used = 0;
+    for (const auto& g : grow) {
+        auto& pg = e->slot_pages[g.first];
+        const int from = static_cast<int>(pg.size());
+        for (int p = from; p < g.second; ++p) {
+            pg.push_back(e->free_pages.back());
+            e->free_pages.pop_back();
+            ++e->page_refs[pg.back()];
+            stage[used + p - from] = pg.back();
+        }
+        VCB_CUDA_OK(cudaMemcpyAsync(e->page_table + static_cast<size_t>(g.first) * e->max_pages_per_slot + from, stage + used,
+                                    (g.second - from) * sizeof(int), cudaMemcpyHostToDevice, st));
+        used += g.second - from;
+    }
+    VCB_CUDA_OK(cudaEventRecord(e->grow_ev[k], st));
+    return 0;
+}
+
 // exp_noise_dev may be null only if every listed slot's group carries its own Philox stream (vcb_prompt::rng_threads)
 int noise_required(vcb_engine* e, const int32_t* slots, int n, const float* noise) {
     if (noise) return 0;
@@ -1100,6 +1204,18 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
     e->w8 = cfg->weight_dtype == VCB_W_INT8;
     e->max_pages_per_slot = (cfg->max_seq_len + KV_PAGE - 1) / KV_PAGE;
     e->n_pages = e->max_pages_per_slot * cfg->max_slots;
+    if (cfg->kv_pool_bytes != 0) {
+        const int64_t pages = cfg->kv_pool_bytes / static_cast<int64_t>(page_bytes_all_layers(e));
+        if (cfg->kv_pool_bytes < 0 || pages < 1 || pages > INT32_MAX) {
+            set_error("kv_pool_bytes %lld: 0 (max_slots * max_pages per slot) or at least one page of %zu bytes",
+                      static_cast<long long>(cfg->kv_pool_bytes), page_bytes_all_layers(e));
+            delete e;
+            return -1;
+        }
+        e->n_pages = static_cast<int>(pages);
+    }
+    static std::atomic<uint64_t> next_id{1};
+    e->id = next_id++;
     for (int p = e->n_pages - 1; p >= 0; --p) e->free_pages.push_back(p);
     e->page_refs.assign(e->n_pages, 0);
     e->slot_pages.resize(cfg->max_slots);
@@ -1273,7 +1389,8 @@ int vcb_finalize_weights(vcb_engine* e) {
         e->page_table.ensure(S * e->max_pages_per_slot, true) || e->tok_log.ensure(S * e->cfg.max_new_tokens * m.K, true) ||
         e->dbg_logits.ensure(R * m.K * m.V, true) || e->st.ensure(S, true) || e->gr.ensure(S, true) ||
         e->d_seqs.ensure(S, true) || e->pf_rec.ensure(S, true) || e->h_pf_rec.ensure(S) || e->sp_tab.ensure(S, true) ||
-        e->pf_src.ensure(S, true) || e->h_pf_src.ensure(S) ||
+        e->pf_src.ensure(S, true) || e->h_pf_src.ensure(S) || e->swap_pages.ensure(e->max_pages_per_slot, true) ||
+        e->grow_stage.ensure(static_cast<size_t>(vcb_engine::GROW_RING) * vcb_engine::GROW_INTS) ||
         e->all_rows.ensure(5 * e->all_rows_cap, true) || e->h_stage.ensure(e->h_stage_ints) || e->d_fork.ensure(S, true) ||
         e->d_pools.ensure(2 * m.L, true))
         return -1;
@@ -1286,6 +1403,8 @@ int vcb_finalize_weights(vcb_engine* e) {
         VCB_CUDA_OK(cudaMemcpy(e->d_pools, pools.data(), pools.size() * sizeof(uint8_t*), cudaMemcpyHostToDevice));
     }
     if (!e->stage_ev && e->stage_ev.create(cudaEventDisableTiming)) return -1;
+    for (Event& ev : e->grow_ev)
+        if (!ev && ev.create(cudaEventDisableTiming)) return -1;
     const int bp[4] = {16, 32, 64, 128};
     for (int i = 0; i < 4; ++i) {
         if (make_tmap_bf16_2d(&e->tm_act_d[i], e->act_d, 2 * bp[i], m.d, m.d, 2 * bp[i]) ||
@@ -1349,7 +1468,8 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
             // one prefill per group; the members share the leader's full prompt pages
             const int shared = static_cast<int>(total / KV_PAGE);
             rows_needed += static_cast<size_t>(total);
-            pages_needed += e->max_pages_per_slot + static_cast<size_t>(P.n_copies - 1) * (e->max_pages_per_slot - shared);
+            pages_needed += P.n_copies == 1 ? grown_pages(e, static_cast<int>(total) - 1)
+                                             : e->max_pages_per_slot + static_cast<size_t>(P.n_copies - 1) * (e->max_pages_per_slot - shared);
         }
         if (static_cast<size_t>(n) > e->free_groups.size()) {
             set_error("no free group");
@@ -1409,7 +1529,9 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
             e->slot_final[slot] = 0;
             auto& pg = e->slot_pages[slot];
             pg.clear();
-            for (int p = 0; p < e->max_pages_per_slot; ++p) {
+            // a one-copy prompt takes the pages of its positions (vcb_decode_step grows them); a group its full reservation
+            const int n_pg = P.n_copies == 1 ? grown_pages(e, total - 1) : e->max_pages_per_slot;
+            for (int p = 0; p < n_pg; ++p) {
                 if (c > 0 && p < shared) {
                     pg.push_back(e->slot_pages[P.slot][p]);
                 } else {
@@ -1449,8 +1571,7 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
     for (size_t i = 0; i < sst.size(); ++i) {
         VCB_CUDA_OK(cudaMemcpy(e->st + sst_slot[i], &sst[i], sizeof(SlotState), cudaMemcpyHostToDevice));
         VCB_CUDA_OK(cudaMemcpy(e->page_table + static_cast<size_t>(sst_slot[i]) * e->max_pages_per_slot,
-                               e->slot_pages[sst_slot[i]].data(), e->max_pages_per_slot * sizeof(int),
-                               cudaMemcpyHostToDevice));
+                               page_row(e, sst_slot[i]).data(), e->max_pages_per_slot * sizeof(int), cudaMemcpyHostToDevice));
     }
     for (size_t i = 0; i < gst.size(); ++i)
         VCB_CUDA_OK(cudaMemcpy(e->gr + gst_id[i], &gst[i], sizeof(GroupState), cudaMemcpyHostToDevice));
@@ -1537,9 +1658,11 @@ int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float*
         return -1;
     }
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
-    if (check_slots(e, slots, n) || noise_required(e, slots, n, exp_noise_dev) || sampling_required(e, slots, n, sp) ||
-        upload_slots(e, slots, n, st))
+    if (check_slots(e, slots, n) || noise_required(e, slots, n, exp_noise_dev) || sampling_required(e, slots, n, sp))
         return -1;
+    static thread_local std::vector<std::pair<int, int>> grow;
+    if (const int rc = plan_growth(e, slots, n, grow)) return rc;
+    if (upload_slots(e, slots, n, st) || apply_growth(e, grow, st)) return -1;
     const bool fold = e->opt_fold && !e->opt_simt;
     Pass p = step_pass(e, n, fold);
     {
@@ -1766,6 +1889,147 @@ int vcb_release(vcb_engine* e, int32_t slot, int32_t n_copies) {
         e->free_groups.push_back(gid);
         e->group_sp[gid] = 0;
     }
+    return 0;
+}
+
+}  // extern "C"
+
+namespace {
+
+// the swap staging region for n pages, and the page list on the device (blocking copy)
+int swap_prepare(vcb_engine* e, const std::vector<int>& pages, size_t words) {
+    if (e->swap_stage.size() < words && e->swap_stage.alloc(words)) return -1;
+    if (!pages.empty())
+        VCB_CUDA_OK(cudaMemcpy(e->swap_pages, pages.data(), pages.size() * sizeof(int), cudaMemcpyHostToDevice));
+    return 0;
+}
+
+template <bool Gather>
+int swap_copy_kernel(vcb_engine* e, int n_pages, cudaStream_t st) {
+    if (n_pages == 0) return 0;
+    const long long page_words = static_cast<long long>(e->m.H) * kv_slab_bytes(e->kv_dtype, e->m.hd) / 16;
+    const long long total = page_words * n_pages * 2 * e->m.L;
+    const int grid = static_cast<int>(std::min<long long>((total + 255) / 256, 4LL * e->num_sms));
+    ProfScope ps(e, PC_MISC, st);
+    kv_pages_copy_kernel<Gather><<<grid, 256, 0, st>>>(e->d_pools, 2 * e->m.L, page_words, e->swap_pages, n_pages, e->swap_stage);
+    VCB_CUDA_OK(cudaGetLastError());
+    LAUNCH_COUNT(e);
+    return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int vcb_swap_out(vcb_engine* e, int32_t slot, vcb_snapshot** out, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!e || !e->finalized || !out || slot < 0 || slot >= e->cfg.max_slots || e->slot_group[slot] < 0) {
+        set_error("vcb_swap_out: slot %d is not open (or a null argument)", slot);
+        return -1;
+    }
+    if (e->slot_copies[slot] != 1) {
+        set_error("vcb_swap_out: slot %d belongs to a best-of-N group of %d: only one-copy utterances swap", slot,
+                  e->slot_copies[slot]);
+        return -1;
+    }
+    VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
+    if (sync_or_report(e, cudaStreamSynchronize(st), "vcb_swap_out")) return -1;
+    const ModelDims& m = e->m;
+    const int gid = e->slot_group[slot];
+    auto snap = std::make_unique<vcb_snapshot>();
+    VCB_CUDA_OK(cudaMemcpy(&snap->S, e->st + slot, sizeof(SlotState), cudaMemcpyDeviceToHost));
+    VCB_CUDA_OK(cudaMemcpy(&snap->G, e->gr + gid, sizeof(GroupState), cudaMemcpyDeviceToHost));
+    snap->has_sp = e->group_sp[gid];
+    if (snap->has_sp) VCB_CUDA_OK(cudaMemcpy(&snap->sp, e->sp_tab + gid, sizeof(SamplingParams), cudaMemcpyDeviceToHost));
+    snap->engine_id = e->id;
+    snap->rng = e->slot_rng[slot];
+    snap->edit = e->slot_edit[slot];
+    snap->final_frames = e->slot_final[slot];
+    const auto& pg = e->slot_pages[slot];
+    snap->n_pages = std::min(static_cast<int>(pg.size()), (snap->S.seq_len + KV_PAGE - 1) / KV_PAGE);
+    const size_t page_bytes = page_bytes_all_layers(e);
+    const size_t n_tok = static_cast<size_t>(snap->S.n_steps) * m.K;
+    if (snap->kv.alloc(snap->n_pages * page_bytes) || snap->tok.alloc(n_tok) || snap->rows.alloc(2 * m.d) ||
+        swap_prepare(e, std::vector<int>(pg.begin(), pg.begin() + snap->n_pages), snap->n_pages * page_bytes / 16) ||
+        swap_copy_kernel<true>(e, snap->n_pages, st))
+        return -1;
+    VCB_CUDA_OK(cudaMemcpyAsync(snap->kv, e->swap_stage, snap->n_pages * page_bytes, cudaMemcpyDeviceToHost, st));
+    VCB_CUDA_OK(cudaMemcpyAsync(snap->tok, e->tok_log + static_cast<size_t>(slot) * e->cfg.max_new_tokens * m.K,
+                                n_tok * sizeof(int), cudaMemcpyDeviceToHost, st));
+    VCB_CUDA_OK(cudaMemcpyAsync(snap->rows, e->x_slot + static_cast<size_t>(slot) * m.d, m.d * sizeof(float),
+                                cudaMemcpyDeviceToHost, st));
+    VCB_CUDA_OK(cudaMemcpyAsync(snap->rows + m.d, e->h_slot + static_cast<size_t>(slot) * m.d, m.d * sizeof(float),
+                                cudaMemcpyDeviceToHost, st));
+    if (sync_or_report(e, cudaStreamSynchronize(st), "vcb_swap_out")) return -1;
+    if (vcb_release(e, slot, 1)) return -1;
+    *out = snap.release();
+    return 0;
+}
+
+int vcb_swap_in(vcb_engine* e, const vcb_snapshot* snap, int32_t slot, void* stream) {
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!e || !e->finalized || !snap || snap->engine_id != e->id) {
+        set_error("vcb_swap_in: not a snapshot of this engine (or a null argument)");
+        return -1;
+    }
+    if (slot < 0 || slot >= e->cfg.max_slots || e->slot_group[slot] >= 0) {
+        set_error("vcb_swap_in: slot %d is not a free slot of this engine", slot);
+        return -1;
+    }
+    if (e->free_groups.empty() || static_cast<size_t>(snap->n_pages) > e->free_pages.size()) {
+        set_error("vcb_swap_in: needs a free group and %d KV pages (%zu free)", snap->n_pages, e->free_pages.size());
+        return -1;
+    }
+    const ModelDims& m = e->m;
+    const size_t page_bytes = page_bytes_all_layers(e);
+    VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
+    if (sync_or_report(e, cudaStreamSynchronize(st), "vcb_swap_in")) return -1;
+    if (swap_prepare(e, {}, snap->n_pages * page_bytes / 16)) return -1;
+    // nothing can fail for want of resources from here on: take the group and the pages
+    const int gid = e->free_groups.back();
+    e->free_groups.pop_back();
+    auto& pg = e->slot_pages[slot];
+    pg.clear();
+    for (int p = 0; p < snap->n_pages; ++p) {
+        pg.push_back(e->free_pages.back());
+        e->free_pages.pop_back();
+        ++e->page_refs[pg.back()];
+    }
+    SlotState S = snap->S;
+    S.group = gid;
+    S.member = 0;
+    GroupState G = snap->G;
+    G.first_slot = slot;
+    e->slot_group[slot] = gid;
+    e->slot_rng[slot] = snap->rng;
+    e->slot_edit[slot] = snap->edit;
+    e->slot_copies[slot] = 1;
+    e->slot_shared[slot] = 0;
+    e->slot_final[slot] = snap->final_frames;
+    e->h_seq_len[slot] = S.seq_len;
+    e->group_sp[gid] = snap->has_sp;
+    e->last_slots.clear();
+    if (swap_prepare(e, pg, 0)) return -1;
+    VCB_CUDA_OK(cudaMemcpy(e->page_table + static_cast<size_t>(slot) * e->max_pages_per_slot, page_row(e, slot).data(),
+                           e->max_pages_per_slot * sizeof(int), cudaMemcpyHostToDevice));
+    VCB_CUDA_OK(cudaMemcpy(e->st + slot, &S, sizeof(SlotState), cudaMemcpyHostToDevice));
+    VCB_CUDA_OK(cudaMemcpy(e->gr + gid, &G, sizeof(GroupState), cudaMemcpyHostToDevice));
+    if (snap->has_sp) VCB_CUDA_OK(cudaMemcpy(e->sp_tab + gid, &snap->sp, sizeof(SamplingParams), cudaMemcpyHostToDevice));
+    VCB_CUDA_OK(cudaMemcpyAsync(e->swap_stage, snap->kv, snap->n_pages * page_bytes, cudaMemcpyHostToDevice, st));
+    if (swap_copy_kernel<false>(e, snap->n_pages, st)) return -1;
+    VCB_CUDA_OK(cudaMemcpyAsync(e->tok_log + static_cast<size_t>(slot) * e->cfg.max_new_tokens * m.K, snap->tok,
+                                static_cast<size_t>(snap->S.n_steps) * m.K * sizeof(int), cudaMemcpyHostToDevice, st));
+    VCB_CUDA_OK(cudaMemcpyAsync(e->x_slot + static_cast<size_t>(slot) * m.d, snap->rows, m.d * sizeof(float),
+                                cudaMemcpyHostToDevice, st));
+    VCB_CUDA_OK(cudaMemcpyAsync(e->h_slot + static_cast<size_t>(slot) * m.d, snap->rows + m.d, m.d * sizeof(float),
+                                cudaMemcpyHostToDevice, st));
+    return sync_or_report(e, cudaStreamSynchronize(st), "vcb_swap_in");
+}
+
+int32_t vcb_snapshot_pages(const vcb_snapshot* snap) { return snap ? snap->n_pages : -1; }
+
+int vcb_snapshot_free(vcb_snapshot* snap) {
+    delete snap;
     return 0;
 }
 
@@ -2267,6 +2531,10 @@ int64_t vcb_counter(vcb_engine* e, const char* name) {
     if (!strcmp(name, "mega_grid")) return e->mega_grid;
     if (!strcmp(name, "poll_frames")) return e->n_poll_frames;
     if (!strcmp(name, "kv_pages_free")) return static_cast<int64_t>(e->free_pages.size());
+    if (!strcmp(name, "kv_pages_total")) return e->n_pages;
+    if (!strcmp(name, "kv_pages_needed")) return e->n_pages_needed;
+    if (!strcmp(name, "kv_page_bytes")) return static_cast<int64_t>(page_bytes_all_layers(e));
+    if (!strcmp(name, "swap_stage_bytes")) return static_cast<int64_t>(e->swap_stage.size() * sizeof(uint4));
     if (!strcmp(name, "prefill_rows")) return e->n_prefill_rows;
     if (!strcmp(name, "weight_bytes")) {         // packed GEMM operands (+ int8 scales) and the int8 prefill scratch
         int64_t b = static_cast<int64_t>(e->w8_wide.size()) * 2;

@@ -162,6 +162,26 @@ __global__ void fork_group_kernel(uint8_t* const* __restrict__ pools /*[n_pools]
     }
 }
 
+// Swap of one utterance's KV pages (vcb_swap_out / vcb_swap_in): the page slabs of every pool (each layer's K, then each
+// layer's V) as one contiguous staging region [pool][page i][page_words], gathered from (Gather) or scattered to (!Gather)
+// the pool pages pages[i].  Whole 16-byte words: a page is H slabs, and every slab size is a multiple of 16 bytes.
+template <bool Gather>
+__global__ void __launch_bounds__(256)
+kv_pages_copy_kernel(uint8_t* const* __restrict__ pools /*[n_pools]*/, int n_pools, long long page_words,
+                     const int* __restrict__ pages, int n_pages, uint4* __restrict__ stage) {
+    const long long per_pool = page_words * n_pages, total = per_pool * n_pools;
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+         i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const long long pool = i / per_pool, r = i % per_pool;
+        uint4* pg = reinterpret_cast<uint4*>(pools[pool]) + static_cast<long long>(pages[r / page_words]) * page_words +
+                    r % page_words;
+        if (Gather)
+            stage[i] = *pg;
+        else
+            *pg = stage[i];
+    }
+}
+
 // The fp8 KV quantizer of the QKV epilogues alone (vcb_debug_kv_quantize): one CTA of hd threads per row
 __global__ void kv_quantize_kernel(const float* __restrict__ x, int hd, uint8_t* __restrict__ bytes, float* __restrict__ scales) {
     __shared__ float red[4];

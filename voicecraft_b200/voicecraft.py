@@ -160,7 +160,8 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         # engine configuration (see configure_engine)
         self._eng = None
         self._eng_key = None
-        self._eng_opts = dict(max_slots=8, max_seq_len=2048, max_new_tokens=4096, kv_dtype="bf16", weight_dtype="bf16")
+        self._eng_opts = dict(max_slots=8, max_seq_len=2048, max_new_tokens=4096, kv_dtype="bf16", weight_dtype="bf16",
+                              kv_pool_gb=None)
         self.noise_fn = None          # optional: callable(shape, device) -> fp32 Exp(1) tensor on `device`
         self.poll_every = 4           # inference_tts*: poll the done flag every N steps (device generator only)
         self._sessions = {}           # first slot -> slot list of every group held by a call, session or batcher (the engine
@@ -184,7 +185,10 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     def configure_engine(self, **opts):
         """max_slots, max_seq_len, max_new_tokens, kv_dtype ('bf16' default | 'fp32' | 'fp8': e4m3 with a power-of-two
         scale per token and head, half the cache bytes of bf16; INTEGRATION.md), weight_dtype ('bf16' default | 'int8': the
-        GEMM weights as int8 with a power-of-two scale per output feature, half the weight bytes; INTEGRATION.md).
+        GEMM weights as int8 with a power-of-two scale per output feature, half the weight bytes; INTEGRATION.md),
+        kv_pool_gb (None default: every slot can reach max_seq_len; a number: a KV page pool of that many GB (1e9 bytes),
+        taken as utterances grow; the batcher and sessions swap utterances to host memory when it runs out;
+        INTEGRATION.md).
         Rebuilds lazily."""
         for k in opts:
             if k not in self._eng_opts:
@@ -193,6 +197,8 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
             raise ValueError(f"kv_dtype {opts['kv_dtype']!r}: one of {sorted(KV_DTYPES)}")
         if "weight_dtype" in opts and opts["weight_dtype"] not in WEIGHT_DTYPES:
             raise ValueError(f"weight_dtype {opts['weight_dtype']!r}: one of {sorted(WEIGHT_DTYPES)}")
+        if opts.get("kv_pool_gb") is not None and not opts["kv_pool_gb"] > 0:
+            raise ValueError(f"kv_pool_gb {opts['kv_pool_gb']!r}: None or a positive number of GB")
         self._eng_opts.update(opts)
         self._drop_engine()
 
@@ -279,7 +285,8 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
             empty_token=a.empty_token, eog=a.eog, audio_pad_token=a.audio_pad_token, eos=a.eos if a.eos > 0 else -1,
             encodec_sr=int(a.encodec_sr), max_n_spans=a.max_n_spans, max_slots=o["max_slots"],
             max_seq_len=o["max_seq_len"], max_new_tokens=o["max_new_tokens"],
-            kv_dtype=KV_DTYPES[o["kv_dtype"]], device=dev.index or 0, weight_dtype=WEIGHT_DTYPES[o["weight_dtype"]])
+            kv_dtype=KV_DTYPES[o["kv_dtype"]], device=dev.index or 0, weight_dtype=WEIGHT_DTYPES[o["weight_dtype"]],
+            kv_pool_bytes=0 if o["kv_pool_gb"] is None else int(o["kv_pool_gb"] * 1e9))
         h = C.c_void_p()
         _lib.check(lib.vcb_create(C.byref(cfg), C.byref(h)))
         try:
@@ -663,6 +670,15 @@ class _Prompt:
             self.y_tok, self.mask_rows, self.more_vals, self.non_mask = model._edit_prompt(self.y0, spans)
             cap, extra = x_len * 10, (K + 3) * (len(spans) + 1)
         self.need_seq = x_len + max(int(self.y_tok.shape[0]), cap + 1) + extra + 8
+        self.total = x_len + int(self.y_tok.shape[0])           # positions the prefill writes
+
+    def pages(self, n_copies, max_pages):
+        """KV pages vcb_prefill takes for it: a one-copy prompt its positions' pages in whole growth chunks, a best-of-N
+        group its full reservation"""
+        if n_copies == 1:
+            g = _lib.KV_GROW_PAGES
+            return min(max_pages, ((self.total + 63) // 64 + g - 1) // g * g)
+        return max_pages + (n_copies - 1) * (max_pages - self.total // 64)
 
     def fill(self, slot, n_copies, seed=None, offset=0, sp=None):
         """its vcb_prompt in slots slot .. slot+n_copies-1, sampling from the Philox stream of a torch CUDA generator at
@@ -1091,6 +1107,8 @@ class DecodeSession:
         `poll_every` steps; returns results() and closes the session"""
         try:
             self.sample()
+            if self.model._eng_opts["kv_pool_gb"] is not None and self.n_copies == 1 and not self._host_noise:
+                return self._run_pooled(poll_every)
             while True:
                 if self.steps % poll_every == 0 and self.all_done():
                     break
@@ -1098,6 +1116,43 @@ class DecodeSession:
             return self.results()
         finally:
             self.close()
+
+    def _run_pooled(self, poll_every):
+        """_run_many's loop under a KV budget (KvPoolPolicy), returning the results: a refused step swaps the youngest
+        utterance out; a finished one is read and leaves its slot and pages at once; swapped-out utterances come back,
+        oldest first, into the session's freed slots"""
+        pool = KvPoolPolicy(_EngineOps(self.eng, self.stream, self.sp), True, self.B)
+        free, done, results = set(), [False] * self.B, [None] * self.B
+        try:
+            while True:
+                out = {t[1] for t in pool.swapped}
+                for i, slot in pool.resume(free, sum(1 for i in range(self.B) if not done[i] and i not in out)):
+                    # a slot the session holds; self.slots may now list a slot twice (a finished utterance's, reused)
+                    # and miss a freed one, which is harmless: every open slot is listed, index 0 (the oldest) is never
+                    # a victim, so _release_slots still finds the session, and releasing a closed slot does nothing
+                    self.slots[i] = slot
+                out = {t[1] for t in pool.swapped}
+                live = [(i, self.slots[i], i, True) for i in range(self.B) if not done[i] and i not in out]
+                if not live:
+                    break
+                for _ in range(poll_every):
+                    live, gone = pool.step(live)
+                    free.update(slot for _, slot in gone)
+                    self.steps += 1
+                st = (_lib.vcb_status * len(live))()
+                _lib.check(self.lib.vcb_poll(self.eng, (C.c_int32 * len(live))(*[u[1] for u in live]), len(live), st,
+                                             self.stream))
+                _check_capacity(st)
+                for (i, slot, _, _), s in zip(live, st):
+                    if s.done:
+                        results[i] = self.prompts[i].result(self.model._read_rows(self.eng, slot, s.n_steps, self.stream), s)
+                        _lib.check(self.lib.vcb_release(self.eng, slot, 1))
+                        done[i] = True
+                        free.add(slot)
+        finally:
+            pool.close()
+            self.c_slots = (C.c_int32 * len(self.slots))(*self.slots)
+        return results
 
     def _run_single(self):
         """The loop of a single call; returns results().  The done flag is polled every model.poll_every steps: a finished
@@ -1173,6 +1228,137 @@ def place_groups(free, sizes, nxt):
     return new, nxt
 
 
+_TOO_SMALL = ("KV pool smaller than one utterance (kv_pool_gb; pages held by other open sessions or batchers of this model "
+              "count against it)")
+
+
+class KvPoolPolicy:
+    """How the batcher and sessions share a KV page pool (DESIGN.md section 7).  `ops` is the engine (_EngineOps; the tests pass a fake):
+    free_pages(), step(slots) -> 0 or VCB_ERR_KV_FULL, swap_out(slot) -> snapshot, swap_in(snapshot, slot),
+    snapshot_pages(snapshot), free(snapshot).  An utterance is (key, slot, age, single): age orders admissions (oldest
+    first), single marks a one-copy utterance (a best-of-N group keeps its full reservation and never swaps).
+      admission  strict FIFO; while anything is swapped out, nothing new; otherwise a ticket needs its prompt pages plus one
+                 growth chunk per active slot free (budget only: the default pool always covers max_slots full slots)
+      victim     a refused step swaps out the youngest single utterance it lists and is retried without it
+      resume     swapped-out utterances come back, oldest first, when their pages plus a chunk per active slot are free
+      bound      at most max_swapped utterances are out at once
+    The pages it counts are the engine's free pages: every open session and batcher of the model shares that engine, so
+    pages another one holds count against this one's pool."""
+
+    def __init__(self, ops, budget, max_swapped, chunk=_lib.KV_GROW_PAGES):
+        self.ops, self.budget, self.max_swapped, self.chunk = ops, bool(budget), int(max_swapped), int(chunk)
+        self.swapped = []                 # [(age, key, snapshot)], oldest first
+        self.swap_outs = self.swap_ins = 0
+
+    def admit_count(self, needs, n_active):
+        """how many of the queued tickets `needs` [(pages, slots)] (FIFO order) the pool takes now next to n_active slots"""
+        if self.swapped:
+            return 0
+        if not self.budget:
+            return len(needs)
+        free, k = self.ops.free_pages(), 0
+        for pages, n in needs:
+            if free < pages + self.chunk * n_active:
+                if n_active == 0:
+                    raise _lib.VcbError(f"{_TOO_SMALL}: its prompt needs {pages} pages, {free} are free")
+                break
+            free, n_active, k = free - pages, n_active + n, k + 1
+        return k
+
+    def resume(self, free_slots, n_active):
+        """swap utterances back in, oldest first, each into the lowest slot of the set free_slots; [(key, slot)]"""
+        back = []
+        while self.swapped and free_slots:
+            age, key, snap = self.swapped[0]
+            pages, free = self.ops.snapshot_pages(snap), self.ops.free_pages()
+            if free < pages + self.chunk * (n_active + 1) and not (n_active == 0 and free >= pages):
+                if n_active == 0:
+                    raise _lib.VcbError(f"{_TOO_SMALL}: it holds {pages} pages, {free} are free")
+                break
+            slot = min(free_slots)
+            self.ops.swap_in(snap, slot)
+            free_slots.discard(slot)
+            self.ops.free(snap)
+            self.swapped.pop(0)
+            self.swap_ins += 1
+            n_active += 1
+            back.append((key, slot))
+        return back
+
+    def step(self, live, leaving=False):
+        """one decode step of the utterances `live` [(key, slot, age, single)]; a refused step swaps out the youngest single
+        one and is retried.  Returns (the utterances that stepped, [(key, slot)] swapped out).
+        leaving: utterances outside `live` hold pages they give back before the caller's next round (finished ones that are
+        not released yet).  A refused step that no victim can resolve then does not raise: it returns (None, swapped out
+        so far) and the caller steps no further this round."""
+        out = []
+        while live:
+            if self.ops.step([u[1] for u in live]) == 0:
+                return live, out
+            singles = [u for u in live if u[3]]
+            if len(live) == 1 or not singles:
+                if leaving:
+                    return None, out
+                raise _lib.VcbError(f"{_TOO_SMALL}: a step of it alone does not fit")
+            if len(self.swapped) >= self.max_swapped:
+                raise _lib.VcbError(f"KV pool too small: {len(self.swapped)} utterances are swapped out already")
+            victim = max(singles, key=lambda u: u[2])
+            snap = self.ops.swap_out(victim[1])
+            self.swapped.append((victim[2], victim[0], snap))
+            self.swapped.sort(key=lambda t: t[0])
+            self.swap_outs += 1
+            live = [u for u in live if u is not victim]
+            out.append((victim[0], victim[1]))
+        return live, out
+
+    def drop(self, key):
+        """forget a swapped-out utterance (a cancelled ticket): frees its snapshot; False if it is not swapped out"""
+        for i, (_, k, snap) in enumerate(self.swapped):
+            if k is key:
+                self.ops.free(snap)
+                del self.swapped[i]
+                return True
+        return False
+
+    def close(self):
+        """frees every snapshot still held"""
+        for _, _, snap in self.swapped:
+            self.ops.free(snap)
+        self.swapped = []
+
+
+class _EngineOps:
+    """KvPoolPolicy's view of an engine: decode steps with device noise and the sampling parameters `sp` (None: each
+    group's own)"""
+
+    def __init__(self, eng, stream, sp=None):
+        self.eng, self.stream, self.lib = eng, stream, _lib.load()
+        self.sp = None if sp is None else C.byref(sp)
+
+    def free_pages(self):
+        return self.lib.vcb_counter(self.eng, b"kv_pages_free")
+
+    def step(self, slots):
+        rc = self.lib.vcb_decode_step(self.eng, (C.c_int32 * len(slots))(*slots), len(slots), None, self.sp, self.stream)
+        if rc != _lib.VCB_ERR_KV_FULL:
+            _lib.check(rc)
+        return rc
+
+    def swap_out(self, slot):
+        snap = C.c_void_p()
+        _lib.check(self.lib.vcb_swap_out(self.eng, slot, C.byref(snap), self.stream))
+        return snap
+
+    def swap_in(self, snap, slot):
+        _lib.check(self.lib.vcb_swap_in(self.eng, snap, slot, self.stream))
+
+    def snapshot_pages(self, snap):
+        return self.lib.vcb_snapshot_pages(snap)
+
+    def free(self, snap):
+        self.lib.vcb_snapshot_free(snap)
+
+
 class ContinuousBatcher:
     """Continuous batching of independent TTS and speech-editing utterances (SURVEY.md section 8f, row f2).
 
@@ -1193,7 +1379,7 @@ class ContinuousBatcher:
         self.defaults = dict(top_k=top_k, top_p=top_p, temperature=temperature, stop_repetition=stop_repetition,
                              silence_tokens=silence_tokens)
         self.queue = []
-        self.stats = dict(steps=0, prefills=0, max_active=0)
+        self.stats = dict(steps=0, prefills=0, max_active=0, swap_outs=0, swap_ins=0)
         self.results, self.errors = [], {}
         self._live = None                  # the running stream()'s state
 
@@ -1285,25 +1471,39 @@ class ContinuousBatcher:
         sizes = [j[2] for j in jobs]
         n_slots = min(self.B, max(1, sum(sizes)))
         eng, slots = m._take_slots(n_slots, max([j[0].need_seq for j in jobs], default=0))
+        max_pages = (m._eng_opts["max_seq_len"] + 63) // 64
         free, active, results, nxt = set(slots), {}, [None] * len(jobs), 0     # active: first slot -> ticket
+        pool = None
         try:
             with torch.cuda.device(dev):
                 stream = torch.cuda.current_stream().cuda_stream
+                pool = KvPoolPolicy(_EngineOps(eng, stream), m._eng_opts["kv_pool_gb"] is not None, self.B)
                 steps = 0
-                while nxt < len(jobs) or active:
-                    # ---- refill free slot runs from the queue, strictly in ticket order
-                    new, nxt = place_groups(free, sizes, nxt)
+                while nxt < len(jobs) or active or pool.swapped:
+                    n_active = sum(sizes[ji] for ji in active.values())
+                    # ---- swapped-out utterances come back first, then free slot runs take queued tickets in order
+                    for ji, slot in pool.resume(free, n_active):
+                        active[slot] = ji
+                    n_active = sum(sizes[ji] for ji in active.values())
+                    k = pool.admit_count([(jobs[t][0].pages(sizes[t], max_pages), sizes[t])
+                                          for t in range(nxt, min(len(jobs), nxt + len(free)))], n_active)
+                    new, nxt = place_groups(free, sizes[:nxt + k], nxt)
                     if new:
                         self._admit(eng, new, jobs, stream)
                         for slot, ji in new:
                             active[slot] = ji
-                    order = sorted(s + c for s, ji in active.items() for c in range(sizes[ji]))
-                    c_slots = (C.c_int32 * len(order))(*order)
-                    self.stats["max_active"] = max(self.stats["max_active"], len(order))
-                    # ---- decode steps for everyone until the next poll
+                    live = [(ji, s + c, ji, sizes[ji] == 1) for s, ji in active.items() for c in range(sizes[ji])]
+                    live.sort(key=lambda u: u[1])
+                    self.stats["max_active"] = max(self.stats["max_active"], len(live))
+                    # ---- decode steps for everyone until the next poll; a refused step swaps the youngest out
                     for _ in range(self.poll_every):
-                        _lib.check(lib.vcb_decode_step(eng, c_slots, len(order), None, None, stream))
+                        live, out = pool.step(live)
+                        for ji, slot in out:
+                            del active[slot]
+                            free.add(slot)
                         steps += 1
+                    order = [u[1] for u in live]
+                    c_slots = (C.c_int32 * len(order))(*order)
                     status = (_lib.vcb_status * len(order))()
                     _lib.check(lib.vcb_poll(eng, c_slots, len(order), status, stream))
                     _check_capacity(status)
@@ -1318,6 +1518,10 @@ class ContinuousBatcher:
                             free.update(range(slot, slot + sizes[ji]))
                 self.stats["steps"] = steps
         finally:
+            if pool is not None:
+                pool.close()
+                self.stats["swap_outs"] += pool.swap_outs
+                self.stats["swap_ins"] += pool.swap_ins
             m._release_slots(slots, [s + c for s, ji in active.items() for c in range(sizes[ji])])
             self.queue = []
         return results
@@ -1354,16 +1558,24 @@ class BatcherStream(_AudioStream):
         refused = {t for t, j in enumerate(jobs) if j[2] > 1}
         st = SimpleNamespace(cb=cb, eng=eng, slots=slots, max_seq=m._eng_opts["max_seq_len"], jobs=jobs,
                              cancelled=set(refused), ended=set(refused), refused=sorted(refused), tok=tokenizer,
-                             chunk_frames=int(chunk_frames), dev=m.mask_embedding.device, sample_rate=sample_rate)
+                             chunk_frames=int(chunk_frames), dev=m.mask_embedding.device, sample_rate=sample_rate,
+                             pool=None)
         cb.results, cb._live = [None] * len(jobs), st
         cb.errors = {t: f"best_of={jobs[t][2]}: stream() serves only best_of=1 tickets" for t in refused}
-        self._start(st, cb.B)
+        # a codec stream id belongs to a ticket from its admission to its end: at most max_concurrency are active and, under
+        # a KV budget, at most as many more are swapped out
+        self._start(st, 2 * cb.B if m._eng_opts["kv_pool_gb"] is not None else cb.B)
 
     @staticmethod
     def _finish(st):
         cb = st.cb
         if cb._live is not st:
             return
+        if st.pool is not None:
+            st.pool.close()
+            cb.stats["swap_outs"] += st.pool.swap_outs
+            cb.stats["swap_ins"] += st.pool.swap_ins
+            st.pool = None
         cb.model._release_slots(st.slots)    # every slot: releasing one that is not open does nothing
         _AudioStream._close_codec(st)
         cb._live, cb.queue = None, []
@@ -1371,12 +1583,14 @@ class BatcherStream(_AudioStream):
     @staticmethod
     @torch.no_grad()
     def _run(st):
-        cb, m, lib = st.cb, st.cb.model, _lib.load()
-        base = st.slots[0]
-        free, active, nxt = list(st.slots), {}, 0        # active: slot -> _Utterance
+        cb, m = st.cb, st.cb.model
+        max_pages = (m._eng_opts["max_seq_len"] + 63) // 64
+        free, active, nxt = set(st.slots), {}, 0         # active: slot -> _Utterance
+        ids = list(range(st.codec.max_streams))          # free codec stream ids
         try:
             with torch.cuda.device(st.dev):
                 stream = torch.cuda.current_stream().cuda_stream
+                pool = st.pool = KvPoolPolicy(_EngineOps(st.eng, stream), m._eng_opts["kv_pool_gb"] is not None, cb.B)
                 push = st.push = _PushStep(m, st.eng, stream, st.tok, st.codec, st.cstream, st.chunk_frames, cb.poll_every,
                                            strict=False)
                 empty = torch.zeros(1, st.tok.channels, 0, device=st.dev)
@@ -1390,30 +1604,52 @@ class BatcherStream(_AudioStream):
                                 cb.results[r.ticket] = cb._result(st.eng, slot, r.status, st.jobs[r.ticket], stream)
                             m._release_slots(st.slots, [slot], keep_held=True)
                             del active[slot]
-                            free.append(slot)
-                    # ---- free slots take the next queued tickets; each slot owns codec stream id slot - base
+                            free.add(slot)
+                            ids.append(r.cid)
+                    for _, r, _ in list(pool.swapped):       # a cancelled ticket that is swapped out: its snapshot goes
+                        if r.ticket in st.cancelled and pool.drop(r):
+                            ids.append(r.cid)
+                    # ---- swapped-out tickets come back first (with their codec stream and state), then free slots take
+                    # the next queued tickets, each with a codec stream id of its own
+                    for r, slot in pool.resume(free, len(active)):
+                        r.slot = slot
+                        active[slot] = r
+                    cands, t = [], nxt
+                    while len(cands) < len(free) and t < len(st.jobs):
+                        if t not in st.cancelled:
+                            cands.append(t)
+                        t += 1
+                    k = pool.admit_count([(st.jobs[c][0].pages(1, max_pages), 1) for c in cands], len(active))
+                    nxt = t if k == len(cands) else cands[k]
                     new = []
-                    while free and nxt < len(st.jobs):
-                        if nxt not in st.cancelled:
-                            new.append((free.pop(0), nxt))
-                        nxt += 1
+                    for c in cands[:k]:
+                        slot = min(free)
+                        free.discard(slot)
+                        new.append((slot, c))
                     if new:
                         cb._admit(st.eng, new, st.jobs, stream)
-                        st.codec.reset([slot - base for slot, _ in new])
-                        for slot, t in new:
-                            active[slot] = _Utterance(slot, slot - base, f"ticket {t}", ticket=t, src=st.jobs[t][0].source())
+                        cids = [ids.pop(0) for _ in new]
+                        st.codec.reset(cids)
+                        for (slot, t), cid in zip(new, cids):
+                            active[slot] = _Utterance(slot, cid, f"ticket {t}", ticket=t, src=st.jobs[t][0].source())
                     if not active:
                         break
                     live = [active[s] for s in sorted(active)]
                     cb.stats["max_active"] = max(cb.stats["max_active"], len(live))
 
                     def advance(status):
-                        go = [r.slot for r, s in zip(live, status) if not s.done and not r.closed]
-                        if go:
-                            c_go = (C.c_int32 * len(go))(*go)
-                            for _ in range(cb.poll_every):
-                                _lib.check(lib.vcb_decode_step(st.eng, c_go, len(go), None, None, stream))
-                            cb.stats["steps"] += cb.poll_every
+                        go = [(r, r.slot, r.ticket, True) for r, s in zip(live, status) if not s.done and not r.closed]
+                        # finished tickets keep their slot and pages until the top of the next round releases them: while
+                        # any does, a step that swapping cannot fit waits for those pages instead of failing
+                        leaving = len(go) < len(live)
+                        for _ in range(cb.poll_every if go else 0):   # a refused step swaps the youngest ticket out
+                            go, out = pool.step(go, leaving)
+                            for r, slot in out:
+                                del active[slot]
+                                free.add(slot)
+                            if go is None:
+                                break
+                            cb.stats["steps"] += 1
                     status, out, failed = push(live, advance)
                     wavs = dict(out)
                     for r, s in zip(live, status):
