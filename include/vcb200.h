@@ -273,6 +273,21 @@ int vcb_debug_kv_quantize(const float* x_dev /*[rows][hd]*/, int32_t rows, int32
  * device. */
 int vcb_debug_kv_pages(vcb_engine* e, int32_t layer, int32_t slot, int32_t first_page, int32_t n_pages, void* k_host,
                        void* v_host);
+/* What the last vcb_prefill (its last chunk) / vcb_sample / vcb_decode_step left in one of its buffers, as fp32
+ * out_dev [rows][width] with hi/lo planes summed (the persistent kernel's tiled images included), rows <= that pass's rows:
+ *   "x"     the residual rows (vcb_sample: each listed slot's last prefill hidden state)       width d
+ *   "q"     the attention queries of the last QKV stage (not vcb_sample)                        width d
+ *   "opnd"  the operand of the next QKV or FFN1 GEMM: LN(x) unfolded, gamma * x folded         width d
+ *   "att"   the attention output                                                               width d
+ *   "ffn"   the FFN1 output after ReLU                                                         width 4 d
+ *   "heads" the first logit-head stage after GELU, codebooks side by side                      width K * audio_vocab/2
+ * With vcb_set_option(e, "stop_stage", s) the three calls run their first s stages only: stage 5 l + {0 QKV, 1 attention,
+ * 2 out-projection, 3 FFN1, 4 FFN2} of layer l, then 5 L (final LayerNorm + first head stage) and 5 L + 1 (second head
+ * stage), the persistent kernel's phases; an unfolded pass's LayerNorm belongs to the GEMM stage after it.  A stopped call
+ * launches nothing after stage s (no sampler, no last-row gather, no best-of-N fork) and leaves its slots mid-step: release
+ * them.  A prefill of several chunks runs all but its last chunk whole.  s = 0 (the default) runs everything, bit for bit
+ * as without the option.  Unknown names and rows above the last pass's are rejected.  Waits for the device. */
+int vcb_debug_stage_read(vcb_engine* e, const char* name, float* out_dev, int32_t rows);
 /* the decode pair "out-projection -> LN2 -> FFN1" on the per-kernel GEMM path (B <= 128 rows, d % 128 == 0, d <= 4096):
  *   x_new = x + a W1^T + b1;  y = LN(x_new; gamma, beta, eps 1e-5) W2^T + b2, ReLU'd when relu != 0 (EPI_ACT, hi + lo)
  * fold = 1: the residual GEMM emits gamma * x_new and per-tile row statistics, the second GEMM folds the LayerNorm into its
@@ -298,7 +313,8 @@ int vcb_gemm_launch_shape(int32_t N, int32_t K, int32_t B, int32_t splits, int32
                           int32_t* out /*[2]*/);
 /* debug timeline of the persistent decode-step kernel (first call enables it): [2 CTAs][n_phases][8 events] globaltimer ns */
 int vcb_debug_mega_timeline(vcb_engine* e, uint64_t* out_host, int32_t max_records, int32_t* n_phases);
-int vcb_set_option(vcb_engine* e, const char* name, int32_t value);   /* "gemm_simt", "pdl", "profile" */
+/* "gemm_simt", "pdl", "profile", "stop_stage" (0 .. 5 L + 2, see vcb_debug_stage_read) */
+int vcb_set_option(vcb_engine* e, const char* name, int32_t value);
 /* profile mode: summed device ms and launch counts per kernel class since the last read
  * (0 gemm, 1 attention, 2 layernorm/reduce, 3 bias/act/qkv finish, 4 sampler, 5 misc) */
 int vcb_profile_read(vcb_engine* e, double* ms_by_class, int64_t* count_by_class, int32_t n_classes);

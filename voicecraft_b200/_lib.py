@@ -87,6 +87,7 @@ PROTOTYPES = {
                                    [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32]),
     "vcb_debug_kv_quantize": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "vcb_debug_kv_pages": (C.c_int, [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 2),
+    "vcb_debug_stage_read": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int32]),
     "vcb_debug_fold_chain": (C.c_int, [C.c_void_p] * 8 + [C.c_int32] * 7 + [C.c_void_p] * 2),
     "vcb_timeline": (C.c_int, [C.c_int32, C.POINTER(C.c_uint64), C.c_int32, C.POINTER(C.c_int32)]),
     "vcb_bench_gemm": (C.c_int, [C.c_int32] * 8 + [C.POINTER(C.c_float)]),

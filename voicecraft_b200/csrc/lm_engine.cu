@@ -174,6 +174,17 @@ struct vcb_engine {
     DevBuf<__nv_bfloat16> mact_d, mact_d2, mact_f, mact_h;   // tiled + swizzled B-operand images
     DevBuf<int> mega_att_cnt;
     int64_t n_launches = 0;
+    // vcb_set_option("stop_stage"): the stages the next vcb_prefill (its last chunk) / vcb_sample / vcb_decode_step runs,
+    // numbered as the persistent kernel's phases (0: all of them)
+    int opt_stop = 0;
+    // the buffers of the last pass of those calls and how many of its stages ran (vcb_debug_stage_read)
+    struct StageView {
+        int rows = 0, bpad = 0, stages = 0;
+        bool fold = false, tiled = false;     // tiled: the persistent kernel's pre-swizzled B-operand images
+        float *x = nullptr, *q = nullptr;
+        const int* x_index = nullptr;         // row r of x is x[x_index[r]] (vcb_sample: h_slot by slot)
+        __nv_bfloat16 *act_d = nullptr, *act_d2 = nullptr, *act_f = nullptr, *act_h = nullptr;
+    } last;
     // profile mode: CUDA events around every launch, by kernel class
     struct ProfRec { int cls; Event a, b; };
     std::vector<ProfRec> prof;
@@ -420,7 +431,28 @@ struct Pass {
     Plane act_d, act_d2, act_f, act_h;        // LayerNorm / attention output, folded FFN1 input, FFN1 output, heads hidden
     float* att_ws = nullptr;
     int* att_cnt = nullptr;
+    int stop = 0;                             // stages to run (vcb_engine::opt_stop; 0: all)
 };
+
+// the pass has run its last stage once `n` stages have run
+bool stops_after(const Pass& p, int n) { return p.stop > 0 && n >= p.stop; }
+
+// records the pass's buffers for vcb_debug_stage_read: `stages` of them run unless the pass stops earlier
+void record_pass(vcb_engine* e, const Pass& p, int stages, bool tiled) {
+    vcb_engine::StageView& v = e->last;
+    v.rows = p.rows;
+    v.bpad = p.bpad;
+    v.stages = p.stop ? std::min(p.stop, stages) : stages;
+    v.fold = p.fold;
+    v.tiled = tiled;
+    v.x = p.x;
+    v.x_index = p.x_index;
+    v.q = p.q;
+    v.act_d = p.act_d.act;
+    v.act_d2 = p.act_d2.act;
+    v.act_f = p.act_f.act;
+    v.act_h = p.act_h.act;
+}
 
 // a pass over at most MAX_ROWS rows on the decode buffers (row tables left to the caller)
 Pass narrow_pass(vcb_engine* e, int rows, bool fold) {
@@ -640,19 +672,26 @@ int launch_ln(vcb_engine* e, const Pass& p, const float* g, const float* b, cuda
 //                out GEMM (+residual), LN2, FFN1 GEMM (+ReLU), FFN2 GEMM (+residual)
 //   fold = true  (decode): 5 launches per layer: LayerNorm is folded into the consuming GEMM's epilogue; the producing
 //                GEMM (or step_prep for layer 0) emits gamma*x as hi/lo rows plus per-tile row statistics.
+// Stage 5 l + {0 QKV, 1 attention, 2 out-projection, 3 FFN1, 4 FFN2}; an unfolded pass's LayerNorm belongs to the GEMM
+// stage after it.  With p.stop the layers end after that many stages.
 int forward_layers(vcb_engine* e, const Pass& p, cudaStream_t st) {
     const ModelDims& m = e->m;
     for (int l = 0; l < m.L; ++l) {
         const Layer& Ly = e->layers[l];
         const LayerEpilogues ep = layer_epilogues(e, l, p);
+        const int s = 5 * l;
         if (!p.fold && launch_ln(e, p, Ly.ln1_g, Ly.ln1_b, st)) return -1;
-        if (pass_gemm(e, p, Ly.qkv, p.act_d, ep.qkv, st, &Ly.out) || launch_attn(e, p, Ly, st) ||
-            pass_gemm(e, p, Ly.out, p.act_d, ep.out, st, &Ly.ff1))
-            return -1;
+        if (pass_gemm(e, p, Ly.qkv, p.act_d, ep.qkv, st, &Ly.out)) return -1;
+        if (stops_after(p, s + 1)) return 0;
+        if (launch_attn(e, p, Ly, st)) return -1;
+        if (stops_after(p, s + 2)) return 0;
+        if (pass_gemm(e, p, Ly.out, p.act_d, ep.out, st, &Ly.ff1)) return -1;
+        if (stops_after(p, s + 3)) return 0;
         if (!p.fold && launch_ln(e, p, Ly.ln2_g, Ly.ln2_b, st)) return -1;
-        if (pass_gemm(e, p, Ly.ff1, p.fold ? p.act_d2 : p.act_d, ep.ff1, st, &Ly.ff2) ||
-            pass_gemm(e, p, Ly.ff2, p.act_f, ep.ff2, st, l + 1 < m.L ? &e->layers[l + 1].qkv : &e->h1))
-            return -1;
+        if (pass_gemm(e, p, Ly.ff1, p.fold ? p.act_d2 : p.act_d, ep.ff1, st, &Ly.ff2)) return -1;
+        if (stops_after(p, s + 4)) return 0;
+        if (pass_gemm(e, p, Ly.ff2, p.act_f, ep.ff2, st, l + 1 < m.L ? &e->layers[l + 1].qkv : &e->h1)) return -1;
+        if (stops_after(p, s + 5)) return 0;
     }
     return 0;
 }
@@ -838,7 +877,9 @@ int mega_setup(vcb_engine* e) {
     return 0;
 }
 
-int mega_step(vcb_engine* e, int n, cudaStream_t st) {
+// one decode step of n rows through the persistent kernel; stop > 0: its first `stop` phases only (no phase waits on a
+// later one, and every role walks phases 0 .. nph-1)
+int mega_step(vcb_engine* e, int n, int stop, cudaStream_t st) {
     const ModelDims& m = e->m;
     const int bpad = bpad_for(n);
     MegaArgs a;
@@ -847,7 +888,7 @@ int mega_step(vcb_engine* e, int n, cudaStream_t st) {
     a.bbase[2] = e->mact_f;
     a.bbase[3] = e->mact_h;
     a.ph = e->d_mega_ph[bpad == 32];
-    a.nph = e->mega_nph;
+    a.nph = stop > 0 ? stop : e->mega_nph;
     a.nvalid = n;
     a.bpad = bpad;
     a.kv_fp32 = e->kv_dtype == KV_FP32;
@@ -1023,10 +1064,13 @@ int sampling_required(vcb_engine* e, const int32_t* slots, int n, const vcb_samp
 int sample_rows(vcb_engine* e, const Pass& p, const float* noise, const vcb_sampling* sp, cudaStream_t st) {
     const ModelDims& m = e->m;
     const int n = p.rows, bpad = p.bpad;
+    // stage 5L: final LayerNorm + first head stage, 5L + 1: second head stage (p.stop: the pass ends after it)
+    if (stops_after(p, 5 * m.L)) return 0;
     // fold: the last FFN2 epilogue already left lnf_gamma * x (hi/lo) and the row statistics for the heads GEMM
     if (!p.fold && launch_ln(e, p, e->lnf_g, e->lnf_b, st)) return -1;
     const int KH = m.K * m.Hh;
     if (pass_gemm(e, p, e->h1, p.act_d, heads_epilogue(e, p), st, &e->h2[0])) return -1;
+    if (stops_after(p, 5 * m.L + 1)) return 0;
     const int ldl = m.K * m.Vpad;
     if (!e->opt_simt) {
         // the K second-stage heads as ONE grouped launch (blockIdx.y = codebook)
@@ -1067,6 +1111,7 @@ int sample_rows(vcb_engine* e, const Pass& p, const float* noise, const vcb_samp
                 return -1;
         }
     }
+    if (stops_after(p, 5 * m.L + 2)) return 0;
     return launch_sampler(e, p, noise, sp, st);
 }
 
@@ -1606,12 +1651,15 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
         p.pos = t_pos + off;
         p.last = t_last + off;
         p.page = t_page + off;
+        p.stop = off + chunk >= total_rows ? e->opt_stop : 0;      // a stop ends the last chunk
         embed_rows_kernel<<<rows, 256, 0, st>>>(e->d_seqs, t_seq + off, t_pos + off, p.x, m.d, m.K, e->E_text,
                                                 e->d_E_audio, e->mask_emb, e->pe, e->alpha_t, e->alpha_a);
         VCB_CUDA_OK(cudaGetLastError());
         LAUNCH_COUNT(e);
         for (int r = 0; r < rows; ++r) p.max_ctx = std::max(p.max_ctx, r_pos[off + r] + 1);
+        record_pass(e, p, 5 * m.L, false);
         if (forward_layers(e, p, st)) return -1;
+        if (p.stop) break;
         {
             ProfScope ps(e, PC_LN, st);
             gather_rows_kernel<<<rows, 256, 0, st>>>(p.x, e->h_slot, p.last, m.d);
@@ -1620,7 +1668,7 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
         LAUNCH_COUNT(e);
     }
     e->n_prefill_rows += static_cast<int64_t>(total_rows);
-    if (!fork.empty()) {
+    if (!fork.empty() && !e->opt_stop) {
         const int page_words = m.H * kv_slab_bytes(e->kv_dtype, m.hd) / 16;
         const long long words = static_cast<long long>(fork.size()) * (2LL * m.L * page_words + m.d / 4);
         const int grid = static_cast<int>(std::min<long long>((words + 255) / 256, 4LL * e->num_sms));
@@ -1647,6 +1695,9 @@ int vcb_sample(vcb_engine* e, const int32_t* slots, int32_t n, const float* exp_
     Pass p = narrow_pass(e, n, false);
     p.x = e->h_slot;
     p.x_index = e->d_slots;
+    p.q = nullptr;
+    p.stop = e->opt_stop;
+    record_pass(e, p, 5 * e->m.L + 2, false);
     return sample_rows(e, p, exp_noise_dev, sp, st);
 }
 
@@ -1677,10 +1728,20 @@ int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float*
     }
     LAUNCH_COUNT(e);
     for (int i = 0; i < n; ++i) p.max_ctx = std::max(p.max_ctx, ++e->h_seq_len[slots[i]]);
+    p.stop = e->opt_stop;
     if (fold && e->mega_grid > 0 && n <= 32) {
-        if (mega_step(e, n, st)) return -1;
+        Pass v = p;                    // the buffers the persistent kernel works on (mega_build)
+        v.bpad = bpad_for(n);
+        v.act_d.act = e->mact_d;
+        v.act_d2.act = e->mact_d2;
+        v.act_f.act = e->mact_f;
+        v.act_h.act = e->mact_h;
+        record_pass(e, v, e->mega_nph, true);
+        if (mega_step(e, n, p.stop, st)) return -1;
+        if (p.stop) return 0;
         return launch_sampler(e, p, exp_noise_dev, sp, st);
     }
+    record_pass(e, p, 5 * e->m.L + 2, false);
     if (forward_layers(e, p, st)) return -1;
     return sample_rows(e, p, exp_noise_dev, sp, st);
 }
@@ -2068,6 +2129,27 @@ __global__ void join_hilo_kernel(const __nv_bfloat16* __restrict__ act, int ld, 
     out[static_cast<size_t>(r) * cols + c] = __bfloat162float(hi) + __bfloat162float(lo);
 }
 
+// vcb_debug_stage_read: fp32 rows (through `index` when given), or hi + lo of activation rows [2 * bpad][cols] -- or of the
+// persistent kernel's image of them: k-block c/64 is a tile of 2 * bpad rows of 64, its 16-byte chunks XORed with row % 8
+__global__ void stage_read_kernel(const float* __restrict__ f32, const int* __restrict__ index,
+                                  const __nv_bfloat16* __restrict__ act, int tiled, int bpad, int cols, float* __restrict__ out) {
+    const int r = blockIdx.y;
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= cols) return;
+    float v;
+    if (f32) {
+        v = f32[static_cast<size_t>(index ? index[r] : r) * cols + c];
+    } else if (!tiled) {
+        v = __bfloat162float(act[static_cast<size_t>(r) * cols + c]) + __bfloat162float(act[static_cast<size_t>(r + bpad) * cols + c]);
+    } else {
+        const int kk = c & 63;
+        const size_t t0 = static_cast<size_t>(c >> 6) * 2 * bpad;
+        auto at = [&](int row) { return __bfloat162float(act[(t0 + row) * 64 + ((((kk >> 3) ^ (row & 7)) << 3) | (kk & 7))]); };
+        v = at(r) + at(r + bpad);
+    }
+    out[static_cast<size_t>(r) * cols + c] = v;
+}
+
 }  // namespace
 
 extern "C" {
@@ -2302,6 +2384,47 @@ int vcb_debug_kv_pages(vcb_engine* e, int32_t layer, int32_t slot, int32_t first
     return 0;
 }
 
+int vcb_debug_stage_read(vcb_engine* e, const char* name, float* out_dev, int32_t rows) {
+    if (!e || !name || !out_dev) {
+        set_error("vcb_debug_stage_read: null argument");
+        return -1;
+    }
+    const vcb_engine::StageView& v = e->last;
+    const ModelDims& m = e->m;
+    if (rows < 1 || rows > v.rows) {
+        set_error("vcb_debug_stage_read: %d rows, the last pass had %d", rows, v.rows);
+        return -1;
+    }
+    // opnd: the operand of the next QKV / FFN1 GEMM.  A folded pass keeps FFN1's (gamma2 * x) in act_d2 from its
+    // out-projection through its FFN1, everything else in act_d; an unfolded pass's LayerNorms write act_d.
+    const int last = v.stages - 1;
+    const bool ffn1_operand = v.fold && last < 5 * m.L && (last % 5 == 2 || last % 5 == 3);
+    const float* f32 = nullptr;
+    const __nv_bfloat16* act = nullptr;
+    int cols = m.d;
+    if (!strcmp(name, "x")) f32 = v.x;
+    else if (!strcmp(name, "q")) f32 = v.q;
+    else if (!strcmp(name, "opnd")) act = ffn1_operand ? v.act_d2 : v.act_d;
+    else if (!strcmp(name, "att")) act = v.act_d;
+    else if (!strcmp(name, "ffn")) act = v.act_f, cols = m.F;
+    else if (!strcmp(name, "heads")) act = v.act_h, cols = m.K * m.Hh;
+    else {
+        set_error("vcb_debug_stage_read: unknown buffer %s (x, q, opnd, att, ffn, heads)", name);
+        return -1;
+    }
+    if (!f32 && !act) {
+        set_error("vcb_debug_stage_read: the last pass has no %s buffer", name);
+        return -1;
+    }
+    VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
+    if (sync_or_report(e, cudaDeviceSynchronize(), "vcb_debug_stage_read")) return -1;
+    stage_read_kernel<<<dim3((cols + 255) / 256, rows), 256>>>(f32, f32 ? v.x_index : nullptr, act, v.tiled, v.bpad, cols,
+                                                               out_dev);
+    VCB_CUDA_OK(cudaGetLastError());
+    VCB_CUDA_OK(cudaDeviceSynchronize());
+    return 0;
+}
+
 // Parity hook of the decode pair "out-projection -> LN2 -> FFN1" on the per-kernel GEMM path; see include/vcb200.h.
 int vcb_debug_fold_chain(const float* x_dev, const float* a_dev, const float* W1_dev, const float* b1_dev,
                          const float* gamma_dev, const float* beta_dev, const float* W2_dev, const float* b2_dev, int32_t B,
@@ -2516,6 +2639,13 @@ int vcb_set_option(vcb_engine* e, const char* name, int32_t value) {
     }
     else if (!strcmp(name, "profile")) e->opt_profile = value;
     else if (!strcmp(name, "pdl")) e->opt_pdl = value;
+    else if (!strcmp(name, "stop_stage")) {
+        if (value < 0 || value > 5 * e->m.L + 2) {
+            set_error("stop_stage %d: 0 (off) or a stage count in [1, %d]", value, 5 * e->m.L + 2);
+            return -1;
+        }
+        e->opt_stop = value;
+    }
     else {
         set_error("unknown option %s", name);
         return -1;
