@@ -44,8 +44,23 @@ int enc_decode(enc_engine* e, const int64_t* codes_dev, float* wav_dev, int32_t 
  * ResidualVectorQuantizer.encode).  Needs the "enc.*" weights: "enc.conv_in.weight", "enc.down{i}.res{j}.conv1.weight",
  * "enc.down{i}.conv.weight" (strided), "enc.lstm.*", "enc.conv_out.weight". */
 int enc_encode(enc_engine* e, const float* wav_dev, int64_t* codes_dev, int32_t B, int32_t N, void* stream);
+/* Ragged batch encode: wav [B][channels][N] fp32 (device), row b's first lens_host[b] samples -> codes [B][n_q][T_N] int64
+ * (device), T_N = frames of N; row b's first frames_host[b] frames are the codes of its own lens_host[b] samples, 0 after.
+ * Mono rows long enough for every reflect padding of the encoder run on the tensor-core encoder (codec_tc.cu): sorted by
+ * length and cut into chunks under VCB_CODEC_WS_GB, each chunk's planes sized for its longest row, every layer causal, so a
+ * row's codes are bit-identical whatever the batch, its order or the chunking.  Its latent follows the fp32 encoder within
+ * the 3-pass bf16 products' error (DESIGN.md section 4.4); the RVQ search is the fp32 one of enc_encode, so the codes are
+ * exactly the nearest codes of that latent.  Every other row (too short, a configuration the tensor-core encoder does not
+ * cover, VCB_CODEC_TC=0) goes alone through the CUDA-core encoder: bit-identical to enc_encode of that row alone.
+ * Rejected before anything is enqueued: B < 1, any lens outside [1, N], missing encoder weights.  Asynchronous on
+ * `stream` (a larger workspace synchronises it first); it shares the engine's workspace with enc_decode and
+ * enc_stream_decode, so calls on one engine must not overlap. */
+int enc_encode_ragged(enc_engine* e, const float* wav_dev, const int32_t* lens_host, int32_t B, int32_t N, int64_t* codes_dev,
+                      int32_t* frames_host, void* stream);
 /* "launches", "hop", "flops_per_frame", "tc_enabled", "tc_decodes", "stream_decodes", "stream_min_frames" (frames a fresh
  * stream's first enc_stream_decode needs; -1 without the tensor-core decoder), "stream_state_bytes" (carried state per stream);
+ * "tc_encoder" (the tensor-core encoder is built), "tc_encodes" (enc_encode_ragged calls that ran it), "encode_rows" (plane
+ * rows of its first stage it ran: per chunk, rows x the chunk's longest row rounded up to the first stride);
  * "live_bytes" / "live_handles" as vcb_counter and "resample_launches" (kernels enc_resample / enc_resampler_push enqueued) are
  * process-wide, valid with a NULL engine */
 int64_t enc_counter(enc_engine* e, const char* name);
@@ -79,8 +94,13 @@ int enc_stream_decode(enc_engine* e, enc_stream* s, const int32_t* ids_host, con
  * workspace arenas, so after a full decode only the tensors of the last stage (and "z", "x0", "u0", "hs*", "c*") still hold
  * their values -- unless the engine was finalized under VCB_CODEC_KEEP=1, which gives every tensor rows of its own: same
  * kernels, launches and arithmetic, a larger workspace (tests/test_codec_numerics.py, scripts/codec_tc_debug.py).
- * "enc.latent": under VCB_CODEC_KEEP=1, the latent the last enc_encode quantised, fp32 dims {B, dimension, T, 0}; this
- * name does not need the tensor-core decoder.  Any other name fails where that decoder is not active. */
+ * "enc.latent": under VCB_CODEC_KEEP=1, the latent the last enc_encode or enc_encode_ragged quantised, fp32 dims
+ * {B, dimension, T, 0} (ragged: row b's frames past frames_host[b] are 0); this name does not need the tensor-core decoder.
+ * The tensor-core encoder's tensors of its last chunk (rows in the chunk's order: longest first): "enc.input" (the input
+ * window planes), "enc.x0" / "enc.x0.elu" (enc.conv_in), per stage i and block j "enc.down{i}.res{j}.h" (ELU'd hidden),
+ * "enc.down{i}.res{j}" / ".elu" (block output; the last block of a stage stores only ".elu", its right padding included),
+ * "enc.down{i}.conv" / ".elu" (the strided conv; the last one is the LSTM input, time-major), "enc.hs{l}", "enc.lstm"
+ * (ELU(LSTM + skip), enc.conv_out's input).  Any other name fails where the tensor-core decoder is not active. */
 int enc_debug_tensor(enc_engine* e, const char* name, float* host_out, int64_t cap, int32_t* dims);
 
 /* Resampling: torchaudio.transforms.Resample(orig_sr, new_sr) with its defaults (sinc_interp_hann, lowpass_filter_width 6,

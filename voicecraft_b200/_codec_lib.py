@@ -18,6 +18,8 @@ PROTOTYPES = {
     "enc_finalize": (C.c_int, [C.c_void_p]),
     "enc_decode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "enc_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
+    "enc_encode_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_void_p,
+                                    C.POINTER(C.c_int32), C.c_void_p]),
     "enc_counter": (C.c_int64, [C.c_void_p, C.c_char_p]),
     "enc_debug_tensor": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64, C.POINTER(C.c_int32)]),
     "enc_stream_create": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p)]),

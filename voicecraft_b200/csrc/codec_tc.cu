@@ -23,6 +23,11 @@
 //                next step, and for the last layer ELU(h + skip) straight into the first ConvTranspose's input.
 //                800 steps x 2 layers = 1 600 dependent launches for the WHOLE batch (was: per 16 utterances), W_hh (16.8 MB
 //                as planes) stays in L2; chained with programmatic dependent launch, weights in flight before the wait.
+//
+// The encoder (enc_encode_ragged) runs on the same kernel from a plan of its own (EncPlan): input staging to 7-sample
+// windows (enc.conv_in = one k-block), the residual blocks as above, each strided conv (k = 2r, stride r) as a 2-tap conv
+// over the input read as folded rows [rows / r][r * C] with its per-utterance right padding written by tc_pad_rows_kernel,
+// the LSTM above, enc.conv_out to fp32 rows; the RVQ search stays the fp32 one of encodec.cu.
 #include "codec_tc.h"
 
 #include <algorithm>
@@ -39,7 +44,7 @@ static constexpr int TC_BM = 128;
 static constexpr int TC_BK = 64;
 static constexpr int TC_EPI_WARPS = 16;
 static constexpr int TC_THREADS = 128 + 32 * TC_EPI_WARPS;
-static constexpr int TC_MAX_KB = 64;
+static constexpr int TC_MAX_KB = 128;               // k-blocks per GEMM: the encoder's last strided conv has K = 2*8*512
 enum { TC_MODE_CONV = 0, TC_MODE_LSTM = 1 };
 
 struct TcTap {
@@ -455,6 +460,73 @@ __global__ void __launch_bounds__(256) tc_carry_kernel(const __grid_constant__ C
         for (int i = threadIdx.x; i < n; i += blockDim.x) s[i] = *at(i, len * a.up - a.halo + (i % per_plane) / per_row);
 }
 
+// Encoder input: fp32 wav rows -> planes whose channel j (< k) at row t holds sample t - (k-1) + j of the utterance, so that
+// enc.conv_in is one k-block: its causal left padding is folded in (reflect, x[-s] = x[s]; or zeros).  Channels >= k and
+// rows at or past the utterance's lens[b] samples are zero.  Chunk row b is wav row rows[b]; plane row(b, t) = b*Tp + t.
+__global__ void __launch_bounds__(256)
+tc_enc_input_kernel(const float* __restrict__ wav, long long wav_ld, const int* __restrict__ rows, const int* __restrict__ lens,
+                    __nv_bfloat16* out, long long plane, int ld, int Tp, int T, int k, int reflect, int B) {
+    const long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+    if (i >= static_cast<long long>(B) * T) return;
+    const int b = static_cast<int>(i / T), t = static_cast<int>(i - static_cast<long long>(b) * T), L = lens[b];
+    const float* x = wav + rows[b] * wav_ld;
+    __nv_bfloat16* o = out + (static_cast<long long>(b) * Tp + t) * ld;
+    for (int c0 = 0; c0 < ld; c0 += 8) {
+        float v[8];
+#pragma unroll
+        for (int u = 0; u < 8; ++u) {
+            int s = t - (k - 1) + c0 + u;
+            if (s < 0 && reflect) s = -s;
+            v[u] = (c0 + u < k && t < L && s >= 0 && s < L) ? x[s] : 0.f;
+        }
+        uint4 hi, lo;
+        tc_split8(v, hi, lo);
+        *reinterpret_cast<uint4*>(o + c0) = hi;
+        *reinterpret_cast<uint4*>(o + plane + c0) = lo;
+    }
+}
+
+// Padding rows of one plane form, block b = utterance b:
+//   lens == null   its left halo, rows -1..-n <- rows 1..n (reflect) -- for a plane whose producer writes no halo (LSTM)
+//   lens != null   the right padding of a strided conv (stride r) over its lens[b] rows: rows L .. ceil(L/r)*r - 1 <- rows
+//                  L-2, L-3, ... (reflect; audiocraft get_extra_padding_for_conv1d), which differs per utterance
+// or zeros (zero != 0).  Rows are [2 planes][rows][ld] bf16, row(b, t) = b*sb + t*st + off.
+__global__ void __launch_bounds__(256)
+tc_pad_rows_kernel(__nv_bfloat16* base, long long plane, int ld, long long sb, long long st, long long off, const int* lens, int n,
+                   int r, int zero) {
+    const int b = blockIdx.x;
+    int cnt = n, d0 = -1, dstep = -1, s0 = 1, sstep = 1;
+    if (lens != nullptr) {
+        const int L = lens[b];
+        cnt = (L + r - 1) / r * r - L;
+        d0 = L; dstep = 1; s0 = L - 2; sstep = -1;
+    }
+    const int per_row = ld / 8, per_plane = cnt * per_row;
+    for (int i = threadIdx.x; i < 2 * per_plane; i += blockDim.x) {
+        const int p = i / per_plane, rr = i - p * per_plane, j = rr / per_row, col = rr - j * per_row;
+        const long long dst = b * sb + static_cast<long long>(d0 + dstep * j) * st + off;
+        const long long src = b * sb + static_cast<long long>(s0 + sstep * j) * st + off;
+        uint4* d = reinterpret_cast<uint4*>(base + p * plane + dst * ld) + col;
+        *d = zero ? make_uint4(0u, 0u, 0u, 0u) : *(reinterpret_cast<const uint4*>(base + p * plane + src * ld) + col);
+    }
+}
+
+// latent rows [B][T][ld] fp32 -> [B][D][T] (the layout of the RVQ search), 32 frames per block through shared memory
+__global__ void __launch_bounds__(256)
+tc_latent_cm_kernel(const float* __restrict__ in, float* __restrict__ out, int D, int ld, int T) {
+    extern __shared__ float tile[];                                 // [32][D + 1]
+    const int b = blockIdx.y, t0 = blockIdx.x * 32;
+    for (int i = threadIdx.x; i < 32 * D; i += blockDim.x) {
+        const int tt = i / D, c = i - tt * D;
+        tile[tt * (D + 1) + c] = t0 + tt < T ? in[(static_cast<size_t>(b) * T + t0 + tt) * ld + c] : 0.f;
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < 32 * D; i += blockDim.x) {
+        const int c = i / 32, tt = i - c * 32;
+        if (t0 + tt < T) out[(static_cast<size_t>(b) * D + c) * T + t0 + tt] = tile[tt * (D + 1) + c];
+    }
+}
+
 // codes outside [0, bins) -> *bad = 1
 __global__ void tc_codes_check_kernel(const long long* __restrict__ codes, long long n, int bins, int* bad) {
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n; i += static_cast<long long>(gridDim.x) * blockDim.x)
@@ -521,7 +593,7 @@ struct PlanTensor {
 };
 
 enum { L_RVQ, L_CONV, L_LSTM_IH, L_LSTM_STEPS, L_CONV_OUT_SPLIT, L_CONV_OUT };
-enum { F32_NONE, F32_X0, F32_PRE, F32_COPART, F32_WAV };      // fp32 destination of a GEMM
+enum { F32_NONE, F32_X0, F32_PRE, F32_COPART, F32_WAV, F32_LAT };   // fp32 destination of a GEMM
 
 struct PlanLayer {
     int kind = L_CONV;
@@ -537,6 +609,40 @@ struct PlanLayer {
 };
 
 struct PlanStage { int up, C, Ch; };   // rows per frame, padded channels of the block tensors and of the hidden tensor
+
+// ---- the encoder plan (SEANetEncoder, oracle/encodec_oracle.py::encoder_plan), over a table of tensors like the decoder's.
+// A tensor belongs to a stage s (its rows are frames of stage s: the input's samples for s = 0, then one stage per strided
+// conv) and holds, per utterance, `halo` rows of left padding and the stage's rows rounded up to the next strided conv's
+// stride.  The input of a strided conv (stride r) has halo r and is read as folded rows [rows / r][r * C] (fold = r).
+enum { E_INPUT, E_CONV, E_DOWN, E_RPAD, E_LSTM_IH, E_LSTM_STEPS, E_LPAD, E_CONV_OUT };
+
+struct EncTensor {
+    int C = 0, halo = 0, halo_kind = HALO_ZERO, stage = 0, fold = 1;
+    bool tm = false;                   // time-major (LSTM planes)
+    int forms = 0, home = HOME_FIXED;  // home: HOME_FIXED or the arena of its stage (HOME_ARENA0 + stage % 2)
+    std::string dbg_raw, dbg_elu;
+};
+
+struct EncLayer {
+    int kind = E_CONV;
+    const char* label = "";
+    const TcGemm* g = nullptr;
+    int in = -1, in_form = FORM_RAW, in2 = -1, out = -1, out_forms = 0, f32 = F32_NONE, nstore = 0, lstm = -1;
+    int stage = 0, r = 1;              // E_DOWN / E_RPAD: the stage and stride of the strided conv
+};
+
+struct EncPlan {
+    std::vector<EncTensor> tensors;
+    std::vector<EncLayer> layers;
+    std::vector<int> ratios;           // stride of stage s's strided conv (the config's ratios reversed)
+};
+
+struct TcEncoder {
+    TcGemm conv_in, conv_out;
+    std::vector<TcGemm> down, pre, step;
+    std::vector<std::vector<TcGemm>> res1, res2;
+    EncPlan plan;
+};
 
 struct TcPlan {
     std::vector<PlanTensor> tensors;
@@ -568,6 +674,9 @@ struct TcCodec {
     std::vector<std::pair<std::string, float>> prof;
     struct Dbg { Plane p; const __nv_bfloat16* ptr; int B; };
     std::map<std::string, Dbg> dbg;      // tensors of the last decoded chunk (debug read-back)
+    std::map<std::string, Dbg> edbg;     // tensors of the last encoded chunk ("enc.*")
+    std::unique_ptr<TcEncoder> enc;      // tensor-core encoder; null: no encoder weights or not covered (enc_reason)
+    const char* enc_reason = "encoder weights (enc.*) not loaded";
     const float* dbg_cst = nullptr;      // its final LSTM cell states [layers][dbg_Bcap][ch0] ("c0", "c1", ...)
     int dbg_B = 0, dbg_Bcap = 0;
 };
@@ -1134,6 +1243,362 @@ int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T,
     return 0;
 }
 
+// ---- encoder ---------------------------------------------------------------------------------------------------------
+
+// enc.conv_in on the input planes: channel j of a row is tap j, so the whole k-tap conv is one k-block
+int build_enc_conv_in(TcGemm& g, const HostW& hw, int k, int Cout) {
+    std::vector<float> w, b;
+    if (hw.get("enc.conv_in.weight", w) || hw.get("enc.conv_in.bias", b)) return -1;
+    const int Cop = cpad(Cout);
+    std::vector<float> W(static_cast<size_t>(Cop) * TC_BK, 0.f);
+    for (int co = 0; co < Cout; ++co)
+        for (int j = 0; j < k; ++j) W[static_cast<size_t>(co) * TC_BK + j] = w[static_cast<size_t>(co) * k + j];
+    g.taps.push_back(TcTap{0, 0, 0});
+    g.Cout = Cop;
+    g.up = 1;
+    return upload_gemm(g, W, b, Cop, TC_BK, 0);
+}
+
+// Strided Conv1d w[Cout][Cin][2r] (stride r, causal left pad r) over the folded input rows [rows / r][r * Cin_pad]: output
+// frame t reads folded rows t-1 (taps 0..r-1) and t (taps r..2r-1), so K = 2 * r * Cin_pad with k = tap * Cin_pad + ci
+int build_down(TcGemm& g, const HostW& hw, const std::string& name, int Cin, int Cout, int r) {
+    std::vector<float> w, b;
+    if (hw.get(name + ".weight", w) || hw.get(name + ".bias", b)) return -1;
+    const int Cip = cpad(Cin), Cop = cpad(Cout), Ktot = 2 * r * Cip;
+    std::vector<float> W(static_cast<size_t>(Cop) * Ktot, 0.f);
+    for (int co = 0; co < Cout; ++co)
+        for (int ci = 0; ci < Cin; ++ci)
+            for (int j = 0; j < 2 * r; ++j) W[static_cast<size_t>(co) * Ktot + j * Cip + ci] = w[(static_cast<size_t>(co) * Cin + ci) * 2 * r + j];
+    for (int half = 0; half < 2; ++half)
+        for (int cb = 0; cb < r * Cip / TC_BK; ++cb) g.taps.push_back(TcTap{0, static_cast<short>(1 - half), cb * TC_BK});
+    g.Cout = Cop;
+    g.up = 1;
+    return upload_gemm(g, W, b, Cop, Ktot, 0);
+}
+
+// the stage lengths of an utterance of N samples: L[0] = N, L[s+1] = ceil(L[s] / r_s)
+std::vector<int> enc_chain(const EncPlan& pl, int N) {
+    std::vector<int> L(1, N);
+    for (int r : pl.ratios) L.push_back((L.back() + r - 1) / r);
+    return L;
+}
+
+// plane rows per utterance of every stage: the stage length rounded up to its strided conv's stride
+std::vector<int> enc_rows(const EncPlan& pl, const std::vector<int>& L) {
+    std::vector<int> R(L);
+    for (size_t s = 0; s < pl.ratios.size(); ++s) R[s] = (L[s] + pl.ratios[s] - 1) / pl.ratios[s] * pl.ratios[s];
+    return R;
+}
+
+Plane enc_geometry(const EncTensor& t, int B, const std::vector<int>& R) {
+    Plane p;
+    p.C = t.C;
+    p.T = R[t.stage];
+    p.halo = t.halo;
+    p.Tp = p.T + t.halo;
+    p.halo_zero = t.halo_kind == HALO_ZERO;
+    p.tm = t.tm;
+    if (t.tm) {
+        const int Bc = bcap(B);
+        p.rcap = p.Tp * Bc;
+        p.sb = 1;
+        p.st = Bc;
+        p.off = static_cast<long long>(t.halo) * Bc;
+    } else {
+        p.rcap = std::max(B * p.Tp, TC_BM * t.fold);     // (whole folded rows; a TMA box never taller than its tensor)
+        p.sb = p.Tp;
+        p.st = 1;
+        p.off = t.halo;
+    }
+    return p;
+}
+
+// The encoder's layers in launch order.  Halo rule as in the decoder (a causal conv reads (k-1)*dilation rows above its output
+// row); a strided conv's input keeps r rows (its causal left pad) plus the per-utterance right padding (E_RPAD).
+void build_enc_plan(TcCodec* tc) {
+    const enc_config& cf = tc->cfg;
+    EncPlan& pl = tc->enc->plan;
+    TcEncoder& E = *tc->enc;
+    const int n = cf.n_ratios, nres = cf.n_residual_layers, nl = cf.lstm, H = tc->ch0;
+    const int kres = cf.residual_kernel_size, kout = cf.last_kernel_size;
+    const int pad = cf.pad_reflect ? HALO_REFLECT : HALO_ZERO;
+    for (int s = 0; s < n; ++s) pl.ratios.push_back(cf.ratios[n - 1 - s]);
+    auto tensor = [&](int C, int halo, int kind, int stage, int fold, bool tm, int forms, std::string dbg_raw, std::string dbg_elu) {
+        EncTensor t;
+        t.C = C; t.halo = halo; t.halo_kind = kind; t.stage = stage; t.fold = fold; t.tm = tm; t.forms = forms;
+        t.home = (tc->keep || stage == n) ? HOME_FIXED : HOME_ARENA0 + (stage & 1);
+        t.dbg_raw = std::move(dbg_raw);
+        t.dbg_elu = std::move(dbg_elu);
+        pl.tensors.push_back(t);
+        return static_cast<int>(pl.tensors.size()) - 1;
+    };
+    auto layer = [&](int kind, const char* label, const TcGemm* g, int nstore, int in, int in_form, int out, int f32) {
+        EncLayer L;
+        L.kind = kind; L.label = label; L.g = g; L.nstore = nstore; L.in = in; L.in_form = in_form; L.out = out; L.f32 = f32;
+        L.out_forms = out >= 0 ? pl.tensors[out].forms : 0;
+        pl.layers.push_back(L);
+        return &pl.layers.back();
+    };
+    // what stage s's first layer reads: its first residual block (conv1 reads kres-1 rows back), or its strided conv
+    auto block_input = [&](int s, int C, const std::string& name) {
+        if (nres > 0) return tensor(C, kres - 1, pad, s, 1, false, FORM_RAW | FORM_ELU, name, name + ".elu");
+        return tensor(C, pl.ratios[s], pad, s, pl.ratios[s], false, FORM_ELU, "", name + ".elu");
+    };
+    int ch = cf.n_filters;
+    const int in0 = tensor(TC_BK, 0, HALO_ZERO, 0, 1, false, FORM_RAW, "enc.input", "");
+    layer(E_INPUT, "enc_input", nullptr, 0, -1, 0, in0, F32_NONE);
+    int cur = block_input(0, cpad(ch), "enc.x0");
+    layer(E_CONV, "enc_conv_in", &E.conv_in, cpad(ch), in0, FORM_RAW, cur, F32_NONE);
+    int u = -1, x0 = -1;
+    for (int s = 0; s < n; ++s) {
+        const int r = pl.ratios[s], hidden = ch / cf.compress;
+        const std::string si = "enc.down" + std::to_string(s);
+        for (int j = 0, dil = 1; j < nres; ++j, dil *= cf.dilation_base) {
+            const std::string sj = si + ".res" + std::to_string(j);
+            const EncTensor& x = pl.tensors[cur];
+            const int hd = tensor(cpad(hidden), x.halo, HALO_UNWRITTEN, s, x.fold, false, FORM_ELU, "", sj + ".h");
+            layer(E_CONV, "enc_res_conv1", &E.res1[s][j], cpad(hidden), cur, FORM_ELU, hd, F32_NONE);
+            const int o = j == nres - 1 ? tensor(cpad(ch), r, pad, s, r, false, FORM_ELU, "", sj + ".elu")
+                                        : tensor(cpad(ch), (kres - 1) * dil * cf.dilation_base, pad, s, 1, false,
+                                                 FORM_RAW | FORM_ELU, sj, sj + ".elu");
+            layer(E_CONV, "enc_res_conv2", &E.res2[s][j], cpad(ch), hd, FORM_ELU, o, F32_NONE)->in2 = cur;
+            cur = o;
+        }
+        EncLayer* rp = layer(E_RPAD, "enc_rpad", nullptr, 0, -1, 0, cur, F32_NONE);
+        rp->stage = s;
+        rp->r = r;
+        ch *= 2;
+        int next;
+        if (s < n - 1) next = block_input(s + 1, cpad(ch), si + ".conv");
+        else if (nl > 0) next = x0 = tensor(H, 0, HALO_ZERO, n, 1, true, FORM_RAW, si + ".conv", "");
+        else next = u = tensor(cpad(ch), kout - 1, pad, n, 1, false, FORM_ELU, "", "enc.lstm");
+        EncLayer* d = layer(E_DOWN, "enc_down", &E.down[s], cpad(ch), cur, FORM_ELU, next, next == x0 ? F32_X0 : F32_NONE);
+        d->stage = s;
+        d->r = r;
+        cur = next;
+    }
+    if (nl > 0) {
+        int hs[2] = {-1, -1};
+        for (int l = 0; l < std::min(nl, 2); ++l)
+            hs[l] = tensor(H, 1, HALO_ZERO, n, 1, true, FORM_RAW, "enc.hs" + std::to_string(l), "");
+        u = tensor(cpad(H), kout - 1, pad, n, 1, false, FORM_ELU, "", "enc.lstm");
+        for (int l = 0; l < nl; ++l) {
+            layer(E_LSTM_IH, "enc_lstm_ih", &E.pre[l], 4 * H, l == 0 ? x0 : hs[(l - 1) & 1], FORM_RAW, -1, F32_PRE)->lstm = l;
+            // the last layer's epilogue writes ELU(h + skip) into enc.conv_out's input, whose halo E_LPAD then fills
+            layer(E_LSTM_STEPS, "enc_lstm_steps", &E.step[l], 4 * H, hs[l & 1], FORM_RAW, l == nl - 1 ? u : -1, F32_NONE)->lstm = l;
+        }
+        layer(E_LPAD, "enc_lpad", nullptr, 0, -1, 0, u, F32_NONE);
+    }
+    layer(E_CONV_OUT, "enc_conv_out", &E.conv_out, tc->Dp, u, FORM_ELU, -1, F32_LAT);
+}
+
+struct EncWs {
+    std::vector<size_t> tensor;
+    size_t x0f = 0, pre = 0, cst = 0, latf = 0, lat = 0, scores = 0, codes = 0, tab = 0, bytes = 0;
+};
+
+// The workspace of an encoder chunk of B utterances of at most N samples: fixed tensors (the LSTM stage's), two arenas that
+// the stages alternate between (stage s's strided conv reads arena s % 2 and writes arena (s+1) % 2), the fp32 buffers,
+// the RVQ scores and codes, the per-utterance table.
+EncWs enc_ws_layout(const TcCodec* tc, int B, int N) {
+    const EncPlan& pl = tc->enc->plan;
+    const enc_config& cf = tc->cfg;
+    const std::vector<int> R = enc_rows(pl, enc_chain(pl, N));
+    const int n = static_cast<int>(pl.ratios.size()), Tn = R[n], Bcap = bcap(B), H = tc->ch0, nl = cf.lstm;
+    EncWs w;
+    w.tensor.resize(pl.tensors.size());
+    size_t off = 0;
+    auto take = [&](size_t bytes) {
+        const size_t o = off;
+        off += align_up(bytes, 1024);
+        return o;
+    };
+    std::vector<size_t> stage_off(n + 1, 0);
+    size_t arena[2] = {0, 0};
+    for (size_t i = 0; i < pl.tensors.size(); ++i) {
+        const EncTensor& t = pl.tensors[i];
+        size_t bytes = 0;
+        for (int f : {FORM_RAW, FORM_ELU})
+            if (t.forms & f) bytes += align_up(form_bytes(enc_geometry(t, B, R)), 1024);
+        if (t.home == HOME_FIXED) {
+            w.tensor[i] = take(bytes);
+        } else {
+            w.tensor[i] = stage_off[t.stage];                  // offset inside its arena for now
+            stage_off[t.stage] += bytes;
+            arena[t.home - HOME_ARENA0] = std::max(arena[t.home - HOME_ARENA0], stage_off[t.stage]);
+        }
+    }
+    const size_t a0 = take(arena[0]), a1 = take(arena[1]);
+    for (size_t i = 0; i < pl.tensors.size(); ++i)
+        if (pl.tensors[i].home != HOME_FIXED) w.tensor[i] += pl.tensors[i].home == HOME_ARENA0 ? a0 : a1;
+    if (nl > 0) {
+        w.x0f = take(static_cast<size_t>(Tn) * Bcap * H * 4);
+        w.pre = take(static_cast<size_t>(Tn) * Bcap * 4 * H * 4);
+        w.cst = take(static_cast<size_t>(nl) * Bcap * H * 4);
+    }
+    w.latf = take(static_cast<size_t>(B) * Tn * tc->Dp * 4);
+    w.lat = take(static_cast<size_t>(B) * cf.dimension * Tn * 4);
+    w.scores = take(static_cast<size_t>(B) * cf.bins * Tn * 4);
+    w.codes = take(static_cast<size_t>(B) * cf.n_q * Tn * 8);
+    w.tab = take(static_cast<size_t>(n + 2) * B * 4);
+    w.bytes = off;
+    return w;
+}
+
+// One chunk: utterance b = wav row rows[b] with lens[b] samples; the chunk's planes are sized for its longest utterance.
+int encode_chunk_tc(TcCodec* tc, const float* wav, long long wav_ld, const int* rows, const int* lens, int B, cudaStream_t st,
+                    int64_t* launches, TcEncOut* out) {
+    const EncPlan& pl = tc->enc->plan;
+    const enc_config& cf = tc->cfg;
+    const int n = static_cast<int>(pl.ratios.size()), Bcap = bcap(B), H = tc->ch0, nl = cf.lstm;
+    const int N = *std::max_element(lens, lens + B);
+    const std::vector<int> R = enc_rows(pl, enc_chain(pl, N));
+    const int Tn = R[n];
+    const EncWs w = enc_ws_layout(tc, B, N);
+    std::vector<Plane> P(pl.tensors.size());
+    tc->edbg.clear();
+    for (size_t i = 0; i < P.size(); ++i) {
+        const EncTensor& t = pl.tensors[i];
+        Plane& p = P[i];
+        p = enc_geometry(t, B, R);
+        uint8_t* base = tc->ws + w.tensor[i];
+        if (t.forms & FORM_RAW) {
+            p.raw = reinterpret_cast<__nv_bfloat16*>(base);
+            base += align_up(form_bytes(p), 1024);
+        }
+        if (t.forms & FORM_ELU) p.elu = reinterpret_cast<__nv_bfloat16*>(base);
+        if (!t.dbg_raw.empty()) tc->edbg[t.dbg_raw] = TcCodec::Dbg{p, p.raw, B};
+        if (!t.dbg_elu.empty()) tc->edbg[t.dbg_elu] = TcCodec::Dbg{p, p.elu, B};
+    }
+    float* x0f = reinterpret_cast<float*>(tc->ws + w.x0f);
+    float* pre = reinterpret_cast<float*>(tc->ws + w.pre);
+    float* cst = reinterpret_cast<float*>(tc->ws + w.cst);
+    float* latf = reinterpret_cast<float*>(tc->ws + w.latf);
+    int* tab = reinterpret_cast<int*>(tc->ws + w.tab);         // [n+1][B] stage lengths, then [B] wav rows
+    {
+        std::vector<int> h(static_cast<size_t>(n + 2) * B);
+        for (int b = 0; b < B; ++b) {
+            const std::vector<int> L = enc_chain(pl, lens[b]);
+            for (int s = 0; s <= n; ++s) h[static_cast<size_t>(s) * B + b] = L[s];
+            h[static_cast<size_t>(n + 1) * B + b] = rows[b];
+        }
+        VCB_CUDA_OK(cudaMemcpyAsync(tab, h.data(), h.size() * 4, cudaMemcpyHostToDevice, st));   // pageable: staged at once
+    }
+    if (nl > 0) VCB_CUDA_OK(cudaMemsetAsync(cst, 0, static_cast<size_t>(nl) * Bcap * H * 4, st));
+    auto clear_h0 = [&](const Plane& hs) -> int {
+        VCB_CUDA_OK(cudaMemsetAsync(hs.raw, 0, static_cast<size_t>(Bcap) * H * 2, st));
+        VCB_CUDA_OK(cudaMemsetAsync(hs.raw + hs.plane(), 0, static_cast<size_t>(Bcap) * H * 2, st));
+        return 0;
+    };
+    for (const EncLayer& L : pl.layers)
+        if (L.kind == E_LSTM_STEPS && L.lstm < 2 && clear_h0(P[L.in])) return -1;
+
+    Prof pf{tc, st};
+    CUtensorMap mA, mB;
+    for (const EncLayer& L : pl.layers) {
+        pf.begin(L.label);
+        if (L.kind == E_INPUT) {
+            const Plane& o = P[L.out];
+            const long long items = static_cast<long long>(B) * o.T;
+            tc_enc_input_kernel<<<static_cast<unsigned>((items + 255) / 256), 256, 0, st>>>(
+                wav, wav_ld, tab + static_cast<size_t>(n + 1) * B, tab, o.raw, o.plane(), o.C, o.Tp, o.T, cf.kernel_size, cf.pad_reflect, B);
+            VCB_CUDA_OK(cudaGetLastError());
+            ++*launches;
+        } else if (L.kind == E_RPAD || L.kind == E_LPAD) {
+            const Plane& o = P[L.out];
+            __nv_bfloat16* base = o.elu ? o.elu : o.raw;
+            tc_pad_rows_kernel<<<B, 256, 0, st>>>(base, o.plane(), o.C, o.sb, o.st, o.off,
+                                                  L.kind == E_RPAD ? tab + static_cast<size_t>(L.stage) * B : nullptr, o.halo, L.r,
+                                                  o.halo_zero);
+            VCB_CUDA_OK(cudaGetLastError());
+            ++*launches;
+        } else {
+            const TcGemm& g = *L.g;
+            Plane in = P[L.in];
+            if (L.kind == E_DOWN) {                          // folded rows: r plane rows of C channels are one row of r*C
+                const int r = L.r;
+                in.C *= r; in.rcap /= r; in.Tp /= r; in.T /= r; in.halo = 1; in.sb = in.Tp; in.off = 1;
+            }
+            if (plane_map(&mA, L.in_form == FORM_ELU ? P[L.in].elu : P[L.in].raw, in) ||
+                (L.in2 >= 0 && plane_map(&mB, P[L.in2].raw, P[L.in2])))
+                return -1;
+            TcCall c{};
+            c.mtiles = ((L.kind == E_LSTM_STEPS ? B : in.rcap) + TC_BM - 1) / TC_BM;
+            if (static_cast<long long>(c.mtiles) * g.ntiles > 0x7fffffffll) {
+                set_error("codec_tc: too many tiles");
+                return -1;
+            }
+            c.total_kb = g.total_kb;
+            c.ntiles = g.ntiles;
+            c.bias = g.bias;
+            c.up = g.up;
+            c.Cout = g.Cout;
+            std::copy(g.taps.begin(), g.taps.end(), c.taps);
+            c.Nstore = L.nstore;
+            c.rows_total = in.rcap;
+            c.rcap[0] = in.rcap;
+            c.B = B;
+            if (L.kind != E_LSTM_STEPS) {
+                c.in_tm = in.tm;
+                c.in_div = in.tm ? static_cast<int>(in.st) : in.Tp;
+                c.in_halo = in.halo;
+                c.T_in = in.T;
+            }
+            if (L.in2 >= 0) c.rcap[1] = P[L.in2].rcap;
+            if (L.out >= 0) {
+                const Plane& o = P[L.out];
+                c.raw = L.out_forms & FORM_RAW ? o.raw : nullptr;
+                c.elu = L.out_forms & FORM_ELU ? o.elu : nullptr;
+                c.o_plane = o.plane();
+                c.o_ld = o.C;
+                c.o_sb = o.sb;
+                c.o_st = o.st;
+                c.o_off = o.off;
+                c.o_halo = pl.tensors[L.out].halo_kind == HALO_UNWRITTEN ? 0 : o.halo;
+                c.o_halo_zero = o.halo_zero;
+            }
+            auto rows_f32 = [&](float* f, int ld, int valid, long long sb, long long stt) {
+                c.f32 = f; c.f_ld = ld; c.f_valid = valid; c.f_sb = sb; c.f_st = stt; c.f_off = 0;
+            };
+            if (L.f32 == F32_X0) rows_f32(x0f, H, H, 1, Bcap);                 // time-major [T][Bcap][H]
+            if (L.f32 == F32_PRE) rows_f32(pre, 4 * H, 4 * H, 1, Bcap);        // time-major [T][Bcap][4H]
+            if (L.f32 == F32_LAT) rows_f32(latf, tc->Dp, cf.dimension, Tn, 1); // [B][T][Dp]
+            const CUtensorMap& a1 = L.in2 >= 0 ? mB : mA;
+            if (L.kind == E_LSTM_STEPS) {
+                c.mode = TC_MODE_LSTM;
+                c.pre = pre;
+                c.cst = cst + static_cast<size_t>(L.lstm) * Bcap * H;
+                c.hseq = P[L.in].raw;
+                c.h_plane = P[L.in].plane();
+                c.Bcap = Bcap;
+                c.H = H;
+                if (L.out >= 0) c.skip = x0f;
+                if (L.lstm >= 2 && clear_h0(P[L.in])) return -1;
+                for (int t = 0; t < Tn; ++t) {
+                    c.t_step = t;
+                    c.row_base = t * Bcap;
+                    if (tc_launch(tc, mA, a1, g, c, st)) return -1;
+                }
+                *launches += Tn;
+            } else {
+                if (tc_launch(tc, mA, a1, g, c, st)) return -1;
+                ++*launches;
+            }
+        }
+        pf.end();
+    }
+    float* lat = reinterpret_cast<float*>(tc->ws + w.lat);
+    tc_latent_cm_kernel<<<dim3((Tn + 31) / 32, B), 256, 32 * (cf.dimension + 1) * 4, st>>>(latf, lat, cf.dimension, tc->Dp, Tn);
+    VCB_CUDA_OK(cudaGetLastError());
+    ++*launches;
+    pf.finish();
+    out->latent = lat;
+    out->scores = reinterpret_cast<float*>(tc->ws + w.scores);
+    out->codes = reinterpret_cast<int64_t*>(tc->ws + w.codes);
+    out->T = Tn;
+    return 0;
+}
+
 }  // namespace
 
 int tc_codec_build(const enc_config& cfg, const std::map<std::string, DevBuf<float>>& w_dev,
@@ -1152,7 +1617,7 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, DevBuf<flo
     if ((ch0 >> cfg.n_ratios) < 1 || cfg.compress < 1) return no("channel plan");
     if (2 * cpad(ch0) / TC_BK > TC_MAX_KB || cfg.kernel_size * cpad(cfg.dimension) / TC_BK > TC_MAX_KB ||
         cfg.residual_kernel_size * cpad(ch0 / 2) / TC_BK > TC_MAX_KB || cfg.last_kernel_size * cpad(cfg.n_filters) / TC_BK > TC_MAX_KB)
-        return no("reduction deeper than 64 k-blocks");
+        return no("reduction deeper than the kernel's k-blocks");
     if (getenv("VCB_CODEC_TC") && atoi(getenv("VCB_CODEC_TC")) == 0) return no("disabled by VCB_CODEC_TC=0");
     TcCodecPtr tc(new TcCodec());
     tc->cfg = cfg;
@@ -1243,8 +1708,95 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, DevBuf<flo
     }
     if (rc) return -1;
     build_plan(tc.get());
+    if (w_dev.count("enc.conv_in.weight")) {
+        // the encoder: the decoder's coverage, plus an input window that fits one k-block and reductions within TC_MAX_KB
+        const int n = cfg.n_ratios, kres = cfg.residual_kernel_size;
+        bool deep = cfg.kernel_size > TC_BK || cfg.last_kernel_size * cpad(ch0) / TC_BK > TC_MAX_KB;
+        for (int s = 0, c = cfg.n_filters; s < n; ++s, c *= 2)
+            deep = deep || 2 * cfg.ratios[n - 1 - s] * cpad(c) / TC_BK > TC_MAX_KB || kres * cpad(c) / TC_BK > TC_MAX_KB;
+        if (deep) {
+            tc->enc_reason = "encoder reduction deeper than the kernel's k-blocks";
+        } else {
+            tc->enc.reset(new TcEncoder());
+            TcEncoder& E = *tc->enc;
+            rc = build_enc_conv_in(E.conv_in, hw, cfg.kernel_size, cfg.n_filters);
+            E.down.resize(n);
+            E.res1.resize(n);
+            E.res2.resize(n);
+            for (int s = 0, c = cfg.n_filters; s < n && !rc; ++s, c *= 2) {
+                E.res1[s].resize(cfg.n_residual_layers);
+                E.res2[s].resize(cfg.n_residual_layers);
+                for (int j = 0, dil = 1; j < cfg.n_residual_layers && !rc; ++j, dil *= cfg.dilation_base) {
+                    snprintf(nm, sizeof(nm), "enc.down%d.res%d.conv1", s, j);
+                    rc = build_conv(E.res1[s][j], hw, nm, c, c / cfg.compress, kres, dil);
+                    snprintf(nm, sizeof(nm), "enc.down%d.res%d", s, j);
+                    if (!rc) rc = build_res_tail(E.res2[s][j], hw, nm, c, c / cfg.compress);
+                }
+                snprintf(nm, sizeof(nm), "enc.down%d.conv", s);
+                if (!rc) rc = build_down(E.down[s], hw, nm, c, 2 * c, cfg.ratios[n - 1 - s]);
+            }
+            E.pre.resize(cfg.lstm);
+            E.step.resize(cfg.lstm);
+            for (int l = 0; l < cfg.lstm && !rc; ++l) {
+                char a[96], b[96], c2[96];
+                snprintf(a, sizeof(a), "enc.lstm.weight_ih_l%d", l);
+                snprintf(b, sizeof(b), "enc.lstm.bias_ih_l%d", l);
+                snprintf(c2, sizeof(c2), "enc.lstm.bias_hh_l%d", l);
+                rc = build_lstm(E.pre[l], hw, a, b, c2, ch0, 0);
+                snprintf(a, sizeof(a), "enc.lstm.weight_hh_l%d", l);
+                if (!rc) rc = build_lstm(E.step[l], hw, a, "", "", ch0, step_bn);
+            }
+            if (!rc) rc = build_conv(E.conv_out, hw, "enc.conv_out", ch0, cfg.dimension, cfg.last_kernel_size, 1);
+            if (rc) return -1;
+            build_enc_plan(tc.get());
+            tc->enc_reason = "";
+        }
+    }
     *out = std::move(tc);
     return 0;
+}
+
+bool tc_encoder_active(const TcCodec* c) { return c != nullptr && c->enc != nullptr; }
+
+const char* tc_encoder_reason(const TcCodec* c) { return c ? c->enc_reason : "the tensor-core codec is not active"; }
+
+// every stage longer than the padding its convolutions reflect (audiocraft pad1d zero-extends a shorter input instead)
+bool tc_encoder_accepts(const TcCodec* c, int len) {
+    if (!tc_encoder_active(c) || len < 1) return false;
+    const enc_config& cf = c->cfg;
+    if (!cf.pad_reflect) return true;
+    const std::vector<int> L = enc_chain(c->enc->plan, len);
+    int dmax = 1;
+    for (int j = 1; j < cf.n_residual_layers; ++j) dmax *= cf.dilation_base;
+    const int res_pad = cf.n_residual_layers > 0 ? (cf.residual_kernel_size - 1) * dmax : 0;
+    if (L[0] <= cf.kernel_size - 1) return false;
+    for (size_t s = 0; s < c->enc->plan.ratios.size(); ++s)
+        if (L[s] <= res_pad || L[s] <= c->enc->plan.ratios[s]) return false;
+    return L.back() > cf.last_kernel_size - 1;
+}
+
+size_t tc_encoder_ws_bytes(const TcCodec* c, int B, int N) { return enc_ws_layout(c, B, N).bytes; }
+
+size_t tc_ws_limit(const TcCodec* c) { return c->ws_limit; }
+
+int64_t tc_encoder_rows(const TcCodec* c, int B, int N) {
+    return static_cast<int64_t>(B) * enc_rows(c->enc->plan, enc_chain(c->enc->plan, N))[0];
+}
+
+int tc_encoder_encode(TcCodec* tc, const float* wav, long long wav_ld, const int* rows, const int* lens, int B, cudaStream_t st,
+                      int64_t* launches, TcEncOut* out) {
+    tc->prof.clear();
+    const size_t need = enc_ws_layout(tc, B, *std::max_element(lens, lens + B)).bytes;
+    if (need > tc->ws.size()) {
+        if (tc->ws) VCB_CUDA_OK(cudaStreamSynchronize(st));      // alloc releases the previous workspace first
+        if (tc->ws.alloc(need)) {
+            const std::string why = get_error();
+            set_error("codec_tc: cannot allocate a %.2f GB encoder workspace for %d utterances (%s)", need / 1073741824.0, B,
+                      why.c_str());
+            return -1;
+        }
+    }
+    return encode_chunk_tc(tc, wav, wav_ld, rows, lens, B, st, launches, out);
 }
 
 bool tc_codec_accepts(const TcCodec* c, int B, int T) { return c != nullptr && B >= 1 && T >= c->plan.min_T; }
@@ -1315,9 +1867,10 @@ int tc_codec_debug_tensor(TcCodec* tc, const char* name, float* host_out, int64_
                                static_cast<size_t>(B) * H * 4, cudaMemcpyDeviceToHost));
         return 0;
     }
-    auto it = tc->dbg.find(name);
-    if (it == tc->dbg.end()) {
-        set_error("codec_tc: no tensor '%s' in the last decode", name);
+    auto& m = strncmp(name, "enc.", 4) ? tc->dbg : tc->edbg;
+    auto it = m.find(name);
+    if (it == m.end()) {
+        set_error("codec_tc: no tensor '%s' in the last decode or tensor-core encode", name);
         return -1;
     }
     const Plane& p = it->second.p;

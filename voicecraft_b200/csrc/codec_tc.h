@@ -46,4 +46,27 @@ const std::vector<std::pair<std::string, float>>& tc_codec_profile(const TcCodec
 // VCB_CODEC_KEEP=1 at tc_codec_build no two tensors share rows, so every one of them holds what its layer stored.
 int tc_codec_debug_tensor(TcCodec* c, const char* name, float* host_out, int64_t cap, int32_t* dims);
 
+// ---- tensor-core encoder (built with the decoder when the enc.* weights are loaded)
+bool tc_encoder_active(const TcCodec* c);
+const char* tc_encoder_reason(const TcCodec* c);
+// whether an utterance of len samples can run here (every stage longer than the padding it reflects)
+bool tc_encoder_accepts(const TcCodec* c, int len);
+// workspace of a chunk of B utterances of at most N samples; the VCB_CODEC_WS_GB limit the host chunks under
+size_t tc_encoder_ws_bytes(const TcCodec* c, int B, int N);
+size_t tc_ws_limit(const TcCodec* c);
+// plane rows a chunk of B utterances of at most N samples runs through (its first stage)
+int64_t tc_encoder_rows(const TcCodec* c, int B, int N);
+// the chunk's fp32 latent [B][dimension][T] (the RVQ search consumes it as its residual), scores scratch [B][bins][T] and
+// codes [B][n_q][T], all in the workspace; T = frames of the chunk's longest utterance
+struct TcEncOut {
+    float* latent;
+    float* scores;
+    int64_t* codes;
+    int T;
+};
+// utterance b = wav row rows[b] (fp32 at wav + rows[b] * wav_ld) with lens[b] samples; asynchronous on st (the
+// workspace may be reallocated first, after a stream synchronisation).  Debug names "enc.*" (tc_codec_debug_tensor).
+int tc_encoder_encode(TcCodec* c, const float* wav, long long wav_ld, const int* rows, const int* lens, int B, cudaStream_t st,
+                      int64_t* launches, TcEncOut* out);
+
 }  // namespace vcb

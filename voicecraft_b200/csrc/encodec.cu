@@ -8,11 +8,14 @@
 //                       ELU fused on the input gather, bias + residual fused in the epilogue
 //   lstm_step_kernel    one time step of one LSTM layer: gates = pre[:, t] + W_hh h ; c, h update ; (+ skip)
 // Since round 2 enc_decode runs the tensor-core decoder of codec_tc.cu whenever the configuration is one it covers (the
-// default 16 kHz codec is); the kernels here remain the path for everything else and for the encoder.
+// default 16 kHz codec is); the kernels here remain the path for everything else and for enc_encode.  enc_encode_ragged
+// runs the tensor-core encoder of codec_tc.cu on the rows it covers and these kernels, one row at a time, on the others;
+// both end in the RVQ search here (rvq_encode).
 #include "../../include/vcb200_codec.h"
 #include "codec_tc.h"
 #include "vcb_internal.h"
 
+#include <algorithm>
 #include <cmath>
 #include <cstring>
 #include <map>
@@ -283,6 +286,10 @@ struct enc_engine {
     const char* tc_reason = "";
     int64_t tc_decodes = 0;
     int64_t stream_decodes = 0;
+    int64_t tc_encodes = 0;             // enc_encode_ragged calls that ran the tensor-core encoder
+    int64_t encode_rows = 0;            // plane rows (first stage) through the tensor-core encoder
+    DevBuf<float> row_wav;              // enc_encode_ragged, CUDA-core rows: one utterance's [channels][len] samples
+    DevBuf<int64_t> row_codes;          // ... and its codes [n_q][T]
     bool keep = false;                  // VCB_CODEC_KEEP=1: enc_encode keeps the latent it quantises ("enc.latent")
     DevBuf<float> latent;               // [lat_B][dimension][lat_T]
     int lat_B = 0, lat_T = 0;
@@ -443,6 +450,8 @@ int res_block(enc_engine* e, const char* prefix, const float* x, float* y, float
     return conv_launch(e, conv_args(e, w2, b2, y, pre, hidden, ch, T, 1, 1, 1, res), B, st);
 }
 
+int rvq_encode(enc_engine* e, float* y, float* pre, int64_t* codes, int B, int T, cudaStream_t st);
+
 // wav [B, channels, N] -> codes [B, n_q, T]: SEANetEncoder (conv k7 -> n x [ResBlock, ELU, strided conv] -> LSTM + skip -> ELU ->
 // conv k7) and residual vector quantisation.  (reference data/tokenizer.py:127-129 -> audiocraft EncodecModel.encode)
 int encode_chunk(enc_engine* e, const float* wav, int64_t* codes, float* latent, int B, int N, cudaStream_t st) {
@@ -478,10 +487,16 @@ int encode_chunk(enc_engine* e, const float* wav, int64_t* codes, float* latent,
     }
     if (enc_need(e, "enc.conv_out.weight", &wt) || enc_need(e, "enc.conv_out.bias", &bs)) return -1;
     if (conv_launch(e, conv_args(e, wt, bs, x, y, ch, c.dimension, t_cur, c.last_kernel_size, 1, 1, nullptr), B, st)) return -1;
-    // ---- residual vector quantisation: y = latent [B, D, T] is consumed as the running residual
     const int T = t_cur;
     if (latent != nullptr)
         VCB_CUDA_OK(cudaMemcpyAsync(latent, y, static_cast<size_t>(B) * c.dimension * T * 4, cudaMemcpyDeviceToDevice, st));
+    return rvq_encode(e, y, pre, codes, B, T, st);
+}
+
+// residual vector quantisation of y = latent [B, D, T], consumed as the running residual; pre: scores scratch [B][bins][T]
+int rvq_encode(enc_engine* e, float* y, float* pre, int64_t* codes, int B, int T, cudaStream_t st) {
+    const enc_config& c = e->cfg;
+    char nm[128];
     for (int q = 0; q < c.n_q; ++q) {
         float *emb, *hsn;
         snprintf(nm, sizeof(nm), "vq.%d.embed", q);
@@ -735,6 +750,99 @@ int enc_encode(enc_engine* e, const float* wav_dev, int64_t* codes_dev, int32_t 
     return 0;
 }
 
+int enc_encode_ragged(enc_engine* e, const float* wav_dev, const int32_t* lens_host, int32_t B, int32_t N, int64_t* codes_dev,
+                      int32_t* frames_host, void* stream) {
+    if (!e || !e->finalized) {
+        set_error("codec engine not finalized");
+        return -1;
+    }
+    if (!e->has_encoder) {
+        set_error("codec: encoder weights (enc.*) were not loaded");
+        return -1;
+    }
+    if (!wav_dev || !lens_host || !codes_dev || !frames_host) {
+        set_error("codec: null argument");
+        return -1;
+    }
+    if (B < 1 || N < 1) {
+        set_error("codec: empty input (B=%d, N=%d)", B, N);
+        return -1;
+    }
+    for (int b = 0; b < B; ++b)
+        if (lens_host[b] < 1 || lens_host[b] > N) {
+            set_error("codec: row %d has %d samples, outside [1, N = %d]", b, lens_host[b], N);
+            return -1;
+        }
+    const enc_config& c = e->cfg;
+    auto frames = [&](int n) {
+        for (int i = c.n_ratios - 1; i >= 0; --i) n = (n + c.ratios[i] - 1) / c.ratios[i];
+        return n;
+    };
+    const int TN = frames(N);
+    for (int b = 0; b < B; ++b) frames_host[b] = frames(lens_host[b]);
+    VCB_CUDA_OK(cudaSetDevice(c.device));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t lat = static_cast<size_t>(c.dimension) * TN;
+    e->lat_B = 0;
+    if (e->keep) {
+        if (e->latent.size() < B * lat && e->latent.alloc(B * lat)) return -1;
+        VCB_CUDA_OK(cudaMemsetAsync(e->latent, 0, B * lat * 4, st));
+        e->lat_B = B;
+        e->lat_T = TN;
+    }
+    VCB_CUDA_OK(cudaMemsetAsync(codes_dev, 0, static_cast<size_t>(B) * c.n_q * TN * 8, st));
+    // the codes (and under VCB_CODEC_KEEP the latent) of utterance b, [n_q][T] with T >= its frames, into its output row
+    auto place = [&](int b, const int64_t* codes, const float* latent, int T) -> int {
+        const int f = frames_host[b];
+        VCB_CUDA_OK(cudaMemcpy2DAsync(codes_dev + static_cast<size_t>(b) * c.n_q * TN, TN * 8, codes, static_cast<size_t>(T) * 8,
+                                      static_cast<size_t>(f) * 8, c.n_q, cudaMemcpyDeviceToDevice, st));
+        if (e->keep && latent != nullptr)
+            VCB_CUDA_OK(cudaMemcpy2DAsync(e->latent + b * lat, TN * 4, latent, static_cast<size_t>(T) * 4, static_cast<size_t>(f) * 4,
+                                          c.dimension, cudaMemcpyDeviceToDevice, st));
+        return 0;
+    };
+    TcCodec* tc = e->tc.get();
+    std::vector<int> tc_rows, cc_rows;
+    for (int b = 0; b < B; ++b) (c.channels == 1 && tc_encoder_accepts(tc, lens_host[b]) ? tc_rows : cc_rows).push_back(b);
+    // tensor-core rows, longest first, in chunks under the workspace limit; a chunk is sized for its longest row
+    std::stable_sort(tc_rows.begin(), tc_rows.end(), [&](int a, int b) { return lens_host[a] > lens_host[b]; });
+    for (size_t i0 = 0; i0 < tc_rows.size();) {
+        const int Nmax = lens_host[tc_rows[i0]];
+        size_t i1 = i0 + 1;
+        while (i1 < tc_rows.size() && tc_encoder_ws_bytes(tc, static_cast<int>(i1 - i0 + 1), Nmax) <= tc_ws_limit(tc)) ++i1;
+        const int nb = static_cast<int>(i1 - i0);
+        std::vector<int> rows(tc_rows.begin() + i0, tc_rows.begin() + i1), lens(nb);
+        for (int j = 0; j < nb; ++j) lens[j] = lens_host[rows[j]];
+        TcEncOut out;
+        if (tc_encoder_encode(tc, wav_dev, N, rows.data(), lens.data(), nb, st, &e->launches, &out)) return -1;
+        // (the latent is kept, in stream order, before the search consumes it as its residual)
+        if (e->keep)
+            for (int j = 0; j < nb; ++j)
+                VCB_CUDA_OK(cudaMemcpy2DAsync(e->latent + rows[j] * lat, TN * 4, out.latent + static_cast<size_t>(j) * c.dimension * out.T,
+                                              static_cast<size_t>(out.T) * 4, static_cast<size_t>(frames_host[rows[j]]) * 4, c.dimension,
+                                              cudaMemcpyDeviceToDevice, st));
+        if (rvq_encode(e, out.latent, out.scores, out.codes, nb, out.T, st)) return -1;
+        for (int j = 0; j < nb; ++j)
+            if (place(rows[j], out.codes + static_cast<size_t>(j) * c.n_q * out.T, nullptr, out.T)) return -1;
+        e->encode_rows += tc_encoder_rows(tc, nb, Nmax);
+        i0 = i1;
+    }
+    if (!tc_rows.empty()) e->tc_encodes++;
+    // every other row alone on the CUDA-core encoder: what enc_encode of that row alone computes
+    for (int b : cc_rows) {
+        const int L = lens_host[b], T = frames_host[b];
+        if (e->row_wav.size() < static_cast<size_t>(c.channels) * L && e->row_wav.alloc(static_cast<size_t>(c.channels) * L)) return -1;
+        if (e->row_codes.size() < static_cast<size_t>(c.n_q) * T && e->row_codes.alloc(static_cast<size_t>(c.n_q) * T)) return -1;
+        VCB_CUDA_OK(cudaMemcpy2DAsync(e->row_wav, static_cast<size_t>(L) * 4, wav_dev + static_cast<size_t>(b) * c.channels * N,
+                                      static_cast<size_t>(N) * 4, static_cast<size_t>(L) * 4, c.channels, cudaMemcpyDeviceToDevice, st));
+        if (ensure_buffers(e, 1, (L + e->hop - 1) / e->hop + 1)) return -1;
+        // (its latent, under VCB_CODEC_KEEP, in buf[2]: scratch of the encoder layers that the RVQ search leaves alone)
+        if (encode_chunk(e, e->row_wav, e->row_codes, e->keep ? e->buf[2].get() : nullptr, 1, L, st)) return -1;
+        if (place(b, e->row_codes, e->buf[2], T)) return -1;
+    }
+    return 0;
+}
+
 int enc_debug_tensor(enc_engine* e, const char* name, float* host_out, int64_t cap, int32_t* dims) {
     if (e && name && !strcmp(name, "enc.latent")) {
         if (e->lat_B == 0) {
@@ -770,6 +878,9 @@ int64_t enc_counter(enc_engine* e, const char* name) {
     if (!strcmp(name, "tc_enabled")) return e->tc != nullptr;
     if (!strcmp(name, "tc_decodes")) return e->tc_decodes;
     if (!strcmp(name, "stream_decodes")) return e->stream_decodes;
+    if (!strcmp(name, "tc_encodes")) return e->tc_encodes;
+    if (!strcmp(name, "encode_rows")) return e->encode_rows;
+    if (!strcmp(name, "tc_encoder")) return tc_encoder_active(e->tc.get());
     if (!strcmp(name, "stream_min_frames")) return e->tc ? tc_stream_min_frames(e->tc.get()) : -1;
     if (!strcmp(name, "stream_state_bytes")) return e->tc ? static_cast<int64_t>(tc_stream_state_bytes(e->tc.get())) : -1;
     return -1;

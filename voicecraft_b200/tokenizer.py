@@ -324,6 +324,63 @@ class AudioTokenizer:
         """Reference signature (data/tokenizer.py:127-129): wav [1,C,N] -> [(codes[1,K,T], None)]."""
         return [(self.encode_codes(wav), None)]
 
+    def frames(self, n_samples: int, sample_rate: int = None) -> int:
+        """Code frames of a prompt of n_samples at sample_rate (default: the codec's): resampled to the codec's rate
+        (ceil(n N / o)), then down-sampled by every ratio, rounded up at each."""
+        n = int(n_samples)
+        if sample_rate is not None and int(sample_rate) != self.sample_rate:
+            o, r = resample_dims(int(sample_rate), self.sample_rate)[:2]
+            n = -(-r * n // o)
+        for r in reversed(list(self.config.ratios)):
+            n = -(-n // int(r))
+        return n
+
+    @property
+    def has_encoder(self) -> bool:
+        return "enc.conv_in.weight" in self._sd
+
+    @torch.no_grad()
+    def encode_many(self, wavs, sample_rate: int = None):
+        """Prompts of different lengths in one call: wavs, a list of [channels_i, N_i] tensors at sample_rate (default: the
+        codec's; a list gives each its own rate) -> list of codes [1, K, T_i].  Each is mixed to the codec's channel count as convert_audio does
+        (mix_channels), resampled on the device when the rate differs (one ragged enc_resample), and all are encoded by one
+        enc_encode_ragged: the tensor-core encoder for the rows it covers, each other row alone on the CUDA-core encoder.
+        A row's codes do not depend on the rows it is batched with.  Runs on the current CUDA stream."""
+        if not self.has_encoder:
+            raise _lib.VcbError("this AudioTokenizer was built without encoder weights (enc.*)")
+        if len(wavs) == 0:
+            return []
+        B = len(wavs)
+        rates = list(sample_rate) if isinstance(sample_rate, (list, tuple)) else [sample_rate] * B
+        rates = [self.sample_rate if r is None else int(r) for r in rates]
+        rows = [mix_channels(torch.as_tensor(w).to(self._device, dtype=torch.float32), self.channels, f"prompt {i}")
+                for i, w in enumerate(wavs)]
+        if min(int(w.shape[1]) for w in rows) < 1:
+            raise _lib.VcbError("encode_many: an empty prompt")
+        for sr in sorted(set(rates) - {self.sample_rate}):           # one ragged resample per rate
+            idx = [i for i in range(B) if rates[i] == sr]
+            lens = [int(rows[i].shape[1]) for i in idx]
+            x = torch.zeros(len(idx), self.channels, max(lens), device=self._device, dtype=torch.float32)
+            for j, i in enumerate(idx):
+                x[j, :, :lens[j]] = rows[i]
+            o, n = resample_dims(sr, self.sample_rate)[:2]
+            y = self.resample(x, sr, lens=lens)
+            for j, i in enumerate(idx):
+                rows[i] = y[j, :, :-(-n * lens[j] // o)]
+        lens = [int(w.shape[1]) for w in rows]
+        N = max(lens)
+        wav = torch.zeros(B, self.channels, N, device=self._device, dtype=torch.float32)
+        for b, w in enumerate(rows):
+            wav[b, :, :lens[b]] = w
+        TN = self.frames(N)
+        codes = torch.empty(B, self.config.n_q, TN, device=self._device, dtype=torch.long)
+        frames = (C.c_int32 * B)()
+        eng = self._engine()
+        with torch.cuda.device(self._device):
+            _lib.check(_lib.load().enc_encode_ragged(eng, wav.data_ptr(), (C.c_int32 * B)(*lens), B, N, codes.data_ptr(), frames,
+                                                     torch.cuda.current_stream().cuda_stream))
+        return [codes[b:b + 1, :, :frames[b]] for b in range(B)]
+
     @torch.no_grad()
     def decode_codes(self, codes: torch.Tensor) -> torch.Tensor:
         """codes [B,K,T] int64 -> wav [B,channels,T*hop] fp32 (batched entry point used by bench.py)."""
@@ -553,19 +610,40 @@ def read_wav(path, offset: int = -1, num_frames: int = -1):
     return np.ascontiguousarray(pcm), sr
 
 
+def mix_channels(wav: torch.Tensor, channels: int, what="audio") -> torch.Tensor:
+    """[C, N] -> [channels, N] as convert_audio (data/tokenizer.py:85-95) mixes: mono or stereo in; the mean over the
+    channels for a mono codec or a multi-channel input, else the single channel broadcast."""
+    if wav.ndim != 2 or wav.shape[0] not in (1, 2):
+        raise ValueError(f"{what}: audio must be [channels, samples], mono or stereo; got shape {tuple(wav.shape)}")
+    if wav.shape[0] != channels:
+        wav = wav.mean(dim=0, keepdim=True).expand(channels, -1) if channels == 1 or wav.shape[0] > 1 \
+            else wav.expand(channels, -1)
+    return wav
+
+
 def tokenize_audio(tokenizer: AudioTokenizer, audio_path: str, offset=-1, num_frames=-1):
     """The reference's helper (data/tokenizer.py:137-149) without the torchaudio dependency: load a WAV file (read_wav;
     optionally the window of `num_frames` frames from `offset` at the file's rate), mix it to the codec's channel count
     and resample it to the codec's rate as convert_audio does (:85-97; AudioTokenizer.resample on the device), encode."""
     pcm, sr = read_wav(audio_path, offset, num_frames)
-    wav = torch.from_numpy(pcm)
-    if wav.shape[0] not in (1, 2):
-        raise ValueError(f"{audio_path}: audio must be mono or stereo, it has {wav.shape[0]} channels")
-    if wav.shape[0] != tokenizer.channels:                    # convert_audio (:85-95): down-mix / broadcast
-        wav = wav.mean(dim=0, keepdim=True).expand(tokenizer.channels, -1) if tokenizer.channels == 1 or wav.shape[0] > 1 \
-            else wav.expand(tokenizer.channels, -1)
-    wav = wav.unsqueeze(0)
+    wav = mix_channels(torch.from_numpy(pcm), tokenizer.channels, audio_path).unsqueeze(0)
     with torch.no_grad():
         if sr != tokenizer.sample_rate:
             wav = tokenizer.resample(wav.to(tokenizer.device), sr)
         return tokenizer.encode(wav)
+
+
+def tokenize_audio_many(tokenizer: AudioTokenizer, paths, offsets=None, num_frames=None):
+    """tokenize_audio over several WAV files in one encode: each file read (read_wav, optionally the window of
+    num_frames[i] frames from offsets[i] at its own rate), mixed to the codec's channels, resampled per rate on the device
+    and encoded with AudioTokenizer.encode_many -> list of codes [1, K, T_i].  Files at one rate are resampled together."""
+    n = len(paths)
+    offsets = [-1] * n if offsets is None else list(offsets)
+    num_frames = [-1] * n if num_frames is None else list(num_frames)
+    pcms = [read_wav(p, o, f) for p, o, f in zip(paths, offsets, num_frames)]
+    out = [None] * n
+    for sr in sorted({sr for _, sr in pcms}):
+        idx = [i for i in range(n) if pcms[i][1] == sr]
+        for i, codes in zip(idx, tokenizer.encode_many([torch.from_numpy(pcms[i][0]) for i in idx], sr)):
+            out[i] = codes
+    return out

@@ -1374,8 +1374,9 @@ class ContinuousBatcher:
     """
 
     def __init__(self, model: "VoiceCraft", max_concurrency=32, poll_every=8, top_k=-100, top_p=1.0, temperature=1.0,
-                 stop_repetition=3, silence_tokens=(1388, 1898, 131)):
+                 stop_repetition=3, silence_tokens=(1388, 1898, 131), tokenizer=None):
         self.model, self.B, self.poll_every = model, int(max_concurrency), max(1, int(poll_every))
+        self.tokenizer = tokenizer         # encodes the prompt audio of submit(audio=...) tickets
         self.defaults = dict(top_k=top_k, top_p=top_p, temperature=temperature, stop_repetition=stop_repetition,
                              silence_tokens=silence_tokens)
         self.queue = []
@@ -1383,9 +1384,14 @@ class ContinuousBatcher:
         self.results, self.errors = [], {}
         self._live = None                  # the running stream()'s state
 
-    def submit(self, x, y, seed=None, best_of=1, mask_interval=None, top_k=None, top_p=None, temperature=None,
-               stop_repetition=None, silence_tokens=None):
+    def submit(self, x, y=None, seed=None, best_of=1, mask_interval=None, top_k=None, top_p=None, temperature=None,
+               stop_repetition=None, silence_tokens=None, audio=None, sample_rate=None):
         """x [1,L] int64, y [1,T,K] int64 (host or device).  Returns the ticket (index into run()'s result list / results).
+        audio [channels, N] (instead of y): the prompt as audio at sample_rate (default: the codec's), encoded by the
+        constructor's tokenizer when the ticket is admitted, together with the other audio tickets admitted with it
+        (AudioTokenizer.encode_many; in stream() on the codec's CUDA stream).  The ticket then returns exactly what it
+        returns given ``y = tokenizer.encode_many([audio], sample_rate)[0].transpose(1, 2)``; an edit ticket's mask_interval
+        is in frames of that encoding.  Its size is known from the sample count, so admission never waits for the encoder.
         best_of: run() samples the utterance best_of times on consecutive slots and keeps the copy that ends first, as
         ``torch.manual_seed(seed); inference_tts_batch(x, ., y, batch_size=best_of)`` does; the copies count against
         max_concurrency.  stream() serves only best_of = 1.
@@ -1395,6 +1401,19 @@ class ContinuousBatcher:
         constructor's value (not inference's or inference_tts' own defaults).
         While a stream() runs, the utterance is admitted at one of its next polls; one that does not fit the engine it
         sized raises VcbError and is not queued."""
+        if (y is None) == (audio is None):
+            raise ValueError("submit takes exactly one of y (codes) and audio")
+        pending = None
+        if audio is not None:
+            tok = self.tokenizer
+            if tok is None or not tok.has_encoder:
+                raise _lib.VcbError("submit(audio=...) needs ContinuousBatcher(..., tokenizer=) with encoder weights (enc.*)")
+            audio = torch.as_tensor(audio)
+            if audio.ndim != 2 or audio.shape[1] < 1:
+                raise ValueError(f"audio must be [channels, samples], got {tuple(audio.shape)}")
+            # placeholder codes of the encoded length: the prompt's layout, positions and pages are those of the real ones
+            y = torch.zeros(1, tok.frames(int(audio.shape[1]), sample_rate), int(self.model.args.n_codebooks), dtype=torch.long)
+            pending = (x, audio, sample_rate)
         best_of = _check_best_of(best_of)
         if best_of > self.B:
             raise ValueError(f"best_of={best_of} copies do not fit max_concurrency={self.B} slots")
@@ -1417,13 +1436,13 @@ class ContinuousBatcher:
         st = self._live
         if st is not None:
             _no_stream_best_of(best_of)
-            job = self._job(x, y, seed, 1, spans, sp)
+            job = self._job(x, y, seed, 1, spans, sp, pending)
             if job[0].need_seq > st.max_seq:
                 raise _lib.VcbError(f"utterance needs {job[0].need_seq} positions, the streaming engine holds {st.max_seq}: "
                                     "configure_engine(max_seq_len=...) before stream()")
             st.jobs.append(job)
             self.results.append(None)
-        self.queue.append((x, y, seed, best_of, spans, sp))
+        self.queue.append((x, y, seed, best_of, spans, sp, pending))
         return len(self.queue) - 1
 
     def cancel(self, ticket) -> bool:
@@ -1437,16 +1456,41 @@ class ContinuousBatcher:
         st.cancelled.add(ticket)
         return True
 
-    def _job(self, x, y, seed, best_of, spans, sp):
-        """(prompt, seed, best_of, vcb_sampling) of a ticket; raises IndexError on an out-of-range id"""
+    def _job(self, x, y, seed, best_of, spans, sp, pending=None):
+        """(prompt, seed, best_of, vcb_sampling, pending audio) of a ticket; raises IndexError on an out-of-range id.  An
+        audio ticket's prompt holds placeholder codes until _encode replaces it; pending = (x, audio, sample_rate)."""
         p = _Prompt(self.model, x, y, spans)
         self.model._check_ids(p.x_ids, p.y_tok)
-        return p, seed, best_of, sp
+        return p, seed, best_of, sp, pending
 
-    def _admit(self, eng, new, jobs, stream):
+    def _encode(self, tickets, jobs, cstream=None):
+        """the prompt audio of the audio tickets among `tickets`, in one encode_many call, and their prompts rebuilt from
+        the codes.  cstream: encode there (the codec's stream, whose workspace the encoder
+        shares) and make the current stream wait for it."""
+        todo = [t for t in tickets if jobs[t][4] is not None]
+        if not todo:
+            return
+        tok, cur = self.tokenizer, torch.cuda.current_stream()
+        if cstream is not None:
+            cstream.wait_stream(cur)
+        with torch.cuda.stream(cstream if cstream is not None else cur):
+            codes = dict(zip(todo, tok.encode_many([jobs[t][4][1] for t in todo], [jobs[t][4][2] for t in todo])))
+        if cstream is not None:
+            cur.wait_stream(cstream)
+            for c in codes.values():
+                c.record_stream(cur)
+        for t in todo:
+            p, seed, best_of, sp, (x, _, _) = jobs[t]
+            real = _Prompt(self.model, x, codes[t].transpose(1, 2), p.spans)
+            assert real.need_seq == p.need_seq and real.total == p.total
+            jobs[t] = (real, seed, best_of, sp, None)
+
+    def _admit(self, eng, new, jobs, stream, cstream=None):
         """one packed prefill + the first sampling step of the newcomers [(first slot, ticket)], each with its ticket's
-        sampling parameters (every sampling call of the batcher passes sp = NULL)"""
+        sampling parameters (every sampling call of the batcher passes sp = NULL); the audio tickets among them are
+        encoded first (_encode)"""
         m, lib = self.model, _lib.load()
+        self._encode([t for _, t in new], jobs, cstream)
         seed0 = int(torch.cuda.default_generators[m.mask_embedding.device.index or 0].initial_seed())
         _prefill(eng, [(jobs[t][0], slot, jobs[t][2], seed0 + t if jobs[t][1] is None else jobs[t][1], 0, jobs[t][3])
                        for slot, t in new], stream)
@@ -1627,7 +1671,7 @@ class BatcherStream(_AudioStream):
                         free.discard(slot)
                         new.append((slot, c))
                     if new:
-                        cb._admit(st.eng, new, st.jobs, stream)
+                        cb._admit(st.eng, new, st.jobs, stream, st.cstream)
                         cids = [ids.pop(0) for _ in new]
                         st.codec.reset(cids)
                         for (slot, t), cid in zip(new, cids):
