@@ -1584,6 +1584,20 @@ int encode_chunk_tc(TcCodec* tc, const float* wav, long long wav_ld, const int* 
                 if (tc_launch(tc, mA, a1, g, c, st)) return -1;
                 ++*launches;
             }
+            // The epilogue zeroes halo row -t from output row t, 1 <= t <= halo, and a GEMM writes in.T rows (a strided
+            // conv ceil(L/r) of the chunk's longest utterance).  With constant padding an utterance may be shorter than a
+            // halo (rows of any length are taken), and a chunk of only such utterances writes no row t for some halo
+            // rows: they are cleared here, or they would keep whatever an earlier chunk left in the workspace.
+            if (L.kind != E_LSTM_STEPS && L.out >= 0 && pl.tensors[L.out].halo_kind == HALO_ZERO && !P[L.out].tm &&
+                in.T <= P[L.out].halo) {
+                const Plane& o = P[L.out];
+                for (__nv_bfloat16* base : {c.raw, c.elu}) {
+                    if (base == nullptr) continue;
+                    tc_pad_rows_kernel<<<B, 256, 0, st>>>(base, o.plane(), o.C, o.sb, o.st, o.off, nullptr, o.halo, 1, 1);
+                    VCB_CUDA_OK(cudaGetLastError());
+                    ++*launches;
+                }
+            }
         }
         pf.end();
     }
