@@ -1,13 +1,17 @@
-"""The tensor-core EnCodec decoder's layer plan (-m gpu): launch counts of a decode and of a stream decode, the carried
+"""The tensor-core EnCodec layer plans (-m gpu).  Decoder: launch counts of a decode and of a stream decode, the carried
 state per stream, the frames a fresh stream needs, and the tensors enc_debug_tensor exposes, with their dims.  The values
 were recorded on an H100 from the decoder as it was before its host side was driven by one plan; they pin the launches,
-the stream-state layout and min_T of every configuration below."""
+the stream-state layout and min_T of every configuration below.  Encoder: see test_encoder_plan_pinned."""
 import ctypes as C
+import json
+import os
 
 import pytest
 import torch
 
 from oracle import encodec_oracle as eo
+from test_encode_numerics import ENC_CONFIGS, enc_tensors, min_accepted
+from test_encode_numerics import hop as enc_hop
 
 SMALL = dict(n_filters=8, dimension=32, bins=64)
 B, T = 4, 100                 # one enc_decode
@@ -93,3 +97,69 @@ def test_codec_plan_pinned(name, monkeypatch):
         cs.decode(codes[:SB, :, :ST])
         torch.cuda.synchronize()
         assert lib.enc_counter(eng, b"launches") - n0 == n_stream
+
+
+# ---- the tensor-core encoder: one seeded ragged encode_many batch per configuration of test_encode_numerics, per knob
+ENC_KNOBS = {
+    "plain": {},
+    "lstm_wide": {"VCB_CODEC_LSTM_WIDE": "1"},
+    "ws_small": {"VCB_CODEC_WS_GB": "0.01"},   # a 10.7 MB workspace limit: chunks of one to three rows
+}
+ENC_CASES = [(c, k) for c in ENC_CONFIGS for k in ENC_KNOBS]
+
+
+def encoder_structure(name, knob, monkeypatch):
+    """(launches, encode_rows, tc_encodes, workspace bytes) of the batch with VCB_CODEC_KEEP off, the workspace bytes being
+    what the first encode of a fresh tokenizer adds to the process-wide live_bytes; then {enc.* name: (B, C, halo + rows,
+    halo)} of the last chunk with VCB_CODEC_KEEP=1"""
+    import gc
+
+    from voicecraft_b200 import _lib
+    from voicecraft_b200.tokenizer import AudioTokenizer
+    lib = _lib.load()
+    cfg = eo.default_config(**ENC_CONFIGS[name])
+    sd = eo.make_state_dict(cfg, seed=11, encoder=True)
+    g = torch.Generator().manual_seed(23)
+    lens = [min_accepted(cfg)] + torch.randint(min_accepted(cfg), 25 * enc_hop(cfg) + 1, (4,), generator=g).tolist()
+    wavs = [0.3 * torch.randn(1, n, generator=g) for n in lens]
+    for k, v in ENC_KNOBS[knob].items():
+        monkeypatch.setenv(k, v)
+    out = {}
+    for keep in ("0", "1"):
+        monkeypatch.setenv("VCB_CODEC_KEEP", keep)
+        gc.collect()
+        tok = AudioTokenizer(device="cuda:0", config=cfg, state_dict=sd)
+        eng = tok._engine()
+        assert lib.enc_counter(eng, b"tc_encoder") == 1
+        torch.cuda.synchronize()
+        live0 = lib.enc_counter(None, b"live_bytes")
+        counts0 = [lib.enc_counter(eng, c) for c in (b"launches", b"encode_rows", b"tc_encodes")]
+        tok.encode_many(wavs)
+        torch.cuda.synchronize()
+        if keep == "0":
+            out["launches"], out["encode_rows"], out["tc_encodes"] = \
+                [lib.enc_counter(eng, c) - c0 for c, c0 in zip((b"launches", b"encode_rows", b"tc_encodes"), counts0)]
+            out["ws_bytes"] = lib.enc_counter(None, b"live_bytes") - live0
+        else:
+            dims = {}
+            for t in enc_tensors(cfg):
+                for nm in (t["raw"], t["elu"]):
+                    if nm is not None:
+                        d = (C.c_int32 * 4)()
+                        assert lib.enc_debug_tensor(eng, nm.encode(), None, 0, d) == 0, nm
+                        dims[nm] = list(d)
+            out["dbg"] = dims
+        del tok, eng
+    return out
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name,knob", ENC_CASES)
+def test_encoder_plan_pinned(name, knob, monkeypatch):
+    """The encoder's launches, encode_rows (and so its chunking), tc_encodes, debug tensor dims and workspace bytes.  The
+    values in golden/encoder_plan.json were recorded on an H100 from the encoder as it was when it had a plan, a workspace
+    layout and an executor of its own, before it shared the decoder's; there the workspace bytes were checked to be
+    exactly its workspace layout of the largest chunk, and nothing else."""
+    with open(os.path.join(os.path.dirname(__file__), "golden", "encoder_plan.json")) as f:
+        pinned = json.load(f)[f"{name}/{knob}"]
+    assert encoder_structure(name, knob, monkeypatch) == pinned

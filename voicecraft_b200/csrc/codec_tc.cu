@@ -1,9 +1,10 @@
-// EnCodec SEANet decoder on the tensor cores (wgmma).
+// EnCodec SEANet decoder and encoder on the tensor cores (wgmma).
 //
-// Replaces, for the configurations it covers, the CUDA-core kernels of encodec.cu behind the same entry point
-// (enc_decode <- AudioTokenizer.decode, reference data/tokenizer.py:131-133 -> audiocraft EncodecModel.decode).
+// Replaces, for the configurations it covers, the CUDA-core kernels of encodec.cu behind the same entry points
+// (enc_decode <- AudioTokenizer.decode, reference data/tokenizer.py:131-133 -> audiocraft EncodecModel.decode;
+// enc_encode_ragged <- AudioTokenizer.encode_many).
 //
-// Every layer of the decoder is one launch of ONE kernel, an implicit GEMM with the time steps as the MMA M dimension:
+// Every GEMM layer is one launch of ONE kernel, an implicit GEMM with the time steps as the MMA M dimension:
 //
 //   activations  channels-last bf16 "planes": x ~= hi + lo (split_bf16), tensor [2 planes][rows][C], a row = one time step of
 //                one utterance, every utterance preceded by `halo` rows that hold its left padding (reflect or zero), so a
@@ -24,10 +25,14 @@
 //                800 steps x 2 layers = 1 600 dependent launches for the WHOLE batch (was: per 16 utterances), W_hh (16.8 MB
 //                as planes) stays in L2; chained with programmatic dependent launch, weights in flight before the wait.
 //
-// The encoder (enc_encode_ragged) runs on the same kernel from a plan of its own (EncPlan): input staging to 7-sample
-// windows (enc.conv_in = one k-block), the residual blocks as above, each strided conv (k = 2r, stride r) as a 2-tap conv
-// over the input read as folded rows [rows / r][r * C] with its per-utterance right padding written by tc_pad_rows_kernel,
-// the LSTM above, enc.conv_out to fp32 rows; the RVQ search stays the fp32 one of encodec.cu.
+// The encoder: input staging to 7-sample windows (enc.conv_in = one k-block), the residual blocks as above, each strided
+// conv (k = 2r, stride r) as a 2-tap conv over the input read as folded rows [rows / r][r * C] with its per-utterance right
+// padding written by tc_pad_rows_kernel, the LSTM above, enc.conv_out to fp32 rows; the RVQ search stays the fp32 one of
+// encodec.cu.
+//
+// Host side: each direction is one Plan (tensors, layers with their GEMMs, fp32 buffers) built by walking the model once
+// (build_dec / build_enc); ws_layout derives a chunk's workspace from it and run_chunk every launch.  A GEMM whose K does not
+// fit the kernel's k-blocks makes the configuration not covered.
 #include "codec_tc.h"
 
 #include <algorithm>
@@ -573,85 +578,70 @@ struct Plane {                         // an activation tensor in the workspace
     int Tp = 0, halo = 0, halo_zero = 0, T = 0, tm = 0;
     long long plane() const { return static_cast<long long>(rcap) * C; }
 };
+struct Dbg { Plane p; const __nv_bfloat16* ptr; int B; };   // a tensor of the last chunk (debug read-back)
 
-// ---- the decoder plan: the layer sequence over a table of tensors, independent of (B, T).  The launches, the workspace,
-// the stream-state layout and min_T are all derived from it.
+// ---- the layer plan of one direction: the layer sequence over a table of tensors, independent of the chunk.  The GEMMs,
+// the launches and the workspace are derived from it, and for the decoder the stream-state layout and min_T.
+//
+// A tensor belongs to a stage: the chunk's plane rows per utterance of every stage are one vector (decoder: T * the product
+// of the ratios so far; encoder: each stage's length, rounded up to its strided conv's stride, from the samples to the
+// frames).  Utterance-major, every utterance holds `halo` rows of left padding and then its rows; the input of an encoder
+// strided conv (stride r) is read as folded rows [rows / r][r * C] (fold = r) and gets its right padding from L_RPAD.
 enum { FORM_RAW = 1, FORM_ELU = 2 };
 // HALO_UNWRITTEN: the rows exist (the tensor shares its block input's row geometry) but nothing stores or reads them
 enum { HALO_REFLECT, HALO_ZERO, HALO_UNWRITTEN };
-enum { HOME_ARENA0, HOME_ARENA1, HOME_HIDDEN, HOME_FIXED };   // ping-pong arenas of the stages, hidden arena, fixed region
 
-struct PlanTensor {
+struct Tensor {
     int C = 0, halo = 0, halo_kind = HALO_ZERO;
-    int up = 1;                        // rows per frame: the product of the ratios so far
+    int stage = 0, fold = 1;
     bool tm = false;                   // time-major, row = (t + halo) * Bcap + b (LSTM planes); else utterance-major
     int forms = 0;                     // FORM_RAW | FORM_ELU stored
-    int home = HOME_FIXED;
-    bool carried = false;              // stream decode carries its halo rows (of the ELU'd form if stored, else raw) ...
+    int arena = -1, group = 0;         // -1: own rows; else an arena, where the tensors of one group stack (see ws_layout)
+    bool carried = false;              // decoder stream: its halo rows (of the ELU'd form if stored, else raw) are carried ...
     size_t state_off = 0;              // ... at this offset of a stream's state
     std::string dbg_raw, dbg_elu;      // enc_debug_tensor names of the two forms ("": not exposed)
 };
 
-enum { L_RVQ, L_CONV, L_LSTM_IH, L_LSTM_STEPS, L_CONV_OUT_SPLIT, L_CONV_OUT };
+// L_RPAD: the right padding of a strided conv's input over the stage's length table; L_LPAD: a left halo no producer writes
+enum { L_RVQ, L_INPUT, L_RPAD, L_LPAD, L_CONV, L_LSTM_IH, L_LSTM_STEPS, L_CONV_OUT_SPLIT, L_CONV_OUT };
 enum { F32_NONE, F32_X0, F32_PRE, F32_COPART, F32_WAV, F32_LAT };   // fp32 destination of a GEMM
+// the workspace's fp32 buffers: LSTM input, pre-activations and cells; the decoder's final-conv partial products; the
+// encoder's latent rows, latent [B][D][T], RVQ scores and codes, per-utterance table
+enum { BUF_X0, BUF_PRE, BUF_CST, BUF_COPART, BUF_LATF, BUF_LAT, BUF_SCORES, BUF_CODES, BUF_TAB, NBUF };
 
-struct PlanLayer {
+struct Layer {
     int kind = L_CONV;
-    const char* label = "";            // VCB_CODEC_PROFILE
+    std::string label;                 // VCB_CODEC_PROFILE
     const TcGemm* g = nullptr;
     int in = -1, in_form = FORM_RAW;   // A source 0
     int in2 = -1;                      // A source 1, raw form: the block input of a residual tail (shortcut)
-    int out = -1, out_forms = 0;
+    int out = -1;                      // stores every form the tensor has
     int f32 = F32_NONE;
     int nstore = 0;                    // GEMM columns stored
     int lstm = -1;                     // LSTM layer
-    size_t h_off = 0, c_off = 0;       // LSTM steps: the layer's carried h and c in a stream's state
+    size_t h_off = 0, c_off = 0;       // decoder stream: the layer's carried h and c in a stream's state
 };
 
-struct PlanStage { int up, C, Ch; };   // rows per frame, padded channels of the block tensors and of the hidden tensor
-
-// ---- the encoder plan (SEANetEncoder, oracle/encodec_oracle.py::encoder_plan), over a table of tensors like the decoder's.
-// A tensor belongs to a stage s (its rows are frames of stage s: the input's samples for s = 0, then one stage per strided
-// conv) and holds, per utterance, `halo` rows of left padding and the stage's rows rounded up to the next strided conv's
-// stride.  The input of a strided conv (stride r) has halo r and is read as folded rows [rows / r][r * C] (fold = r).
-enum { E_INPUT, E_CONV, E_DOWN, E_RPAD, E_LSTM_IH, E_LSTM_STEPS, E_LPAD, E_CONV_OUT };
-
-struct EncTensor {
-    int C = 0, halo = 0, halo_kind = HALO_ZERO, stage = 0, fold = 1;
-    bool tm = false;                   // time-major (LSTM planes)
-    int forms = 0, home = HOME_FIXED;  // home: HOME_FIXED or the arena of its stage (HOME_ARENA0 + stage % 2)
-    std::string dbg_raw, dbg_elu;
-};
-
-struct EncLayer {
-    int kind = E_CONV;
-    const char* label = "";
-    const TcGemm* g = nullptr;
-    int in = -1, in_form = FORM_RAW, in2 = -1, out = -1, out_forms = 0, f32 = F32_NONE, nstore = 0, lstm = -1;
-    int stage = 0, r = 1;              // E_DOWN / E_RPAD: the stage and stride of the strided conv
-};
-
-struct EncPlan {
-    std::vector<EncTensor> tensors;
-    std::vector<EncLayer> layers;
-    std::vector<int> ratios;           // stride of stage s's strided conv (the config's ratios reversed)
-};
-
-struct TcEncoder {
-    TcGemm conv_in, conv_out;
-    std::vector<TcGemm> down, pre, step;
-    std::vector<std::vector<TcGemm>> res1, res2;
-    EncPlan plan;
-};
-
-struct TcPlan {
-    std::vector<PlanTensor> tensors;
-    std::vector<PlanLayer> layers;
-    std::vector<PlanStage> stages;
-    int u0 = -1;                       // input of the first ConvTranspose (its zero halo is cleared before every chunk)
-    int arena_halo = 1;                // halo rows every arena is sized for
+struct Plan {
+    std::vector<Tensor> tensors;
+    std::vector<Layer> layers;
+    std::vector<std::unique_ptr<TcGemm>> gemms;   // the layers' weights (a layer's pointer stays valid as more are added)
+    std::vector<int> bufs;             // the fp32 buffers the layers use, in workspace order
+    int top = 0;                       // the stage of the LSTM and the latent frames
+    std::vector<int> up;               // decoder: plane rows per frame of every stage
+    std::vector<int> ratios;           // encoder: stride of stage s's strided conv (the config's ratios reversed)
+    int u0 = -1;                       // decoder: input of the first ConvTranspose (its zero halo is cleared before every chunk)
     int min_T = 8;
-    size_t stream_bytes = 0;           // carried state of one stream
+    size_t stream_bytes = 0;           // decoder: carried state of one stream
+    std::map<std::string, Dbg> dbg;    // the tensors of the last chunk by debug name
+
+    TcGemm& gemm() { return *gemms.emplace_back(std::make_unique<TcGemm>()); }
+    Layer& layer(int kind, std::string label, const TcGemm* g, int nstore, int in, int in_form, int out, int f32) {
+        Layer& L = layers.emplace_back();
+        L.kind = kind; L.label = std::move(label); L.g = g; L.nstore = nstore;
+        L.in = in; L.in_form = in_form; L.out = out; L.f32 = f32;
+        return L;
+    }
 };
 
 }  // namespace
@@ -660,24 +650,15 @@ struct TcCodec {
     enc_config cfg;
     int hop = 1, D = 0, Dp = 0, ch0 = 0, num_sms = 132;
     DevBuf<const float*> d_embed;
-    TcGemm conv_in, conv_out;
-    TcGemm conv_out_p;                 // final conv as per-tap partial products (N = k), summed by tc_diag_sum_kernel
-    bool co_split = false;
-    float co_bias = 0.f;
-    std::vector<TcGemm> pre, step, up; // step: 64-column tiles, or 128 with VCB_CODEC_LSTM_WIDE=1
-    std::vector<std::vector<TcGemm>> res1, res2;
-    TcPlan plan;
+    float co_bias = 0.f;               // bias of the split final conv, added by tc_diag_sum_kernel
+    Plan dec;
+    std::unique_ptr<Plan> enc;         // tensor-core encoder; null: no encoder weights, or not covered
     DevBuf<uint8_t> ws;
     size_t ws_limit = 0;
     bool profile = false;
-    bool keep = false;                 // VCB_CODEC_KEEP=1: every plan tensor has its own rows, so all survive a decode
+    bool keep = false;                 // VCB_CODEC_KEEP=1: every plan tensor has its own rows, so all survive a chunk
     std::vector<std::pair<std::string, float>> prof;
-    struct Dbg { Plane p; const __nv_bfloat16* ptr; int B; };
-    std::map<std::string, Dbg> dbg;      // tensors of the last decoded chunk (debug read-back)
-    std::map<std::string, Dbg> edbg;     // tensors of the last encoded chunk ("enc.*")
-    std::unique_ptr<TcEncoder> enc;      // tensor-core encoder; null: no encoder weights or not covered (enc_reason)
-    const char* enc_reason = "encoder weights (enc.*) not loaded";
-    const float* dbg_cst = nullptr;      // its final LSTM cell states [layers][dbg_Bcap][ch0] ("c0", "c1", ...)
+    const float* dbg_cst = nullptr;    // the last decoded chunk's final LSTM cell states [layers][dbg_Bcap][ch0] ("c0", ...)
     int dbg_B = 0, dbg_Bcap = 0;
 };
 
@@ -685,8 +666,10 @@ namespace {
 
 inline int tc_num_sms(const TcCodec* tc) { return tc->num_sms; }
 
+// 0: uploaded; 1: K is outside the kernel's k-blocks (the configuration is not covered); -1: error
 int upload_gemm(TcGemm& g, const std::vector<float>& W, const std::vector<float>& bias, int N, int Ktot, int bn_hint) {
-    if (Ktot % TC_BK || Ktot / TC_BK > TC_MAX_KB) {
+    if (Ktot < TC_BK || Ktot > TC_MAX_KB * TC_BK) return 1;
+    if (Ktot % TC_BK) {
         set_error("codec_tc: K = %d outside the kernel's range", Ktot);
         return -1;
     }
@@ -846,12 +829,12 @@ int plane_map(CUtensorMap* tm, const __nv_bfloat16* base, const Plane& p) {
 
 inline int bcap(int B) { return (B + 127) / 128 * 128; }
 
-// a plan tensor's rows for a chunk of B utterances of T frames: utterance-major, every utterance = halo rows + its rows; or
-// time-major, row = (t + halo) * Bcap + b
-Plane geometry(const PlanTensor& t, int B, int T) {
+// a plan tensor's rows for a chunk of B utterances with plane rows R per stage: utterance-major, every utterance = halo rows +
+// its rows; or time-major, row = (t + halo) * Bcap + b
+Plane geometry(const Tensor& t, int B, const std::vector<int>& R) {
     Plane p;
     p.C = t.C;
-    p.T = T * t.up;
+    p.T = R[t.stage];
     p.Tp = p.T + t.halo;
     p.halo = t.halo;
     p.halo_zero = t.halo_kind == HALO_ZERO;
@@ -863,7 +846,7 @@ Plane geometry(const PlanTensor& t, int B, int T) {
         p.st = Bc;
         p.off = static_cast<long long>(t.halo) * Bc;
     } else {
-        p.rcap = std::max(B * p.Tp, TC_BM);               // (a TMA box never taller than its tensor)
+        p.rcap = std::max(B * p.Tp, TC_BM * t.fold);     // (whole folded rows; a TMA box never taller than its tensor)
         p.sb = p.Tp;
         p.st = 1;
         p.off = t.halo;
@@ -899,354 +882,9 @@ struct Prof {
     }
 };
 
-// The decoder's layers in launch order.  Every halo rule is here: a causal convolution reads (k-1)*dilation rows above its
-// output row, so its input keeps that many halo rows, padded like the reference (reflect or zeros); a ConvTranspose reads
-// x[t-1], so its input keeps one zero row.  A stream's state holds the carried tensors and the LSTM (h, c) per layer, in
-// the order the carries run.
-void build_plan(TcCodec* tc) {
-    const enc_config& cf = tc->cfg;
-    TcPlan& pl = tc->plan;
-    const int H = tc->ch0, nl = cf.lstm, nres = cf.n_residual_layers;
-    const int kres = cf.residual_kernel_size, kout = cf.last_kernel_size;
-    const int pad = cf.pad_reflect ? HALO_REFLECT : HALO_ZERO;
-    auto tensor = [&](int C, int halo, int kind, int up, bool tm, int forms, int home, bool carried, std::string dbg_raw,
-                      std::string dbg_elu) {
-        PlanTensor t;
-        t.C = C; t.halo = halo; t.halo_kind = kind; t.up = up; t.tm = tm;
-        t.forms = forms; t.home = tc->keep ? HOME_FIXED : home; t.carried = carried;
-        t.dbg_raw = std::move(dbg_raw);
-        t.dbg_elu = std::move(dbg_elu);
-        pl.tensors.push_back(t);
-        return static_cast<int>(pl.tensors.size()) - 1;
-    };
-    auto layer = [](int kind, const char* label, const TcGemm* g, int nstore, int in, int in_form, int out, int out_forms, int f32) {
-        PlanLayer L;
-        L.kind = kind; L.label = label; L.g = g; L.nstore = nstore;
-        L.in = in; L.in_form = in_form; L.out = out; L.out_forms = out_forms; L.f32 = f32;
-        return L;
-    };
-    auto add = [&](PlanLayer L) {
-        if (L.kind == L_LSTM_STEPS) {
-            L.h_off = pl.stream_bytes;
-            L.c_off = pl.stream_bytes + static_cast<size_t>(H) * 4;
-            pl.stream_bytes += static_cast<size_t>(H) * 8;
-        }
-        if (L.out >= 0) {
-            PlanTensor& t = pl.tensors[L.out];
-            if (t.carried && t.halo > 0) {
-                t.state_off = pl.stream_bytes;
-                pl.stream_bytes += static_cast<size_t>(t.halo) * t.C * 4;
-            }
-        }
-        pl.layers.push_back(L);
-    };
-    // the input of a ConvTranspose, or of the final conv after the last stage
-    auto feed = [&](bool last_stage, int& halo, int& kind) {
-        halo = last_stage ? kout - 1 : 1;
-        kind = last_stage ? pad : HALO_ZERO;
-    };
-
-    const int z = tensor(tc->Dp, cf.kernel_size - 1, pad, 1, false, FORM_RAW, HOME_FIXED, true, "z", "");
-    pl.u0 = tensor(cpad(H), 1, HALO_ZERO, 1, false, FORM_ELU, HOME_FIXED, true, "", "u0");
-    int x0 = -1, hs[2] = {-1, -1};
-    if (nl > 0) {
-        x0 = tensor(H, 0, HALO_ZERO, 1, true, FORM_RAW, HOME_FIXED, false, "x0", "");
-        for (int l = 0; l < std::min(nl, 2); ++l)                 // h planes: slot t+1 = h_t, layers alternate
-            hs[l] = tensor(H, 1, HALO_ZERO, 1, true, FORM_RAW, HOME_FIXED, false, "hs" + std::to_string(l), "");
-    }
-    add(layer(L_RVQ, "rvq", nullptr, 0, -1, 0, z, FORM_RAW, F32_NONE));
-    if (nl > 0) add(layer(L_CONV, "conv_in", &tc->conv_in, cpad(H), z, FORM_RAW, x0, FORM_RAW, F32_X0));
-    else add(layer(L_CONV, "conv_in", &tc->conv_in, cpad(H), z, FORM_RAW, pl.u0, FORM_ELU, F32_NONE));
-    for (int l = 0; l < nl; ++l) {
-        PlanLayer ih = layer(L_LSTM_IH, "lstm_ih", &tc->pre[l], 4 * H, l == 0 ? x0 : hs[(l - 1) & 1], FORM_RAW, -1, 0, F32_PRE);
-        ih.lstm = l;
-        add(ih);
-        // the last layer's epilogue writes ELU(h + skip) straight into the first ConvTranspose's input
-        const bool last = l == nl - 1;
-        PlanLayer steps = layer(L_LSTM_STEPS, "lstm_steps", &tc->step[l], 4 * H, hs[l & 1], FORM_RAW, last ? pl.u0 : -1,
-                                last ? FORM_ELU : 0, F32_NONE);
-        steps.lstm = l;
-        add(steps);
-    }
-    // up-sampling stages: ConvTranspose -> X; per residual block conv1 (on ELU(X)) -> hidden, then conv2 (on the hidden) +
-    // shortcut (on raw X) -> O, the next block's X.  X and O alternate between the two arenas.
-    int cur = pl.u0, ch = H, up = 1, side = HOME_ARENA0;
-    for (int i = 0; i < cf.n_ratios; ++i) {
-        const int r = cf.ratios[i], cout = ch / 2, hidden = cout / cf.compress;
-        const bool last_stage = i == cf.n_ratios - 1;
-        const std::string s = std::to_string(i + 1);
-        ch = cout;
-        up *= r;
-        pl.stages.push_back(PlanStage{up, cpad(cout), cpad(hidden)});
-        int halo = kres - 1, kind = pad;
-        if (nres == 0) feed(last_stage, halo, kind);
-        int x = tensor(cpad(cout), halo, kind, up, false, (nres > 0 ? FORM_RAW : 0) | FORM_ELU, side, true,
-                       nres > 0 ? "x" + s + ".raw" : "", "x" + s + ".elu");
-        add(layer(L_CONV, "convtr", &tc->up[i], r * cpad(cout), cur, FORM_ELU, x, pl.tensors[x].forms, F32_NONE));
-        for (int j = 0, dil = 1; j < nres; ++j, dil *= cf.dilation_base) {
-            const std::string sj = s + "." + std::to_string(j);
-            const int hd = tensor(cpad(hidden), pl.tensors[x].halo, HALO_UNWRITTEN, up, false, FORM_ELU, HOME_HIDDEN, false, "",
-                                  "h" + sj);
-            add(layer(L_CONV, "res_conv1", &tc->res1[i][j], cpad(hidden), x, FORM_ELU, hd, FORM_ELU, F32_NONE));
-            // the next block's conv1 reads (kres-1) * its dilation rows back.  min_T takes this term for the last block too.
-            const int next = (kres - 1) * dil * cf.dilation_base;
-            pl.min_T = std::max(pl.min_T, next + 2);
-            halo = next;
-            kind = pad;
-            if (j == nres - 1) feed(last_stage, halo, kind);
-            const int o = tensor(cpad(cout), halo, kind, up, false, (j < nres - 1 ? FORM_RAW : 0) | FORM_ELU, side ^ 1, true,
-                                 j < nres - 1 ? "o" + sj + ".raw" : "", "o" + sj);
-            PlanLayer tail = layer(L_CONV, "res_conv2", &tc->res2[i][j], cpad(cout), hd, FORM_ELU, o, pl.tensors[o].forms, F32_NONE);
-            tail.in2 = x;
-            add(tail);
-            x = o;
-            side ^= 1;
-        }
-        cur = x;
-        side ^= 1;                                                 // the next ConvTranspose must not write over `cur`
-    }
-    // final conv: k <= DS_LD partial products (the first 16-column chunk), or one output column (f_valid = 1)
-    if (tc->co_split) add(layer(L_CONV_OUT_SPLIT, "conv_out", &tc->conv_out_p, 16, cur, FORM_ELU, -1, 0, F32_COPART));
-    else add(layer(L_CONV_OUT, "conv_out", &tc->conv_out, 32, cur, FORM_ELU, -1, 0, F32_WAV));
-    pl.min_T = std::max(pl.min_T, std::max(cf.kernel_size, kout) + 1);
-    for (const PlanTensor& t : pl.tensors)
-        if (t.home != HOME_FIXED) pl.arena_halo = std::max(pl.arena_halo, t.halo);
-}
-
-// The workspace of a chunk: the fixed tensors, the fp32 buffers, the two stage arenas, the hidden arena, the final conv's
-// partial products.  tensor[i] = offset of plan tensor i's first stored form (an ELU'd form follows a raw one).
-struct WsLayout {
-    std::vector<size_t> tensor;
-    size_t x0f = 0, pre = 0, cst = 0, copart = 0, bytes = 0;
-};
-
-WsLayout ws_layout(const TcCodec* tc, int B, int T) {
-    const TcPlan& pl = tc->plan;
-    const int Bcap = bcap(B), H = tc->ch0, nl = tc->cfg.lstm;
-    WsLayout w;
-    w.tensor.resize(pl.tensors.size());
-    size_t off = 0;
-    auto take = [&](size_t bytes) {
-        const size_t o = off;
-        off += align_up(bytes, 1024);
-        return o;
-    };
-    for (size_t i = 0; i < pl.tensors.size(); ++i) {
-        const PlanTensor& t = pl.tensors[i];
-        if (t.home != HOME_FIXED) continue;
-        w.tensor[i] = off;
-        for (int f : {FORM_RAW, FORM_ELU})
-            if (t.forms & f) take(form_bytes(geometry(t, B, T)));
-    }
-    if (nl > 0) {
-        w.x0f = take(static_cast<size_t>(T) * Bcap * H * 4);
-        w.pre = take(static_cast<size_t>(T) * Bcap * 4 * H * 4);
-        w.cst = take(static_cast<size_t>(nl) * Bcap * H * 4);
-    }
-    size_t ax = 0, ah = 0;
-    for (const PlanStage& s : pl.stages) {
-        const size_t rows = static_cast<size_t>(B) * (T * s.up + pl.arena_halo);
-        ax = std::max(ax, align_up(rows * s.C * 4, 1024) * 2);
-        ah = std::max(ah, align_up(rows * s.Ch * 4, 1024));
-    }
-    const size_t region[3] = {take(ax), take(ax), take(ah)};
-    for (size_t i = 0; i < pl.tensors.size(); ++i)
-        if (pl.tensors[i].home != HOME_FIXED) w.tensor[i] = region[pl.tensors[i].home];
-    if (tc->co_split) {
-        const PlanTensor& in = pl.tensors[pl.layers.back().in];
-        w.copart = take((static_cast<size_t>(B) * (T * in.up + std::max(in.halo, 1)) + TC_BM) * DS_LD * 4);
-    }
-    w.bytes = off;
-    return w;
-}
-
-// One chunk of B utterances.  sc = stream decode: every plane a layer reads as left context, and the LSTM state, continue
-// the utterance's stream (tc_carry_kernel).
-int decode_chunk_tc(TcCodec* tc, const int64_t* codes, float* wav, int B, int T, cudaStream_t st, int64_t* launches,
-                    const TcStreamCtx* sc) {
-    const TcPlan& pl = tc->plan;
-    const enc_config& cf = tc->cfg;
-    const int Bcap = bcap(B), H = tc->ch0, nl = cf.lstm;
-    const WsLayout w = ws_layout(tc, B, T);
-    std::vector<Plane> P(pl.tensors.size());
-    tc->dbg.clear();
-    for (size_t i = 0; i < P.size(); ++i) {
-        const PlanTensor& t = pl.tensors[i];
-        Plane& p = P[i];
-        p = geometry(t, B, T);
-        uint8_t* base = tc->ws + w.tensor[i];
-        if (t.forms & FORM_RAW) {
-            p.raw = reinterpret_cast<__nv_bfloat16*>(base);
-            base += align_up(form_bytes(p), 1024);
-        }
-        if (t.forms & FORM_ELU) p.elu = reinterpret_cast<__nv_bfloat16*>(base);
-        if (!t.dbg_raw.empty()) tc->dbg[t.dbg_raw] = TcCodec::Dbg{p, p.raw, B};
-        if (!t.dbg_elu.empty()) tc->dbg[t.dbg_elu] = TcCodec::Dbg{p, p.elu, B};
-    }
-    float* x0f = reinterpret_cast<float*>(tc->ws + w.x0f);
-    float* pre = reinterpret_cast<float*>(tc->ws + w.pre);
-    float* cst = reinterpret_cast<float*>(tc->ws + w.cst);
-    float* copart = reinterpret_cast<float*>(tc->ws + w.copart);
-    tc->dbg_cst = nl > 0 ? cst : nullptr;
-    tc->dbg_B = B;
-    tc->dbg_Bcap = Bcap;
-
-    // state that the kernels only ever read: U0's zero halo (the LSTM epilogue writes none), c_0 and h_{-1}
-    const Plane& u0 = P[pl.u0];
-    VCB_CUDA_OK(cudaMemset2DAsync(u0.elu, static_cast<size_t>(u0.Tp) * u0.C * 2, 0, static_cast<size_t>(u0.C) * 2, B, st));
-    VCB_CUDA_OK(cudaMemset2DAsync(u0.elu + u0.plane(), static_cast<size_t>(u0.Tp) * u0.C * 2, 0, static_cast<size_t>(u0.C) * 2, B, st));
-    auto clear_h0 = [&](const Plane& hs) -> int {
-        VCB_CUDA_OK(cudaMemsetAsync(hs.raw, 0, static_cast<size_t>(Bcap) * H * 2, st));
-        VCB_CUDA_OK(cudaMemsetAsync(hs.raw + hs.plane(), 0, static_cast<size_t>(Bcap) * H * 2, st));
-        return 0;
-    };
-    if (nl > 0) {
-        VCB_CUDA_OK(cudaMemsetAsync(cst, 0, static_cast<size_t>(nl) * Bcap * H * 4, st));
-        for (const PlanLayer& L : pl.layers)
-            if (L.kind == L_LSTM_STEPS && L.lstm < 2 && clear_h0(P[L.in])) return -1;
-    }
-
-    auto carry = [&](void* base, long long plane_bytes, long long sb, long long stt, long long off, int row_bytes, int halo, int up,
-                     int restore, int save, size_t state_off) -> int {
-        const CarryArgs a{static_cast<uint8_t*>(base), plane_bytes, sb, stt, off, row_bytes, halo, up, restore, save, sc->table,
-                          sc->state, static_cast<long long>(pl.stream_bytes), static_cast<long long>(state_off)};
-        VCB_CUDA_OK(launch_k_pdl(1, tc_carry_kernel, dim3(B), dim3(256), 0, st, a));
-        ++*launches;
-        return 0;
-    };
-    // a plane's halo: restore a continuing stream's tail over the padding the producer wrote, save the new tail
-    auto carry_plane = [&](int i) -> int {
-        const PlanTensor& t = pl.tensors[i];
-        const Plane& p = P[i];
-        if (sc == nullptr || !t.carried || p.halo == 0) return 0;
-        return carry(p.elu ? p.elu : p.raw, p.plane() * 2, p.sb, p.st, p.off, p.C * 2, p.halo, t.up, 1, 1, t.state_off);
-    };
-    // stream decode: h_{-1} (slot 0) and c continue the stream; after the layer, h of the last valid step (slot frames) and
-    // the frozen c are saved.  As a time-major plane with one halo row, row(b, t) = (t + 1) * Bcap + b.
-    auto carry_lstm = [&](const PlanLayer& L, const Plane& hs, float* cl, int restore, int save) -> int {
-        if (sc == nullptr) return 0;
-        return carry(hs.raw, hs.plane() * 2, hs.sb, hs.st, hs.off, H * 2, 1, 1, restore, save, L.h_off) ||
-               carry(cl, 0, 1, 0, 0, H * 4, 1, 1, restore, save, L.c_off);
-    };
-    // the call of a plan GEMM: its weights, its A rows, its epilogue (the LSTM steps then only move t_step and row_base)
-    auto gemm_call = [&](const PlanLayer& L, TcCall& c) -> int {
-        const TcGemm& g = *L.g;
-        const Plane& in = P[L.in];
-        c = TcCall{};
-        c.mtiles = ((L.kind == L_LSTM_STEPS ? B : in.rcap) + TC_BM - 1) / TC_BM;
-        if (static_cast<long long>(c.mtiles) * g.ntiles > 0x7fffffffll) {
-            set_error("codec_tc: too many tiles");
-            return -1;
-        }
-        c.total_kb = g.total_kb;
-        c.ntiles = g.ntiles;
-        c.bias = g.bias;
-        c.up = g.up;
-        c.Cout = g.Cout;
-        std::copy(g.taps.begin(), g.taps.end(), c.taps);
-        c.Nstore = L.nstore;
-        c.rows_total = in.rcap;
-        c.rcap[0] = in.rcap;
-        c.B = B;
-        if (L.kind != L_LSTM_STEPS) {
-            c.in_tm = in.tm;
-            c.in_div = in.tm ? static_cast<int>(in.st) : in.Tp;
-            c.in_halo = in.halo;
-            c.T_in = in.T;
-        }
-        if (L.in2 >= 0) c.rcap[1] = P[L.in2].rcap;
-        if (L.out >= 0) {
-            const Plane& o = P[L.out];
-            c.raw = L.out_forms & FORM_RAW ? o.raw : nullptr;
-            c.elu = L.out_forms & FORM_ELU ? o.elu : nullptr;
-            c.o_plane = o.plane();
-            c.o_ld = o.C;
-            c.o_sb = o.sb;
-            c.o_st = o.st;
-            c.o_off = o.off;
-            c.o_halo = pl.tensors[L.out].halo_kind == HALO_UNWRITTEN ? 0 : o.halo;
-            c.o_halo_zero = o.halo_zero;
-        }
-        auto rows = [&](float* f, int ld, long long sb, long long stt, long long off) {
-            c.f32 = f;
-            c.f_ld = ld;
-            c.f_valid = ld;
-            c.f_sb = sb;
-            c.f_st = stt;
-            c.f_off = off;
-        };
-        if (L.f32 == F32_X0) rows(x0f, H, 1, Bcap, 0);                // time-major [T][Bcap][H]
-        if (L.f32 == F32_PRE) rows(pre, 4 * H, 1, Bcap, 0);           // time-major [T][Bcap][4H]
-        if (L.f32 == F32_COPART) {                                    // the input's rows, halo included
-            rows(copart, DS_LD, in.sb, 1, in.off);
-            c.in_store_halo = 1;
-        }
-        if (L.f32 == F32_WAV) {                                       // [B][T * hop]
-            rows(wav, 1, in.T, 1, 0);
-            c.f_scalar = 1;
-        }
-        if (L.kind == L_LSTM_STEPS) {
-            c.mode = TC_MODE_LSTM;
-            c.pre = pre;
-            c.cst = cst + static_cast<size_t>(L.lstm) * Bcap * H;
-            c.hseq = in.raw;
-            c.h_plane = in.plane();
-            c.Bcap = Bcap;
-            c.H = H;
-            if (L.out >= 0) c.skip = x0f;
-            if (sc != nullptr) c.stab = sc->table;
-        }
-        return 0;
-    };
-
-    Prof pf{tc, st};
-    CUtensorMap mA, mB;
-    TcCall c;
-    for (const PlanLayer& L : pl.layers) {
-        pf.begin(L.label);
-        if (L.kind == L_RVQ) {
-            const Plane& z = P[L.out];
-            tc_rvq_planes_kernel<<<dim3((T + 15) / 16, B), 128, 0, st>>>(reinterpret_cast<const long long*>(codes), tc->d_embed, z.raw,
-                                                                         z.plane(), cf.n_q, tc->D, z.C, T, z.Tp, z.halo, z.halo_zero);
-            VCB_CUDA_OK(cudaGetLastError());
-            ++*launches;
-        } else {
-            const Plane& in = P[L.in];
-            if (gemm_call(L, c) || plane_map(&mA, L.in_form == FORM_ELU ? in.elu : in.raw, in) ||
-                (L.in2 >= 0 && plane_map(&mB, P[L.in2].raw, P[L.in2])))
-                return -1;
-            const CUtensorMap& a1 = L.in2 >= 0 ? mB : mA;
-            if (L.kind == L_LSTM_STEPS) {
-                if (L.lstm >= 2 && clear_h0(in)) return -1;
-                if (carry_lstm(L, in, c.cst, 1, 0)) return -1;
-                for (int t = 0; t < T; ++t) {
-                    c.t_step = t;
-                    c.row_base = t * Bcap;
-                    if (tc_launch(tc, mA, a1, *L.g, c, st)) return -1;
-                }
-                *launches += T;
-                if (carry_lstm(L, in, c.cst, 0, 1)) return -1;
-            } else {
-                if (tc_launch(tc, mA, a1, *L.g, c, st)) return -1;
-                ++*launches;
-            }
-            if (L.kind == L_CONV_OUT_SPLIT) {
-                VCB_CUDA_OK(launch_k_pdl(1, tc_diag_sum_kernel, dim3((in.rcap + DS_ROWS - 1) / DS_ROWS), dim3(DS_ROWS), 0, st,
-                                         copart, cf.last_kernel_size, tc->co_bias, wav, in.rcap, in.Tp, in.halo, in.T, B));
-                ++*launches;
-            }
-        }
-        if (L.out >= 0 && carry_plane(L.out)) return -1;
-        pf.end();
-    }
-    pf.finish();
-    return 0;
-}
-
-// ---- encoder ---------------------------------------------------------------------------------------------------------
-
 // enc.conv_in on the input planes: channel j of a row is tap j, so the whole k-tap conv is one k-block
 int build_enc_conv_in(TcGemm& g, const HostW& hw, int k, int Cout) {
+    if (k > TC_BK) return 1;                                       // the input window does not fit one k-block
     std::vector<float> w, b;
     if (hw.get("enc.conv_in.weight", w) || hw.get("enc.conv_in.bias", b)) return -1;
     const int Cop = cpad(Cout);
@@ -1276,136 +914,273 @@ int build_down(TcGemm& g, const HostW& hw, const std::string& name, int Cin, int
     return upload_gemm(g, W, b, Cop, Ktot, 0);
 }
 
-// the stage lengths of an utterance of N samples: L[0] = N, L[s+1] = ceil(L[s] / r_s)
-std::vector<int> enc_chain(const EncPlan& pl, int N) {
-    std::vector<int> L(1, N);
-    for (int r : pl.ratios) L.push_back((L.back() + r - 1) / r);
-    return L;
+// the decoder's final conv (k <= DS_LD) as per-tap partial products: GEMM row j = tap j, summed by tc_diag_sum_kernel
+int build_conv_out_split(TcGemm& g, const HostW& hw, int C, int k, float* bias) {
+    std::vector<float> w, b;
+    if (hw.get("dec.conv_out.weight", w) || hw.get("dec.conv_out.bias", b)) return -1;
+    const int Cp = cpad(C);
+    std::vector<float> W(static_cast<size_t>(k) * Cp, 0.f);
+    for (int ci = 0; ci < C; ++ci)
+        for (int j = 0; j < k; ++j) W[static_cast<size_t>(j) * Cp + ci] = w[static_cast<size_t>(ci) * k + j];
+    for (int cb = 0; cb < Cp / TC_BK; ++cb) g.taps.push_back(TcTap{0, 0, cb * TC_BK});
+    g.Cout = 32;
+    g.up = 1;
+    *bias = b[0];
+    return upload_gemm(g, W, std::vector<float>(), k, Cp, 32);
 }
 
-// plane rows per utterance of every stage: the stage length rounded up to its strided conv's stride
-std::vector<int> enc_rows(const EncPlan& pl, const std::vector<int>& L) {
-    std::vector<int> R(L);
-    for (size_t s = 0; s < pl.ratios.size(); ++s) R[s] = (L[s] + pl.ratios[s] - 1) / pl.ratios[s] * pl.ratios[s];
-    return R;
+// One residual block (weights `name`, profile labels prefixed by `lp`): conv1 (kres taps, dilation dil) on ELU(x) -> the
+// hidden tensor hd, then conv2 on hd and the 1x1 shortcut on raw x as one GEMM -> o.  C and hidden are real channels.
+int res_block(Plan& pl, const HostW& hw, const std::string& name, const std::string& lp, int x, int hd, int o, int C,
+              int hidden, int kres, int dil) {
+    TcGemm& g1 = pl.gemm();
+    if (int rc = build_conv(g1, hw, name + ".conv1", C, hidden, kres, dil)) return rc;
+    pl.layer(L_CONV, lp + "res_conv1", &g1, cpad(hidden), x, FORM_ELU, hd, F32_NONE);
+    TcGemm& g2 = pl.gemm();
+    if (int rc = build_res_tail(g2, hw, name, C, hidden)) return rc;
+    pl.layer(L_CONV, lp + "res_conv2", &g2, cpad(C), hd, FORM_ELU, o, F32_NONE).in2 = x;
+    return 0;
 }
 
-Plane enc_geometry(const EncTensor& t, int B, const std::vector<int>& R) {
-    Plane p;
-    p.C = t.C;
-    p.T = R[t.stage];
-    p.halo = t.halo;
-    p.Tp = p.T + t.halo;
-    p.halo_zero = t.halo_kind == HALO_ZERO;
-    p.tm = t.tm;
-    if (t.tm) {
-        const int Bc = bcap(B);
-        p.rcap = p.Tp * Bc;
-        p.sb = 1;
-        p.st = Bc;
-        p.off = static_cast<long long>(t.halo) * Bc;
-    } else {
-        p.rcap = std::max(B * p.Tp, TC_BM * t.fold);     // (whole folded rows; a TMA box never taller than its tensor)
-        p.sb = p.Tp;
-        p.st = 1;
-        p.off = t.halo;
+// The LSTM stack (weights `dir`.lstm.*): per layer, W_ih for all steps as one GEMM into the fp32 pre-activations (layer 0
+// reads x0, layer l the h planes of layer l-1), then the steps over the layer's h planes hs[l % 2].  The last layer's
+// epilogue writes ELU(h + skip) straight into `out`.
+int lstm_stack(Plan& pl, const HostW& hw, const std::string& dir, const std::string& lp, int H, int x0, const int* hs, int out,
+               int step_bn, int nl) {
+    for (int l = 0; l < nl; ++l) {
+        const std::string w = dir + ".lstm.weight_", b = dir + ".lstm.bias_", sl = "_l" + std::to_string(l);
+        TcGemm& ih = pl.gemm();
+        if (int rc = build_lstm(ih, hw, w + "ih" + sl, b + "ih" + sl, b + "hh" + sl, H, 0)) return rc;
+        pl.layer(L_LSTM_IH, lp + "lstm_ih", &ih, 4 * H, l == 0 ? x0 : hs[(l - 1) & 1], FORM_RAW, -1, F32_PRE).lstm = l;
+        TcGemm& step = pl.gemm();
+        if (int rc = build_lstm(step, hw, w + "hh" + sl, "", "", H, step_bn)) return rc;
+        pl.layer(L_LSTM_STEPS, lp + "lstm_steps", &step, 4 * H, hs[l & 1], FORM_RAW, l == nl - 1 ? out : -1, F32_NONE).lstm = l;
     }
-    return p;
+    return 0;
 }
 
-// The encoder's layers in launch order.  Halo rule as in the decoder (a causal conv reads (k-1)*dilation rows above its output
-// row); a strided conv's input keeps r rows (its causal left pad) plus the per-utterance right padding (E_RPAD).
-void build_enc_plan(TcCodec* tc) {
+// The decoder's layers in launch order, each with its GEMM.  Every halo rule is here: a causal convolution reads
+// (k-1)*dilation rows above its output row, so its input keeps that many halo rows, padded like the reference (reflect or
+// zeros); a ConvTranspose reads x[t-1], so its input keeps one zero row.  A stream's state holds the carried tensors and
+// the LSTM (h, c) per layer, in the order the carries run.  0: built; 1: not covered; -1: error.
+int build_dec(TcCodec* tc, const HostW& hw, int step_bn) {
     const enc_config& cf = tc->cfg;
-    EncPlan& pl = tc->enc->plan;
-    TcEncoder& E = *tc->enc;
-    const int n = cf.n_ratios, nres = cf.n_residual_layers, nl = cf.lstm, H = tc->ch0;
+    Plan& pl = tc->dec;
+    const int H = tc->ch0, nl = cf.lstm, nres = cf.n_residual_layers;
     const int kres = cf.residual_kernel_size, kout = cf.last_kernel_size;
     const int pad = cf.pad_reflect ? HALO_REFLECT : HALO_ZERO;
-    for (int s = 0; s < n; ++s) pl.ratios.push_back(cf.ratios[n - 1 - s]);
-    auto tensor = [&](int C, int halo, int kind, int stage, int fold, bool tm, int forms, std::string dbg_raw, std::string dbg_elu) {
-        EncTensor t;
-        t.C = C; t.halo = halo; t.halo_kind = kind; t.stage = stage; t.fold = fold; t.tm = tm; t.forms = forms;
-        t.home = (tc->keep || stage == n) ? HOME_FIXED : HOME_ARENA0 + (stage & 1);
+    enum { ARENA_X0, ARENA_X1, ARENA_HIDDEN };   // the stages' ping-pong arenas, and the hidden tensors'
+    // arena tensors are each a group of their own: they all start at their arena's first byte
+    auto tensor = [&](int C, int halo, int kind, int stage, bool tm, int forms, int arena, bool carried, std::string dbg_raw,
+                      std::string dbg_elu) {
+        Tensor t;
+        t.C = C; t.halo = halo; t.halo_kind = kind; t.stage = stage; t.tm = tm;
+        t.forms = forms; t.arena = tc->keep ? -1 : arena; t.group = static_cast<int>(pl.tensors.size()); t.carried = carried;
         t.dbg_raw = std::move(dbg_raw);
         t.dbg_elu = std::move(dbg_elu);
         pl.tensors.push_back(t);
         return static_cast<int>(pl.tensors.size()) - 1;
     };
-    auto layer = [&](int kind, const char* label, const TcGemm* g, int nstore, int in, int in_form, int out, int f32) {
-        EncLayer L;
-        L.kind = kind; L.label = label; L.g = g; L.nstore = nstore; L.in = in; L.in_form = in_form; L.out = out; L.f32 = f32;
-        L.out_forms = out >= 0 ? pl.tensors[out].forms : 0;
-        pl.layers.push_back(L);
-        return &pl.layers.back();
+    // the input of a ConvTranspose, or of the final conv after the last stage
+    auto feed = [&](bool last_stage, int& halo, int& kind) {
+        halo = last_stage ? kout - 1 : 1;
+        kind = last_stage ? pad : HALO_ZERO;
+    };
+    char nm[96];
+
+    pl.up.push_back(1);
+    const int z = tensor(tc->Dp, cf.kernel_size - 1, pad, 0, false, FORM_RAW, -1, true, "z", "");
+    pl.u0 = tensor(cpad(H), 1, HALO_ZERO, 0, false, FORM_ELU, -1, true, "", "u0");
+    int x0 = -1, hs[2] = {-1, -1};
+    if (nl > 0) {
+        x0 = tensor(H, 0, HALO_ZERO, 0, true, FORM_RAW, -1, false, "x0", "");
+        for (int l = 0; l < std::min(nl, 2); ++l)                 // h planes: slot t+1 = h_t, layers alternate
+            hs[l] = tensor(H, 1, HALO_ZERO, 0, true, FORM_RAW, -1, false, "hs" + std::to_string(l), "");
+        pl.bufs = {BUF_X0, BUF_PRE, BUF_CST};
+    }
+    pl.layer(L_RVQ, "rvq", nullptr, 0, -1, 0, z, F32_NONE);
+    TcGemm& ci = pl.gemm();
+    if (int rc = build_conv(ci, hw, "dec.conv_in", cf.dimension, H, cf.kernel_size, 1)) return rc;
+    pl.layer(L_CONV, "conv_in", &ci, cpad(H), z, FORM_RAW, nl > 0 ? x0 : pl.u0, nl > 0 ? F32_X0 : F32_NONE);
+    if (int rc = lstm_stack(pl, hw, "dec", "", H, x0, hs, pl.u0, step_bn, nl)) return rc;
+    // up-sampling stages: ConvTranspose -> X; per residual block conv1 (on ELU(X)) -> hidden, then conv2 (on the hidden) +
+    // shortcut (on raw X) -> O, the next block's X.  X and O alternate between the two arenas.
+    int cur = pl.u0, ch = H, side = ARENA_X0;
+    for (int i = 0; i < cf.n_ratios; ++i) {
+        const int r = cf.ratios[i], cout = ch / 2, hidden = cout / cf.compress, stage = i + 1;
+        const bool last_stage = i == cf.n_ratios - 1;
+        const std::string s = std::to_string(i + 1);
+        pl.up.push_back(pl.up.back() * r);
+        int halo = kres - 1, kind = pad;
+        if (nres == 0) feed(last_stage, halo, kind);
+        int x = tensor(cpad(cout), halo, kind, stage, false, (nres > 0 ? FORM_RAW : 0) | FORM_ELU, side, true,
+                       nres > 0 ? "x" + s + ".raw" : "", "x" + s + ".elu");
+        TcGemm& up = pl.gemm();
+        snprintf(nm, sizeof(nm), "dec.up%d.convtr", i);
+        if (int rc = build_convtr(up, hw, nm, ch, cout, r)) return rc;
+        pl.layer(L_CONV, "convtr", &up, r * cpad(cout), cur, FORM_ELU, x, F32_NONE);
+        ch = cout;
+        for (int j = 0, dil = 1; j < nres; ++j, dil *= cf.dilation_base) {
+            const std::string sj = s + "." + std::to_string(j);
+            const int hd = tensor(cpad(hidden), pl.tensors[x].halo, HALO_UNWRITTEN, stage, false, FORM_ELU, ARENA_HIDDEN, false,
+                                  "", "h" + sj);
+            // the next block's conv1 reads (kres-1) * its dilation rows back.  min_T takes this term for the last block too.
+            const int next = (kres - 1) * dil * cf.dilation_base;
+            pl.min_T = std::max(pl.min_T, next + 2);
+            halo = next;
+            kind = pad;
+            if (j == nres - 1) feed(last_stage, halo, kind);
+            const int o = tensor(cpad(cout), halo, kind, stage, false, (j < nres - 1 ? FORM_RAW : 0) | FORM_ELU, side ^ 1, true,
+                                 j < nres - 1 ? "o" + sj + ".raw" : "", "o" + sj);
+            snprintf(nm, sizeof(nm), "dec.up%d.res%d", i, j);
+            if (int rc = res_block(pl, hw, nm, "", x, hd, o, cout, hidden, kres, dil)) return rc;
+            x = o;
+            side ^= 1;
+        }
+        cur = x;
+        side ^= 1;                                                 // the next ConvTranspose must not write over `cur`
+    }
+    // final conv: k <= DS_LD partial products (the first 16-column chunk), or one output column (f_valid = 1)
+    TcGemm& co = pl.gemm();
+    if (int rc = build_conv(co, hw, "dec.conv_out", ch, 1, kout, 1, 32)) return rc;
+    if (kout <= DS_LD && !(getenv("VCB_CODEC_CONVOUT_TC") && atoi(getenv("VCB_CODEC_CONVOUT_TC")))) {
+        TcGemm& cop = pl.gemm();
+        if (int rc = build_conv_out_split(cop, hw, ch, kout, &tc->co_bias)) return rc;
+        pl.layer(L_CONV_OUT_SPLIT, "conv_out", &cop, 16, cur, FORM_ELU, -1, F32_COPART);
+        pl.bufs.push_back(BUF_COPART);
+    } else {
+        pl.layer(L_CONV_OUT, "conv_out", &co, 32, cur, FORM_ELU, -1, F32_WAV);
+    }
+    pl.min_T = std::max(pl.min_T, std::max(cf.kernel_size, kout) + 1);
+    for (Layer& L : pl.layers) {                                   // the stream state, in the order the carries run
+        if (L.kind == L_LSTM_STEPS) {
+            L.h_off = pl.stream_bytes;
+            L.c_off = pl.stream_bytes + static_cast<size_t>(H) * 4;
+            pl.stream_bytes += static_cast<size_t>(H) * 8;
+        }
+        Tensor* t = L.out >= 0 ? &pl.tensors[L.out] : nullptr;
+        if (t && t->carried && t->halo > 0) {
+            t->state_off = pl.stream_bytes;
+            pl.stream_bytes += static_cast<size_t>(t->halo) * t->C * 4;
+        }
+    }
+    return 0;
+}
+
+// The encoder's layers in launch order (SEANetEncoder, oracle/encodec_oracle.py::encoder_plan), each with its GEMM.  Stage
+// s holds the rows of the s-th strided conv's input (stage 0: the samples; stage n: the frames).  Halo rule as in the
+// decoder; a strided conv's input keeps r rows (its causal left pad) plus the per-utterance right padding (L_RPAD).
+// 0: built; 1: not covered; -1: error.
+int build_enc(TcCodec* tc, const HostW& hw, int step_bn) {
+    const enc_config& cf = tc->cfg;
+    Plan& pl = *tc->enc;
+    const int n = cf.n_ratios, nres = cf.n_residual_layers, nl = cf.lstm, H = tc->ch0;
+    const int kres = cf.residual_kernel_size, kout = cf.last_kernel_size;
+    const int pad = cf.pad_reflect ? HALO_REFLECT : HALO_ZERO;
+    for (int s = 0; s < n; ++s) pl.ratios.push_back(cf.ratios[n - 1 - s]);
+    pl.top = n;
+    // the stages alternate between two arenas (stage s's strided conv reads arena s % 2 and writes arena (s+1) % 2), where
+    // the tensors of a stage stack; the LSTM stage's tensors have their own rows
+    auto tensor = [&](int C, int halo, int kind, int stage, int fold, bool tm, int forms, std::string dbg_raw, std::string dbg_elu) {
+        Tensor t;
+        t.C = C; t.halo = halo; t.halo_kind = kind; t.stage = stage; t.fold = fold; t.tm = tm; t.forms = forms;
+        t.arena = (tc->keep || stage == n) ? -1 : stage & 1;
+        t.group = stage;
+        t.dbg_raw = std::move(dbg_raw);
+        t.dbg_elu = std::move(dbg_elu);
+        pl.tensors.push_back(t);
+        return static_cast<int>(pl.tensors.size()) - 1;
     };
     // what stage s's first layer reads: its first residual block (conv1 reads kres-1 rows back), or its strided conv
     auto block_input = [&](int s, int C, const std::string& name) {
         if (nres > 0) return tensor(C, kres - 1, pad, s, 1, false, FORM_RAW | FORM_ELU, name, name + ".elu");
         return tensor(C, pl.ratios[s], pad, s, pl.ratios[s], false, FORM_ELU, "", name + ".elu");
     };
+    char nm[96];
     int ch = cf.n_filters;
     const int in0 = tensor(TC_BK, 0, HALO_ZERO, 0, 1, false, FORM_RAW, "enc.input", "");
-    layer(E_INPUT, "enc_input", nullptr, 0, -1, 0, in0, F32_NONE);
+    pl.layer(L_INPUT, "enc_input", nullptr, 0, -1, 0, in0, F32_NONE);
     int cur = block_input(0, cpad(ch), "enc.x0");
-    layer(E_CONV, "enc_conv_in", &E.conv_in, cpad(ch), in0, FORM_RAW, cur, F32_NONE);
+    TcGemm& ci = pl.gemm();
+    if (int rc = build_enc_conv_in(ci, hw, cf.kernel_size, cf.n_filters)) return rc;
+    pl.layer(L_CONV, "enc_conv_in", &ci, cpad(ch), in0, FORM_RAW, cur, F32_NONE);
     int u = -1, x0 = -1;
     for (int s = 0; s < n; ++s) {
         const int r = pl.ratios[s], hidden = ch / cf.compress;
         const std::string si = "enc.down" + std::to_string(s);
         for (int j = 0, dil = 1; j < nres; ++j, dil *= cf.dilation_base) {
             const std::string sj = si + ".res" + std::to_string(j);
-            const EncTensor& x = pl.tensors[cur];
+            const Tensor x = pl.tensors[cur];
             const int hd = tensor(cpad(hidden), x.halo, HALO_UNWRITTEN, s, x.fold, false, FORM_ELU, "", sj + ".h");
-            layer(E_CONV, "enc_res_conv1", &E.res1[s][j], cpad(hidden), cur, FORM_ELU, hd, F32_NONE);
             const int o = j == nres - 1 ? tensor(cpad(ch), r, pad, s, r, false, FORM_ELU, "", sj + ".elu")
                                         : tensor(cpad(ch), (kres - 1) * dil * cf.dilation_base, pad, s, 1, false,
                                                  FORM_RAW | FORM_ELU, sj, sj + ".elu");
-            layer(E_CONV, "enc_res_conv2", &E.res2[s][j], cpad(ch), hd, FORM_ELU, o, F32_NONE)->in2 = cur;
+            if (int rc = res_block(pl, hw, sj, "enc_", cur, hd, o, ch, hidden, kres, dil)) return rc;
             cur = o;
         }
-        EncLayer* rp = layer(E_RPAD, "enc_rpad", nullptr, 0, -1, 0, cur, F32_NONE);
-        rp->stage = s;
-        rp->r = r;
-        ch *= 2;
+        pl.layer(L_RPAD, "enc_rpad", nullptr, 0, -1, 0, cur, F32_NONE);
         int next;
-        if (s < n - 1) next = block_input(s + 1, cpad(ch), si + ".conv");
+        if (s < n - 1) next = block_input(s + 1, cpad(2 * ch), si + ".conv");
         else if (nl > 0) next = x0 = tensor(H, 0, HALO_ZERO, n, 1, true, FORM_RAW, si + ".conv", "");
-        else next = u = tensor(cpad(ch), kout - 1, pad, n, 1, false, FORM_ELU, "", "enc.lstm");
-        EncLayer* d = layer(E_DOWN, "enc_down", &E.down[s], cpad(ch), cur, FORM_ELU, next, next == x0 ? F32_X0 : F32_NONE);
-        d->stage = s;
-        d->r = r;
+        else next = u = tensor(cpad(2 * ch), kout - 1, pad, n, 1, false, FORM_ELU, "", "enc.lstm");
+        TcGemm& d = pl.gemm();
+        snprintf(nm, sizeof(nm), "enc.down%d.conv", s);
+        if (int rc = build_down(d, hw, nm, ch, 2 * ch, r)) return rc;
+        pl.layer(L_CONV, "enc_down", &d, cpad(2 * ch), cur, FORM_ELU, next, next == x0 ? F32_X0 : F32_NONE);
         cur = next;
+        ch *= 2;
     }
     if (nl > 0) {
         int hs[2] = {-1, -1};
         for (int l = 0; l < std::min(nl, 2); ++l)
             hs[l] = tensor(H, 1, HALO_ZERO, n, 1, true, FORM_RAW, "enc.hs" + std::to_string(l), "");
         u = tensor(cpad(H), kout - 1, pad, n, 1, false, FORM_ELU, "", "enc.lstm");
-        for (int l = 0; l < nl; ++l) {
-            layer(E_LSTM_IH, "enc_lstm_ih", &E.pre[l], 4 * H, l == 0 ? x0 : hs[(l - 1) & 1], FORM_RAW, -1, F32_PRE)->lstm = l;
-            // the last layer's epilogue writes ELU(h + skip) into enc.conv_out's input, whose halo E_LPAD then fills
-            layer(E_LSTM_STEPS, "enc_lstm_steps", &E.step[l], 4 * H, hs[l & 1], FORM_RAW, l == nl - 1 ? u : -1, F32_NONE)->lstm = l;
-        }
-        layer(E_LPAD, "enc_lpad", nullptr, 0, -1, 0, u, F32_NONE);
+        // the last layer's epilogue writes ELU(h + skip) into enc.conv_out's input, whose halo L_LPAD then fills
+        if (int rc = lstm_stack(pl, hw, "enc", "enc_", H, x0, hs, u, step_bn, nl)) return rc;
+        pl.layer(L_LPAD, "enc_lpad", nullptr, 0, -1, 0, u, F32_NONE);
+        pl.bufs = {BUF_X0, BUF_PRE, BUF_CST};
     }
-    layer(E_CONV_OUT, "enc_conv_out", &E.conv_out, tc->Dp, u, FORM_ELU, -1, F32_LAT);
+    TcGemm& co = pl.gemm();
+    if (int rc = build_conv(co, hw, "enc.conv_out", H, cf.dimension, kout, 1)) return rc;
+    pl.layer(L_CONV_OUT, "enc_conv_out", &co, tc->Dp, u, FORM_ELU, -1, F32_LAT);
+    pl.bufs.insert(pl.bufs.end(), {BUF_LATF, BUF_LAT, BUF_SCORES, BUF_CODES, BUF_TAB});
+    return 0;
 }
 
-struct EncWs {
+// the stage lengths of an utterance of N samples: L[0] = N, L[s+1] = ceil(L[s] / r_s)
+std::vector<int> enc_chain(const Plan& pl, int N) {
+    std::vector<int> L(1, N);
+    for (int r : pl.ratios) L.push_back((L.back() + r - 1) / r);
+    return L;
+}
+
+// plane rows per utterance of every stage: the stage length rounded up to its strided conv's stride
+std::vector<int> enc_rows(const Plan& pl, const std::vector<int>& L) {
+    std::vector<int> R(L);
+    for (size_t s = 0; s < pl.ratios.size(); ++s) R[s] = (L[s] + pl.ratios[s] - 1) / pl.ratios[s] * pl.ratios[s];
+    return R;
+}
+
+// the decoder's plane rows per utterance of every stage for T frames
+std::vector<int> dec_rows(const Plan& pl, int T) {
+    std::vector<int> R;
+    for (int u : pl.up) R.push_back(T * u);
+    return R;
+}
+
+// The workspace of a chunk of B utterances with plane rows R per stage: the tensors with rows of their own, the arenas, the
+// fp32 buffers.  In an arena, the tensors of a group stack, and every group starts at the arena's first byte: the arena is
+// as large as its largest group.  tensor[i] = offset of plan tensor i's first stored form (an ELU'd form follows a raw one).
+struct WsLayout {
     std::vector<size_t> tensor;
-    size_t x0f = 0, pre = 0, cst = 0, latf = 0, lat = 0, scores = 0, codes = 0, tab = 0, bytes = 0;
+    size_t buf[NBUF] = {};
+    size_t bytes = 0;
 };
 
-// The workspace of an encoder chunk of B utterances of at most N samples: fixed tensors (the LSTM stage's), two arenas that
-// the stages alternate between (stage s's strided conv reads arena s % 2 and writes arena (s+1) % 2), the fp32 buffers,
-// the RVQ scores and codes, the per-utterance table.
-EncWs enc_ws_layout(const TcCodec* tc, int B, int N) {
-    const EncPlan& pl = tc->enc->plan;
+WsLayout ws_layout(const TcCodec* tc, const Plan& pl, int B, const std::vector<int>& R) {
     const enc_config& cf = tc->cfg;
-    const std::vector<int> R = enc_rows(pl, enc_chain(pl, N));
-    const int n = static_cast<int>(pl.ratios.size()), Tn = R[n], Bcap = bcap(B), H = tc->ch0, nl = cf.lstm;
-    EncWs w;
+    const size_t Bn = B, Bc = bcap(B), H = tc->ch0, Tn = R[pl.top];
+    WsLayout w;
     w.tensor.resize(pl.tensors.size());
     size_t off = 0;
     auto take = [&](size_t bytes) {
@@ -1413,117 +1188,176 @@ EncWs enc_ws_layout(const TcCodec* tc, int B, int N) {
         off += align_up(bytes, 1024);
         return o;
     };
-    std::vector<size_t> stage_off(n + 1, 0);
-    size_t arena[2] = {0, 0};
+    std::map<int, size_t> group_end;
+    size_t arena[3] = {0, 0, 0};
     for (size_t i = 0; i < pl.tensors.size(); ++i) {
-        const EncTensor& t = pl.tensors[i];
+        const Tensor& t = pl.tensors[i];
         size_t bytes = 0;
         for (int f : {FORM_RAW, FORM_ELU})
-            if (t.forms & f) bytes += align_up(form_bytes(enc_geometry(t, B, R)), 1024);
-        if (t.home == HOME_FIXED) {
+            if (t.forms & f) bytes += align_up(form_bytes(geometry(t, B, R)), 1024);
+        if (t.arena < 0) {
             w.tensor[i] = take(bytes);
         } else {
-            w.tensor[i] = stage_off[t.stage];                  // offset inside its arena for now
-            stage_off[t.stage] += bytes;
-            arena[t.home - HOME_ARENA0] = std::max(arena[t.home - HOME_ARENA0], stage_off[t.stage]);
+            w.tensor[i] = group_end[t.group];                     // offset inside its arena for now
+            group_end[t.group] += bytes;
+            arena[t.arena] = std::max(arena[t.arena], group_end[t.group]);
         }
     }
-    const size_t a0 = take(arena[0]), a1 = take(arena[1]);
+    const size_t a[3] = {take(arena[0]), take(arena[1]), take(arena[2])};
     for (size_t i = 0; i < pl.tensors.size(); ++i)
-        if (pl.tensors[i].home != HOME_FIXED) w.tensor[i] += pl.tensors[i].home == HOME_ARENA0 ? a0 : a1;
-    if (nl > 0) {
-        w.x0f = take(static_cast<size_t>(Tn) * Bcap * H * 4);
-        w.pre = take(static_cast<size_t>(Tn) * Bcap * 4 * H * 4);
-        w.cst = take(static_cast<size_t>(nl) * Bcap * H * 4);
+        if (pl.tensors[i].arena >= 0) w.tensor[i] += a[pl.tensors[i].arena];
+    for (int b : pl.bufs) {
+        size_t bytes = 0;
+        switch (b) {
+            case BUF_X0: bytes = Tn * Bc * H * 4; break;           // time-major [T][Bcap][H]
+            case BUF_PRE: bytes = Tn * Bc * 4 * H * 4; break;      // time-major [T][Bcap][4H]
+            case BUF_CST: bytes = cf.lstm * Bc * H * 4; break;     // [layers][Bcap][H]
+            case BUF_COPART: {                                     // the final conv's input rows, halo included, + a tile
+                const Tensor& in = pl.tensors[pl.layers.back().in];
+                bytes = (Bn * (R[in.stage] + std::max(in.halo, 1)) + TC_BM) * DS_LD * 4;
+                break;
+            }
+            case BUF_LATF: bytes = Bn * Tn * tc->Dp * 4; break;    // [B][T][Dp]
+            case BUF_LAT: bytes = Bn * cf.dimension * Tn * 4; break;
+            case BUF_SCORES: bytes = Bn * cf.bins * Tn * 4; break;
+            case BUF_CODES: bytes = Bn * cf.n_q * Tn * 8; break;
+            case BUF_TAB: bytes = (R.size() + 1) * Bn * 4; break;  // [stages][B] lengths, then [B] wav rows
+        }
+        w.buf[b] = take(bytes);
     }
-    w.latf = take(static_cast<size_t>(B) * Tn * tc->Dp * 4);
-    w.lat = take(static_cast<size_t>(B) * cf.dimension * Tn * 4);
-    w.scores = take(static_cast<size_t>(B) * cf.bins * Tn * 4);
-    w.codes = take(static_cast<size_t>(B) * cf.n_q * Tn * 8);
-    w.tab = take(static_cast<size_t>(n + 2) * B * 4);
     w.bytes = off;
     return w;
 }
 
-// One chunk: utterance b = wav row rows[b] with lens[b] samples; the chunk's planes are sized for its longest utterance.
-int encode_chunk_tc(TcCodec* tc, const float* wav, long long wav_ld, const int* rows, const int* lens, int B, cudaStream_t st,
-                    int64_t* launches, TcEncOut* out) {
-    const EncPlan& pl = tc->enc->plan;
+// grows the workspace to at least `need` bytes (alloc releases the previous one first, so the stream is drained before)
+int grow_ws(TcCodec* tc, size_t need, cudaStream_t st, const std::string& what) {
+    if (need <= tc->ws.size()) return 0;
+    if (tc->ws) VCB_CUDA_OK(cudaStreamSynchronize(st));
+    if (tc->ws.alloc(need) == 0) return 0;
+    const std::string why = get_error();
+    set_error("codec_tc: cannot allocate a %.2f GB %s (%s)", need / 1073741824.0, what.c_str(), why.c_str());
+    return -1;
+}
+
+// what a chunk reads and writes outside the workspace
+struct ChunkIO {
+    const int64_t* codes = nullptr;    // decoder: codes [B][n_q][T]
+    float* wav = nullptr;              // decoder: waveform [B][T * hop]
+    const float* wav_in = nullptr;     // encoder: fp32 wav rows (the table's rows) of wav_ld samples
+    long long wav_ld = 0;
+    const TcStreamCtx* sc = nullptr;   // decoder stream: every plane a layer reads as left context, and the LSTM state,
+                                       // continue the utterance's stream (tc_carry_kernel)
+};
+
+// One chunk of B utterances through plan pl, with plane rows R per stage, in the workspace laid out as w.
+int run_chunk(TcCodec* tc, Plan& pl, const WsLayout& w, int B, const std::vector<int>& R, cudaStream_t st, int64_t* launches,
+              const ChunkIO& io) {
     const enc_config& cf = tc->cfg;
-    const int n = static_cast<int>(pl.ratios.size()), Bcap = bcap(B), H = tc->ch0, nl = cf.lstm;
-    const int N = *std::max_element(lens, lens + B);
-    const std::vector<int> R = enc_rows(pl, enc_chain(pl, N));
-    const int Tn = R[n];
-    const EncWs w = enc_ws_layout(tc, B, N);
+    const int Bcap = bcap(B), H = tc->ch0, nl = cf.lstm;
+    const TcStreamCtx* sc = io.sc;
+    auto buf = [&](int b) { return reinterpret_cast<float*>(tc->ws + w.buf[b]); };
+    int* tab = reinterpret_cast<int*>(buf(BUF_TAB));                // encoder: [stages][B] lengths, then [B] wav rows
     std::vector<Plane> P(pl.tensors.size());
-    tc->edbg.clear();
+    pl.dbg.clear();
     for (size_t i = 0; i < P.size(); ++i) {
-        const EncTensor& t = pl.tensors[i];
+        const Tensor& t = pl.tensors[i];
         Plane& p = P[i];
-        p = enc_geometry(t, B, R);
+        p = geometry(t, B, R);
         uint8_t* base = tc->ws + w.tensor[i];
         if (t.forms & FORM_RAW) {
             p.raw = reinterpret_cast<__nv_bfloat16*>(base);
             base += align_up(form_bytes(p), 1024);
         }
         if (t.forms & FORM_ELU) p.elu = reinterpret_cast<__nv_bfloat16*>(base);
-        if (!t.dbg_raw.empty()) tc->edbg[t.dbg_raw] = TcCodec::Dbg{p, p.raw, B};
-        if (!t.dbg_elu.empty()) tc->edbg[t.dbg_elu] = TcCodec::Dbg{p, p.elu, B};
+        if (!t.dbg_raw.empty()) pl.dbg[t.dbg_raw] = Dbg{p, p.raw, B};
+        if (!t.dbg_elu.empty()) pl.dbg[t.dbg_elu] = Dbg{p, p.elu, B};
     }
-    float* x0f = reinterpret_cast<float*>(tc->ws + w.x0f);
-    float* pre = reinterpret_cast<float*>(tc->ws + w.pre);
-    float* cst = reinterpret_cast<float*>(tc->ws + w.cst);
-    float* latf = reinterpret_cast<float*>(tc->ws + w.latf);
-    int* tab = reinterpret_cast<int*>(tc->ws + w.tab);         // [n+1][B] stage lengths, then [B] wav rows
-    {
-        std::vector<int> h(static_cast<size_t>(n + 2) * B);
-        for (int b = 0; b < B; ++b) {
-            const std::vector<int> L = enc_chain(pl, lens[b]);
-            for (int s = 0; s <= n; ++s) h[static_cast<size_t>(s) * B + b] = L[s];
-            h[static_cast<size_t>(n + 1) * B + b] = rows[b];
-        }
-        VCB_CUDA_OK(cudaMemcpyAsync(tab, h.data(), h.size() * 4, cudaMemcpyHostToDevice, st));   // pageable: staged at once
+
+    // state that the kernels only ever read: U0's zero halo (the LSTM epilogue writes none), c_0 and h_{-1}
+    if (pl.u0 >= 0) {
+        const Plane& u0 = P[pl.u0];
+        VCB_CUDA_OK(cudaMemset2DAsync(u0.elu, static_cast<size_t>(u0.Tp) * u0.C * 2, 0, static_cast<size_t>(u0.C) * 2, B, st));
+        VCB_CUDA_OK(cudaMemset2DAsync(u0.elu + u0.plane(), static_cast<size_t>(u0.Tp) * u0.C * 2, 0, static_cast<size_t>(u0.C) * 2, B, st));
     }
-    if (nl > 0) VCB_CUDA_OK(cudaMemsetAsync(cst, 0, static_cast<size_t>(nl) * Bcap * H * 4, st));
     auto clear_h0 = [&](const Plane& hs) -> int {
         VCB_CUDA_OK(cudaMemsetAsync(hs.raw, 0, static_cast<size_t>(Bcap) * H * 2, st));
         VCB_CUDA_OK(cudaMemsetAsync(hs.raw + hs.plane(), 0, static_cast<size_t>(Bcap) * H * 2, st));
         return 0;
     };
-    for (const EncLayer& L : pl.layers)
-        if (L.kind == E_LSTM_STEPS && L.lstm < 2 && clear_h0(P[L.in])) return -1;
+    if (nl > 0) {
+        VCB_CUDA_OK(cudaMemsetAsync(buf(BUF_CST), 0, static_cast<size_t>(nl) * Bcap * H * 4, st));
+        for (const Layer& L : pl.layers)
+            if (L.kind == L_LSTM_STEPS && L.lstm < 2 && clear_h0(P[L.in])) return -1;
+    }
+
+    auto carry = [&](void* base, long long plane_bytes, long long sb, long long stt, long long off, int row_bytes, int halo, int up,
+                     int restore, int save, size_t state_off) -> int {
+        const CarryArgs a{static_cast<uint8_t*>(base), plane_bytes, sb, stt, off, row_bytes, halo, up, restore, save, sc->table,
+                          sc->state, static_cast<long long>(pl.stream_bytes), static_cast<long long>(state_off)};
+        VCB_CUDA_OK(launch_k_pdl(1, tc_carry_kernel, dim3(B), dim3(256), 0, st, a));
+        ++*launches;
+        return 0;
+    };
+    // a plane's halo: restore a continuing stream's tail over the padding the producer wrote, save the new tail
+    auto carry_plane = [&](int i) -> int {
+        const Tensor& t = pl.tensors[i];
+        const Plane& p = P[i];
+        if (sc == nullptr || !t.carried || p.halo == 0) return 0;
+        return carry(p.elu ? p.elu : p.raw, p.plane() * 2, p.sb, p.st, p.off, p.C * 2, p.halo, pl.up[t.stage], 1, 1, t.state_off);
+    };
+    // stream decode: h_{-1} (slot 0) and c continue the stream; after the layer, h of the last valid step (slot frames) and
+    // the frozen c are saved.  As a time-major plane with one halo row, row(b, t) = (t + 1) * Bcap + b.
+    auto carry_lstm = [&](const Layer& L, const Plane& hs, float* cl, int restore, int save) -> int {
+        if (sc == nullptr) return 0;
+        return carry(hs.raw, hs.plane() * 2, hs.sb, hs.st, hs.off, H * 2, 1, 1, restore, save, L.h_off) ||
+               carry(cl, 0, 1, 0, 0, H * 4, 1, 1, restore, save, L.c_off);
+    };
+    auto pad_rows = [&](__nv_bfloat16* base, const Plane& o, const int* lens, int r, int zero) -> int {
+        tc_pad_rows_kernel<<<B, 256, 0, st>>>(base, o.plane(), o.C, o.sb, o.st, o.off, lens, o.halo, r, zero);
+        VCB_CUDA_OK(cudaGetLastError());
+        ++*launches;
+        return 0;
+    };
 
     Prof pf{tc, st};
     CUtensorMap mA, mB;
-    for (const EncLayer& L : pl.layers) {
-        pf.begin(L.label);
-        if (L.kind == E_INPUT) {
+    for (const Layer& L : pl.layers) {
+        pf.begin(L.label.c_str());
+        if (L.kind == L_RVQ) {
+            const Plane& z = P[L.out];
+            tc_rvq_planes_kernel<<<dim3((z.T + 15) / 16, B), 128, 0, st>>>(reinterpret_cast<const long long*>(io.codes), tc->d_embed,
+                                                                           z.raw, z.plane(), cf.n_q, tc->D, z.C, z.T, z.Tp, z.halo,
+                                                                           z.halo_zero);
+            VCB_CUDA_OK(cudaGetLastError());
+            ++*launches;
+        } else if (L.kind == L_INPUT) {
             const Plane& o = P[L.out];
             const long long items = static_cast<long long>(B) * o.T;
             tc_enc_input_kernel<<<static_cast<unsigned>((items + 255) / 256), 256, 0, st>>>(
-                wav, wav_ld, tab + static_cast<size_t>(n + 1) * B, tab, o.raw, o.plane(), o.C, o.Tp, o.T, cf.kernel_size, cf.pad_reflect, B);
+                io.wav_in, io.wav_ld, tab + R.size() * B, tab, o.raw, o.plane(), o.C, o.Tp, o.T, cf.kernel_size, cf.pad_reflect, B);
             VCB_CUDA_OK(cudaGetLastError());
             ++*launches;
-        } else if (L.kind == E_RPAD || L.kind == E_LPAD) {
+        } else if (L.kind == L_RPAD || L.kind == L_LPAD) {
+            const Tensor& t = pl.tensors[L.out];
             const Plane& o = P[L.out];
-            __nv_bfloat16* base = o.elu ? o.elu : o.raw;
-            tc_pad_rows_kernel<<<B, 256, 0, st>>>(base, o.plane(), o.C, o.sb, o.st, o.off,
-                                                  L.kind == E_RPAD ? tab + static_cast<size_t>(L.stage) * B : nullptr, o.halo, L.r,
-                                                  o.halo_zero);
-            VCB_CUDA_OK(cudaGetLastError());
-            ++*launches;
+            const bool right = L.kind == L_RPAD;
+            if (pad_rows(o.elu ? o.elu : o.raw, o, right ? tab + static_cast<size_t>(t.stage) * B : nullptr, right ? t.fold : 1,
+                         o.halo_zero))
+                return -1;
         } else {
             const TcGemm& g = *L.g;
             Plane in = P[L.in];
-            if (L.kind == E_DOWN) {                          // folded rows: r plane rows of C channels are one row of r*C
-                const int r = L.r;
+            const int r = pl.tensors[L.in].fold;
+            if (r > 1) {                                     // folded rows: r plane rows of C channels are one row of r*C
                 in.C *= r; in.rcap /= r; in.Tp /= r; in.T /= r; in.halo = 1; in.sb = in.Tp; in.off = 1;
             }
             if (plane_map(&mA, L.in_form == FORM_ELU ? P[L.in].elu : P[L.in].raw, in) ||
                 (L.in2 >= 0 && plane_map(&mB, P[L.in2].raw, P[L.in2])))
                 return -1;
+            const CUtensorMap& a1 = L.in2 >= 0 ? mB : mA;
+            // the call of a plan GEMM: its weights, its A rows, its epilogue (the LSTM steps then only move t_step and row_base)
             TcCall c{};
-            c.mtiles = ((L.kind == E_LSTM_STEPS ? B : in.rcap) + TC_BM - 1) / TC_BM;
+            c.mtiles = ((L.kind == L_LSTM_STEPS ? B : in.rcap) + TC_BM - 1) / TC_BM;
             if (static_cast<long long>(c.mtiles) * g.ntiles > 0x7fffffffll) {
                 set_error("codec_tc: too many tiles");
                 return -1;
@@ -1538,7 +1372,7 @@ int encode_chunk_tc(TcCodec* tc, const float* wav, long long wav_ld, const int* 
             c.rows_total = in.rcap;
             c.rcap[0] = in.rcap;
             c.B = B;
-            if (L.kind != E_LSTM_STEPS) {
+            if (L.kind != L_LSTM_STEPS) {
                 c.in_tm = in.tm;
                 c.in_div = in.tm ? static_cast<int>(in.st) : in.Tp;
                 c.in_halo = in.halo;
@@ -1547,8 +1381,8 @@ int encode_chunk_tc(TcCodec* tc, const float* wav, long long wav_ld, const int* 
             if (L.in2 >= 0) c.rcap[1] = P[L.in2].rcap;
             if (L.out >= 0) {
                 const Plane& o = P[L.out];
-                c.raw = L.out_forms & FORM_RAW ? o.raw : nullptr;
-                c.elu = L.out_forms & FORM_ELU ? o.elu : nullptr;
+                c.raw = o.raw;
+                c.elu = o.elu;
                 c.o_plane = o.plane();
                 c.o_ld = o.C;
                 c.o_sb = o.sb;
@@ -1557,59 +1391,63 @@ int encode_chunk_tc(TcCodec* tc, const float* wav, long long wav_ld, const int* 
                 c.o_halo = pl.tensors[L.out].halo_kind == HALO_UNWRITTEN ? 0 : o.halo;
                 c.o_halo_zero = o.halo_zero;
             }
-            auto rows_f32 = [&](float* f, int ld, int valid, long long sb, long long stt) {
-                c.f32 = f; c.f_ld = ld; c.f_valid = valid; c.f_sb = sb; c.f_st = stt; c.f_off = 0;
+            auto rows = [&](float* f, int ld, int valid, long long sb, long long stt, long long off) {
+                c.f32 = f; c.f_ld = ld; c.f_valid = valid; c.f_sb = sb; c.f_st = stt; c.f_off = off;
             };
-            if (L.f32 == F32_X0) rows_f32(x0f, H, H, 1, Bcap);                 // time-major [T][Bcap][H]
-            if (L.f32 == F32_PRE) rows_f32(pre, 4 * H, 4 * H, 1, Bcap);        // time-major [T][Bcap][4H]
-            if (L.f32 == F32_LAT) rows_f32(latf, tc->Dp, cf.dimension, Tn, 1); // [B][T][Dp]
-            const CUtensorMap& a1 = L.in2 >= 0 ? mB : mA;
-            if (L.kind == E_LSTM_STEPS) {
+            if (L.f32 == F32_X0) rows(buf(BUF_X0), H, H, 1, Bcap, 0);                  // time-major [T][Bcap][H]
+            if (L.f32 == F32_PRE) rows(buf(BUF_PRE), 4 * H, 4 * H, 1, Bcap, 0);         // time-major [T][Bcap][4H]
+            if (L.f32 == F32_COPART) {                                                // the input's rows, halo included
+                rows(buf(BUF_COPART), DS_LD, DS_LD, in.sb, 1, in.off);
+                c.in_store_halo = 1;
+            }
+            if (L.f32 == F32_WAV) {                                                   // [B][T * hop]
+                rows(io.wav, 1, 1, in.T, 1, 0);
+                c.f_scalar = 1;
+            }
+            if (L.f32 == F32_LAT) rows(buf(BUF_LATF), tc->Dp, cf.dimension, in.T, 1, 0);  // [B][T][Dp]
+            if (L.kind == L_LSTM_STEPS) {
                 c.mode = TC_MODE_LSTM;
-                c.pre = pre;
-                c.cst = cst + static_cast<size_t>(L.lstm) * Bcap * H;
-                c.hseq = P[L.in].raw;
-                c.h_plane = P[L.in].plane();
+                c.pre = buf(BUF_PRE);
+                c.cst = buf(BUF_CST) + static_cast<size_t>(L.lstm) * Bcap * H;
+                c.hseq = in.raw;
+                c.h_plane = in.plane();
                 c.Bcap = Bcap;
                 c.H = H;
-                if (L.out >= 0) c.skip = x0f;
-                if (L.lstm >= 2 && clear_h0(P[L.in])) return -1;
-                for (int t = 0; t < Tn; ++t) {
+                if (L.out >= 0) c.skip = buf(BUF_X0);
+                if (sc != nullptr) c.stab = sc->table;
+                if (L.lstm >= 2 && clear_h0(in)) return -1;
+                if (carry_lstm(L, in, c.cst, 1, 0)) return -1;
+                for (int t = 0; t < in.T; ++t) {                                      // one step per row of its stage
                     c.t_step = t;
                     c.row_base = t * Bcap;
                     if (tc_launch(tc, mA, a1, g, c, st)) return -1;
                 }
-                *launches += Tn;
+                *launches += in.T;
+                if (carry_lstm(L, in, c.cst, 0, 1)) return -1;
             } else {
                 if (tc_launch(tc, mA, a1, g, c, st)) return -1;
                 ++*launches;
+                // The epilogue zeroes halo row -t from output row t, 1 <= t <= halo, and a GEMM writes in.T rows (an
+                // encoder strided conv ceil(L/r) of the chunk's longest utterance).  With constant padding an utterance
+                // may be shorter than a halo (the encoder takes rows of any length), and a chunk of only such utterances
+                // writes no row t for some halo rows: they are cleared here, or they would keep whatever an earlier chunk
+                // left in the workspace.  The decoder's tensors are carried: its T >= min_T exceeds every halo, or (a stream
+                // decode of continuing streams only) each halo is the stream's saved tail.
+                const Tensor* t = L.out >= 0 ? &pl.tensors[L.out] : nullptr;
+                if (t && t->halo_kind == HALO_ZERO && !t->tm && !t->carried && in.T <= t->halo)
+                    for (__nv_bfloat16* base : {c.raw, c.elu})
+                        if (base != nullptr && pad_rows(base, P[L.out], nullptr, 1, 1)) return -1;
             }
-            // The epilogue zeroes halo row -t from output row t, 1 <= t <= halo, and a GEMM writes in.T rows (a strided
-            // conv ceil(L/r) of the chunk's longest utterance).  With constant padding an utterance may be shorter than a
-            // halo (rows of any length are taken), and a chunk of only such utterances writes no row t for some halo
-            // rows: they are cleared here, or they would keep whatever an earlier chunk left in the workspace.
-            if (L.kind != E_LSTM_STEPS && L.out >= 0 && pl.tensors[L.out].halo_kind == HALO_ZERO && !P[L.out].tm &&
-                in.T <= P[L.out].halo) {
-                const Plane& o = P[L.out];
-                for (__nv_bfloat16* base : {c.raw, c.elu}) {
-                    if (base == nullptr) continue;
-                    tc_pad_rows_kernel<<<B, 256, 0, st>>>(base, o.plane(), o.C, o.sb, o.st, o.off, nullptr, o.halo, 1, 1);
-                    VCB_CUDA_OK(cudaGetLastError());
-                    ++*launches;
-                }
+            if (L.kind == L_CONV_OUT_SPLIT) {
+                VCB_CUDA_OK(launch_k_pdl(1, tc_diag_sum_kernel, dim3((in.rcap + DS_ROWS - 1) / DS_ROWS), dim3(DS_ROWS), 0, st,
+                                         buf(BUF_COPART), cf.last_kernel_size, tc->co_bias, io.wav, in.rcap, in.Tp, in.halo, in.T, B));
+                ++*launches;
             }
         }
+        if (L.out >= 0 && carry_plane(L.out)) return -1;
         pf.end();
     }
-    float* lat = reinterpret_cast<float*>(tc->ws + w.lat);
-    tc_latent_cm_kernel<<<dim3((Tn + 31) / 32, B), 256, 32 * (cf.dimension + 1) * 4, st>>>(latf, lat, cf.dimension, tc->Dp, Tn);
-    VCB_CUDA_OK(cudaGetLastError());
-    ++*launches;
     pf.finish();
-    out->latent = lat;
-    out->scores = reinterpret_cast<float*>(tc->ws + w.scores);
-    out->codes = reinterpret_cast<int64_t*>(tc->ws + w.codes);
-    out->T = Tn;
     return 0;
 }
 
@@ -1629,9 +1467,6 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, DevBuf<flo
     if (cfg.lstm > 0 && ch0 % 64) return no("LSTM width not a multiple of 64");
     if (cfg.lstm == 0 && ch0 % 64) return no("first stage narrower than one k-block");
     if ((ch0 >> cfg.n_ratios) < 1 || cfg.compress < 1) return no("channel plan");
-    if (2 * cpad(ch0) / TC_BK > TC_MAX_KB || cfg.kernel_size * cpad(cfg.dimension) / TC_BK > TC_MAX_KB ||
-        cfg.residual_kernel_size * cpad(ch0 / 2) / TC_BK > TC_MAX_KB || cfg.last_kernel_size * cpad(cfg.n_filters) / TC_BK > TC_MAX_KB)
-        return no("reduction deeper than the kernel's k-blocks");
     if (getenv("VCB_CODEC_TC") && atoi(getenv("VCB_CODEC_TC")) == 0) return no("disabled by VCB_CODEC_TC=0");
     TcCodecPtr tc(new TcCodec());
     tc->cfg = cfg;
@@ -1653,118 +1488,33 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, DevBuf<flo
     const char* lim = getenv("VCB_CODEC_WS_GB");
     tc->ws_limit = static_cast<size_t>((lim ? atof(lim) : 100.0) * (1ull << 30));
     HostW hw{w_dev, shapes};
-    char nm[160];
-    int rc = 0;
     {
         std::vector<const float*> emb(cfg.n_q);
-        for (int q = 0; q < cfg.n_q && !rc; ++q) {
+        for (int q = 0; q < cfg.n_q; ++q) {
+            char nm[32];
             snprintf(nm, sizeof(nm), "vq.%d.embed", q);
             auto it = w_dev.find(nm);
             if (it == w_dev.end()) {
                 set_error("codec: missing weight %s", nm);
-                rc = -1;
-            } else {
-                emb[q] = it->second;
+                return -1;
             }
+            emb[q] = it->second;
         }
-        if (!rc && (tc->d_embed.alloc(cfg.n_q) ||
-                    cudaMemcpy(tc->d_embed, emb.data(), cfg.n_q * sizeof(float*), cudaMemcpyHostToDevice) != cudaSuccess)) {
+        if (tc->d_embed.alloc(cfg.n_q) || cudaMemcpy(tc->d_embed, emb.data(), cfg.n_q * sizeof(float*), cudaMemcpyHostToDevice) != cudaSuccess) {
             set_error("codec_tc: codebook pointer table");
-            rc = -1;
+            return -1;
         }
     }
-    if (!rc) rc = build_conv(tc->conv_in, hw, "dec.conv_in", cfg.dimension, ch0, cfg.kernel_size, 1);
-    tc->pre.resize(cfg.lstm);
-    tc->step.resize(cfg.lstm);
-    for (int l = 0; l < cfg.lstm && !rc; ++l) {
-        char a[96], b[96], c2[96];
-        snprintf(a, sizeof(a), "dec.lstm.weight_ih_l%d", l);
-        snprintf(b, sizeof(b), "dec.lstm.bias_ih_l%d", l);
-        snprintf(c2, sizeof(c2), "dec.lstm.bias_hh_l%d", l);
-        rc = build_lstm(tc->pre[l], hw, a, b, c2, ch0, 0);
-        snprintf(a, sizeof(a), "dec.lstm.weight_hh_l%d", l);
-        if (!rc) rc = build_lstm(tc->step[l], hw, a, "", "", ch0, step_bn);
-    }
-    tc->up.resize(cfg.n_ratios);
-    tc->res1.resize(cfg.n_ratios);
-    tc->res2.resize(cfg.n_ratios);
-    int ch = ch0;
-    for (int i = 0; i < cfg.n_ratios && !rc; ++i) {
-        snprintf(nm, sizeof(nm), "dec.up%d.convtr", i);
-        rc = build_convtr(tc->up[i], hw, nm, ch, ch / 2, cfg.ratios[i]);
-        ch /= 2;
-        tc->res1[i].resize(cfg.n_residual_layers);
-        tc->res2[i].resize(cfg.n_residual_layers);
-        for (int j = 0, dil = 1; j < cfg.n_residual_layers && !rc; ++j, dil *= cfg.dilation_base) {
-            snprintf(nm, sizeof(nm), "dec.up%d.res%d.conv1", i, j);
-            rc = build_conv(tc->res1[i][j], hw, nm, ch, ch / cfg.compress, cfg.residual_kernel_size, dil);
-            snprintf(nm, sizeof(nm), "dec.up%d.res%d", i, j);
-            if (!rc) rc = build_res_tail(tc->res2[i][j], hw, nm, ch, ch / cfg.compress);
-        }
-    }
-    if (!rc) rc = build_conv(tc->conv_out, hw, "dec.conv_out", ch, 1, cfg.last_kernel_size, 1, 32);
-    if (!rc && cfg.last_kernel_size <= DS_LD && !(getenv("VCB_CODEC_CONVOUT_TC") && atoi(getenv("VCB_CODEC_CONVOUT_TC")))) {
-        std::vector<float> w, b;
-        rc = hw.get("dec.conv_out.weight", w) || hw.get("dec.conv_out.bias", b) ? -1 : 0;
-        if (!rc) {
-            const int Cp = cpad(ch), k = cfg.last_kernel_size;
-            std::vector<float> W(static_cast<size_t>(k) * Cp, 0.f);          // GEMM row j = tap j
-            for (int ci = 0; ci < ch; ++ci)
-                for (int j = 0; j < k; ++j) W[static_cast<size_t>(j) * Cp + ci] = w[static_cast<size_t>(ci) * k + j];
-            TcGemm& g = tc->conv_out_p;
-            for (int cb = 0; cb < Cp / TC_BK; ++cb) g.taps.push_back(TcTap{0, 0, cb * TC_BK});
-            g.Cout = 32;
-            g.up = 1;
-            rc = upload_gemm(g, W, std::vector<float>(), k, Cp, 32);
-            tc->co_bias = b[0];
-            tc->co_split = rc == 0;
-        }
-    }
-    if (rc) return -1;
-    build_plan(tc.get());
+    const int rc = build_dec(tc.get(), hw, step_bn);
+    if (rc > 0) return no("reduction deeper than the kernel's k-blocks");
+    if (rc < 0) return -1;
     if (w_dev.count("enc.conv_in.weight")) {
-        // the encoder: the decoder's coverage, plus an input window that fits one k-block and reductions within TC_MAX_KB
-        const int n = cfg.n_ratios, kres = cfg.residual_kernel_size;
-        bool deep = cfg.kernel_size > TC_BK || cfg.last_kernel_size * cpad(ch0) / TC_BK > TC_MAX_KB;
-        for (int s = 0, c = cfg.n_filters; s < n; ++s, c *= 2)
-            deep = deep || 2 * cfg.ratios[n - 1 - s] * cpad(c) / TC_BK > TC_MAX_KB || kres * cpad(c) / TC_BK > TC_MAX_KB;
-        if (deep) {
-            tc->enc_reason = "encoder reduction deeper than the kernel's k-blocks";
-        } else {
-            tc->enc.reset(new TcEncoder());
-            TcEncoder& E = *tc->enc;
-            rc = build_enc_conv_in(E.conv_in, hw, cfg.kernel_size, cfg.n_filters);
-            E.down.resize(n);
-            E.res1.resize(n);
-            E.res2.resize(n);
-            for (int s = 0, c = cfg.n_filters; s < n && !rc; ++s, c *= 2) {
-                E.res1[s].resize(cfg.n_residual_layers);
-                E.res2[s].resize(cfg.n_residual_layers);
-                for (int j = 0, dil = 1; j < cfg.n_residual_layers && !rc; ++j, dil *= cfg.dilation_base) {
-                    snprintf(nm, sizeof(nm), "enc.down%d.res%d.conv1", s, j);
-                    rc = build_conv(E.res1[s][j], hw, nm, c, c / cfg.compress, kres, dil);
-                    snprintf(nm, sizeof(nm), "enc.down%d.res%d", s, j);
-                    if (!rc) rc = build_res_tail(E.res2[s][j], hw, nm, c, c / cfg.compress);
-                }
-                snprintf(nm, sizeof(nm), "enc.down%d.conv", s);
-                if (!rc) rc = build_down(E.down[s], hw, nm, c, 2 * c, cfg.ratios[n - 1 - s]);
-            }
-            E.pre.resize(cfg.lstm);
-            E.step.resize(cfg.lstm);
-            for (int l = 0; l < cfg.lstm && !rc; ++l) {
-                char a[96], b[96], c2[96];
-                snprintf(a, sizeof(a), "enc.lstm.weight_ih_l%d", l);
-                snprintf(b, sizeof(b), "enc.lstm.bias_ih_l%d", l);
-                snprintf(c2, sizeof(c2), "enc.lstm.bias_hh_l%d", l);
-                rc = build_lstm(E.pre[l], hw, a, b, c2, ch0, 0);
-                snprintf(a, sizeof(a), "enc.lstm.weight_hh_l%d", l);
-                if (!rc) rc = build_lstm(E.step[l], hw, a, "", "", ch0, step_bn);
-            }
-            if (!rc) rc = build_conv(E.conv_out, hw, "enc.conv_out", ch0, cfg.dimension, cfg.last_kernel_size, 1);
-            if (rc) return -1;
-            build_enc_plan(tc.get());
-            tc->enc_reason = "";
-        }
+        // the encoder where the decoder is covered, its input window fits one k-block and every reduction fits the kernel;
+        // otherwise enc_encode_ragged encodes every row on the CUDA cores
+        tc->enc.reset(new Plan());
+        const int erc = build_enc(tc.get(), hw, step_bn);
+        if (erc < 0) return -1;
+        if (erc > 0) tc->enc.reset();
     }
     *out = std::move(tc);
     return 0;
@@ -1772,85 +1522,106 @@ int tc_codec_build(const enc_config& cfg, const std::map<std::string, DevBuf<flo
 
 bool tc_encoder_active(const TcCodec* c) { return c != nullptr && c->enc != nullptr; }
 
-const char* tc_encoder_reason(const TcCodec* c) { return c ? c->enc_reason : "the tensor-core codec is not active"; }
-
 // every stage longer than the padding its convolutions reflect (audiocraft pad1d zero-extends a shorter input instead)
 bool tc_encoder_accepts(const TcCodec* c, int len) {
     if (!tc_encoder_active(c) || len < 1) return false;
     const enc_config& cf = c->cfg;
     if (!cf.pad_reflect) return true;
-    const std::vector<int> L = enc_chain(c->enc->plan, len);
+    const std::vector<int> L = enc_chain(*c->enc, len);
     int dmax = 1;
     for (int j = 1; j < cf.n_residual_layers; ++j) dmax *= cf.dilation_base;
     const int res_pad = cf.n_residual_layers > 0 ? (cf.residual_kernel_size - 1) * dmax : 0;
     if (L[0] <= cf.kernel_size - 1) return false;
-    for (size_t s = 0; s < c->enc->plan.ratios.size(); ++s)
-        if (L[s] <= res_pad || L[s] <= c->enc->plan.ratios[s]) return false;
+    for (size_t s = 0; s < c->enc->ratios.size(); ++s)
+        if (L[s] <= res_pad || L[s] <= c->enc->ratios[s]) return false;
     return L.back() > cf.last_kernel_size - 1;
 }
 
-size_t tc_encoder_ws_bytes(const TcCodec* c, int B, int N) { return enc_ws_layout(c, B, N).bytes; }
+size_t tc_encoder_ws_bytes(const TcCodec* c, int B, int N) {
+    return ws_layout(c, *c->enc, B, enc_rows(*c->enc, enc_chain(*c->enc, N))).bytes;
+}
 
 size_t tc_ws_limit(const TcCodec* c) { return c->ws_limit; }
 
 int64_t tc_encoder_rows(const TcCodec* c, int B, int N) {
-    return static_cast<int64_t>(B) * enc_rows(c->enc->plan, enc_chain(c->enc->plan, N))[0];
+    return static_cast<int64_t>(B) * enc_rows(*c->enc, enc_chain(*c->enc, N))[0];
 }
 
+// One chunk: utterance b = wav row rows[b] with lens[b] samples; the chunk's planes are sized for its longest utterance.
 int tc_encoder_encode(TcCodec* tc, const float* wav, long long wav_ld, const int* rows, const int* lens, int B, cudaStream_t st,
                       int64_t* launches, TcEncOut* out) {
     tc->prof.clear();
-    const size_t need = enc_ws_layout(tc, B, *std::max_element(lens, lens + B)).bytes;
-    if (need > tc->ws.size()) {
-        if (tc->ws) VCB_CUDA_OK(cudaStreamSynchronize(st));      // alloc releases the previous workspace first
-        if (tc->ws.alloc(need)) {
-            const std::string why = get_error();
-            set_error("codec_tc: cannot allocate a %.2f GB encoder workspace for %d utterances (%s)", need / 1073741824.0, B,
-                      why.c_str());
-            return -1;
+    const Plan& pl = *tc->enc;
+    const int n = static_cast<int>(pl.ratios.size());
+    const std::vector<int> R = enc_rows(pl, enc_chain(pl, *std::max_element(lens, lens + B)));
+    const WsLayout w = ws_layout(tc, pl, B, R);
+    if (grow_ws(tc, w.bytes, st, "encoder workspace for " + std::to_string(B) + " utterances")) return -1;
+    {
+        std::vector<int> h(static_cast<size_t>(n + 2) * B);
+        for (int b = 0; b < B; ++b) {
+            const std::vector<int> L = enc_chain(pl, lens[b]);
+            for (int s = 0; s <= n; ++s) h[static_cast<size_t>(s) * B + b] = L[s];
+            h[static_cast<size_t>(n + 1) * B + b] = rows[b];
         }
+        VCB_CUDA_OK(cudaMemcpyAsync(tc->ws + w.buf[BUF_TAB], h.data(), h.size() * 4, cudaMemcpyHostToDevice, st));   // pageable: staged at once
     }
-    return encode_chunk_tc(tc, wav, wav_ld, rows, lens, B, st, launches, out);
+    ChunkIO io;
+    io.wav_in = wav;
+    io.wav_ld = wav_ld;
+    if (run_chunk(tc, *tc->enc, w, B, R, st, launches, io)) return -1;
+    const int Tn = R[n];
+    const float* latf = reinterpret_cast<const float*>(tc->ws + w.buf[BUF_LATF]);
+    float* lat = reinterpret_cast<float*>(tc->ws + w.buf[BUF_LAT]);
+    tc_latent_cm_kernel<<<dim3((Tn + 31) / 32, B), 256, 32 * (tc->D + 1) * 4, st>>>(latf, lat, tc->D, tc->Dp, Tn);
+    VCB_CUDA_OK(cudaGetLastError());
+    ++*launches;
+    out->latent = lat;
+    out->scores = reinterpret_cast<float*>(tc->ws + w.buf[BUF_SCORES]);
+    out->codes = reinterpret_cast<int64_t*>(tc->ws + w.buf[BUF_CODES]);
+    out->T = Tn;
+    return 0;
 }
 
-bool tc_codec_accepts(const TcCodec* c, int B, int T) { return c != nullptr && B >= 1 && T >= c->plan.min_T; }
+bool tc_codec_accepts(const TcCodec* c, int B, int T) { return c != nullptr && B >= 1 && T >= c->dec.min_T; }
 
 int tc_codec_decode(TcCodec* tc, const int64_t* codes, float* wav, int B, int T, cudaStream_t st, int64_t* launches,
                     const TcStreamCtx* sc) {
     tc->prof.clear();
+    const std::vector<int> R = dec_rows(tc->dec, T);
     // chunk the batch so the workspace stays under the limit -- and halve the chunk again if the device cannot give that much
     int chunk = B;
     for (;;) {
-        const size_t need = ws_layout(tc, chunk, T).bytes;
+        const size_t need = ws_layout(tc, tc->dec, chunk, R).bytes;
         if (need > tc->ws_limit && chunk > 1) {
             chunk = (chunk + 1) / 2;
             continue;
         }
-        if (need <= tc->ws.size()) break;
-        if (tc->ws) VCB_CUDA_OK(cudaStreamSynchronize(st));   // alloc releases the previous workspace first
-        if (tc->ws.alloc(need) == 0) break;
-        if (chunk == 1) {
-            const std::string why = get_error();
-            set_error("codec_tc: cannot allocate a %.2f GB workspace for one utterance of %d frames (%s)", need / 1073741824.0, T,
-                      why.c_str());
-            return -1;
-        }
+        if (grow_ws(tc, need, st, "workspace for one utterance of " + std::to_string(T) + " frames") == 0) break;
+        if (chunk == 1) return -1;
         chunk = (chunk + 1) / 2;
     }
     for (int b0 = 0; b0 < B; b0 += chunk) {
         const int nb = std::min(chunk, B - b0);
+        const WsLayout w = ws_layout(tc, tc->dec, nb, R);
         TcStreamCtx part;
-        if (sc != nullptr) part = TcStreamCtx{sc->table + 4 * b0, sc->state};
-        if (decode_chunk_tc(tc, codes + static_cast<size_t>(b0) * tc->cfg.n_q * T, wav + static_cast<size_t>(b0) * T * tc->hop, nb, T, st,
-                            launches, sc != nullptr ? &part : nullptr))
-            return -1;
+        ChunkIO io;
+        io.codes = codes + static_cast<size_t>(b0) * tc->cfg.n_q * T;
+        io.wav = wav + static_cast<size_t>(b0) * T * tc->hop;
+        if (sc != nullptr) {
+            part = TcStreamCtx{sc->table + 4 * b0, sc->state};
+            io.sc = &part;
+        }
+        tc->dbg_cst = tc->cfg.lstm > 0 ? reinterpret_cast<const float*>(tc->ws + w.buf[BUF_CST]) : nullptr;
+        tc->dbg_B = nb;
+        tc->dbg_Bcap = bcap(nb);
+        if (run_chunk(tc, tc->dec, w, nb, R, st, launches, io)) return -1;
     }
     return 0;
 }
 
-size_t tc_stream_state_bytes(const TcCodec* c) { return c->plan.stream_bytes; }
+size_t tc_stream_state_bytes(const TcCodec* c) { return c->dec.stream_bytes; }
 
-int tc_stream_min_frames(const TcCodec* c) { return c->plan.min_T; }
+int tc_stream_min_frames(const TcCodec* c) { return c->dec.min_T; }
 
 int tc_codes_check(const int64_t* codes, long long n, int bins, int* bad_dev, int* bad_host, cudaStream_t st) {
     VCB_CUDA_OK(cudaMemsetAsync(bad_dev, 0, sizeof(int), st));
@@ -1881,9 +1652,9 @@ int tc_codec_debug_tensor(TcCodec* tc, const char* name, float* host_out, int64_
                                static_cast<size_t>(B) * H * 4, cudaMemcpyDeviceToHost));
         return 0;
     }
-    auto& m = strncmp(name, "enc.", 4) ? tc->dbg : tc->edbg;
-    auto it = m.find(name);
-    if (it == m.end()) {
+    const Plan* plan = strncmp(name, "enc.", 4) ? &tc->dec : tc->enc.get();
+    const auto it = plan ? plan->dbg.find(name) : std::map<std::string, Dbg>::const_iterator();
+    if (plan == nullptr || it == plan->dbg.end()) {
         set_error("codec_tc: no tensor '%s' in the last decode or tensor-core encode", name);
         return -1;
     }

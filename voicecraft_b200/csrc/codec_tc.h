@@ -1,4 +1,4 @@
-// Interface between encodec.cu (C ABI, weight store, CUDA-core kernels) and codec_tc.cu (tensor-core decoder).
+// Interface between encodec.cu (C ABI, weight store, CUDA-core kernels) and codec_tc.cu (tensor-core decoder and encoder).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -46,9 +46,8 @@ const std::vector<std::pair<std::string, float>>& tc_codec_profile(const TcCodec
 // VCB_CODEC_KEEP=1 at tc_codec_build no two tensors share rows, so every one of them holds what its layer stored.
 int tc_codec_debug_tensor(TcCodec* c, const char* name, float* host_out, int64_t cap, int32_t* dims);
 
-// ---- tensor-core encoder (built with the decoder when the enc.* weights are loaded)
+// ---- tensor-core encoder (built with the decoder when the enc.* weights are loaded and it is covered)
 bool tc_encoder_active(const TcCodec* c);
-const char* tc_encoder_reason(const TcCodec* c);
 // whether an utterance of len samples can run here (every stage longer than the padding it reflects)
 bool tc_encoder_accepts(const TcCodec* c, int len);
 // workspace of a chunk of B utterances of at most N samples; the VCB_CODEC_WS_GB limit the host chunks under
