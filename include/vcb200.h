@@ -311,6 +311,10 @@ int vcb_bench_gemm(int32_t N, int32_t K, int32_t B, int32_t splits, int32_t stag
  * CTA or a k-block per split). */
 int vcb_gemm_launch_shape(int32_t N, int32_t K, int32_t B, int32_t splits, int32_t stages, int32_t cluster_cap,
                           int32_t* out /*[2]*/);
+/* the persistent kernel's ring configuration for VCB_MEGA_NS / _NB / _FLIGHT = ns / nb / flight, as an engine built with
+ * them runs it: out = {ns, nb, flight clamped to [1, ns]}.  Fails, as building the engine does, unless 2 <= ns <= 12,
+ * 3 <= nb <= 8 and ns * 16 KB + nb * 8 KB <= 224 KB. */
+int vcb_mega_ring_config(int32_t ns, int32_t nb, int32_t flight, int32_t* out /*[3]*/);
 /* debug timeline of the persistent decode-step kernel (first call enables it): [2 CTAs][n_phases][8 events] globaltimer ns */
 int vcb_debug_mega_timeline(vcb_engine* e, uint64_t* out_host, int32_t max_records, int32_t* n_phases);
 /* "gemm_simt", "pdl", "profile", "stop_stage" (0 .. 5 L + 2, see vcb_debug_stage_read) */
@@ -321,7 +325,9 @@ int vcb_profile_read(vcb_engine* e, double* ms_by_class, int64_t* count_by_class
 /* "launches", "kv_bytes", "kv_pages_free", "kv_pages_total" (pool size), "kv_pages_needed" (pages the last refused
  * vcb_decode_step lacked), "kv_page_bytes" (one page: 64 positions of K and V in every layer), "swap_stage_bytes" (device
  * staging of the swap kernels), "prefill_rows" (rows through the prefill since create), "weight_bytes" (device
- * bytes of the packed GEMM operands with their int8 scales, and the int8 prefill scratch once a prefill allocated it), ...; "live_bytes" / "live_handles" (any e, NULL included): device and pinned bytes, and allocations
+ * bytes of the packed GEMM operands with their int8 scales, and the int8 prefill scratch once a prefill allocated it),
+ * "mega_grid" (the persistent kernel's grid, 0: not available), "mega_ns" / "mega_nb" / "mega_flight" / "mega_pf" (the ring
+ * configuration it runs, 0 without it), ...; "live_bytes" / "live_handles" (any e, NULL included): device and pinned bytes, and allocations
  * plus events, the library holds now across every engine, codec engine and stream of the process */
 int64_t vcb_counter(vcb_engine* e, const char* name);
 

@@ -92,6 +92,7 @@ PROTOTYPES = {
     "vcb_timeline": (C.c_int, [C.c_int32, C.POINTER(C.c_uint64), C.c_int32, C.POINTER(C.c_int32)]),
     "vcb_bench_gemm": (C.c_int, [C.c_int32] * 8 + [C.POINTER(C.c_float)]),
     "vcb_gemm_launch_shape": (C.c_int, [C.c_int32] * 6 + [C.POINTER(C.c_int32)]),
+    "vcb_mega_ring_config": (C.c_int, [C.c_int32] * 3 + [C.POINTER(C.c_int32)]),
     "vcb_debug_mega_timeline": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64), C.c_int32, C.POINTER(C.c_int32)]),
     "vcb_set_option": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int32]),
     "vcb_profile_read": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int64), C.c_int32]),

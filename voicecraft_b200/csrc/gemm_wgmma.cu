@@ -1061,21 +1061,27 @@ int gemm_launch(const GemmCall& g, cudaStream_t st) {
         }
         return 0;
     }
-    int splits = 0, stages = 0;
+    int splits = 0;
+    if (gemm_tc_splits(g, splits)) return -1;
+    return (g.w8 ? find_variant_w8(g.bpad) : find_variant(g.bpad)).launch(g, splits, st);
+}
+
+// The split count the tensor-core launch of g runs, or -1 with the reason where gemm_launch would refuse it.
+int gemm_tc_splits(const GemmCall& g, int& splits) {
+    int stages = 0;
     if (gemm_launch_shape(g, 0, splits, stages)) return -1;
-    if (!g.w8) return find_variant(g.bpad).launch(g, splits, st);
+    if (!g.w8) return 0;
     // int8 weights: the bf16 kernel's launch shape (split count and K slices), on 128-k tiles
     if (g.Kdim % 128) {
         set_error("gemm: int8 weights need K %% 128 == 0 (K=%d)", g.Kdim);
         return -1;
     }
-    const GemmVariant v = find_variant_w8(g.bpad);
-    const int placeable = v.occupancy().max_cluster;
+    const int placeable = find_variant_w8(g.bpad).occupancy().max_cluster;
     if (placeable < splits) {
         if (placeable) set_error("gemm: the int8-weight kernel for bpad %d places clusters of at most %d, not %d", g.bpad, placeable, splits);
         return -1;
     }
-    return v.launch(g, splits, st);
+    return 0;
 }
 
 // Cluster size (= K splits) of a launch of `groups` x ceil(Nout / 128) tiles.  `room` = CTAs of this kernel the device

@@ -343,6 +343,29 @@ int run_gemm(vcb_engine* e, const Matrix& W, const CUtensorMap* tmB, const __nv_
     return gemm_launch(g, st);
 }
 
+// The VCB_SPLITS entries of a pass at `bpad` rows through run_gemm's matrices (the layers' four and the first head stage),
+// checked as gemm_launch checks them.  A step calls this before it enqueues anything: an entry the launcher refuses then
+// fails the step with its slots as they were, not mid-step with the positions advanced and nothing written.
+int check_split_overrides(const vcb_engine* e, int bpad) {
+    if (e->opt_splits.empty() || e->opt_simt) return 0;
+    const ModelDims& m = e->m;
+    const int shapes[5][2] = {{3 * m.d, m.d}, {m.d, m.d}, {m.F, m.d}, {m.d, m.F}, {m.K * m.Hh, m.d}};
+    for (const auto& o : e->opt_splits)
+        for (const auto& sh : shapes) {
+            if (o[0] != sh[0] || o[1] != sh[1]) continue;
+            GemmCall g;
+            g.Nout = sh[0];
+            g.Kdim = sh[1];
+            g.bpad = bpad;
+            g.splits = o[2];
+            g.w8 = e->w8;
+            int s = 0;
+            if (gemm_tc_splits(g, s)) return -1;
+            break;
+        }
+    return 0;
+}
+
 // One launch of attn_rows_kernel over `rows` rows of H heads whose contexts are at most max_ctx tokens.  The engine and
 // vcb_debug_attention both go through here, so the chunk count, grid and balance decisions under test are the engine's.
 struct AttnLaunch {
@@ -819,6 +842,13 @@ int mega_setup(vcb_engine* e) {
     e->mega_grid = 0;
     // (the persistent kernel has no fp8 KV path: fp8 engines take the per-kernel step)
     if (!e->opt_mega || !e->opt_fold || e->opt_simt || e->kv_dtype == KV_FP8 || e->w8 || m.hd != 128 || m.d % 128 || m.F % 128 || (m.K * m.Hh) % 128 || m.Hh % 64) return 0;
+    if (getenv("VCB_MEGA_NS")) e->mega_ns = atoi(getenv("VCB_MEGA_NS"));
+    if (getenv("VCB_MEGA_NB")) e->mega_nb = atoi(getenv("VCB_MEGA_NB"));
+    if (getenv("VCB_MEGA_PF")) e->mega_pf = atoi(getenv("VCB_MEGA_PF"));
+    if (getenv("VCB_MEGA_FLIGHT")) e->mega_flight = atoi(getenv("VCB_MEGA_FLIGHT"));
+    int ring[3];
+    if (mega_ring_config(e->mega_ns, e->mega_nb, e->mega_flight, ring)) return -1;
+    e->mega_flight = ring[2];
     int grid = std::min(mega_max_grid(32, e->kv_dtype == KV_FP32), mega_max_grid(16, e->kv_dtype == KV_FP32));
     if (getenv("VCB_MEGA_GRID")) grid = std::min(grid, atoi(getenv("VCB_MEGA_GRID")));
     if (grid < 1) return 0;
@@ -864,14 +894,6 @@ int mega_setup(vcb_engine* e) {
     wp[4 * m.L] = e->h1.w;
     for (int k = 0; k < m.K; ++k) wp[4 * m.L + 1 + k] = e->h2[k].w;
     VCB_CUDA_OK(cudaMemcpy(e->d_wptrs, wp.data(), wp.size() * sizeof(void*), cudaMemcpyHostToDevice));
-    if (getenv("VCB_MEGA_NS")) e->mega_ns = atoi(getenv("VCB_MEGA_NS"));
-    if (getenv("VCB_MEGA_NB")) e->mega_nb = atoi(getenv("VCB_MEGA_NB"));
-    if (getenv("VCB_MEGA_PF")) e->mega_pf = atoi(getenv("VCB_MEGA_PF"));
-    if (getenv("VCB_MEGA_FLIGHT")) e->mega_flight = std::max(1, atoi(getenv("VCB_MEGA_FLIGHT")));
-    if (e->mega_ns < 2 || e->mega_ns > 13 || e->mega_nb < 3 || e->mega_nb > 8 || e->mega_ns * 16384 + e->mega_nb * 8192 > 14 * 16384) {
-        set_error("VCB_MEGA_NS / VCB_MEGA_NB: need 2 <= ns <= 13, 3 <= nb <= 8, ns * 16 KB + nb * 8 KB <= 224 KB");
-        return -1;
-    }
     e->mega_grid = grid;
     if (mega_build(e, 16) || mega_build(e, 32)) return -1;
     return 0;
@@ -1711,10 +1733,12 @@ int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float*
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
     if (check_slots(e, slots, n) || noise_required(e, slots, n, exp_noise_dev) || sampling_required(e, slots, n, sp))
         return -1;
+    const bool fold = e->opt_fold && !e->opt_simt;
+    const bool mega = fold && e->mega_grid > 0 && n <= 32;
+    if (!mega && check_split_overrides(e, bpad_for(n))) return -1;
     static thread_local std::vector<std::pair<int, int>> grow;
     if (const int rc = plan_growth(e, slots, n, grow)) return rc;
     if (upload_slots(e, slots, n, st) || apply_growth(e, grow, st)) return -1;
-    const bool fold = e->opt_fold && !e->opt_simt;
     Pass p = step_pass(e, n, fold);
     {
         ProfScope ps(e, PC_MISC, st);
@@ -1724,12 +1748,12 @@ int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float*
                              e->ln_stats, e->page_table, e->max_pages_per_slot, e->row_page, e->row_pages, e->row_forced,
                              e->mega_flags, e->mega_flags ? e->mega_nph : 0, reinterpret_cast<unsigned int*>(e->mega_tile_cnt.get()),
                              e->mega_flags ? e->mega_nph * e->mega_cnt_stride : 0,
-                             (fold && e->mega_grid > 0 && n <= 32) ? e->mact_d : static_cast<__nv_bfloat16*>(nullptr)));
+                             mega ? e->mact_d : static_cast<__nv_bfloat16*>(nullptr)));
     }
     LAUNCH_COUNT(e);
     for (int i = 0; i < n; ++i) p.max_ctx = std::max(p.max_ctx, ++e->h_seq_len[slots[i]]);
     p.stop = e->opt_stop;
-    if (fold && e->mega_grid > 0 && n <= 32) {
+    if (mega) {
         Pass v = p;                    // the buffers the persistent kernel works on (mega_build)
         v.bpad = bpad_for(n);
         v.act_d.act = e->mact_d;
@@ -2572,6 +2596,17 @@ int vcb_gemm_launch_shape(int32_t N, int32_t Kd, int32_t B, int32_t splits, int3
     return 0;
 }
 
+int vcb_mega_ring_config(int32_t ns, int32_t nb, int32_t flight, int32_t* out) {
+    if (!out) {
+        set_error("vcb_mega_ring_config: an output array required");
+        return -1;
+    }
+    int r[3];
+    if (mega_ring_config(ns, nb, flight, r)) return -1;
+    std::copy(r, r + 3, out);
+    return 0;
+}
+
 // Debug timeline: device-side (tag, globaltimer) records written by CTA 0 of the instrumented kernels.
 int vcb_timeline(int32_t enable, uint64_t* out_host, int32_t max_records, int32_t* n_out) {
     static unsigned long long* buf = nullptr;
@@ -2659,6 +2694,10 @@ int64_t vcb_counter(vcb_engine* e, const char* name) {
     if (!strcmp(name, "launches")) return e->n_launches;
     if (!strcmp(name, "num_sms")) return e->num_sms;
     if (!strcmp(name, "mega_grid")) return e->mega_grid;
+    if (!strcmp(name, "mega_ns")) return e->mega_grid ? e->mega_ns : 0;
+    if (!strcmp(name, "mega_nb")) return e->mega_grid ? e->mega_nb : 0;
+    if (!strcmp(name, "mega_flight")) return e->mega_grid ? e->mega_flight : 0;
+    if (!strcmp(name, "mega_pf")) return e->mega_grid ? e->mega_pf : 0;
     if (!strcmp(name, "poll_frames")) return e->n_poll_frames;
     if (!strcmp(name, "kv_pages_free")) return static_cast<int64_t>(e->free_pages.size());
     if (!strcmp(name, "kv_pages_total")) return e->n_pages;

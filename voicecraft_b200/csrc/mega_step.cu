@@ -32,10 +32,12 @@ namespace vcb {
 
 static constexpr int MG_THREADS = 384;
 static constexpr int MG_SLOT = 16384;          // ring slot = one 128 x 64 bf16 weight block = one bf16 K (or V) slab
-static constexpr int MG_NS_MAX = 13;           // ring slots (MegaArgs::ns of them are used)
-static constexpr int MG_NB_MAX = 8;            // activation (B operand) ring slots (MegaArgs::nb)
 static constexpr int MG_POOL = 14 * 16384;     // bytes shared by the two rings: ns * 16 KB + nb * 8 KB <= MG_POOL
 static constexpr int MG_BSLOT = 8192;          // 64 rows (32 hi + 32 lo) x 64 k, bf16
+static constexpr int MG_NB_MIN = 3;            // activation (B operand) ring slots (MegaArgs::nb): the attention scratch
+static constexpr int MG_NB_MAX = 8;            //   aliases three of them
+static constexpr int MG_NS_MIN = 2;            // ring slots (MegaArgs::ns): at most what the pool leaves beside the
+static constexpr int MG_NS_MAX = (MG_POOL - MG_NB_MIN * MG_BSLOT) / MG_SLOT;   //   smallest B ring (12)
 static constexpr int MG_HD = 128;
 static constexpr int MG_PAGE = 64;
 static constexpr int MG_CHUNK = 4;             // attention: pages per work item (a chunk of one (row, head))
@@ -54,7 +56,7 @@ struct MegaSmem {
     static constexpr int A_Q = A_CHUNKS + MG_MAXCH * MG_PSTR * 4;   // q * scale * log2(e) of this / the next chunk [2][128]
     static constexpr int A_END = A_Q + 2 * MG_HD * 4;
 };
-static_assert(MegaSmem::A_END <= 3 * MG_BSLOT, "attention scratch must fit three B slots (nb >= 3)");
+static_assert(MegaSmem::A_END <= MG_NB_MIN * MG_BSLOT, "attention scratch must fit the smallest B ring");
 static_assert(MegaSmem::TOTAL <= 232448, "shared memory budget of one CTA per SM");
 
 __device__ __forceinline__ unsigned int mg_ld_acquire(const unsigned int* p) {
@@ -1046,5 +1048,20 @@ int mega_max_grid(int bpad, int kv_fp32) {
 }
 
 size_t mega_part_floats(int grid, int bpad) { return static_cast<size_t>(grid) * MEGA_MAXSEG * bpad * 128; }
+
+// The ring depths must fit the pool.  The ring producer may have at most ns loads in flight: it waits for the oldest
+// in-flight load on its slot's full barrier with that load's phase parity, and with more than ns in flight the slot has
+// been refilled since, so the parity names a later phase that only loads it has not issued yet can complete.
+int mega_ring_config(int ns, int nb, int flight, int* out) {
+    if (ns < MG_NS_MIN || ns > MG_NS_MAX || nb < MG_NB_MIN || nb > MG_NB_MAX || ns * MG_SLOT + nb * MG_BSLOT > MG_POOL) {
+        set_error("VCB_MEGA_NS / VCB_MEGA_NB = %d / %d: need %d <= ns <= %d, %d <= nb <= %d and ns * 16 KB + nb * 8 KB <= %d KB", ns,
+                  nb, MG_NS_MIN, MG_NS_MAX, MG_NB_MIN, MG_NB_MAX, MG_POOL / 1024);
+        return -1;
+    }
+    out[0] = ns;
+    out[1] = nb;
+    out[2] = std::min(std::max(flight, 1), ns);
+    return 0;
+}
 
 }  // namespace vcb

@@ -270,7 +270,7 @@ struct MegaArgs {
     int nph = 0, nvalid = 0, bpad = 0, kv_fp32 = 0;
     int ns = 11, nb = 6;                // ring depths: ns * 16 KB + nb * 8 KB <= 224 KB
     int pf = 0;                         // L2 prefetch distance in ring items (0 = off)
-    int flight = 5;                     // ring loads in flight (issued, not landed) per SM
+    int flight = 5;                     // ring loads in flight (issued, not landed) per SM, 1 .. ns
     unsigned int* flags = nullptr;      // [nph] completion counters (zeroed by step_prep)
     int* tile_cnt = nullptr;            // [nph][max tiles] split-K arrival counters (self-resetting)
     int tile_cnt_stride = 0;
@@ -292,6 +292,9 @@ struct MegaArgs {
 int mega_launch(const MegaArgs& a, int grid, cudaStream_t st);
 int mega_max_grid(int bpad, int kv_fp32);
 size_t mega_part_floats(int grid, int bpad);
+// ring depths (ns, nb) and loads in flight as the kernel runs them: out = {ns, nb, flight clamped to [1, ns]}; -1 and the
+// rule in vcb_last_error where (ns, nb) does not fit the shared-memory pool
+int mega_ring_config(int ns, int nb, int flight, int* out);
 
 // Grouped launch of gemm_w_xT_cluster (blockIdx.y = group): weight tensor maps in a device array, per-group bias pointers.
 struct GemmGroup {
@@ -320,6 +323,9 @@ int gemm_launch(const GemmCall& g, cudaStream_t st);
 // What gemm_launch would launch for g: the pipeline stages and the split count after the fallback to the largest cluster
 // the device can place (cluster_cap > 0: as if it could place none larger).  -1 (and the error) where gemm_launch rejects g.
 int gemm_launch_shape(const GemmCall& g, int cluster_cap, int& splits, int& stages);
+// ... and with g.w8's own limit: the split count of the tensor-core launch of g, -1 (and the error) where gemm_launch
+// rejects it.  Host only: nothing is enqueued.
+int gemm_tc_splits(const GemmCall& g, int& splits);
 
 // Rows-as-M GEMM for prefill (gemm_rows.cu): activations [2][rcap][Kdim] (hi plane, lo plane), packed weights as above.
 struct RowsGemmCall {
