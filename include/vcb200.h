@@ -265,6 +265,24 @@ int vcb_debug_attention_groups(const float* q_dev, const void* kpool_dev, const 
                                int32_t max_pages, int32_t chunk_pages, int32_t balance, int32_t repeats,
                                float* out_dev /*[rows][H*hd]*/, const int32_t* group_first, const int32_t* group_shared,
                                int32_t n_groups);
+/* the attention phase of the persistent decode-step kernel (csrc/mega_step.cu, VCB_MEGA=1) alone, through its cooperative
+ * launch: out[r][h*128 + e] = hi + lo of softmax over keys 0..pos[r]-1 of row r's pages (row_pages[r][*], max_pages wide)
+ * and the current key knew[r][h] / value vnew[r][h] at position pos[r], scores q[r][h] . k / sqrt(128).  kv_dtype
+ * VCB_KV_BF16 or VCB_KV_FP32 (the kernel has no fp8 path); hd = 128.  pos[r] = -1: inactive row, whose image is left as
+ * filled (every bit set), so out[r] reads back NaN.  Rows 1..16 run the kernel's BPAD 16 instantiation, 17..32 BPAD 32.
+ * Work items are chunks of 4 pages of one (row, head); CTA c of a grid of G takes the chunks that start in its share
+ * [c*U/G, (c+1)*U/G) of the U (row, head, page) units.  An item of up to 16 chunks (pos < 4096) that one CTA owns folds
+ * on chip; an item shared between CTAs, or of more chunks, folds its chunk states through a workspace.
+ * Launch i runs on grids[i] CTAs (host array, `launches` entries), all on one workspace and one set of arrival counters;
+ * the image is refilled before each launch, and after each launch every arrival counter must be back at 0 (else -1).
+ * Rejected on the host before anything is allocated or launched: rows outside [1, 32], H < 1, max_pages < 1, a kv_dtype
+ * other than bf16 / fp32, a grid outside [1, the kernel's co-resident CTAs], a position beyond max_pages pages and
+ * H * rows * max_pages * (grid + 1) >= 2^31 (the kernel's work split is 32-bit).  Synchronous. */
+int vcb_debug_mega_attention(const float* q_dev /*[rows][H][128]*/, const float* knew_dev /*[rows][H][128]*/,
+                             const float* vnew_dev, const void* kpool_dev, const void* vpool_dev, int32_t kv_dtype,
+                             const int32_t* row_pages_dev /*[rows][max_pages]*/, const int32_t* pos_dev, int32_t rows,
+                             int32_t H, int32_t max_pages, const int32_t* grids, int32_t launches,
+                             float* out_dev /*[rows][H*128]*/);
 /* the fp8 KV quantizer of the QKV epilogues on `rows` rows of hd fp32 values (hd 64 or 128): out gets the e4m3 bytes
  * [rows][hd], then the fp32 scales [rows].  Synchronous. */
 int vcb_debug_kv_quantize(const float* x_dev /*[rows][hd]*/, int32_t rows, int32_t hd, uint8_t* out_dev);

@@ -37,17 +37,19 @@ KINDS = ("wide", "diffuse", "max_first_of_chunk", "max_last", "max_early_chunk",
 Q_SCALE = {"wide": 20.0, "diffuse": 0.3}         # logit std: "wide" spans +-80, "diffuse" spreads the weight over every key
 
 
-def _attn_case(hd, kv, chunk_pages, seed=0):
+def _attn_case(hd, kv, chunk_pages, seed=0, positions=POSITIONS, kinds=KINDS, H=2, plant=None):
     """rows of every (position, score distribution) pair plus two inactive rows; K / V pools [page][H][64][hd] shared by
-    every row through shuffled page lists (one list per row, in a shuffled slot order)."""
-    H = 2
+    every row through shuffled page lists (one list per row, in a shuffled slot order).
+    Kinds beyond KINDS: "underflow_cached" (logit 140 on a cached key of a middle chunk: every other chunk and the key at
+    pos underflow against it) and "self_min" (logit -140 on the key at pos).  Any other kind is planted by
+    plant(r, pos, kind) -> (key index, or one per head, logit) or None, with pos the case's positions (-1: inactive)."""
     g = torch.Generator(device="cpu").manual_seed(1000 * hd + 10 * chunk_pages + (kv == "bf16") + seed)
-    max_pages = (max(POSITIONS) + PAGE) // PAGE + 1
+    max_pages = (max(positions) + PAGE) // PAGE + 1
     n_pool = max_pages + 14
-    n_slots = len(POSITIONS) * len(KINDS) + 2
+    n_slots = len(positions) * len(kinds) + 2
     Kp = torch.randn(n_pool, H, PAGE, hd, generator=g)
     Vp = torch.randn(n_pool, H, PAGE, hd, generator=g)
-    rows = [(p, k) for p in POSITIONS for k in KINDS]
+    rows = [(p, k) for p in positions for k in kinds]
     pos = [p for p, _ in rows]
     q = torch.empty(len(rows), H, hd)
     for r, (p, kind) in enumerate(rows):
@@ -71,19 +73,30 @@ def _attn_case(hd, kv, chunk_pages, seed=0):
             t, logit = p, 40.0
         elif kind == "max_early_chunk":
             t, logit = min(p, 5), 40.0                        # chunk 0, while the row has more chunks after it
-        else:
+        elif kind == "underflow":
             t, logit = p, 140.0                               # every other chunk's weights underflow in fp32
+        elif kind == "underflow_cached":
+            t, logit = min((p // span) // 2 * span + span // 2, max(p - 1, 0)), 140.0
+        elif kind == "self_min":
+            t, logit = p, -140.0
+        else:
+            planted = plant(r, pos, kind)
+            if planted is None:
+                continue
+            t, logit = planted
         plants[r] = (t, logit)
+    heads = {r: sorted(set(t)) if isinstance(t, list) else [t] for r, (t, _) in plants.items()}
     while True:
         page_table = torch.stack([torch.randperm(n_pool, generator=g)[:max_pages] for _ in range(n_slots)]).int()
-        keys = [(int(page_table[row_slot[r], t // PAGE]), t % PAGE) for r, (t, _) in plants.items()]
+        keys = [(int(page_table[row_slot[r], t // PAGE]), t % PAGE) for r in plants for t in heads[r]]
         if len(set(keys)) == len(keys):
             break
     for r, (t, logit) in plants.items():
-        page = int(page_table[row_slot[r], t // PAGE])
         for h in range(H):
+            th = t[h] if isinstance(t, list) else t
+            page = int(page_table[row_slot[r], th // PAGE])
             qv = q[r, h]
-            Kp[page, h, t % PAGE] = qv * (logit * math.sqrt(hd) / float(qv.dot(qv)))
+            Kp[page, h, th % PAGE] = qv * (logit * math.sqrt(hd) / float(qv.dot(qv)))
     if kv == "bf16":
         Kp, Vp = Kp.to(torch.bfloat16), Vp.to(torch.bfloat16)
     return dict(H=H, hd=hd, q=q, Kp=Kp, Vp=Vp, page_table=page_table, row_slot=row_slot,

@@ -85,6 +85,8 @@ PROTOTYPES = {
     "vcb_debug_attention": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 4 + [C.c_int32] * 7 + [C.c_void_p]),
     "vcb_debug_attention_groups": (C.c_int, [C.c_void_p] * 3 + [C.c_int32] + [C.c_void_p] * 2 + [C.c_int32] * 7 +
                                    [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32]),
+    "vcb_debug_mega_attention": (C.c_int, [C.c_void_p] * 5 + [C.c_int32] + [C.c_void_p] * 2 + [C.c_int32] * 3 +
+                                 [C.POINTER(C.c_int32), C.c_int32, C.c_void_p]),
     "vcb_debug_kv_quantize": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]),
     "vcb_debug_kv_pages": (C.c_int, [C.c_void_p] + [C.c_int32] * 4 + [C.c_void_p] * 2),
     "vcb_debug_stage_read": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int32]),

@@ -2375,6 +2375,114 @@ int vcb_debug_attention_groups(const float* q_dev, const void* kpool_dev, const 
                            max_pages, chunk_pages, balance, repeats, out_dev, group_first, group_shared, n_groups);
 }
 
+// Parity hook of the persistent kernel's attention phase; see include/vcb200.h.  A one-phase table (MEGA_ATTN, waiting for
+// nothing) through mega_launch; the buffers are sized and zeroed as mega_setup allocates them, and the completion flag is
+// cleared before every launch as step_prep_kernel clears it before every step.
+int vcb_debug_mega_attention(const float* q_dev, const float* knew_dev, const float* vnew_dev, const void* kpool_dev,
+                             const void* vpool_dev, int32_t kv_dtype, const int32_t* row_pages_dev, const int32_t* pos_dev,
+                             int32_t rows, int32_t H, int32_t max_pages, const int32_t* grids, int32_t launches,
+                             float* out_dev) {
+    constexpr int HD = 128;
+    if (rows < 1 || rows > 32 || H < 1 || max_pages < 1 || launches < 1 || !grids || !q_dev || !knew_dev || !vnew_dev ||
+        !kpool_dev || !vpool_dev || !row_pages_dev || !pos_dev || !out_dev) {
+        set_error("vcb_debug_mega_attention: 1 <= rows <= 32, H >= 1, max_pages >= 1, launches >= 1 and non-null pointers "
+                  "required (rows %d, H %d, max_pages %d, launches %d)", rows, H, max_pages, launches);
+        return -1;
+    }
+    if (kv_dtype != KV_BF16 && kv_dtype != KV_FP32) {
+        set_error("vcb_debug_mega_attention: kv_dtype %d: the persistent kernel reads bf16 or fp32 pages only", kv_dtype);
+        return -1;
+    }
+    const int bpad = rows <= 16 ? 16 : 32, kv_fp32 = kv_dtype == KV_FP32;
+    const int gmax = mega_max_grid(bpad, kv_fp32);
+    for (int i = 0; i < launches; ++i) {
+        if (grids[i] < 1 || grids[i] > gmax) {
+            set_error("vcb_debug_mega_attention: launch %d: grid %d outside [1, %d] (the launch is cooperative)", i, grids[i], gmax);
+            return -1;
+        }
+        if (static_cast<long long>(H) * rows * max_pages * (grids[i] + 1) >= (1ll << 31)) {
+            set_error("vcb_debug_mega_attention: launch %d: H * rows * max_pages * (grid + 1) = %d * %d * %d * %d >= 2^31 (the "
+                      "kernel's work split is 32-bit)", i, H, rows, max_pages, grids[i] + 1);
+            return -1;
+        }
+    }
+    std::vector<int> pos(rows);
+    VCB_CUDA_OK(cudaMemcpy(pos.data(), pos_dev, rows * sizeof(int), cudaMemcpyDeviceToHost));
+    for (int r = 0; r < rows; ++r)
+        if (pos[r] >= max_pages * KV_PAGE) {
+            set_error("vcb_debug_mega_attention: row %d: position %d beyond %d pages", r, pos[r], max_pages);
+            return -1;
+        }
+    const size_t cols = static_cast<size_t>(H) * HD;
+    MegaPhase P;
+    P.type = MEGA_ATTN;
+    P.kpool = kpool_dev;
+    P.vpool = vpool_dev;
+    P.dep_target = 0;
+    DevBuf<MegaPhase> ph;
+    DevBuf<unsigned int> flags;
+    DevBuf<int> tile_cnt, att_cnt;
+    DevBuf<float> part, att_ws;
+    DevBuf<__nv_bfloat16> att_out;
+    PinnedBuf<unsigned int> dbg;
+    const SyncOnExit sync;
+    if (ph.alloc(1) || flags.alloc(1, true) || tile_cnt.alloc(1, true) || part.alloc(1, true) ||
+        att_ws.alloc(static_cast<size_t>(32) * H * max_pages * 132, true) || att_cnt.alloc(static_cast<size_t>(32) * H, true) ||
+        att_out.alloc(2 * bpad * cols) || dbg.alloc(16, true, true))
+        return -1;
+    VCB_CUDA_OK(cudaMemcpy(ph, &P, sizeof(P), cudaMemcpyHostToDevice));
+    MegaArgs a;
+    a.ph = ph;
+    a.nph = 1;
+    a.nvalid = rows;
+    a.bpad = bpad;
+    a.kv_fp32 = kv_fp32;
+    a.flags = flags;
+    a.tile_cnt = tile_cnt;
+    a.tile_cnt_stride = 1;
+    a.part = part;
+    a.dbg = dbg.dev();
+    a.qbuf = q_dev;
+    a.knew = knew_dev;
+    a.vnew = vnew_dev;
+    a.att_out = att_out;
+    a.att_ws = att_ws;
+    a.att_cnt = att_cnt;
+    a.row_pos = pos_dev;
+    a.row_pages = row_pages_dev;
+    a.max_pages = max_pages;
+    a.H = H;
+    a.d = static_cast<int>(cols);
+    a.scale = 1.0f / sqrtf(static_cast<float>(HD));
+    std::vector<int> cnt(static_cast<size_t>(32) * H);
+    for (int i = 0; i < launches; ++i) {
+        VCB_CUDA_OK(cudaMemset(att_out, 0xff, 2 * bpad * cols * sizeof(__nv_bfloat16)));
+        VCB_CUDA_OK(cudaMemset(flags, 0, sizeof(unsigned int)));
+        if (mega_launch(a, grids[i], 0)) return -1;
+        const cudaError_t se = cudaDeviceSynchronize();
+        if (se != cudaSuccess) {
+            if (dbg[0])
+                set_error("vcb_debug_mega_attention: launch %d: bounded wait expired (role %u, phase %u, cta %u, info 0x%x): %s", i,
+                          dbg[1], dbg[2], dbg[3], dbg[4], cudaGetErrorString(se));
+            else
+                set_error("vcb_debug_mega_attention: launch %d: %s", i, cudaGetErrorString(se));
+            return -1;
+        }
+        VCB_CUDA_OK(cudaMemcpy(cnt.data(), att_cnt, cnt.size() * sizeof(int), cudaMemcpyDeviceToHost));
+        for (size_t j = 0; j < cnt.size(); ++j)
+            if (cnt[j] != 0) {
+                set_error("vcb_debug_mega_attention: launch %d (grid %d) left arrival counter %zu (row %zu, head %zu) at %d", i,
+                          grids[i], j, j / H, j % H, cnt[j]);
+                return -1;
+            }
+    }
+    stage_read_kernel<<<dim3(static_cast<unsigned int>((cols + 255) / 256), rows), 256>>>(nullptr, nullptr, att_out, 1, bpad,
+                                                                                          static_cast<int>(cols), out_dev);
+    VCB_CUDA_OK(cudaGetLastError());
+    VCB_CUDA_OK(cudaDeviceSynchronize());
+    return 0;
+}
+
 // Parity hooks of the fp8 KV policy: the epilogues' quantizer alone, and the raw slabs an engine wrote; see include/vcb200.h.
 int vcb_debug_kv_quantize(const float* x_dev, int32_t rows, int32_t hd, uint8_t* out_dev) {
     if (!x_dev || !out_dev || rows < 1 || (hd != 64 && hd != 128)) {

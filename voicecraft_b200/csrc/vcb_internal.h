@@ -244,7 +244,6 @@ __device__ __forceinline__ void ln_row_stats(const float* stats, int tiles, int 
 // ---------------------------------------------------------------------------------------------------
 enum { MEGA_GEMM = 0, MEGA_ATTN = 1 };
 static constexpr int MEGA_MAXSEG = 8;          // output tiles a CTA's block range may touch in one GEMM phase
-static constexpr int MEGA_ATT_MAXC = 16;       // CTAs that may share one (row, head) attention item
 struct MegaPhase {
     int type = MEGA_GEMM;
     // GEMM: `groups` matrices of tiles_per_group x kb 16 KB weight blocks (groups > 1: the K second-stage logit heads)
@@ -282,8 +281,8 @@ struct MegaArgs {
     const float* knew = nullptr;
     const float* vnew = nullptr;
     __nv_bfloat16* att_out = nullptr;   // act_d (hi/lo rows)
-    float* att_ws = nullptr;            // [rows*H][max_pages][132]: page partials (acc[128], m, l) of items shared between CTAs
-    int* att_cnt = nullptr;             // [nph? no: rows*H] arrival counters (self-resetting)
+    float* att_ws = nullptr;            // [rows*H][max_pages][132]: chunk states (acc[128], m, l) of items folded through L2
+    int* att_cnt = nullptr;             // [rows*H] arrival counters of those items (self-resetting)
     const int* row_pos = nullptr;
     const int* row_pages = nullptr;
     int max_pages = 0, H = 0, d = 0;
