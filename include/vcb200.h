@@ -14,7 +14,8 @@
  *   vcb_prefill                    once per utterance batch: waits for `stream`, uploads the slot / page / row tables and
  *                                  the groups' sampling parameters with blocking copies, then enqueues the prefill kernels
  *                                  asynchronously
- *   vcb_poll / vcb_read_tokens     wait for `stream`, then copy state / tokens to the host
+ *   vcb_poll / vcb_read_tokens /   wait for `stream`, then copy state / tokens / log-probabilities to the host
+ *   vcb_read_logprobs
  *   vcb_poll_frames(_ex)           enqueues the frame gather on `stream` (_ex: after one small pinned H2D copy of the
  *                                  sources), then waits for `stream` once; the codes stay on the device, the status and
  *                                  per-slot results arrive in one small copy.  _ex reads each edit source's y0 on `stream`
@@ -174,12 +175,19 @@ int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float*
 int vcb_poll(vcb_engine* e, const int32_t* slots, int32_t n, vcb_status* out_host, void* stream);
 /* copies the raw (still delayed) sampled tokens [n_steps][K] int32 to host memory */
 int vcb_read_tokens(vcb_engine* e, int32_t slot, int32_t* out_host, int32_t max_steps, void* stream);
+/* copies the log-probabilities of those tokens [n_steps][K] fp32 to host memory, row for row and entry for entry as
+ * vcb_read_tokens.  Entry [t][k] = log p_model(token | context) under the softmax of that step's raw logit row of
+ * codebook k (the heads' output with bias, what vcb_debug_logits reports): taken before the end / empty masks, the
+ * silence-repetition scaling, temperature, top-k and top-p, so it does not depend on the sampling parameters.  Forced
+ * tokens (the first steps' empty tokens, the end-token cascade, a forced end token) get the log-probability of the token
+ * written.  Edit hand-over steps write no row.  Computed by the sampler in fp32 (DESIGN.md section 2.2). */
+int vcb_read_logprobs(vcb_engine* e, int32_t slot, float* out_host, int32_t max_steps, void* stream);
 /* closes slots slot .. slot+n_copies-1 (slots that are not open are skipped); a KV page goes back to the free list when
  * the last slot holding it is released, and a group's id with its last slot, in any release order */
 int vcb_release(vcb_engine* e, int32_t slot, int32_t n_copies);
 /* Swap a one-copy utterance out to host memory and back, byte for byte (DESIGN.md section 3).  vcb_swap_out copies what the
  * slot's continuation depends on -- the K and V slabs of its written pages in every layer, its SlotState and GroupState
- * (Philox offset included), its sampling parameters, token-log rows [0, n_steps), its next-input and last-hidden rows and
+ * (Philox offset included), its sampling parameters, token-log and log-probability rows [0, n_steps), its next-input and last-hidden rows and
  * the host-side slot flags -- into a snapshot, then releases the slot.  Rejected before anything changes: a slot that is not
  * open or belongs to a best-of-N group.
  * vcb_swap_in restores a snapshot of this engine into the free `slot` on newly taken pages and a free group id; rejected
@@ -233,6 +241,13 @@ int vcb_debug_exponential(float* out_dev, int64_t numel, uint64_t seed, uint64_t
 int vcb_debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t seed, uint64_t offset, int32_t rng_threads,
                       const vcb_sampling* sp, int32_t n, int32_t K, int32_t V, int32_t empty_token, int32_t eog, int32_t eos,
                       int32_t encodec_sr, const int32_t* state_host, int32_t* tokens_host, int32_t* state_out_host);
+/* vcb_debug_sampler that also returns lp_host [n][K]: the log-probability the step stores with each written token (as
+ * vcb_read_logprobs reports it).  Tokens and state are vcb_debug_sampler's bit for bit; a written token id >= V gets -inf.
+ * Rejected as vcb_debug_sampler, and lp_host == NULL. */
+int vcb_debug_sampler_lp(const float* logits_dev, const float* noise_dev, uint64_t seed, uint64_t offset,
+                         int32_t rng_threads, const vcb_sampling* sp, int32_t n, int32_t K, int32_t V, int32_t empty_token,
+                         int32_t eog, int32_t eos, int32_t encodec_sr, const int32_t* state_host, int32_t* tokens_host,
+                         int32_t* state_out_host, float* lp_host);
 int vcb_debug_gemm(const float* W_dev /*[N][K]*/, const float* X_dev /*[B][K]*/, float* out_dev /*[B][N]*/, int32_t N,
                    int32_t K, int32_t B, int32_t splits /*<=0: auto*/, int32_t simt);
 /* the int8 weight rule of vcb_finalize_weights on fp32 W [N][K]: q_out [N][K] int8 and e_out [N] with W_deq = q * 2^e.

@@ -1,0 +1,61 @@
+"""sampler_kernel time per decode step at 830M (profile class 4: one CUDA event pair around each sampler launch), B = 32
+and 64 utterances, top-k 40, one device Philox stream per utterance, contexts from 231 on.  Prints one JSON line per batch
+with the card, its power limit and SM clock.  --root: the tree whose voicecraft_b200 package (and library) to measure,
+for A/B runs against another build.
+
+usage: bench_sampler.py [--root DIR] [--batches 32,64] [--warmup 20] [--steps 200]"""
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+
+ap = argparse.ArgumentParser()
+ap.add_argument("--root", default=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ap.add_argument("--batches", default="32,64")
+ap.add_argument("--warmup", type=int, default=20)
+ap.add_argument("--steps", type=int, default=200)
+args = ap.parse_args()
+sys.path.insert(0, os.path.abspath(args.root))
+
+import torch  # noqa: E402
+
+import bench  # noqa: E402
+from voicecraft_b200 import _lib  # noqa: E402
+from voicecraft_b200.voicecraft import VoiceCraft  # noqa: E402
+
+batches = [int(b) for b in args.batches.split(",")]
+card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                      capture_output=True, text=True).stdout.strip()
+
+
+class A:
+    model, batch, codebooks, text_len, prompt = "830M", max(batches), 4, 80, 150
+
+
+cfg, sd, utts = bench.make_model_inputs(A)
+m = VoiceCraft(cfg)
+m.load_state_dict(sd)
+m = m.cuda().eval()
+m.configure_engine(max_slots=max(batches), max_seq_len=1024, max_new_tokens=args.warmup + args.steps + 8)
+lib = _lib.load()
+for B in batches:
+    sess = m.open_tts_session([u[0].cuda() for u in utts[:B]], [u[2].cuda() for u in utts[:B]], top_k=40,
+                              seeds=list(range(B)))
+    try:
+        sess.sample()
+        for _ in range(args.warmup):
+            sess.step()
+        torch.cuda.synchronize()
+        lib.vcb_set_option(sess.eng, b"profile", 1)
+        for _ in range(args.steps):
+            sess.step()
+        torch.cuda.synchronize()
+        ms, cnt = (C.c_double * 7)(), (C.c_int64 * 7)()
+        _lib.check(lib.vcb_profile_read(sess.eng, ms, cnt, 7))
+        lib.vcb_set_option(sess.eng, b"profile", 0)
+    finally:
+        sess.close()
+    print(json.dumps(dict(root=os.path.abspath(args.root), B=B, steps=args.steps, sampler_us_per_step=1e3 * ms[4] / args.steps,
+                          sampler_launches_per_step=cnt[4] / args.steps, card=card)), flush=True)

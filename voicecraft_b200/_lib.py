@@ -69,6 +69,7 @@ PROTOTYPES = {
                                      C.POINTER(C.c_int32), C.c_int32, C.c_int64, C.c_int64, C.c_void_p, C.POINTER(vcb_status),
                                      C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p]),
     "vcb_read_tokens": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_void_p]),
+    "vcb_read_logprobs": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_float), C.c_int32, C.c_void_p]),
     "vcb_release": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "vcb_swap_out": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), C.c_void_p]),
     "vcb_swap_in": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),
@@ -78,6 +79,8 @@ PROTOTYPES = {
     "vcb_debug_exponential": (C.c_int, [C.c_void_p, C.c_int64, C.c_uint64, C.c_uint64, C.c_int32, C.c_void_p]),
     "vcb_debug_sampler": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int32, C.POINTER(vcb_sampling)] +
                           [C.c_int32] * 7 + [C.POINTER(C.c_int32)] * 3),
+    "vcb_debug_sampler_lp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int32, C.POINTER(vcb_sampling)] +
+                             [C.c_int32] * 7 + [C.POINTER(C.c_int32)] * 3 + [C.POINTER(C.c_float)]),
     "vcb_debug_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "vcb_debug_weight_quantize": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "vcb_debug_gemm_w8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),

@@ -128,6 +128,7 @@ struct vcb_engine {
     int n_row_groups = 0;
     std::vector<int> slot_shared;     // host mirror: full prompt pages the slot shares with its group (0: none)
     DevBuf<int> tok_log;
+    DevBuf<float> lp_log;             // [max_slots][max_new_tokens][K]: log-probability of each token-log entry
     DevBuf<float> dbg_logits;
     DevBuf<SlotState> st;
     DevBuf<GroupState> gr;
@@ -217,6 +218,7 @@ struct vcb_snapshot {
     int final_frames = 0;             // slot_final
     PinnedBuf<uint8_t> kv;            // [2L pools][n_pages][H slabs], as kv_pages_copy_kernel stages them
     PinnedBuf<int> tok;               // token-log rows [0, n_steps) x K
+    PinnedBuf<float> lp;              // log-probability rows [0, n_steps) x K
     PinnedBuf<float> rows;            // x_slot row (next input), h_slot row (last prefill hidden state)
 };
 
@@ -1167,6 +1169,7 @@ int launch_sampler(vcb_engine* e, const Pass& p, const float* noise, const vcb_s
     a.noise = noise;
     a.dbg_logits = e->dbg_logits;
     a.tok_log = e->tok_log;
+    a.lp_log = e->lp_log;
     a.max_steps = e->cfg.max_new_tokens;
     a.max_seq = e->cfg.max_seq_len;
     a.x_slot = e->x_slot;
@@ -1454,6 +1457,7 @@ int vcb_finalize_weights(vcb_engine* e) {
         e->row_pos.ensure(R, true) || e->row_last.ensure(R, true) || e->row_page.ensure(R, true) ||
         e->row_forced.ensure(R, true) || e->row_pages.ensure(R * e->max_pages_per_slot, true) || e->d_slots.ensure(3 * R + 1, true) ||
         e->page_table.ensure(S * e->max_pages_per_slot, true) || e->tok_log.ensure(S * e->cfg.max_new_tokens * m.K, true) ||
+        e->lp_log.ensure(S * e->cfg.max_new_tokens * m.K, true) ||
         e->dbg_logits.ensure(R * m.K * m.V, true) || e->st.ensure(S, true) || e->gr.ensure(S, true) ||
         e->d_seqs.ensure(S, true) || e->pf_rec.ensure(S, true) || e->h_pf_rec.ensure(S) || e->sp_tab.ensure(S, true) ||
         e->pf_src.ensure(S, true) || e->h_pf_src.ensure(S) || e->swap_pages.ensure(e->max_pages_per_slot, true) ||
@@ -1945,14 +1949,32 @@ int vcb_poll_frames_ex(vcb_engine* e, const int32_t* slots, int32_t n, const vcb
                        bad_host, stream, "vcb_poll_frames_ex");
 }
 
-int vcb_read_tokens(vcb_engine* e, int32_t slot, int32_t* out_host, int32_t max_steps, void* stream) {
+}  // extern "C"
+
+namespace {
+
+// rows [0, min(max_steps, max_new_tokens)) of a slot's token log or log-probability log, after `stream`
+template <typename T>
+int read_log_rows(vcb_engine* e, const T* log, int32_t slot, T* out_host, int32_t max_steps, void* stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
     VCB_CUDA_OK(cudaStreamSynchronize(st));
     const int nn = std::min(max_steps, e->cfg.max_new_tokens);
-    VCB_CUDA_OK(cudaMemcpy(out_host, e->tok_log + static_cast<size_t>(slot) * e->cfg.max_new_tokens * e->m.K,
-                           static_cast<size_t>(nn) * e->m.K * sizeof(int), cudaMemcpyDeviceToHost));
+    VCB_CUDA_OK(cudaMemcpy(out_host, log + static_cast<size_t>(slot) * e->cfg.max_new_tokens * e->m.K,
+                           static_cast<size_t>(nn) * e->m.K * sizeof(T), cudaMemcpyDeviceToHost));
     return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int vcb_read_tokens(vcb_engine* e, int32_t slot, int32_t* out_host, int32_t max_steps, void* stream) {
+    return read_log_rows<int>(e, e->tok_log, slot, out_host, max_steps, stream);
+}
+
+int vcb_read_logprobs(vcb_engine* e, int32_t slot, float* out_host, int32_t max_steps, void* stream) {
+    return read_log_rows<float>(e, e->lp_log, slot, out_host, max_steps, stream);
 }
 
 int vcb_release(vcb_engine* e, int32_t slot, int32_t n_copies) {
@@ -2034,13 +2056,16 @@ int vcb_swap_out(vcb_engine* e, int32_t slot, vcb_snapshot** out, void* stream) 
     snap->n_pages = std::min(static_cast<int>(pg.size()), (snap->S.seq_len + KV_PAGE - 1) / KV_PAGE);
     const size_t page_bytes = page_bytes_all_layers(e);
     const size_t n_tok = static_cast<size_t>(snap->S.n_steps) * m.K;
-    if (snap->kv.alloc(snap->n_pages * page_bytes) || snap->tok.alloc(n_tok) || snap->rows.alloc(2 * m.d) ||
+    if (snap->kv.alloc(snap->n_pages * page_bytes) || snap->tok.alloc(n_tok) || snap->lp.alloc(n_tok) ||
+        snap->rows.alloc(2 * m.d) ||
         swap_prepare(e, std::vector<int>(pg.begin(), pg.begin() + snap->n_pages), snap->n_pages * page_bytes / 16) ||
         swap_copy_kernel<true>(e, snap->n_pages, st))
         return -1;
     VCB_CUDA_OK(cudaMemcpyAsync(snap->kv, e->swap_stage, snap->n_pages * page_bytes, cudaMemcpyDeviceToHost, st));
     VCB_CUDA_OK(cudaMemcpyAsync(snap->tok, e->tok_log + static_cast<size_t>(slot) * e->cfg.max_new_tokens * m.K,
                                 n_tok * sizeof(int), cudaMemcpyDeviceToHost, st));
+    VCB_CUDA_OK(cudaMemcpyAsync(snap->lp, e->lp_log + static_cast<size_t>(slot) * e->cfg.max_new_tokens * m.K,
+                                n_tok * sizeof(float), cudaMemcpyDeviceToHost, st));
     VCB_CUDA_OK(cudaMemcpyAsync(snap->rows, e->x_slot + static_cast<size_t>(slot) * m.d, m.d * sizeof(float),
                                 cudaMemcpyDeviceToHost, st));
     VCB_CUDA_OK(cudaMemcpyAsync(snap->rows + m.d, e->h_slot + static_cast<size_t>(slot) * m.d, m.d * sizeof(float),
@@ -2104,6 +2129,8 @@ int vcb_swap_in(vcb_engine* e, const vcb_snapshot* snap, int32_t slot, void* str
     if (swap_copy_kernel<false>(e, snap->n_pages, st)) return -1;
     VCB_CUDA_OK(cudaMemcpyAsync(e->tok_log + static_cast<size_t>(slot) * e->cfg.max_new_tokens * m.K, snap->tok,
                                 static_cast<size_t>(snap->S.n_steps) * m.K * sizeof(int), cudaMemcpyHostToDevice, st));
+    VCB_CUDA_OK(cudaMemcpyAsync(e->lp_log + static_cast<size_t>(slot) * e->cfg.max_new_tokens * m.K, snap->lp,
+                                static_cast<size_t>(snap->S.n_steps) * m.K * sizeof(float), cudaMemcpyHostToDevice, st));
     VCB_CUDA_OK(cudaMemcpyAsync(e->x_slot + static_cast<size_t>(slot) * m.d, snap->rows, m.d * sizeof(float),
                                 cudaMemcpyHostToDevice, st));
     VCB_CUDA_OK(cudaMemcpyAsync(e->h_slot + static_cast<size_t>(slot) * m.d, snap->rows + m.d, m.d * sizeof(float),
@@ -2839,30 +2866,36 @@ int vcb_debug_exponential(float* out_dev, int64_t numel, uint64_t seed, uint64_t
     return 0;
 }
 
+}  // extern "C"
+
+namespace {
+
 // Parity hook of the fused sampler alone: one sampling step of n one-member groups through sampler_kernel; see
-// include/vcb200.h.  Every argument is checked before anything is allocated or launched.
-int vcb_debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t seed, uint64_t offset, int32_t rng_threads,
-                      const vcb_sampling* sp, int32_t n, int32_t K, int32_t V, int32_t empty_token, int32_t eog, int32_t eos,
-                      int32_t encodec_sr, const int32_t* state_host, int32_t* tokens_host, int32_t* state_out_host) {
+// include/vcb200.h.  lp_host null: the kernel stores no log-probability (vcb_debug_sampler).  Every argument is checked
+// before anything is allocated or launched; `fn` names the entry point in the error messages.
+int debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t seed, uint64_t offset, int32_t rng_threads,
+                  const vcb_sampling* sp, int32_t n, int32_t K, int32_t V, int32_t empty_token, int32_t eog, int32_t eos,
+                  int32_t encodec_sr, const int32_t* state_host, int32_t* tokens_host, int32_t* state_out_host,
+                  float* lp_host, const char* fn) {
     constexpr int D = 32, MAX_Y = 65536, STEPS = 4;
     if (!logits_dev || !sp || !state_host || !tokens_host || !state_out_host || (!noise_dev && rng_threads < 1)) {
-        set_error("vcb_debug_sampler: null argument (or no noise and rng_threads < 1)");
+        set_error("%s: null argument (or no noise and rng_threads < 1)", fn);
         return -1;
     }
     if (n < 1 || K < 1 || K > 8 || V < 1 || V > SAMP_MAXV * SAMP_THREADS) {
-        set_error("vcb_debug_sampler: n >= 1, 1 <= K <= 8, 1 <= V <= %d required (n=%d K=%d V=%d)",
+        set_error("%s: n >= 1, 1 <= K <= 8, 1 <= V <= %d required (n=%d K=%d V=%d)", fn,
                   SAMP_MAXV * SAMP_THREADS, n, K, V);
         return -1;
     }
     if (empty_token < 0 || empty_token >= V + 2 || eog < 0 || eog >= V + 2 || eos >= V + 2) {
-        set_error("vcb_debug_sampler: special ids must lie in [0, V+2) (eos <= 0: unused)");
+        set_error("%s: special ids must lie in [0, V+2) (eos <= 0: unused)", fn);
         return -1;
     }
     int max_y = 0;
     for (int i = 0; i < n; ++i) {
         const int32_t* s = state_host + 7 * i;      // mode, n_eog, cur_num_gen, prev_token, consec, x_len, y_len
         if ((s[0] != 0 && s[0] != 1) || s[1] < 0 || s[1] >= K || s[5] < 0 || s[6] < 0 || s[6] >= MAX_Y) {
-            set_error("vcb_debug_sampler: row %d: mode in {0, 1}, 0 <= n_eog < K, x_len >= 0, 0 <= y_len < %d required", i,
+            set_error("%s: row %d: mode in {0, 1}, 0 <= n_eog < K, x_len >= 0, 0 <= y_len < %d required", fn, i,
                       MAX_Y);
             return -1;
         }
@@ -2872,13 +2905,15 @@ int vcb_debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t 
     DevBuf<float> logits, tables, pe, mask_emb, x_slot;
     DevBuf<float*> E_audio;
     DevBuf<int> slots, tok_log;
+    DevBuf<float> lp_log;
     DevBuf<SlotState> st;
     DevBuf<GroupState> gr;
     const SyncOnExit sync;
     if (logits.alloc(static_cast<size_t>(rows) * Vpad) || tables.alloc(static_cast<size_t>(K) * (V + 2) * D, true) ||
         pe.alloc(static_cast<size_t>(max_y + 1) * D, true) || mask_emb.alloc(8 * D, true) ||
         x_slot.alloc(static_cast<size_t>(n) * D, true) || E_audio.alloc(K) || slots.alloc(n) ||
-        tok_log.alloc(static_cast<size_t>(n) * STEPS * K, true) || st.alloc(n) || gr.alloc(n))
+        tok_log.alloc(static_cast<size_t>(n) * STEPS * K, true) || st.alloc(n) || gr.alloc(n) ||
+        (lp_host && lp_log.alloc(static_cast<size_t>(n) * STEPS * K, true)))
         return -1;
     // the engine's padded layout; pad columns V..Vpad-1 hold 0x70707070 = +2.98e29 (finite after any temperature >= 0.01),
     // so a kernel that reads past V picks a pad column
@@ -2932,6 +2967,7 @@ int vcb_debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t 
     a.noise = noise_dev;
     a.dbg_logits = nullptr;
     a.tok_log = tok_log;
+    a.lp_log = lp_host ? static_cast<float*>(lp_log) : nullptr;
     a.max_steps = STEPS;
     a.max_seq = 1 << 30;
     a.x_slot = x_slot;
@@ -2962,7 +2998,36 @@ int vcb_debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t 
         o[2] = hg[i].n_eog;
         o[3] = hg[i].done;
     }
+    if (lp_host) {
+        std::vector<float> lps(static_cast<size_t>(n) * STEPS * K);
+        VCB_CUDA_OK(cudaMemcpy(lps.data(), lp_log, lps.size() * sizeof(float), cudaMemcpyDeviceToHost));
+        for (int i = 0; i < n; ++i)
+            for (int k = 0; k < K; ++k) lp_host[i * K + k] = lps[static_cast<size_t>(i) * STEPS * K + k];
+    }
     return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int vcb_debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t seed, uint64_t offset, int32_t rng_threads,
+                      const vcb_sampling* sp, int32_t n, int32_t K, int32_t V, int32_t empty_token, int32_t eog, int32_t eos,
+                      int32_t encodec_sr, const int32_t* state_host, int32_t* tokens_host, int32_t* state_out_host) {
+    return debug_sampler(logits_dev, noise_dev, seed, offset, rng_threads, sp, n, K, V, empty_token, eog, eos, encodec_sr,
+                         state_host, tokens_host, state_out_host, nullptr, "vcb_debug_sampler");
+}
+
+int vcb_debug_sampler_lp(const float* logits_dev, const float* noise_dev, uint64_t seed, uint64_t offset,
+                         int32_t rng_threads, const vcb_sampling* sp, int32_t n, int32_t K, int32_t V, int32_t empty_token,
+                         int32_t eog, int32_t eos, int32_t encodec_sr, const int32_t* state_host, int32_t* tokens_host,
+                         int32_t* state_out_host, float* lp_host) {
+    if (!lp_host) {
+        set_error("vcb_debug_sampler_lp: lp_host is null");
+        return -1;
+    }
+    return debug_sampler(logits_dev, noise_dev, seed, offset, rng_threads, sp, n, K, V, empty_token, eog, eos, encodec_sr,
+                         state_host, tokens_host, state_out_host, lp_host, "vcb_debug_sampler_lp");
 }
 
 // Debug timeline of the persistent decode-step kernel: the first call enables recording, later calls copy the last

@@ -839,6 +839,8 @@ struct SamplerArgs {
     const float* noise;       // [n*K][V], or null: generated from the group's Philox stream (GroupState::rng_*)
     float* dbg_logits;        // [n*K][V] or null
     int* tok_log;             // [max_slots][max_steps][K]
+    float* lp_log = nullptr;  // laid out like tok_log: log-probability of the written token under the raw row (DESIGN.md
+                              // section 2.2), or null: not stored
     int max_steps, max_seq;
     float* x_slot;            // [max_slots][d]
     const float* const* E_audio;
@@ -857,8 +859,17 @@ static constexpr int SAMP_SORT_N = 4096;
 
 __device__ void sampler_finish_slot(const SamplerArgs& a, const SamplingParams& sp, int slot, float* sred);
 
+// (max, sum of exp(u - max)) pairs of two parts of a row, merged.  A part with no entries is (-inf, 0); the part that holds
+// the maximum keeps its sum unscaled, so two empty parts merge to (-inf, 0), never to NaN.
+__device__ __forceinline__ void lse_merge(float& m, float& s, float om, float os) {
+    const float mm = fmaxf(m, om);
+    s = (m == mm ? s : s * expf(m - mm)) + (om == mm ? os : os * expf(om - mm));
+    m = mm;
+}
+
 __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const __grid_constant__ SamplerArgs a) {
     __shared__ float sred[8];
+    __shared__ float s_lse_m[8], s_lse_s[8];            // per warp: (max, sum) of the raw row, for the log-probability
     __shared__ int sidx[8];
     __shared__ int hist[256];
     __shared__ uint32_t s_prefix;
@@ -919,13 +930,16 @@ __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const __grid_cons
     const int row = i * K + k;
 
     // ---- load logits (split-K reduce + bias), apply the reference's in-place edits -----------------
-    float l[SAMP_MAXV];
+    float l[SAMP_MAXV], raw[SAMP_MAXV];
+    float lse_m = -INFINITY;             // this thread's max of the raw (unedited) entries
 #pragma unroll
     for (int j = 0; j < SAMP_MAXV; ++j) {
         const int v = tid + j * SAMP_THREADS;
         float u = -INFINITY;
         if (v < V) {
             u = a.logits[static_cast<size_t>(i) * a.ldl + k * a.Vpad + v];
+            raw[j] = u;
+            lse_m = fmaxf(lse_m, u);
             if (a.dbg_logits) a.dbg_logits[static_cast<size_t>(row) * V + v] = u;
             if (a.eos > 0 && v == (tts ? a.eog : a.eos)) u = -10000.f;                   // :1091-1093 / :816-818
             if (n_eog == 0) {
@@ -944,6 +958,19 @@ __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const __grid_cons
             }
         }
         l[j] = u;
+    }
+    // log-sum-exp of the raw row, before the edits above and before temperature / top-k / top-p: this thread's entries
+    // summed in index order, then merged across the warp here and across the 8 warps by thread 0 at the end (the
+    // block_argmax barriers below publish s_lse_*)
+    {
+        float lse_s = 0.f;
+#pragma unroll
+        for (int j = 0; j < SAMP_MAXV; ++j)
+            if (tid + j * SAMP_THREADS < V) lse_s += expf(raw[j] - lse_m);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1)
+            lse_merge(lse_m, lse_s, __shfl_xor_sync(0xffffffffu, lse_m, o), __shfl_xor_sync(0xffffffffu, lse_s, o));
+        if (lane == 0) { s_lse_m[warp] = lse_m; s_lse_s[warp] = lse_s; }
     }
 
     // the Exp(1) draws are independent of everything below: fetch them now, not after the softmax
@@ -1190,7 +1217,16 @@ __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const __grid_cons
             if (k < n_eog) tok = a.empty_token;
             else if (k == n_eog) tok = E;
         }
-        a.tok_log[(static_cast<size_t>(slot) * a.max_steps + S.n_steps) * K + k] = tok;
+        const size_t at = (static_cast<size_t>(slot) * a.max_steps + S.n_steps) * K + k;
+        a.tok_log[at] = tok;
+        if (a.lp_log) {
+            // lp = (u_tok - M) - log sum_v exp(u_v - M) of the raw row, for the written token, drawn or forced
+            float m = s_lse_m[0], s = s_lse_s[0];
+#pragma unroll
+            for (int w = 1; w < 8; ++w) lse_merge(m, s, s_lse_m[w], s_lse_s[w]);
+            a.lp_log[at] = tok < V ? (a.logits[static_cast<size_t>(i) * a.ldl + k * a.Vpad + tok] - m) - logf(s)
+                                   : -INFINITY;
+        }
         __threadfence();
         s_flag = (atomicAdd(&S.arrive, 1) == K - 1);
     }

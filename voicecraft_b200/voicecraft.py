@@ -353,6 +353,13 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         _lib.check(_lib.load().vcb_read_tokens(eng, slot, buf, n_steps, stream))
         return np.frombuffer(buf, dtype=np.int32).reshape(n_steps, K).astype(np.int64)
 
+    def _read_lp(self, eng, slot, n_steps, stream):
+        """log-probability rows [n_steps, K] fp32 of the slot's delayed token rows (vcb_read_logprobs)"""
+        K = self.args.n_codebooks
+        buf = (C.c_float * (n_steps * K))()
+        _lib.check(_lib.load().vcb_read_logprobs(eng, slot, buf, n_steps, stream))
+        return np.frombuffer(buf, dtype=np.float32).reshape(n_steps, K).copy()
+
     @staticmethod
     def _undelay(rows: np.ndarray, K: int) -> np.ndarray:
         """rows [n,K] (delayed, as sampled) -> [K, n-K]   (reference voicecraft.py:1126-1137).  For a finished
@@ -366,18 +373,22 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     @torch.no_grad()
     def inference_tts(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, top_k: int = -100,
                       top_p: float = 1.0, temperature: float = 1.0, stop_repetition: int = 3, kvcache: int = 1,
-                      silence_tokens: List[int] = [1388, 1898, 131], *kargs):
-        res, gen = self._tts_impl(x, x_lens, y, top_k, top_p, temperature, stop_repetition, silence_tokens, 1)
-        return res, gen
+                      silence_tokens: List[int] = [1388, 1898, 131], *kargs, logprobs: bool = False):
+        """logprobs=True: returns (res, gen, lp), lp [1,K,G] fp32 the log-probability of each frame of gen under the
+        model's raw distribution (vcb_read_logprobs)"""
+        return self._tts_impl(x, x_lens, y, top_k, top_p, temperature, stop_repetition, silence_tokens, 1, logprobs)
 
     @torch.no_grad()
     def inference_tts_batch(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, top_k: int = -100,
                             top_p: float = 1.0, temperature: float = 1.0, stop_repetition: int = 3, kvcache: int = 1,
-                            batch_size: int = 5, silence_tokens: List[int] = [1388, 1898, 131], *kargs):
-        """Best-of-N: the first sample to end wins (reference voicecraft.py:1156-1439)."""
-        return self._tts_impl(x, x_lens, y, top_k, top_p, temperature, stop_repetition, silence_tokens, batch_size)
+                            batch_size: int = 5, silence_tokens: List[int] = [1388, 1898, 131], *kargs,
+                            logprobs: bool = False):
+        """Best-of-N: the first sample to end wins (reference voicecraft.py:1156-1439).  logprobs=True: returns
+        (res, gen, lp) as inference_tts does, lp the kept copy's."""
+        return self._tts_impl(x, x_lens, y, top_k, top_p, temperature, stop_repetition, silence_tokens, batch_size,
+                              logprobs)
 
-    def _tts_impl(self, x, x_lens, y, top_k, top_p, temperature, stop_repetition, silence_tokens, n_copies):
+    def _tts_impl(self, x, x_lens, y, top_k, top_p, temperature, stop_repetition, silence_tokens, n_copies, logprobs):
         assert x.ndim == 2, x.shape
         assert x_lens.ndim == 1, x_lens.shape
         assert y.ndim == 3, y.shape
@@ -387,12 +398,12 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
                              n_copies=n_copies)
         try:
-            (res, gen), = sess._run_single()
+            out, = sess._run_single(logprobs)
         finally:
             sess.close()
         keep = sess._kept(0, sess.status)
         self.last_stats = dict(steps=int(sess.status[keep].n_steps), keep=int(keep))
-        return res, gen
+        return out
 
     # ------------------------------------------------------------------------------------------------
     # speech editing  (reference voicecraft.py:561-906)
@@ -453,7 +464,9 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     @torch.no_grad()
     def inference(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, mask_interval: torch.Tensor,
                   top_k: int = -100, top_p: float = 1.0, temperature: float = 1.0, stop_repetition: int = -1,
-                  kvcache: int = 1, silence_tokens: List[int] = [1388, 1898, 131]) -> torch.Tensor:
+                  kvcache: int = 1, silence_tokens: List[int] = [1388, 1898, 131], *, logprobs: bool = False):
+        """logprobs=True: returns (res, lp), lp [1,K,T'] fp32 aligned with res: the log-probability of each generated
+        frame under the model's raw distribution (vcb_read_logprobs), NaN on the frames copied from y"""
         assert x.ndim == 2, x.shape
         assert x_lens.ndim == 1, x_lens.shape
         assert y.ndim == 3, y.shape
@@ -464,11 +477,11 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
                              mask_intervals=[mask_interval], n_copies=1)
         try:
-            (res, _), = sess._run_single()
+            out, = sess._run_single(logprobs)
         finally:
             sess.close()
         self.last_stats = dict(steps=int(sess.status[0].n_steps))
-        return res
+        return (out[0], out[2]) if logprobs else out[0]
 
     # ------------------------------------------------------------------------------------------------
     # driver-level batching of INDEPENDENT utterances (SURVEY.md section 8f row f2; BASELINE config 2).
@@ -483,9 +496,11 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
                              mask_intervals=mask_intervals, seeds=seeds, noise_fns=noise_fns)
 
     @torch.no_grad()
-    def inference_many(self, xs, ys, mask_intervals, poll_every: int = 4, **kw):
-        """Batched counterpart of `inference` (speech editing) for independent utterances."""
-        return [r[0] for r in self.open_edit_session(xs, ys, mask_intervals, **kw)._run_many(poll_every)]
+    def inference_many(self, xs, ys, mask_intervals, poll_every: int = 4, logprobs: bool = False, **kw):
+        """Batched counterpart of `inference` (speech editing) for independent utterances; logprobs=True: a list of
+        (res, lp) as inference(..., logprobs=True) returns them."""
+        out = self.open_edit_session(xs, ys, mask_intervals, **kw)._run_many(poll_every, logprobs)
+        return [(r[0], r[2]) if logprobs else r[0] for r in out]
 
     def open_tts_session(self, xs, ys, top_k=-100, top_p=1.0, temperature=1.0, stop_repetition=3,
                          silence_tokens=(1388, 1898, 131), seeds=None, noise_fns=None, best_of=1):
@@ -504,10 +519,10 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
                              seeds=seeds, noise_fns=noise_fns, best_of=best_of)
 
     @torch.no_grad()
-    def inference_tts_many(self, xs, ys, poll_every: int = 8, **kw):
+    def inference_tts_many(self, xs, ys, poll_every: int = 8, logprobs: bool = False, **kw):
         """Returns a list of (res [1,K,T+G], gen [1,K,G]) like inference_tts (inference_tts_batch with best_of > 1), one
-        per utterance."""
-        return self.open_tts_session(xs, ys, **kw)._run_many(poll_every)
+        per utterance; logprobs=True: (res, gen, lp) as inference_tts(..., logprobs=True) returns them."""
+        return self.open_tts_session(xs, ys, **kw)._run_many(poll_every, logprobs)
 
     # ------------------------------------------------------------------------------------------------
     # streaming: audio while the tokens are generated (TtsStream)
@@ -709,34 +724,45 @@ class _Prompt:
                 src.spans[j][0], src.spans[j][1] = s0, s1
         return src
 
-    def result(self, rows, st):
+    def result(self, rows, st, lp_rows=None):
         """(res [1,K,T+G], gen [1,K,G]) as inference_tts returns them, or (res, None) with res as inference returns it,
         from the utterance's delayed token rows [n,K] and its vcb_status.  A TTS utterance that is not done (a truncated
-        session) keeps its final frames only: the still-delayed tail is dropped."""
+        session) keeps its final frames only: the still-delayed tail is dropped.
+        lp_rows: the log-probability rows [n,K] of those tokens (vcb_read_logprobs); the result then also holds lp, fp32
+        on the model's device, un-delayed as the codes: [1,K,G] aligned with gen, or [1,K,T'] aligned with an edit's res,
+        NaN on the frames copied from the original."""
         a = self.model.args
         K, dev = a.n_codebooks, self.y0.device
-        gen = None
+        gen, lp = None, None
         if self.spans is None:
             n = rows.shape[0] - K if st.done else final_frames(rows, K, _end_token(a))
             gen = torch.from_numpy(frame_codes(rows, K, 0, n)).to(dev)
             res = torch.cat([self.y0, gen], dim=1).unsqueeze(0)
             expected = self.y0.shape[1] + n
             assert res.shape == torch.Size((1, K, expected)), f"res.shape: {res.shape}, expected_y_len: {expected}"
+            if lp_rows is not None:
+                lp = frame_codes(lp_rows, K, 0, n)
         else:
             assert st.done, "edit session results() needs finished utterances"
             ends = [st.span_ends[j] for j in range(st.n_spans_done)]
             assert len(ends) == len(self.spans), f"len(generated): {len(ends)}, num_mask: {len(self.spans)}"
-            pieces, lo = [], 0
+            pieces, lps, lo = [], [], 0
             for (s0, s1), hi in zip(self.non_mask, ends):
                 pieces.append(self.y0[:, s0:s1])
                 pieces.append(torch.from_numpy(VoiceCraft._undelay(rows[lo:hi], K)).to(dev))
+                if lp_rows is not None:
+                    lps += [np.full((K, s1 - s0), np.nan, np.float32), VoiceCraft._undelay(lp_rows[lo:hi], K)]
                 lo = hi
-            pieces.append(self.y0[:, self.non_mask[-1][0]: self.non_mask[-1][1]])
+            s0, s1 = self.non_mask[-1]
+            pieces.append(self.y0[:, s0:s1])
             res = torch.cat(pieces, dim=1).unsqueeze(0)
+            if lp_rows is not None:
+                lp = np.concatenate(lps + [np.full((K, s1 - s0), np.nan, np.float32)], axis=1)
         if a.special_first:
             res = res - int(a.n_special)
             gen = None if gen is None else gen - int(a.n_special)
-        return res, None if gen is None else gen.unsqueeze(0)
+        out = res, None if gen is None else gen.unsqueeze(0)
+        return out if lp_rows is None else out + (torch.from_numpy(lp).unsqueeze(0).to(dev),)
 
 
 def _prefill(eng, prompts, stream):
@@ -826,12 +852,17 @@ class TtsStream(_AudioStream):
             raise _lib.VcbError("streaming an edit needs the device generators (model.noise_fn / noise_fns must be None): "
                                 "the polls do not follow the forced hand-over steps, so host noise would be drawn for them")
         self._start(SimpleNamespace(sess=sess, dev=sess.dev, tok=tokenizer, chunk_frames=int(chunk_frames),
-                                    poll_every=int(poll_every), results=None, first_audio_steps=None,
+                                    poll_every=int(poll_every), results=None, logprobs=None, first_audio_steps=None,
                                     sample_rate=sample_rate), sess.B)
 
     @property
     def results(self):
         return self._st.results
+
+    @property
+    def logprobs(self):
+        """after the iteration: utterance i's lp, as DecodeSession.results(logprobs=True) returns it"""
+        return self._st.logprobs
 
     @property
     def first_audio_steps(self):
@@ -877,7 +908,9 @@ class TtsStream(_AudioStream):
                         yield r.cid, w
                     if done and all(r.closed for r in live):
                         break
-                st.results = sess.results()
+                out = sess.results(logprobs=True)
+                st.results = [(res, gen) for res, gen, _ in out]
+                st.logprobs = [lp for _, _, lp in out]
                 if sess.edit:                        # what inference_many / inference return: res alone
                     st.results = [res for res, _ in st.results]
         finally:
@@ -1016,6 +1049,12 @@ class _SingleTtsStream(TtsStream):
     def result(self):
         return None if self.results is None else self.results[0]
 
+    @property
+    def logprobs(self):
+        """after the iteration: the lp that inference_tts / inference return with logprobs=True"""
+        lps = TtsStream.logprobs.fget(self)
+        return None if lps is None else lps[0]
+
 
 class DecodeSession:
     """A batch of independent utterances resident in the engine, one random stream each, and one slot each or, best-of-N,
@@ -1102,22 +1141,22 @@ class DecodeSession:
         _check_capacity(st)
         return all(s.done for s in st)
 
-    def _run_many(self, poll_every):
+    def _run_many(self, poll_every, logprobs=False):
         """inference_many / inference_tts_many: sample and step until every utterance is done, polling every
-        `poll_every` steps; returns results() and closes the session"""
+        `poll_every` steps; returns results(logprobs) and closes the session"""
         try:
             self.sample()
             if self.model._eng_opts["kv_pool_gb"] is not None and self.n_copies == 1 and not self._host_noise:
-                return self._run_pooled(poll_every)
+                return self._run_pooled(poll_every, logprobs)
             while True:
                 if self.steps % poll_every == 0 and self.all_done():
                     break
                 self.step()
-            return self.results()
+            return self.results(logprobs)
         finally:
             self.close()
 
-    def _run_pooled(self, poll_every):
+    def _run_pooled(self, poll_every, logprobs=False):
         """_run_many's loop under a KV budget (KvPoolPolicy), returning the results: a refused step swaps the youngest
         utterance out; a finished one is read and leaves its slot and pages at once; swapped-out utterances come back,
         oldest first, into the session's freed slots"""
@@ -1145,7 +1184,7 @@ class DecodeSession:
                 _check_capacity(st)
                 for (i, slot, _, _), s in zip(live, st):
                     if s.done:
-                        results[i] = self.prompts[i].result(self.model._read_rows(self.eng, slot, s.n_steps, self.stream), s)
+                        results[i] = self._result(i, slot, s, logprobs)
                         _lib.check(self.lib.vcb_release(self.eng, slot, 1))
                         done[i] = True
                         free.add(slot)
@@ -1154,7 +1193,7 @@ class DecodeSession:
             self.c_slots = (C.c_int32 * len(self.slots))(*self.slots)
         return results
 
-    def _run_single(self):
+    def _run_single(self, logprobs=False):
         """The loop of a single call; returns results().  The done flag is polled every model.poll_every steps: a finished
         group ignores further steps and consumes nothing, so the device generator still ends exactly where the reference's
         would.  Edits, host noise and trace_logits poll every step; a forced hand-over step then draws no host noise and
@@ -1171,7 +1210,7 @@ class DecodeSession:
                 self._launch(self.lib.vcb_decode_step, self._noise(draw=not forced))
                 if not forced:
                     self._trace()
-            return self._results(self.status)
+            return self._results(self.status, logprobs)
 
     def _trace(self):
         """append the raw logits [n*K, V] of the last sampling step to model.trace_logits (when it is a list)"""
@@ -1190,19 +1229,27 @@ class DecodeSession:
             j += st[j].keep
         return self.model._read_rows(self.eng, self.slots[j], st[j].n_steps, self.stream)
 
-    def results(self):
-        return self._results(self.poll())
+    def results(self, logprobs=False):
+        """one (res, gen) per utterance as inference_tts returns it ((res, None) for an edit); logprobs=True: (res, gen,
+        lp) with lp as inference_tts(..., logprobs=True) / inference(..., logprobs=True) return it"""
+        return self._results(self.poll(), logprobs)
 
     def _kept(self, i, st):
         """index in `st` of utterance i's result: the copy of its best-of-N group that ended first, or its slot"""
         j = i * self.n_copies
         return j + (st[j].keep if self.n_copies > 1 else 0)
 
-    def _results(self, st):
+    def _result(self, i, slot, st, logprobs):
+        """utterance i's result from its slot (its kept copy's) and vcb_status"""
+        m = self.model
+        lp = m._read_lp(self.eng, slot, st.n_steps, self.stream) if logprobs else None
+        return self.prompts[i].result(m._read_rows(self.eng, slot, st.n_steps, self.stream), st, lp)
+
+    def _results(self, st, logprobs=False):
         out = []
-        for i, p in enumerate(self.prompts):
+        for i in range(len(self.prompts)):
             j = self._kept(i, st)
-            out.append(p.result(self.model._read_rows(self.eng, self.slots[j], st[j].n_steps, self.stream), st[j]))
+            out.append(self._result(i, self.slots[j], st[j], logprobs))
         if self._gen is not None:
             self._gen.set_offset(int(st[0].rng_offset))
         return out
@@ -1382,6 +1429,7 @@ class ContinuousBatcher:
         self.queue = []
         self.stats = dict(steps=0, prefills=0, max_active=0, swap_outs=0, swap_ins=0)
         self.results, self.errors = [], {}
+        self.logprobs = []                 # lp of results[ticket] (as inference_tts / inference return it), None with it
         self._live = None                  # the running stream()'s state
 
     def submit(self, x, y=None, seed=None, best_of=1, mask_interval=None, top_k=None, top_p=None, temperature=None,
@@ -1442,6 +1490,7 @@ class ContinuousBatcher:
                                     "configure_engine(max_seq_len=...) before stream()")
             st.jobs.append(job)
             self.results.append(None)
+            self.logprobs.append(None)
         self.queue.append((x, y, seed, best_of, spans, sp, pending))
         return len(self.queue) - 1
 
@@ -1499,9 +1548,13 @@ class ContinuousBatcher:
         _lib.check(lib.vcb_sample(eng, c_new, len(rows), None, None, stream))
         self.stats["prefills"] += 1
 
-    def _result(self, eng, slot, st, job, stream):
-        """(res, gen) of a finished slot, as inference_tts returns them; (res, None) of an edit, res as inference returns it"""
-        return job[0].result(self.model._read_rows(eng, slot, st.n_steps, stream), st)
+    def _result(self, eng, slot, st, job, stream, ticket):
+        """(res, gen) of a finished slot, as inference_tts returns them; (res, None) of an edit, res as inference returns
+        it; its lp goes to logprobs[ticket]"""
+        m = self.model
+        res, gen, self.logprobs[ticket] = job[0].result(m._read_rows(eng, slot, st.n_steps, stream), st,
+                                                        m._read_lp(eng, slot, st.n_steps, stream))
+        return res, gen
 
     @torch.no_grad()
     def run(self):
@@ -1517,6 +1570,7 @@ class ContinuousBatcher:
         eng, slots = m._take_slots(n_slots, max([j[0].need_seq for j in jobs], default=0))
         max_pages = (m._eng_opts["max_seq_len"] + 63) // 64
         free, active, results, nxt = set(slots), {}, [None] * len(jobs), 0     # active: first slot -> ticket
+        self.logprobs = [None] * len(jobs)
         pool = None
         try:
             with torch.cuda.device(dev):
@@ -1556,7 +1610,7 @@ class ContinuousBatcher:
                         st = by_slot[slot]
                         if st.done:
                             kept = slot + (st.keep if sizes[ji] > 1 else 0)
-                            results[ji] = self._result(eng, kept, by_slot[kept], jobs[ji], stream)
+                            results[ji] = self._result(eng, kept, by_slot[kept], jobs[ji], stream, ji)
                             m._release_slots(slots, [slot], n_copies=sizes[ji], keep_held=True)
                             del active[slot]
                             free.update(range(slot, slot + sizes[ji]))
@@ -1604,7 +1658,7 @@ class BatcherStream(_AudioStream):
                              cancelled=set(refused), ended=set(refused), refused=sorted(refused), tok=tokenizer,
                              chunk_frames=int(chunk_frames), dev=m.mask_embedding.device, sample_rate=sample_rate,
                              pool=None)
-        cb.results, cb._live = [None] * len(jobs), st
+        cb.results, cb.logprobs, cb._live = [None] * len(jobs), [None] * len(jobs), st
         cb.errors = {t: f"best_of={jobs[t][2]}: stream() serves only best_of=1 tickets" for t in refused}
         # a codec stream id belongs to a ticket from its admission to its end: at most max_concurrency are active and, under
         # a KV budget, at most as many more are swapped out
@@ -1645,7 +1699,8 @@ class BatcherStream(_AudioStream):
                     for slot, r in list(active.items()):
                         if r.closed or r.ticket in st.cancelled:
                             if r.closed and r.ticket not in cb.errors:
-                                cb.results[r.ticket] = cb._result(st.eng, slot, r.status, st.jobs[r.ticket], stream)
+                                cb.results[r.ticket] = cb._result(st.eng, slot, r.status, st.jobs[r.ticket], stream,
+                                                                  r.ticket)
                             m._release_slots(st.slots, [slot], keep_held=True)
                             del active[slot]
                             free.add(slot)
