@@ -107,6 +107,8 @@ struct vcb_engine {
     DevBuf<int> row_page;             // KV page of every row's position (step_prep / prefill fill it)
     DevBuf<int> row_forced;           // decode steps: SlotState::forced per row as of step_prep (sampler snapshot)
     DevBuf<int> row_pages;            // decode steps: per-row copy of the slot's page list [rows][max_pages_per_slot]
+    DevBuf<unsigned long long> row_epoch;   // decode steps: the step whose row tables step_prep last published, per row
+    unsigned long long step_epoch = 0;      // decode steps enqueued since create (the epoch step_prep publishes)
     std::vector<char> slot_rng;       // host mirror: the slot's group generates its own sampling noise
     std::vector<char> slot_edit;      // host mirror: masked spans of the slot's edit prompt (0: a TTS prompt)
     std::vector<int> slot_copies;     // host mirror: n_copies of the slot's prompt (best-of-N group size)
@@ -151,6 +153,9 @@ struct vcb_engine {
 
     std::vector<std::array<int, 3>> opt_splits;
     int opt_simt = 0, opt_pdl = 0, opt_profile = 0, opt_prefetch = 0, opt_att_balance = 1;
+    // VCB_ATT_EARLY: decode attention starts its K/V stream before griddepcontrol.wait and copies only the live tokens of
+    // the last page (0: after the wait, whole pages).  VCB_ATT_POISON (debug): attention fills its K/V ring with NaN first
+    int opt_att_early = 1, opt_att_poison = 0;
     // wide prefill (gemm_rows.cu): up to wide_rows prompt rows per pass through the layers, own activation planes;
     // opt_prefill_wide = minimum number of prompt rows that takes this path (0: never; VCB_PREFILL_WIDE)
     int opt_prefill_wide = 1, wide_rows = 0;      // 1: every prompt takes the rows-as-M path, so a row's K/V bits do not
@@ -385,6 +390,10 @@ struct AttnLaunch {
     // grp_shared[g] pages are the same; n_groups = 0: every row on its own (GMAX = 1)
     const int *grp_first = nullptr, *grp_shared = nullptr;
     int n_groups = 0;
+    // decode steps: step_prep's per-row epochs and this step's; null: the producer issues nothing before the wait
+    const unsigned long long* row_epoch = nullptr;
+    unsigned long long epoch = 0;
+    int opts = ATT_LIVE_TAIL;             // ATT_LIVE_TAIL | ATT_POISON
 };
 
 template <typename KVT, int HD, int GMAX>
@@ -410,7 +419,7 @@ int launch_attn_hd(const AttnLaunch& a, cudaStream_t st) {
     VCB_CUDA_OK(launch_k_pdl(a.pdl, attn_rows_kernel<KVT, HD, GMAX>, dim3(grid), dim3(ATT_THREADS + 32), L::TOTAL, st, a.q,
                              static_cast<const KVT*>(a.kpool), static_cast<const KVT*>(a.vpool), a.page_table, a.max_pages,
                              a.row_slot, a.row_pos, a.H, a.act, a.ld_act, a.bpad, scale, a.ws, a.cnt, a.maxch, a.chunk_pages,
-                             n_rh, nch, a.row_pages, a.grp_first, a.grp_shared));
+                             n_rh, nch, a.row_pages, a.grp_first, a.grp_shared, a.row_epoch, a.epoch, a.opts));
     return 0;
 }
 
@@ -447,6 +456,7 @@ struct Pass {
     bool wide = false;                        // GEMMs through the rows-as-M kernel (gemm_rows.cu), else the cluster decode GEMM
     const int *slot = nullptr, *pos = nullptr, *last = nullptr, *page = nullptr;
     const int* pages = nullptr;               // [rows][max_pages_per_slot] page lists, or null: pages through page_table + slot
+    const unsigned long long* epochs = nullptr;   // decode steps: step_prep's per-row epochs (attention's early start)
     const int* forced = nullptr;              // decode steps: SlotState::forced per row as of step_prep (sampler snapshot)
     const int *grp_first = nullptr, *grp_shared = nullptr;   // decode steps: row groups (AttnLaunch), n_groups of them
     int n_groups = 0;
@@ -505,6 +515,7 @@ Pass step_pass(vcb_engine* e, int n, bool fold) {
     p.last = e->row_last;
     p.page = e->row_page;
     p.pages = e->row_pages;
+    p.epochs = e->row_epoch;
     p.forced = e->row_forced;
     p.n_groups = e->n_row_groups;
     p.grp_first = e->d_slots + n;
@@ -676,6 +687,9 @@ int launch_attn(vcb_engine* e, const Pass& p, const Layer& Ly, cudaStream_t st) 
     a.grp_first = p.grp_first;
     a.grp_shared = p.grp_shared;
     a.n_groups = p.n_groups;
+    a.row_epoch = e->opt_att_early ? p.epochs : nullptr;
+    a.epoch = e->step_epoch;
+    a.opts = (e->opt_att_early ? ATT_LIVE_TAIL : 0) | (e->opt_att_poison ? ATT_POISON : 0);
     ProfScope ps(e, PC_ATTN, st);
     if (launch_attn_rows(a, st)) return -1;
     LAUNCH_COUNT(e);
@@ -1305,6 +1319,8 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
     e->opt_pdl = pdl ? atoi(pdl) : 1;
     if (getenv("VCB_PREFETCH")) e->opt_prefetch = atoi(getenv("VCB_PREFETCH"));
     if (getenv("VCB_ATT_BALANCE")) e->opt_att_balance = atoi(getenv("VCB_ATT_BALANCE"));
+    if (getenv("VCB_ATT_EARLY")) e->opt_att_early = atoi(getenv("VCB_ATT_EARLY"));
+    if (getenv("VCB_ATT_POISON")) e->opt_att_poison = atoi(getenv("VCB_ATT_POISON"));
     if (getenv("VCB_PREFILL_WIDE")) e->opt_prefill_wide = atoi(getenv("VCB_PREFILL_WIDE"));
     if (const char* sp = getenv("VCB_SPLITS")) {
         int n = 0, k = 0, sv = 0, used = 0;
@@ -1455,7 +1471,8 @@ int vcb_finalize_weights(vcb_engine* e) {
         e->att_ws.ensure(R * m.H * e->att_maxch * (m.hd + 2), true) || e->att_cnt.ensure(R * m.H, true) ||
         e->ln_stats.ensure(static_cast<size_t>(128) * STATS_ROWS * 2, true) || e->row_slot.ensure(R, true) ||
         e->row_pos.ensure(R, true) || e->row_last.ensure(R, true) || e->row_page.ensure(R, true) ||
-        e->row_forced.ensure(R, true) || e->row_pages.ensure(R * e->max_pages_per_slot, true) || e->d_slots.ensure(3 * R + 1, true) ||
+        e->row_forced.ensure(R, true) || e->row_pages.ensure(R * e->max_pages_per_slot, true) || e->row_epoch.ensure(R, true) ||
+        e->d_slots.ensure(3 * R + 1, true) ||
         e->page_table.ensure(S * e->max_pages_per_slot, true) || e->tok_log.ensure(S * e->cfg.max_new_tokens * m.K, true) ||
         e->lp_log.ensure(S * e->cfg.max_new_tokens * m.K, true) ||
         e->dbg_logits.ensure(R * m.K * m.V, true) || e->st.ensure(S, true) || e->gr.ensure(S, true) ||
@@ -1752,7 +1769,7 @@ int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float*
                              e->ln_stats, e->page_table, e->max_pages_per_slot, e->row_page, e->row_pages, e->row_forced,
                              e->mega_flags, e->mega_flags ? e->mega_nph : 0, reinterpret_cast<unsigned int*>(e->mega_tile_cnt.get()),
                              e->mega_flags ? e->mega_nph * e->mega_cnt_stride : 0,
-                             mega ? e->mact_d : static_cast<__nv_bfloat16*>(nullptr)));
+                             mega ? e->mact_d : static_cast<__nv_bfloat16*>(nullptr), e->row_epoch, ++e->step_epoch));
     }
     LAUNCH_COUNT(e);
     for (int i = 0; i < n; ++i) p.max_ctx = std::max(p.max_ctx, ++e->h_seq_len[slots[i]]);
@@ -2833,6 +2850,8 @@ int64_t vcb_counter(vcb_engine* e, const char* name) {
     if (!strcmp(name, "mega_nb")) return e->mega_grid ? e->mega_nb : 0;
     if (!strcmp(name, "mega_flight")) return e->mega_grid ? e->mega_flight : 0;
     if (!strcmp(name, "mega_pf")) return e->mega_grid ? e->mega_pf : 0;
+    if (!strcmp(name, "att_early")) return e->opt_att_early;
+    if (!strcmp(name, "att_poison")) return e->opt_att_poison;
     if (!strcmp(name, "poll_frames")) return e->n_poll_frames;
     if (!strcmp(name, "kv_pages_free")) return static_cast<int64_t>(e->free_pages.size());
     if (!strcmp(name, "kv_pages_total")) return e->n_pages;

@@ -289,8 +289,42 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// Options of attn_rows_kernel (its `opts` argument)
+static constexpr int ATT_LIVE_TAIL = 1;     // copy only the token rows 0 .. pos % KV_PAGE of the page that holds pos
+static constexpr int ATT_POISON = 2;        // debug: fill the K / V ring with NaN first (shows that no uncopied byte is read)
+
+// One (page, head) slab of K and of V into one ring stage: its first ntok token rows (fp8: and their scales, whose copy
+// is rounded up to 16 bytes and stays inside the slab).  The stage's full barrier expects exactly the bytes copied.
+template <typename KVT, int HD>
+__device__ __forceinline__ void att_issue(KVT* dK, KVT* dV, const KVT* gK, const KVT* gV, int ntok, uint64_t* bar,
+                                          uint64_t pol) {
+    constexpr uint32_t PAGE_BYTES = kv_slab_bytes(kv_dtype_of<KVT>(), HD);
+    if (ntok == KV_PAGE) {
+        mbar_arrive_expect_tx(bar, 2 * PAGE_BYTES);
+        tma_bulk_g2s_hint(dK, gK, PAGE_BYTES, bar, pol);
+        tma_bulk_g2s_hint(dV, gV, PAGE_BYTES, bar, pol);
+        return;
+    }
+    const uint32_t rows = static_cast<uint32_t>(ntok) * HD * sizeof(KVT);      // a multiple of 16: HD is 64 or 128
+    if constexpr (sizeof(KVT) == 1) {
+        const uint32_t scb = (static_cast<uint32_t>(ntok) * 4 + 15) & ~15u;
+        mbar_arrive_expect_tx(bar, 2 * (rows + scb));
+        tma_bulk_g2s_hint(dK, gK, rows, bar, pol);
+        tma_bulk_g2s_hint(dK + KV_PAGE * HD, gK + KV_PAGE * HD, scb, bar, pol);
+        tma_bulk_g2s_hint(dV, gV, rows, bar, pol);
+        tma_bulk_g2s_hint(dV + KV_PAGE * HD, gV + KV_PAGE * HD, scb, bar, pol);
+    } else {
+        mbar_arrive_expect_tx(bar, 2 * rows);
+        tma_bulk_g2s_hint(dK, gK, rows, bar, pol);
+        tma_bulk_g2s_hint(dV, gV, rows, bar, pol);
+    }
+}
+
 // One page of one row's online softmax: the scores of this warp's keys (into sc, then one barrier over the consumers),
 // the running max / sum, and PV for this warp's keys.  Both instantiations of attn_rows_kernel run every row through it.
+// Keys past pos are never read from the stage (the producer may not have copied them, ATT_LIVE_TAIL): their score is
+// -inf without a dot product and PV stops before them.  The result is that of scoring them -inf and adding their
+// weight-0 products: e^-inf = 0 adds nothing to l, and fmaf(0, v, acc) == acc for the finite v a written page holds.
 template <typename KVT, int HD>
 __device__ __forceinline__ void att_page(const KVT* K, const KVT* V, float* sc, float* pw, const float (&q)[8], int p,
                                          int pos, float scale, float& m_run, float& l_run, float (&acc)[HD / 32]) {
@@ -302,20 +336,27 @@ __device__ __forceinline__ void att_page(const KVT* K, const KVT* V, float* sc, 
     const float* vscale = reinterpret_cast<const float*>(V + KV_PAGE * HD);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int sub = lane % LPT;
+    const int last = pos - p * KV_PAGE;  // keys t <= last of this page are in the context (every key when last >= 63)
     // ---- scores for this warp's KPW keys
     constexpr int KPW = KV_PAGE / ATT_CWARPS;
 #pragma unroll
     for (int itq = 0; itq < KPW / TPW; ++itq) {
         const int t = warp * KPW + itq * TPW + lane / LPT;
-        float kv[8];
-        load_kv_vec<KVT, 8>(K + t * HD + sub * 8, kv);
         float dsum = 0.f;
+        if (t <= last) {
+            float kv[8];
+            load_kv_vec<KVT, 8>(K + t * HD + sub * 8, kv);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) dsum = fmaf(q[i], kv[i], dsum);
+            for (int i = 0; i < 8; ++i) dsum = fmaf(q[i], kv[i], dsum);
+        }
 #pragma unroll
         for (int o = LPT / 2; o > 0; o >>= 1) dsum += __shfl_xor_sync(0xffffffffu, dsum, o);
-        if constexpr (FP8) dsum *= kscale[t];
-        if (sub == 0) sc[t] = (p * KV_PAGE + t <= pos) ? dsum * scale : -INFINITY;
+        if (t <= last) {
+            if constexpr (FP8) dsum *= kscale[t];
+            if (sub == 0) sc[t] = dsum * scale;
+        } else if (sub == 0) {
+            sc[t] = -INFINITY;
+        }
     }
     named_bar_sync(1, ATT_THREADS);
     // ---- online softmax bookkeeping (every warp redundantly over all 64 scores: identical m, l)
@@ -325,8 +366,8 @@ __device__ __forceinline__ void att_page(const KVT* K, const KVT* V, float* sc, 
     const float e0 = expf(s0 - m_new), e1 = expf(s1 - m_new);
     float* mypw = pw + warp * KV_PAGE;
     if constexpr (FP8) {
-        mypw[lane] = e0 * vscale[lane];
-        mypw[lane + 32] = e1 * vscale[lane + 32];
+        mypw[lane] = lane <= last ? e0 * vscale[lane] : 0.f;
+        mypw[lane + 32] = lane + 32 <= last ? e1 * vscale[lane + 32] : 0.f;
     } else {
         mypw[lane] = e0;
         mypw[lane + 32] = e1;
@@ -340,6 +381,7 @@ __device__ __forceinline__ void att_page(const KVT* K, const KVT* V, float* sc, 
 #pragma unroll
     for (int tt = 0; tt < KPW; ++tt) {
         const int t = warp * KPW + tt;
+        if (t > last) break;
         const float pt_ = mypw[t];
         float vv[DPT];
         load_kv_vec<KVT, DPT>(V + t * HD + lane * DPT, vv);
@@ -413,6 +455,18 @@ __device__ __forceinline__ void att_finish(const float (&acc)[HD / 32], float m_
     named_bar_sync(1, ATT_THREADS);                       // s_last / red[] reused by the next item
 }
 
+// Decode steps: step_prep_kernel stores the step's epoch to row_epoch[r] (release) after it wrote row r's tables, and it
+// writes them only after its own griddepcontrol.wait, when every kernel and copy enqueued before it has completed.  So an
+// acquire load that sees this step's epoch makes row_pos[r], row_pages[r], the group table and every KV page written
+// before the step readable, by the TMA too (the proxy fence), while this grid's predecessors may still be running.
+__device__ __forceinline__ bool att_row_ready(const unsigned long long* row_epoch, int r, unsigned long long epoch) {
+    unsigned long long v;
+    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(row_epoch + r) : "memory");
+    if (v != epoch) return false;
+    asm volatile("fence.proxy.async.global;" ::: "memory");
+    return true;
+}
+
 // Persistent, warp-specialised version: grid = a few CTAs per SM; each CTA walks a static list of work items
 // (row*head, context chunk).  Warp 4 is the TMA producer: it runs ahead ACROSS items, so the HBM stream never drains
 // at an item boundary (short CTAs with a cold start leave HBM idle).
@@ -431,7 +485,8 @@ attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, 
                  const int* __restrict__ row_pos, int H, __nv_bfloat16* __restrict__ act, int ld_act, int bpad,
                  float scale, float* __restrict__ ws, int* __restrict__ cnt, int maxch, int chunk_pages, int n_rh,
                  int n_chunks, const int* __restrict__ row_pages, const int* __restrict__ grp_first,
-                 const int* __restrict__ grp_shared) {
+                 const int* __restrict__ grp_shared, const unsigned long long* __restrict__ row_epoch,
+                 unsigned long long epoch, int opts) {
     using L = AttSmem<KVT, HD>;
     constexpr int LPT = HD / 8;          // lanes per key in QK
     constexpr int DPT = HD / 32;         // output dims per lane in PV
@@ -447,7 +502,14 @@ attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, 
     __shared__ int s_last;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    // row_epoch (decode steps only): the producer issues the first ring stages before griddepcontrol.wait (DESIGN.md 4.1)
+    const bool early = row_epoch != nullptr;
     pdl_launch_dependents();
+    if (opts & ATT_POISON) {
+        uint32_t* ring = reinterpret_cast<uint32_t*>(att_smem);
+        for (int i = threadIdx.x; i < 2 * ATT_STAGES * L::PAGE_BYTES / 4; i += blockDim.x) ring[i] = 0xffffffffu;
+        fence_proxy_async_smem();          // the NaN lands before any copy into the ring
+    }
     if (threadIdx.x == 0) {
         for (int s = 0; s < ATT_STAGES; ++s) {
             mbar_init(&full[s], 1);
@@ -458,9 +520,14 @@ attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, 
         tl_mark_all(0x300);
     }
     __syncthreads();
-    pdl_wait();
+    if (!early || warp != ATT_CWARPS) pdl_wait();
     if (threadIdx.x == 0) { tl_mark(0x310); tl_mark_all(0x310); }
     const int n_items = n_rh * n_chunks;
+    // Producer before griddepcontrol.wait: it reads row r's tables and pages only once att_row_ready(r) saw this step's
+    // epoch, and issues at most ATT_STAGES slabs (no wait on a consumer), all of pages strictly before the one holding
+    // pos, which this layer's QKV epilogue writes.  Everything else, q included, is read after the wait.
+    bool waited = !early;
+    const bool live_tail = opts & ATT_LIVE_TAIL;
 
     if constexpr (GMAX == 1) {
         if (warp == ATT_CWARPS) {
@@ -471,6 +538,10 @@ attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, 
                 for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
                     const int chunk = item / n_rh, rh = item - chunk * n_rh;
                     const int r = rh / H, h = rh - r * H;
+                    if (!waited && !att_row_ready(row_epoch, r, epoch)) {
+                        pdl_wait();
+                        waited = true;
+                    }
                     const int pos = row_pos[r];
                     if (pos < 0) continue;
                     const int npages = pos / KV_PAGE + 1;
@@ -481,12 +552,15 @@ attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, 
                     // L2 round trip away (row -> pages) instead of two (row -> slot -> pages)
                     const int* pt = row_pages ? row_pages + r * max_pages : page_table + row_slot[r] * max_pages;
                     for (int p = p0; p < p1; ++p, ++it) {
+                        if (!waited && (it >= ATT_STAGES || p == npages - 1)) {
+                            pdl_wait();
+                            waited = true;
+                        }
                         const int s = it % ATT_STAGES;
                         if (it >= ATT_STAGES) mbar_wait(&empty[s], ((it / ATT_STAGES) - 1) & 1);
                         const size_t off = (static_cast<size_t>(pt[p]) * H + h) * SLAB;
-                        mbar_arrive_expect_tx(&full[s], 2 * L::PAGE_BYTES);
-                        tma_bulk_g2s_hint(sK + s * SLAB, kpool + off, L::PAGE_BYTES, &full[s], pol);
-                        tma_bulk_g2s_hint(sV + s * SLAB, vpool + off, L::PAGE_BYTES, &full[s], pol);
+                        const int ntok = live_tail && p == npages - 1 ? pos % KV_PAGE + 1 : KV_PAGE;
+                        att_issue<KVT, HD>(sK + s * SLAB, sV + s * SLAB, kpool + off, vpool + off, ntok, &full[s], pol);
                     }
                 }
             }
@@ -604,6 +678,19 @@ attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, 
                 int it = 0;
                 for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
                     const int chunk = item / n_rh, gh = item - chunk * n_rh;
+                    // row 0 published: step_prep has passed its wait, so the group table uploaded before it is in place
+                    if (!waited && !att_row_ready(row_epoch, 0, epoch)) {
+                        pdl_wait();
+                        waited = true;
+                    }
+                    if (!waited) {
+                        const int g = gh / H;
+                        for (int r = grp_first[g]; r < grp_first[g + 1] && !waited; ++r)
+                            if (!att_row_ready(row_epoch, r, epoch)) {
+                                pdl_wait();
+                                waited = true;
+                            }
+                    }
                     int r0, size, h, pos;
                     unsigned live;
                     group_of(gh, r0, size, h, live, pos);
@@ -617,12 +704,15 @@ attn_rows_kernel(const float* __restrict__ qbuf, const KVT* __restrict__ kpool, 
                     for (int p = p0; p < p1; ++p) {
                         for (int j = 0; j < size; ++j) {
                             if (!(live >> j & 1) || (p < S && r0 + j != lead)) continue;
+                            if (!waited && (it >= ATT_STAGES || p == npages - 1)) {
+                                pdl_wait();
+                                waited = true;
+                            }
                             const int s = it % ATT_STAGES;
                             if (it >= ATT_STAGES) mbar_wait(&empty[s], ((it / ATT_STAGES) - 1) & 1);
                             const size_t off = (static_cast<size_t>(pages_of(r0 + j)[p]) * H + h) * SLAB;
-                            mbar_arrive_expect_tx(&full[s], 2 * L::PAGE_BYTES);
-                            tma_bulk_g2s_hint(sK + s * SLAB, kpool + off, L::PAGE_BYTES, &full[s], pol);
-                            tma_bulk_g2s_hint(sV + s * SLAB, vpool + off, L::PAGE_BYTES, &full[s], pol);
+                            const int ntok = live_tail && p == npages - 1 ? pos % KV_PAGE + 1 : KV_PAGE;
+                            att_issue<KVT, HD>(sK + s * SLAB, sV + s * SLAB, kpool + off, vpool + off, ntok, &full[s], pol);
                             ++it;
                         }
                     }
@@ -698,7 +788,8 @@ step_prep_kernel(const int* __restrict__ slots, int n, SlotState* __restrict__ s
                  const int* __restrict__ page_table, int max_pages, int* __restrict__ row_page,
                  int* __restrict__ row_pages, int* __restrict__ row_forced, unsigned int* __restrict__ phase_flags,
                  int n_phase_flags, unsigned int* __restrict__ tile_counters, int n_tile_counters,
-                 __nv_bfloat16* __restrict__ act_tiled) {
+                 __nv_bfloat16* __restrict__ act_tiled, unsigned long long* __restrict__ row_epoch,
+                 unsigned long long epoch) {
     __shared__ float red[8];
     pdl_launch_dependents();
     pdl_wait();
@@ -726,6 +817,10 @@ step_prep_kernel(const int* __restrict__ slots, int n, SlotState* __restrict__ s
     for (int j = threadIdx.x; j < max_pages; j += blockDim.x)       // the attention producer reads these by row
         row_pages[static_cast<size_t>(r) * max_pages + j] = page_table[slot * max_pages + j];
     __syncthreads();
+    if (threadIdx.x == 0) {              // row r's tables are this step's: attention may start its K/V stream (att_row_ready)
+        __threadfence();
+        asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(row_epoch + r), "l"(epoch) : "memory");
+    }
     if (s_pos < 0) return;
     // x row + (LayerNorm folding) gamma0 * x as hi/lo rows and the row statistics for layer 0's QKV GEMM
     float s1 = 0.f, s2 = 0.f;
