@@ -486,11 +486,20 @@ class CodecStream:
         ids = [int(i) for i in ids]
         return self._resampled(None, ids, [0] * len(ids), [True] * len(ids))
 
-    def reset(self, ids):
-        """The listed streams start over at frame 0 (and with an empty resampler)."""
+    @torch.no_grad()
+    def push_audio(self, wav: torch.Tensor, ids, final=None) -> torch.Tensor:
+        """Resampled streams only: continue the listed streams' resamplers with codec-rate audio decoded elsewhere,
+        wav [B, channels, N] -> wav [B, channels, n], row b's first out_lens[b] samples; final[b] as in decode."""
+        if self._rs is None:
+            raise _lib.VcbError("CodecStream.push_audio: this stream runs at the codec's rate; there is nothing to resample")
+        B, ch, N = wav.shape
+        return self._resampled(wav.reshape(B * ch, N), [int(i) for i in ids], [N] * B, final)
+
+    def reset(self, ids, resampler: bool = True):
+        """The listed streams start over at frame 0 (and, unless resampler is False, with an empty resampler)."""
         ids = [int(i) for i in ids]
         _lib.check(self._lib.enc_stream_reset(self._h, (C.c_int32 * max(len(ids), 1))(*ids), len(ids)))
-        if self._rs is not None:
+        if self._rs is not None and resampler:
             self._rs.reset(self._rows(ids))
 
     def close(self):

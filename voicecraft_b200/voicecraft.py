@@ -574,6 +574,48 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
                              mask_intervals=[mask_interval], n_copies=1)
         return _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every, sample_rate)
 
+    # ------------------------------------------------------------------------------------------------
+    # Long TTS  (reference gradio_app.py run, mode "Long TTS"): one prompt, one sentence after another
+    # ------------------------------------------------------------------------------------------------
+    def _long_ticket(self, xs, y, best_of, top_k, top_p, temperature, stop_repetition, silence_tokens):
+        """a one-ticket ContinuousBatcher holding xs as a long ticket on the device generator's stream at its current
+        offset, and the ticket's _Chain"""
+        if self.noise_fn is not None:
+            raise _lib.VcbError("Long TTS samples from the device generator (model.noise_fn must be None)")
+        gen = torch.cuda.default_generators[self.mask_embedding.device.index or 0]
+        cb = ContinuousBatcher(self, max_concurrency=_check_best_of(best_of), top_k=top_k, top_p=top_p,
+                               temperature=temperature, stop_repetition=stop_repetition, silence_tokens=silence_tokens)
+        chain = _Chain(list(xs), int(gen.get_offset()))
+        cb.submit(chain, y, seed=int(gen.initial_seed()), best_of=best_of)
+        return cb, chain, gen
+
+    @torch.no_grad()
+    def inference_long_tts(self, xs, y: torch.Tensor, best_of: int = 1, logprobs: bool = False, top_k: int = -100,
+                           top_p: float = 1.0, temperature: float = 1.0, stop_repetition: int = 3, kvcache: int = 1,
+                           silence_tokens: List[int] = [1388, 1898, 131]):
+        """The reference's Long TTS loop as one call: xs a list of [1,L_i] text-token tensors, one per sentence, all
+        prompted by y [1,T,K].  Returns one (res, gen) per sentence ((res, gen, lp) with logprobs=True), equal to
+        ``[inference_tts(x_i, ., y, ...) for x_i in xs]`` (inference_tts_batch(..., batch_size=best_of) with best_of > 1),
+        and leaves the device generator where that loop leaves it: sentence i+1 samples from where sentence i ended.
+        Runs as one long ticket of a ContinuousBatcher (submit with a list of x); the device generator only."""
+        cb, chain, gen = self._long_ticket(xs, y, best_of, top_k, top_p, temperature, stop_repetition, silence_tokens)
+        out = cb.run()[0]
+        gen.set_offset(chain.offset)
+        self.last_stats = dict(steps=cb.stats["steps"])
+        return [r + (lp,) for r, lp in zip(out, cb.logprobs[0])] if logprobs else out
+
+    def inference_long_tts_stream(self, xs, y: torch.Tensor, tokenizer, chunk_frames: int = 25, sample_rate: int = None,
+                                  top_k: int = -100, top_p: float = 1.0, temperature: float = 1.0,
+                                  stop_repetition: int = 3, kvcache: int = 1, silence_tokens: List[int] = [1388, 1898, 131]):
+        """inference_long_tts with the audio handed out while it is generated: iterates wav chunks [1, channels, n], the
+        sentences in order; concatenated they equal ``torch.cat([tokenizer.decode([(gen_i, None)]) for gen_i in gens],
+        -1)`` (each sentence decoded from a fresh codec state), and with sample_rate the tokenizer.resample of that
+        concatenation.  Afterwards ``.results`` is what inference_long_tts returns, ``.logprobs`` its lp per sentence,
+        and the device generator is left where inference_long_tts leaves it.  best_of = 1 only: the kept copy of a
+        best-of-N sentence is known only when its group ends."""
+        cb, chain, gen = self._long_ticket(xs, y, 1, top_k, top_p, temperature, stop_repetition, silence_tokens)
+        return LongTtsStream(cb, chain, gen, tokenizer, chunk_frames, sample_rate)
+
 
 def _check_best_of(best_of) -> int:
     if isinstance(best_of, bool) or int(best_of) != best_of or best_of < 1:
@@ -919,13 +961,17 @@ class TtsStream(_AudioStream):
 
 class _Utterance:
     """An utterance of a streaming loop: engine slot, codec stream id, its vcb_edit_source (_Prompt.source), frames sent
-    to the codec (pushed), all of its audio handed out (closed), its vcb_status at the last poll."""
-    __slots__ = ("slot", "cid", "label", "ticket", "src", "pushed", "closed", "status")
+    to the codec (pushed), all of its audio handed out (closed), its vcb_status at the last poll.  A sentence of a long
+    ticket shares its codec stream id, and so its resampler stream, with the ticket's other sentences: `more` marks one
+    that a later sentence follows (its resampler stream is not finished with it), `carry` one that an earlier sentence
+    preceded (its resampler stream may hold that sentence's pending samples)."""
+    __slots__ = ("slot", "cid", "label", "ticket", "src", "pushed", "closed", "status", "more", "carry")
 
-    def __init__(self, slot, cid, label, ticket=None, src=None):
+    def __init__(self, slot, cid, label, ticket=None, src=None, more=False, carry=False):
         self.slot, self.cid, self.label, self.ticket = slot, cid, label, ticket
         self.src = _lib.vcb_edit_source() if src is None else src
         self.pushed, self.closed, self.status = 0, False, None
+        self.more, self.carry = more, carry
 
 
 class _PushStep:
@@ -973,13 +1019,15 @@ class _PushStep:
             fin, f = bool(status[j].done), int(final[j])
             new = f - r.pushed
             if r.pushed == 0 and fin and f < self.codec.min_frames:
+                if f == 0 and r.carry and not r.more and self.resampled:     # the earlier sentences' tail is pending
+                    flush.append(j)
                 whole[j] = f
             elif new > 0 and (fin or new >= (self.first if r.pushed == 0 else self.chunk_frames)):
                 push[j] = min(new, mf)
             else:
                 r.closed = fin and r.pushed == f
-                if r.closed and r.pushed > 0 and self.resampled:     # its last push was not final: the tail is pending
-                    flush.append(j)
+                if r.closed and r.pushed > 0 and self.resampled and not r.more:  # its last push was not final: the tail
+                    flush.append(j)                                               # is pending
                 continue
             if bad[3 * j] >= 0:
                 failed[r] = (f"{r.label}: frame {bad[3 * j]} holds the non-audio token {bad[3 * j + 2]} in codebook "
@@ -1001,16 +1049,26 @@ class _PushStep:
                     rows = list(push)
                     wav = self.codec.decode(codes[rows, :, :max(push.values())], ids=[live[j].cid for j in rows],
                                             lens=list(push.values()),
-                                            final=[live[j].closed for j in rows] if self.resampled else None)
+                                            final=[live[j].closed and not live[j].more for j in rows]
+                                            if self.resampled else None)
                     wav_lens = self.codec.out_lens
                 if flush:
                     tail = self.codec.flush([live[j].cid for j in flush])
                     tail_lens = self.codec.out_lens
                 for j, f in whole.items():
-                    if f > 0:
-                        wavs[j] = self.tok.decode_codes(codes[j:j + 1, :, :f])
-                        if self.resampled:
-                            wavs[j] = self.tok.resample(wavs[j], self.tok.sample_rate, self.codec.sample_rate)
+                    r = live[j]
+                    if f == 0:
+                        continue
+                    w = self.tok.decode_codes(codes[j:j + 1, :, :f])
+                    if self.resampled and (r.more or r.carry):     # a long ticket's resampler runs across its sentences
+                        w = self.codec.push_audio(w, [r.cid], [not r.more])
+                        n_out = self.codec.out_lens[0]
+                        if n_out == 0:
+                            continue
+                        w = w[:, :, :n_out]
+                    elif self.resampled:
+                        w = self.tok.resample(w, self.tok.sample_rate, self.codec.sample_rate)
+                    wavs[j] = w
             ev = torch.cuda.Event()
             ev.record(self.cstream)
         t1 = time.perf_counter()
@@ -1054,6 +1112,43 @@ class _SingleTtsStream(TtsStream):
         """after the iteration: the lp that inference_tts / inference return with logprobs=True"""
         lps = TtsStream.logprobs.fget(self)
         return None if lps is None else lps[0]
+
+
+class LongTtsStream:
+    """Iterator of VoiceCraft.inference_long_tts_stream: the wav chunks of its one long ticket (a BatcherStream), in
+    sentence order.  A sentence holding a non-audio frame raises VcbError.  Closing it early releases the engine slots
+    and the codec streams, and leaves the device generator where it was."""
+
+    def __init__(self, cb, chain, gen, tokenizer, chunk_frames, sample_rate):
+        self._cb, self._chain, self._gen = cb, chain, gen
+        self.results = self.logprobs = None
+        self._it = cb.stream(tokenizer, chunk_frames, sample_rate)
+
+    def __iter__(self):
+        return self
+
+    def __next__(self):
+        try:
+            _, w, _ = next(self._it)
+        except StopIteration:
+            cb = self._cb
+            if cb.results and cb.results[0] is not None:
+                self.results, self.logprobs = cb.results[0], cb.logprobs[0]
+                self._gen.set_offset(self._chain.offset)
+            raise
+        if w is None:
+            self.close()
+            raise _lib.VcbError(self._cb.errors[0])
+        return w
+
+    def close(self):
+        self._it.close()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
 
 
 class DecodeSession:
@@ -1275,6 +1370,44 @@ def place_groups(free, sizes, nxt):
     return new, nxt
 
 
+class _Chain:
+    """The sentences of a long ticket (ContinuousBatcher.submit with a list of x): they run one after another on the
+    ticket's slot(s), sentence i+1 sampling from the ticket's Philox stream at the offset where sentence i ended, as the
+    reference's Long TTS loop calls inference_tts once per sentence on one generator.  `offset` is where the next sentence
+    starts (first: 0, or the device generator's offset for VoiceCraft.inference_long_tts), and once the chain is done where
+    its stream ended; `results` / `logprobs` hold the finished sentences'."""
+
+    def __init__(self, xs, offset=0):
+        self.xs, self.offset0 = list(xs), int(offset)
+        self.start([])
+
+    def start(self, prompts):
+        """(re)start the chain with one _Prompt per sentence"""
+        self.prompts, self.offset, self.results, self.logprobs = prompts, self.offset0, [], []
+
+    @property
+    def need_seq(self):
+        return max(p.need_seq for p in self.prompts)
+
+    @property
+    def prompt(self):
+        """the prompt of the sentence to run now"""
+        return self.prompts[len(self.results)]
+
+    def ended(self, result, lp, offset) -> bool:
+        """the sentence running now ended with `result`, `lp`, its stream at `offset` (vcb_status.rng_offset of its slot,
+        its group's first): True when another sentence follows"""
+        self.results.append(result)
+        self.logprobs.append(lp)
+        self.offset = int(offset)
+        return len(self.results) < len(self.prompts)
+
+
+def _need_seq(job):
+    """engine positions a ticket (ContinuousBatcher._job) can reach: a long ticket's longest sentence's"""
+    return job[0].need_seq if job[5] is None else job[5].need_seq
+
+
 _TOO_SMALL = ("KV pool smaller than one utterance (kv_pool_gb; pages held by other open sessions or batchers of this model "
               "count against it)")
 
@@ -1285,7 +1418,8 @@ class KvPoolPolicy:
     snapshot_pages(snapshot), free(snapshot).  An utterance is (key, slot, age, single): age orders admissions (oldest
     first), single marks a one-copy utterance (a best-of-N group keeps its full reservation and never swaps).
       admission  strict FIFO; while anything is swapped out, nothing new; otherwise a ticket needs its prompt pages plus one
-                 growth chunk per active slot free (budget only: the default pool always covers max_slots full slots)
+                 growth chunk per active slot free (budget only: the default pool always covers max_slots full slots).
+                 The next sentence of a long ticket keeps its slots and goes first, swapped-out utterances or not
       victim     a refused step swaps out the youngest single utterance it lists and is retried without it
       resume     swapped-out utterances come back, oldest first, when their pages plus a chunk per active slot are free
       bound      at most max_swapped utterances are out at once
@@ -1297,9 +1431,11 @@ class KvPoolPolicy:
         self.swapped = []                 # [(age, key, snapshot)], oldest first
         self.swap_outs = self.swap_ins = 0
 
-    def admit_count(self, needs, n_active):
-        """how many of the queued tickets `needs` [(pages, slots)] (FIFO order) the pool takes now next to n_active slots"""
-        if self.swapped:
+    def admit_count(self, needs, n_active, held=False):
+        """how many of the queued tickets `needs` [(pages, slots)] (FIFO order) the pool takes now next to n_active slots.
+        held: they already hold their slots (the next sentences of long tickets), so swapped-out utterances, which wait
+        for free slots, do not hold them back"""
+        if self.swapped and not held:
             return 0
         if not self.budget:
             return len(needs)
@@ -1417,7 +1553,9 @@ class ContinuousBatcher:
     y, **params)`` -- or, for an edit ticket, ``model.inference(x, x_lens, y, mask_interval, **params)`` -- returns,
     whatever it was batched with.  run() returns the token lists once the queue has drained; stream() hands out every
     utterance's audio while it is generated and takes submit() / cancel() during the iteration.  A best-of-N ticket
-    (submit(..., best_of=N), run() only) decodes as a group on N consecutive slots; max_concurrency counts slots.
+    (submit(..., best_of=N), run() only) decodes as a group on N consecutive slots; max_concurrency counts slots.  A long
+    ticket (submit with a list of sentences) is the reference's Long TTS loop: its sentences run one after another on its
+    slots, each from where the previous one's random stream ended.
     """
 
     def __init__(self, model: "VoiceCraft", max_concurrency=32, poll_every=8, top_k=-100, top_p=1.0, temperature=1.0,
@@ -1448,9 +1586,28 @@ class ContinuousBatcher:
         top_k, top_p, temperature, stop_repetition, silence_tokens: this ticket's sampling parameters; None takes the
         constructor's value (not inference's or inference_tts' own defaults).
         While a stream() runs, the utterance is admitted at one of its next polls; one that does not fit the engine it
-        sized raises VcbError and is not queued."""
+        sized raises VcbError and is not queued.
+
+        x a list of [1,L_i] tensors, one per sentence: a long ticket, the reference's Long TTS mode (gradio_app.py run):
+        one prompt (y or audio, encoded once, at admission), one set of sampling parameters, and its result a list with
+        one (res, gen) per sentence (logprobs[ticket] likewise) equal to ``torch.manual_seed(seed); [inference_tts(x_i, .,
+        y) for x_i in x]`` (inference_tts_batch(..., batch_size=best_of) with best_of > 1).  Its sentences run one after
+        another on the ticket's slot(s): when one ends, the next is prefilled there at the next poll, from the offset its
+        predecessor's stream ended at, ahead of every queued ticket.  In stream() (best_of = 1) its chunks come in
+        sentence order, each sentence decoded from a fresh codec state as the reference decodes each gen_i, and resampled
+        across sentence boundaries by one resampler stream, so they equal ``resample(torch.cat([decode_codes(gen_i)],
+        -1))``; last=True marks the final sentence's last chunk; cancel() drops the rest of the chain; a sentence that
+        fails fails the ticket and errors[ticket] names it.  Raises ValueError on an empty list, on a list with
+        mask_interval and, while a stream() runs, on a sentence that does not fit its engine."""
         if (y is None) == (audio is None):
             raise ValueError("submit takes exactly one of y (codes) and audio")
+        if isinstance(x, (list, tuple)):
+            x = _Chain(x)
+        if isinstance(x, _Chain):
+            if not x.xs:
+                raise ValueError("a long ticket needs at least one sentence")
+            if mask_interval is not None:
+                raise ValueError("a list of sentences is a long TTS ticket; an edit ticket (mask_interval) takes one x")
         pending = None
         if audio is not None:
             tok = self.tokenizer
@@ -1485,6 +1642,9 @@ class ContinuousBatcher:
         if st is not None:
             _no_stream_best_of(best_of)
             job = self._job(x, y, seed, 1, spans, sp, pending)
+            if job[5] is not None and job[5].need_seq > st.max_seq:
+                raise ValueError(f"a sentence needs {job[5].need_seq} positions, the streaming engine holds {st.max_seq}: "
+                                 "configure_engine(max_seq_len=...) before stream()")
             if job[0].need_seq > st.max_seq:
                 raise _lib.VcbError(f"utterance needs {job[0].need_seq} positions, the streaming engine holds {st.max_seq}: "
                                     "configure_engine(max_seq_len=...) before stream()")
@@ -1506,11 +1666,35 @@ class ContinuousBatcher:
         return True
 
     def _job(self, x, y, seed, best_of, spans, sp, pending=None):
-        """(prompt, seed, best_of, vcb_sampling, pending audio) of a ticket; raises IndexError on an out-of-range id.  An
-        audio ticket's prompt holds placeholder codes until _encode replaces it; pending = (x, audio, sample_rate)."""
-        p = _Prompt(self.model, x, y, spans)
-        self.model._check_ids(p.x_ids, p.y_tok)
-        return p, seed, best_of, sp, pending
+        """(prompt, seed, best_of, vcb_sampling, pending audio, chain) of a ticket; raises IndexError on an out-of-range
+        id.  An audio ticket's prompt holds placeholder codes until _encode replaces it; pending = (x, audio,
+        sample_rate).  A long ticket's chain (x, a _Chain) holds the prompts of its sentences; prompt is the one that
+        runs now."""
+        if not isinstance(x, _Chain):
+            p = _Prompt(self.model, x, y, spans)
+            self.model._check_ids(p.x_ids, p.y_tok)
+            return p, seed, best_of, sp, pending, None
+        x.start([_Prompt(self.model, xi, y) for xi in x.xs])
+        self.model._check_ids(torch.cat([p.x_ids for p in x.prompts]), x.prompts[0].y_tok)
+        return x.prompt, seed, best_of, sp, pending, x
+
+    def _ended(self, eng, slot, st, jobs, t, stream, offset):
+        """A finished utterance of ticket t: its result read from `slot` (its kept copy's) with vcb_status st, its lp to
+        logprobs[t].  Returns (res, gen) as inference_tts returns them ((res, None) of an edit, res as inference returns
+        it); of a long ticket, the list of its sentences' once the last one ends, and None while a sentence follows, its
+        prompt then in jobs[t] and its stream starting at `offset` (rng_offset of the group's first slot)."""
+        m, job = self.model, jobs[t]
+        res, gen, lp = job[0].result(m._read_rows(eng, slot, st.n_steps, stream), st,
+                                     m._read_lp(eng, slot, st.n_steps, stream))
+        chain = job[5]
+        if chain is None:
+            self.logprobs[t] = lp
+            return res, gen
+        if chain.ended((res, gen), lp, offset):
+            jobs[t] = (chain.prompt,) + job[1:]
+            return None
+        self.logprobs[t] = chain.logprobs
+        return chain.results
 
     def _encode(self, tickets, jobs, cstream=None):
         """the prompt audio of the audio tickets among `tickets`, in one encode_many call, and their prompts rebuilt from
@@ -1529,32 +1713,29 @@ class ContinuousBatcher:
             for c in codes.values():
                 c.record_stream(cur)
         for t in todo:
-            p, seed, best_of, sp, (x, _, _) = jobs[t]
-            real = _Prompt(self.model, x, codes[t].transpose(1, 2), p.spans)
+            p, seed, best_of, sp, (x, _, _), chain = jobs[t]
+            y = codes[t].transpose(1, 2)
+            if chain is None:
+                real = _Prompt(self.model, x, y, p.spans)
+            else:                                # every sentence of a long ticket: one encode for the chain
+                chain.start([_Prompt(self.model, xi, y) for xi in chain.xs])
+                real = chain.prompt
             assert real.need_seq == p.need_seq and real.total == p.total
-            jobs[t] = (real, seed, best_of, sp, None)
+            jobs[t] = (real, seed, best_of, sp, None, chain)
 
     def _admit(self, eng, new, jobs, stream, cstream=None):
         """one packed prefill + the first sampling step of the newcomers [(first slot, ticket)], each with its ticket's
         sampling parameters (every sampling call of the batcher passes sp = NULL); the audio tickets among them are
-        encoded first (_encode)"""
+        encoded first (_encode).  A long ticket's sentence starts at its chain's offset, any other ticket at 0."""
         m, lib = self.model, _lib.load()
         self._encode([t for _, t in new], jobs, cstream)
         seed0 = int(torch.cuda.default_generators[m.mask_embedding.device.index or 0].initial_seed())
-        _prefill(eng, [(jobs[t][0], slot, jobs[t][2], seed0 + t if jobs[t][1] is None else jobs[t][1], 0, jobs[t][3])
-                       for slot, t in new], stream)
+        _prefill(eng, [(jobs[t][0], slot, jobs[t][2], seed0 + t if jobs[t][1] is None else jobs[t][1],
+                        0 if jobs[t][5] is None else jobs[t][5].offset, jobs[t][3]) for slot, t in new], stream)
         rows = [s + c for s, t in new for c in range(jobs[t][2])]
         c_new = (C.c_int32 * len(rows))(*rows)
         _lib.check(lib.vcb_sample(eng, c_new, len(rows), None, None, stream))
         self.stats["prefills"] += 1
-
-    def _result(self, eng, slot, st, job, stream, ticket):
-        """(res, gen) of a finished slot, as inference_tts returns them; (res, None) of an edit, res as inference returns
-        it; its lp goes to logprobs[ticket]"""
-        m = self.model
-        res, gen, self.logprobs[ticket] = job[0].result(m._read_rows(eng, slot, st.n_steps, stream), st,
-                                                        m._read_lp(eng, slot, st.n_steps, stream))
-        return res, gen
 
     @torch.no_grad()
     def run(self):
@@ -1567,9 +1748,10 @@ class ContinuousBatcher:
         jobs = [self._job(*q) for q in self.queue]
         sizes = [j[2] for j in jobs]
         n_slots = min(self.B, max(1, sum(sizes)))
-        eng, slots = m._take_slots(n_slots, max([j[0].need_seq for j in jobs], default=0))
+        eng, slots = m._take_slots(n_slots, max([_need_seq(j) for j in jobs], default=0))
         max_pages = (m._eng_opts["max_seq_len"] + 63) // 64
         free, active, results, nxt = set(slots), {}, [None] * len(jobs), 0     # active: first slot -> ticket
+        follow = []                      # [(first slot, ticket)]: long tickets whose next sentence waits in their slots
         self.logprobs = [None] * len(jobs)
         pool = None
         try:
@@ -1577,14 +1759,22 @@ class ContinuousBatcher:
                 stream = torch.cuda.current_stream().cuda_stream
                 pool = KvPoolPolicy(_EngineOps(eng, stream), m._eng_opts["kv_pool_gb"] is not None, self.B)
                 steps = 0
-                while nxt < len(jobs) or active or pool.swapped:
+                while nxt < len(jobs) or active or pool.swapped or follow:
                     n_active = sum(sizes[ji] for ji in active.values())
-                    # ---- swapped-out utterances come back first, then free slot runs take queued tickets in order
-                    for ji, slot in pool.resume(free, n_active):
+                    # ---- the next sentences of long tickets go first, into the slots their tickets kept
+                    k = pool.admit_count([(jobs[t][0].pages(sizes[t], max_pages), sizes[t]) for _, t in follow],
+                                         n_active, held=True) if follow else 0
+                    if k:
+                        self._admit(eng, follow[:k], jobs, stream)
+                        active.update(follow[:k])
+                        follow = follow[k:]
+                    # ---- then swapped-out utterances come back, then free slot runs take queued tickets in order
+                    n_active = sum(sizes[ji] for ji in active.values())
+                    for ji, slot in ([] if follow else pool.resume(free, n_active)):
                         active[slot] = ji
                     n_active = sum(sizes[ji] for ji in active.values())
-                    k = pool.admit_count([(jobs[t][0].pages(sizes[t], max_pages), sizes[t])
-                                          for t in range(nxt, min(len(jobs), nxt + len(free)))], n_active)
+                    k = 0 if follow else pool.admit_count([(jobs[t][0].pages(sizes[t], max_pages), sizes[t])
+                                                           for t in range(nxt, min(len(jobs), nxt + len(free)))], n_active)
                     new, nxt = place_groups(free, sizes[:nxt + k], nxt)
                     if new:
                         self._admit(eng, new, jobs, stream)
@@ -1610,10 +1800,13 @@ class ContinuousBatcher:
                         st = by_slot[slot]
                         if st.done:
                             kept = slot + (st.keep if sizes[ji] > 1 else 0)
-                            results[ji] = self._result(eng, kept, by_slot[kept], jobs[ji], stream, ji)
+                            results[ji] = self._ended(eng, kept, by_slot[kept], jobs, ji, stream, st.rng_offset)
                             m._release_slots(slots, [slot], n_copies=sizes[ji], keep_held=True)
                             del active[slot]
-                            free.update(range(slot, slot + sizes[ji]))
+                            if results[ji] is None:         # a long ticket's next sentence: its slots and pages wait
+                                follow.append((slot, ji))   # for the top of the next round
+                            else:
+                                free.update(range(slot, slot + sizes[ji]))
                 self.stats["steps"] = steps
         finally:
             if pool is not None:
@@ -1651,7 +1844,7 @@ class BatcherStream(_AudioStream):
         if chunk_frames < 1:
             raise ValueError("chunk_frames must be >= 1")
         jobs = [cb._job(*q) for q in cb.queue]
-        eng, slots = m._take_slots(cb.B, max([j[0].need_seq for j in jobs], default=0))
+        eng, slots = m._take_slots(cb.B, max([_need_seq(j) for j in jobs], default=0))
         # a queued best-of-N ticket fails (its kept copy is known only when its group ends); the others are served
         refused = {t for t, j in enumerate(jobs) if j[2] > 1}
         st = SimpleNamespace(cb=cb, eng=eng, slots=slots, max_seq=m._eng_opts["max_seq_len"], jobs=jobs,
@@ -1684,6 +1877,7 @@ class BatcherStream(_AudioStream):
         cb, m = st.cb, st.cb.model
         max_pages = (m._eng_opts["max_seq_len"] + 63) // 64
         free, active, nxt = set(st.slots), {}, 0         # active: slot -> _Utterance
+        follow = []                                      # sentences of long tickets that end, their next one waiting
         ids = list(range(st.codec.max_streams))          # free codec stream ids
         try:
             with torch.cuda.device(st.dev):
@@ -1698,23 +1892,44 @@ class BatcherStream(_AudioStream):
                     # ---- finished, failed and cancelled utterances leave
                     for slot, r in list(active.items()):
                         if r.closed or r.ticket in st.cancelled:
+                            out = None
                             if r.closed and r.ticket not in cb.errors:
-                                cb.results[r.ticket] = cb._result(st.eng, slot, r.status, st.jobs[r.ticket], stream,
-                                                                  r.ticket)
+                                out = cb.results[r.ticket] = cb._ended(st.eng, slot, r.status, st.jobs, r.ticket, stream,
+                                                                       r.status.rng_offset)
                             m._release_slots(st.slots, [slot], keep_held=True)
                             del active[slot]
-                            free.add(slot)
-                            ids.append(r.cid)
+                            if r.more and out is None and r.ticket not in st.cancelled and r.ticket not in cb.errors:
+                                follow.append(r)             # its next sentence: same slot, same codec stream id
+                            else:
+                                free.add(slot)
+                                ids.append(r.cid)
+                    for r in [r for r in follow if r.ticket in st.cancelled]:    # cancelled between two sentences
+                        follow.remove(r)
+                        free.add(r.slot)
+                        ids.append(r.cid)
                     for _, r, _ in list(pool.swapped):       # a cancelled ticket that is swapped out: its snapshot goes
                         if r.ticket in st.cancelled and pool.drop(r):
                             ids.append(r.cid)
-                    # ---- swapped-out tickets come back first (with their codec stream and state), then free slots take
+                    # ---- the next sentences of long tickets go first, into the slots their tickets kept: each from a
+                    # fresh codec state, its resampler stream carried on
+                    k = pool.admit_count([(st.jobs[r.ticket][0].pages(1, max_pages), 1) for r in follow], len(active),
+                                         held=True) if follow else 0
+                    if k:
+                        cb._admit(st.eng, [(r.slot, r.ticket) for r in follow[:k]], st.jobs, stream, st.cstream)
+                        st.codec.reset([r.cid for r in follow[:k]], resampler=False)
+                        for r in follow[:k]:
+                            chain = st.jobs[r.ticket][5]
+                            i = len(chain.results)
+                            active[r.slot] = _Utterance(r.slot, r.cid, f"ticket {r.ticket} sentence {i}", ticket=r.ticket,
+                                                        more=i + 1 < len(chain.prompts), carry=True)
+                        follow = follow[k:]
+                    # ---- then swapped-out tickets come back (with their codec stream and state), then free slots take
                     # the next queued tickets, each with a codec stream id of its own
-                    for r, slot in pool.resume(free, len(active)):
+                    for r, slot in ([] if follow else pool.resume(free, len(active))):
                         r.slot = slot
                         active[slot] = r
                     cands, t = [], nxt
-                    while len(cands) < len(free) and t < len(st.jobs):
+                    while not follow and len(cands) < len(free) and t < len(st.jobs):
                         if t not in st.cancelled:
                             cands.append(t)
                         t += 1
@@ -1730,8 +1945,12 @@ class BatcherStream(_AudioStream):
                         cids = [ids.pop(0) for _ in new]
                         st.codec.reset(cids)
                         for (slot, t), cid in zip(new, cids):
-                            active[slot] = _Utterance(slot, cid, f"ticket {t}", ticket=t, src=st.jobs[t][0].source())
-                    if not active:
+                            chain = st.jobs[t][5]
+                            active[slot] = (_Utterance(slot, cid, f"ticket {t}", ticket=t, src=st.jobs[t][0].source())
+                                            if chain is None else
+                                            _Utterance(slot, cid, f"ticket {t} sentence 0", ticket=t,
+                                                       more=len(chain.prompts) > 1))
+                    if not active and not follow:
                         break
                     live = [active[s] for s in sorted(active)]
                     cb.stats["max_active"] = max(cb.stats["max_active"], len(live))
@@ -1755,15 +1974,16 @@ class BatcherStream(_AudioStream):
                         r.status = s
                         if r in failed:
                             cb.errors[r.ticket] = failed[r]
-                        if r.closed:
+                        if r.closed and (not r.more or r in failed):
                             st.ended.add(r.ticket)
                     for r in live:
-                        if r.ticket in st.cancelled and not r.closed:
+                        if r.ticket in st.cancelled and (not r.closed or r.more):
                             continue
                         if r in failed:
                             yield r.ticket, None, True
                         elif r in wavs:
-                            w = wavs[r]
-                            yield r.ticket, (empty if w is None else w), r.closed
+                            w, last = wavs[r], r.closed and not r.more
+                            if w is not None or last:     # a sentence that ends with no new audio yields nothing
+                                yield r.ticket, (empty if w is None else w), last
         finally:
             BatcherStream._finish(st)
