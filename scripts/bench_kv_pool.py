@@ -7,7 +7,7 @@
   python scripts/bench_kv_pool.py --queue 64         ContinuousBatcher.stream() of 64 bench.py-shaped tickets (text 80,
                                                      150-frame prompt) at max_concurrency 32, alternating an unconstrained
                                                      pool and a --pool-pages budget that forces preemptions: seconds to
-                                                     all audio, p50 / p90 time to first audio, swap counts, equal tokens
+                                                     all audio, p50 / p90 time to first audio, cb.stats, equal tokens
   python scripts/bench_kv_pool.py --ab PARENT_TREE   each tree's `bench.py --gpus 1 --steps 100 --warmup 10 --no-cpu`,
                                                      alternating processes for --rounds rounds (the parent's own Python
                                                      binding: this build's declares symbols the parent library lacks)
@@ -128,8 +128,8 @@ def queue(args):
         total = time.perf_counter() - t0
         fa = sorted(first.values())
         return dict(seconds_to_all_audio=round(total, 3), first_audio_ms_p50=round(statistics.median(fa) * 1e3, 1),
-                    first_audio_ms_p90=round(fa[int(0.9 * (len(fa) - 1))] * 1e3, 1), swap_outs=cb.stats["swap_outs"],
-                    swap_ins=cb.stats["swap_ins"], steps=cb.stats["steps"]), [r[1] for r in cb.results]
+                    first_audio_ms_p90=round(fa[int(0.9 * (len(fa) - 1))] * 1e3, 1), stats=dict(cb.stats)), \
+            [r[1] for r in cb.results]
     for name, gb in pools.items():                           # warm-up of each pool
         run(gb)
     gens = {}

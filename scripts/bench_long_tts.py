@@ -93,7 +93,7 @@ def main():
         for t, _, _ in it:
             now = time.perf_counter() - t0
             # sentences finished when the chunk came: a chain appends a sentence's result after its last chunk
-            sent = len(cb._live.jobs[t][5].results)
+            sent = len(cb._live.jobs[t].chain.results)
             first.setdefault(t, now)
             if t in last_at:
                 gaps["boundary" if sent != last_at[t][1] else "inside"].append(now - last_at[t][0])
@@ -101,7 +101,7 @@ def main():
         torch.cuda.synchronize()
         dt = time.perf_counter() - t0
         frames = sum(int(gen.shape[-1]) for r in cb.results[:n] for _, gen in r)
-        return [first[t] for t in range(n)], dt, frames, gaps
+        return [first[t] for t in range(n)], dt, frames, gaps, dict(cb.stats)
 
     def sequential(n):
         first, frames = {}, 0
@@ -122,7 +122,7 @@ def main():
         sequential(1)
     clocks = bench.ClockSampler(0)
     clocks.start()
-    fa, dt, frames, gaps = batcher(N)
+    fa, dt, frames, gaps, stats = batcher(N)
     seq = sequential(min(args.seq_texts, N)) if args.seq_texts else None
     clk = clocks.stop()
     out = {
@@ -137,7 +137,7 @@ def main():
                     "chunk_gap_ms": {k: {"max": max(v) * 1e3 if v else None,
                                          "median": statistics.median(v) * 1e3 if v else None, "n": len(v)}
                                      for k, v in gaps.items()},
-                    "seconds": dt, "generated_frames": frames, "codec_tokens_per_s": frames * K / dt},
+                    "seconds": dt, "generated_frames": frames, "codec_tokens_per_s": frames * K / dt, "stats": stats},
         "gpu": gpu_identity(0), "clocks": clk,
         "note": "one timed call per arm after an untimed warm-up; wall clock from the arm's start"}
     if seq is not None:

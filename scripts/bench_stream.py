@@ -13,7 +13,7 @@ Every non-audio token except the length cap's end token is suppressed, so every 
 --queue N instead serves N utterances with B slots, their text lengths spread by a fixed seed over
 [--text-len-min, --text-len] (with equal lengths every utterance ends at the same step and continuous batching has nothing
 to gain), two arms alternating in one call:
-  batcher  all N submitted to ContinuousBatcher(max_concurrency=B).stream();
+  batcher  all N submitted to ContinuousBatcher(max_concurrency=B).stream(), its cb.stats reported;
   static   ceil(N/B) consecutive inference_tts_many_stream calls of B utterances.
 
 value = codec tokens/s of the streaming arm, tokens to waveform end to end; first_audio_ms (median / max over the
@@ -166,7 +166,7 @@ def queue(args, cfg, model, tok, xs, ys, seeds, kw):
             first.setdefault(t, time.perf_counter() - t0)
         torch.cuda.synchronize()
         return [first[t] for t in range(N)], time.perf_counter() - t0, sum(int(r[1].shape[-1]) for r in cb.results), \
-            it.push_host_seconds
+            it.push_host_seconds, dict(cb.stats)
 
     def static():
         first, frames, push_s = {}, 0, 0.0
@@ -179,7 +179,7 @@ def queue(args, cfg, model, tok, xs, ys, seeds, kw):
             frames += sum(int(r[1].shape[-1]) for r in ts.results)
             push_s += ts.push_host_seconds
         torch.cuda.synchronize()
-        return [first[t] for t in range(N)], time.perf_counter() - t0, frames, push_s
+        return [first[t] for t in range(N)], time.perf_counter() - t0, frames, push_s, None
 
     batcher(), static()                          # untimed warm-up
     clocks = bench.ClockSampler(0)
@@ -197,6 +197,8 @@ def queue(args, cfg, model, tok, xs, ys, seeds, kw):
                                          "max": fa[-1] * 1e3},
                       "seconds_to_all_audio": r[1], "generated_frames": r[2],
                       "codec_tokens_per_s": r[2] * K / r[1], "push_host_ms": r[3] * 1e3, "seconds_all": [v[1] for v in rs]}
+        if r[4] is not None:
+            arms[name]["stats"] = r[4]
     print(json.dumps({
         "metric": f"seconds to all audio (giga{args.model} streaming TTS, {N} queued utterances, {B} slots)",
         "value": arms["batcher"]["seconds_to_all_audio"], "unit": "s", "n_gpus": 1, "higher_is_better": False,

@@ -1,10 +1,11 @@
 """KV pool budget: pages taken as utterances grow, refusal of a step the pool cannot cover, and swapping an utterance to host
-memory and back byte for byte.  CPU: the batcher's pool policy (KvPoolPolicy) against a fake engine, and the default
-vcb_config.  GPU (-m gpu): page accounting under a budget, a refused step against an engine that was never refused, swaps
-against uninterrupted runs (logits, tokens, KV bytes) in every KV / weight policy, head dim and step path, snapshot
-lifetimes, and ContinuousBatcher.run() under a budget that forces swaps."""
+memory and back byte for byte.  CPU: the batcher's pool policy (KvPoolPolicy) and its admission round against a fake
+engine, and the default vcb_config.  GPU (-m gpu): page accounting under a budget, a refused step against an engine that
+was never refused, swaps against uninterrupted runs (logits, tokens, KV bytes) in every KV / weight policy, head dim and
+step path, snapshot lifetimes, and ContinuousBatcher.run() under a budget that forces swaps."""
 import ctypes as C
 import gc
+from types import SimpleNamespace
 
 import numpy as np
 import pytest
@@ -21,6 +22,7 @@ KW = dict(top_k=40, top_p=1.0, temperature=1.0, stop_repetition=3)
 # ---------------------------------------------------------------------------------------------------------------------
 class FakeEngine:
     """every listed slot takes one more page per step; a step the free pages cannot cover is refused and changes nothing"""
+    stream = None                                      # the CUDA stream of _EngineOps, which the batcher's state takes
 
     def __init__(self, pool):
         self.pool, self.held, self.log = pool, {}, []
@@ -146,6 +148,113 @@ def test_policy_caps_the_swapped_out_utterances():
         pol.step([("a", 0, 0, True), ("b", 1, 1, True), ("c", 2, 2, True)])
     assert [t[1] for t in pol.swapped] == ["c"]
     pol.close()
+
+
+def _serving(eng, n_slots, tickets, cancelled=(), budget=True):
+    """ContinuousBatcher's serving state over the fake engine, with no model: tickets lists (best_of, sentences), with
+    sentences None for a plain ticket, whose prompt asks admission for a page per slot, and for a long ticket the pages
+    each sentence's prompt asks per slot.  The prefill (_admit) takes one page per slot and logs ("admit", [(slot,
+    ticket)]) next to the engine's steps and swaps; releasing a slot gives its pages back; every result is ("res", "gen")"""
+    from voicecraft_b200.voicecraft import ContinuousBatcher, _Chain, _Ticket
+
+    def prompt(pages):
+        return SimpleNamespace(pages=lambda n, max_pages: n * pages, source=_lib.vcb_edit_source,
+                               result=lambda *a: ("res", "gen", "lp"))
+
+    def release(held, starts, n_copies=1, keep_held=False):
+        for s in starts:
+            for c in range(n_copies):
+                eng.held.pop(s + c, None)
+
+    def admit(s, new):
+        eng.log.append(("admit", list(new)))
+        eng.held.update({slot + c: 1 for slot, t in new for c in range(s.jobs[t].best_of)})
+    model = SimpleNamespace(_eng_opts=dict(max_seq_len=64, kv_pool_gb=1.0 if budget else None), _release_slots=release,
+                            _read_rows=lambda *a: None, _read_lp=lambda *a: None)
+    cb = ContinuousBatcher(model, max_concurrency=n_slots, poll_every=1)
+    cb._admit, cb.logprobs = admit, [None] * len(tickets)
+    jobs = []
+    for n, sentences in tickets:
+        chain = None if sentences is None else _Chain(["x"] * len(sentences))
+        if chain is not None:
+            chain.start([prompt(pages) for pages in sentences])
+        jobs.append(_Ticket(prompt(1) if chain is None else chain.prompt, None, n, None, chain=chain))
+    s = SimpleNamespace(eng=None, slots=list(range(n_slots)), jobs=jobs, results=[None] * len(jobs),
+                        cancelled=set(cancelled), cstream=None, pool=None)
+    cb._open(s, eng)
+    s.pool.chunk = 1                                   # the fake engine's slots grow a page per step
+    return cb, s
+
+
+def _ended(r, offset=0, keep=0):
+    r.status = SimpleNamespace(n_steps=0, rng_offset=offset, keep=keep)
+    return r.slot + keep, r.status
+
+
+def test_batcher_round_order_under_a_budget():
+    """One admission round, shared by run() and stream(): a held next sentence first, no swapped-out utterance back
+    while it waits, then swapped-out utterances, then the queue in order, cancelled tickets skipped; freed slots are
+    reused lowest first"""
+    eng = FakeEngine(9)
+    # ticket 0: a long ticket whose second sentence asks 6 pages; 3 is cancelled; 4 is a best-of-2 group
+    cb, s = _serving(eng, 5, [(1, [1, 6]), (1, None), (1, None), (1, None), (2, None), (1, None)], cancelled={3})
+    followed, new = cb._round(s)
+    # 1 + 2 + 3 + (2 + 3) of 9 pages; ticket 5 would need 1 + 5 of the 4 left
+    assert eng.log == [("admit", [(0, 0), (1, 1), (2, 2), (3, 4)])] and followed == []
+    assert [(r.slot, r.ticket) for r in new] == [(0, 0), (1, 1), (2, 2), (3, 4)] and s.nxt == 5 and s.free == set()
+    assert cb.stats["max_active"] == 5
+    # five slots, four free pages: the step is refused and the youngest one-copy utterance (ticket 2) goes out
+    r2 = s.active[2]
+    assert cb._steps(s, [s.active[k] for k in sorted(s.active)]) == 1
+    assert eng.log[1:] == [("refused", (0, 1, 2, 3, 4)), ("out", 2), ("step", (0, 1, 3, 4))]
+    assert sorted(s.active) == [0, 1, 3] and s.free == {2} and [k for _, k, _ in s.pool.swapped] == [r2]
+    assert cb._leave(s, s.active[1], _ended(s.active[1])) is True
+    r0 = s.active[0]
+    assert cb._leave(s, r0, _ended(r0, offset=480)) is False          # its next sentence keeps slot 0
+    assert s.follow == [r0] and s.free == {1, 2} and s.results[:2] == [None, ("res", "gen")]
+    assert s.jobs[0].chain.offset == 480
+    # 5 pages free: the next sentence (6 + a chunk per active slot) waits, and ticket 2 (1 + 3), which the pool would take,
+    # does not come back before it
+    n_log = len(eng.log)
+    assert cb._round(s) == ([], []) and len(eng.log) == n_log and s.follow == [r0] and s.nxt == 5
+    r4 = s.active[3]
+    assert cb._leave(s, r4, _ended(r4, keep=1)) is True and s.free == {1, 2, 3, 4} and eng.held == {}
+    followed, new = cb._round(s)
+    assert eng.log[n_log:] == [("admit", [(0, 0)]), ("in", 1), ("admit", [(2, 5)])]
+    (r,) = followed
+    assert (r.slot, r.cid, r.label, r.carry, r.more) == (0, r0.cid, "ticket 0 sentence 1", True, False)
+    assert s.active[1] is r2 and r2.slot == 1                          # back into the lowest free slot, not its own
+    assert [(r.slot, r.ticket) for r in new] == [(2, 5)] and s.nxt == 6 and s.free == {3, 4} and s.follow == []
+
+
+def test_batcher_round_keeps_a_group_ahead_of_later_tickets():
+    """a best-of-N group that finds no run of free slots stops the admission; a cancelled ticket is passed over"""
+    eng = FakeEngine(0)
+    cb, s = _serving(eng, 4, [(1, None), (1, None), (1, None), (2, None), (1, None), (1, None), (1, None)],
+                     cancelled={5}, budget=False)
+    cb._round(s)
+    assert eng.log == [("admit", [(0, 0), (1, 1), (2, 2)])] and s.nxt == 3 and s.free == {3}
+    cb._leave(s, s.active[1], _ended(s.active[1]))
+    assert cb._round(s) == ([], []) and len(eng.log) == 1 and s.nxt == 3 and s.free == {1, 3}
+    cb._leave(s, s.active[2], _ended(s.active[2]))
+    _, new = cb._round(s)
+    assert eng.log[1:] == [("admit", [(1, 3), (3, 4)])] and s.nxt == 6 and s.free == set()
+    assert [r.label for r in new] == ["ticket 3", "ticket 4"]
+
+
+def test_batcher_round_admits_no_queued_ticket_while_a_next_sentence_waits():
+    eng = FakeEngine(5)
+    cb, s = _serving(eng, 3, [(1, [1, 6]), (1, None), (1, None), (1, None)])
+    cb._round(s)
+    assert eng.log == [("admit", [(0, 0), (1, 1), (2, 2)])] and s.nxt == 3
+    cb._leave(s, s.active[1], _ended(s.active[1]))
+    assert cb._leave(s, s.active[0], _ended(s.active[0])) is False
+    # 4 pages free: the next sentence (6 + 1) waits, and ticket 3 (1 + 1), which the pool would take, is not admitted
+    assert cb._round(s) == ([], []) and len(eng.log) == 1 and s.nxt == 3 and s.free == {1}
+    eng.pool = 9                                       # pages another user of the engine held come back
+    followed, new = cb._round(s)
+    assert eng.log[1:] == [("admit", [(0, 0)]), ("admit", [(1, 3)])]
+    assert [r.ticket for r in followed] == [0] and [r.ticket for r in new] == [3] and s.nxt == 4
 
 
 def test_default_config_is_todays_pool():

@@ -1354,7 +1354,7 @@ class DecodeSession:
 
 
 def place_groups(free, sizes, nxt):
-    """Admission of ContinuousBatcher.run(): tickets nxt, nxt+1, ... in order, ticket t needing sizes[t] consecutive slots
+    """Admission of ContinuousBatcher: tickets nxt, nxt+1, ... in order, ticket t needing sizes[t] consecutive slots
     (its best-of-N group).  Each takes the lowest run of that many consecutive slots in the set `free`; the first ticket
     that finds none stops the admission, so a later ticket never overtakes it.  Removes the taken slots from `free` and
     returns ([(first slot, ticket)], the next ticket to admit)."""
@@ -1403,9 +1403,23 @@ class _Chain:
         return len(self.results) < len(self.prompts)
 
 
-def _need_seq(job):
-    """engine positions a ticket (ContinuousBatcher._job) can reach: a long ticket's longest sentence's"""
-    return job[0].need_seq if job[5] is None else job[5].need_seq
+class _Ticket:
+    """A ContinuousBatcher ticket: `prompt` the _Prompt that runs now (placeholder codes until _encode replaces them),
+    `seed`, `best_of`, `sp` its vcb_sampling, `pending` (x, audio, sample_rate) of audio not encoded yet, and `chain` a
+    long ticket's _Chain."""
+    __slots__ = ("prompt", "seed", "best_of", "sp", "pending", "chain")
+
+    def __init__(self, prompt, seed, best_of, sp, pending=None, chain=None):
+        self.prompt, self.seed, self.best_of, self.sp, self.pending, self.chain = prompt, seed, best_of, sp, pending, chain
+
+    @property
+    def need_seq(self):
+        """engine positions the ticket can reach: a long ticket's longest sentence's"""
+        return self.prompt.need_seq if self.chain is None else self.chain.need_seq
+
+    def pages(self, max_pages):
+        """KV pages the prefill of its prompt takes for its group of best_of copies"""
+        return self.prompt.pages(self.best_of, max_pages)
 
 
 _TOO_SMALL = ("KV pool smaller than one utterance (kv_pool_gb; pages held by other open sessions or batchers of this model "
@@ -1642,12 +1656,12 @@ class ContinuousBatcher:
         if st is not None:
             _no_stream_best_of(best_of)
             job = self._job(x, y, seed, 1, spans, sp, pending)
-            if job[5] is not None and job[5].need_seq > st.max_seq:
-                raise ValueError(f"a sentence needs {job[5].need_seq} positions, the streaming engine holds {st.max_seq}: "
+            if job.chain is not None and job.chain.need_seq > st.max_seq:
+                raise ValueError(f"a sentence needs {job.chain.need_seq} positions, the streaming engine holds {st.max_seq}: "
                                  "configure_engine(max_seq_len=...) before stream()")
-            if job[0].need_seq > st.max_seq:
-                raise _lib.VcbError(f"utterance needs {job[0].need_seq} positions, the streaming engine holds {st.max_seq}: "
-                                    "configure_engine(max_seq_len=...) before stream()")
+            if job.prompt.need_seq > st.max_seq:
+                raise _lib.VcbError(f"utterance needs {job.prompt.need_seq} positions, the streaming engine holds "
+                                    f"{st.max_seq}: configure_engine(max_seq_len=...) before stream()")
             st.jobs.append(job)
             self.results.append(None)
             self.logprobs.append(None)
@@ -1666,75 +1680,158 @@ class ContinuousBatcher:
         return True
 
     def _job(self, x, y, seed, best_of, spans, sp, pending=None):
-        """(prompt, seed, best_of, vcb_sampling, pending audio, chain) of a ticket; raises IndexError on an out-of-range
-        id.  An audio ticket's prompt holds placeholder codes until _encode replaces it; pending = (x, audio,
-        sample_rate).  A long ticket's chain (x, a _Chain) holds the prompts of its sentences; prompt is the one that
-        runs now."""
+        """the _Ticket of submit's arguments; raises IndexError on an out-of-range id.  A long ticket's chain (x, a
+        _Chain) gets the prompts of its sentences."""
         if not isinstance(x, _Chain):
             p = _Prompt(self.model, x, y, spans)
             self.model._check_ids(p.x_ids, p.y_tok)
-            return p, seed, best_of, sp, pending, None
+            return _Ticket(p, seed, best_of, sp, pending)
         x.start([_Prompt(self.model, xi, y) for xi in x.xs])
         self.model._check_ids(torch.cat([p.x_ids for p in x.prompts]), x.prompts[0].y_tok)
-        return x.prompt, seed, best_of, sp, pending, x
+        return _Ticket(x.prompt, seed, best_of, sp, pending, x)
 
-    def _ended(self, eng, slot, st, jobs, t, stream, offset):
-        """A finished utterance of ticket t: its result read from `slot` (its kept copy's) with vcb_status st, its lp to
-        logprobs[t].  Returns (res, gen) as inference_tts returns them ((res, None) of an edit, res as inference returns
-        it); of a long ticket, the list of its sentences' once the last one ends, and None while a sentence follows, its
-        prompt then in jobs[t] and its stream starting at `offset` (rng_offset of the group's first slot)."""
-        m, job = self.model, jobs[t]
-        res, gen, lp = job[0].result(m._read_rows(eng, slot, st.n_steps, stream), st,
-                                     m._read_lp(eng, slot, st.n_steps, stream))
-        chain = job[5]
-        if chain is None:
-            self.logprobs[t] = lp
-            return res, gen
-        if chain.ended((res, gen), lp, offset):
-            jobs[t] = (chain.prompt,) + job[1:]
-            return None
-        self.logprobs[t] = chain.logprobs
-        return chain.results
+    def _open(self, s, ops):
+        """The state of run() / stream(), `s`, holds eng, slots, jobs, results, cancelled and cstream (the codec's CUDA
+        stream; None in run()).  Adds: every slot `free`, nothing `active` (first slot -> _Utterance) or in `follow`
+        (utterances whose next sentence waits in their slots), `nxt` the first queued ticket, and the `pool` policy over
+        `ops` (_EngineOps) on its CUDA `stream`."""
+        o = self.model._eng_opts
+        s.stream, s.max_pages = ops.stream, (o["max_seq_len"] + 63) // 64
+        s.free, s.active, s.follow, s.nxt = set(s.slots), {}, [], 0
+        s.pool = KvPoolPolicy(ops, o["kv_pool_gb"] is not None, self.B)
 
-    def _encode(self, tickets, jobs, cstream=None):
-        """the prompt audio of the audio tickets among `tickets`, in one encode_many call, and their prompts rebuilt from
+    def _close(self, s):
+        """frees the pool's snapshots, adds its swap counts to stats and releases every slot"""
+        if s.pool is not None:
+            s.pool.close()
+            self.stats["swap_outs"] += s.pool.swap_outs
+            self.stats["swap_ins"] += s.pool.swap_ins
+        self.model._release_slots(s.slots)    # every slot: releasing one that is not open does nothing
+        self.queue = []
+
+    def _leave(self, s, r, kept=None):
+        """r leaves `active` and its slots are released.  kept: (slot, vcb_status) of its kept copy when it finished
+        (r.status: its group's first slot's): results[ticket] is then (res, gen) as inference_tts returns them ((res,
+        None) of an edit, res as inference returns it), logprobs[ticket] its lp, and a long ticket's the lists of its
+        sentences' once the last one ends; until then its next sentence (the ticket's prompt now, its stream starting at
+        r.status.rng_offset) keeps the slots in `follow`.  Otherwise they go back to `free` and it returns True."""
+        m, t, job = self.model, r.ticket, s.jobs[r.ticket]
+        follows = False
+        if kept is not None:
+            slot, st = kept
+            res, gen, lp = job.prompt.result(m._read_rows(s.eng, slot, st.n_steps, s.stream), st,
+                                             m._read_lp(s.eng, slot, st.n_steps, s.stream))
+            if job.chain is None:
+                s.results[t], self.logprobs[t] = (res, gen), lp
+            elif job.chain.ended((res, gen), lp, r.status.rng_offset):
+                job.prompt, follows = job.chain.prompt, True
+            else:
+                s.results[t], self.logprobs[t] = job.chain.results, job.chain.logprobs
+        m._release_slots(s.slots, [r.slot], n_copies=job.best_of, keep_held=True)
+        del s.active[r.slot]
+        if follows:
+            s.follow.append(r)
+        else:
+            s.free.update(range(r.slot, r.slot + job.best_of))
+        return not follows
+
+    def _round(self, s):
+        """The admissions of a round: the next sentences of long tickets first, into the slots they kept; while none
+        waits, swapped-out utterances come back, then the next queued tickets that are not cancelled, at most one per free
+        slot, as many as the pool takes, placed by place_groups.  Returns (the next sentences' utterances, the new
+        tickets'), both now in `active`."""
+        jobs, pool = s.jobs, s.pool
+
+        def needs(ts):
+            return [(jobs[t].pages(s.max_pages), jobs[t].best_of) for t in ts]
+
+        def n_active():
+            return sum(jobs[r.ticket].best_of for r in s.active.values())
+
+        def admit(new, cids):
+            if new:
+                self._admit(s, new)
+            for (slot, t), cid in zip(new, cids):
+                chain = jobs[t].chain
+                i = 0 if chain is None else len(chain.results)
+                s.active[slot] = _Utterance(slot, cid, f"ticket {t}" + ("" if chain is None else f" sentence {i}"),
+                                            ticket=t, src=jobs[t].prompt.source(), carry=i > 0,
+                                            more=chain is not None and i + 1 < len(chain.prompts))
+            return [s.active[slot] for slot, _ in new]
+
+        k = pool.admit_count(needs([r.ticket for r in s.follow]), n_active(), held=True) if s.follow else 0
+        followed = admit([(r.slot, r.ticket) for r in s.follow[:k]], [r.cid for r in s.follow[:k]])
+        s.follow, new = s.follow[k:], []
+        if not s.follow:
+            for r, slot in pool.resume(s.free, n_active()):
+                r.slot = slot
+                s.active[slot] = r
+            cands, t = [], s.nxt
+            while len(cands) < len(s.free) and t < len(jobs):
+                if t not in s.cancelled:
+                    cands.append(t)
+                t += 1
+            k = pool.admit_count(needs(cands), n_active())
+            placed, i = place_groups(s.free, [jobs[c].best_of for c in cands[:k]], 0)
+            s.nxt = t if i == len(cands) else cands[i]
+            new = admit([(slot, cands[j]) for slot, j in placed], [None] * len(placed))
+        self.stats["max_active"] = max(self.stats["max_active"], n_active())
+        return followed, new
+
+    def _steps(self, s, live, leaving=False):
+        """Up to poll_every decode steps of the utterances `live` (KvPoolPolicy.step: one swapped out leaves `active`, its
+        slot goes back to `free`; with `leaving`, a step no swap can fit ends the poll early).  Returns the steps taken."""
+        go = [(r, r.slot + c, r.ticket, s.jobs[r.ticket].best_of == 1)
+              for r in live for c in range(s.jobs[r.ticket].best_of)]
+        n = 0
+        for _ in range(self.poll_every if go else 0):
+            go, out = s.pool.step(go, leaving)
+            for r, slot in out:
+                del s.active[slot]
+                s.free.add(slot)
+            if go is None:
+                break
+            n += 1
+        return n
+
+    def _encode(self, jobs, cstream=None):
+        """the prompt audio of the audio tickets among `jobs`, in one encode_many call, and their prompts rebuilt from
         the codes.  cstream: encode there (the codec's stream, whose workspace the encoder
         shares) and make the current stream wait for it."""
-        todo = [t for t in tickets if jobs[t][4] is not None]
+        todo = [j for j in jobs if j.pending is not None]
         if not todo:
             return
         tok, cur = self.tokenizer, torch.cuda.current_stream()
         if cstream is not None:
             cstream.wait_stream(cur)
         with torch.cuda.stream(cstream if cstream is not None else cur):
-            codes = dict(zip(todo, tok.encode_many([jobs[t][4][1] for t in todo], [jobs[t][4][2] for t in todo])))
+            codes = tok.encode_many([j.pending[1] for j in todo], [j.pending[2] for j in todo])
         if cstream is not None:
             cur.wait_stream(cstream)
-            for c in codes.values():
+            for c in codes:
                 c.record_stream(cur)
-        for t in todo:
-            p, seed, best_of, sp, (x, _, _), chain = jobs[t]
-            y = codes[t].transpose(1, 2)
-            if chain is None:
-                real = _Prompt(self.model, x, y, p.spans)
+        for j, c in zip(todo, codes):
+            y = c.transpose(1, 2)
+            if j.chain is None:
+                real = _Prompt(self.model, j.pending[0], y, j.prompt.spans)
             else:                                # every sentence of a long ticket: one encode for the chain
-                chain.start([_Prompt(self.model, xi, y) for xi in chain.xs])
-                real = chain.prompt
-            assert real.need_seq == p.need_seq and real.total == p.total
-            jobs[t] = (real, seed, best_of, sp, None, chain)
+                j.chain.start([_Prompt(self.model, xi, y) for xi in j.chain.xs])
+                real = j.chain.prompt
+            assert real.need_seq == j.prompt.need_seq and real.total == j.prompt.total
+            j.prompt, j.pending = real, None
 
-    def _admit(self, eng, new, jobs, stream, cstream=None):
+    def _admit(self, s, new):
         """one packed prefill + the first sampling step of the newcomers [(first slot, ticket)], each with its ticket's
         sampling parameters (every sampling call of the batcher passes sp = NULL); the audio tickets among them are
         encoded first (_encode).  A long ticket's sentence starts at its chain's offset, any other ticket at 0."""
-        m, lib = self.model, _lib.load()
-        self._encode([t for _, t in new], jobs, cstream)
+        m, lib, jobs = self.model, _lib.load(), s.jobs
+        self._encode([jobs[t] for _, t in new], s.cstream)
         seed0 = int(torch.cuda.default_generators[m.mask_embedding.device.index or 0].initial_seed())
-        _prefill(eng, [(jobs[t][0], slot, jobs[t][2], seed0 + t if jobs[t][1] is None else jobs[t][1],
-                        0 if jobs[t][5] is None else jobs[t][5].offset, jobs[t][3]) for slot, t in new], stream)
-        rows = [s + c for s, t in new for c in range(jobs[t][2])]
+        _prefill(s.eng, [(jobs[t].prompt, slot, jobs[t].best_of, seed0 + t if jobs[t].seed is None else jobs[t].seed,
+                          0 if jobs[t].chain is None else jobs[t].chain.offset, jobs[t].sp) for slot, t in new], s.stream)
+        rows = [slot + c for slot, t in new for c in range(jobs[t].best_of)]
         c_new = (C.c_int32 * len(rows))(*rows)
-        _lib.check(lib.vcb_sample(eng, c_new, len(rows), None, None, stream))
+        _lib.check(lib.vcb_sample(s.eng, c_new, len(rows), None, None, s.stream))
         self.stats["prefills"] += 1
 
     @torch.no_grad()
@@ -1746,76 +1843,36 @@ class ContinuousBatcher:
             raise _lib.VcbError("a stream() of this ContinuousBatcher is running")
         dev, lib = m.mask_embedding.device, _lib.load()
         jobs = [self._job(*q) for q in self.queue]
-        sizes = [j[2] for j in jobs]
-        n_slots = min(self.B, max(1, sum(sizes)))
-        eng, slots = m._take_slots(n_slots, max([_need_seq(j) for j in jobs], default=0))
-        max_pages = (m._eng_opts["max_seq_len"] + 63) // 64
-        free, active, results, nxt = set(slots), {}, [None] * len(jobs), 0     # active: first slot -> ticket
-        follow = []                      # [(first slot, ticket)]: long tickets whose next sentence waits in their slots
+        n_slots = min(self.B, max(1, sum(j.best_of for j in jobs)))
+        eng, slots = m._take_slots(n_slots, max([j.need_seq for j in jobs], default=0))
+        s = SimpleNamespace(eng=eng, slots=slots, jobs=jobs, results=[None] * len(jobs), cancelled=set(), cstream=None,
+                            pool=None)
         self.logprobs = [None] * len(jobs)
-        pool = None
         try:
             with torch.cuda.device(dev):
-                stream = torch.cuda.current_stream().cuda_stream
-                pool = KvPoolPolicy(_EngineOps(eng, stream), m._eng_opts["kv_pool_gb"] is not None, self.B)
+                self._open(s, _EngineOps(eng, torch.cuda.current_stream().cuda_stream))
                 steps = 0
-                while nxt < len(jobs) or active or pool.swapped or follow:
-                    n_active = sum(sizes[ji] for ji in active.values())
-                    # ---- the next sentences of long tickets go first, into the slots their tickets kept
-                    k = pool.admit_count([(jobs[t][0].pages(sizes[t], max_pages), sizes[t]) for _, t in follow],
-                                         n_active, held=True) if follow else 0
-                    if k:
-                        self._admit(eng, follow[:k], jobs, stream)
-                        active.update(follow[:k])
-                        follow = follow[k:]
-                    # ---- then swapped-out utterances come back, then free slot runs take queued tickets in order
-                    n_active = sum(sizes[ji] for ji in active.values())
-                    for ji, slot in ([] if follow else pool.resume(free, n_active)):
-                        active[slot] = ji
-                    n_active = sum(sizes[ji] for ji in active.values())
-                    k = 0 if follow else pool.admit_count([(jobs[t][0].pages(sizes[t], max_pages), sizes[t])
-                                                           for t in range(nxt, min(len(jobs), nxt + len(free)))], n_active)
-                    new, nxt = place_groups(free, sizes[:nxt + k], nxt)
-                    if new:
-                        self._admit(eng, new, jobs, stream)
-                        for slot, ji in new:
-                            active[slot] = ji
-                    live = [(ji, s + c, ji, sizes[ji] == 1) for s, ji in active.items() for c in range(sizes[ji])]
-                    live.sort(key=lambda u: u[1])
-                    self.stats["max_active"] = max(self.stats["max_active"], len(live))
-                    # ---- decode steps for everyone until the next poll; a refused step swaps the youngest out
-                    for _ in range(self.poll_every):
-                        live, out = pool.step(live)
-                        for ji, slot in out:
-                            del active[slot]
-                            free.add(slot)
-                        steps += 1
-                    order = [u[1] for u in live]
+                while True:
+                    self._round(s)
+                    if not s.active and not s.follow:
+                        break
+                    steps += self._steps(s, [s.active[k] for k in sorted(s.active)])
+                    # ---- poll; the utterances that ended leave (a best-of-N group's result is its kept copy's)
+                    order = [k + c for k in sorted(s.active) for c in range(jobs[s.active[k].ticket].best_of)]
                     c_slots = (C.c_int32 * len(order))(*order)
                     status = (_lib.vcb_status * len(order))()
-                    _lib.check(lib.vcb_poll(eng, c_slots, len(order), status, stream))
+                    _lib.check(lib.vcb_poll(eng, c_slots, len(order), status, s.stream))
                     _check_capacity(status)
                     by_slot = dict(zip(order, status))
-                    for slot, ji in list(active.items()):
-                        st = by_slot[slot]
+                    for slot, r in list(s.active.items()):
+                        st = r.status = by_slot[slot]
                         if st.done:
-                            kept = slot + (st.keep if sizes[ji] > 1 else 0)
-                            results[ji] = self._ended(eng, kept, by_slot[kept], jobs, ji, stream, st.rng_offset)
-                            m._release_slots(slots, [slot], n_copies=sizes[ji], keep_held=True)
-                            del active[slot]
-                            if results[ji] is None:         # a long ticket's next sentence: its slots and pages wait
-                                follow.append((slot, ji))   # for the top of the next round
-                            else:
-                                free.update(range(slot, slot + sizes[ji]))
+                            kept = slot + (st.keep if jobs[r.ticket].best_of > 1 else 0)
+                            self._leave(s, r, (kept, by_slot[kept]))
                 self.stats["steps"] = steps
         finally:
-            if pool is not None:
-                pool.close()
-                self.stats["swap_outs"] += pool.swap_outs
-                self.stats["swap_ins"] += pool.swap_ins
-            m._release_slots(slots, [s + c for s, ji in active.items() for c in range(sizes[ji])])
-            self.queue = []
-        return results
+            self._close(s)
+        return s.results
 
     def stream(self, tokenizer, chunk_frames: int = 25, sample_rate: int = None) -> "BatcherStream":
         """run() with every utterance's audio handed out while it is generated: iterates (ticket, wav [1, channels, n*hop],
@@ -1844,15 +1901,15 @@ class BatcherStream(_AudioStream):
         if chunk_frames < 1:
             raise ValueError("chunk_frames must be >= 1")
         jobs = [cb._job(*q) for q in cb.queue]
-        eng, slots = m._take_slots(cb.B, max([_need_seq(j) for j in jobs], default=0))
+        eng, slots = m._take_slots(cb.B, max([j.need_seq for j in jobs], default=0))
         # a queued best-of-N ticket fails (its kept copy is known only when its group ends); the others are served
-        refused = {t for t, j in enumerate(jobs) if j[2] > 1}
+        refused = {t for t, j in enumerate(jobs) if j.best_of > 1}
         st = SimpleNamespace(cb=cb, eng=eng, slots=slots, max_seq=m._eng_opts["max_seq_len"], jobs=jobs,
-                             cancelled=set(refused), ended=set(refused), refused=sorted(refused), tok=tokenizer,
-                             chunk_frames=int(chunk_frames), dev=m.mask_embedding.device, sample_rate=sample_rate,
-                             pool=None)
-        cb.results, cb.logprobs, cb._live = [None] * len(jobs), [None] * len(jobs), st
-        cb.errors = {t: f"best_of={jobs[t][2]}: stream() serves only best_of=1 tickets" for t in refused}
+                             results=[None] * len(jobs), cancelled=set(refused), ended=set(refused),
+                             refused=sorted(refused), tok=tokenizer, chunk_frames=int(chunk_frames),
+                             dev=m.mask_embedding.device, sample_rate=sample_rate, pool=None)
+        cb.results, cb.logprobs, cb._live = st.results, [None] * len(jobs), st
+        cb.errors = {t: f"best_of={jobs[t].best_of}: stream() serves only best_of=1 tickets" for t in refused}
         # a codec stream id belongs to a ticket from its admission to its end: at most max_concurrency are active and, under
         # a KV budget, at most as many more are swapped out
         self._start(st, 2 * cb.B if m._eng_opts["kv_pool_gb"] is not None else cb.B)
@@ -1862,112 +1919,55 @@ class BatcherStream(_AudioStream):
         cb = st.cb
         if cb._live is not st:
             return
-        if st.pool is not None:
-            st.pool.close()
-            cb.stats["swap_outs"] += st.pool.swap_outs
-            cb.stats["swap_ins"] += st.pool.swap_ins
-            st.pool = None
-        cb.model._release_slots(st.slots)    # every slot: releasing one that is not open does nothing
+        cb._close(st)
         _AudioStream._close_codec(st)
-        cb._live, cb.queue = None, []
+        cb._live = None
 
     @staticmethod
     @torch.no_grad()
     def _run(st):
         cb, m = st.cb, st.cb.model
-        max_pages = (m._eng_opts["max_seq_len"] + 63) // 64
-        free, active, nxt = set(st.slots), {}, 0         # active: slot -> _Utterance
-        follow = []                                      # sentences of long tickets that end, their next one waiting
         ids = list(range(st.codec.max_streams))          # free codec stream ids
         try:
             with torch.cuda.device(st.dev):
-                stream = torch.cuda.current_stream().cuda_stream
-                pool = st.pool = KvPoolPolicy(_EngineOps(st.eng, stream), m._eng_opts["kv_pool_gb"] is not None, cb.B)
-                push = st.push = _PushStep(m, st.eng, stream, st.tok, st.codec, st.cstream, st.chunk_frames, cb.poll_every,
-                                           strict=False)
+                cb._open(st, _EngineOps(st.eng, torch.cuda.current_stream().cuda_stream))
+                push = st.push = _PushStep(m, st.eng, st.stream, st.tok, st.codec, st.cstream, st.chunk_frames,
+                                           cb.poll_every, strict=False)
                 empty = torch.zeros(1, st.tok.channels, 0, device=st.dev)
                 for t in st.refused:
                     yield t, None, True
                 while True:
-                    # ---- finished, failed and cancelled utterances leave
-                    for slot, r in list(active.items()):
+                    # ---- finished, failed and cancelled utterances leave; a next sentence keeps the codec stream id
+                    for r in list(st.active.values()):
                         if r.closed or r.ticket in st.cancelled:
-                            out = None
-                            if r.closed and r.ticket not in cb.errors:
-                                out = cb.results[r.ticket] = cb._ended(st.eng, slot, r.status, st.jobs, r.ticket, stream,
-                                                                       r.status.rng_offset)
-                            m._release_slots(st.slots, [slot], keep_held=True)
-                            del active[slot]
-                            if r.more and out is None and r.ticket not in st.cancelled and r.ticket not in cb.errors:
-                                follow.append(r)             # its next sentence: same slot, same codec stream id
-                            else:
-                                free.add(slot)
+                            done = r.closed and r.ticket not in cb.errors
+                            if cb._leave(st, r, (r.slot, r.status) if done else None):
                                 ids.append(r.cid)
-                    for r in [r for r in follow if r.ticket in st.cancelled]:    # cancelled between two sentences
-                        follow.remove(r)
-                        free.add(r.slot)
+                    for r in [r for r in st.follow if r.ticket in st.cancelled]:    # no next sentence of a cancelled ticket
+                        st.follow.remove(r)
+                        st.free.add(r.slot)
                         ids.append(r.cid)
-                    for _, r, _ in list(pool.swapped):       # a cancelled ticket that is swapped out: its snapshot goes
-                        if r.ticket in st.cancelled and pool.drop(r):
+                    for _, r, _ in list(st.pool.swapped):    # a cancelled ticket that is swapped out: its snapshot goes
+                        if r.ticket in st.cancelled and st.pool.drop(r):
                             ids.append(r.cid)
-                    # ---- the next sentences of long tickets go first, into the slots their tickets kept: each from a
-                    # fresh codec state, its resampler stream carried on
-                    k = pool.admit_count([(st.jobs[r.ticket][0].pages(1, max_pages), 1) for r in follow], len(active),
-                                         held=True) if follow else 0
-                    if k:
-                        cb._admit(st.eng, [(r.slot, r.ticket) for r in follow[:k]], st.jobs, stream, st.cstream)
-                        st.codec.reset([r.cid for r in follow[:k]], resampler=False)
-                        for r in follow[:k]:
-                            chain = st.jobs[r.ticket][5]
-                            i = len(chain.results)
-                            active[r.slot] = _Utterance(r.slot, r.cid, f"ticket {r.ticket} sentence {i}", ticket=r.ticket,
-                                                        more=i + 1 < len(chain.prompts), carry=True)
-                        follow = follow[k:]
-                    # ---- then swapped-out tickets come back (with their codec stream and state), then free slots take
-                    # the next queued tickets, each with a codec stream id of its own
-                    for r, slot in ([] if follow else pool.resume(free, len(active))):
-                        r.slot = slot
-                        active[slot] = r
-                    cands, t = [], nxt
-                    while not follow and len(cands) < len(free) and t < len(st.jobs):
-                        if t not in st.cancelled:
-                            cands.append(t)
-                        t += 1
-                    k = pool.admit_count([(st.jobs[c][0].pages(1, max_pages), 1) for c in cands], len(active))
-                    nxt = t if k == len(cands) else cands[k]
-                    new = []
-                    for c in cands[:k]:
-                        slot = min(free)
-                        free.discard(slot)
-                        new.append((slot, c))
+                    followed, new = cb._round(st)
+                    # a next sentence starts from a fresh codec state, its resampler stream carried on; a new ticket
+                    # takes a codec stream id of its own
+                    if followed:
+                        st.codec.reset([r.cid for r in followed], resampler=False)
                     if new:
-                        cb._admit(st.eng, new, st.jobs, stream, st.cstream)
-                        cids = [ids.pop(0) for _ in new]
-                        st.codec.reset(cids)
-                        for (slot, t), cid in zip(new, cids):
-                            chain = st.jobs[t][5]
-                            active[slot] = (_Utterance(slot, cid, f"ticket {t}", ticket=t, src=st.jobs[t][0].source())
-                                            if chain is None else
-                                            _Utterance(slot, cid, f"ticket {t} sentence 0", ticket=t,
-                                                       more=len(chain.prompts) > 1))
-                    if not active and not follow:
+                        for r in new:
+                            r.cid = ids.pop(0)
+                        st.codec.reset([r.cid for r in new])
+                    if not st.active and not st.follow:
                         break
-                    live = [active[s] for s in sorted(active)]
-                    cb.stats["max_active"] = max(cb.stats["max_active"], len(live))
+                    live = [st.active[s] for s in sorted(st.active)]
 
                     def advance(status):
-                        go = [(r, r.slot, r.ticket, True) for r, s in zip(live, status) if not s.done and not r.closed]
+                        go = [r for r, s in zip(live, status) if not s.done and not r.closed]
                         # finished tickets keep their slot and pages until the top of the next round releases them: while
                         # any does, a step that swapping cannot fit waits for those pages instead of failing
-                        leaving = len(go) < len(live)
-                        for _ in range(cb.poll_every if go else 0):   # a refused step swaps the youngest ticket out
-                            go, out = pool.step(go, leaving)
-                            for r, slot in out:
-                                del active[slot]
-                                free.add(slot)
-                            if go is None:
-                                break
-                            cb.stats["steps"] += 1
+                        cb.stats["steps"] += cb._steps(st, go, len(go) < len(live))
                     status, out, failed = push(live, advance)
                     wavs = dict(out)
                     for r, s in zip(live, status):
