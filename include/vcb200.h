@@ -357,7 +357,8 @@ int vcb_set_option(vcb_engine* e, const char* name, int32_t value);
 int vcb_profile_read(vcb_engine* e, double* ms_by_class, int64_t* count_by_class, int32_t n_classes);
 /* "launches", "kv_bytes", "kv_pages_free", "kv_pages_total" (pool size), "kv_pages_needed" (pages the last refused
  * vcb_decode_step lacked), "kv_page_bytes" (one page: 64 positions of K and V in every layer), "swap_stage_bytes" (device
- * staging of the swap kernels), "prefill_rows" (rows through the prefill since create), "weight_bytes" (device
+ * staging of the swap kernels), "prefill_rows" (rows through the prefill since create), "wide_rows" (rows per pass of
+ * the rows-as-M prefill, fixed by its first use; 0 until a prefill took that path), "weight_bytes" (device
  * bytes of the packed GEMM operands with their int8 scales, and the int8 prefill scratch once a prefill allocated it),
  * "mega_grid" (the persistent kernel's grid, 0: not available), "mega_ns" / "mega_nb" / "mega_flight" / "mega_pf" (the ring
  * configuration it runs, 0 without it), ...; "live_bytes" / "live_handles" (any e, NULL included): device and pinned bytes, and allocations

@@ -2859,6 +2859,7 @@ int64_t vcb_counter(vcb_engine* e, const char* name) {
     if (!strcmp(name, "kv_page_bytes")) return static_cast<int64_t>(page_bytes_all_layers(e));
     if (!strcmp(name, "swap_stage_bytes")) return static_cast<int64_t>(e->swap_stage.size() * sizeof(uint4));
     if (!strcmp(name, "prefill_rows")) return e->n_prefill_rows;
+    if (!strcmp(name, "wide_rows")) return e->wide_rows;
     if (!strcmp(name, "weight_bytes")) {         // packed GEMM operands (+ int8 scales) and the int8 prefill scratch
         int64_t b = static_cast<int64_t>(e->w8_wide.size()) * 2;
         auto add = [&](const Matrix& M) { b += static_cast<int64_t>(M.bytes() + (M.is_w8() ? M.rows * sizeof(float) : 0)); };
