@@ -79,7 +79,19 @@ typedef struct {
                              * layer (vcb_counter "kv_page_bytes"); vcb_create rejects a negative value or one below a page */
 } vcb_config;
 
-/* Sampling arguments of inference_tts / inference / inference_tts_batch (voicecraft.py:908-920). */
+/* Sampling arguments of inference_tts / inference / inference_tts_batch (voicecraft.py:908-920), then two controls the
+ * reference lacks, both off at 0 (DESIGN.md section 2.2):
+ *   Repetition-aware sampling (VALL-E 2), ras_window = W in [1, 256], ras_threshold = c in [1, W]: per slot and codebook,
+ *   the token t drawn as the reference draws it (masks, temperature, top-k, top-p, argmax(p / q1)) is redrawn as
+ *   argmax(p_full / q2) when t occurs >= c times among the last min(W, steps of the current generation) tokens of that
+ *   codebook in the slot's token log.  p_full is the softmax of the row after the reference's masks and temperature,
+ *   before top-k / top-p.  Tokens the state machine forces afterwards overwrite as before, and the end-token triggers
+ *   see the final token.  A group with ras_window > 0 consumes two draws of [n_copies*K, V] per step whether or not a
+ *   redraw fires (q1 at the stream's offset, q2 at the next), so it needs the device generator (vcb_prompt.rng_threads)
+ *   and caller noise is rejected for it.
+ *   Length bounds in generated frames (codebook-0 sampling steps of the TTS output or of each edit span): min_frames > 0
+ *   masks the end token on codebook 0 while fewer have been generated; max_frames > 0 forces it at max_frames, as the
+ *   reference's length cap does (the cap still applies).  min_frames <= max_frames when both are set. */
 typedef struct {
     int32_t top_k;
     float top_p;
@@ -87,6 +99,10 @@ typedef struct {
     int32_t stop_repetition;
     int32_t n_silence;
     int32_t silence_tokens[8];
+    int32_t ras_window;
+    int32_t ras_threshold;
+    int32_t min_frames;
+    int32_t max_frames;
 } vcb_sampling;
 
 /* One utterance (or one best-of-N group) to prefill.  `y_tokens` is the already arranged prompt:
@@ -115,7 +131,8 @@ typedef struct {
     int32_t rng_threads, rng_reserved;
     /* The group's own sampling parameters, used by vcb_sample / vcb_decode_step called with sp == NULL; NULL: none (those
      * calls then reject the group's slots).  Rejected with the prompt: n_silence outside [0, 8], a temperature that is not
-     * finite and > 0, a NaN top_p. */
+     * finite and > 0, a NaN top_p, sampling controls outside the ranges vcb_sampling states, ras_window > 0 with
+     * rng_threads == 0. */
     const vcb_sampling* sampling;
 } vcb_prompt;
 
@@ -162,7 +179,8 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
  * exp_noise_dev: [n * K][V] fp32 Exp(1) noise, the draw torch.multinomial makes (voicecraft.py:85); NULL = every listed
  * slot draws from its own generator (vcb_prompt.rng_*), one stream per utterance / best-of-N group.
  * sp: the sampling parameters of every listed slot; NULL = each slot uses its group's (vcb_prompt.sampling), and a slot whose
- * group was prefilled without them is rejected before anything is enqueued. */
+ * group was prefilled without them is rejected before anything is enqueued.  Also rejected before anything is enqueued:
+ * exp_noise_dev set while a listed slot samples with ras_window > 0, an sp whose controls vcb_prefill would reject. */
 int vcb_sample(vcb_engine* e, const int32_t* slots, int32_t n, const float* exp_noise_dev,
                const vcb_sampling* sp, void* stream);
 /* one transformer step on the embeddings produced by the previous sample, then vcb_sample.  Before it enqueues anything,
@@ -248,6 +266,17 @@ int vcb_debug_sampler_lp(const float* logits_dev, const float* noise_dev, uint64
                          int32_t rng_threads, const vcb_sampling* sp, int32_t n, int32_t K, int32_t V, int32_t empty_token,
                          int32_t eog, int32_t eos, int32_t encodec_sr, const int32_t* state_host, int32_t* tokens_host,
                          int32_t* state_out_host, float* lp_host);
+/* vcb_debug_sampler_lp with repetition-aware sampling on (sp->ras_window = W >= 1): hist_host [n][K][W] is each row's
+ * token history per codebook, oldest first, of which the last min(W, cur_num_gen) entries are the token-log rows ahead of
+ * the step.  noise2_dev [n*K][V] is the second Exp(1) plane (q2), given exactly when noise_dev is; with both NULL the rows
+ * draw q1 at (seed, offset) and q2 at the next offset of the stream, as the engine does.  redrew_host [n][K] out: 1 where
+ * the redraw fired, else 0.  lp_host may be NULL.  Rejected as vcb_debug_sampler, and: ras_window < 1, sampling controls
+ * the engine rejects, hist_host or redrew_host NULL, exactly one of noise_dev / noise2_dev NULL, cur_num_gen < 0. */
+int vcb_debug_sampler_ras(const float* logits_dev, const float* noise_dev, const float* noise2_dev, uint64_t seed,
+                          uint64_t offset, int32_t rng_threads, const vcb_sampling* sp, int32_t n, int32_t K, int32_t V,
+                          int32_t empty_token, int32_t eog, int32_t eos, int32_t encodec_sr, const int32_t* state_host,
+                          const int32_t* hist_host, int32_t* tokens_host, int32_t* state_out_host, float* lp_host,
+                          int32_t* redrew_host);
 int vcb_debug_gemm(const float* W_dev /*[N][K]*/, const float* X_dev /*[B][K]*/, float* out_dev /*[B][N]*/, int32_t N,
                    int32_t K, int32_t B, int32_t splits /*<=0: auto*/, int32_t simt);
 /* the int8 weight rule of vcb_finalize_weights on fp32 W [N][K]: q_out [N][K] int8 and e_out [N] with W_deq = q * 2^e.

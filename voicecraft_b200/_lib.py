@@ -28,7 +28,8 @@ KV_GROW_PAGES = 4           # pages a one-copy utterance's page list grows by (V
 
 class vcb_sampling(C.Structure):
     _fields_ = [("top_k", C.c_int32), ("top_p", C.c_float), ("temperature", C.c_float),
-                ("stop_repetition", C.c_int32), ("n_silence", C.c_int32), ("silence_tokens", C.c_int32 * 8)]
+                ("stop_repetition", C.c_int32), ("n_silence", C.c_int32), ("silence_tokens", C.c_int32 * 8),
+                ("ras_window", C.c_int32), ("ras_threshold", C.c_int32), ("min_frames", C.c_int32), ("max_frames", C.c_int32)]
 
 
 class vcb_prompt(C.Structure):
@@ -81,6 +82,9 @@ PROTOTYPES = {
                           [C.c_int32] * 7 + [C.POINTER(C.c_int32)] * 3),
     "vcb_debug_sampler_lp": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int32, C.POINTER(vcb_sampling)] +
                              [C.c_int32] * 7 + [C.POINTER(C.c_int32)] * 3 + [C.POINTER(C.c_float)]),
+    "vcb_debug_sampler_ras": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_int32,
+                                        C.POINTER(vcb_sampling)] + [C.c_int32] * 7 + [C.POINTER(C.c_int32)] * 4 +
+                              [C.POINTER(C.c_float), C.POINTER(C.c_int32)]),
     "vcb_debug_gemm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "vcb_debug_weight_quantize": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
     "vcb_debug_gemm_w8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),

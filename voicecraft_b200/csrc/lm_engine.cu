@@ -59,6 +59,13 @@ struct Layer {
 using namespace vcb;
 static_assert(KV_BF16 == VCB_KV_BF16 && KV_FP32 == VCB_KV_FP32 && KV_FP8 == VCB_KV_FP8, "KV policy ids of vcb_internal.h");
 
+// vcb_engine::group_sp, bits: the group was prefilled with sampling parameters of its own; they turn on repetition-aware
+// sampling or a length bound (its steps run the sampler instance with those controls); they turn on repetition-aware
+// sampling (its steps take no caller noise)
+enum : char { GROUP_SP_OWN = 1, GROUP_SP_CTL = 2, GROUP_SP_RAS = 4 };
+
+static bool controls_on(const vcb_sampling* q) { return q->ras_window != 0 || q->min_frames != 0 || q->max_frames != 0; }
+
 struct vcb_engine {
     vcb_config cfg;
     ModelDims m;
@@ -73,7 +80,7 @@ struct vcb_engine {
     std::vector<std::vector<int>> slot_pages;
     std::vector<int> slot_group;      // host mirror: group id per slot (-1 closed)
     std::vector<int> free_groups;
-    std::vector<char> group_sp;       // host mirror: the group was prefilled with its own sampling parameters (sp_tab)
+    std::vector<char> group_sp;       // host mirror: GROUP_SP_* bits of the group's own sampling parameters (sp_tab)
 
     std::map<std::string, DevBuf<float>> f32;     // every loaded fp32 tensor (device)
     std::map<std::string, std::vector<int64_t>> shapes;
@@ -769,7 +776,7 @@ int wide_alloc(vcb_engine* e) {
     return 0;
 }
 
-int launch_sampler(vcb_engine* e, const Pass& p, const float* noise, const vcb_sampling* sp, cudaStream_t st);
+int launch_sampler(vcb_engine* e, const Pass& p, const float* noise, const vcb_sampling* sp, bool ctl, cudaStream_t st);
 
 // ---- decode step through the persistent kernel (mega_step.cu) ---------------------------------------------------------------
 // Phase table of one decode step for a given bpad: L x (QKV, attention, out-proj, FFN1, FFN2), heads stage 1, heads stage 2
@@ -1074,15 +1081,33 @@ int apply_growth(vcb_engine* e, const std::vector<std::pair<int, int>>& grow, cu
     return 0;
 }
 
-// exp_noise_dev may be null only if every listed slot's group carries its own Philox stream (vcb_prompt::rng_threads)
-int noise_required(vcb_engine* e, const int32_t* slots, int n, const float* noise) {
-    if (noise) return 0;
+// exp_noise_dev may be null only if every listed slot's group carries its own Philox stream (vcb_prompt::rng_threads),
+// and must be null when a listed slot samples with repetition-aware sampling (sp, or its group's parameters, with
+// ras_window > 0): its second draw comes from that stream
+int noise_required(vcb_engine* e, const int32_t* slots, int n, const float* noise, const vcb_sampling* sp) {
+    if (noise) {
+        for (int i = 0; i < n; ++i)
+            if (sp ? sp->ras_window > 0 : (e->group_sp[e->slot_group[slots[i]]] & GROUP_SP_RAS) != 0) {
+                set_error("slot %d samples with repetition-aware sampling, which draws from the device generator: "
+                          "exp_noise_dev must be null", slots[i]);
+                return -1;
+            }
+        return 0;
+    }
     for (int i = 0; i < n; ++i)
         if (!e->slot_rng[slots[i]]) {
             set_error("slot %d has no device generator (vcb_prompt.rng_threads == 0): exp_noise_dev must not be null", slots[i]);
             return -1;
         }
     return 0;
+}
+
+// whether the sampler needs its instance with repetition-aware sampling and the length bounds for these slots
+bool sampler_controls(vcb_engine* e, const int32_t* slots, int n, const vcb_sampling* sp) {
+    if (sp) return controls_on(sp);
+    for (int i = 0; i < n; ++i)
+        if (e->group_sp[e->slot_group[slots[i]]] & GROUP_SP_CTL) return true;
+    return false;
 }
 
 // sp may be null only if every listed slot's group was prefilled with its own parameters (vcb_prompt::sampling)
@@ -1099,7 +1124,7 @@ int sampling_required(vcb_engine* e, const int32_t* slots, int n, const vcb_samp
 
 // final LayerNorm + logit heads + fused sampler for the pass's rows, those of the slots in d_slots (already uploaded).
 // Their hidden states are p.x, through p.x_index (vcb_sample: h_slot[slot]; decode: x_rows[row]).
-int sample_rows(vcb_engine* e, const Pass& p, const float* noise, const vcb_sampling* sp, cudaStream_t st) {
+int sample_rows(vcb_engine* e, const Pass& p, const float* noise, const vcb_sampling* sp, bool ctl, cudaStream_t st) {
     const ModelDims& m = e->m;
     const int n = p.rows, bpad = p.bpad;
     // stage 5L: final LayerNorm + first head stage, 5L + 1: second head stage (p.stop: the pass ends after it)
@@ -1150,7 +1175,7 @@ int sample_rows(vcb_engine* e, const Pass& p, const float* noise, const vcb_samp
         }
     }
     if (stops_after(p, 5 * m.L + 2)) return 0;
-    return launch_sampler(e, p, noise, sp, st);
+    return launch_sampler(e, p, noise, sp, ctl, st);
 }
 
 SamplingParams sampling_params(const vcb_sampling* sp) {
@@ -1161,14 +1186,32 @@ SamplingParams sampling_params(const vcb_sampling* sp) {
     s.stop_repetition = sp->stop_repetition;
     s.n_silence = std::min(sp->n_silence, 8);
     for (int i = 0; i < 8; ++i) s.silence_tokens[i] = sp->silence_tokens[i];
+    s.ras_window = sp->ras_window;
+    s.ras_threshold = sp->ras_threshold;
+    s.min_frames = sp->min_frames;
+    s.max_frames = sp->max_frames;
     return s;
+}
+
+// the repetition-aware sampling and length-bound fields of vcb_sampling (include/vcb200.h); `what` names the caller
+int check_controls(const vcb_sampling* q, const char* what) {
+    const bool ras_ok = q->ras_window == 0 ? q->ras_threshold == 0
+                                           : q->ras_window > 0 && q->ras_window <= 256 && q->ras_threshold >= 1 &&
+                                                 q->ras_threshold <= q->ras_window;
+    if (!ras_ok || q->min_frames < 0 || q->max_frames < 0 || (q->max_frames > 0 && q->min_frames > q->max_frames)) {
+        set_error("%s: bad sampling controls (ras_window=%d in [0, 256], ras_threshold=%d in [1, ras_window] or both 0; "
+                  "min_frames=%d, max_frames=%d >= 0, min_frames <= max_frames when max_frames > 0)", what,
+                  q->ras_window, q->ras_threshold, q->min_frames, q->max_frames);
+        return -1;
+    }
+    return 0;
 }
 
 // dynamic shared memory of sampler_kernel: the top-p sort buffer, then the rank of each of the V entries
 size_t sampler_smem(int V) { return SAMP_SORT_N * 8 + static_cast<size_t>(V) * 4; }
 
-// fused sampler over the pass's rows, one CTA per (row, codebook)
-int launch_sampler(vcb_engine* e, const Pass& p, const float* noise, const vcb_sampling* sp, cudaStream_t st) {
+// fused sampler over the pass's rows, one CTA per (row, codebook); ctl: sampler_controls of the listed slots
+int launch_sampler(vcb_engine* e, const Pass& p, const float* noise, const vcb_sampling* sp, bool ctl, cudaStream_t st) {
     const ModelDims& m = e->m;
     const int n = p.rows;
     const int ldl = m.K * m.Vpad;
@@ -1204,7 +1247,8 @@ int launch_sampler(vcb_engine* e, const Pass& p, const float* noise, const vcb_s
     else
         a.sp_tab = e->sp_tab;
     ProfScope ps(e, PC_SAMPLER, st);
-    VCB_CUDA_OK(launch_k(e, sampler_kernel, dim3(n * m.K), dim3(SAMP_THREADS), sampler_smem(m.V), st, a));
+    VCB_CUDA_OK(launch_k(e, ctl ? sampler_kernel<true> : sampler_kernel<false>, dim3(n * m.K), dim3(SAMP_THREADS),
+                         sampler_smem(m.V), st, a));
     LAUNCH_COUNT(e);
     return 0;
 }
@@ -1545,6 +1589,14 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
                               static_cast<double>(q->top_p));
                     return -1;
                 }
+                char what[32];
+                snprintf(what, sizeof(what), "prompt %d", i);
+                if (check_controls(q, what)) return -1;
+                if (q->ras_window > 0 && P.rng_threads == 0) {
+                    set_error("prompt %d: repetition-aware sampling draws from the device generator: rng_threads must be "
+                              "> 0", i);
+                    return -1;
+                }
             }
             for (int c = 0; c < P.n_copies; ++c) {
                 if (e->slot_group[P.slot + c] >= 0 || claimed[P.slot + c]) {
@@ -1596,7 +1648,9 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
         G.off_hi = static_cast<unsigned int>(P.rng_offset >> 32);
         gst.push_back(G);
         gst_id.push_back(gid);
-        e->group_sp[gid] = P.sampling != nullptr;
+        e->group_sp[gid] = !P.sampling ? 0
+                                       : GROUP_SP_OWN | (controls_on(P.sampling) ? GROUP_SP_CTL : 0) |
+                                             (P.sampling->ras_window > 0 ? GROUP_SP_RAS : 0);
         if (P.sampling) gsp.emplace_back(gid, sampling_params(P.sampling));
         EmbedSeq es;
         es.text_ids = reinterpret_cast<const long long*>(P.text_ids_dev);
@@ -1732,7 +1786,8 @@ int vcb_sample(vcb_engine* e, const int32_t* slots, int32_t n, const float* exp_
         return -1;
     }
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
-    if (check_slots(e, slots, n) || noise_required(e, slots, n, exp_noise_dev) || sampling_required(e, slots, n, sp) ||
+    if (check_slots(e, slots, n) || noise_required(e, slots, n, exp_noise_dev, sp) || sampling_required(e, slots, n, sp) ||
+        (sp && check_controls(sp, "sp")) ||
         upload_slots(e, slots, n, st))
         return -1;
     Pass p = narrow_pass(e, n, false);
@@ -1741,7 +1796,7 @@ int vcb_sample(vcb_engine* e, const int32_t* slots, int32_t n, const float* exp_
     p.q = nullptr;
     p.stop = e->opt_stop;
     record_pass(e, p, 5 * e->m.L + 2, false);
-    return sample_rows(e, p, exp_noise_dev, sp, st);
+    return sample_rows(e, p, exp_noise_dev, sp, sampler_controls(e, slots, n, sp), st);
 }
 
 int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float* exp_noise_dev, const vcb_sampling* sp,
@@ -1752,7 +1807,8 @@ int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float*
         return -1;
     }
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
-    if (check_slots(e, slots, n) || noise_required(e, slots, n, exp_noise_dev) || sampling_required(e, slots, n, sp))
+    if (check_slots(e, slots, n) || noise_required(e, slots, n, exp_noise_dev, sp) || sampling_required(e, slots, n, sp) ||
+        (sp && check_controls(sp, "sp")))
         return -1;
     const bool fold = e->opt_fold && !e->opt_simt;
     const bool mega = fold && e->mega_grid > 0 && n <= 32;
@@ -1784,11 +1840,11 @@ int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float*
         record_pass(e, v, e->mega_nph, true);
         if (mega_step(e, n, p.stop, st)) return -1;
         if (p.stop) return 0;
-        return launch_sampler(e, p, exp_noise_dev, sp, st);
+        return launch_sampler(e, p, exp_noise_dev, sp, sampler_controls(e, slots, n, sp), st);
     }
     record_pass(e, p, 5 * e->m.L + 2, false);
     if (forward_layers(e, p, st)) return -1;
-    return sample_rows(e, p, exp_noise_dev, sp, st);
+    return sample_rows(e, p, exp_noise_dev, sp, sampler_controls(e, slots, n, sp), st);
 }
 
 // a failed synchronisation: if the persistent kernel's watchdog fired, say where (the record is in mapped host memory)
@@ -2891,17 +2947,28 @@ int vcb_debug_exponential(float* out_dev, int64_t numel, uint64_t seed, uint64_t
 namespace {
 
 // Parity hook of the fused sampler alone: one sampling step of n one-member groups through sampler_kernel; see
-// include/vcb200.h.  lp_host null: the kernel stores no log-probability (vcb_debug_sampler).  Every argument is checked
-// before anything is allocated or launched; `fn` names the entry point in the error messages.
+// include/vcb200.h.  lp_host null: the kernel stores no log-probability (vcb_debug_sampler).  hist_host [n][K][W]
+// (W = sp->ras_window > 0, vcb_debug_sampler_ras): each row's last tokens, oldest first, of which the last
+// min(W, cur_num_gen) go into the token log ahead of the step; noise2_dev the second noise plane, redrew_host [n][K] out.
+// Every argument is checked before anything is allocated or launched; `fn` names the entry point in the error messages.
 int debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t seed, uint64_t offset, int32_t rng_threads,
                   const vcb_sampling* sp, int32_t n, int32_t K, int32_t V, int32_t empty_token, int32_t eog, int32_t eos,
                   int32_t encodec_sr, const int32_t* state_host, int32_t* tokens_host, int32_t* state_out_host,
-                  float* lp_host, const char* fn) {
-    constexpr int D = 32, MAX_Y = 65536, STEPS = 4;
+                  float* lp_host, const char* fn, const float* noise2_dev = nullptr, const int32_t* hist_host = nullptr,
+                  int32_t* redrew_host = nullptr) {
+    constexpr int D = 32, MAX_Y = 65536;
     if (!logits_dev || !sp || !state_host || !tokens_host || !state_out_host || (!noise_dev && rng_threads < 1)) {
         set_error("%s: null argument (or no noise and rng_threads < 1)", fn);
         return -1;
     }
+    if (check_controls(sp, fn)) return -1;
+    const int W = sp->ras_window;
+    if (W > 0 && (!hist_host || !redrew_host || (!noise_dev != !noise2_dev))) {
+        set_error("%s: ras_window > 0 needs hist_host and redrew_host, and noise_dev and noise2_dev both set or both null",
+                  fn);
+        return -1;
+    }
+    const int STEPS = W + 4;      // the history rows, the step's row and the capacity margin of sampler_finish_slot
     if (n < 1 || K < 1 || K > 8 || V < 1 || V > SAMP_MAXV * SAMP_THREADS) {
         set_error("%s: n >= 1, 1 <= K <= 8, 1 <= V <= %d required (n=%d K=%d V=%d)", fn,
                   SAMP_MAXV * SAMP_THREADS, n, K, V);
@@ -2920,11 +2987,15 @@ int debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t seed
             return -1;
         }
         max_y = std::max(max_y, s[6]);
+        if (W > 0 && s[2] < 0) {
+            set_error("%s: row %d: cur_num_gen >= 0 required with ras_window > 0", fn, i);
+            return -1;
+        }
     }
     const int Vpad = (V + 3) & ~3, rows = n * K;
     DevBuf<float> logits, tables, pe, mask_emb, x_slot;
     DevBuf<float*> E_audio;
-    DevBuf<int> slots, tok_log;
+    DevBuf<int> slots, tok_log, redrew;
     DevBuf<float> lp_log;
     DevBuf<SlotState> st;
     DevBuf<GroupState> gr;
@@ -2933,7 +3004,8 @@ int debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t seed
         pe.alloc(static_cast<size_t>(max_y + 1) * D, true) || mask_emb.alloc(8 * D, true) ||
         x_slot.alloc(static_cast<size_t>(n) * D, true) || E_audio.alloc(K) || slots.alloc(n) ||
         tok_log.alloc(static_cast<size_t>(n) * STEPS * K, true) || st.alloc(n) || gr.alloc(n) ||
-        (lp_host && lp_log.alloc(static_cast<size_t>(n) * STEPS * K, true)))
+        (lp_host && lp_log.alloc(static_cast<size_t>(n) * STEPS * K, true)) ||
+        (W > 0 && redrew.alloc(static_cast<size_t>(rows), true)))
         return -1;
     // the engine's padded layout; pad columns V..Vpad-1 hold 0x70707070 = +2.98e29 (finite after any temperature >= 0.01),
     // so a kernel that reads past V picks a pad column
@@ -2946,6 +3018,8 @@ int debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t seed
     std::vector<int> sl(n);
     std::vector<SlotState> hs(n);
     std::vector<GroupState> hg(n);
+    std::vector<int> toks(static_cast<size_t>(n) * STEPS * K, 0);
+    std::vector<int> row0(n, 0);                   // token-log row the step writes: the history's length
     for (int i = 0; i < n; ++i) {
         const int32_t* s = state_host + 7 * i;
         sl[i] = i;
@@ -2957,6 +3031,14 @@ int debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t seed
         S.prev_token = s[3];
         S.consec = s[4];
         S.active = 1;
+        if (W > 0) {
+            const int h = std::min(W, s[2]);
+            for (int j = 0; j < h; ++j)
+                for (int k = 0; k < K; ++k)
+                    toks[(static_cast<size_t>(i) * STEPS + j) * K + k] =
+                        hist_host[(static_cast<size_t>(i) * K + k) * W + (W - h + j)];
+            S.n_steps = row0[i] = h;
+        }
         GroupState& G = hg[i];
         G = GroupState{};
         G.mode = s[0];
@@ -2974,6 +3056,7 @@ int debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t seed
         }
     }
     VCB_CUDA_OK(cudaMemcpy(slots, sl.data(), n * sizeof(int), cudaMemcpyHostToDevice));
+    VCB_CUDA_OK(cudaMemcpy(tok_log, toks.data(), toks.size() * sizeof(int), cudaMemcpyHostToDevice));
     VCB_CUDA_OK(cudaMemcpy(st, hs.data(), n * sizeof(SlotState), cudaMemcpyHostToDevice));
     VCB_CUDA_OK(cudaMemcpy(gr, hg.data(), n * sizeof(GroupState), cudaMemcpyHostToDevice));
     SamplerArgs a;
@@ -3004,14 +3087,18 @@ int debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t seed
     a.eos = eos > 0 ? eos : -1;
     a.encodec_sr = encodec_sr;
     a.sp = sampling_params(sp);
-    sampler_kernel<<<rows, SAMP_THREADS, sampler_smem(V)>>>(a);
+    a.noise2 = noise2_dev;
+    a.ras_redrew = W > 0 ? static_cast<int*>(redrew) : nullptr;
+    if (controls_on(sp))
+        sampler_kernel<true><<<rows, SAMP_THREADS, sampler_smem(V)>>>(a);
+    else
+        sampler_kernel<false><<<rows, SAMP_THREADS, sampler_smem(V)>>>(a);
     VCB_CUDA_OK(cudaGetLastError());
-    std::vector<int> toks(static_cast<size_t>(n) * STEPS * K);
     VCB_CUDA_OK(cudaMemcpy(toks.data(), tok_log, toks.size() * sizeof(int), cudaMemcpyDeviceToHost));
     VCB_CUDA_OK(cudaMemcpy(hs.data(), st, n * sizeof(SlotState), cudaMemcpyDeviceToHost));
     VCB_CUDA_OK(cudaMemcpy(hg.data(), gr, n * sizeof(GroupState), cudaMemcpyDeviceToHost));
     for (int i = 0; i < n; ++i) {
-        for (int k = 0; k < K; ++k) tokens_host[i * K + k] = toks[static_cast<size_t>(i) * STEPS * K + k];
+        for (int k = 0; k < K; ++k) tokens_host[i * K + k] = toks[(static_cast<size_t>(i) * STEPS + row0[i]) * K + k];
         int32_t* o = state_out_host + 4 * i;
         o[0] = hs[i].prev_token;
         o[1] = hs[i].consec;
@@ -3022,8 +3109,9 @@ int debug_sampler(const float* logits_dev, const float* noise_dev, uint64_t seed
         std::vector<float> lps(static_cast<size_t>(n) * STEPS * K);
         VCB_CUDA_OK(cudaMemcpy(lps.data(), lp_log, lps.size() * sizeof(float), cudaMemcpyDeviceToHost));
         for (int i = 0; i < n; ++i)
-            for (int k = 0; k < K; ++k) lp_host[i * K + k] = lps[static_cast<size_t>(i) * STEPS * K + k];
+            for (int k = 0; k < K; ++k) lp_host[i * K + k] = lps[(static_cast<size_t>(i) * STEPS + row0[i]) * K + k];
     }
+    if (W > 0) VCB_CUDA_OK(cudaMemcpy(redrew_host, redrew, static_cast<size_t>(rows) * sizeof(int), cudaMemcpyDeviceToHost));
     return 0;
 }
 
@@ -3048,6 +3136,20 @@ int vcb_debug_sampler_lp(const float* logits_dev, const float* noise_dev, uint64
     }
     return debug_sampler(logits_dev, noise_dev, seed, offset, rng_threads, sp, n, K, V, empty_token, eog, eos, encodec_sr,
                          state_host, tokens_host, state_out_host, lp_host, "vcb_debug_sampler_lp");
+}
+
+int vcb_debug_sampler_ras(const float* logits_dev, const float* noise_dev, const float* noise2_dev, uint64_t seed,
+                          uint64_t offset, int32_t rng_threads, const vcb_sampling* sp, int32_t n, int32_t K, int32_t V,
+                          int32_t empty_token, int32_t eog, int32_t eos, int32_t encodec_sr, const int32_t* state_host,
+                          const int32_t* hist_host, int32_t* tokens_host, int32_t* state_out_host, float* lp_host,
+                          int32_t* redrew_host) {
+    if (sp && sp->ras_window < 1) {
+        set_error("vcb_debug_sampler_ras: sp->ras_window >= 1 required (vcb_debug_sampler_lp covers RAS off)");
+        return -1;
+    }
+    return debug_sampler(logits_dev, noise_dev, seed, offset, rng_threads, sp, n, K, V, empty_token, eog, eos, encodec_sr,
+                         state_host, tokens_host, state_out_host, lp_host, "vcb_debug_sampler_ras", noise2_dev, hist_host,
+                         redrew_host);
 }
 
 // Debug timeline of the persistent decode-step kernel: the first call enables recording, later calls copy the last

@@ -946,6 +946,10 @@ struct SamplerArgs {
     int empty_token, eog, eos, encodec_sr;
     SamplingParams sp;
     const SamplingParams* sp_tab = nullptr;   // [max_slots] by group id: each slot samples with its group's parameters; null: `sp`
+    // vcb_debug_sampler_ras only: the second Exp(1) plane of a repetition-aware redraw, laid out like `noise` (used when
+    // `noise` is set), and a flag per row set where the redraw fired; the engine leaves both null
+    const float* noise2 = nullptr;
+    int* ras_redrew = nullptr;
 };
 
 static constexpr int SAMP_THREADS = 256;
@@ -962,6 +966,10 @@ __device__ __forceinline__ void lse_merge(float& m, float& s, float om, float os
     m = mm;
 }
 
+// CTL: some listed slot samples with repetition-aware sampling or a length bound (vcb_sampling.ras_window / min_frames /
+// max_frames).  The instance without them is the sampler as it was before those controls, instruction for instruction:
+// steps that use none of them pay nothing for them.
+template <bool CTL>
 __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const __grid_constant__ SamplerArgs a) {
     __shared__ float sred[8];
     __shared__ float s_lse_m[8], s_lse_s[8];            // per warp: (max, sum) of the raw row, for the log-probability
@@ -1025,6 +1033,26 @@ __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const __grid_cons
     const int row = i * K + k;
 
     // ---- load logits (split-K reduce + bias), apply the reference's in-place edits -----------------
+    // the edits of entry v < V with raw logit u (also applied to the full row of a repetition-aware redraw)
+    auto edit = [&](int v, float u) {
+        if (a.eos > 0 && v == (tts ? a.eog : a.eos)) u = -10000.f;                   // :1091-1093 / :816-818
+        if (n_eog == 0) {
+            if (k >= 1 && (v == E || v == a.empty_token)) u = -10000.f;                // :1021-1023
+            if (k == 0 && tts && cur <= a.encodec_sr / 5 && v == E) u = -10000.f;     // :1024-1025
+            if (CTL && k == 0 && cur < sp.min_frames && v == E) u = -10000.f;         // length bound, like :1024-1025
+            if (k == 0 && sp.stop_repetition > 0 && v == S.prev_token && S.consec > sp.stop_repetition) {
+                bool sil = false;
+                for (int t = 0; t < sp.n_silence; ++t) sil |= (sp.silence_tokens[t] == v);
+                if (sil) {                                                             // :1027-1031
+                    const float f = static_cast<float>(S.consec - (sp.stop_repetition - 1));
+                    u = (u < 0.f) ? u * f : u / f;
+                }
+            }
+        } else {
+            if (k > n_eog && (v == E || v == a.empty_token)) u = -10000.f;            // :1056-1058
+        }
+        return u;
+    };
     float l[SAMP_MAXV], raw[SAMP_MAXV];
     float lse_m = -INFINITY;             // this thread's max of the raw (unedited) entries
 #pragma unroll
@@ -1036,21 +1064,7 @@ __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const __grid_cons
             raw[j] = u;
             lse_m = fmaxf(lse_m, u);
             if (a.dbg_logits) a.dbg_logits[static_cast<size_t>(row) * V + v] = u;
-            if (a.eos > 0 && v == (tts ? a.eog : a.eos)) u = -10000.f;                   // :1091-1093 / :816-818
-            if (n_eog == 0) {
-                if (k >= 1 && (v == E || v == a.empty_token)) u = -10000.f;                // :1021-1023
-                if (k == 0 && tts && cur <= a.encodec_sr / 5 && v == E) u = -10000.f;     // :1024-1025
-                if (k == 0 && sp.stop_repetition > 0 && v == S.prev_token && S.consec > sp.stop_repetition) {
-                    bool sil = false;
-                    for (int t = 0; t < sp.n_silence; ++t) sil |= (sp.silence_tokens[t] == v);
-                    if (sil) {                                                             // :1027-1031
-                        const float f = static_cast<float>(S.consec - (sp.stop_repetition - 1));
-                        u = (u < 0.f) ? u * f : u / f;
-                    }
-                }
-            } else {
-                if (k > n_eog && (v == E || v == a.empty_token)) u = -10000.f;            // :1056-1058
-            }
+            u = edit(v, u);
         }
         l[j] = u;
     }
@@ -1297,13 +1311,56 @@ __global__ void __launch_bounds__(SAMP_THREADS) sampler_kernel(const __grid_cons
     block_argmax(best, besti);
     int tok = besti;
 
+    // ---- repetition-aware sampling (DESIGN.md section 2.2): count `tok` in the last min(W, cur) entries of this
+    // codebook's column of the token log (written by earlier steps of this generation); at >= c, redraw from the full
+    // tempered row with the group's second draw of this step.  The count is block-wide, so the branch is uniform.
+    if (CTL && sp.ras_window > 0) {
+        const int h = min(min(sp.ras_window, cur), S.n_steps);
+        const int* col = a.tok_log + (static_cast<size_t>(slot) * a.max_steps + (S.n_steps - h)) * K + k;
+        if (__syncthreads_count(tid < h && col[static_cast<size_t>(tid) * K] == tok) >= sp.ras_threshold) {
+            const unsigned long long base = (static_cast<unsigned long long>(S.member) * K + k) * V;
+            const unsigned long long seed = (static_cast<unsigned long long>(G.seed_hi) << 32) | G.seed_lo;
+            const unsigned long long off = ((static_cast<unsigned long long>(G.off_hi) << 32) | G.off_lo) +
+                torch_draw_offset(static_cast<unsigned long long>(G.size) * K * V, G.rng_threads);
+            // exp(u / temperature - bm) of entry v < V of the edited row: p_full * sum, bm being that row's maximum.
+            // Recomputed in both passes below, which are not unrolled, rather than held: the kernel's register count is
+            // its maximum over all paths, and the redraw must not raise it for steps that take the others
+            auto e_full = [&](int v) {
+                float u = edit(v, a.logits[static_cast<size_t>(i) * a.ldl + k * a.Vpad + v]);
+                if (sp.temperature != 1.0f) u = __fdiv_rn(u, sp.temperature);
+                return expf(u - bm);
+            };
+            float es = 0.f;
+#pragma unroll 1
+            for (int j = 0; j < SAMP_MAXV; ++j)
+                if (tid + j * SAMP_THREADS < V) es += e_full(tid + j * SAMP_THREADS);
+            const float tot2 = block_sum_256(es, sred);
+            best = -1.f;
+            besti = 0x7fffffff;
+#pragma unroll 1
+            for (int j = 0; j < SAMP_MAXV; ++j) {
+                const int v = tid + j * SAMP_THREADS;
+                if (v < V) {
+                    const float q2 = a.noise2 ? a.noise2[static_cast<size_t>(row) * V + v]
+                                              : torch_exponential_at(seed, off, G.rng_threads, base + v);
+                    const float sc = (e_full(v) / tot2) / q2;
+                    if (sc > best || (sc == best && v < besti)) { best = sc; besti = v; }
+                }
+            }
+            block_argmax(best, besti);
+            tok = besti;
+            if (a.ras_redrew && tid == 0) a.ras_redrew[row] = 1;
+        }
+    }
+
     // ---- forced values / end-token logic ----------------------------------------------------------------
     if (tid == 0) {
         if (n_eog == 0) {
             if (cur < K - 1 && k > cur) tok = a.empty_token;                                 // :1037-1039
             if (k == 0) {
                 const int cap = tts ? S.x_len * (a.encodec_sr / 5) : S.x_len * 10;
-                if (tok == E || argmax_raw == E || S.y_len > cap) {                          // :1041-1045
+                if (tok == E || argmax_raw == E || S.y_len > cap ||                          // :1041-1045
+                    (CTL && sp.max_frames > 0 && cur >= sp.max_frames)) {                    // length bound
                     tok = E;
                     atomicMax(&G.trig_keep, S.member + 1);
                 }
@@ -1363,9 +1420,10 @@ __device__ void sampler_finish_slot(const SamplerArgs& a, const SamplingParams& 
     __threadfence();
     // ---- group finalize
     G.arrive = 0;
-    if (G.rng_threads) {                    // one draw of [size*K, V] consumed, whether or not the caller supplied noise
-        unsigned long long off = (static_cast<unsigned long long>(G.off_hi) << 32) | G.off_lo;
-        off += torch_draw_offset(static_cast<unsigned long long>(G.size) * K * a.V, G.rng_threads);
+    if (G.rng_threads) {                    // one draw of [size*K, V] consumed, whether or not the caller supplied noise;
+        unsigned long long off = (static_cast<unsigned long long>(G.off_hi) << 32) | G.off_lo;   // two under RAS
+        off += (sp.ras_window > 0 ? 2ull : 1ull) * torch_draw_offset(static_cast<unsigned long long>(G.size) * K * a.V,
+                                                                     G.rng_threads);
         G.off_lo = static_cast<unsigned int>(off);
         G.off_hi = static_cast<unsigned int>(off >> 32);
     }

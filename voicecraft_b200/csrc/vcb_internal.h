@@ -405,6 +405,8 @@ struct SamplingParams {
     int stop_repetition;
     int silence_tokens[8];
     int n_silence;
+    int ras_window, ras_threshold;      // repetition-aware sampling, 0: off (include/vcb200.h vcb_sampling)
+    int min_frames, max_frames;         // length bounds of the current generation, 0: none
 };
 
 struct ModelDims {

@@ -16,6 +16,10 @@ stream of the model device's default generator and leave it advanced as the refe
 give every utterance its own seed, so row *i* of a batch equals the single call of utterance *i* under that
 seed.  ``noise_fn`` replaces the generator (tests feed CPU-generator noise to compare with the CPU oracle).
 
+Sampling controls the reference lacks, accepted wherever ``top_k`` is and off by default (see sampling_controls):
+``ras_window`` / ``ras_tau`` turn on repetition-aware sampling, ``min_frames`` / ``max_frames`` bound each generation's
+length in frames.
+
 Out of scope (training): ``forward`` and ``prepare_mask_intervals`` raise NotImplementedError.
 """
 import copy
@@ -47,6 +51,47 @@ except Exception:  # pragma: no cover
 KV_DTYPES = {"bf16": 0, "fp32": 1, "fp8": 2}
 # configure_engine(weight_dtype=...) -> vcb_config.weight_dtype (VCB_W_* of include/vcb200.h)
 WEIGHT_DTYPES = {"bf16": 0, "int8": 1}
+
+
+def sampling_controls(ras_window=0, ras_tau=0.1, min_frames=0, max_frames=None):
+    """The vcb_sampling fields (ras_window, ras_threshold, min_frames, max_frames) of the sampling controls the
+    reference lacks (include/vcb200.h, DESIGN.md section 2.2); the defaults change nothing.
+
+    ras_window = W in [0, 256], ras_tau = tau in (0, 1]: repetition-aware sampling (VALL-E 2) for W > 0.  A drawn token
+    that already occurs >= ceil(tau * W) times (computed in float64) among the last W tokens of its codebook in the
+    current generation is redrawn from the full tempered distribution, without top-k / top-p.  Every sampling step then
+    consumes two noise draws of the generator, so the utterance must sample from the device generator: caller noise
+    (model.noise_fn, noise_fns) is rejected.
+    min_frames >= 0: the end token cannot come before that many frames of the TTS output or of each edit span.
+    max_frames None or >= 1: the end token is forced at that many frames, as the reference's length cap forces it.
+    Raises ValueError on a value outside these ranges and on min_frames > max_frames."""
+    def whole(v, name):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+            raise ValueError(f"{name} must be an integer, got {v!r}")
+        return int(v)
+    W, lo = whole(ras_window, "ras_window"), whole(min_frames, "min_frames")
+    if not 0 <= W <= 256:
+        raise ValueError(f"ras_window must lie in [0, 256], got {W}")
+    tau = float(ras_tau)
+    if not 0.0 < tau <= 1.0:
+        raise ValueError(f"ras_tau must lie in (0, 1], got {ras_tau!r}")
+    if lo < 0:
+        raise ValueError(f"min_frames must be >= 0, got {lo}")
+    hi = 0
+    if max_frames is not None:
+        hi = whole(max_frames, "max_frames")
+        if hi < 1:
+            raise ValueError(f"max_frames must be None or >= 1, got {hi}")
+        if lo > hi:
+            raise ValueError(f"min_frames={lo} exceeds max_frames={hi}")
+    return W, (math.ceil(tau * W) if W else 0), lo, hi
+
+
+def _no_host_noise_under_ras(ras_window, host_noise):
+    """repetition-aware sampling draws its second noise plane from the utterance's own device generator"""
+    if ras_window > 0 and host_noise:
+        raise ValueError("ras_window > 0 samples from the device generator: caller noise (model.noise_fn / noise_fns) "
+                         "cannot drive its second draw")
 
 
 def sine_pe(length: int, dim: int) -> torch.Tensor:
@@ -309,9 +354,12 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     # ------------------------------------------------------------------------------------------------
     # helpers
     # ------------------------------------------------------------------------------------------------
-    def _sampling(self, top_k, top_p, temperature, stop_repetition, silence_tokens):
+    def _sampling(self, top_k, top_p, temperature, stop_repetition, silence_tokens, ras_window=0, ras_tau=0.1,
+                  min_frames=0, max_frames=None):
+        W, c, lo, hi = sampling_controls(ras_window, ras_tau, min_frames, max_frames)
         sp = _lib.vcb_sampling(top_k=int(top_k), top_p=float(top_p), temperature=float(temperature),
-                               stop_repetition=int(stop_repetition), n_silence=min(len(silence_tokens), 8))
+                               stop_repetition=int(stop_repetition), n_silence=min(len(silence_tokens), 8),
+                               ras_window=W, ras_threshold=c, min_frames=lo, max_frames=hi)
         for i, t in enumerate(list(silence_tokens)[:8]):
             sp.silence_tokens[i] = int(t)
         return sp
@@ -373,30 +421,36 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     @torch.no_grad()
     def inference_tts(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, top_k: int = -100,
                       top_p: float = 1.0, temperature: float = 1.0, stop_repetition: int = 3, kvcache: int = 1,
-                      silence_tokens: List[int] = [1388, 1898, 131], *kargs, logprobs: bool = False):
+                      silence_tokens: List[int] = [1388, 1898, 131], *kargs, logprobs: bool = False,
+                      ras_window: int = 0, ras_tau: float = 0.1, min_frames: int = 0,
+                      max_frames: Optional[int] = None):
         """logprobs=True: returns (res, gen, lp), lp [1,K,G] fp32 the log-probability of each frame of gen under the
-        model's raw distribution (vcb_read_logprobs)"""
-        return self._tts_impl(x, x_lens, y, top_k, top_p, temperature, stop_repetition, silence_tokens, 1, logprobs)
+        model's raw distribution (vcb_read_logprobs).  ras_window, ras_tau, min_frames, max_frames: see
+        sampling_controls"""
+        sp = self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens, ras_window, ras_tau, min_frames,
+                            max_frames)
+        return self._tts_impl(x, x_lens, y, sp, silence_tokens, 1, logprobs)
 
     @torch.no_grad()
     def inference_tts_batch(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, top_k: int = -100,
                             top_p: float = 1.0, temperature: float = 1.0, stop_repetition: int = 3, kvcache: int = 1,
                             batch_size: int = 5, silence_tokens: List[int] = [1388, 1898, 131], *kargs,
-                            logprobs: bool = False):
+                            logprobs: bool = False, ras_window: int = 0, ras_tau: float = 0.1, min_frames: int = 0,
+                            max_frames: Optional[int] = None):
         """Best-of-N: the first sample to end wins (reference voicecraft.py:1156-1439).  logprobs=True: returns
         (res, gen, lp) as inference_tts does, lp the kept copy's."""
-        return self._tts_impl(x, x_lens, y, top_k, top_p, temperature, stop_repetition, silence_tokens, batch_size,
-                              logprobs)
+        sp = self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens, ras_window, ras_tau, min_frames,
+                            max_frames)
+        return self._tts_impl(x, x_lens, y, sp, silence_tokens, batch_size, logprobs)
 
-    def _tts_impl(self, x, x_lens, y, top_k, top_p, temperature, stop_repetition, silence_tokens, n_copies, logprobs):
+    def _tts_impl(self, x, x_lens, y, sp, silence_tokens, n_copies, logprobs):
         assert x.ndim == 2, x.shape
         assert x_lens.ndim == 1, x_lens.shape
         assert y.ndim == 3, y.shape
         assert y.shape[0] == 1 and y.shape[2] == self.args.n_codebooks, y.transpose(2, 1).shape
         logging.info(f"silence tokens: {silence_tokens}, note that if you are not using the pretrained encodec "
                      f"6f79c6a8, make sure you specified it yourself, rather than using the default")
-        sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
-                             n_copies=n_copies)
+        sess = DecodeSession(self, [x], [y], sp, n_copies=n_copies)
         try:
             out, = sess._run_single(logprobs)
         finally:
@@ -464,9 +518,12 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     @torch.no_grad()
     def inference(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, mask_interval: torch.Tensor,
                   top_k: int = -100, top_p: float = 1.0, temperature: float = 1.0, stop_repetition: int = -1,
-                  kvcache: int = 1, silence_tokens: List[int] = [1388, 1898, 131], *, logprobs: bool = False):
+                  kvcache: int = 1, silence_tokens: List[int] = [1388, 1898, 131], *, logprobs: bool = False,
+                  ras_window: int = 0, ras_tau: float = 0.1, min_frames: int = 0,
+                  max_frames: Optional[int] = None):
         """logprobs=True: returns (res, lp), lp [1,K,T'] fp32 aligned with res: the log-probability of each generated
-        frame under the model's raw distribution (vcb_read_logprobs), NaN on the frames copied from y"""
+        frame under the model's raw distribution (vcb_read_logprobs), NaN on the frames copied from y.  ras_window,
+        ras_tau, min_frames, max_frames: see sampling_controls; the length bounds hold per masked span"""
         assert x.ndim == 2, x.shape
         assert x_lens.ndim == 1, x_lens.shape
         assert y.ndim == 3, y.shape
@@ -474,7 +531,8 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         assert mask_interval.shape == torch.Size((1, mask_interval.shape[1], 2)), mask_interval
         logging.info(f"silence tokens: {silence_tokens}, note that if you are not using the pretrained encodec "
                      f"6f79c6a8, make sure you specified it yourself, rather than using the default")
-        sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
+        sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens,
+                                                            ras_window, ras_tau, min_frames, max_frames),
                              mask_intervals=[mask_interval], n_copies=1)
         try:
             out, = sess._run_single(logprobs)
@@ -489,10 +547,13 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     # state machine; one Exp(1) draw of shape [B*K, V] per step feeds all of them.
     # ------------------------------------------------------------------------------------------------
     def open_edit_session(self, xs, ys, mask_intervals, top_k=-100, top_p=1.0, temperature=1.0, stop_repetition=-1,
-                          silence_tokens=(1388, 1898, 131), seeds=None, noise_fns=None):
+                          silence_tokens=(1388, 1898, 131), seeds=None, noise_fns=None, ras_window=0, ras_tau=0.1,
+                          min_frames=0, max_frames=None):
         """Independent speech-editing utterances decoded as one batch (BASELINE config 3).  mask_intervals: list of
-        [1,M,2] tensors.  Returns a DecodeSession; results() gives the edited [1,K,T'] per utterance."""
-        return DecodeSession(self, xs, ys, self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
+        [1,M,2] tensors.  Returns a DecodeSession; results() gives the edited [1,K,T'] per utterance.  ras_window,
+        ras_tau, min_frames, max_frames: see sampling_controls."""
+        return DecodeSession(self, xs, ys, self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens,
+                                                          ras_window, ras_tau, min_frames, max_frames),
                              mask_intervals=mask_intervals, seeds=seeds, noise_fns=noise_fns)
 
     @torch.no_grad()
@@ -503,7 +564,8 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         return [(r[0], r[2]) if logprobs else r[0] for r in out]
 
     def open_tts_session(self, xs, ys, top_k=-100, top_p=1.0, temperature=1.0, stop_repetition=3,
-                         silence_tokens=(1388, 1898, 131), seeds=None, noise_fns=None, best_of=1):
+                         silence_tokens=(1388, 1898, 131), seeds=None, noise_fns=None, best_of=1, ras_window=0,
+                         ras_tau=0.1, min_frames=0, max_frames=None):
         """xs: list of [1,L] int64, ys: list of [1,T,K] int64 (any device).  Prefills every utterance (one packed,
         chunked pass) and returns a DecodeSession whose .step() runs one decode step for all of them.
 
@@ -514,8 +576,10 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         oracle).
         best_of: each utterance is sampled best_of times and keeps the copy that ends first, what
         ``inference_tts_batch(x_i, ., y_i, batch_size=best_of)`` returns under the same seed.  The copies share one
-        prefill and the KV pages of the prompt's full pages."""
-        return DecodeSession(self, xs, ys, self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
+        prefill and the KV pages of the prompt's full pages.
+        ras_window, ras_tau, min_frames, max_frames: see sampling_controls."""
+        return DecodeSession(self, xs, ys, self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens,
+                                                          ras_window, ras_tau, min_frames, max_frames),
                              seeds=seeds, noise_fns=noise_fns, best_of=best_of)
 
     @torch.no_grad()
@@ -541,13 +605,15 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     def inference_tts_stream(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, tokenizer, chunk_frames: int = 25,
                              poll_every: int = 8, top_k: int = -100, top_p: float = 1.0, temperature: float = 1.0,
                              stop_repetition: int = 3, silence_tokens: List[int] = [1388, 1898, 131],
-                             sample_rate: int = None):
+                             sample_rate: int = None, ras_window: int = 0, ras_tau: float = 0.1, min_frames: int = 0,
+                             max_frames: Optional[int] = None):
         """inference_tts with the audio handed out while it is generated: iterates wav chunks [1, channels, n*hop] whose
         concatenation equals ``tokenizer.decode([(gen, None)])``.  Afterwards ``.result`` is (res, gen), what inference_tts
         returns: the utterance samples from the device generator's stream at its current offset and leaves it advanced by
         the steps it ran, as inference_tts does."""
         assert x.ndim == 2 and x.shape[0] == 1 and x_lens.ndim == 1 and y.ndim == 3 and y.shape[0] == 1, (x.shape, y.shape)
-        sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
+        sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens,
+                                                            ras_window, ras_tau, min_frames, max_frames),
                              n_copies=1)
         return _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every, sample_rate)
 
@@ -563,28 +629,35 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     def inference_stream(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, mask_interval: torch.Tensor, tokenizer,
                          chunk_frames: int = 25, poll_every: int = 8, top_k: int = -100, top_p: float = 1.0,
                          temperature: float = 1.0, stop_repetition: int = -1, kvcache: int = 1,
-                         silence_tokens: List[int] = [1388, 1898, 131], sample_rate: int = None):
+                         silence_tokens: List[int] = [1388, 1898, 131], sample_rate: int = None,
+                         ras_window: int = 0, ras_tau: float = 0.1, min_frames: int = 0,
+                         max_frames: Optional[int] = None):
         """inference (speech editing) with the audio handed out while it is generated: iterates wav chunks
         [1, channels, n*hop] whose concatenation equals ``tokenizer.decode_codes(res)``, the whole edited utterance.
         Afterwards ``.result`` is res, what inference returns, and the device generator is left where inference leaves
         it.  The device generator only (model.noise_fn must be None)."""
         assert x.ndim == 2 and x.shape[0] == 1 and x_lens.ndim == 1 and y.ndim == 3 and y.shape[0] == 1, (x.shape, y.shape)
         assert mask_interval.shape == torch.Size((1, mask_interval.shape[1], 2)), mask_interval
-        sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens),
+        sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens,
+                                                            ras_window, ras_tau, min_frames, max_frames),
                              mask_intervals=[mask_interval], n_copies=1)
         return _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every, sample_rate)
 
     # ------------------------------------------------------------------------------------------------
     # Long TTS  (reference gradio_app.py run, mode "Long TTS"): one prompt, one sentence after another
     # ------------------------------------------------------------------------------------------------
-    def _long_ticket(self, xs, y, best_of, top_k, top_p, temperature, stop_repetition, silence_tokens):
+    def _long_ticket(self, xs, y, best_of, top_k, top_p, temperature, stop_repetition, silence_tokens, ras_window, ras_tau,
+                     min_frames, max_frames):
         """a one-ticket ContinuousBatcher holding xs as a long ticket on the device generator's stream at its current
         offset, and the ticket's _Chain"""
+        _no_host_noise_under_ras(sampling_controls(ras_window, ras_tau, min_frames, max_frames)[0],
+                                 self.noise_fn is not None)
         if self.noise_fn is not None:
             raise _lib.VcbError("Long TTS samples from the device generator (model.noise_fn must be None)")
         gen = torch.cuda.default_generators[self.mask_embedding.device.index or 0]
         cb = ContinuousBatcher(self, max_concurrency=_check_best_of(best_of), top_k=top_k, top_p=top_p,
-                               temperature=temperature, stop_repetition=stop_repetition, silence_tokens=silence_tokens)
+                               temperature=temperature, stop_repetition=stop_repetition, silence_tokens=silence_tokens,
+                               ras_window=ras_window, ras_tau=ras_tau, min_frames=min_frames, max_frames=max_frames)
         chain = _Chain(list(xs), int(gen.get_offset()))
         cb.submit(chain, y, seed=int(gen.initial_seed()), best_of=best_of)
         return cb, chain, gen
@@ -592,13 +665,16 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     @torch.no_grad()
     def inference_long_tts(self, xs, y: torch.Tensor, best_of: int = 1, logprobs: bool = False, top_k: int = -100,
                            top_p: float = 1.0, temperature: float = 1.0, stop_repetition: int = 3, kvcache: int = 1,
-                           silence_tokens: List[int] = [1388, 1898, 131]):
+                           silence_tokens: List[int] = [1388, 1898, 131], ras_window: int = 0, ras_tau: float = 0.1,
+                           min_frames: int = 0, max_frames: Optional[int] = None):
         """The reference's Long TTS loop as one call: xs a list of [1,L_i] text-token tensors, one per sentence, all
         prompted by y [1,T,K].  Returns one (res, gen) per sentence ((res, gen, lp) with logprobs=True), equal to
         ``[inference_tts(x_i, ., y, ...) for x_i in xs]`` (inference_tts_batch(..., batch_size=best_of) with best_of > 1),
         and leaves the device generator where that loop leaves it: sentence i+1 samples from where sentence i ended.
-        Runs as one long ticket of a ContinuousBatcher (submit with a list of x); the device generator only."""
-        cb, chain, gen = self._long_ticket(xs, y, best_of, top_k, top_p, temperature, stop_repetition, silence_tokens)
+        Runs as one long ticket of a ContinuousBatcher (submit with a list of x); the device generator only.
+        ras_window, ras_tau, min_frames, max_frames: see sampling_controls; they apply to every sentence."""
+        cb, chain, gen = self._long_ticket(xs, y, best_of, top_k, top_p, temperature, stop_repetition, silence_tokens,
+                                           ras_window, ras_tau, min_frames, max_frames)
         out = cb.run()[0]
         gen.set_offset(chain.offset)
         self.last_stats = dict(steps=cb.stats["steps"])
@@ -606,14 +682,17 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
 
     def inference_long_tts_stream(self, xs, y: torch.Tensor, tokenizer, chunk_frames: int = 25, sample_rate: int = None,
                                   top_k: int = -100, top_p: float = 1.0, temperature: float = 1.0,
-                                  stop_repetition: int = 3, kvcache: int = 1, silence_tokens: List[int] = [1388, 1898, 131]):
+                                  stop_repetition: int = 3, kvcache: int = 1, silence_tokens: List[int] = [1388, 1898, 131],
+                                  ras_window: int = 0, ras_tau: float = 0.1, min_frames: int = 0,
+                                  max_frames: Optional[int] = None):
         """inference_long_tts with the audio handed out while it is generated: iterates wav chunks [1, channels, n], the
         sentences in order; concatenated they equal ``torch.cat([tokenizer.decode([(gen_i, None)]) for gen_i in gens],
         -1)`` (each sentence decoded from a fresh codec state), and with sample_rate the tokenizer.resample of that
         concatenation.  Afterwards ``.results`` is what inference_long_tts returns, ``.logprobs`` its lp per sentence,
         and the device generator is left where inference_long_tts leaves it.  best_of = 1 only: the kept copy of a
         best-of-N sentence is known only when its group ends."""
-        cb, chain, gen = self._long_ticket(xs, y, 1, top_k, top_p, temperature, stop_repetition, silence_tokens)
+        cb, chain, gen = self._long_ticket(xs, y, 1, top_k, top_p, temperature, stop_repetition, silence_tokens,
+                                           ras_window, ras_tau, min_frames, max_frames)
         return LongTtsStream(cb, chain, gen, tokenizer, chunk_frames, sample_rate)
 
 
@@ -701,10 +780,11 @@ def _check_capacity(status):
 class _Prompt:
     """One utterance's prompt, held on the model's device: the TTS layout (the prompt delayed by the codebook pattern,
     reference voicecraft.py:961-967) or, given `spans`, the speech-editing layout (VoiceCraft._edit_prompt).  `need_seq`
-    bounds the engine positions its generation can reach.  Raises ValueError on more than 8 spans; the caller checks the
-    id ranges (VoiceCraft._check_ids) before it takes a slot."""
+    bounds the engine positions its generation can reach, with max_frames > 0 (vcb_sampling.max_frames) that bound's.
+    Raises ValueError on more than 8 spans; the caller checks the id ranges (VoiceCraft._check_ids) before it takes a
+    slot."""
 
-    def __init__(self, model, x, y, spans=None):
+    def __init__(self, model, x, y, spans=None, max_frames=0):
         a = model.args
         K, dev = a.n_codebooks, model.mask_embedding.device
         self.model, self.spans = model, spans
@@ -726,7 +806,12 @@ class _Prompt:
                 raise ValueError(f"{len(spans)} masked spans: at most min(8, max_n_spans={a.max_n_spans}) per utterance")
             self.y_tok, self.mask_rows, self.more_vals, self.non_mask = model._edit_prompt(self.y0, spans)
             cap, extra = x_len * 10, (K + 3) * (len(spans) + 1)
-        self.need_seq = x_len + max(int(self.y_tok.shape[0]), cap + 1) + extra + 8
+        rows = int(self.y_tok.shape[0])
+        if max_frames > 0:
+            # the forced end token comes at max_frames steps of a generation: the TTS output or, for an edit, each span,
+            # whose K - 1 closing steps and hand-over columns `extra` already counts.  The reference's cap still holds.
+            cap = min(cap, rows + max_frames * (1 if spans is None else len(spans)))
+        self.need_seq = x_len + max(rows, cap + 1) + extra + 8
         self.total = x_len + int(self.y_tok.shape[0])           # positions the prefill writes
 
     def pages(self, n_copies, max_pages):
@@ -1171,11 +1256,12 @@ class DecodeSession:
             raise ValueError("seeds: one per utterance")
         if noise_fns is not None and len(noise_fns) != self.B:
             raise ValueError("noise_fns: one per utterance")
+        _no_host_noise_under_ras(sp.ras_window, noise_fns is not None or model.noise_fn is not None)
         self.prompts = []
         for i, (x, y) in enumerate(zip(xs, ys)):
             assert x.ndim == 2 and y.ndim == 3 and y.shape[2] == K
             spans = [(int(s), int(e)) for s, e in mask_intervals[i][0].tolist()] if self.edit else None
-            self.prompts.append(_Prompt(model, x, y, spans))
+            self.prompts.append(_Prompt(model, x, y, spans, sp.max_frames))
         # one range check for the whole batch (the reference's embedding lookups raise on a bad id)
         model._check_ids(torch.cat([p.x_ids for p in self.prompts]), torch.cat([p.y_tok.reshape(-1) for p in self.prompts]))
         self.eng, self.slots = model._take_slots(self.B * self.n_copies, max(p.need_seq for p in self.prompts))
@@ -1573,11 +1659,15 @@ class ContinuousBatcher:
     """
 
     def __init__(self, model: "VoiceCraft", max_concurrency=32, poll_every=8, top_k=-100, top_p=1.0, temperature=1.0,
-                 stop_repetition=3, silence_tokens=(1388, 1898, 131), tokenizer=None):
+                 stop_repetition=3, silence_tokens=(1388, 1898, 131), tokenizer=None, ras_window=0, ras_tau=0.1,
+                 min_frames=0, max_frames=None):
+        """ras_window, ras_tau, min_frames, max_frames: the tickets' default sampling controls (sampling_controls)"""
+        sampling_controls(ras_window, ras_tau, min_frames, max_frames)
         self.model, self.B, self.poll_every = model, int(max_concurrency), max(1, int(poll_every))
         self.tokenizer = tokenizer         # encodes the prompt audio of submit(audio=...) tickets
         self.defaults = dict(top_k=top_k, top_p=top_p, temperature=temperature, stop_repetition=stop_repetition,
-                             silence_tokens=silence_tokens)
+                             silence_tokens=silence_tokens, ras_window=ras_window, ras_tau=ras_tau, min_frames=min_frames,
+                             max_frames=max_frames)
         self.queue = []
         self.stats = dict(steps=0, prefills=0, max_active=0, swap_outs=0, swap_ins=0)
         self.results, self.errors = [], {}
@@ -1585,7 +1675,8 @@ class ContinuousBatcher:
         self._live = None                  # the running stream()'s state
 
     def submit(self, x, y=None, seed=None, best_of=1, mask_interval=None, top_k=None, top_p=None, temperature=None,
-               stop_repetition=None, silence_tokens=None, audio=None, sample_rate=None):
+               stop_repetition=None, silence_tokens=None, audio=None, sample_rate=None, ras_window=None, ras_tau=None,
+               min_frames=None, max_frames=None):
         """x [1,L] int64, y [1,T,K] int64 (host or device).  Returns the ticket (index into run()'s result list / results).
         audio [channels, N] (instead of y): the prompt as audio at sample_rate (default: the codec's), encoded by the
         constructor's tokenizer when the ticket is admitted, together with the other audio tickets admitted with it
@@ -1597,8 +1688,10 @@ class ContinuousBatcher:
         max_concurrency.  stream() serves only best_of = 1.
         mask_interval [1,M,2]: a speech-editing ticket (best_of = 1, at most min(8, max_n_spans) spans); its result is
         (res, None) with res what ``inference(x, ., y, mask_interval, ...)`` returns.
-        top_k, top_p, temperature, stop_repetition, silence_tokens: this ticket's sampling parameters; None takes the
-        constructor's value (not inference's or inference_tts' own defaults).
+        top_k, top_p, temperature, stop_repetition, silence_tokens, ras_window, ras_tau, min_frames, max_frames: this
+        ticket's sampling parameters (sampling_controls for the last four); None takes the constructor's value (not
+        inference's or inference_tts' own defaults).  A ticket with max_frames needs, and is admitted against, the
+        positions and KV pages that bound lets it reach.
         While a stream() runs, the utterance is admitted at one of its next polls; one that does not fit the engine it
         sized raises VcbError and is not queued.
 
@@ -1647,11 +1740,13 @@ class ContinuousBatcher:
             if len(spans) > min(8, int(self.model.args.max_n_spans)):
                 raise ValueError(f"{len(spans)} masked spans: at most min(8, max_n_spans={self.model.args.max_n_spans})")
         given = dict(top_k=top_k, top_p=top_p, temperature=temperature, stop_repetition=stop_repetition,
-                     silence_tokens=silence_tokens)
+                     silence_tokens=silence_tokens, ras_window=ras_window, ras_tau=ras_tau, min_frames=min_frames,
+                     max_frames=max_frames)
         params = {k: self.defaults[k] if v is None else v for k, v in given.items()}
         if not (math.isfinite(params["temperature"]) and params["temperature"] > 0) or math.isnan(params["top_p"]):
             raise ValueError(f"temperature must be finite and > 0 and top_p a number, got {params}")
         sp = self.model._sampling(**params)
+        _no_host_noise_under_ras(sp.ras_window, self.model.noise_fn is not None)
         st = self._live
         if st is not None:
             _no_stream_best_of(best_of)
@@ -1683,10 +1778,10 @@ class ContinuousBatcher:
         """the _Ticket of submit's arguments; raises IndexError on an out-of-range id.  A long ticket's chain (x, a
         _Chain) gets the prompts of its sentences."""
         if not isinstance(x, _Chain):
-            p = _Prompt(self.model, x, y, spans)
+            p = _Prompt(self.model, x, y, spans, sp.max_frames)
             self.model._check_ids(p.x_ids, p.y_tok)
             return _Ticket(p, seed, best_of, sp, pending)
-        x.start([_Prompt(self.model, xi, y) for xi in x.xs])
+        x.start([_Prompt(self.model, xi, y, None, sp.max_frames) for xi in x.xs])
         self.model._check_ids(torch.cat([p.x_ids for p in x.prompts]), x.prompts[0].y_tok)
         return _Ticket(x.prompt, seed, best_of, sp, pending, x)
 
@@ -1813,9 +1908,9 @@ class ContinuousBatcher:
         for j, c in zip(todo, codes):
             y = c.transpose(1, 2)
             if j.chain is None:
-                real = _Prompt(self.model, j.pending[0], y, j.prompt.spans)
+                real = _Prompt(self.model, j.pending[0], y, j.prompt.spans, j.sp.max_frames)
             else:                                # every sentence of a long ticket: one encode for the chain
-                j.chain.start([_Prompt(self.model, xi, y) for xi in j.chain.xs])
+                j.chain.start([_Prompt(self.model, xi, y, None, j.sp.max_frames) for xi in j.chain.xs])
                 real = j.chain.prompt
             assert real.need_seq == j.prompt.need_seq and real.total == j.prompt.total
             j.prompt, j.pending = real, None
