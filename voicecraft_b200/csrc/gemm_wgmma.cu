@@ -492,12 +492,27 @@ gemm_w_xT_cluster(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             const int nrows = min(min(4, R - rr0), nvalid - row0);
             if (nrows <= 0) break;
             float sum[4], xnew[4] = {0.f, 0.f, 0.f, 0.f};
+            // the S partials of rows rr0 .. rr0 + 3, summed in writer order.  With R >= 4 the four rows are one 16-byte
+            // word per writer (R and rr0 are multiples of 4): one conflict-free vector load instead of four loads at a
+            // stride of R words, which conflict 4- to 16-way.  Rows past nrows were sent too; they stay 0 as before.
+            float part[4] = {0.f, 0.f, 0.f, 0.f};
+            if (R >= 4) {
+                for (int zz = 0; zz < S; ++zz) {
+                    const float4 v = *reinterpret_cast<const float4*>(red + (zz * GEMM_BM + ml) * R + rr0);
+                    part[0] += v.x;
+                    part[1] += v.y;
+                    part[2] += v.z;
+                    part[3] += v.w;
+                }
+            } else {
+#pragma unroll
+                for (int u = 0; u < 4; ++u)
+                    if (u < nrows)
+                        for (int zz = 0; zz < S; ++zz) part[u] += red[(zz * GEMM_BM + ml) * R + rr0 + u];
+            }
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
-                float a = 0.f;
-                if (u < nrows) {
-                    for (int zz = 0; zz < S; ++zz) a += red[(zz * GEMM_BM + ml) * R + rr0 + u];
-                }
+                float a = u < nrows ? part[u] : 0.f;
                 if constexpr (W8) a *= w_scale;             // exact: a power of two
                 if (ep.ln_fold) {
                     float mean, rstd;
