@@ -56,6 +56,8 @@ enum { VCB_W_BF16 = 0, VCB_W_INT8 = 1 };
 enum { VCB_ERR_KV_FULL = -3 };
 /* pages a one-copy utterance's page list grows by (64 positions each) */
 enum { VCB_KV_GROW_PAGES = 4 };
+/* largest vcb_config.align_text_cap, and the largest X of vcb_align_monotonic */
+enum { VCB_ALIGN_MAX_TEXT = 4096 };
 
 typedef struct vcb_snapshot vcb_snapshot;
 
@@ -74,6 +76,13 @@ typedef struct {
     int32_t device;         /* CUDA device ordinal */
     int32_t weight_dtype;   /* VCB_W_BF16 (default) or VCB_W_INT8 (d_model and audio_vocab_size / 2 multiples of 128);
                              * vcb_create rejects any other value */
+    int32_t align_text_cap; /* alignment (DESIGN.md section 4.6): text tokens an alignment row holds, in [0, VCB_ALIGN_MAX_TEXT];
+                             * 0 = alignment unavailable.  The alignment log [max_slots][max_seq_len][align_text_cap] fp32 is
+                             * allocated by the first prefill that asks for alignment (vcb_counter "align_bytes").  It sits in
+                             * what was the padding before kv_pool_bytes: the struct's size and kv_pool_bytes' offset are
+                             * unchanged, and a zero-initialised config leaves alignment off.  A caller built against
+                             * the older header that fills the struct field by field without zeroing it first must now
+                             * set this field (0), or vcb_create may reject or misread the padding's old bytes */
     int64_t kv_pool_bytes;  /* KV page pool: 0 = max_slots * ceil(max_seq_len / 64) pages (every slot can reach max_seq_len);
                              * > 0: floor(kv_pool_bytes / page bytes) pages, a page being 64 positions of K and V in every
                              * layer (vcb_counter "kv_page_bytes"); vcb_create rejects a negative value or one below a page */
@@ -134,6 +143,12 @@ typedef struct {
      * finite and > 0, a NaN top_p, sampling controls outside the ranges vcb_sampling states, ras_window > 0 with
      * rng_threads == 0. */
     const vcb_sampling* sampling;
+    /* Alignment (DESIGN.md section 4.6): host array [num_layers] of head bitmasks, or NULL (off).  Each audio row of the
+     * group's copies -- the prompt's in vcb_prefill, each step's in vcb_decode_step -- records at its position the mean over
+     * the selected (layer, head) pairs of that head's attention weights on the x_len text keys (vcb_read_alignment).  The
+     * probe only reads: tokens, log-probabilities, logits and KV bytes are those of a run without it.  Rejected with the
+     * prompt: a bit >= nhead, no bit set, x_len > vcb_config.align_text_cap, VCB_MODE_EDIT. */
+    const uint32_t* align_heads;
 } vcb_prompt;
 
 /* Source of an edit slot's output frames for vcb_poll_frames_ex: the original codes y0 [K][T] int64 on the device, as the
@@ -200,6 +215,17 @@ int vcb_read_tokens(vcb_engine* e, int32_t slot, int32_t* out_host, int32_t max_
  * tokens (the first steps' empty tokens, the end-token cascade, a forced end token) get the log-probability of the token
  * written.  Edit hand-over steps write no row.  Computed by the sampler in fp32 (DESIGN.md section 2.2). */
 int vcb_read_logprobs(vcb_engine* e, int32_t slot, float* out_host, int32_t max_steps, void* stream);
+/* waits for `stream`, then copies the alignment rows of positions first_pos .. first_pos+n_pos-1 of a slot prefilled with
+ * align_heads to host memory: out_host [n_pos][x_len] fp32, x_len the slot's.  Row p holds what the probe recorded for the
+ * row at position p (its attention weights on the text keys, averaged over the selected heads); rows of positions the slot
+ * has not written, and text positions (< x_len), are unspecified.  Rejected: a slot that is not open or has no alignment,
+ * first_pos < 0, n_pos < 1, first_pos + n_pos > max_seq_len. */
+int vcb_read_alignment(vcb_engine* e, int32_t slot, float* out_host, int32_t first_pos, int32_t n_pos, void* stream);
+/* Monotonic alignment search (Glow-TTS) on the device, one CTA: logp_dev [T][X] fp32 -> durations_dev [X] int32 summing to T,
+ * the path from (0, 0) to (T-1, X-1) that assigns each frame one token, never goes back, and gives every token a frame,
+ * maximising the fp32 sum of logp along it (accumulated frame by frame).  Ties stay on the current token.  Asynchronous on
+ * `stream` (a stream-ordered scratch of T * X bytes).  Rejected: T < X, X < 1, X > VCB_ALIGN_MAX_TEXT, null pointers. */
+int vcb_align_monotonic(const float* logp_dev, int32_t T, int32_t X, int32_t* durations_dev, void* stream);
 /* closes slots slot .. slot+n_copies-1 (slots that are not open are skipped); a KV page goes back to the free list when
  * the last slot holding it is released, and a group's id with its last slot, in any release order */
 int vcb_release(vcb_engine* e, int32_t slot, int32_t n_copies);
@@ -327,6 +353,14 @@ int vcb_debug_mega_attention(const float* q_dev /*[rows][H][128]*/, const float*
                              const int32_t* row_pages_dev /*[rows][max_pages]*/, const int32_t* pos_dev, int32_t rows,
                              int32_t H, int32_t max_pages, const int32_t* grids, int32_t launches,
                              float* out_dev /*[rows][H*128]*/);
+/* the alignment probe of vcb_prompt.align_heads alone, one layer: for each row r with pos[r] >= x_len, out[r][j] (j < x_len)
+ * = mean over the heads h of head_mask of softmax_j(q[r][h] . k_j / sqrt(hd)) over the keys 0..pos[r] of row r's pages
+ * (row_pages[r][*], max_pages wide; pools as vcb_debug_attention's).  Rows with pos[r] < x_len are left untouched.
+ * Rejected: H outside [1, 32], hd not 64 / 128, an empty mask or one with a bit >= H, x_len outside [1, VCB_ALIGN_MAX_TEXT].
+ * Synchronous. */
+int vcb_debug_align_probe(const float* q_dev /*[rows][H][hd]*/, const void* kpool_dev, int32_t kv_dtype,
+                          const int32_t* row_pages_dev, const int32_t* pos_dev, int32_t rows, int32_t H, int32_t hd,
+                          int32_t max_pages, uint32_t head_mask, int32_t x_len, float* out_dev /*[rows][x_len]*/);
 /* the fp8 KV quantizer of the QKV epilogues on `rows` rows of hd fp32 values (hd 64 or 128): out gets the e4m3 bytes
  * [rows][hd], then the fp32 scales [rows].  Synchronous. */
 int vcb_debug_kv_quantize(const float* x_dev /*[rows][hd]*/, int32_t rows, int32_t hd, uint8_t* out_dev);
@@ -385,7 +419,7 @@ int vcb_set_option(vcb_engine* e, const char* name, int32_t value);
  * (0 gemm, 1 attention, 2 layernorm/reduce, 3 bias/act/qkv finish, 4 sampler, 5 misc) */
 int vcb_profile_read(vcb_engine* e, double* ms_by_class, int64_t* count_by_class, int32_t n_classes);
 /* "launches", "kv_bytes", "kv_pages_free", "kv_pages_total" (pool size), "kv_pages_needed" (pages the last refused
- * vcb_decode_step lacked), "kv_page_bytes" (one page: 64 positions of K and V in every layer), "swap_stage_bytes" (device
+ * vcb_decode_step lacked), "kv_page_bytes" (one page: 64 positions of K and V in every layer), "align_bytes" (the alignment log and masks, 0 until a prefill asked for alignment), "swap_stage_bytes" (device
  * staging of the swap kernels), "prefill_rows" (rows through the prefill since create), "wide_rows" (rows per pass of
  * the rows-as-M prefill, fixed by its first use; 0 until a prefill took that path), "weight_bytes" (device
  * bytes of the packed GEMM operands with their int8 scales, and the int8 prefill scratch once a prefill allocated it),

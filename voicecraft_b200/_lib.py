@@ -19,11 +19,12 @@ class vcb_config(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "d_model", "nhead", "num_layers", "n_codebooks", "audio_vocab_size", "n_special", "text_vocab_rows",
         "empty_token", "eog", "audio_pad_token", "eos", "encodec_sr", "max_n_spans", "max_slots", "max_seq_len",
-        "max_new_tokens", "kv_dtype", "device", "weight_dtype")] + [("kv_pool_bytes", C.c_int64)]
+        "max_new_tokens", "kv_dtype", "device", "weight_dtype", "align_text_cap")] + [("kv_pool_bytes", C.c_int64)]
 
 
 VCB_ERR_KV_FULL = -3        # vcb_decode_step: the KV pool cannot cover the listed slots' next positions; nothing was done
 KV_GROW_PAGES = 4           # pages a one-copy utterance's page list grows by (VCB_KV_GROW_PAGES)
+ALIGN_MAX_TEXT = 4096       # largest align_text_cap and vcb_align_monotonic X (VCB_ALIGN_MAX_TEXT)
 
 
 class vcb_sampling(C.Structure):
@@ -37,7 +38,7 @@ class vcb_prompt(C.Structure):
                 ("text_ids_dev", C.c_void_p), ("y_len", C.c_int32), ("y_tokens_dev", C.c_void_p),
                 ("mask_rows_dev", C.c_void_p), ("n_more_spans", C.c_int32), ("more_mask_rows", C.c_int32 * 8),
                 ("rng_seed", C.c_uint64), ("rng_offset", C.c_uint64), ("rng_threads", C.c_int32), ("rng_reserved", C.c_int32),
-                ("sampling", C.POINTER(vcb_sampling))]
+                ("sampling", C.POINTER(vcb_sampling)), ("align_heads", C.POINTER(C.c_uint32))]
 
 
 class vcb_edit_source(C.Structure):
@@ -71,6 +72,10 @@ PROTOTYPES = {
                                      C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_void_p]),
     "vcb_read_tokens": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.c_int32, C.c_void_p]),
     "vcb_read_logprobs": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_float), C.c_int32, C.c_void_p]),
+    "vcb_read_alignment": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_float), C.c_int32, C.c_int32, C.c_void_p]),
+    "vcb_align_monotonic": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
+    "vcb_debug_align_probe": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32,
+                                        C.c_int32, C.c_int32, C.c_uint32, C.c_int32, C.c_void_p]),
     "vcb_release": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "vcb_swap_out": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), C.c_void_p]),
     "vcb_swap_in": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p]),

@@ -138,6 +138,11 @@ struct vcb_engine {
     std::vector<int> slot_shared;     // host mirror: full prompt pages the slot shares with its group (0: none)
     DevBuf<int> tok_log;
     DevBuf<float> lp_log;             // [max_slots][max_new_tokens][K]: log-probability of each token-log entry
+    // alignment (vcb_prompt.align_heads, DESIGN.md section 4.6): allocated by the first prefill that asks for it
+    DevBuf<float> align_log;          // [max_slots][max_seq_len][align_text_cap]
+    DevBuf<uint32_t> align_masks;     // [max_slots][L] head bitmasks of each slot's prompt (0: off)
+    std::vector<uint32_t> slot_align; // host copy of align_masks (what the device holds)
+    std::vector<char> pass_align;     // [L]: the pass being enqueued has a row that probes layer l
     DevBuf<float> dbg_logits;
     DevBuf<SlotState> st;
     DevBuf<GroupState> gr;
@@ -232,6 +237,8 @@ struct vcb_snapshot {
     PinnedBuf<int> tok;               // token-log rows [0, n_steps) x K
     PinnedBuf<float> lp;              // log-probability rows [0, n_steps) x K
     PinnedBuf<float> rows;            // x_slot row (next input), h_slot row (last prefill hidden state)
+    std::vector<uint32_t> align;      // the slot's alignment head masks [L] (empty: alignment off)
+    PinnedBuf<float> align_rows;      // its alignment-log rows [0, seq_len) x align_text_cap
 };
 
 enum { PC_GEMM = 0, PC_ATTN = 1, PC_LN = 2, PC_FINISH = 3, PC_SAMPLER = 4, PC_MISC = 5, PC_MEGA = 6, PC_N = 7 };
@@ -474,6 +481,7 @@ struct Pass {
     float* att_ws = nullptr;
     int* att_cnt = nullptr;
     int stop = 0;                             // stages to run (vcb_engine::opt_stop; 0: all)
+    bool align = false;                       // some row probes a layer (vcb_engine::pass_align)
 };
 
 // the pass has run its last stage once `n` stages have run
@@ -703,6 +711,49 @@ int launch_attn(vcb_engine* e, const Pass& p, const Layer& Ly, cudaStream_t st) 
     return 0;
 }
 
+// The alignment probe of layer l over the pass's rows (align.cu), after that layer's attention and before the next
+// layer's QKV GEMM rewrites p.q.  Launched without PDL, so it starts once attention has finished.
+int launch_align(vcb_engine* e, const Pass& p, int l, cudaStream_t st) {
+    const ModelDims& m = e->m;
+    AlignProbeArgs a;
+    a.q = p.q;
+    a.q_ld = m.d;
+    a.kpool = e->layers[l].kpool;
+    a.kv_dtype = e->kv_dtype;
+    a.page_table = e->page_table;
+    a.row_slot = p.slot;
+    a.row_pos = p.pos;
+    a.row_pages = p.pages;
+    a.max_pages = e->max_pages_per_slot;
+    a.rows = p.rows;
+    a.H = m.H;
+    a.hd = m.hd;
+    a.L = m.L;
+    a.layer = l;
+    a.masks = e->align_masks;
+    a.slot_xlen = &e->st.get()->x_len;
+    a.xlen_stride = sizeof(SlotState) / sizeof(int);
+    a.cap = e->cfg.align_text_cap;
+    a.max_seq = e->cfg.max_seq_len;
+    a.scale = 1.0f / sqrtf(static_cast<float>(m.hd));
+    a.log = e->align_log;
+    ProfScope ps(e, PC_MISC, st);
+    if (align_probe_launch(a, st)) return -1;
+    LAUNCH_COUNT(e);
+    return 0;
+}
+
+// pass_align for the rows of `slots` (the slots whose rows the pass runs); true when any layer is probed
+bool plan_align(vcb_engine* e, const int* slots, int n) {
+    e->pass_align.assign(e->m.L, 0);
+    if (e->slot_align.empty()) return false;
+    bool any = false;
+    for (int i = 0; i < n; ++i)
+        for (int l = 0; l < e->m.L; ++l)
+            if (e->slot_align[static_cast<size_t>(slots[i]) * e->m.L + l]) any = e->pass_align[l] = 1;
+    return any;
+}
+
 // LayerNorm of the pass's residual rows (p.x, through p.x_index) into the hi/lo rows of p.act_d
 int launch_ln(vcb_engine* e, const Pass& p, const float* g, const float* b, cudaStream_t st) {
     const int d = e->m.d;
@@ -730,6 +781,7 @@ int forward_layers(vcb_engine* e, const Pass& p, cudaStream_t st) {
         if (pass_gemm(e, p, Ly.qkv, p.act_d, ep.qkv, st, &Ly.out)) return -1;
         if (stops_after(p, s + 1)) return 0;
         if (launch_attn(e, p, Ly, st)) return -1;
+        if (p.align && e->pass_align[l] && launch_align(e, p, l, st)) return -1;
         if (stops_after(p, s + 2)) return 0;
         if (pass_gemm(e, p, Ly.out, p.act_d, ep.out, st, &Ly.ff1)) return -1;
         if (stops_after(p, s + 3)) return 0;
@@ -1290,6 +1342,10 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
                   cfg->audio_vocab_size);
         return -1;
     }
+    if (cfg->align_text_cap < 0 || cfg->align_text_cap > VCB_ALIGN_MAX_TEXT) {
+        set_error("align_text_cap %d: in [0, %d]", cfg->align_text_cap, VCB_ALIGN_MAX_TEXT);
+        return -1;
+    }
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         set_error("no CUDA device: libvcb200 has no CPU fallback");
@@ -1568,6 +1624,9 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
     std::vector<int> gst_id;
     std::vector<std::pair<int, SamplingParams>> gsp;   // (group id, parameters) of the groups prefilled with their own
     std::vector<ForkPair> fork;
+    std::vector<std::array<int, 3>> align_fork;        // (leader, member, prompt positions) of the aligning groups
+    std::vector<int> align_set;                         // slots whose align_masks row this prefill rewrites
+    bool aligning = false;
     // ---- validate everything before touching host or device state (a failed call must leave no slot, group or page held)
     {
         size_t rows_needed = 0, pages_needed = 0;
@@ -1598,6 +1657,20 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
                     return -1;
                 }
             }
+            if (const uint32_t* hm = P.align_heads) {
+                uint32_t any = 0, over = 0;
+                for (int l = 0; l < m.L; ++l) {
+                    any |= hm[l];
+                    if (m.H < 32) over |= hm[l] >> m.H;
+                }
+                if (e->cfg.align_text_cap == 0 || P.mode == VCB_MODE_EDIT || P.x_len > e->cfg.align_text_cap || !any || over) {
+                    set_error("prompt %d: alignment needs align_text_cap > 0 (is %d) and >= x_len (%d), a TTS prompt (mode %d), "
+                              "and head masks with some bit set and none >= nhead (%d)", i, e->cfg.align_text_cap, P.x_len,
+                              P.mode, m.H);
+                    return -1;
+                }
+                aligning = true;
+            }
             for (int c = 0; c < P.n_copies; ++c) {
                 if (e->slot_group[P.slot + c] >= 0 || claimed[P.slot + c]) {
                     set_error("slot %d already open", P.slot + c);
@@ -1626,6 +1699,16 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
         if (static_cast<size_t>(n) > static_cast<size_t>(e->cfg.max_slots)) {
             set_error("too many prompts");
             return -1;
+        }
+        if (aligning && !e->align_log) {
+            const size_t rows = static_cast<size_t>(e->cfg.max_slots) * e->cfg.max_seq_len;
+            if (e->align_log.alloc(rows * e->cfg.align_text_cap, true) ||
+                e->align_masks.alloc(static_cast<size_t>(e->cfg.max_slots) * m.L, true)) {
+                e->align_log.reset();
+                e->align_masks.reset();
+                return -1;
+            }
+            e->slot_align.assign(static_cast<size_t>(e->cfg.max_slots) * m.L, 0);
         }
     }
     for (int i = 0; i < n; ++i) {
@@ -1685,6 +1768,17 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
             if (c > 0) {
                 const bool tail = total % KV_PAGE != 0;
                 fork.push_back({P.slot, slot, tail ? e->slot_pages[P.slot][shared] : -1, tail ? pg[shared] : -1});
+                if (P.align_heads) align_fork.push_back({P.slot, slot, total});
+            }
+            if (!e->slot_align.empty()) {
+                uint32_t* row = &e->slot_align[static_cast<size_t>(slot) * m.L];
+                bool changed = false;
+                for (int l = 0; l < m.L; ++l) {
+                    const uint32_t v = P.align_heads ? P.align_heads[l] : 0u;
+                    changed |= row[l] != v;
+                    row[l] = v;
+                }
+                if (changed) align_set.push_back(slot);
             }
             SlotState S;
             memset(&S, 0, sizeof(S));
@@ -1722,6 +1816,12 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
     VCB_CUDA_OK(cudaMemcpy(e->d_seqs, seqs.data(), seqs.size() * sizeof(EmbedSeq), cudaMemcpyHostToDevice));
     if (!fork.empty())
         VCB_CUDA_OK(cudaMemcpy(e->d_fork, fork.data(), fork.size() * sizeof(ForkPair), cudaMemcpyHostToDevice));
+    for (int slot : align_set)
+        VCB_CUDA_OK(cudaMemcpy(e->align_masks + static_cast<size_t>(slot) * m.L, &e->slot_align[static_cast<size_t>(slot) * m.L],
+                               m.L * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    std::vector<int> leaders(n);
+    for (int i = 0; i < n; ++i) leaders[i] = prompts[i].slot;
+    const bool probe = plan_align(e, leaders.data(), n);
     // ---- chunked prefill: <= 128 rows per pass through the same kernels as a decode step ----------------
     const size_t total_rows = r_seq.size();
     int* t_seq = e->all_rows;
@@ -1749,6 +1849,7 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
         p.last = t_last + off;
         p.page = t_page + off;
         p.stop = off + chunk >= total_rows ? e->opt_stop : 0;      // a stop ends the last chunk
+        p.align = probe;
         embed_rows_kernel<<<rows, 256, 0, st>>>(e->d_seqs, t_seq + off, t_pos + off, p.x, m.d, m.K, e->E_text,
                                                 e->d_E_audio, e->mask_emb, e->pe, e->alpha_t, e->alpha_a);
         VCB_CUDA_OK(cudaGetLastError());
@@ -1774,6 +1875,12 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
                                                 e->h_slot, m.d);
         VCB_CUDA_OK(cudaGetLastError());
         LAUNCH_COUNT(e);
+        // each copy of an aligning group starts from the prompt rows the leader recorded
+        const size_t slot_floats = static_cast<size_t>(e->cfg.max_seq_len) * e->cfg.align_text_cap;
+        for (const auto& f : align_fork)
+            VCB_CUDA_OK(cudaMemcpyAsync(e->align_log + f[1] * slot_floats, e->align_log + f[0] * slot_floats,
+                                        static_cast<size_t>(f[2]) * e->cfg.align_text_cap * sizeof(float),
+                                        cudaMemcpyDeviceToDevice, st));
     }
     return 0;
 }
@@ -1811,7 +1918,8 @@ int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float*
         (sp && check_controls(sp, "sp")))
         return -1;
     const bool fold = e->opt_fold && !e->opt_simt;
-    const bool mega = fold && e->mega_grid > 0 && n <= 32;
+    const bool probe = plan_align(e, slots, n);          // a step with alignment rows runs the per-kernel chain
+    const bool mega = fold && e->mega_grid > 0 && n <= 32 && !probe;
     if (!mega && check_split_overrides(e, bpad_for(n))) return -1;
     static thread_local std::vector<std::pair<int, int>> grow;
     if (const int rc = plan_growth(e, slots, n, grow)) return rc;
@@ -1843,6 +1951,7 @@ int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float*
         return launch_sampler(e, p, exp_noise_dev, sp, sampler_controls(e, slots, n, sp), st);
     }
     record_pass(e, p, 5 * e->m.L + 2, false);
+    p.align = probe;
     if (forward_layers(e, p, st)) return -1;
     return sample_rows(e, p, exp_noise_dev, sp, sampler_controls(e, slots, n, sp), st);
 }
@@ -2050,6 +2159,29 @@ int vcb_read_logprobs(vcb_engine* e, int32_t slot, float* out_host, int32_t max_
     return read_log_rows<float>(e, e->lp_log, slot, out_host, max_steps, stream);
 }
 
+int vcb_read_alignment(vcb_engine* e, int32_t slot, float* out_host, int32_t first_pos, int32_t n_pos, void* stream) {
+    if (!e || !out_host || slot < 0 || slot >= e->cfg.max_slots || e->slot_group[slot] < 0 || e->slot_align.empty() ||
+        first_pos < 0 || n_pos < 1 || static_cast<long long>(first_pos) + n_pos > e->cfg.max_seq_len) {
+        set_error("vcb_read_alignment: slot %d not open, or bad rows [%d, +%d) (max_seq_len %d)", slot, first_pos, n_pos,
+                  e ? e->cfg.max_seq_len : 0);
+        return -1;
+    }
+    const uint32_t* row = &e->slot_align[static_cast<size_t>(slot) * e->m.L];
+    if (std::all_of(row, row + e->m.L, [](uint32_t v) { return v == 0; })) {
+        set_error("vcb_read_alignment: slot %d was prefilled without align_heads", slot);
+        return -1;
+    }
+    VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
+    VCB_CUDA_OK(cudaStreamSynchronize(static_cast<cudaStream_t>(stream)));
+    SlotState S;
+    VCB_CUDA_OK(cudaMemcpy(&S, e->st + slot, sizeof(SlotState), cudaMemcpyDeviceToHost));
+    const size_t cap = e->cfg.align_text_cap;
+    VCB_CUDA_OK(cudaMemcpy2D(out_host, S.x_len * sizeof(float),
+                             e->align_log + (static_cast<size_t>(slot) * e->cfg.max_seq_len + first_pos) * cap,
+                             cap * sizeof(float), S.x_len * sizeof(float), n_pos, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
 int vcb_release(vcb_engine* e, int32_t slot, int32_t n_copies) {
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
     VCB_CUDA_OK(cudaDeviceSynchronize());
@@ -2143,6 +2275,17 @@ int vcb_swap_out(vcb_engine* e, int32_t slot, vcb_snapshot** out, void* stream) 
                                 cudaMemcpyDeviceToHost, st));
     VCB_CUDA_OK(cudaMemcpyAsync(snap->rows + m.d, e->h_slot + static_cast<size_t>(slot) * m.d, m.d * sizeof(float),
                                 cudaMemcpyDeviceToHost, st));
+    if (!e->slot_align.empty()) {
+        const uint32_t* row = &e->slot_align[static_cast<size_t>(slot) * m.L];
+        if (std::any_of(row, row + m.L, [](uint32_t v) { return v != 0; })) {
+            const size_t n = static_cast<size_t>(snap->S.seq_len) * e->cfg.align_text_cap;
+            snap->align.assign(row, row + m.L);
+            if (snap->align_rows.alloc(n)) return -1;
+            VCB_CUDA_OK(cudaMemcpyAsync(snap->align_rows, e->align_log + static_cast<size_t>(slot) * e->cfg.max_seq_len *
+                                                                             e->cfg.align_text_cap,
+                                        n * sizeof(float), cudaMemcpyDeviceToHost, st));
+        }
+    }
     if (sync_or_report(e, cudaStreamSynchronize(st), "vcb_swap_out")) return -1;
     if (vcb_release(e, slot, 1)) return -1;
     *out = snap.release();
@@ -2208,6 +2351,20 @@ int vcb_swap_in(vcb_engine* e, const vcb_snapshot* snap, int32_t slot, void* str
                                 cudaMemcpyHostToDevice, st));
     VCB_CUDA_OK(cudaMemcpyAsync(e->h_slot + static_cast<size_t>(slot) * m.d, snap->rows + m.d, m.d * sizeof(float),
                                 cudaMemcpyHostToDevice, st));
+    // the slot's head masks (a snapshot with alignment comes from an engine whose log exists: this one)
+    if (!e->slot_align.empty()) {
+        uint32_t* row = &e->slot_align[static_cast<size_t>(slot) * m.L];
+        std::vector<uint32_t> want = snap->align.empty() ? std::vector<uint32_t>(m.L, 0u) : snap->align;
+        if (!std::equal(want.begin(), want.end(), row)) {
+            std::copy(want.begin(), want.end(), row);
+            VCB_CUDA_OK(cudaMemcpy(e->align_masks + static_cast<size_t>(slot) * m.L, row, m.L * sizeof(uint32_t),
+                                   cudaMemcpyHostToDevice));
+        }
+        if (!snap->align.empty())
+            VCB_CUDA_OK(cudaMemcpyAsync(e->align_log + static_cast<size_t>(slot) * e->cfg.max_seq_len * e->cfg.align_text_cap,
+                                        snap->align_rows, static_cast<size_t>(snap->S.seq_len) * e->cfg.align_text_cap *
+                                        sizeof(float), cudaMemcpyHostToDevice, st));
+    }
     return sync_or_report(e, cudaStreamSynchronize(st), "vcb_swap_in");
 }
 
@@ -2914,6 +3071,8 @@ int64_t vcb_counter(vcb_engine* e, const char* name) {
     if (!strcmp(name, "kv_pages_needed")) return e->n_pages_needed;
     if (!strcmp(name, "kv_page_bytes")) return static_cast<int64_t>(page_bytes_all_layers(e));
     if (!strcmp(name, "swap_stage_bytes")) return static_cast<int64_t>(e->swap_stage.size() * sizeof(uint4));
+    if (!strcmp(name, "align_bytes"))            // the alignment log and its head masks (0 until a prefill asked for it)
+        return static_cast<int64_t>(e->align_log.size() * sizeof(float) + e->align_masks.size() * sizeof(uint32_t));
     if (!strcmp(name, "prefill_rows")) return e->n_prefill_rows;
     if (!strcmp(name, "wide_rows")) return e->wide_rows;
     if (!strcmp(name, "weight_bytes")) {         // packed GEMM operands (+ int8 scales) and the int8 prefill scratch

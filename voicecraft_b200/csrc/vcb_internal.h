@@ -168,6 +168,31 @@ __device__ __forceinline__ float2 kv_fp8_unpack2(uint32_t v) {
 }
 
 // ---------------------------------------------------------------------------------------------------
+// Alignment probe (align.cu): for each row r with pos = row_pos[r] >= x_len of its slot and mask = masks[slot][layer] != 0,
+// the softmax of scale * q[r][h] . k_j over keys j <= pos (pages through row_pages[r] or page_table[slot]) for each head h
+// of mask, summed over those heads at keys j < x_len.  With `log`, the sum goes to log[slot][pos][0 .. x_len) -- added to
+// what the slot's earlier selected layers left there, and divided by the slot's selected heads in its last one -- else to
+// out[r][0 .. x_len) (one layer, L = 1).  Rows with pos < 0, no mask or pos < x_len are skipped.
+// ---------------------------------------------------------------------------------------------------
+struct AlignProbeArgs {
+    const float* q = nullptr;             // [rows][q_ld]: head h at h * hd
+    int q_ld = 0;
+    const void* kpool = nullptr;
+    int kv_dtype = KV_BF16;
+    const int *page_table = nullptr, *row_slot = nullptr, *row_pos = nullptr, *row_pages = nullptr;
+    int max_pages = 0, rows = 0, H = 0, hd = 0, L = 1, layer = 0;
+    const uint32_t* masks = nullptr;      // [slots][L]
+    const int* slot_xlen = nullptr;       // x_len of slot s at slot_xlen[s * xlen_stride]
+    int xlen_stride = 1;
+    int cap = 0;                          // log row width; x_len is clamped to it
+    int max_seq = 0;                      // log rows per slot
+    float scale = 0.f;
+    float* log = nullptr;                 // [slots][max_seq][cap]
+    float* out = nullptr;                 // [rows][cap] (log == null)
+};
+int align_probe_launch(const AlignProbeArgs& a, cudaStream_t st);
+
+// ---------------------------------------------------------------------------------------------------
 // GEMM (gemm_wgmma.cu)
 // ---------------------------------------------------------------------------------------------------
 enum { EPI_QKV = 0, EPI_RESID = 1, EPI_ACT = 2, EPI_LOGITS = 3 };

@@ -37,6 +37,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from .alignment import Alignment, head_masks
 from .codebooks_patterns import DelayedPatternProvider
 
 try:  # same mixin as the reference (voicecraft.py:23, 89-95); optional so the hot path has no hard dependency
@@ -206,7 +207,7 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         self._eng = None
         self._eng_key = None
         self._eng_opts = dict(max_slots=8, max_seq_len=2048, max_new_tokens=4096, kv_dtype="bf16", weight_dtype="bf16",
-                              kv_pool_gb=None)
+                              kv_pool_gb=None, align_text_cap=0)
         self.noise_fn = None          # optional: callable(shape, device) -> fp32 Exp(1) tensor on `device`
         self.poll_every = 4           # inference_tts*: poll the done flag every N steps (device generator only)
         self._sessions = {}           # first slot -> slot list of every group held by a call, session or batcher (the engine
@@ -233,7 +234,8 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         GEMM weights as int8 with a power-of-two scale per output feature, half the weight bytes; INTEGRATION.md),
         kv_pool_gb (None default: every slot can reach max_seq_len; a number: a KV page pool of that many GB (1e9 bytes),
         taken as utterances grow; the batcher and sessions swap utterances to host memory when it runs out;
-        INTEGRATION.md).
+        INTEGRATION.md), align_text_cap (0 default: no alignment; n: calls may ask for alignment= of texts up to n tokens,
+        and the first one allocates a log of max_slots * max_seq_len * n fp32; INTEGRATION.md).
         Rebuilds lazily."""
         for k in opts:
             if k not in self._eng_opts:
@@ -244,6 +246,9 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
             raise ValueError(f"weight_dtype {opts['weight_dtype']!r}: one of {sorted(WEIGHT_DTYPES)}")
         if opts.get("kv_pool_gb") is not None and not opts["kv_pool_gb"] > 0:
             raise ValueError(f"kv_pool_gb {opts['kv_pool_gb']!r}: None or a positive number of GB")
+        cap = opts.get("align_text_cap", 0)
+        if not isinstance(cap, (int, np.integer)) or not 0 <= cap <= _lib.ALIGN_MAX_TEXT:
+            raise ValueError(f"align_text_cap {cap!r}: an int in [0, {_lib.ALIGN_MAX_TEXT}]")
         self._eng_opts.update(opts)
         self._drop_engine()
 
@@ -331,7 +336,7 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
             encodec_sr=int(a.encodec_sr), max_n_spans=a.max_n_spans, max_slots=o["max_slots"],
             max_seq_len=o["max_seq_len"], max_new_tokens=o["max_new_tokens"],
             kv_dtype=KV_DTYPES[o["kv_dtype"]], device=dev.index or 0, weight_dtype=WEIGHT_DTYPES[o["weight_dtype"]],
-            kv_pool_bytes=0 if o["kv_pool_gb"] is None else int(o["kv_pool_gb"] * 1e9))
+            kv_pool_bytes=0 if o["kv_pool_gb"] is None else int(o["kv_pool_gb"] * 1e9), align_text_cap=int(o["align_text_cap"]))
         h = C.c_void_p()
         _lib.check(lib.vcb_create(C.byref(cfg), C.byref(h)))
         try:
@@ -423,34 +428,36 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
                       top_p: float = 1.0, temperature: float = 1.0, stop_repetition: int = 3, kvcache: int = 1,
                       silence_tokens: List[int] = [1388, 1898, 131], *kargs, logprobs: bool = False,
                       ras_window: int = 0, ras_tau: float = 0.1, min_frames: int = 0,
-                      max_frames: Optional[int] = None):
+                      max_frames: Optional[int] = None, alignment=None):
         """logprobs=True: returns (res, gen, lp), lp [1,K,G] fp32 the log-probability of each frame of gen under the
         model's raw distribution (vcb_read_logprobs).  ras_window, ras_tau, min_frames, max_frames: see
-        sampling_controls"""
+        sampling_controls.  alignment (None: off; True: every head of every layer, L * H probes per row; {layer: [heads]}):
+        the result also ends with an Alignment of res (voicecraft_b200/alignment.py); needs
+        configure_engine(align_text_cap >= the text's tokens).  Tokens are those of a call without it."""
         sp = self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens, ras_window, ras_tau, min_frames,
                             max_frames)
-        return self._tts_impl(x, x_lens, y, sp, silence_tokens, 1, logprobs)
+        return self._tts_impl(x, x_lens, y, sp, silence_tokens, 1, logprobs, alignment)
 
     @torch.no_grad()
     def inference_tts_batch(self, x: torch.Tensor, x_lens: torch.Tensor, y: torch.Tensor, top_k: int = -100,
                             top_p: float = 1.0, temperature: float = 1.0, stop_repetition: int = 3, kvcache: int = 1,
                             batch_size: int = 5, silence_tokens: List[int] = [1388, 1898, 131], *kargs,
                             logprobs: bool = False, ras_window: int = 0, ras_tau: float = 0.1, min_frames: int = 0,
-                            max_frames: Optional[int] = None):
+                            max_frames: Optional[int] = None, alignment=None):
         """Best-of-N: the first sample to end wins (reference voicecraft.py:1156-1439).  logprobs=True: returns
-        (res, gen, lp) as inference_tts does, lp the kept copy's."""
+        (res, gen, lp) as inference_tts does, lp the kept copy's; alignment: likewise, the kept copy's Alignment."""
         sp = self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens, ras_window, ras_tau, min_frames,
                             max_frames)
-        return self._tts_impl(x, x_lens, y, sp, silence_tokens, batch_size, logprobs)
+        return self._tts_impl(x, x_lens, y, sp, silence_tokens, batch_size, logprobs, alignment)
 
-    def _tts_impl(self, x, x_lens, y, sp, silence_tokens, n_copies, logprobs):
+    def _tts_impl(self, x, x_lens, y, sp, silence_tokens, n_copies, logprobs, alignment=None):
         assert x.ndim == 2, x.shape
         assert x_lens.ndim == 1, x_lens.shape
         assert y.ndim == 3, y.shape
         assert y.shape[0] == 1 and y.shape[2] == self.args.n_codebooks, y.transpose(2, 1).shape
         logging.info(f"silence tokens: {silence_tokens}, note that if you are not using the pretrained encodec "
                      f"6f79c6a8, make sure you specified it yourself, rather than using the default")
-        sess = DecodeSession(self, [x], [y], sp, n_copies=n_copies)
+        sess = DecodeSession(self, [x], [y], sp, n_copies=n_copies, alignment=alignment)
         try:
             out, = sess._run_single(logprobs)
         finally:
@@ -565,7 +572,7 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
 
     def open_tts_session(self, xs, ys, top_k=-100, top_p=1.0, temperature=1.0, stop_repetition=3,
                          silence_tokens=(1388, 1898, 131), seeds=None, noise_fns=None, best_of=1, ras_window=0,
-                         ras_tau=0.1, min_frames=0, max_frames=None):
+                         ras_tau=0.1, min_frames=0, max_frames=None, alignment=None):
         """xs: list of [1,L] int64, ys: list of [1,T,K] int64 (any device).  Prefills every utterance (one packed,
         chunked pass) and returns a DecodeSession whose .step() runs one decode step for all of them.
 
@@ -577,15 +584,17 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
         best_of: each utterance is sampled best_of times and keeps the copy that ends first, what
         ``inference_tts_batch(x_i, ., y_i, batch_size=best_of)`` returns under the same seed.  The copies share one
         prefill and the KV pages of the prompt's full pages.
-        ras_window, ras_tau, min_frames, max_frames: see sampling_controls."""
+        ras_window, ras_tau, min_frames, max_frames: see sampling_controls.
+        alignment: as inference_tts's, for every utterance; results() then ends each tuple with its Alignment."""
         return DecodeSession(self, xs, ys, self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens,
                                                           ras_window, ras_tau, min_frames, max_frames),
-                             seeds=seeds, noise_fns=noise_fns, best_of=best_of)
+                             seeds=seeds, noise_fns=noise_fns, best_of=best_of, alignment=alignment)
 
     @torch.no_grad()
     def inference_tts_many(self, xs, ys, poll_every: int = 8, logprobs: bool = False, **kw):
         """Returns a list of (res [1,K,T+G], gen [1,K,G]) like inference_tts (inference_tts_batch with best_of > 1), one
-        per utterance; logprobs=True: (res, gen, lp) as inference_tts(..., logprobs=True) returns them."""
+        per utterance; logprobs=True: (res, gen, lp) as inference_tts(..., logprobs=True) returns them; alignment= (see
+        open_tts_session): each tuple ends with the utterance's Alignment."""
         return self.open_tts_session(xs, ys, **kw)._run_many(poll_every, logprobs)
 
     # ------------------------------------------------------------------------------------------------
@@ -597,7 +606,8 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
                                   sample_rate: int = None, **kw):
         """inference_tts_many with the audio handed out while it is generated: iterates (i, wav [1, channels, n*hop]),
         utterance i's chunks in order; concatenated they equal ``tokenizer.decode_codes(gen_i)``.  Afterwards
-        ``.results`` equals what inference_tts_many returns.  `seeds` as in open_tts_session."""
+        ``.results`` equals what inference_tts_many returns.  `seeds` and alignment= as in open_tts_session; with
+        alignment, ``.alignments`` holds utterance i's Alignment."""
         _no_stream_best_of(kw.get("best_of", 1))
         sess = self.open_tts_session(xs, ys, seeds=seeds, **kw)
         return TtsStream(sess, tokenizer, chunk_frames, poll_every, sample_rate)
@@ -606,15 +616,15 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
                              poll_every: int = 8, top_k: int = -100, top_p: float = 1.0, temperature: float = 1.0,
                              stop_repetition: int = 3, silence_tokens: List[int] = [1388, 1898, 131],
                              sample_rate: int = None, ras_window: int = 0, ras_tau: float = 0.1, min_frames: int = 0,
-                             max_frames: Optional[int] = None):
+                             max_frames: Optional[int] = None, alignment=None):
         """inference_tts with the audio handed out while it is generated: iterates wav chunks [1, channels, n*hop] whose
         concatenation equals ``tokenizer.decode([(gen, None)])``.  Afterwards ``.result`` is (res, gen), what inference_tts
         returns: the utterance samples from the device generator's stream at its current offset and leaves it advanced by
-        the steps it ran, as inference_tts does."""
+        the steps it ran, as inference_tts does.  alignment=: ``.alignment`` is then the Alignment inference_tts returns."""
         assert x.ndim == 2 and x.shape[0] == 1 and x_lens.ndim == 1 and y.ndim == 3 and y.shape[0] == 1, (x.shape, y.shape)
         sess = DecodeSession(self, [x], [y], self._sampling(top_k, top_p, temperature, stop_repetition, silence_tokens,
                                                             ras_window, ras_tau, min_frames, max_frames),
-                             n_copies=1)
+                             n_copies=1, alignment=alignment)
         return _SingleTtsStream(sess, tokenizer, chunk_frames, poll_every, sample_rate)
 
     def inference_many_stream(self, xs, ys, mask_intervals, tokenizer, chunk_frames: int = 25, poll_every: int = 8,
@@ -647,7 +657,7 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
     # Long TTS  (reference gradio_app.py run, mode "Long TTS"): one prompt, one sentence after another
     # ------------------------------------------------------------------------------------------------
     def _long_ticket(self, xs, y, best_of, top_k, top_p, temperature, stop_repetition, silence_tokens, ras_window, ras_tau,
-                     min_frames, max_frames):
+                     min_frames, max_frames, alignment=None):
         """a one-ticket ContinuousBatcher holding xs as a long ticket on the device generator's stream at its current
         offset, and the ticket's _Chain"""
         _no_host_noise_under_ras(sampling_controls(ras_window, ras_tau, min_frames, max_frames)[0],
@@ -659,40 +669,46 @@ class VoiceCraft(nn.Module, *_HubBase, **_HUB_KW):
                                temperature=temperature, stop_repetition=stop_repetition, silence_tokens=silence_tokens,
                                ras_window=ras_window, ras_tau=ras_tau, min_frames=min_frames, max_frames=max_frames)
         chain = _Chain(list(xs), int(gen.get_offset()))
-        cb.submit(chain, y, seed=int(gen.initial_seed()), best_of=best_of)
+        cb.submit(chain, y, seed=int(gen.initial_seed()), best_of=best_of, alignment=alignment)
         return cb, chain, gen
 
     @torch.no_grad()
     def inference_long_tts(self, xs, y: torch.Tensor, best_of: int = 1, logprobs: bool = False, top_k: int = -100,
                            top_p: float = 1.0, temperature: float = 1.0, stop_repetition: int = 3, kvcache: int = 1,
                            silence_tokens: List[int] = [1388, 1898, 131], ras_window: int = 0, ras_tau: float = 0.1,
-                           min_frames: int = 0, max_frames: Optional[int] = None):
+                           min_frames: int = 0, max_frames: Optional[int] = None, alignment=None):
         """The reference's Long TTS loop as one call: xs a list of [1,L_i] text-token tensors, one per sentence, all
-        prompted by y [1,T,K].  Returns one (res, gen) per sentence ((res, gen, lp) with logprobs=True), equal to
+        prompted by y [1,T,K].  Returns one (res, gen) per sentence ((res, gen, lp) with logprobs=True, and the sentence's
+        Alignment last with alignment=, as inference_tts returns them), equal to
         ``[inference_tts(x_i, ., y, ...) for x_i in xs]`` (inference_tts_batch(..., batch_size=best_of) with best_of > 1),
         and leaves the device generator where that loop leaves it: sentence i+1 samples from where sentence i ended.
         Runs as one long ticket of a ContinuousBatcher (submit with a list of x); the device generator only.
         ras_window, ras_tau, min_frames, max_frames: see sampling_controls; they apply to every sentence."""
         cb, chain, gen = self._long_ticket(xs, y, best_of, top_k, top_p, temperature, stop_repetition, silence_tokens,
-                                           ras_window, ras_tau, min_frames, max_frames)
+                                           ras_window, ras_tau, min_frames, max_frames, alignment)
         out = cb.run()[0]
         gen.set_offset(chain.offset)
         self.last_stats = dict(steps=cb.stats["steps"])
-        return [r + (lp,) for r, lp in zip(out, cb.logprobs[0])] if logprobs else out
+        if logprobs:
+            out = [r + (lp,) for r, lp in zip(out, cb.logprobs[0])]
+        if cb.alignments[0] is not None:
+            out = [r + (al,) for r, al in zip(out, cb.alignments[0])]
+        return out
 
     def inference_long_tts_stream(self, xs, y: torch.Tensor, tokenizer, chunk_frames: int = 25, sample_rate: int = None,
                                   top_k: int = -100, top_p: float = 1.0, temperature: float = 1.0,
                                   stop_repetition: int = 3, kvcache: int = 1, silence_tokens: List[int] = [1388, 1898, 131],
                                   ras_window: int = 0, ras_tau: float = 0.1, min_frames: int = 0,
-                                  max_frames: Optional[int] = None):
+                                  max_frames: Optional[int] = None, alignment=None):
         """inference_long_tts with the audio handed out while it is generated: iterates wav chunks [1, channels, n], the
         sentences in order; concatenated they equal ``torch.cat([tokenizer.decode([(gen_i, None)]) for gen_i in gens],
         -1)`` (each sentence decoded from a fresh codec state), and with sample_rate the tokenizer.resample of that
         concatenation.  Afterwards ``.results`` is what inference_long_tts returns, ``.logprobs`` its lp per sentence,
+        ``.alignments`` (with alignment=) its Alignment per sentence,
         and the device generator is left where inference_long_tts leaves it.  best_of = 1 only: the kept copy of a
         best-of-N sentence is known only when its group ends."""
         cb, chain, gen = self._long_ticket(xs, y, 1, top_k, top_p, temperature, stop_repetition, silence_tokens,
-                                           ras_window, ras_tau, min_frames, max_frames)
+                                           ras_window, ras_tau, min_frames, max_frames, alignment)
         return LongTtsStream(cb, chain, gen, tokenizer, chunk_frames, sample_rate)
 
 
@@ -813,6 +829,7 @@ class _Prompt:
             cap = min(cap, rows + max_frames * (1 if spans is None else len(spans)))
         self.need_seq = x_len + max(rows, cap + 1) + extra + 8
         self.total = x_len + int(self.y_tok.shape[0])           # positions the prefill writes
+        self.align = None                                       # vcb_prompt.align_heads (ctypes uint32 array) or None
 
     def pages(self, n_copies, max_pages):
         """KV pages vcb_prefill takes for it: a one-copy prompt its positions' pages in whole growth chunks, a best-of-N
@@ -834,6 +851,8 @@ class _Prompt:
             P.more_mask_rows[i] = int(v)
         if sp is not None:
             P.sampling = C.pointer(sp)
+        if self.align is not None:
+            P.align_heads = self.align
         if seed is not None:
             m = self.model
             P.rng_seed = int(seed) & 0xFFFFFFFFFFFFFFFF
@@ -890,6 +909,32 @@ class _Prompt:
             gen = None if gen is None else gen - int(a.n_special)
         out = res, None if gen is None else gen.unsqueeze(0)
         return out if lp_rows is None else out + (torch.from_numpy(lp).unsqueeze(0).to(dev),)
+
+
+def _align_heads(model, alignment, xs, edit=False):
+    """alignment= of a call as the vcb_prompt.align_heads of its prompts (a ctypes uint32 array, or None: off), checked
+    against the texts xs ([1,L] tensors) and the engine's align_text_cap; raises ValueError"""
+    masks = head_masks(alignment, model.args.num_decoder_layers, model.args.nhead)
+    if masks is None:
+        return None
+    if edit:
+        raise ValueError("alignment: speech edits are not supported (TTS results only)")
+    cap = model._eng_opts["align_text_cap"]
+    longest = max(int(x.shape[-1]) for x in xs)
+    if longest > cap:
+        raise ValueError(f"alignment of a {longest}-token text needs configure_engine(align_text_cap >= {longest}) "
+                         f"(align_text_cap is {cap})")
+    return (C.c_uint32 * len(masks))(*[int(v) for v in masks])
+
+
+def _read_alignment(model, eng, slot, prompt, frames, stream):
+    """the Alignment of the first `frames` frames of the result in `slot` (prefilled from `prompt` with align_heads):
+    frame t is the row at position x_len + t (voicecraft_b200/alignment.py)"""
+    x_len = int(prompt.x_ids.shape[0])
+    buf = np.empty((frames, x_len), dtype=np.float32)
+    _lib.check(_lib.load().vcb_read_alignment(eng, slot, buf.ctypes.data_as(C.POINTER(C.c_float)), x_len, frames, stream))
+    soft = torch.from_numpy(buf).to(prompt.y0.device)
+    return Alignment.from_soft(soft, model.args.encodec_sr, prompt.x_ids)
 
 
 def _prefill(eng, prompts, stream):
@@ -979,7 +1024,8 @@ class TtsStream(_AudioStream):
             raise _lib.VcbError("streaming an edit needs the device generators (model.noise_fn / noise_fns must be None): "
                                 "the polls do not follow the forced hand-over steps, so host noise would be drawn for them")
         self._start(SimpleNamespace(sess=sess, dev=sess.dev, tok=tokenizer, chunk_frames=int(chunk_frames),
-                                    poll_every=int(poll_every), results=None, logprobs=None, first_audio_steps=None,
+                                    poll_every=int(poll_every), results=None, logprobs=None, alignments=None,
+                                    first_audio_steps=None,
                                     sample_rate=sample_rate), sess.B)
 
     @property
@@ -990,6 +1036,11 @@ class TtsStream(_AudioStream):
     def logprobs(self):
         """after the iteration: utterance i's lp, as DecodeSession.results(logprobs=True) returns it"""
         return self._st.logprobs
+
+    @property
+    def alignments(self):
+        """after the iteration, for a session opened with alignment=: utterance i's Alignment (else None)"""
+        return self._st.alignments
 
     @property
     def first_audio_steps(self):
@@ -1036,8 +1087,9 @@ class TtsStream(_AudioStream):
                     if done and all(r.closed for r in live):
                         break
                 out = sess.results(logprobs=True)
-                st.results = [(res, gen) for res, gen, _ in out]
-                st.logprobs = [lp for _, _, lp in out]
+                st.results = [(o[0], o[1]) for o in out]
+                st.logprobs = [o[2] for o in out]
+                st.alignments = [o[3] for o in out] if sess.align else None
                 if sess.edit:                        # what inference_many / inference return: res alone
                     st.results = [res for res, _ in st.results]
         finally:
@@ -1198,6 +1250,12 @@ class _SingleTtsStream(TtsStream):
         lps = TtsStream.logprobs.fget(self)
         return None if lps is None else lps[0]
 
+    @property
+    def alignment(self):
+        """after the iteration: the Alignment inference_tts returns with alignment= (None without it)"""
+        als = TtsStream.alignments.fget(self)
+        return None if als is None else als[0]
+
 
 class LongTtsStream:
     """Iterator of VoiceCraft.inference_long_tts_stream: the wav chunks of its one long ticket (a BatcherStream), in
@@ -1206,7 +1264,7 @@ class LongTtsStream:
 
     def __init__(self, cb, chain, gen, tokenizer, chunk_frames, sample_rate):
         self._cb, self._chain, self._gen = cb, chain, gen
-        self.results = self.logprobs = None
+        self.results = self.logprobs = self.alignments = None
         self._it = cb.stream(tokenizer, chunk_frames, sample_rate)
 
     def __iter__(self):
@@ -1218,7 +1276,7 @@ class LongTtsStream:
         except StopIteration:
             cb = self._cb
             if cb.results and cb.results[0] is not None:
-                self.results, self.logprobs = cb.results[0], cb.logprobs[0]
+                self.results, self.logprobs, self.alignments = cb.results[0], cb.logprobs[0], cb.alignments[0]
                 self._gen.set_offset(self._chain.offset)
             raise
         if w is None:
@@ -1241,7 +1299,7 @@ class DecodeSession:
     one group of consecutive slots each."""
 
     def __init__(self, model: "VoiceCraft", xs, ys, sp, mask_intervals=None, seeds=None, noise_fns=None, *, best_of=1,
-                 n_copies=None):
+                 n_copies=None, alignment=None):
         """best_of: each utterance is sampled in best_of slots and keeps the copy that ends first (inference_tts_batch).
         n_copies (the single calls inference_tts, inference_tts_batch, inference and inference_tts_stream): best_of, and
         the one utterance samples from the device generator's stream at its current offset, and results() leaves the
@@ -1264,6 +1322,10 @@ class DecodeSession:
             self.prompts.append(_Prompt(model, x, y, spans, sp.max_frames))
         # one range check for the whole batch (the reference's embedding lookups raise on a bad id)
         model._check_ids(torch.cat([p.x_ids for p in self.prompts]), torch.cat([p.y_tok.reshape(-1) for p in self.prompts]))
+        c_masks = _align_heads(model, alignment, xs, self.edit)
+        self.align = c_masks is not None
+        for p in self.prompts:
+            p.align = c_masks
         self.eng, self.slots = model._take_slots(self.B * self.n_copies, max(p.need_seq for p in self.prompts))
         try:
             n = len(self.slots)
@@ -1421,10 +1483,14 @@ class DecodeSession:
         return j + (st[j].keep if self.n_copies > 1 else 0)
 
     def _result(self, i, slot, st, logprobs):
-        """utterance i's result from its slot (its kept copy's) and vcb_status"""
+        """utterance i's result from its slot (its kept copy's) and vcb_status; with alignment, its Alignment last"""
         m = self.model
         lp = m._read_lp(self.eng, slot, st.n_steps, self.stream) if logprobs else None
-        return self.prompts[i].result(m._read_rows(self.eng, slot, st.n_steps, self.stream), st, lp)
+        out = self.prompts[i].result(m._read_rows(self.eng, slot, st.n_steps, self.stream), st, lp)
+        return out + (self._alignment(i, slot, out[0].shape[-1]),) if self.align else out
+
+    def _alignment(self, i, slot, frames):
+        return _read_alignment(self.model, self.eng, slot, self.prompts[i], frames, self.stream)
 
     def _results(self, st, logprobs=False):
         out = []
@@ -1469,7 +1535,7 @@ class _Chain:
 
     def start(self, prompts):
         """(re)start the chain with one _Prompt per sentence"""
-        self.prompts, self.offset, self.results, self.logprobs = prompts, self.offset0, [], []
+        self.prompts, self.offset, self.results, self.logprobs, self.alignments = prompts, self.offset0, [], [], []
 
     @property
     def need_seq(self):
@@ -1480,23 +1546,25 @@ class _Chain:
         """the prompt of the sentence to run now"""
         return self.prompts[len(self.results)]
 
-    def ended(self, result, lp, offset) -> bool:
-        """the sentence running now ended with `result`, `lp`, its stream at `offset` (vcb_status.rng_offset of its slot,
-        its group's first): True when another sentence follows"""
+    def ended(self, result, lp, offset, al=None) -> bool:
+        """the sentence running now ended with `result`, `lp`, `al` (its Alignment or None), its stream at `offset`
+        (vcb_status.rng_offset of its slot, its group's first): True when another sentence follows"""
         self.results.append(result)
         self.logprobs.append(lp)
+        self.alignments.append(al)
         self.offset = int(offset)
         return len(self.results) < len(self.prompts)
 
 
 class _Ticket:
     """A ContinuousBatcher ticket: `prompt` the _Prompt that runs now (placeholder codes until _encode replaces them),
-    `seed`, `best_of`, `sp` its vcb_sampling, `pending` (x, audio, sample_rate) of audio not encoded yet, and `chain` a
-    long ticket's _Chain."""
-    __slots__ = ("prompt", "seed", "best_of", "sp", "pending", "chain")
+    `seed`, `best_of`, `sp` its vcb_sampling, `pending` (x, audio, sample_rate) of audio not encoded yet, `chain` a
+    long ticket's _Chain and `align` its vcb_prompt.align_heads (None: no alignment), which every prompt it runs carries."""
+    __slots__ = ("prompt", "seed", "best_of", "sp", "pending", "chain", "align")
 
-    def __init__(self, prompt, seed, best_of, sp, pending=None, chain=None):
+    def __init__(self, prompt, seed, best_of, sp, pending=None, chain=None, align=None):
         self.prompt, self.seed, self.best_of, self.sp, self.pending, self.chain = prompt, seed, best_of, sp, pending, chain
+        self.align = align
 
     @property
     def need_seq(self):
@@ -1660,9 +1728,14 @@ class ContinuousBatcher:
 
     def __init__(self, model: "VoiceCraft", max_concurrency=32, poll_every=8, top_k=-100, top_p=1.0, temperature=1.0,
                  stop_repetition=3, silence_tokens=(1388, 1898, 131), tokenizer=None, ras_window=0, ras_tau=0.1,
-                 min_frames=0, max_frames=None):
-        """ras_window, ras_tau, min_frames, max_frames: the tickets' default sampling controls (sampling_controls)"""
+                 min_frames=0, max_frames=None, alignment=None):
+        """ras_window, ras_tau, min_frames, max_frames: the tickets' default sampling controls (sampling_controls).
+        alignment: the TTS tickets' default alignment= (as inference_tts takes it); alignments[ticket] then holds the
+        ticket's Alignment next to results / logprobs (a long ticket's: one per sentence), None for a ticket without"""
         sampling_controls(ras_window, ras_tau, min_frames, max_frames)
+        if alignment is not None:
+            head_masks(alignment, model.args.num_decoder_layers, model.args.nhead)
+        self.alignment = alignment
         self.model, self.B, self.poll_every = model, int(max_concurrency), max(1, int(poll_every))
         self.tokenizer = tokenizer         # encodes the prompt audio of submit(audio=...) tickets
         self.defaults = dict(top_k=top_k, top_p=top_p, temperature=temperature, stop_repetition=stop_repetition,
@@ -1672,11 +1745,12 @@ class ContinuousBatcher:
         self.stats = dict(steps=0, prefills=0, max_active=0, swap_outs=0, swap_ins=0)
         self.results, self.errors = [], {}
         self.logprobs = []                 # lp of results[ticket] (as inference_tts / inference return it), None with it
+        self.alignments = []               # Alignment of results[ticket] (a list for a long ticket), None without
         self._live = None                  # the running stream()'s state
 
     def submit(self, x, y=None, seed=None, best_of=1, mask_interval=None, top_k=None, top_p=None, temperature=None,
                stop_repetition=None, silence_tokens=None, audio=None, sample_rate=None, ras_window=None, ras_tau=None,
-               min_frames=None, max_frames=None):
+               min_frames=None, max_frames=None, alignment=None):
         """x [1,L] int64, y [1,T,K] int64 (host or device).  Returns the ticket (index into run()'s result list / results).
         audio [channels, N] (instead of y): the prompt as audio at sample_rate (default: the codec's), encoded by the
         constructor's tokenizer when the ticket is admitted, together with the other audio tickets admitted with it
@@ -1705,7 +1779,9 @@ class ContinuousBatcher:
         across sentence boundaries by one resampler stream, so they equal ``resample(torch.cat([decode_codes(gen_i)],
         -1))``; last=True marks the final sentence's last chunk; cancel() drops the rest of the chain; a sentence that
         fails fails the ticket and errors[ticket] names it.  Raises ValueError on an empty list, on a list with
-        mask_interval and, while a stream() runs, on a sentence that does not fit its engine."""
+        mask_interval and, while a stream() runs, on a sentence that does not fit its engine.
+        alignment: as inference_tts's; None takes the constructor's value, False is off.  An edit ticket refuses one (the
+        constructor's default does not apply to edits), as does a text longer than align_text_cap (ValueError)."""
         if (y is None) == (audio is None):
             raise ValueError("submit takes exactly one of y (codes) and audio")
         if isinstance(x, (list, tuple)):
@@ -1747,10 +1823,13 @@ class ContinuousBatcher:
             raise ValueError(f"temperature must be finite and > 0 and top_p a number, got {params}")
         sp = self.model._sampling(**params)
         _no_host_noise_under_ras(sp.ras_window, self.model.noise_fn is not None)
+        if alignment is None and spans is None:
+            alignment = self.alignment
+        align = _align_heads(self.model, alignment, x.xs if isinstance(x, _Chain) else [x], spans is not None)
         st = self._live
         if st is not None:
             _no_stream_best_of(best_of)
-            job = self._job(x, y, seed, 1, spans, sp, pending)
+            job = self._job(x, y, seed, 1, spans, sp, pending, align)
             if job.chain is not None and job.chain.need_seq > st.max_seq:
                 raise ValueError(f"a sentence needs {job.chain.need_seq} positions, the streaming engine holds {st.max_seq}: "
                                  "configure_engine(max_seq_len=...) before stream()")
@@ -1760,7 +1839,8 @@ class ContinuousBatcher:
             st.jobs.append(job)
             self.results.append(None)
             self.logprobs.append(None)
-        self.queue.append((x, y, seed, best_of, spans, sp, pending))
+            self.alignments.append(None)
+        self.queue.append((x, y, seed, best_of, spans, sp, pending, align))
         return len(self.queue) - 1
 
     def cancel(self, ticket) -> bool:
@@ -1774,16 +1854,19 @@ class ContinuousBatcher:
         st.cancelled.add(ticket)
         return True
 
-    def _job(self, x, y, seed, best_of, spans, sp, pending=None):
+    def _job(self, x, y, seed, best_of, spans, sp, pending=None, align=None):
         """the _Ticket of submit's arguments; raises IndexError on an out-of-range id.  A long ticket's chain (x, a
         _Chain) gets the prompts of its sentences."""
         if not isinstance(x, _Chain):
             p = _Prompt(self.model, x, y, spans, sp.max_frames)
             self.model._check_ids(p.x_ids, p.y_tok)
-            return _Ticket(p, seed, best_of, sp, pending)
+            p.align = align
+            return _Ticket(p, seed, best_of, sp, pending, align=align)
         x.start([_Prompt(self.model, xi, y, None, sp.max_frames) for xi in x.xs])
+        for p in x.prompts:
+            p.align = align
         self.model._check_ids(torch.cat([p.x_ids for p in x.prompts]), x.prompts[0].y_tok)
-        return _Ticket(x.prompt, seed, best_of, sp, pending, x)
+        return _Ticket(x.prompt, seed, best_of, sp, pending, x, align)
 
     def _open(self, s, ops):
         """The state of run() / stream(), `s`, holds eng, slots, jobs, results, cancelled and cstream (the codec's CUDA
@@ -1816,12 +1899,17 @@ class ContinuousBatcher:
             slot, st = kept
             res, gen, lp = job.prompt.result(m._read_rows(s.eng, slot, st.n_steps, s.stream), st,
                                              m._read_lp(s.eng, slot, st.n_steps, s.stream))
+            al = None if job.align is None else _read_alignment(m, s.eng, slot, job.prompt, res.shape[-1], s.stream)
             if job.chain is None:
                 s.results[t], self.logprobs[t] = (res, gen), lp
-            elif job.chain.ended((res, gen), lp, r.status.rng_offset):
+                if al is not None:
+                    self.alignments[t] = al
+            elif job.chain.ended((res, gen), lp, r.status.rng_offset, al):
                 job.prompt, follows = job.chain.prompt, True
             else:
                 s.results[t], self.logprobs[t] = job.chain.results, job.chain.logprobs
+                if job.align is not None:
+                    self.alignments[t] = job.chain.alignments
         m._release_slots(s.slots, [r.slot], n_copies=job.best_of, keep_held=True)
         del s.active[r.slot]
         if follows:
@@ -1909,8 +1997,11 @@ class ContinuousBatcher:
             y = c.transpose(1, 2)
             if j.chain is None:
                 real = _Prompt(self.model, j.pending[0], y, j.prompt.spans, j.sp.max_frames)
+                real.align = j.align
             else:                                # every sentence of a long ticket: one encode for the chain
                 j.chain.start([_Prompt(self.model, xi, y, None, j.sp.max_frames) for xi in j.chain.xs])
+                for p in j.chain.prompts:
+                    p.align = j.align
                 real = j.chain.prompt
             assert real.need_seq == j.prompt.need_seq and real.total == j.prompt.total
             j.prompt, j.pending = real, None
@@ -1943,6 +2034,7 @@ class ContinuousBatcher:
         s = SimpleNamespace(eng=eng, slots=slots, jobs=jobs, results=[None] * len(jobs), cancelled=set(), cstream=None,
                             pool=None)
         self.logprobs = [None] * len(jobs)
+        self.alignments = [None] * len(jobs)
         try:
             with torch.cuda.device(dev):
                 self._open(s, _EngineOps(eng, torch.cuda.current_stream().cuda_stream))
@@ -2003,7 +2095,7 @@ class BatcherStream(_AudioStream):
                              results=[None] * len(jobs), cancelled=set(refused), ended=set(refused),
                              refused=sorted(refused), tok=tokenizer, chunk_frames=int(chunk_frames),
                              dev=m.mask_embedding.device, sample_rate=sample_rate, pool=None)
-        cb.results, cb.logprobs, cb._live = st.results, [None] * len(jobs), st
+        cb.results, cb.logprobs, cb.alignments, cb._live = st.results, [None] * len(jobs), [None] * len(jobs), st
         cb.errors = {t: f"best_of={jobs[t].best_of}: stream() serves only best_of=1 tickets" for t in refused}
         # a codec stream id belongs to a ticket from its admission to its end: at most max_concurrency are active and, under
         # a KV budget, at most as many more are swapped out
