@@ -231,8 +231,8 @@ int vcb_align_monotonic(const float* logp_dev, int32_t T, int32_t X, int32_t* du
 int vcb_release(vcb_engine* e, int32_t slot, int32_t n_copies);
 /* Swap a one-copy utterance out to host memory and back, byte for byte (DESIGN.md section 3).  vcb_swap_out copies what the
  * slot's continuation depends on -- the K and V slabs of its written pages in every layer, its SlotState and GroupState
- * (Philox offset included), its sampling parameters, token-log and log-probability rows [0, n_steps), its next-input and last-hidden rows and
- * the host-side slot flags -- into a snapshot, then releases the slot.  Rejected before anything changes: a slot that is not
+ * (Philox offset included), its sampling parameters, token-log and log-probability rows [0, n_steps), its next-input and last-hidden rows,
+ * its alignment rows [0, seq_len) when it aligns, and the slot's host record -- into a snapshot, then releases the slot.  Rejected before anything changes: a slot that is not
  * open or belongs to a best-of-N group.
  * vcb_swap_in restores a snapshot of this engine into the free `slot` on newly taken pages and a free group id; rejected
  * before anything changes: a snapshot of another engine, a slot that is open, no free group, fewer free pages than

@@ -5,6 +5,7 @@
 // per-slot / per-group device state, step workspaces.  The caller (Python/torch) owns inputs, outputs and the stream.
 #include "../../include/vcb200.h"
 #include "lm_kernels.cuh"
+#include "slot_table.h"
 
 #include <algorithm>
 #include <array>
@@ -59,11 +60,6 @@ struct Layer {
 using namespace vcb;
 static_assert(KV_BF16 == VCB_KV_BF16 && KV_FP32 == VCB_KV_FP32 && KV_FP8 == VCB_KV_FP8, "KV policy ids of vcb_internal.h");
 
-// vcb_engine::group_sp, bits: the group was prefilled with sampling parameters of its own; they turn on repetition-aware
-// sampling or a length bound (its steps run the sampler instance with those controls); they turn on repetition-aware
-// sampling (its steps take no caller noise)
-enum : char { GROUP_SP_OWN = 1, GROUP_SP_CTL = 2, GROUP_SP_RAS = 4 };
-
 static bool controls_on(const vcb_sampling* q) { return q->ras_window != 0 || q->min_frames != 0 || q->max_frames != 0; }
 
 struct vcb_engine {
@@ -75,12 +71,7 @@ struct vcb_engine {
     uint64_t id = 0;                  // process-unique: a snapshot names the engine it came from
     int max_pages_per_slot = 0, n_pages = 0;
     int64_t n_pages_needed = 0;       // pages the last refused vcb_decode_step lacked (VCB_ERR_KV_FULL)
-    std::vector<int> free_pages;
-    std::vector<int> page_refs;       // slots whose page list holds the page (a best-of-N group shares its full prompt pages)
-    std::vector<std::vector<int>> slot_pages;
-    std::vector<int> slot_group;      // host mirror: group id per slot (-1 closed)
-    std::vector<int> free_groups;
-    std::vector<char> group_sp;       // host mirror: GROUP_SP_* bits of the group's own sampling parameters (sp_tab)
+    SlotTable slots;                  // host records of the slots and groups, and the KV page allocator
 
     std::map<std::string, DevBuf<float>> f32;     // every loaded fp32 tensor (device)
     std::map<std::string, std::vector<int64_t>> shapes;
@@ -106,8 +97,6 @@ struct vcb_engine {
     DevBuf<int> att_cnt;              // per (row, head) arrival counters
     int att_maxch = 1, att_chunk_pages = ATT_CHUNK_PAGES;
     std::vector<float*> h_bias2;      // host copy of the K second-stage bias pointers
-    std::vector<int> h_seq_len;       // host upper bound of SlotState::seq_len: the attention grid, and the position the next
-                                      // step writes (page growth)
     DevBuf<__nv_bfloat16> act_d, act_d2, act_f, act_h;
     CUtensorMap tm_act_d[4], tm_act_d2[4], tm_act_f[4], tm_act_h[4];   // bpad = 16, 32, 64, 128
     DevBuf<int> row_slot, row_pos, row_last, page_table;   // decode-step rows
@@ -116,10 +105,6 @@ struct vcb_engine {
     DevBuf<int> row_pages;            // decode steps: per-row copy of the slot's page list [rows][max_pages_per_slot]
     DevBuf<unsigned long long> row_epoch;   // decode steps: the step whose row tables step_prep last published, per row
     unsigned long long step_epoch = 0;      // decode steps enqueued since create (the epoch step_prep publishes)
-    std::vector<char> slot_rng;       // host mirror: the slot's group generates its own sampling noise
-    std::vector<char> slot_edit;      // host mirror: masked spans of the slot's edit prompt (0: a TTS prompt)
-    std::vector<int> slot_copies;     // host mirror: n_copies of the slot's prompt (best-of-N group size)
-    std::vector<int> slot_final;      // final frames vcb_poll_frames last reported for the slot (they only grow)
     DevBuf<PollFramesRec> pf_rec;     // vcb_poll_frames results [max_slots]
     PinnedBuf<PollFramesRec> h_pf_rec;
     DevBuf<vcb_edit_source> pf_src;   // vcb_poll_frames_ex sources [max_slots], staged through h_pf_src
@@ -135,13 +120,11 @@ struct vcb_engine {
     // decode rows in groups of one best-of-N group's consecutive slots (attn_rows_kernel<.., ATT_GMAX>): d_slots holds the
     // n slots, then grp_first [n_row_groups + 1], then grp_shared [n_row_groups]; n_row_groups = 0: no shared group listed
     int n_row_groups = 0;
-    std::vector<int> slot_shared;     // host mirror: full prompt pages the slot shares with its group (0: none)
     DevBuf<int> tok_log;
     DevBuf<float> lp_log;             // [max_slots][max_new_tokens][K]: log-probability of each token-log entry
     // alignment (vcb_prompt.align_heads, DESIGN.md section 4.6): allocated by the first prefill that asks for it
     DevBuf<float> align_log;          // [max_slots][max_seq_len][align_text_cap]
     DevBuf<uint32_t> align_masks;     // [max_slots][L] head bitmasks of each slot's prompt (0: off)
-    std::vector<uint32_t> slot_align; // host copy of align_masks (what the device holds)
     std::vector<char> pass_align;     // [L]: the pass being enqueued has a row that probes layer l
     DevBuf<float> dbg_logits;
     DevBuf<SlotState> st;
@@ -231,14 +214,10 @@ struct vcb_snapshot {
     SlotState S;                      // group / member rewritten by vcb_swap_in
     GroupState G;                     // Philox offset included; first_slot rewritten
     SamplingParams sp;                // the group's own parameters (has_sp)
-    char has_sp = 0, rng = 0, edit = 0;
-    int final_frames = 0;             // slot_final
+    char has_sp = 0;                  // GROUP_SP_* bits of the group
+    SlotRec rec;                      // the slot's host record; vcb_swap_in takes its pages anew
     PinnedBuf<uint8_t> kv;            // [2L pools][n_pages][H slabs], as kv_pages_copy_kernel stages them
-    PinnedBuf<int> tok;               // token-log rows [0, n_steps) x K
-    PinnedBuf<float> lp;              // log-probability rows [0, n_steps) x K
-    PinnedBuf<float> rows;            // x_slot row (next input), h_slot row (last prefill hidden state)
-    std::vector<uint32_t> align;      // the slot's alignment head masks [L] (empty: alignment off)
-    PinnedBuf<float> align_rows;      // its alignment-log rows [0, seq_len) x align_text_cap
+    PinnedBuf<uint8_t> rows;          // the live bytes of the slot's swap_rows, back to back
 };
 
 enum { PC_GEMM = 0, PC_ATTN = 1, PC_LN = 2, PC_FINISH = 3, PC_SAMPLER = 4, PC_MISC = 5, PC_MEGA = 6, PC_N = 7 };
@@ -746,11 +725,12 @@ int launch_align(vcb_engine* e, const Pass& p, int l, cudaStream_t st) {
 // pass_align for the rows of `slots` (the slots whose rows the pass runs); true when any layer is probed
 bool plan_align(vcb_engine* e, const int* slots, int n) {
     e->pass_align.assign(e->m.L, 0);
-    if (e->slot_align.empty()) return false;
     bool any = false;
-    for (int i = 0; i < n; ++i)
-        for (int l = 0; l < e->m.L; ++l)
-            if (e->slot_align[static_cast<size_t>(slots[i]) * e->m.L + l]) any = e->pass_align[l] = 1;
+    for (int i = 0; i < n; ++i) {
+        const std::vector<uint32_t>& masks = e->slots[slots[i]].align;
+        for (size_t l = 0; l < masks.size(); ++l)
+            if (masks[l]) any = e->pass_align[l] = 1;
+    }
     return any;
 }
 
@@ -1023,7 +1003,7 @@ int check_slots(vcb_engine* e, const int32_t* slots, int n) {
         return -1;
     }
     for (int i = 0; i < n; ++i)
-        if (slots[i] < 0 || slots[i] >= e->cfg.max_slots || e->slot_group[slots[i]] < 0) {
+        if (!e->slots.is_open(slots[i])) {
             set_error("slot %d is not open", slots[i]);
             return -1;
         }
@@ -1039,10 +1019,10 @@ int upload_slots(vcb_engine* e, const int32_t* slots, int n, cudaStream_t st) {
     std::vector<int> tab(slots, slots + n), first{0}, shared;
     bool grouped = false;
     for (int i = 0; i < n;) {
-        const int S = e->slot_shared[slots[i]];
+        const int S = e->slots[slots[i]].shared;
         int j = i + 1;
         while (S > 0 && j < n && j - i < ATT_GMAX && slots[j] == slots[j - 1] + 1 &&
-               e->slot_group[slots[j]] == e->slot_group[slots[i]])
+               e->slots[slots[j]].group == e->slots[slots[i]].group)
             ++j;
         grouped |= j - i > 1;
         first.push_back(j);
@@ -1057,55 +1037,9 @@ int upload_slots(vcb_engine* e, const int32_t* slots, int n, cudaStream_t st) {
     return upload_ints(e, tab.data(), tab.size(), e->d_slots, st);
 }
 
-// page-list length of a one-copy utterance that writes positions [0, pos]: whole growth chunks, at most max_pages_per_slot
-int grown_pages(const vcb_engine* e, int pos) {
-    const int want = pos / KV_PAGE + 1;
-    return std::min(e->max_pages_per_slot, (want + VCB_KV_GROW_PAGES - 1) / VCB_KV_GROW_PAGES * VCB_KV_GROW_PAGES);
-}
-
 // one KV page of every layer, K and V (the unit of kv_pool_bytes)
 size_t page_bytes_all_layers(const vcb_engine* e) {
     return 2ull * e->m.L * e->m.H * kv_slab_bytes(e->kv_dtype, e->m.hd);
-}
-
-// a page-table row of `slot` as the device holds it: the slot's pages, then page 0 (never read: attention and the QKV
-// epilogues read positions up to the one a step writes)
-std::vector<int> page_row(const vcb_engine* e, int slot) {
-    std::vector<int> row(e->slot_pages[slot]);
-    row.resize(e->max_pages_per_slot, 0);
-    return row;
-}
-
-// Page growth of a decode step, planned on the host without touching any state: every listed one-copy slot needs a page
-// for position h_seq_len (it writes at most there).  Slots take whole chunks when the free list covers them all, else the
-// pages they need; VCB_ERR_KV_FULL (kv_pages_needed set) when it cannot cover even that.  grow: (slot, new page count).
-int plan_growth(vcb_engine* e, const int32_t* slots, int n, std::vector<std::pair<int, int>>& grow) {
-    grow.clear();
-    size_t need = 0, chunked = 0;
-    std::vector<int> want;
-    for (int i = 0; i < n; ++i) {
-        const int s = slots[i];
-        const int have = static_cast<int>(e->slot_pages[s].size());
-        const int need_s = std::min(e->max_pages_per_slot, e->h_seq_len[s] / KV_PAGE + 1);
-        if (e->slot_copies[s] != 1 || need_s <= have ||
-            std::any_of(grow.begin(), grow.end(), [s](const std::pair<int, int>& g) { return g.first == s; }))
-            continue;
-        const int chunk = grown_pages(e, e->h_seq_len[s]);
-        grow.emplace_back(s, chunk);
-        want.push_back(need_s);
-        need += need_s - have;
-        chunked += chunk - have;
-    }
-    if (need > e->free_pages.size()) {
-        e->n_pages_needed = static_cast<int64_t>(need - e->free_pages.size());
-        set_error("vcb_decode_step: KV pool full: the listed slots need %zu more pages, %zu are free", need,
-                  e->free_pages.size());
-        grow.clear();
-        return VCB_ERR_KV_FULL;
-    }
-    if (chunked > e->free_pages.size())
-        for (size_t i = 0; i < grow.size(); ++i) grow[i].second = want[i];
-    return 0;
 }
 
 // takes the planned pages and enqueues the new page-table entries on `st` (one pinned staging entry of the ring)
@@ -1117,19 +1051,29 @@ int apply_growth(vcb_engine* e, const std::vector<std::pair<int, int>>& grow, cu
     int* stage = e->grow_stage + static_cast<size_t>(k) * vcb_engine::GROW_INTS;
     int used = 0;
     for (const auto& g : grow) {
-        auto& pg = e->slot_pages[g.first];
-        const int from = static_cast<int>(pg.size());
-        for (int p = from; p < g.second; ++p) {
-            pg.push_back(e->free_pages.back());
-            e->free_pages.pop_back();
-            ++e->page_refs[pg.back()];
-            stage[used + p - from] = pg.back();
-        }
+        const int from = static_cast<int>(e->slots[g.first].pages.size());
+        e->slots.grow_to(g.first, g.second);
+        std::copy(e->slots[g.first].pages.begin() + from, e->slots[g.first].pages.end(), stage + used);
         VCB_CUDA_OK(cudaMemcpyAsync(e->page_table + static_cast<size_t>(g.first) * e->max_pages_per_slot + from, stage + used,
                                     (g.second - from) * sizeof(int), cudaMemcpyHostToDevice, st));
         used += g.second - from;
     }
     VCB_CUDA_OK(cudaEventRecord(e->grow_ev[k], st));
+    return 0;
+}
+
+// the device rows of a slot just opened (vcb_prefill, vcb_swap_in): its SlotState S, its page-table row and, once the
+// alignment log exists, its head masks (zero when it does not align)
+int write_slot_rows(vcb_engine* e, int slot, const SlotState& S) {
+    VCB_CUDA_OK(cudaMemcpy(e->st + slot, &S, sizeof(SlotState), cudaMemcpyHostToDevice));
+    VCB_CUDA_OK(cudaMemcpy(e->page_table + static_cast<size_t>(slot) * e->max_pages_per_slot, e->slots.page_row(slot).data(),
+                           e->max_pages_per_slot * sizeof(int), cudaMemcpyHostToDevice));
+    if (e->align_masks) {
+        std::vector<uint32_t> masks(e->slots[slot].align);
+        masks.resize(e->m.L, 0u);
+        VCB_CUDA_OK(cudaMemcpy(e->align_masks + static_cast<size_t>(slot) * e->m.L, masks.data(), e->m.L * sizeof(uint32_t),
+                               cudaMemcpyHostToDevice));
+    }
     return 0;
 }
 
@@ -1139,7 +1083,7 @@ int apply_growth(vcb_engine* e, const std::vector<std::pair<int, int>>& grow, cu
 int noise_required(vcb_engine* e, const int32_t* slots, int n, const float* noise, const vcb_sampling* sp) {
     if (noise) {
         for (int i = 0; i < n; ++i)
-            if (sp ? sp->ras_window > 0 : (e->group_sp[e->slot_group[slots[i]]] & GROUP_SP_RAS) != 0) {
+            if (sp ? sp->ras_window > 0 : (e->slots.sp_bits(slots[i]) & GROUP_SP_RAS) != 0) {
                 set_error("slot %d samples with repetition-aware sampling, which draws from the device generator: "
                           "exp_noise_dev must be null", slots[i]);
                 return -1;
@@ -1147,7 +1091,7 @@ int noise_required(vcb_engine* e, const int32_t* slots, int n, const float* nois
         return 0;
     }
     for (int i = 0; i < n; ++i)
-        if (!e->slot_rng[slots[i]]) {
+        if (!e->slots[slots[i]].rng) {
             set_error("slot %d has no device generator (vcb_prompt.rng_threads == 0): exp_noise_dev must not be null", slots[i]);
             return -1;
         }
@@ -1158,7 +1102,7 @@ int noise_required(vcb_engine* e, const int32_t* slots, int n, const float* nois
 bool sampler_controls(vcb_engine* e, const int32_t* slots, int n, const vcb_sampling* sp) {
     if (sp) return controls_on(sp);
     for (int i = 0; i < n; ++i)
-        if (e->group_sp[e->slot_group[slots[i]]] & GROUP_SP_CTL) return true;
+        if (e->slots.sp_bits(slots[i]) & GROUP_SP_CTL) return true;
     return false;
 }
 
@@ -1166,7 +1110,7 @@ bool sampler_controls(vcb_engine* e, const int32_t* slots, int n, const vcb_samp
 int sampling_required(vcb_engine* e, const int32_t* slots, int n, const vcb_sampling* sp) {
     if (sp) return 0;
     for (int i = 0; i < n; ++i)
-        if (!e->group_sp[e->slot_group[slots[i]]]) {
+        if (!e->slots.sp_bits(slots[i])) {
             set_error("slot %d has no sampling parameters of its own (vcb_prompt.sampling == NULL): sp must not be null",
                       slots[i]);
             return -1;
@@ -1400,18 +1344,7 @@ int vcb_create(const vcb_config* cfg, vcb_engine** out) {
     }
     static std::atomic<uint64_t> next_id{1};
     e->id = next_id++;
-    for (int p = e->n_pages - 1; p >= 0; --p) e->free_pages.push_back(p);
-    e->page_refs.assign(e->n_pages, 0);
-    e->slot_pages.resize(cfg->max_slots);
-    e->slot_group.assign(cfg->max_slots, -1);
-    e->slot_rng.assign(cfg->max_slots, 0);
-    e->slot_edit.assign(cfg->max_slots, 0);
-    e->group_sp.assign(cfg->max_slots, 0);
-    e->slot_copies.assign(cfg->max_slots, 0);
-    e->slot_shared.assign(cfg->max_slots, 0);
-    e->slot_final.assign(cfg->max_slots, 0);
-    e->h_seq_len.assign(cfg->max_slots, 0);
-    for (int g = cfg->max_slots - 1; g >= 0; --g) e->free_groups.push_back(g);
+    e->slots = SlotTable(e->n_pages, cfg->max_slots, e->max_pages_per_slot, KV_PAGE);
     e->layers.resize(m.L);
     e->h2.resize(m.K);
     e->opt_simt = simt && !strcmp(simt, "simt");
@@ -1625,7 +1558,6 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
     std::vector<std::pair<int, SamplingParams>> gsp;   // (group id, parameters) of the groups prefilled with their own
     std::vector<ForkPair> fork;
     std::vector<std::array<int, 3>> align_fork;        // (leader, member, prompt positions) of the aligning groups
-    std::vector<int> align_set;                         // slots whose align_masks row this prefill rewrites
     bool aligning = false;
     // ---- validate everything before touching host or device state (a failed call must leave no slot, group or page held)
     {
@@ -1672,23 +1604,20 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
                 aligning = true;
             }
             for (int c = 0; c < P.n_copies; ++c) {
-                if (e->slot_group[P.slot + c] >= 0 || claimed[P.slot + c]) {
+                if (e->slots.is_open(P.slot + c) || claimed[P.slot + c]) {
                     set_error("slot %d already open", P.slot + c);
                     return -1;
                 }
                 claimed[P.slot + c] = 1;
             }
-            // one prefill per group; the members share the leader's full prompt pages
-            const int shared = static_cast<int>(total / KV_PAGE);
-            rows_needed += static_cast<size_t>(total);
-            pages_needed += P.n_copies == 1 ? grown_pages(e, static_cast<int>(total) - 1)
-                                             : e->max_pages_per_slot + static_cast<size_t>(P.n_copies - 1) * (e->max_pages_per_slot - shared);
+            rows_needed += static_cast<size_t>(total);         // one prefill per group
+            pages_needed += e->slots.prompt_pages(static_cast<int>(total), P.n_copies);
         }
-        if (static_cast<size_t>(n) > e->free_groups.size()) {
+        if (static_cast<size_t>(n) > e->slots.groups_left()) {
             set_error("no free group");
             return -1;
         }
-        if (pages_needed > e->free_pages.size()) {
+        if (pages_needed > e->slots.free_list().size()) {
             set_error("KV pool exhausted");
             return -1;
         }
@@ -1708,14 +1637,30 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
                 e->align_masks.reset();
                 return -1;
             }
-            e->slot_align.assign(static_cast<size_t>(e->cfg.max_slots) * m.L, 0);
         }
     }
     for (int i = 0; i < n; ++i) {
         const vcb_prompt& P = prompts[i];
         const int total = P.x_len + P.y_len;
-        const int gid = e->free_groups.back();
-        e->free_groups.pop_back();
+        SlotRec rec;
+        rec.seq_len = total;
+        rec.copies = P.n_copies;
+        rec.shared = P.n_copies > 1 ? total / KV_PAGE : 0;    // full prompt pages: written by the prefill only, never by a step
+        rec.rng = P.rng_threads != 0;
+        rec.edit = static_cast<char>(P.mode == VCB_MODE_EDIT ? P.n_more_spans + 1 : 0);
+        if (P.align_heads) rec.align.assign(P.align_heads, P.align_heads + m.L);
+        const char sp_bits = !P.sampling ? 0
+                                         : GROUP_SP_OWN | (controls_on(P.sampling) ? GROUP_SP_CTL : 0) |
+                                               (P.sampling->ras_window > 0 ? GROUP_SP_RAS : 0);
+        const int gid = e->slots.open(P.slot, rec, e->slots.open_pages(total, P.n_copies), -1, sp_bits);
+        for (int c = 1; c < P.n_copies; ++c) {
+            const int slot = P.slot + c;
+            e->slots.open(slot, rec, e->slots.open_pages(total, P.n_copies), P.slot, 0);
+            const bool tail = total % KV_PAGE != 0;
+            fork.push_back({P.slot, slot, tail ? e->slots[P.slot].pages[rec.shared] : -1,
+                            tail ? e->slots[slot].pages[rec.shared] : -1});
+            if (P.align_heads) align_fork.push_back({P.slot, slot, total});
+        }
         GroupState G;
         memset(&G, 0, sizeof(G));
         G.mode = P.mode;
@@ -1731,9 +1676,6 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
         G.off_hi = static_cast<unsigned int>(P.rng_offset >> 32);
         gst.push_back(G);
         gst_id.push_back(gid);
-        e->group_sp[gid] = !P.sampling ? 0
-                                       : GROUP_SP_OWN | (controls_on(P.sampling) ? GROUP_SP_CTL : 0) |
-                                             (P.sampling->ras_window > 0 ? GROUP_SP_RAS : 0);
         if (P.sampling) gsp.emplace_back(gid, sampling_params(P.sampling));
         EmbedSeq es;
         es.text_ids = reinterpret_cast<const long long*>(P.text_ids_dev);
@@ -1743,72 +1685,32 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
         es.y_len = P.y_len;
         const int seq_idx = static_cast<int>(seqs.size());
         seqs.push_back(es);
-        const int shared = total / KV_PAGE;           // full prompt pages: written by the prefill only, never by a step
+        SlotState S;
+        memset(&S, 0, sizeof(S));
+        S.x_len = P.x_len;
+        S.seq_len = total;
+        S.y_len = P.y_len;
+        S.group = gid;
+        S.prev_token = -1;
+        S.active = 1;
         for (int c = 0; c < P.n_copies; ++c) {
-            const int slot = P.slot + c;
-            e->slot_group[slot] = gid;
-            e->slot_rng[slot] = P.rng_threads != 0;
-            e->slot_edit[slot] = static_cast<char>(P.mode == VCB_MODE_EDIT ? P.n_more_spans + 1 : 0);
-            e->slot_copies[slot] = P.n_copies;
-            e->slot_shared[slot] = P.n_copies > 1 ? shared : 0;
-            e->slot_final[slot] = 0;
-            auto& pg = e->slot_pages[slot];
-            pg.clear();
-            // a one-copy prompt takes the pages of its positions (vcb_decode_step grows them); a group its full reservation
-            const int n_pg = P.n_copies == 1 ? grown_pages(e, total - 1) : e->max_pages_per_slot;
-            for (int p = 0; p < n_pg; ++p) {
-                if (c > 0 && p < shared) {
-                    pg.push_back(e->slot_pages[P.slot][p]);
-                } else {
-                    pg.push_back(e->free_pages.back());
-                    e->free_pages.pop_back();
-                }
-                ++e->page_refs[pg.back()];
-            }
-            if (c > 0) {
-                const bool tail = total % KV_PAGE != 0;
-                fork.push_back({P.slot, slot, tail ? e->slot_pages[P.slot][shared] : -1, tail ? pg[shared] : -1});
-                if (P.align_heads) align_fork.push_back({P.slot, slot, total});
-            }
-            if (!e->slot_align.empty()) {
-                uint32_t* row = &e->slot_align[static_cast<size_t>(slot) * m.L];
-                bool changed = false;
-                for (int l = 0; l < m.L; ++l) {
-                    const uint32_t v = P.align_heads ? P.align_heads[l] : 0u;
-                    changed |= row[l] != v;
-                    row[l] = v;
-                }
-                if (changed) align_set.push_back(slot);
-            }
-            SlotState S;
-            memset(&S, 0, sizeof(S));
-            S.x_len = P.x_len;
-            S.seq_len = total;
-            S.y_len = P.y_len;
-            S.group = gid;
             S.member = c;
-            S.prev_token = -1;
-            S.active = 1;
-            e->h_seq_len[slot] = total;
             sst.push_back(S);
-            sst_slot.push_back(slot);
-            for (int t = 0; c == 0 && t < total; ++t) {
-                r_seq.push_back(seq_idx);
-                r_pos.push_back(t);
-                r_slot.push_back(slot);
-                r_last.push_back(t == total - 1 ? slot : -1);
-                r_page.push_back(e->slot_pages[slot][t / KV_PAGE]);
-            }
+            sst_slot.push_back(P.slot + c);
+        }
+        for (int t = 0; t < total; ++t) {
+            r_seq.push_back(seq_idx);
+            r_pos.push_back(t);
+            r_slot.push_back(P.slot);
+            r_last.push_back(t == total - 1 ? P.slot : -1);
+            r_page.push_back(e->slots[P.slot].pages[t / KV_PAGE]);
         }
     }
     e->last_slots.clear();                   // the row groups of the next step's slot list may have changed
     // state + page tables (synchronous copies: prefill is a once-per-utterance call)
     VCB_CUDA_OK(cudaStreamSynchronize(st));
-    for (size_t i = 0; i < sst.size(); ++i) {
-        VCB_CUDA_OK(cudaMemcpy(e->st + sst_slot[i], &sst[i], sizeof(SlotState), cudaMemcpyHostToDevice));
-        VCB_CUDA_OK(cudaMemcpy(e->page_table + static_cast<size_t>(sst_slot[i]) * e->max_pages_per_slot,
-                               page_row(e, sst_slot[i]).data(), e->max_pages_per_slot * sizeof(int), cudaMemcpyHostToDevice));
-    }
+    for (size_t i = 0; i < sst.size(); ++i)
+        if (write_slot_rows(e, sst_slot[i], sst[i])) return -1;
     for (size_t i = 0; i < gst.size(); ++i)
         VCB_CUDA_OK(cudaMemcpy(e->gr + gst_id[i], &gst[i], sizeof(GroupState), cudaMemcpyHostToDevice));
     for (const auto& g : gsp)
@@ -1816,9 +1718,6 @@ int vcb_prefill(vcb_engine* e, const vcb_prompt* prompts, int32_t n, void* strea
     VCB_CUDA_OK(cudaMemcpy(e->d_seqs, seqs.data(), seqs.size() * sizeof(EmbedSeq), cudaMemcpyHostToDevice));
     if (!fork.empty())
         VCB_CUDA_OK(cudaMemcpy(e->d_fork, fork.data(), fork.size() * sizeof(ForkPair), cudaMemcpyHostToDevice));
-    for (int slot : align_set)
-        VCB_CUDA_OK(cudaMemcpy(e->align_masks + static_cast<size_t>(slot) * m.L, &e->slot_align[static_cast<size_t>(slot) * m.L],
-                               m.L * sizeof(uint32_t), cudaMemcpyHostToDevice));
     std::vector<int> leaders(n);
     for (int i = 0; i < n; ++i) leaders[i] = prompts[i].slot;
     const bool probe = plan_align(e, leaders.data(), n);
@@ -1922,7 +1821,13 @@ int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float*
     const bool mega = fold && e->mega_grid > 0 && n <= 32 && !probe;
     if (!mega && check_split_overrides(e, bpad_for(n))) return -1;
     static thread_local std::vector<std::pair<int, int>> grow;
-    if (const int rc = plan_growth(e, slots, n, grow)) return rc;
+    size_t need = 0;
+    if (e->slots.plan_growth(slots, n, grow, need)) {
+        const size_t free = e->slots.free_list().size();
+        e->n_pages_needed = static_cast<int64_t>(need - free);
+        set_error("vcb_decode_step: KV pool full: the listed slots need %zu more pages, %zu are free", need, free);
+        return VCB_ERR_KV_FULL;
+    }
     if (upload_slots(e, slots, n, st) || apply_growth(e, grow, st)) return -1;
     Pass p = step_pass(e, n, fold);
     {
@@ -1936,7 +1841,7 @@ int vcb_decode_step(vcb_engine* e, const int32_t* slots, int32_t n, const float*
                              mega ? e->mact_d : static_cast<__nv_bfloat16*>(nullptr), e->row_epoch, ++e->step_epoch));
     }
     LAUNCH_COUNT(e);
-    for (int i = 0; i < n; ++i) p.max_ctx = std::max(p.max_ctx, ++e->h_seq_len[slots[i]]);
+    for (int i = 0; i < n; ++i) p.max_ctx = std::max(p.max_ctx, ++e->slots[slots[i]].seq_len);
     p.stop = e->opt_stop;
     if (mega) {
         Pass v = p;                    // the buffers the persistent kernel works on (mega_build)
@@ -1981,12 +1886,12 @@ int vcb_poll(vcb_engine* e, const int32_t* slots, int32_t n, vcb_status* out, vo
     VCB_CUDA_OK(cudaMemcpy(hg.data(), e->gr, hg.size() * sizeof(GroupState), cudaMemcpyDeviceToHost));
     for (int i = 0; i < n; ++i) {
         const int slot = slots[i];
-        if (slot < 0 || slot >= e->cfg.max_slots || e->slot_group[slot] < 0) {
+        if (!e->slots.is_open(slot)) {
             set_error("slot %d is not open", slot);
             return -1;
         }
         const SlotState& S = hs[slot];
-        const GroupState& G = hg[e->slot_group[slot]];
+        const GroupState& G = hg[e->slots[slot].group];
         out[i].done = G.done;
         out[i].forced = S.forced;
         out[i].n_steps = S.n_steps;
@@ -2035,24 +1940,24 @@ int poll_frames(vcb_engine* e, const int32_t* slots, int32_t n, const vcb_edit_s
     }
     for (int i = 0; i < n; ++i) {
         const int slot = slots[i];
-        if (slot < 0 || slot >= e->cfg.max_slots || e->slot_group[slot] < 0) {
+        if (!e->slots.is_open(slot)) {
             set_error("slot %d is not open", slot);
             return -1;
         }
-        if ((e->slot_edit[slot] && !src) || e->slot_copies[slot] != 1) {
+        const SlotRec& r = e->slots[slot];
+        if ((r.edit && !src) || r.copies != 1) {
             set_error("%s: slot %d decodes %s: only single TTS utterances stream%s", fn, slot,
-                      e->slot_edit[slot] ? "an edit prompt" : "a best-of-N group",
-                      e->slot_edit[slot] ? " (edits: vcb_poll_frames_ex)" : "");
+                      r.edit ? "an edit prompt" : "a best-of-N group", r.edit ? " (edits: vcb_poll_frames_ex)" : "");
             return -1;
         }
-        if (src && e->slot_edit[slot] && check_edit_source(slot, e->slot_edit[slot], src[i])) return -1;
-        if (src && !e->slot_edit[slot] && (src[i].orig_dev || src[i].n_spans)) {
+        if (src && r.edit && check_edit_source(slot, r.edit, src[i])) return -1;
+        if (src && !r.edit && (src[i].orig_dev || src[i].n_spans)) {
             set_error("%s: slot %d decodes a TTS prompt but was given an edit source", fn, slot);
             return -1;
         }
-        if (from_host[i] < 0 || from_host[i] > e->slot_final[slot]) {
+        if (from_host[i] < 0 || from_host[i] > r.final_frames) {
             set_error("%s: slot %d: from %d outside [0, %d], the final frames reported so far", fn, slot, from_host[i],
-                      e->slot_final[slot]);
+                      r.final_frames);
             return -1;
         }
     }
@@ -2104,7 +2009,7 @@ int poll_frames(vcb_engine* e, const int32_t* slots, int32_t n, const vcb_edit_s
         bad_host[3 * i] = r.bad_frame;
         bad_host[3 * i + 1] = r.bad_k;
         bad_host[3 * i + 2] = r.bad_tok;
-        e->slot_final[slots[i]] = std::max(e->slot_final[slots[i]], r.final_frames);
+        e->slots[slots[i]].final_frames = std::max(e->slots[slots[i]].final_frames, r.final_frames);
     }
     return 0;
 }
@@ -2160,14 +2065,13 @@ int vcb_read_logprobs(vcb_engine* e, int32_t slot, float* out_host, int32_t max_
 }
 
 int vcb_read_alignment(vcb_engine* e, int32_t slot, float* out_host, int32_t first_pos, int32_t n_pos, void* stream) {
-    if (!e || !out_host || slot < 0 || slot >= e->cfg.max_slots || e->slot_group[slot] < 0 || e->slot_align.empty() ||
+    if (!e || !out_host || !e->slots.is_open(slot) || !e->align_masks ||
         first_pos < 0 || n_pos < 1 || static_cast<long long>(first_pos) + n_pos > e->cfg.max_seq_len) {
         set_error("vcb_read_alignment: slot %d not open, or bad rows [%d, +%d) (max_seq_len %d)", slot, first_pos, n_pos,
                   e ? e->cfg.max_seq_len : 0);
         return -1;
     }
-    const uint32_t* row = &e->slot_align[static_cast<size_t>(slot) * e->m.L];
-    if (std::all_of(row, row + e->m.L, [](uint32_t v) { return v == 0; })) {
+    if (e->slots[slot].align.empty()) {
         set_error("vcb_read_alignment: slot %d was prefilled without align_heads", slot);
         return -1;
     }
@@ -2185,21 +2089,10 @@ int vcb_read_alignment(vcb_engine* e, int32_t slot, float* out_host, int32_t fir
 int vcb_release(vcb_engine* e, int32_t slot, int32_t n_copies) {
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
     VCB_CUDA_OK(cudaDeviceSynchronize());
-    int gid = -1;
-    for (int c = 0; c < n_copies; ++c) {
-        const int s = slot + c;
-        if (s < 0 || s >= e->cfg.max_slots || e->slot_group[s] < 0) continue;
-        gid = e->slot_group[s];
-        e->slot_group[s] = -1;
-        for (int p : e->slot_pages[s])
-            if (--e->page_refs[p] == 0) e->free_pages.push_back(p);
-        e->slot_pages[s].clear();
+    for (int s = slot; s < slot + n_copies; ++s) {
+        if (!e->slots.is_open(s)) continue;
+        e->slots.close(s);                          // the group id goes back with the last of its slots
         VCB_CUDA_OK(cudaMemset(e->st + s, 0, sizeof(SlotState)));
-    }
-    // the group id goes back with the last of its slots, whichever call releases it
-    if (gid >= 0 && std::find(e->slot_group.begin(), e->slot_group.end(), gid) == e->slot_group.end()) {
-        e->free_groups.push_back(gid);
-        e->group_sp[gid] = 0;
     }
     return 0;
 }
@@ -2207,6 +2100,28 @@ int vcb_release(vcb_engine* e, int32_t slot, int32_t n_copies) {
 }  // extern "C"
 
 namespace {
+
+// A device row of every slot that a swap carries besides the KV pages: slot s's row starts at base + s * stride, and its
+// first `bytes` are live
+struct SwapRow {
+    char* base;
+    size_t stride, bytes;
+};
+
+// the rows a swap carries of a slot in state S (DESIGN.md section 3): its token log and log-probability log [0, n_steps),
+// next input (x_slot), last prefill hidden state (h_slot) and, when it aligns, its alignment log [0, seq_len)
+std::vector<SwapRow> swap_rows(const vcb_engine* e, const SlotState& S, bool align) {
+    const ModelDims& m = e->m;
+    const size_t log_row = static_cast<size_t>(e->cfg.max_new_tokens) * m.K, live = static_cast<size_t>(S.n_steps) * m.K;
+    const size_t align_row = static_cast<size_t>(e->cfg.align_text_cap) * sizeof(float);
+    std::vector<SwapRow> rows = {{reinterpret_cast<char*>(e->tok_log.get()), log_row * sizeof(int), live * sizeof(int)},
+                                 {reinterpret_cast<char*>(e->lp_log.get()), log_row * sizeof(float), live * sizeof(float)},
+                                 {reinterpret_cast<char*>(e->x_slot.get()), m.d * sizeof(float), m.d * sizeof(float)},
+                                 {reinterpret_cast<char*>(e->h_slot.get()), m.d * sizeof(float), m.d * sizeof(float)}};
+    if (align)
+        rows.push_back({reinterpret_cast<char*>(e->align_log.get()), e->cfg.max_seq_len * align_row, S.seq_len * align_row});
+    return rows;
+}
 
 // the swap staging region for n pages, and the page list on the device (blocking copy)
 int swap_prepare(vcb_engine* e, const std::vector<int>& pages, size_t words) {
@@ -2235,56 +2150,41 @@ extern "C" {
 
 int vcb_swap_out(vcb_engine* e, int32_t slot, vcb_snapshot** out, void* stream) {
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (!e || !e->finalized || !out || slot < 0 || slot >= e->cfg.max_slots || e->slot_group[slot] < 0) {
+    if (!e || !e->finalized || !out || !e->slots.is_open(slot)) {
         set_error("vcb_swap_out: slot %d is not open (or a null argument)", slot);
         return -1;
     }
-    if (e->slot_copies[slot] != 1) {
+    if (e->slots[slot].copies != 1) {
         set_error("vcb_swap_out: slot %d belongs to a best-of-N group of %d: only one-copy utterances swap", slot,
-                  e->slot_copies[slot]);
+                  e->slots[slot].copies);
         return -1;
     }
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
     if (sync_or_report(e, cudaStreamSynchronize(st), "vcb_swap_out")) return -1;
-    const ModelDims& m = e->m;
-    const int gid = e->slot_group[slot];
+    const int gid = e->slots[slot].group;
     auto snap = std::make_unique<vcb_snapshot>();
     VCB_CUDA_OK(cudaMemcpy(&snap->S, e->st + slot, sizeof(SlotState), cudaMemcpyDeviceToHost));
     VCB_CUDA_OK(cudaMemcpy(&snap->G, e->gr + gid, sizeof(GroupState), cudaMemcpyDeviceToHost));
-    snap->has_sp = e->group_sp[gid];
+    snap->has_sp = e->slots.sp_bits(slot);
     if (snap->has_sp) VCB_CUDA_OK(cudaMemcpy(&snap->sp, e->sp_tab + gid, sizeof(SamplingParams), cudaMemcpyDeviceToHost));
     snap->engine_id = e->id;
-    snap->rng = e->slot_rng[slot];
-    snap->edit = e->slot_edit[slot];
-    snap->final_frames = e->slot_final[slot];
-    const auto& pg = e->slot_pages[slot];
+    snap->rec = e->slots[slot];
+    snap->rec.pages.clear();
+    const auto& pg = e->slots[slot].pages;
     snap->n_pages = std::min(static_cast<int>(pg.size()), (snap->S.seq_len + KV_PAGE - 1) / KV_PAGE);
     const size_t page_bytes = page_bytes_all_layers(e);
-    const size_t n_tok = static_cast<size_t>(snap->S.n_steps) * m.K;
-    if (snap->kv.alloc(snap->n_pages * page_bytes) || snap->tok.alloc(n_tok) || snap->lp.alloc(n_tok) ||
-        snap->rows.alloc(2 * m.d) ||
+    const std::vector<SwapRow> rows = swap_rows(e, snap->S, !snap->rec.align.empty());
+    size_t row_bytes = 0;
+    for (const SwapRow& r : rows) row_bytes += r.bytes;
+    if (snap->kv.alloc(snap->n_pages * page_bytes) || snap->rows.alloc(row_bytes) ||
         swap_prepare(e, std::vector<int>(pg.begin(), pg.begin() + snap->n_pages), snap->n_pages * page_bytes / 16) ||
         swap_copy_kernel<true>(e, snap->n_pages, st))
         return -1;
     VCB_CUDA_OK(cudaMemcpyAsync(snap->kv, e->swap_stage, snap->n_pages * page_bytes, cudaMemcpyDeviceToHost, st));
-    VCB_CUDA_OK(cudaMemcpyAsync(snap->tok, e->tok_log + static_cast<size_t>(slot) * e->cfg.max_new_tokens * m.K,
-                                n_tok * sizeof(int), cudaMemcpyDeviceToHost, st));
-    VCB_CUDA_OK(cudaMemcpyAsync(snap->lp, e->lp_log + static_cast<size_t>(slot) * e->cfg.max_new_tokens * m.K,
-                                n_tok * sizeof(float), cudaMemcpyDeviceToHost, st));
-    VCB_CUDA_OK(cudaMemcpyAsync(snap->rows, e->x_slot + static_cast<size_t>(slot) * m.d, m.d * sizeof(float),
-                                cudaMemcpyDeviceToHost, st));
-    VCB_CUDA_OK(cudaMemcpyAsync(snap->rows + m.d, e->h_slot + static_cast<size_t>(slot) * m.d, m.d * sizeof(float),
-                                cudaMemcpyDeviceToHost, st));
-    if (!e->slot_align.empty()) {
-        const uint32_t* row = &e->slot_align[static_cast<size_t>(slot) * m.L];
-        if (std::any_of(row, row + m.L, [](uint32_t v) { return v != 0; })) {
-            const size_t n = static_cast<size_t>(snap->S.seq_len) * e->cfg.align_text_cap;
-            snap->align.assign(row, row + m.L);
-            if (snap->align_rows.alloc(n)) return -1;
-            VCB_CUDA_OK(cudaMemcpyAsync(snap->align_rows, e->align_log + static_cast<size_t>(slot) * e->cfg.max_seq_len *
-                                                                             e->cfg.align_text_cap,
-                                        n * sizeof(float), cudaMemcpyDeviceToHost, st));
-        }
+    size_t off = 0;
+    for (const SwapRow& r : rows) {
+        VCB_CUDA_OK(cudaMemcpyAsync(snap->rows + off, r.base + slot * r.stride, r.bytes, cudaMemcpyDeviceToHost, st));
+        off += r.bytes;
     }
     if (sync_or_report(e, cudaStreamSynchronize(st), "vcb_swap_out")) return -1;
     if (vcb_release(e, slot, 1)) return -1;
@@ -2298,72 +2198,37 @@ int vcb_swap_in(vcb_engine* e, const vcb_snapshot* snap, int32_t slot, void* str
         set_error("vcb_swap_in: not a snapshot of this engine (or a null argument)");
         return -1;
     }
-    if (slot < 0 || slot >= e->cfg.max_slots || e->slot_group[slot] >= 0) {
+    if (slot < 0 || slot >= e->cfg.max_slots || e->slots.is_open(slot)) {
         set_error("vcb_swap_in: slot %d is not a free slot of this engine", slot);
         return -1;
     }
-    if (e->free_groups.empty() || static_cast<size_t>(snap->n_pages) > e->free_pages.size()) {
-        set_error("vcb_swap_in: needs a free group and %d KV pages (%zu free)", snap->n_pages, e->free_pages.size());
+    const size_t free = e->slots.free_list().size();
+    if (e->slots.groups_left() == 0 || static_cast<size_t>(snap->n_pages) > free) {
+        set_error("vcb_swap_in: needs a free group and %d KV pages (%zu free)", snap->n_pages, free);
         return -1;
     }
-    const ModelDims& m = e->m;
     const size_t page_bytes = page_bytes_all_layers(e);
     VCB_CUDA_OK(cudaSetDevice(e->cfg.device));
     if (sync_or_report(e, cudaStreamSynchronize(st), "vcb_swap_in")) return -1;
     if (swap_prepare(e, {}, snap->n_pages * page_bytes / 16)) return -1;
     // nothing can fail for want of resources from here on: take the group and the pages
-    const int gid = e->free_groups.back();
-    e->free_groups.pop_back();
-    auto& pg = e->slot_pages[slot];
-    pg.clear();
-    for (int p = 0; p < snap->n_pages; ++p) {
-        pg.push_back(e->free_pages.back());
-        e->free_pages.pop_back();
-        ++e->page_refs[pg.back()];
-    }
+    const int gid = e->slots.open(slot, snap->rec, snap->n_pages, -1, snap->has_sp);
+    e->slots[slot].seq_len = snap->S.seq_len;
     SlotState S = snap->S;
     S.group = gid;
     S.member = 0;
     GroupState G = snap->G;
     G.first_slot = slot;
-    e->slot_group[slot] = gid;
-    e->slot_rng[slot] = snap->rng;
-    e->slot_edit[slot] = snap->edit;
-    e->slot_copies[slot] = 1;
-    e->slot_shared[slot] = 0;
-    e->slot_final[slot] = snap->final_frames;
-    e->h_seq_len[slot] = S.seq_len;
-    e->group_sp[gid] = snap->has_sp;
     e->last_slots.clear();
-    if (swap_prepare(e, pg, 0)) return -1;
-    VCB_CUDA_OK(cudaMemcpy(e->page_table + static_cast<size_t>(slot) * e->max_pages_per_slot, page_row(e, slot).data(),
-                           e->max_pages_per_slot * sizeof(int), cudaMemcpyHostToDevice));
-    VCB_CUDA_OK(cudaMemcpy(e->st + slot, &S, sizeof(SlotState), cudaMemcpyHostToDevice));
+    if (swap_prepare(e, e->slots[slot].pages, 0) || write_slot_rows(e, slot, S)) return -1;
     VCB_CUDA_OK(cudaMemcpy(e->gr + gid, &G, sizeof(GroupState), cudaMemcpyHostToDevice));
     if (snap->has_sp) VCB_CUDA_OK(cudaMemcpy(e->sp_tab + gid, &snap->sp, sizeof(SamplingParams), cudaMemcpyHostToDevice));
     VCB_CUDA_OK(cudaMemcpyAsync(e->swap_stage, snap->kv, snap->n_pages * page_bytes, cudaMemcpyHostToDevice, st));
     if (swap_copy_kernel<false>(e, snap->n_pages, st)) return -1;
-    VCB_CUDA_OK(cudaMemcpyAsync(e->tok_log + static_cast<size_t>(slot) * e->cfg.max_new_tokens * m.K, snap->tok,
-                                static_cast<size_t>(snap->S.n_steps) * m.K * sizeof(int), cudaMemcpyHostToDevice, st));
-    VCB_CUDA_OK(cudaMemcpyAsync(e->lp_log + static_cast<size_t>(slot) * e->cfg.max_new_tokens * m.K, snap->lp,
-                                static_cast<size_t>(snap->S.n_steps) * m.K * sizeof(float), cudaMemcpyHostToDevice, st));
-    VCB_CUDA_OK(cudaMemcpyAsync(e->x_slot + static_cast<size_t>(slot) * m.d, snap->rows, m.d * sizeof(float),
-                                cudaMemcpyHostToDevice, st));
-    VCB_CUDA_OK(cudaMemcpyAsync(e->h_slot + static_cast<size_t>(slot) * m.d, snap->rows + m.d, m.d * sizeof(float),
-                                cudaMemcpyHostToDevice, st));
-    // the slot's head masks (a snapshot with alignment comes from an engine whose log exists: this one)
-    if (!e->slot_align.empty()) {
-        uint32_t* row = &e->slot_align[static_cast<size_t>(slot) * m.L];
-        std::vector<uint32_t> want = snap->align.empty() ? std::vector<uint32_t>(m.L, 0u) : snap->align;
-        if (!std::equal(want.begin(), want.end(), row)) {
-            std::copy(want.begin(), want.end(), row);
-            VCB_CUDA_OK(cudaMemcpy(e->align_masks + static_cast<size_t>(slot) * m.L, row, m.L * sizeof(uint32_t),
-                                   cudaMemcpyHostToDevice));
-        }
-        if (!snap->align.empty())
-            VCB_CUDA_OK(cudaMemcpyAsync(e->align_log + static_cast<size_t>(slot) * e->cfg.max_seq_len * e->cfg.align_text_cap,
-                                        snap->align_rows, static_cast<size_t>(snap->S.seq_len) * e->cfg.align_text_cap *
-                                        sizeof(float), cudaMemcpyHostToDevice, st));
+    size_t off = 0;
+    for (const SwapRow& r : swap_rows(e, snap->S, !snap->rec.align.empty())) {
+        VCB_CUDA_OK(cudaMemcpyAsync(r.base + slot * r.stride, snap->rows + off, r.bytes, cudaMemcpyHostToDevice, st));
+        off += r.bytes;
     }
     return sync_or_report(e, cudaStreamSynchronize(st), "vcb_swap_in");
 }
@@ -2756,7 +2621,7 @@ int vcb_debug_kv_pages(vcb_engine* e, int32_t layer, int32_t slot, int32_t first
                        void* v_host) {
     if (!e || !k_host || !v_host || layer < 0 || layer >= e->m.L || !e->layers[layer].kpool || slot < 0 ||
         slot >= e->cfg.max_slots || first_page < 0 || n_pages < 1 ||
-        static_cast<size_t>(first_page) + n_pages > e->slot_pages[slot].size()) {
+        static_cast<size_t>(first_page) + n_pages > e->slots[slot].pages.size()) {
         set_error("vcb_debug_kv_pages: layer %d, slot %d, pages %d .. %d: not a finalized engine's layer or the slot's pages",
                   layer, slot, first_page, first_page + n_pages - 1);
         return -1;
@@ -2766,7 +2631,7 @@ int vcb_debug_kv_pages(vcb_engine* e, int32_t layer, int32_t slot, int32_t first
     const size_t page_bytes = static_cast<size_t>(e->m.H) * kv_slab_bytes(e->kv_dtype, e->m.hd);
     const Layer& Ly = e->layers[layer];
     for (int i = 0; i < n_pages; ++i) {
-        const size_t src = static_cast<size_t>(e->slot_pages[slot][first_page + i]) * page_bytes;
+        const size_t src = static_cast<size_t>(e->slots[slot].pages[first_page + i]) * page_bytes;
         VCB_CUDA_OK(cudaMemcpy(static_cast<uint8_t*>(k_host) + i * page_bytes, Ly.kpool + src, page_bytes, cudaMemcpyDeviceToHost));
         VCB_CUDA_OK(cudaMemcpy(static_cast<uint8_t*>(v_host) + i * page_bytes, Ly.vpool + src, page_bytes, cudaMemcpyDeviceToHost));
     }
@@ -3066,7 +2931,7 @@ int64_t vcb_counter(vcb_engine* e, const char* name) {
     if (!strcmp(name, "att_early")) return e->opt_att_early;
     if (!strcmp(name, "att_poison")) return e->opt_att_poison;
     if (!strcmp(name, "poll_frames")) return e->n_poll_frames;
-    if (!strcmp(name, "kv_pages_free")) return static_cast<int64_t>(e->free_pages.size());
+    if (!strcmp(name, "kv_pages_free")) return static_cast<int64_t>(e->slots.free_list().size());
     if (!strcmp(name, "kv_pages_total")) return e->n_pages;
     if (!strcmp(name, "kv_pages_needed")) return e->n_pages_needed;
     if (!strcmp(name, "kv_page_bytes")) return static_cast<int64_t>(page_bytes_all_layers(e));
